@@ -107,7 +107,9 @@ int npair_bwd_exchange_mode(const npair_ctx* ctx);
 /* fills proto defaults (caffe.proto:4-7,19-22), world=1, rank=0, num_tops=5, fp32-faithful fp16x2, tensor-core GEMMs, extensions off */
 void npair_config_default(npair_config* cfg, int32_t Q, int32_t D);
 
-/* Workspace the context will allocate on the device for this configuration (bytes). */
+/* Device memory (bytes) a context created for this configuration allocates, computed for an H100 SXM (132 SMs: the split-K
+ * buffer of the gradient GEMM depends on the SM count).  world > 1: what a context created with a communicator and peer
+ * access between all ranks allocates (its peer-memory exchange region included). */
 size_t npair_workspace_bytes(const npair_config* cfg);
 
 /* 128-byte NCCL unique id (rank 0 calls this and ships the bytes to the other ranks out of band). */

@@ -16,12 +16,13 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
 
 #include "../../include/npair_b200.h"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "grad_fused.cuh"
 #include "kernels.cuh"
 
@@ -181,8 +182,7 @@ static cudaError_t launch_sim_gemm(int prec, bool sym_tiles, const CUtensorMap& 
   return sym_tiles ? launch_split_gemm_t<1, true, EPI_SIM_SYM, 64>(a, b, sm, p, sms, st) : launch_split_gemm_t<1, true, EPI_SIM, 64>(a, b, sm, p, sms, st);
 }
 // Gradient GEMM: A = split gradient weights, B = split transposed features (EPI_OUT)
-static cudaError_t launch_split_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  (void)epi;
+static cudaError_t launch_split_gemm(int prec, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
   if (prec == PREC_BF16) return launch_split_gemm_t<1, true, EPI_OUT, 64>(a, b, sm, p, sms, st);
   if (prec == PREC_FP16X2) return launch_split_gemm_t<2, false, EPI_OUT, 32>(a, b, sm, p, sms, st);
   return launch_split_gemm_t<3, true, EPI_OUT, 32>(a, b, sm, p, sms, st);
@@ -277,10 +277,8 @@ static cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long l
   return cudaGetLastError();
 }
 
-// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K)
 // ---- peer-memory exchange (world > 1, one process per GPU, NVLink / NVSwitch) ----
-// Every rank owns one exported region (cudaIpc-mapped into all ranks):
-//     X[2][N][D] fp32 | LAB[2][N] | REC[2][N][8] | XCH[2][world][8192] (small world-scope reductions) | FLAGS[3 kinds][2][world] uint32
+// Every rank owns one exported region (cudaIpc-mapped into all ranks, laid out by XchgLayout below)
 // and PUSHES its own rows into every rank's region with plain stores over NVLink, then raises one flag per peer (release.sys);
 // consumers wait for the world's flags (acquire.sys).  Replaces GatherFeatureAndLabel's MPI_Allgather (reference .cu:17-43) and the
 // backward's exchange (row records instead of the N x D all-reduce, .cu:462-489) without a collective rendezvous: nothing
@@ -321,6 +319,7 @@ __global__ void p2p_wait_kernel(const uint32_t* __restrict__ flags /*[world]*/, 
   }
 }
 
+// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K)
 __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, long long n, float* __restrict__ out, float beta) {
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
   for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
@@ -339,17 +338,22 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
     }
   }
 }
-// choose a split-K factor that fills the SMs when the output has few tiles (strong scaling: Q = B/world shrinks)
-static void plan_splits(GemmParams* gp, int sms, long long max_part_floats) {
-  const int tiles = gp->tiles_m * gp->tiles_n;
+// Split-K of a gradient GEMM: when its output has too few tiles to fill the SMs (strong scaling: Q = B/world shrinks), the K range
+// is cut into at most 16 slices of at least min_kb K blocks each; splitk_reduce_kernel sums the slices' partial products.
+struct SplitK { int splits, kb_per_split; };
+static SplitK split_k(int num_kblocks, int tiles, int sms, int min_kb) {
   int splits = sms / (tiles > 0 ? tiles : 1);
   if (splits > 16) splits = 16;
-  if (splits > gp->num_kblocks / 4) splits = gp->num_kblocks / 4;       // keep >= 4 k-blocks per split
-  while (splits > 1 && static_cast<long long>(splits) * gp->M * gp->ldo > max_part_floats) --splits;
+  if (splits > num_kblocks / min_kb) splits = num_kblocks / min_kb;
   if (splits < 1) splits = 1;
-  int kpb = (gp->num_kblocks + splits - 1) / splits;
-  splits = (gp->num_kblocks + kpb - 1) / kpb;                            // no empty split
-  gp->splits = splits; gp->kb_per_split = kpb;
+  const int kpb = (num_kblocks + splits - 1) / splits;
+  return SplitK{(num_kblocks + kpb - 1) / kpb, kpb};                    // no empty split
+}
+
+// blocks of 256 threads for `work` items: at least one, at most max_blocks
+static inline int grid_for(long long work, int max_blocks) {
+  const long long nb = (work + 255) / 256;
+  return static_cast<int>(nb < 1 ? 1 : (nb > max_blocks ? max_blocks : nb));
 }
 
 static inline long long round_up(long long v, long long m) { return (v + m - 1) / m * m; }
@@ -361,50 +365,168 @@ using namespace npair;
 #define NPAIR_PROF_PHASES 9
 #define NPAIR_INTERNAL_FULL_TILES (1 << 30)   // npair_config.flags, internal: world == 1 computes every tile (symmetry self-check)
 #define NPAIR_XCH_FLOATS 8192          // largest small exchange: two sides x 2048 64-bit digit counts
+#define NPAIR_H100_SXM_SMS 132         // SM count of an H100 SXM (PCIe: 114), for sizing without a device at hand
+
+// ------------------------------------------------------------------------------------------------ buffer plan
+// One rank's peer-memory exchange region, in floats.  Each part is double-buffered by the step parity and holds every rank's rows:
+//     X[2][N][D] | LAB[2][N rounded up to 4] | REC[2][N][8] | XCH[2][world][NPAIR_XCH_FLOATS] (world scope) | FLAGS[3 kinds][2][world] uint32
+enum { XP_X, XP_LAB, XP_REC, XP_XCH, XP_COUNT };
+struct XchgLayout {
+  long long base[XP_COUNT], par_stride[XP_COUNT], rank_stride[XP_COUNT], flags, floats;
+  long long off(int part, long long par, int rank) const { return base[part] + par * par_stride[part] + rank * rank_stride[part]; }
+};
+static XchgLayout xchg_layout(int Q, int D, int world, bool world_scope) {
+  const long long N = static_cast<long long>(Q) * world;
+  const long long rank_floats[XP_COUNT] = {static_cast<long long>(Q) * D, Q, 8ll * Q, world_scope ? NPAIR_XCH_FLOATS : 0};
+  const long long par_floats[XP_COUNT] = {N * D, round_up(N, 4), 8 * N, world * rank_floats[XP_XCH]};
+  XchgLayout l;
+  long long o = 0;
+  for (int p = 0; p < XP_COUNT; ++p) { l.base[p] = o; l.par_stride[p] = par_floats[p]; l.rank_stride[p] = rank_floats[p]; o += 2 * par_floats[p]; }
+  l.flags = o;
+  l.floats = o + round_up(6ll * world, 4);
+  return l;
+}
+// Index of the flag `rank` raises after an exchange of `kind` into the buffers of parity `par`; rank 0's starts the world's flags
+enum { XCHG_FEATURES, XCHG_RECORDS, XCHG_SMALL };
+static inline int xchg_flag(int kind, int par, int world, int rank) { return (2 * kind + par) * world + rank; }
+
+// world == 1: S = X X^T is symmetric, so the similarity GEMM computes only the tiles (m_blk, n_blk) whose 256 columns reach the
+// 128-row block's diagonal or beyond
+static std::vector<int2> sym_tile_list(int Q, int N) {
+  std::vector<int2> tl;
+  const int tm = (Q + 127) / 128, tn = (N + 255) / 256;
+  for (int mb = 0; mb < tm; ++mb)
+    for (int nb = mb / 2; nb < tn; ++nb) tl.push_back(make_int2(mb, nb));
+  return tl;
+}
+
+// device buffers of a context
+enum { B_XTOT, B_LABTOT, B_YNORM, B_DY, B_INV_NORM, B_S, B_XS, B_XST, B_XCAT_A, B_XCAT_B, B_H, B_XLT, B_HT, B_OUT2, B_RS_TOTAL,
+       B_PART, B_ROWS, B_BS, B_PARTIAL, B_GHIST, B_GCAND, B_SYM_TILES, B_XCH_SRC, B_XCH_ALL, B_P2P_REGION, B_P2P_TICKET, B_P2P_PEERS,
+       B_COUNT };
+
+// What a context decides from its configuration and two device facts, and the byte size of every device buffer it allocates
+// (0: not allocated).  The peer-memory exchange buffers are sized as if the context had a communicator and peer access.
+struct Plan {
+  int N, nsplit, bk_sim, bk_grad;
+  long long Dp, Np, Qp, ldS;     // padded feature / all-rows / local-rows extents of the operand pieces, row stride of S
+  int bwd_mode;                  // NPAIR_BWDMODE_*
+  bool fused_grad;               // the gradient weights are produced inside the gradient GEMM: no H in HBM
+  bool cat;                      // the similarity GEMM reads the K-concatenated operands XcatA / XcatB, not Xs
+  unsigned int gcand_cap;        // entries per side of the GLOBAL radix select's candidate lists
+  int grad_chunk_kb;             // accumulation chunk of the gradient GEMM in 32-column K blocks (grad_fused.cuh); 0 = unchunked
+  int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
+  SplitK grad_split;             // and its split-K
+  int n_sym_tiles;
+  bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
+  XchgLayout xl;
+  size_t bytes[B_COUNT];
+};
+
+static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
+  Plan p{};
+  const int prec = cfg.sim_precision, W = cfg.world;
+  const long long Q = cfg.Q, D = cfg.D, N = Q * W;
+  const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
+  p.N = static_cast<int>(N);
+  p.nsplit = nsplit_of_prec(prec); p.bk_sim = bk_of(prec, EPI_SIM); p.bk_grad = bk_of(prec, EPI_OUT);
+  p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
+  // The row-record exchange needs S[j][m] on rank r to equal S[m][j] on the rank that owns row m BIT FOR BIT, i.e. a tensor-core
+  // MMA whose result does not change when the operand roles are swapped; without one the reference's reduce-scatter form is used.
+  p.bwd_mode = !multi ? NPAIR_BWDMODE_SINGLE
+             : (cfg.bwd_exchange == NPAIR_BWD_AUTO && (!tc || mma_symmetric)) ? NPAIR_BWDMODE_ROW_SCALARS : NPAIR_BWDMODE_REDUCE_SCATTER;
+  const bool rs = p.bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER;
+  p.fused_grad = tc && !rs && !(cfg.flags & NPAIR_FLAG_NO_FUSED_GRAD);
+  p.cat = tc && prec != PREC_BF16;
+  // GLOBAL relative select with a general SN: candidate lists of the chosen first-digit bucket (1/8 of the block, at most
+  // 32 M entries per side; a bigger bucket -- heavily tied data -- takes the three-sweep path)
+  if ((is_rel(cfg.ap_method) && cfg.ap_region == NPAIR_GLOBAL) || (is_rel(cfg.an_method) && cfg.an_region == NPAIR_GLOBAL)) {
+    const long long cap = Q * N / 8 + 4096;
+    p.gcand_cap = static_cast<unsigned int>(cap < (32ll << 20) ? cap : (32ll << 20));
+  }
+  // default: 2048 database columns; negative: one accumulator for the whole K range (diagnostic)
+  p.grad_chunk_kb = cfg.grad_chunk_cols > 0 ? (cfg.grad_chunk_cols + 31) / 32 : (cfg.grad_chunk_cols < 0 ? 0 : 64);
+  // the fused kernel walks K in 32-column blocks and keeps >= 8 of them (256 columns) per split; the split GEMM keeps >= 4
+  p.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
+  const int tiles = static_cast<int>(((Q + 127) / 128) * ((D + 255) / 256));
+  p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
+  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_list(cfg.Q, p.N).size());
+  p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
+  p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
+  const bool wscope = cfg.global_scope && multi;
+  if (p.want_p2p_feat || p.want_p2p_rec) p.xl = xchg_layout(cfg.Q, cfg.D, W, wscope);
+
+  size_t* b = p.bytes;
+  const size_t f = sizeof(float), ns = p.nsplit;
+  if (multi) { b[B_XTOT] = f * N * D; b[B_LABTOT] = f * N; }                    // all-gather targets
+  if (cfg.normalize_input) { b[B_YNORM] = b[B_DY] = f * Q * D; b[B_INV_NORM] = f * Q; }   // y, dy, 1/||x||
+  b[B_S] = f * Q * p.ldS;
+  if (!p.cat) b[B_XS] = 2 * ns * N * p.Dp;                                      // operand pieces [ns][N][Dp]
+  b[B_XST] = 2 * ns * D * p.Np;                                                 // transposed pieces [ns][D][Np]
+  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * kcat_mult(prec) * p.Dp;        // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  if (!p.fused_grad) b[B_H] = 2 * ns * Q * p.Np;                                // materialised gradient weights
+  if (rs) { b[B_XLT] = 2 * ns * D * p.Qp; b[B_HT] = 2 * ns * N * p.Qp; b[B_OUT2] = f * N * D; }
+  if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = f * 8 * N;        // gathered row records
+  if (p.grad_split.splits > 1) b[B_PART] = f * p.grad_split.splits * Q * D;     // split-K partial products
+  b[B_ROWS] = 4 * 21 * Q + 64;   // 13 row arrays of Q 4-byte words (RowArrays) + the 32-byte aligned [Q][8] row records
+  b[B_BS] = sizeof(BlockScalars);
+  b[B_PARTIAL] = f * 2048;
+  b[B_GHIST] = sizeof(unsigned long long) * 4096;
+  b[B_GCAND] = sizeof(uint32_t) * 2ull * p.gcand_cap;
+  b[B_SYM_TILES] = sizeof(int2) * p.n_sym_tiles;
+  if (wscope) { b[B_XCH_SRC] = f * NPAIR_XCH_FLOATS; b[B_XCH_ALL] = f * NPAIR_XCH_FLOATS * W; }   // the latter for NCCL
+  if (p.want_p2p_feat || p.want_p2p_rec) {
+    b[B_P2P_REGION] = f * p.xl.floats; b[B_P2P_TICKET] = sizeof(unsigned int); b[B_P2P_PEERS] = sizeof(float*) * W;
+  }
+  return p;
+}
+
+// cudaMalloc of a planned buffer: nothing for 0 bytes, optionally zero-filled
+template <class T>
+static cudaError_t dev_alloc(T** p, size_t bytes, bool zero) {
+  if (bytes == 0) return cudaSuccess;
+  cudaError_t e = cudaMalloc(p, bytes);
+  if (e == cudaSuccess && zero) e = cudaMemset(*p, 0, bytes);
+  return e;
+}
 
 // ------------------------------------------------------------------------------------------------ context
-struct npair_ctx {
+// A context is its plan plus the buffers and per-step state.
+struct npair_ctx : Plan {
   npair_config cfg;
-  int Q, N, D, world, rank, prec, nsplit, bk_sim, bk_grad, sms, device;
-  long long Dp, Np, Qp, ldS;
+  int Q, D, world, rank, prec, sms, device;
   // device scratch
   float* Xtot_buf = nullptr;     // world > 1: all-gather target
   float* labtot_buf = nullptr;
   float* S = nullptr;
   uint16_t *Xs = nullptr, *XsT = nullptr, *XlT = nullptr, *H = nullptr, *HT = nullptr;
   float* OUT2 = nullptr;         // world > 1: N x D transposed-term product before the reduce-scatter
-  int bwd_mode = 0;              // NPAIR_BWDMODE_*
-  uint16_t *XcatA = nullptr, *XcatB = nullptr;   // row-scalar mode, fp16x2: K-concatenated operands [N][3*Dp]
+  uint16_t *XcatA = nullptr, *XcatB = nullptr;   // K-concatenated operands [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
   float* rs_total = nullptr;     // row-scalar mode: all-gathered [N][8] row records
   CUtensorMap tm_catA, tm_catB;
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
-  int grad_chunk_kb = 64;        // accumulation chunk of the gradient GEMM in 32-column K blocks (grad_fused.cuh); 0 = unchunked
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
-  bool fused_grad = false;
   bool rs_gathered = false;
   bool ext_gathered = false;      // the current forward came through npair_forward_gathered (external collectives)
   bool defer_sync = false;        // npair_forward_backward: the forward returns after enqueueing, the caller synchronises later
   // peer-memory exchange (world > 1 with a communicator; NPAIR_FLAG_NCCL_FEATURES / _RECORDS fall back to NCCL)
   bool p2p_feat = false, p2p_rec = false;
-  float* p2p_region = nullptr;         // X[2][N][D] | LAB[2][N] | REC[2][N][8] | FLAGS
-  long long p2p_offX = 0, p2p_offLab = 0, p2p_offRec = 0, p2p_offXch = 0, p2p_offFlags = 0;   // in floats
+  float* p2p_region = nullptr;         // laid out by xl (XchgLayout)
   uint32_t xch_epoch = 0;              // small exchanges of the world-scope mode (several per step)
   float* xch_src = nullptr;            // [8192] staging of this rank's contribution
   float* xch_all = nullptr;            // NCCL fallback: gathered [world][8192]
-  float** p2p_peer_base = nullptr;     // device array [world] of the ranks' regions
+  float** p2p_peer_base = nullptr;     // device array [world] of the ranks' regions; set only once every peer's region is mapped
   unsigned int* p2p_ticket = nullptr;
   std::vector<void*> p2p_opened;
   uint32_t p2p_fwd_epoch = 0, p2p_rec_epoch = 0;
   int2* sym_tiles = nullptr;     // world == 1: (m_blk, n_blk) of the similarity tiles touching the upper triangle
-  int n_sym_tiles = 0;
   float* part = nullptr;         // split-K partial products of the gradient GEMM
-  long long part_floats = 0;
   void* row_block = nullptr;     // backing store of RowArrays
   RowArrays ra;
   BlockScalars* bs = nullptr;
   float* partial = nullptr;
   unsigned long long* ghist = nullptr;   // [2][2048] 64-bit digit counts of the GLOBAL radix select
-  uint32_t* gcand = nullptr; unsigned int gcand_cap = 0;   // [2][cap] compacted candidates of the GLOBAL radix select
+  uint32_t* gcand = nullptr;     // [2][gcand_cap] compacted candidates of the GLOBAL radix select
   float* tops_pinned = nullptr;  // host-mapped: 5 tops + err(int) + sequence number of the forward that wrote them
   unsigned int tops_seq = 0;
   float* tops_dev = nullptr;
@@ -417,7 +539,6 @@ struct npair_ctx {
   const float *x_total = nullptr, *lab_total = nullptr;
   bool fwd_done = false;
   cudaStream_t last_stream = nullptr;
-  size_t bytes = 0;
   std::string err;
   // optional per-phase CUDA-event timing (npair_profile_enable)
   bool prof = false;
@@ -445,7 +566,6 @@ struct PhaseTimer {
     }                                                                                                    \
   } while (0)
 
-static inline bool is_rel_cfg(int m) { return m == NPAIR_RELATIVE_HARD || m == NPAIR_RELATIVE_EASY; }
 static int validate(const npair_config* c, std::string* err) {
   if (!c) { *err = "null config"; return NPAIR_E_ARG; }
   if (c->Q < 1 || c->D < 1) { *err = "Q and D must be >= 1"; return NPAIR_E_ARG; }
@@ -465,41 +585,6 @@ static int validate(const npair_config* c, std::string* err) {
   return NPAIR_OK;
 }
 
-static inline bool is_rel_cfg_early(int m) { return m == NPAIR_RELATIVE_HARD || m == NPAIR_RELATIVE_EASY; }
-struct Sizes { long long N, Dp, Np, Qp, ldS; int ns; size_t total; };
-static Sizes sizes_of(const npair_config* c) {
-  Sizes s;
-  s.N = static_cast<long long>(c->Q) * c->world;
-  s.Dp = round_up(c->D, 64); s.Np = round_up(s.N, 64); s.Qp = round_up(c->Q, 64); s.ldS = round_up(s.N, 32);
-  s.ns = nsplit_of_prec(c->sim_precision);
-  const bool tc = c->gemm_backend == NPAIR_GEMM_TCGEN05;
-  const bool rs = c->world > 1 && c->bwd_exchange != NPAIR_BWD_AUTO;
-  const bool fused = tc && !rs;
-  size_t t = 0;
-  if (c->world > 1) t += sizeof(float) * (s.N * c->D + s.N);                       // all-gather targets
-  t += sizeof(float) * c->Q * s.ldS;                                                // S
-  t += 2ull * s.ns * s.N * s.Dp + 2ull * s.ns * c->D * s.Np;                        // operand pieces, transposed pieces
-  if (tc && c->sim_precision != NPAIR_PREC_BF16) t += 2ull * 2 * s.N * kcat_mult(c->sim_precision) * s.Dp;   // K-concatenated operands
-  if (!fused) t += 2ull * s.ns * c->Q * s.Np;                                       // materialised gradient weights
-  if (rs) { t += 2ull * s.ns * c->D * s.Qp + 2ull * s.ns * s.N * s.Qp + sizeof(float) * s.N * c->D; }
-  if (c->world > 1 && !rs) t += sizeof(float) * 8ull * s.N;                         // gathered row records
-  if (c->normalize_input) t += sizeof(float) * (2ull * c->Q * c->D + c->Q) + (c->world > 1 ? 0 : 0);   // y, dy, 1/||x||
-  if (tc) {                                                                         // split-K partials of the gradient GEMM
-    const int tiles = ((c->Q + 127) / 128) * ((c->D + 255) / 256);
-    int smax = 132 / (tiles > 0 ? tiles : 1); if (smax > 16) smax = 16;   // upper bound: 132 SMs (H100 SXM; PCIe: 114)
-    if (smax > 1) t += sizeof(float) * static_cast<size_t>(smax) * c->Q * c->D;
-  }
-  if (tc && (is_rel_cfg_early(c->ap_method) && c->ap_region == NPAIR_GLOBAL || is_rel_cfg_early(c->an_method) && c->an_region == NPAIR_GLOBAL)) {
-    unsigned long long cap = static_cast<unsigned long long>(c->Q) * s.N / 8 + 4096;           // candidate lists of the GLOBAL radix select
-    if (cap > (32ull << 20)) cap = 32ull << 20;
-    t += 8ull * cap;
-  }
-  if (c->world > 1) t += sizeof(float) * (2ull * s.N * c->D + 2ull * s.N + 16ull * s.N) + (c->global_scope ? 8ull * c->world * 8192 : 0);   // exchange region
-  t += 4ull * 21 * c->Q + 65536;                                                    // row arrays, records, scalars
-  s.total = t;
-  return s;
-}
-
 extern "C" {
 
 const char* npair_version(void) { return "npairloss_b200 0.1 (abi 1; sm_90a wgmma/TMA)"; }
@@ -517,7 +602,10 @@ void npair_config_default(npair_config* c, int32_t Q, int32_t D) {
 size_t npair_workspace_bytes(const npair_config* cfg) {
   std::string e;
   if (validate(cfg, &e) != NPAIR_OK) return 0;
-  return sizes_of(cfg).total;
+  const Plan p = plan_of(*cfg, NPAIR_H100_SXM_SMS, true);
+  size_t total = 0;
+  for (size_t b : p.bytes) total += b;
+  return total;
 }
 
 const char* npair_last_error(const npair_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
@@ -622,70 +710,36 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     npair_destroy(c); return NPAIR_E_CUDA;
   }
   c->sms = prop.multiProcessorCount;
-  const Sizes sz = sizes_of(cfg);
-  c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->N = static_cast<int>(sz.N);
-  c->prec = cfg->sim_precision; c->nsplit = sz.ns; c->bk_sim = bk_of(c->prec, EPI_SIM); c->bk_grad = bk_of(c->prec, EPI_OUT);
-  c->Dp = sz.Dp; c->Np = sz.Np; c->Qp = sz.Qp; c->ldS = sz.ldS; c->bytes = sz.total;
+  // only the multi-rank row-record backward on the tensor cores depends on the check, which itself creates a single-rank context
+  const bool ask_sym = cfg->world > 1 && cfg->bwd_exchange == NPAIR_BWD_AUTO && cfg->gemm_backend == NPAIR_GEMM_TCGEN05;
+  static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, !ask_sym || mma_is_symmetric(cfg->sim_precision, c->device));
+  c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
   const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit;
-  if (c->world > 1) {
-    CREATE_TRY(cudaMalloc(&c->Xtot_buf, sizeof(float) * static_cast<size_t>(N) * D));
-    CREATE_TRY(cudaMalloc(&c->labtot_buf, sizeof(float) * N));
-  }
-  if (cfg->normalize_input) {
-    CREATE_TRY(cudaMalloc(&c->Ynorm, sizeof(float) * static_cast<size_t>(Q) * D));
-    CREATE_TRY(cudaMalloc(&c->dY, sizeof(float) * static_cast<size_t>(Q) * D));
-    CREATE_TRY(cudaMalloc(&c->inv_norm, sizeof(float) * Q));
-  }
-  CREATE_TRY(cudaMalloc(&c->S, sizeof(float) * static_cast<size_t>(Q) * c->ldS));
-  CREATE_TRY(cudaMemset(c->S, 0, sizeof(float) * static_cast<size_t>(Q) * c->ldS));
-  CREATE_TRY(cudaMalloc(&c->Xs, 2ull * ns * N * c->Dp));
-  CREATE_TRY(cudaMemset(c->Xs, 0, 2ull * ns * N * c->Dp));
-  CREATE_TRY(cudaMalloc(&c->XsT, 2ull * ns * D * c->Np));
-  CREATE_TRY(cudaMemset(c->XsT, 0, 2ull * ns * D * c->Np));
-  // gradient weights are only materialised when the fused tensor-memory kernel is not used
-  // (reduce-scatter exchange, SIMT cross-check backend, NPAIR_NO_FUSED_GRAD)
-  {
-    const bool multi_rs = c->world > 1 && (cfg->bwd_exchange != NPAIR_BWD_AUTO ||
-                                           (cfg->gemm_backend == NPAIR_GEMM_TCGEN05 && !mma_is_symmetric(cfg->sim_precision, c->device)));
-    c->fused_grad = cfg->gemm_backend == NPAIR_GEMM_TCGEN05 && !multi_rs && !(cfg->flags & NPAIR_FLAG_NO_FUSED_GRAD);
-  }
-  if (!c->fused_grad) {
-    CREATE_TRY(cudaMalloc(&c->H, 2ull * ns * Q * c->Np));
-    CREATE_TRY(cudaMemset(c->H, 0, 2ull * ns * Q * c->Np));
-  }
-  // The row-record exchange needs S[j][m] on rank r to equal S[m][j] on the rank that owns row m BIT FOR BIT, i.e. a tensor-core
-  // MMA whose result does not change when the operand roles are swapped.  Checked
-  // once per process and format on this device -- if it ever fails, the reference's reduce-scatter form is used instead.
-  const bool sym_ok = c->world == 1 || cfg->bwd_exchange != NPAIR_BWD_AUTO || cfg->gemm_backend != NPAIR_GEMM_TCGEN05 || mma_is_symmetric(cfg->sim_precision, c->device);
-  c->bwd_mode = c->world == 1 ? NPAIR_BWDMODE_SINGLE
-              : ((cfg->bwd_exchange == NPAIR_BWD_AUTO && sym_ok) ? NPAIR_BWDMODE_ROW_SCALARS : NPAIR_BWDMODE_REDUCE_SCATTER);
-  if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) CREATE_TRY(cudaMalloc(&c->rs_total, sizeof(float) * 8ull * N));
-  if (c->prec != PREC_BF16 && cfg->gemm_backend == NPAIR_GEMM_TCGEN05) {
-    const size_t cat_bytes = 2ull * N * kcat_mult(c->prec) * c->Dp;
-    CREATE_TRY(cudaMalloc(&c->XcatA, cat_bytes));
-    CREATE_TRY(cudaMemset(c->XcatA, 0, cat_bytes));
-    CREATE_TRY(cudaMalloc(&c->XcatB, cat_bytes));
-    CREATE_TRY(cudaMemset(c->XcatB, 0, cat_bytes));
-  }
-  if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) {
-    CREATE_TRY(cudaMalloc(&c->XlT, 2ull * ns * D * c->Qp));
-    CREATE_TRY(cudaMemset(c->XlT, 0, 2ull * ns * D * c->Qp));
-    CREATE_TRY(cudaMalloc(&c->HT, 2ull * ns * N * c->Qp));
-    CREATE_TRY(cudaMemset(c->HT, 0, 2ull * ns * N * c->Qp));
-    CREATE_TRY(cudaMalloc(&c->OUT2, sizeof(float) * static_cast<size_t>(N) * D));
-  }
-  {
-    // split-K workspace for the gradient GEMM: at most (SMs / tiles) partial Q x D products, capped at 16
-    const int tiles = ((Q + 127) / 128) * ((D + 255) / 256);
-    int smax = c->sms / (tiles > 0 ? tiles : 1); if (smax > 16) smax = 16;
-    if (smax > 1) {
-      c->part_floats = static_cast<long long>(smax) * Q * D;
-      CREATE_TRY(cudaMalloc(&c->part, sizeof(float) * c->part_floats));
-    }
-  }
-  // row arrays: 5 uint32/int stats, 2 thr, 3 fwd, 3 hits = 13 arrays of Q 4-byte words + the [Q][8] row records
-  CREATE_TRY(cudaMalloc(&c->row_block, 4ull * 21 * Q + 64));
-  CREATE_TRY(cudaMemset(c->row_block, 0, 4ull * 21 * Q + 64));
+  const size_t* b = c->bytes;
+  CREATE_TRY(dev_alloc(&c->Xtot_buf, b[B_XTOT], false));
+  CREATE_TRY(dev_alloc(&c->labtot_buf, b[B_LABTOT], false));
+  CREATE_TRY(dev_alloc(&c->Ynorm, b[B_YNORM], false));
+  CREATE_TRY(dev_alloc(&c->dY, b[B_DY], false));
+  CREATE_TRY(dev_alloc(&c->inv_norm, b[B_INV_NORM], false));
+  CREATE_TRY(dev_alloc(&c->S, b[B_S], true));
+  CREATE_TRY(dev_alloc(&c->Xs, b[B_XS], true));
+  CREATE_TRY(dev_alloc(&c->XsT, b[B_XST], true));
+  CREATE_TRY(dev_alloc(&c->XcatA, b[B_XCAT_A], true));
+  CREATE_TRY(dev_alloc(&c->XcatB, b[B_XCAT_B], true));
+  CREATE_TRY(dev_alloc(&c->H, b[B_H], true));
+  CREATE_TRY(dev_alloc(&c->XlT, b[B_XLT], true));
+  CREATE_TRY(dev_alloc(&c->HT, b[B_HT], true));
+  CREATE_TRY(dev_alloc(&c->OUT2, b[B_OUT2], false));
+  CREATE_TRY(dev_alloc(&c->rs_total, b[B_RS_TOTAL], false));
+  CREATE_TRY(dev_alloc(&c->part, b[B_PART], false));
+  CREATE_TRY(dev_alloc(&c->row_block, b[B_ROWS], true));
+  CREATE_TRY(dev_alloc(&c->bs, b[B_BS], true));
+  CREATE_TRY(dev_alloc(&c->partial, b[B_PARTIAL], false));
+  CREATE_TRY(dev_alloc(&c->ghist, b[B_GHIST], true));
+  CREATE_TRY(dev_alloc(&c->gcand, b[B_GCAND], false));
+  CREATE_TRY(dev_alloc(&c->sym_tiles, b[B_SYM_TILES], false));
+  CREATE_TRY(dev_alloc(&c->xch_src, b[B_XCH_SRC], false));
+  CREATE_TRY(dev_alloc(&c->xch_all, b[B_XCH_ALL], false));
   {
     uint32_t* w = static_cast<uint32_t*>(c->row_block);
     RowArrays& ra = c->ra;
@@ -697,21 +751,9 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     w = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(w) + 31) & ~static_cast<uintptr_t>(31));
     ra.rowscal = reinterpret_cast<float*>(w); w += 8ll * Q;
   }
-  CREATE_TRY(cudaMalloc(&c->bs, sizeof(BlockScalars)));
-  CREATE_TRY(cudaMemset(c->bs, 0, sizeof(BlockScalars)));
-  CREATE_TRY(cudaMalloc(&c->partial, sizeof(float) * 2048));
-  CREATE_TRY(cudaMalloc(&c->ghist, sizeof(unsigned long long) * 4096));
-  CREATE_TRY(cudaMemset(c->ghist, 0, sizeof(unsigned long long) * 4096));
-  {
-    // GLOBAL relative select with a general SN: candidate lists of the chosen first-digit bucket (1/8 of the block, at most
-    // 32 M entries per side; a bigger bucket -- heavily tied data -- takes the three-sweep path)
-    const bool need = (is_rel_cfg(cfg->ap_method) && cfg->ap_region == NPAIR_GLOBAL) || (is_rel_cfg(cfg->an_method) && cfg->an_region == NPAIR_GLOBAL);
-    if (need) {
-      unsigned long long cap = static_cast<unsigned long long>(Q) * N / 8 + 4096;
-      if (cap > (32ull << 20)) cap = 32ull << 20;
-      c->gcand_cap = static_cast<unsigned int>(cap);
-      CREATE_TRY(cudaMalloc(&c->gcand, sizeof(uint32_t) * 2ull * cap));
-    }
+  if (c->sym_tiles) {
+    const std::vector<int2> tl = sym_tile_list(Q, N);
+    CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), b[B_SYM_TILES], cudaMemcpyHostToDevice));
   }
   CREATE_TRY(cudaHostAlloc(&c->tops_pinned, 64, cudaHostAllocMapped));
   memset(c->tops_pinned, 0, 64);
@@ -721,9 +763,10 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     std::string te;
     const int bks = c->bk_sim, bkg = c->bk_grad;
     bool ok = true;
-    // similarity: A = local rows of Xs, B = all rows of Xs; K = D
-    ok = ok && make_tmap_pieces(&c->tm_simA, c->Xs + static_cast<long long>(c->rank) * Q * c->Dp, D, Q, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 128, &te);
-    ok = ok && make_tmap_pieces(&c->tm_simB, c->Xs, D, N, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 256, &te);
+    if (c->Xs) {          // similarity: A = local rows of Xs, B = all rows of Xs; K = D
+      ok = ok && make_tmap_pieces(&c->tm_simA, c->Xs + static_cast<long long>(c->rank) * Q * c->Dp, D, Q, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 128, &te);
+      ok = ok && make_tmap_pieces(&c->tm_simB, c->Xs, D, N, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 256, &te);
+    }
     ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, Q, c->ldS, &te);
     // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
     if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, &te);
@@ -743,20 +786,6 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     }
     if (!ok) { g_create_err = te; npair_destroy(c); return NPAIR_E_CUDA; }
   }
-  if (c->world == 1 && cfg->gemm_backend == NPAIR_GEMM_TCGEN05 && !(cfg->flags & NPAIR_INTERNAL_FULL_TILES)) {
-    // S = X X^T is symmetric: only tiles (m_blk, n_blk) whose 256 columns reach the 128-row block's diagonal or beyond
-    std::vector<int2> tl;
-    const int tm = (Q + 127) / 128, tn = (N + 255) / 256;
-    for (int mb = 0; mb < tm; ++mb)
-      for (int nb = mb / 2; nb < tn; ++nb) tl.push_back(make_int2(mb, nb));
-    c->n_sym_tiles = static_cast<int>(tl.size());
-    CREATE_TRY(cudaMalloc(&c->sym_tiles, sizeof(int2) * tl.size()));
-    CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), sizeof(int2) * tl.size(), cudaMemcpyHostToDevice));
-  }
-  {
-    c->grad_chunk_kb = cfg->grad_chunk_cols > 0 ? (cfg->grad_chunk_cols + 31) / 32 : 64;     // default: 2048 database columns
-    if (cfg->grad_chunk_cols < 0) c->grad_chunk_kb = 0;                                        // negative: one accumulator for the whole K range (diagnostic)
-  }
   // ---- NCCL ----
   if (c->world > 1 && (id128 || ext_comm)) {
     NcclApi* api = nccl_api();
@@ -768,57 +797,45 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       c->own_comm = true;
     }
   }
-  if (c->comm && c->world > 1 && c->world <= 32 && !getenv("NPAIR_NO_P2P")) {
-    const bool want_feat = !(cfg->flags & NPAIR_FLAG_NCCL_FEATURES);
-    const bool want_rec = !(cfg->flags & NPAIR_FLAG_NCCL_RECORDS) && c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
-    if (want_feat || want_rec) {
-      // one exported region per rank; handles travel over the NCCL communicator once (a 64-byte all-gather)
-      NcclApi* api = nccl_api();
-      const int W = c->world;
-      const long long nX = static_cast<long long>(N) * D, nL = round_up(N, 4), nR = 8ll * N;
-      c->p2p_offX = 0; c->p2p_offLab = 2 * nX; c->p2p_offRec = c->p2p_offLab + 2 * nL; c->p2p_offXch = c->p2p_offRec + 2 * nR;
-      c->p2p_offFlags = c->p2p_offXch + (cfg->global_scope ? 2ll * W * NPAIR_XCH_FLOATS : 0);
-      const long long total = c->p2p_offFlags + round_up(6ll * W, 4);
-      CREATE_TRY(cudaMalloc(&c->p2p_region, sizeof(float) * static_cast<size_t>(total)));
-      CREATE_TRY(cudaMemset(c->p2p_region, 0, sizeof(float) * static_cast<size_t>(total)));
-      CREATE_TRY(cudaMalloc(&c->p2p_ticket, sizeof(unsigned int)));
-      CREATE_TRY(cudaMemset(c->p2p_ticket, 0, sizeof(unsigned int)));
-      cudaIpcMemHandle_t mine;
-      static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-      CREATE_TRY(cudaIpcGetMemHandle(&mine, c->p2p_region));
-      float *d_mine = nullptr, *d_all = nullptr;
-      CREATE_TRY(cudaMalloc(&d_mine, 64));
-      CREATE_TRY(cudaMalloc(&d_all, 64ull * W));
-      CREATE_TRY(cudaMemcpy(d_mine, &mine, 64, cudaMemcpyHostToDevice));
-      CREATE_TRY(cudaDeviceSynchronize());                       // the memset above has landed before any peer can write into the region
-      int r = api->AllGather(d_mine, d_all, 16, NCCL_FLOAT32, c->comm, nullptr);
-      if (r != 0) { g_create_err = fmt("ncclAllGather(ipc handles): %s", api->GetErrorString(r)); cudaFree(d_mine); cudaFree(d_all); npair_destroy(c); return NPAIR_E_NCCL; }
-      CREATE_TRY(cudaStreamSynchronize(nullptr));
-      std::vector<cudaIpcMemHandle_t> all(W);
-      CREATE_TRY(cudaMemcpy(all.data(), d_all, 64ull * W, cudaMemcpyDeviceToHost));
-      cudaFree(d_mine); cudaFree(d_all);
-      std::vector<float*> pb(W);
-      bool mapped = true;
-      for (int q = 0; q < W && mapped; ++q) {
-        if (q == c->rank) { pb[q] = c->p2p_region; continue; }
-        void* a = nullptr;
-        if (cudaIpcOpenMemHandle(&a, all[q], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); mapped = false; break; }
-        c->p2p_opened.push_back(a);
-        pb[q] = static_cast<float*>(a);
-      }
-      if (mapped) {
-        CREATE_TRY(cudaMalloc(&c->p2p_peer_base, sizeof(float*) * W));
-        CREATE_TRY(cudaMemcpy(c->p2p_peer_base, pb.data(), sizeof(float*) * W, cudaMemcpyHostToDevice));
-        c->p2p_feat = want_feat; c->p2p_rec = want_rec;
-      }
-      // (no peer access between some pair of GPUs: the NCCL paths are used; every rank takes the same decision only if the
-      // topology is symmetric, which holds on an NVSwitch box -- a mixed outcome is reported by the first exchange's timeout)
+  if (c->comm && b[B_P2P_REGION] && !getenv("NPAIR_NO_P2P")) {
+    // one exported region per rank; handles travel over the NCCL communicator once (a 64-byte all-gather)
+    NcclApi* api = nccl_api();
+    const int W = c->world;
+    CREATE_TRY(dev_alloc(&c->p2p_region, b[B_P2P_REGION], true));
+    CREATE_TRY(dev_alloc(&c->p2p_ticket, b[B_P2P_TICKET], true));
+    cudaIpcMemHandle_t mine;
+    static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
+    CREATE_TRY(cudaIpcGetMemHandle(&mine, c->p2p_region));
+    char* d_all = nullptr;                                     // [world] gathered handles, then this rank's own
+    CREATE_TRY(cudaMalloc(&d_all, 64ull * (W + 1)));
+    const std::unique_ptr<char, cudaError_t (*)(void*)> free_handles(d_all, cudaFree);
+    char* d_mine = d_all + 64ull * W;
+    CREATE_TRY(cudaMemcpy(d_mine, &mine, 64, cudaMemcpyHostToDevice));
+    CREATE_TRY(cudaDeviceSynchronize());                       // the memset above has landed before any peer can write into the region
+    int r = api->AllGather(d_mine, d_all, 16, NCCL_FLOAT32, c->comm, nullptr);
+    if (r != 0) { g_create_err = fmt("ncclAllGather(ipc handles): %s", api->GetErrorString(r)); npair_destroy(c); return NPAIR_E_NCCL; }
+    CREATE_TRY(cudaStreamSynchronize(nullptr));
+    std::vector<cudaIpcMemHandle_t> all(W);
+    CREATE_TRY(cudaMemcpy(all.data(), d_all, 64ull * W, cudaMemcpyDeviceToHost));
+    std::vector<float*> pb(W);
+    bool mapped = true;
+    for (int q = 0; q < W && mapped; ++q) {
+      if (q == c->rank) { pb[q] = c->p2p_region; continue; }
+      void* a = nullptr;
+      if (cudaIpcOpenMemHandle(&a, all[q], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); mapped = false; break; }
+      c->p2p_opened.push_back(a);
+      pb[q] = static_cast<float*>(a);
     }
+    if (mapped) {
+      CREATE_TRY(dev_alloc(&c->p2p_peer_base, b[B_P2P_PEERS], false));
+      CREATE_TRY(cudaMemcpy(c->p2p_peer_base, pb.data(), b[B_P2P_PEERS], cudaMemcpyHostToDevice));
+      c->p2p_feat = c->want_p2p_feat; c->p2p_rec = c->want_p2p_rec;
+    }
+    // (no peer access between some pair of GPUs: the NCCL paths are used; every rank takes the same decision only if the
+    // topology is symmetric, which holds on an NVSwitch box -- a mixed outcome is reported by the first exchange's timeout)
   }
-  if (cfg->global_scope && c->world > 1) {
-    if (!c->comm) { g_create_err = "global_scope with world > 1 needs a communicator (the world-scope reductions are internal)"; npair_destroy(c); return NPAIR_E_ARG; }
-    CREATE_TRY(cudaMalloc(&c->xch_src, sizeof(float) * NPAIR_XCH_FLOATS));
-    if (!c->p2p_region) CREATE_TRY(cudaMalloc(&c->xch_all, sizeof(float) * static_cast<size_t>(NPAIR_XCH_FLOATS) * c->world));
+  if (cfg->global_scope && c->world > 1 && !c->comm) {
+    g_create_err = "global_scope with world > 1 needs a communicator (the world-scope reductions are internal)"; npair_destroy(c); return NPAIR_E_ARG;
   }
 #undef CREATE_TRY
   *out = c;
@@ -831,21 +848,31 @@ int npair_create_with_comm(const npair_config* cfg, void* comm, npair_ctx** out)
   return create_impl(cfg, nullptr, comm, out);
 }
 
+// Peer-memory exchange of `kind`: pushes this rank's nA floats of srcA (and nB of srcB) into part partA (partB) of every rank's
+// region, in the buffers of the epoch's parity, then raises this rank's flag of (kind, parity) in every region.
+static void p2p_push(npair_ctx* c, int kind, uint32_t ep, int blocks, const float* srcA, long long nA, int partA,
+                     const float* srcB, long long nB, int partB, cudaStream_t st) {
+  const long long par = ep & 1u;
+  p2p_push_kernel<<<blocks, 256, 0, st>>>(srcA, nA, c->xl.off(partA, par, c->rank), srcB, nB, srcB ? c->xl.off(partB, par, c->rank) : 0,
+                                          c->p2p_peer_base, c->xl.flags, xchg_flag(kind, par, c->world, c->rank), c->world, ep, c->p2p_ticket);
+  count_launch();
+}
+// Waits until every rank has raised its flag of (kind, parity of ep) in this rank's region; returns the world's rows of `part`.
+static const float* p2p_wait(npair_ctx* c, int kind, uint32_t ep, int part, cudaStream_t st) {
+  const long long par = ep & 1u;
+  p2p_wait_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const uint32_t*>(c->p2p_region + c->xl.flags) + xchg_flag(kind, par, c->world, 0), c->world, ep);
+  count_launch();
+  return c->p2p_region + c->xl.off(part, par, 0);
+}
+
 // World-scope mode: every rank contributes `n` floats (in c->xch_src, or `src` copied there) and gets the world's contributions as
 // [world][NPAIR_XCH_FLOATS]; all ranks then reduce them in rank order, so decisions are identical everywhere.
 static int xchg_small(npair_ctx* c, const float* src, int n, const float** all, cudaStream_t st) {
   if (src != c->xch_src) CUDA_TRY(c, cudaMemcpyAsync(c->xch_src, src, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-  if (c->p2p_region) {
+  if (c->p2p_peer_base) {
     const uint32_t ep = ++c->xch_epoch;
-    const long long par = ep & 1u;
-    const long long off = c->p2p_offXch + (par * c->world + c->rank) * NPAIR_XCH_FLOATS;
-    int nb = (n / 4 + 255) / 256; if (nb > 8) nb = 8; if (nb < 1) nb = 1;
-    p2p_push_kernel<<<nb, 256, 0, st>>>(c->xch_src, n, off, nullptr, 0, 0, c->p2p_peer_base, c->p2p_offFlags,
-                                        4 * c->world + static_cast<int>(par) * c->world + c->rank, c->world, ep, c->p2p_ticket);
-    count_launch();
-    p2p_wait_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const uint32_t*>(c->p2p_region + c->p2p_offFlags) + 4 * c->world + par * c->world, c->world, ep);
-    count_launch();
-    *all = c->p2p_region + c->p2p_offXch + par * c->world * NPAIR_XCH_FLOATS;
+    p2p_push(c, XCHG_SMALL, ep, grid_for(n / 4, 8), c->xch_src, n, XP_XCH, nullptr, 0, XP_XCH, st);
+    *all = p2p_wait(c, XCHG_SMALL, ep, XP_XCH, st);
   } else {
     NcclApi* api = nccl_api();
     int r = api->AllGather(c->xch_src, c->xch_all, NPAIR_XCH_FLOATS, NCCL_FLOAT32, c->comm, st);
@@ -861,14 +888,13 @@ static MiningParams mining_of(const npair_config& c) {
   mp.margin_ident = c.margin_ident; mp.margin_diff = c.margin_diff; mp.identsn = c.identsn; mp.diffsn = c.diffsn;
   return mp;
 }
-static inline bool is_rel_m(int m) { return m == NPAIR_RELATIVE_HARD || m == NPAIR_RELATIVE_EASY; }
-static inline bool sn_max(float sn) { return sn >= 0.f && static_cast<int>(sn) == 0; }
 
 // The reference blocks after its forward (host reads of loss / asum, .cu:384,400).  The five tops land in mapped pinned memory followed by
 // this forward's sequence number: polling that word returns a few microseconds earlier than a stream synchronisation and does not
 // wait for anything enqueued behind the row pass (the row-record push, a backward).  A fault in a kernel never writes the number:
-// after ~2 s fall back to the synchronisation, which reports the error.
-static int wait_tops(npair_ctx* c, cudaStream_t st) {
+// after ~2 s fall back to the synchronisation, which reports the error.  Then the device error bits become the return code, and the
+// tops are copied out.
+static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
   volatile unsigned int* seqp = reinterpret_cast<volatile unsigned int*>(c->tops_pinned) + 6;
   unsigned long long spins = 0;
   while (*seqp != c->tops_seq) {
@@ -877,6 +903,10 @@ static int wait_tops(npair_ctx* c, cudaStream_t st) {
     if ((spins & 0x3FFull) == 0) sched_yield();   // ranks that share a core (fewer cores than ranks, an inherited binding) take turns quickly
   }
   __sync_synchronize();
+  const int derr = reinterpret_cast<int*>(c->tops_pinned)[5];
+  if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
+  if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
+  for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned[t] : 0.f;
   return NPAIR_OK;
 }
 
@@ -898,17 +928,10 @@ int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float
   if (c->world > 1 && c->p2p_feat) {
     PhaseTimer pt(c, 0, st);
     const uint32_t ep = ++c->p2p_fwd_epoch;
-    const long long par = ep & 1u, N = c->N;
-    const long long offX = c->p2p_offX + par * N * D + static_cast<long long>(c->rank) * Q * D;
-    const long long offL = c->p2p_offLab + par * round_up(N, 4) + static_cast<long long>(c->rank) * Q;
-    int nb = static_cast<int>((static_cast<long long>(Q) * D / 4 + 255) / 256); if (nb > 2 * c->sms) nb = 2 * c->sms; if (nb < 1) nb = 1;
-    p2p_push_kernel<<<nb, 256, 0, st>>>(d_feat, static_cast<long long>(Q) * D, offX, d_label, Q, offL, c->p2p_peer_base, c->p2p_offFlags,
-                                        static_cast<int>(par) * c->world + c->rank, c->world, ep, c->p2p_ticket);
-    count_launch();
-    p2p_wait_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const uint32_t*>(c->p2p_region + c->p2p_offFlags) + par * c->world, c->world, ep);
-    count_launch();
-    c->x_total = c->p2p_region + c->p2p_offX + par * N * D;
-    c->lab_total = c->p2p_region + c->p2p_offLab + par * round_up(N, 4);
+    const long long QD = static_cast<long long>(Q) * D;
+    p2p_push(c, XCHG_FEATURES, ep, grid_for(QD / 4, 2 * c->sms), d_feat, QD, XP_X, d_label, Q, XP_LAB, st);
+    c->x_total = p2p_wait(c, XCHG_FEATURES, ep, XP_X, st);
+    c->lab_total = c->p2p_region + c->xl.off(XP_LAB, ep & 1u, 0);
   } else if (c->world > 1) {
     if (!c->comm) { c->err = "context was created without a communicator: use npair_forward_gathered"; return NPAIR_E_STATE; }
     PhaseTimer pt(c, 0, st);
@@ -952,11 +975,9 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   // ---- operand preparation: |x| sum (top asum, .cu:400), power-of-two pre-scale, split to tensor-core pieces ----
   {
     PhaseTimer pt(c, 1, st);
-    // Xs (the un-concatenated K-major pieces) is only read by the single-pass bf16 similarity GEMM and the SIMT backend
-    uint16_t* xs_dst = (c->XcatA && c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05) ? nullptr : c->Xs;
     launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->x_total, static_cast<long long>(N) * D, c->partial,
                        c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-    launch_split(c->x_total, N, D, c->prec, c->bs, xs_dst, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    launch_split(c->x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
   }
   // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) ----
   GemmParams gp; memset(&gp, 0, sizeof(gp));
@@ -971,8 +992,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   if (c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05) {
     PhaseTimer pt(c, 2, st);
     if (c->sym_tiles) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
-    if (c->XcatA) { gp.num_kblocks = static_cast<int>(kcat_mult(c->prec) * c->Dp / 64); gp.kb_per_split = gp.num_kblocks; }
-    if (c->XcatA) {
+    if (c->cat) {
+      gp.num_kblocks = static_cast<int>(kcat_mult(c->prec) * c->Dp / 64); gp.kb_per_split = gp.num_kblocks;
       CUDA_TRY(c, launch_sim_gemm(c->prec, c->sym_tiles != nullptr, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st));
     } else
       CUDA_TRY(c, launch_sim_gemm(c->prec, c->sym_tiles != nullptr, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st));
@@ -995,8 +1016,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   {
     // general relative SN: radix selects; both sides of a region share one sweep of S
     int local_mask = 0, global_mask = 0;
-    if (is_rel_m(mp.ap_method) && !sn_max(mp.identsn)) (mp.ap_region == NPAIR_LOCAL ? local_mask : global_mask) |= 1;
-    if (is_rel_m(mp.an_method) && !sn_max(mp.diffsn)) (mp.an_region == NPAIR_LOCAL ? local_mask : global_mask) |= 2;
+    if (is_rel(mp.ap_method) && !sn_is_max(mp.identsn)) (mp.ap_region == NPAIR_LOCAL ? local_mask : global_mask) |= 1;
+    if (is_rel(mp.an_method) && !sn_is_max(mp.diffsn)) (mp.an_region == NPAIR_LOCAL ? local_mask : global_mask) |= 2;
     if (global_mask) {
       for (int pass = 0; pass < 3; ++pass) {
         launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, global_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
@@ -1026,38 +1047,18 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
       launch_tops_world(all, NPAIR_XCH_FLOATS, c->world, N, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     }
   }
-  c->rs_gathered = false;
-  // The NCCL row-record gather is enqueued at the start of npair_backward (gather_in_fwd below would place it here instead).
+  c->rs_gathered = false;          // the NCCL row-record gather is enqueued at the start of the backward
   if (c->p2p_rec && c->comm && c->x_total != nullptr && !c->ext_gathered) {
     // peer-memory exchange: push this rank's 32-byte row records to every rank now; the backward only waits for the flags
     PhaseTimer pt(c, 8, st);
     const uint32_t ep = ++c->p2p_rec_epoch;
-    const long long par = ep & 1u;
-    const long long offR = c->p2p_offRec + par * 8ll * N + 8ll * c->rank * Q;
-    int nb = (2 * Q + 255) / 256; if (nb > 64) nb = 64; if (nb < 1) nb = 1;
-    p2p_push_kernel<<<nb, 256, 0, st>>>(c->ra.rowscal, 8ll * Q, offR, nullptr, 0, 0, c->p2p_peer_base, c->p2p_offFlags,
-                                        2 * c->world + static_cast<int>(par) * c->world + c->rank, c->world, ep, c->p2p_ticket);
-    count_launch();
-  }
-  const bool gather_in_fwd = false;      // the gather stays in the backward
-  if (gather_in_fwd && !c->p2p_rec && c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS && c->comm) {
-    // The only backward exchange (8*Q floats per rank, replaces the N x D MPI_Allreduce of .cu:462-489) does not depend on
-    // the loss weight, so it is enqueued here: it runs while the host wakes up from the synchronisation below.
-    PhaseTimer pt(c, 8, st);
-    NcclApi* api = nccl_api();
-    int r = api->AllGather(c->ra.rowscal, c->rs_total, 8ull * Q, NCCL_FLOAT32, c->comm, st);
-    if (r != 0) { c->err = fmt("ncclAllGather(row records): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
-    c->rs_gathered = true;
+    p2p_push(c, XCHG_RECORDS, ep, grid_for(2ll * Q, 64), c->ra.rowscal, 8ll * Q, XP_REC, nullptr, 0, XP_REC, st);
   }
   CUDA_TRY(c, cudaGetLastError());
   if (c->defer_sync) return NPAIR_OK;              // npair_forward_backward enqueues the backward first, then waits once
-  { const int wrc = wait_tops(c, st); if (wrc != NPAIR_OK) return wrc; }
-  const int derr = reinterpret_cast<int*>(c->tops_pinned)[5];
-  if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
-  if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
-  for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned[t] : 0.f;
-  c->fwd_done = true;
-  return NPAIR_OK;
+  const int rc = finish_forward(c, tops_host, st);
+  c->fwd_done = rc == NPAIR_OK;
+  return rc;
 }
 
 static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const float* d_rs_ext, cudaStream_t st);
@@ -1103,13 +1104,9 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
   rc = backward_impl(c, loss_weight, d_diff, nullptr, nullptr, st);
   if (rc != NPAIR_OK) { c->fwd_done = false; return rc; }
   // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step
-  { const int wrc = wait_tops(c, st); if (wrc != NPAIR_OK) { c->fwd_done = false; return wrc; } }
-  const int derr = reinterpret_cast<int*>(c->tops_pinned)[5];
-  if (derr) c->fwd_done = false;
-  if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
-  if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
-  for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned[t] : 0.f;
-  return NPAIR_OK;
+  rc = finish_forward(c, tops_host, st);
+  if (rc != NPAIR_OK) c->fwd_done = false;
+  return rc;
 }
 
 /* External-collectives variant of Backward_gpu up to the all-reduce (.cu:420-460):
@@ -1147,6 +1144,13 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
   return backward_impl(c, loss_weight, d_diff, nullptr, d_rs_total, st);
 }
 
+// d_diff = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
+static void reduce_splits(npair_ctx* c, int splits, float* d_diff, float beta, cudaStream_t st) {
+  const long long n = static_cast<long long>(c->Q) * c->D;
+  splitk_reduce_kernel<<<grid_for(n / 4, 8 * c->sms), 256, 0, st>>>(c->part, splits, n, d_diff, beta);
+  count_launch();
+}
+
 static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const float* d_rs_ext, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
@@ -1164,11 +1168,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     else {
       if (c->p2p_rec && !c->ext_gathered) {
         PhaseTimer pt(c, 8, st);
-        const uint32_t ep = c->p2p_rec_epoch;
-        const long long par = ep & 1u;
-        p2p_wait_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const uint32_t*>(c->p2p_region + c->p2p_offFlags) + 2 * c->world + par * c->world, c->world, ep);
-        count_launch();
-        rs_total = c->p2p_region + c->p2p_offRec + par * 8ll * N;
+        rs_total = p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st);
       } else if (!c->rs_gathered) {
         // the only backward exchange: 8*Q floats per rank (replaces the N x D MPI_Allreduce of .cu:462-489)
         if (!c->comm) { c->err = "no communicator: use npair_backward_gathered with externally gathered row records"; return NPAIR_E_STATE; }
@@ -1184,7 +1184,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   if (tc && c->fused_grad) {
     // weights are produced inside the gradient GEMM: no H in HBM
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));
-    fp.Q = Q; fp.N = N; fp.D = D; fp.num_kblocks = (N + 31) / 32;
+    fp.Q = Q; fp.N = N; fp.D = D; fp.num_kblocks = c->grad_kblocks;
     fp.tiles_m = (Q + 127) / 128; fp.tiles_n = (D + 255) / 256;
     fp.rowrec = c->ra.rowscal; fp.colrec = rs_total ? rs_total : c->ra.rowscal;
     fp.self_offset = self_off; fp.inv_world = wscope ? 1.f : 1.f / static_cast<float>(c->world);
@@ -1192,27 +1192,12 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     fp.sgn_p = (mp.ap_method == M_EASY || mp.ap_method == M_RELATIVE_EASY) ? -1.f : 1.f;
     fp.sgn_n = (mp.an_method == M_HARD || mp.an_method == M_RELATIVE_HARD) ? -1.f : 1.f;
     fp.out = d_diff; fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
-    fp.part = c->part; fp.splits = 1; fp.kb_per_split = fp.num_kblocks;
+    fp.part = c->part; fp.splits = c->grad_split.splits; fp.kb_per_split = c->grad_split.kb_per_split;
     fp.chunk_kb = c->grad_chunk_kb;
-    if (c->part) {
-      const int tiles = fp.tiles_m * fp.tiles_n;
-      int splits = c->sms / (tiles > 0 ? tiles : 1);
-      if (splits > 16) splits = 16;
-      if (splits > fp.num_kblocks / 8) splits = fp.num_kblocks / 8;        // keep >= 8 K blocks (256 columns) per split
-      while (splits > 1 && static_cast<long long>(splits) * Q * D > c->part_floats) --splits;
-      if (splits < 1) splits = 1;
-      const int kpb = (fp.num_kblocks + splits - 1) / splits;
-      fp.splits = (fp.num_kblocks + kpb - 1) / kpb; fp.kb_per_split = kpb;
-    }
     {
       PhaseTimer pt(c, 6, st);
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
-      if (fp.splits > 1) {
-        const long long n = static_cast<long long>(Q) * D;
-        int nb = static_cast<int>((n / 4 + 255) / 256); if (nb > c->sms * 8) nb = c->sms * 8; if (nb < 1) nb = 1;
-        splitk_reduce_kernel<<<nb, 256, 0, st>>>(c->part, fp.splits, n, d_diff, 0.f);
-        count_launch();
-      }
+      if (fp.splits > 1) reduce_splits(c, fp.splits, d_diff, 0.f, st);
     }
     CUDA_TRY(c, cudaGetLastError());
     return NPAIR_OK;
@@ -1231,7 +1216,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     gp.out = d_total_ext ? d_total_ext : c->OUT2; gp.ldo = D; gp.alpha = 0.5f * (1.f / static_cast<float>(c->world)) * lw_over_q; gp.beta = 0.f;
     {
       PhaseTimer pt(c, 7, st);
-      if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, EPI_OUT, c->tm_b2A, c->tm_b2B, c->tm_S, gp, c->sms, st));
+      if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, c->tm_b2A, c->tm_b2B, c->tm_S, gp, c->sms, st));
       else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->HT, c->Qp, static_cast<long long>(N) * c->Qp, c->XlT, c->Qp, static_cast<long long>(D) * c->Qp, Q, gp, st));
     }
     if (!d_total_ext) {
@@ -1242,21 +1227,15 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     }
   }
   // d_diff = (1/2)(lw/Q) * H . X_total  (H = G + G^T/world in the symmetric modes; accumulated onto the scattered term otherwise)
-  gp.M = Q; gp.Nn = D; gp.num_kblocks = static_cast<int>((N + c->bk_grad - 1) / c->bk_grad);
+  gp.M = Q; gp.Nn = D; gp.num_kblocks = c->grad_kblocks;
   gp.tiles_m = (Q + 127) / 128; gp.tiles_n = (D + 255) / 256;
   gp.out = d_diff; gp.ldo = D; gp.alpha = 0.5f * lw_over_q; gp.beta = (rs_path && !d_total_ext) ? 1.f : 0.f;
-  gp.splits = 1; gp.kb_per_split = gp.num_kblocks; gp.part = c->part;
-  if (tc && c->part) plan_splits(&gp, c->sms, c->part_floats);
+  gp.splits = c->grad_split.splits; gp.kb_per_split = c->grad_split.kb_per_split; gp.part = c->part;
   {
     PhaseTimer pt(c, 6, st);
-    if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, EPI_OUT, c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
+    if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
     else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->H, c->Np, static_cast<long long>(Q) * c->Np, c->XsT, c->Np, static_cast<long long>(D) * c->Np, N, gp, st));
-    if (tc && gp.splits > 1) {
-      const long long n = static_cast<long long>(Q) * D;
-      int nb = static_cast<int>((n / 4 + 255) / 256); if (nb > c->sms * 8) nb = c->sms * 8; if (nb < 1) nb = 1;
-      splitk_reduce_kernel<<<nb, 256, 0, st>>>(c->part, gp.splits, n, d_diff, gp.beta);
-      count_launch();
-    }
+    if (gp.splits > 1) reduce_splits(c, gp.splits, d_diff, gp.beta, st);
   }
   CUDA_TRY(c, cudaGetLastError());
   return NPAIR_OK;
@@ -1354,16 +1333,14 @@ __global__ void cvt_f2d_kernel(const float* __restrict__ in, double* __restrict_
 int npair_util_f64_to_f32(const double* d_src, float* d_dst, size_t n, void* stream) {
   if (!d_src || !d_dst) return NPAIR_E_ARG;
   if (n == 0) return NPAIR_OK;
-  int nb = static_cast<int>((n + 255) / 256); if (nb > 148 * 16) nb = 148 * 16;
-  cvt_d2f_kernel<<<nb, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_dst, n);
+  cvt_d2f_kernel<<<grid_for(static_cast<long long>(n), 16 * NPAIR_H100_SXM_SMS), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_dst, n);
   count_launch();
   return cudaGetLastError() == cudaSuccess ? NPAIR_OK : NPAIR_E_CUDA;
 }
 int npair_util_f32_to_f64(const float* d_src, double* d_dst, size_t n, void* stream) {
   if (!d_src || !d_dst) return NPAIR_E_ARG;
   if (n == 0) return NPAIR_OK;
-  int nb = static_cast<int>((n + 255) / 256); if (nb > 148 * 16) nb = 148 * 16;
-  cvt_f2d_kernel<<<nb, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_dst, n);
+  cvt_f2d_kernel<<<grid_for(static_cast<long long>(n), 16 * NPAIR_H100_SXM_SMS), 256, 0, static_cast<cudaStream_t>(stream)>>>(d_src, d_dst, n);
   count_launch();
   return cudaGetLastError() == cudaSuccess ? NPAIR_OK : NPAIR_E_CUDA;
 }
@@ -1394,7 +1371,7 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
   uint16_t *As = nullptr, *Bs = nullptr, *dummyT = nullptr;
   BlockScalars* bs = nullptr; float* partial = nullptr;
   int rc = NPAIR_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = NPAIR_H100_SXM_SMS;
   cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 #define DG_TRY(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { g_create_err = fmt("%s: %s", #call, cudaGetErrorString(e__)); rc = NPAIR_E_CUDA; goto done; } } while (0)
   {
@@ -1434,7 +1411,7 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
       CUtensorMap ta, tb; std::string te;
       if (!make_tmap_pieces(&ta, As, K, M, ns, Kp, static_cast<long long>(M) * Kp, bk, 128, &te) ||
           !make_tmap_pieces(&tb, Bs, K, Nn, ns, Kp, static_cast<long long>(Nn) * Kp, bk, 256, &te)) { g_create_err = te; rc = NPAIR_E_CUDA; goto done; }
-      DG_TRY(launch_split_gemm(precision, EPI_OUT, ta, tb, ta, gp, sms, st));
+      DG_TRY(launch_split_gemm(precision, ta, tb, ta, gp, sms, st));
     } else {
       DG_TRY(launch_simt_gemm(precision, EPI_OUT, As, Kp, static_cast<long long>(M) * Kp, Bs, Kp, static_cast<long long>(Nn) * Kp, K, gp, st));
     }

@@ -16,7 +16,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "ptx.cuh"
 
 namespace npair {

@@ -38,7 +38,7 @@ __device__ __forceinline__ float warp_min(float v) {
   return v;
 }
 
-// split an fp32 value into 2-byte pieces (see gemm_tcgen05.cuh header)
+// split an fp32 value into 2-byte pieces (see gemm_wgmma.cuh header)
 template <int PREC>
 __device__ __forceinline__ void split3(float v, uint16_t& p0, uint16_t& p1, uint16_t& p2) {
   if (PREC == PREC_BF16) {
@@ -1777,10 +1777,6 @@ void launch_build_weights(const float* S, long long ldS, int Q, int N, const flo
 #undef NPAIR_BW_ARGS
 }
 
-__global__ void axpy_kernel(float* __restrict__ dst, const float* __restrict__ src, long long n, float a) {
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) dst[i] += a * src[i];
-}
 // --------------------------------------------------------------------------------------------
 // L2Normalize producer (usage/def.prototxt:115-120; the layer's source is not in the reference tree, so the semantics are
 // stated here): y = x / ||x||_2 per sample, a zero row stays zero; backward dx = (dy - y (y . dy)) / ||x||.
@@ -1859,12 +1855,6 @@ void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_n
 }
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st) {
   l2norm_bwd_kernel<<<(rows + 7) / 8, 256, 0, st>>>(y, inv_norm, dy, rows, dim, dx);
-  count_launch();
-}
-
-void launch_axpy_rows(float* dst, const float* src, long long n, float a, cudaStream_t st) {
-  int nb = static_cast<int>((n + 255) / 256); if (nb > 148 * 8) nb = 148 * 8; if (nb < 1) nb = 1;
-  axpy_kernel<<<nb, 256, 0, st>>>(dst, src, n, a);
   count_launch();
 }
 

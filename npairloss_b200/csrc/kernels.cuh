@@ -13,7 +13,7 @@ enum { M_HARD = 0, M_EASY = 1, M_RAND = 2, M_RELATIVE_HARD = 3, M_RELATIVE_EASY 
 // device error bits (the reference has undefined behaviour in these cases: SURVEY.md 9.4 Q5)
 enum { DERR_EMPTY_LIST = 1, DERR_POS_RANGE = 2 };
 
-// operand split formats (see gemm_tcgen05.cuh)
+// operand split formats (see gemm_wgmma.cuh)
 enum { PREC_BF16X3 = 0, PREC_BF16 = 1, PREC_FP16X2 = 2 };
 
 // Global (per-rank-block) scalars living in device memory.
@@ -116,6 +116,5 @@ void launch_build_weights(const float* S, long long ldS, int Q, int N, const flo
                           uint16_t* H, long long ldH /*Np*/, uint16_t* HT, long long ldHT /*Qp*/, cudaStream_t st);
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);
-void launch_axpy_rows(float* dst, const float* src, long long n, float a, cudaStream_t st);
 
 }  // namespace npair

@@ -24,7 +24,7 @@ __device__ __forceinline__ bool pos_index(float sn, unsigned long long size, uns
 }
 __device__ __forceinline__ float clamp_thr(float v) { return v >= 0.f ? v : -FLT_MAX; }   // .cu:288,303,319,334
 
-__device__ __forceinline__ bool is_rel(int m) { return m == M_RELATIVE_HARD || m == M_RELATIVE_EASY; }
+__host__ __device__ __forceinline__ bool is_rel(int m) { return m == M_RELATIVE_HARD || m == M_RELATIVE_EASY; }
 __host__ __device__ inline bool sn_is_max(float sn) { return sn >= 0.f && static_cast<int>(sn) == 0; }   // pos = size-1
 
 // Block-wide (or, world scope, world-wide) sizes / extrema -> GLOBAL-region thresholds and the arming of the radix selects (.cu:292-337)

@@ -76,3 +76,25 @@ def test_config_defaults_cover_the_abi2_extensions():
         c2 = capi.make_config(64, 32, **{field: bad})
         assert L.npair_workspace_bytes(C.byref(c2)) == 0, field
     assert L.npair_workspace_bytes(C.byref(capi.make_config(64, 32, normalize_input=1))) > L.npair_workspace_bytes(C.byref(capi.make_config(64, 32)))
+
+
+def _workspace(Q, D, **kw):
+    return capi.lib().npair_workspace_bytes(C.byref(capi.make_config(Q, D, **kw)))
+
+
+def test_workspace_counts_the_materialised_gradient_weights():
+    """NPAIR_FLAG_NO_FUSED_GRAD materialises the gradient weights H: ns pieces of Q x Np 2-byte values (fp16x2: ns = 2).
+    At this shape both gradient paths split K the same way, so H is the whole difference."""
+    Q, D = 4096, 512
+    ns, Np = 2, Q
+    assert _workspace(Q, D, flags=capi.FLAG_NO_FUSED_GRAD) - _workspace(Q, D) == 2 * ns * Q * Np
+
+
+@pytest.mark.parametrize("side", ["ap", "an"])
+def test_workspace_counts_the_global_select_candidates_on_every_backend(side):
+    """A GLOBAL RELATIVE_* side needs two candidate lists of cap 4-byte entries, whichever GEMM backend computes S."""
+    Q, D = 1024, 256
+    cap = min(Q * Q // 8 + 4096, 32 << 20)
+    base = dict(gemm_backend=capi.GEMM_SIMT_CHECK)
+    rel = dict(base, **{f"{side}_region": capi.GLOBAL, f"{side}_method": capi.RELATIVE_HARD})
+    assert _workspace(Q, D, **rel) - _workspace(Q, D, **base) == 8 * cap
