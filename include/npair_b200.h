@@ -99,6 +99,19 @@ enum {
   NPAIR_FLAG_LSEL_WARP = 32       /* LOCAL RELATIVE_* select: warp-per-row kernel also for rows that fit the block-per-row one */
 };
 
+/* Row-block similarity mode: flags bits 16-27 hold a block height in units of 128 rows (0 = off: the whole Q x N similarity matrix S
+ * stays in device memory from the forward to the backward).  With a height h*128 < Q the context keeps only an (h*128) x N block of S:
+ * the forward sweeps the rank's block once for the row statistics and thresholds without storing S, then recomputes S block by
+ * block for the row pass; the backward recomputes each block once more for the gradient kernel.  Tops, gradient and every per-row
+ * npair_debug_read array are bit for bit those of the materialised path.  The step costs about twice as much when a block has
+ * enough 128-row tiles to fill the GPU in the gradient kernel, more with smaller blocks (DESIGN 4.2).  A height
+ * >= Q leaves the context on the materialised path.  Accepted: tensor-core backend, fused gradient kernel, bwd_exchange AUTO,
+ * global_scope 0, and no GLOBAL RELATIVE_* side with a general SN (SN >= 0 with floor(SN) = 0, the closed-form maximum, is fine);
+ * anything else is NPAIR_E_ARG (npair_workspace_bytes returns 0).  npair_create also refuses it when the device's MMA is not
+ * bitwise symmetric (npair_debug_mma_symmetric).  npair_debug_read(which = 0) returns NPAIR_E_STATE. */
+#define NPAIR_SIM_BLOCK_SHIFT 16
+#define NPAIR_SIM_BLOCK_ROWS(rows) ((((rows) + 127) / 128) << NPAIR_SIM_BLOCK_SHIFT)
+
 enum { NPAIR_BWD_AUTO = 0, NPAIR_BWD_REDUCE_SCATTER = 1 };
 /* what a context actually uses: 0 = single rank (symmetric tiles), 1 = reduce-scatter, 2 = row-scalar exchange */
 enum { NPAIR_BWDMODE_SINGLE = 0, NPAIR_BWDMODE_REDUCE_SCATTER = 1, NPAIR_BWDMODE_ROW_SCALARS = 2 };
@@ -174,7 +187,9 @@ const char* npair_version(void);
 /* Per-phase CUDA-event timing on the caller's stream (used by bench.py for the roofline of the dominant kernel).
  * ms_out[9]: 0 forward all-gather  1 operand prep  2 similarity GEMM (+fused statistics)  3 thresholds / radix selects
  *            4 forward row pass + finalize  5 backward weight builder  6 gradient GEMM  7 transposed gradient GEMM
- *            8 backward exchange (row-scalar all-gather or reduce-scatter) */
+ *            8 backward exchange (row-scalar all-gather or reduce-scatter)
+ * Row-block similarity mode: 2 = the statistics sweep (+ fused threshold pick), 3 = 0, 4 = the forward's block recomputes, LOCAL
+ * relative selects and row passes + finalize, 6 = the backward's block recomputes and gradient kernels. */
 int npair_profile_enable(npair_ctx* ctx, int on);
 int npair_profile_read(npair_ctx* ctx, float ms_out[9]);
 /* Cumulative number of CUDA kernels this library has launched in the calling process (all contexts).  bench.py reports
@@ -187,7 +202,7 @@ int npair_util_f64_to_f32(const double* d_src, float* d_dst, size_t n, void* str
 int npair_util_f32_to_f64(const float* d_src, double* d_dst, size_t n, void* stream);
 
 /* Introspection for parity tests (copies device scratch to host; synchronises the context's last stream).
- * which: 0 = S (Q x N similarities, row-major, ld = N)      1 = posi_thr[Q]   2 = nega_thr[Q]
+ * which: 0 = S (Q x N similarities, row-major, ld = N; NPAIR_E_STATE in row-block similarity mode)      1 = posi_thr[Q]   2 = nega_thr[Q]
  *        3 = min_within[Q]  4 = max_between[Q]  5 = max_all[Q]  6 = A[Q]  7 = T[Q]  8 = same-label count[Q]
  *        9 = max_within[Q]  10 = operand pre-scale (1 float) */
 int npair_debug_read(npair_ctx* ctx, int which, float* host_dst, size_t n_floats);

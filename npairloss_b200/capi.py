@@ -27,6 +27,16 @@ class NpairConfig(C.Structure):
 
 
 FLAG_NO_FUSED_GRAD, FLAG_SIM_1CTA, FLAG_GRAD_1CTA, FLAG_NCCL_RECORDS, FLAG_NCCL_FEATURES, FLAG_LSEL_WARP = 1, 2, 4, 8, 16, 32
+# row-block similarity mode: flags bits 16-27 = block height in units of 128 rows (NPAIR_SIM_BLOCK_ROWS)
+SIM_BLOCK_SHIFT, SIM_BLOCK_MAX_UNITS = 16, 0xFFF
+
+
+def sim_block_flags(rows: int) -> int:
+    """flags bits of a row-block height of `rows` (rounded up to a multiple of 128); 0 = S materialised whole."""
+    units = (int(rows) + 127) // 128
+    if rows < 0 or units > SIM_BLOCK_MAX_UNITS:
+        raise ValueError(f"sim_block_rows must be in [0, {128 * SIM_BLOCK_MAX_UNITS}]")
+    return units << SIM_BLOCK_SHIFT
 
 
 EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_id", "npair_create", "npair_create_with_comm",
@@ -89,10 +99,12 @@ def lib():
 def make_config(Q, D, world=1, rank=0, num_tops=5, margin_ident=0.0, margin_diff=0.0, identsn=-1.0, diffsn=-1.0,
                 ap_region=LOCAL, ap_method=RAND, an_region=LOCAL, an_method=RAND, sim_precision=PREC_FP32_FP16X2,
                 gemm_backend=GEMM_TCGEN05, device=-1, bwd_exchange=0, global_scope=0, normalize_input=0, grad_chunk_cols=0,
-                flags=0) -> NpairConfig:
+                flags=0, sim_block_rows=0) -> NpairConfig:
+    """sim_block_rows > 0: row-block similarity mode with blocks of that many rows (rounded up to a multiple of 128), folded into
+    flags; the library keeps one block of the Q x N similarity matrix instead of all of it (include/npair_b200.h)."""
     return NpairConfig(Q, D, world, rank, num_tops, margin_ident, margin_diff, identsn, diffsn, ap_region, ap_method,
                        an_region, an_method, sim_precision, gemm_backend, device, bwd_exchange, global_scope, normalize_input,
-                       grad_chunk_cols, flags)
+                       grad_chunk_cols, flags | sim_block_flags(sim_block_rows))
 
 
 def nccl_unique_id() -> bytes:

@@ -176,10 +176,20 @@ static cudaError_t launch_split_gemm_t(const CUtensorMap& a, const CUtensorMap& 
   return cudaGetLastError();
 }
 // `sm`: fp32 tensor map of the similarity matrix for EPI_SIM's TMA stores (ignored by EPI_OUT: pass any valid map)
-// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.
-static cudaError_t launch_sim_gemm(int prec, bool sym_tiles, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  if (prec == PREC_FP16X2) return sym_tiles ? launch_split_gemm_t<1, false, EPI_SIM_SYM, 64>(a, b, sm, p, sms, st) : launch_split_gemm_t<1, false, EPI_SIM, 64>(a, b, sm, p, sms, st);
-  return sym_tiles ? launch_split_gemm_t<1, true, EPI_SIM_SYM, 64>(a, b, sm, p, sms, st) : launch_split_gemm_t<1, true, EPI_SIM, 64>(a, b, sm, p, sms, st);
+// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  `epi`: one of the
+// EPI_SIM* epilogues (gemm_wgmma.cuh).
+template <bool BF16>
+static cudaError_t launch_sim_gemm_t(int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
+  switch (epi) {
+    case EPI_SIM_SYM: return launch_split_gemm_t<1, BF16, EPI_SIM_SYM, 64>(a, b, sm, p, sms, st);
+    case EPI_SIM_STATS: return launch_split_gemm_t<1, BF16, EPI_SIM_STATS, 64>(a, b, sm, p, sms, st);
+    case EPI_SIM_SYM_STATS: return launch_split_gemm_t<1, BF16, EPI_SIM_SYM_STATS, 64>(a, b, sm, p, sms, st);
+    case EPI_SIM_STORE: return launch_split_gemm_t<1, BF16, EPI_SIM_STORE, 64>(a, b, sm, p, sms, st);
+    default: return launch_split_gemm_t<1, BF16, EPI_SIM, 64>(a, b, sm, p, sms, st);
+  }
+}
+static cudaError_t launch_sim_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
+  return prec == PREC_FP16X2 ? launch_sim_gemm_t<false>(epi, a, b, sm, p, sms, st) : launch_sim_gemm_t<true>(epi, a, b, sm, p, sms, st);
 }
 // Gradient GEMM: A = split gradient weights, B = split transposed features (EPI_OUT)
 static cudaError_t launch_split_gemm(int prec, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
@@ -400,6 +410,13 @@ static std::vector<int2> sym_tile_list(int Q, int N) {
   return tl;
 }
 
+// Row-block similarity mode (NPAIR_SIM_BLOCK_ROWS): the block height in rows, a multiple of 128; 0 when the mode is off or the
+// height reaches Q (the materialised path)
+static int sim_block_rows(const npair_config& c) {
+  const long long h = 128ll * ((c.flags >> NPAIR_SIM_BLOCK_SHIFT) & 0xFFF);
+  return h < c.Q ? static_cast<int>(h) : 0;
+}
+
 // device buffers of a context
 enum { B_XTOT, B_LABTOT, B_YNORM, B_DY, B_INV_NORM, B_S, B_XS, B_XST, B_XCAT_A, B_XCAT_B, B_H, B_XLT, B_HT, B_OUT2, B_RS_TOTAL,
        B_PART, B_ROWS, B_BS, B_PARTIAL, B_GHIST, B_GCAND, B_SYM_TILES, B_XCH_SRC, B_XCH_ALL, B_P2P_REGION, B_P2P_TICKET, B_P2P_PEERS,
@@ -418,6 +435,8 @@ struct Plan {
   int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
   SplitK grad_split;             // and its split-K
   int n_sym_tiles;
+  int blk_rows;                  // row-block similarity mode: rows of S kept in device memory (0: all Q rows, S materialised)
+  int s_rows;                    // rows of the S buffer
   bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
   XchgLayout xl;
   size_t bytes[B_COUNT];
@@ -431,6 +450,8 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.N = static_cast<int>(N);
   p.nsplit = nsplit_of_prec(prec); p.bk_sim = bk_of(prec, EPI_SIM); p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
+  p.blk_rows = sim_block_rows(cfg);
+  p.s_rows = p.blk_rows ? p.blk_rows : cfg.Q;
   // The row-record exchange needs S[j][m] on rank r to equal S[m][j] on the rank that owns row m BIT FOR BIT, i.e. a tensor-core
   // MMA whose result does not change when the operand roles are swapped; without one the reference's reduce-scatter form is used.
   p.bwd_mode = !multi ? NPAIR_BWDMODE_SINGLE
@@ -460,7 +481,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const size_t f = sizeof(float), ns = p.nsplit;
   if (multi) { b[B_XTOT] = f * N * D; b[B_LABTOT] = f * N; }                    // all-gather targets
   if (cfg.normalize_input) { b[B_YNORM] = b[B_DY] = f * Q * D; b[B_INV_NORM] = f * Q; }   // y, dy, 1/||x||
-  b[B_S] = f * Q * p.ldS;
+  b[B_S] = f * p.s_rows * p.ldS;
   if (!p.cat) b[B_XS] = 2 * ns * N * p.Dp;                                      // operand pieces [ns][N][Dp]
   b[B_XST] = 2 * ns * D * p.Np;                                                 // transposed pieces [ns][D][Np]
   if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * kcat_mult(prec) * p.Dp;        // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
@@ -520,6 +541,7 @@ struct npair_ctx : Plan {
   std::vector<void*> p2p_opened;
   uint32_t p2p_fwd_epoch = 0, p2p_rec_epoch = 0;
   int2* sym_tiles = nullptr;     // world == 1: (m_blk, n_blk) of the similarity tiles touching the upper triangle
+  int s_block_row0 = -1;         // row-block similarity mode: first row of the block S holds (-1: none)
   float* part = nullptr;         // split-K partial products of the gradient GEMM
   void* row_block = nullptr;     // backing store of RowArrays
   RowArrays ra;
@@ -581,6 +603,18 @@ static int validate(const npair_config* c, std::string* err) {
   if (c->grad_chunk_cols > 0 && (c->grad_chunk_cols & 31)) { *err = "grad_chunk_cols must be a multiple of 32"; return NPAIR_E_ARG; }
   if (c->global_scope && c->world > 1 && (c->bwd_exchange != NPAIR_BWD_AUTO || c->gemm_backend != NPAIR_GEMM_TCGEN05 || (c->flags & NPAIR_FLAG_NO_FUSED_GRAD))) {
     *err = "global_scope needs the row-record backward (bwd_exchange AUTO, tensor-core backend, fused gradient kernel)"; return NPAIR_E_ARG;
+  }
+  if (sim_block_rows(*c)) {
+    if (c->gemm_backend != NPAIR_GEMM_TCGEN05 || (c->flags & NPAIR_FLAG_NO_FUSED_GRAD) || c->bwd_exchange != NPAIR_BWD_AUTO) {
+      *err = "row-block similarity mode needs the tensor-core backend, the fused gradient kernel and bwd_exchange AUTO"; return NPAIR_E_ARG;
+    }
+    if (c->global_scope) { *err = "row-block similarity mode does not support global_scope"; return NPAIR_E_ARG; }
+    const bool gsel_ap = c->ap_region == NPAIR_GLOBAL && is_rel(c->ap_method) && !sn_is_max(c->identsn);
+    const bool gsel_an = c->an_region == NPAIR_GLOBAL && is_rel(c->an_method) && !sn_is_max(c->diffsn);
+    if (gsel_ap || gsel_an) {
+      *err = "row-block similarity mode: a GLOBAL RELATIVE_* side needs SN >= 0 with floor(SN) = 0 (its general-SN select sweeps the whole block)";
+      return NPAIR_E_ARG;
+    }
   }
   return NPAIR_OK;
 }
@@ -710,9 +744,17 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     npair_destroy(c); return NPAIR_E_CUDA;
   }
   c->sms = prop.multiProcessorCount;
-  // only the multi-rank row-record backward on the tensor cores depends on the check, which itself creates a single-rank context
-  const bool ask_sym = cfg->world > 1 && cfg->bwd_exchange == NPAIR_BWD_AUTO && cfg->gemm_backend == NPAIR_GEMM_TCGEN05;
-  static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, !ask_sym || mma_is_symmetric(cfg->sim_precision, c->device));
+  // only the multi-rank row-record backward on the tensor cores and the row-block similarity mode depend on the check, which itself
+  // creates a single-rank context
+  const bool blocks = sim_block_rows(*cfg) > 0;
+  const bool ask_sym = (cfg->world > 1 && cfg->bwd_exchange == NPAIR_BWD_AUTO && cfg->gemm_backend == NPAIR_GEMM_TCGEN05) || blocks;
+  const bool sym = !ask_sym || mma_is_symmetric(cfg->sim_precision, c->device);
+  if (blocks && !sym) {
+    g_create_err = "row-block similarity mode: the similarity GEMM is not bitwise symmetric on this device, so a recomputed block of S "
+                   "would not match the rows the statistics were taken from";
+    npair_destroy(c); return NPAIR_E_ARG;
+  }
+  static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym);
   c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
   const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit;
   const size_t* b = c->bytes;
@@ -767,13 +809,13 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       ok = ok && make_tmap_pieces(&c->tm_simA, c->Xs + static_cast<long long>(c->rank) * Q * c->Dp, D, Q, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 128, &te);
       ok = ok && make_tmap_pieces(&c->tm_simB, c->Xs, D, N, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 256, &te);
     }
-    ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, Q, c->ldS, &te);
+    ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, c->s_rows, c->ldS, &te);
     // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
     if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, &te);
     ok = ok && make_tmap_pieces(&c->tm_b1B, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, bkg, 256, &te);
     if (c->fused_grad) {
       ok = ok && make_tmap_pieces(&c->tm_fB, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, &te);
-      ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, Q, c->ldS, &te, 128);
+      ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, &te, 128);
     }
     if (c->XcatA) {       // bitwise-symmetric similarity: one pass over K_cat = 3*Dp (fp16x2) / 6*Dp (bf16x3)
       const long long kc = kcat_mult(c->prec) * c->Dp;
@@ -967,6 +1009,33 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
   return forward_impl(c, d_feat_total + static_cast<long long>(c->rank) * c->Q * c->D, d_label_total + static_cast<long long>(c->rank) * c->Q, tops_host, st);
 }
 
+// The per-row arrays from row r0 on, for kernels that see rows [r0, ..) as their rows [0, ..).  `hits` ([3][Q]) cannot be offset this
+// way: such kernels must not use it.
+static RowArrays rows_from(const RowArrays& ra, int r0) {
+  RowArrays v = ra;
+  v.st_minw += r0; v.st_maxw += r0; v.st_maxb += r0; v.st_maxall += r0; v.cnt_same += r0;
+  v.posi_thr += r0; v.nega_thr += r0; v.A += r0; v.T += r0; v.logv += r0;
+  v.hits = nullptr;
+  v.rowscal += 8ll * r0;
+  return v;
+}
+
+// Row-block similarity mode: rows [r0, r0 + blk_rows) of the rank's S into the S buffer (full tiles, store only).  The similarity GEMM is
+// bitwise deterministic and symmetric, so these are the bits the materialised path holds in those rows.
+static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
+  if (c->s_block_row0 == r0) return cudaSuccess;
+  const int rows = c->Q - r0 < c->blk_rows ? c->Q - r0 : c->blk_rows;
+  GemmParams gp; memset(&gp, 0, sizeof(gp));
+  gp.M = rows; gp.Nn = c->N; gp.a_row0 = r0;
+  gp.num_kblocks = static_cast<int>(c->cat ? kcat_mult(c->prec) * c->Dp / 64 : (c->D + c->bk_sim - 1) / c->bk_sim);
+  gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (c->N + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+  gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
+  const cudaError_t e = c->cat ? launch_sim_gemm(c->prec, EPI_SIM_STORE, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st)
+                               : launch_sim_gemm(c->prec, EPI_SIM_STORE, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
+  c->s_block_row0 = e == cudaSuccess ? r0 : -1;
+  return e;
+}
+
 static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
@@ -991,12 +1060,15 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   gp.fuse_thr = fuse_thr ? 1 : 0; gp.ra = c->ra; gp.mp = mp; gp.bs = c->bs;
   if (c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05) {
     PhaseTimer pt(c, 2, st);
+    // row-block mode: the same sweep without the stores (S is recomputed block by block below)
+    const int epi = c->sym_tiles ? (c->blk_rows ? EPI_SIM_SYM_STATS : EPI_SIM_SYM) : (c->blk_rows ? EPI_SIM_STATS : EPI_SIM);
+    c->s_block_row0 = -1;
     if (c->sym_tiles) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
     if (c->cat) {
       gp.num_kblocks = static_cast<int>(kcat_mult(c->prec) * c->Dp / 64); gp.kb_per_split = gp.num_kblocks;
-      CUDA_TRY(c, launch_sim_gemm(c->prec, c->sym_tiles != nullptr, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st));
+      CUDA_TRY(c, launch_sim_gemm(c->prec, epi, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st));
     } else
-      CUDA_TRY(c, launch_sim_gemm(c->prec, c->sym_tiles != nullptr, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st));
+      CUDA_TRY(c, launch_sim_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st));
   } else {
     CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_SIM, c->Xs + static_cast<long long>(self_off) * c->Dp, c->Dp, static_cast<long long>(N) * c->Dp,
                                  c->Xs, c->Dp, static_cast<long long>(N) * c->Dp, D, gp, st));
@@ -1030,16 +1102,33 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
         }
       }
     }
-    if (local_mask) launch_local_select(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, local_mask, mp.identsn, mp.diffsn, c->ra, c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
+    if (local_mask && !c->blk_rows) launch_local_select(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, local_mask, mp.identsn, mp.diffsn, c->ra, c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
   }
   }
   // ---- selection + counts + exp + masked sums + log + retrieval in one pass (.cu:343-398) ----
-  {
+  if (c->blk_rows) {
+    // row-block mode: per block of rows, recompute S, the LOCAL relative selects, the row pass; then the tops over all Q rows
+    PhaseTimer pt(c, 4, st);
+    int local_mask = 0;
+    if (is_rel(mp.ap_method) && !sn_is_max(mp.identsn)) local_mask |= 1;     // GLOBAL general-SN selects are refused by validate()
+    if (is_rel(mp.an_method) && !sn_is_max(mp.diffsn)) local_mask |= 2;
+    ++c->tops_seq;
+    for (int r0 = 0; r0 < Q; r0 += c->blk_rows) {
+      const int rows = Q - r0 < c->blk_rows ? Q - r0 : c->blk_rows;
+      CUDA_TRY(c, recompute_sim_block(c, r0, st));
+      if (local_mask)
+        launch_local_select(c->S, c->ldS, rows, N, d_label + r0, c->lab_total, self_off + r0, local_mask, mp.identsn, mp.diffsn, rows_from(c->ra, r0),
+                            c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
+      launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
+                      nullptr, c->tops_seq, r0, rows, false, st);
+    }
+    launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
+  } else {
     PhaseTimer pt(c, 4, st);
     const bool wscope = c->cfg.global_scope && c->world > 1;
     ++c->tops_seq;
     launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
-                    wscope ? c->xch_src : nullptr, c->tops_seq, st);
+                    wscope ? c->xch_src : nullptr, c->tops_seq, 0, Q, true, st);
     if (wscope) {       // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
       const float* all = nullptr;
       const int rc = xchg_small(c, c->xch_src, 8, &all, st);
@@ -1144,9 +1233,9 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
   return backward_impl(c, loss_weight, d_diff, nullptr, d_rs_total, st);
 }
 
-// d_diff = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
-static void reduce_splits(npair_ctx* c, int splits, float* d_diff, float beta, cudaStream_t st) {
-  const long long n = static_cast<long long>(c->Q) * c->D;
+// d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
+static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, float beta, cudaStream_t st) {
+  const long long n = static_cast<long long>(rows) * c->D;
   splitk_reduce_kernel<<<grid_for(n / 4, 8 * c->sms), 256, 0, st>>>(c->part, splits, n, d_diff, beta);
   count_launch();
 }
@@ -1194,10 +1283,26 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     fp.out = d_diff; fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
     fp.part = c->part; fp.splits = c->grad_split.splits; fp.kb_per_split = c->grad_split.kb_per_split;
     fp.chunk_kb = c->grad_chunk_kb;
-    {
+    if (c->blk_rows) {
+      // row-block mode: per block of rows (the one the forward left in the buffer first), recompute S, then the gradient rows.  The
+      // split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output bit is the materialised path's
+      PhaseTimer pt(c, 6, st);
+      const int nblk = (Q + c->blk_rows - 1) / c->blk_rows;
+      const int first = c->s_block_row0 >= 0 ? c->s_block_row0 / c->blk_rows : 0;
+      for (int k = 0; k < nblk; ++k) {
+        const int bi = (first + k) % nblk;
+        const int r0 = bi * c->blk_rows, rows = Q - r0 < c->blk_rows ? Q - r0 : c->blk_rows;
+        CUDA_TRY(c, recompute_sim_block(c, r0, st));
+        FusedGradParams fb = fp;
+        fb.Q = rows; fb.tiles_m = (rows + 127) / 128; fb.m_blk0 = r0 / 128;
+        fb.rowrec = c->ra.rowscal + 8ll * r0; fb.self_offset = self_off + r0; fb.out = d_diff + static_cast<long long>(r0) * D;
+        CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fb, c->sms, st));
+        if (fb.splits > 1) reduce_splits(c, fb.splits, rows, fb.out, 0.f, st);
+      }
+    } else {
       PhaseTimer pt(c, 6, st);
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
-      if (fp.splits > 1) reduce_splits(c, fp.splits, d_diff, 0.f, st);
+      if (fp.splits > 1) reduce_splits(c, fp.splits, Q, d_diff, 0.f, st);
     }
     CUDA_TRY(c, cudaGetLastError());
     return NPAIR_OK;
@@ -1235,7 +1340,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     PhaseTimer pt(c, 6, st);
     if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
     else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->H, c->Np, static_cast<long long>(Q) * c->Np, c->XsT, c->Np, static_cast<long long>(D) * c->Np, N, gp, st));
-    if (gp.splits > 1) reduce_splits(c, gp.splits, d_diff, gp.beta, st);
+    if (gp.splits > 1) reduce_splits(c, gp.splits, Q, d_diff, gp.beta, st);
   }
   CUDA_TRY(c, cudaGetLastError());
   return NPAIR_OK;
@@ -1286,6 +1391,7 @@ int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
   CUDA_TRY(c, cudaStreamSynchronize(c->last_stream));
   const int Q = c->Q, N = c->N;
   if (which == 0) {
+    if (c->blk_rows) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
     if (n < static_cast<size_t>(Q) * N) { c->err = "buffer too small"; return NPAIR_E_ARG; }
     CUDA_TRY(c, cudaMemcpy2D(dst, sizeof(float) * N, c->S, sizeof(float) * c->ldS, sizeof(float) * N, Q, cudaMemcpyDeviceToHost));
     return NPAIR_OK;

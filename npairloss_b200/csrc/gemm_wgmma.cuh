@@ -32,7 +32,14 @@ namespace npair {
 //               (tile list from the host, ~52 % of the tiles); every strictly-upper 128-column block is also written
 //               MIRRORED (second TMA store) and contributes COLUMN statistics (warp redux) to the rows it mirrors into.
 //               S comes out bitwise symmetric, which the backward weight builder relies on.
-enum { EPI_SIM = 0, EPI_OUT = 1, EPI_SIM_SYM = 2 };
+// Row-block similarity mode (S is never materialised whole, see DESIGN 4.2):
+// EPI_SIM_STATS     : EPI_SIM without the stores to S: fused row statistics (and threshold pick) only
+// EPI_SIM_SYM_STATS : EPI_SIM_SYM without the stores to S; mirrored blocks still go through the staging tile for their column statistics
+// EPI_SIM_STORE     : store-only recompute of a row block [a_row0, a_row0 + M) of S into a buffer of M rows; no statistics
+enum { EPI_SIM = 0, EPI_OUT = 1, EPI_SIM_SYM = 2, EPI_SIM_STATS = 3, EPI_SIM_SYM_STATS = 4, EPI_SIM_STORE = 5 };
+__host__ __device__ constexpr bool epi_sym(int e) { return e == EPI_SIM_SYM || e == EPI_SIM_SYM_STATS; }
+__host__ __device__ constexpr bool epi_stores_s(int e) { return e == EPI_SIM || e == EPI_SIM_SYM || e == EPI_SIM_STORE; }
+__host__ __device__ constexpr bool epi_stats(int e) { return e != EPI_OUT && e != EPI_SIM_STORE; }
 
 struct GemmParams {
   int M, Nn;           // logical output extent
@@ -64,6 +71,8 @@ struct GemmParams {
   float* out;          // [M x ldo]
   long long ldo;
   float alpha, beta;   // out = alpha*acc + beta*out
+  // ---- EPI_SIM_STORE ----
+  int a_row0;          // row of the A operand (and of the rank's S) that output row 0 stands for; a multiple of 128
 };
 
 // BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
@@ -156,6 +165,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   using Cfg = GemmCfg<NSPLIT, BK_, EPI>;
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
+  constexpr bool SYM = epi_sym(EPI), STORE = epi_stores_s(EPI), STATS = epi_stats(EPI);
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer in the shared address space (offset arithmetic, no integer round trip): LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -177,7 +187,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmapA);
     ptx::prefetch_tmap(&tmapB);
-    if (EPI != EPI_OUT) ptx::prefetch_tmap(&tmapS);
+    if (STORE) ptx::prefetch_tmap(&tmapS);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }
@@ -200,7 +210,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s) {
-            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, &full_bar[stage], kb * BK, m_blk * BM, s);
+            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, &full_bar[stage], kb * BK, m_blk * BM + (EPI == EPI_SIM_STORE ? p.a_row0 : 0), s);
             ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, &full_bar[stage], kb * BK, n_blk * BN, s);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -226,11 +236,11 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       const int row = m_blk * BM + ew * 32 + lane;
       const int col_base = n_blk * BN;
       float lab_i = 0.f;
-      if (EPI != EPI_OUT) {
+      if (STATS) {
         asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers are done with s_lab
         s_lab[et] = (col_base + et < p.Nn) ? p.lab_cols[col_base + et] : 0.f;
         if (row < p.M) lab_i = p.lab_rows[row];
-        if (EPI == EPI_SIM_SYM && half == 0) s_labr[ew * 32 + lane] = lab_i;
+        if (SYM && half == 0) s_labr[ew * 32 + lane] = lab_i;
         asm volatile("bar.sync 1, 256;" ::: "memory");
         // label range of every 32-column chunk (consumer warp w: chunk w) and of every 32-row group (warps 0..3): a row whose label
         // lies outside a chunk's range has no same-label pair in it, and its statistics reduce to one running maximum
@@ -240,7 +250,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) { mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o)); mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o)); }
           if (lane == 0) s_rng[cw] = make_float2(mn, mx);
-          if (EPI == EPI_SIM_SYM && cw < 4) {
+          if (SYM && cw < 4) {
             const float lr = s_labr[cw * 32 + lane];
             float rn = lr, rx = lr;
 #pragma unroll
@@ -332,16 +342,18 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         const int col0 = col_base + ch * 32;
         const int cb = col0 >> 7;                          // 128-wide column block (EPI_SIM_SYM bookkeeping)
         // lower-triangle half of a straddling tile: produced by mirroring
-        if ((EPI == EPI_SIM_SYM && cb < m_blk) || col0 >= p.Nn) continue;
+        if ((SYM && cb < m_blk) || col0 >= p.Nn) continue;
         float v[32];
+        if (STATS) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
-          v[4 * q] = t4.x * out_scale; v[4 * q + 1] = t4.y * out_scale; v[4 * q + 2] = t4.z * out_scale; v[4 * q + 3] = t4.w * out_scale;
+          for (int q = 0; q < 8; ++q) {
+            const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
+            v[4 * q] = t4.x * out_scale; v[4 * q + 1] = t4.y * out_scale; v[4 * q + 2] = t4.z * out_scale; v[4 * q + 3] = t4.w * out_scale;
+          }
         }
         // direct store, 4 rows x 128 bytes per instruction (whole lines); ldS is a multiple of 32, so a partial last chunk stores
         // zeros (zero-filled operand rows) into the row padding
-        {
+        if (STORE) {
           const int cq = lane & 7;
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
@@ -353,7 +365,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             if (grow < p.M) *reinterpret_cast<float4*>(p.S + static_cast<long long>(grow) * p.ldS + col0 + 4 * cq) = o;
           }
         }
-        {
+        if (STATS) {
           const float2 rg = s_rng[ch];
           // warp-uniform: every row of this warp is outside the chunk's label range (and the chunk is whole: the self pair is a
           // same-label pair, so it cannot be in such a chunk)
@@ -363,16 +375,16 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             stats32(v, s_lab + ch * 32, lab_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col,
                     minw, maxw, maxb, cnt);
         }
-        if (EPI == EPI_SIM_SYM && cb > m_blk && m_blk * BM + ew * 32 < p.M) {
+        if (SYM && cb > m_blk && m_blk * BM + ew * 32 < p.M) {
           // ---- mirrored store: staging row c holds S[col0 + c][rows of this warp]; box lands at (x = row block, y = col0) ----
-          if (lane == 0) ptx::tma_store_wait_read<0>();   // this warp's previous box has been read out of smem
+          if (STORE && lane == 0) ptx::tma_store_wait_read<0>();   // this warp's previous box has been read out of smem
           __syncwarp();
 #pragma unroll
           for (int c = 0; c < 32; ++c)
             *reinterpret_cast<float*>(stg + c * 128 + ((((lane >> 2) ^ (c & 7))) << 4) + ((lane & 3) << 2)) = v[c];
-          ptx::fence_proxy_async_smem();
+          if (STORE) ptx::fence_proxy_async_smem();
           __syncwarp();
-          if (lane == 0) { ptx::tma_store_2d(&tmapS, stg, m_blk * BM + ew * 32, col0); ptx::tma_store_commit(); }
+          if (STORE && lane == 0) { ptx::tma_store_2d(&tmapS, stg, m_blk * BM + ew * 32, col0); ptx::tma_store_commit(); }
           // ---- mirrored statistics: the staging tile is the transposed chunk, so lane L reads back ROW gc = col0 + L of the
           //      symmetric matrix (32 entries against this warp's 32 row labels) and reuses the per-thread statistics ----
           const int gc = col0 + lane;
@@ -401,7 +413,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           }
         }
       }
-      if (row < p.M) {
+      if (STATS && row < p.M) {
         maxall = fmaxf(maxw, maxb);                       // every valid column is either same- or diff-label
         if (cnt) {
           atomicMin(&p.st_minw[row], f2ord(minw));
@@ -413,9 +425,9 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       }
     }
   }
-  if (EPI != EPI_OUT && warp >= 4 && lane == 0) ptx::tma_store_wait<0>();   // bulk stores complete before exit
+  if (STORE && warp >= 4 && lane == 0) ptx::tma_store_wait<0>();   // bulk stores complete before exit
   __syncthreads();
-  if (EPI != EPI_OUT && p.fuse_thr) {
+  if (STATS && p.fuse_thr) {
     // every CTA's statistics atomics are out; the last CTA to get here picks the thresholds for the whole block of rows
     // (a static __shared__ flag would push static + dynamic shared memory past the 227 KB a CTA may ask for)
     volatile int& s_last_cta = *reinterpret_cast<volatile int*>(aux + 192);

@@ -39,6 +39,8 @@ struct FusedGradParams {
   float* out; long long ldo;
   float alpha, beta;
   const float* dev_scale;       // inverse operand pre-scale (power of two) or NULL
+  int m_blk0;                   // row-block mode: the rank's 128-row tile that local tile 0 stands for (0 otherwise).  Only the
+                                // accumulation-chunk key uses it; rowrec / out / self_offset are passed already offset
 };
 
 template <int NSPLIT>
@@ -203,7 +205,7 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
       const int mn = tile / p.splits, split = tile - mn * p.splits;
       const int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
       const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kblocks, kb0 + p.kb_per_split);
-      const int ckey = (m_blk >> 1) + n_blk + split;
+      const int ckey = ((p.m_blk0 + m_blk) >> 1) + n_blk + split;
       float* obase = p.splits > 1 ? p.part + static_cast<long long>(split) * p.Q * p.ldo : p.out;
       const float beta = p.splits > 1 ? 0.f : p.beta;
       float acc[128];

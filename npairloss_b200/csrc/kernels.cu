@@ -1407,7 +1407,62 @@ __device__ __forceinline__ void lse_elem(float sv, float lab, float li, float sc
   if (same) A += es;
 }
 
-// The last block to finish also performs the job of the old finalize kernel (loss, retrieval ratios, asum, error word).
+// Loss, retrieval ratios, asum and error word from the Q rows' results, by one block.  The summation order depends on the block
+// size only (threads stride the rows, then warps in order), so a separate launch with the same size gives the same bits.
+__device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockScalars* bs, int num_tops, float* __restrict__ tops,
+                                                   float* __restrict__ xout, unsigned int seq) {
+  const int lane = threadIdx.x & 31;
+  __shared__ double s_l[8];
+  __shared__ int s_h[3][8];
+  double ls = 0.0; int h[3] = {0, 0, 0};
+  // FU rows per thread and trip, all 4*FU loads issued before the first use: with one row per trip this tail was a chain of 32 L2
+  // latencies at Q = 8192 (~20 us of the row pass).  The per-thread summation order (r ascending) is unchanged.
+  constexpr int FU = 8;
+  for (int r0 = threadIdx.x; r0 < Q; r0 += FU * blockDim.x) {
+    float lv[FU]; int h0[FU], h1[FU], h2[FU];
+#pragma unroll
+    for (int u = 0; u < FU; ++u) {
+      const int r = r0 + u * blockDim.x;
+      const bool ok = r < Q;
+      lv[u] = ok ? __ldcg(&ra.logv[r]) : 0.f;
+      h0[u] = ok ? __ldcg(&ra.hits[r]) : 0; h1[u] = ok ? __ldcg(&ra.hits[Q + r]) : 0; h2[u] = ok ? __ldcg(&ra.hits[2 * Q + r]) : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < FU; ++u) { ls += lv[u]; h[0] += h0[u]; h[1] += h1[u]; h[2] += h2[u]; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ls += __shfl_xor_sync(0xffffffffu, ls, o);
+    h[0] += __shfl_xor_sync(0xffffffffu, h[0], o); h[1] += __shfl_xor_sync(0xffffffffu, h[1], o); h[2] += __shfl_xor_sync(0xffffffffu, h[2], o);
+  }
+  const int w = threadIdx.x >> 5;
+  if (lane == 0) { s_l[w] = ls; s_h[0][w] = h[0]; s_h[1][w] = h[1]; s_h[2][w] = h[2]; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ls = 0.0; h[0] = h[1] = h[2] = 0;
+    for (int k = 0; k < (blockDim.x >> 5); ++k) { ls += s_l[k]; h[0] += s_h[0][k]; h[1] += s_h[1][k]; h[2] += s_h[2][k]; }
+    if (xout) {        // world scope: sums only; tops_world_kernel divides by the world's N after the exchange
+      const unsigned long long lb = static_cast<unsigned long long>(__double_as_longlong(ls));
+      xout[0] = __uint_as_float(static_cast<uint32_t>(lb)); xout[1] = __uint_as_float(static_cast<uint32_t>(lb >> 32));
+      xout[2] = __int_as_float(h[0]); xout[3] = __int_as_float(h[1]); xout[4] = __int_as_float(h[2]);
+      xout[5] = bs->asum; xout[6] = __int_as_float(bs->err);
+      bs->ticket = 0;
+      return;
+    }
+    float out[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    out[0] = static_cast<float>(ls) / static_cast<float>(-Q);                       // .cu:384-385
+    for (int t = 1; t <= num_tops - 2 && t <= 3; ++t) out[t] = static_cast<float>(h[t - 1]) / static_cast<float>(Q);   // .cu:205
+    out[num_tops - 1] = bs->asum / static_cast<float>(Q);                           // .cu:400-401 (always the LAST top)
+    for (int t = 0; t < 5; ++t) tops[t] = out[t];
+    reinterpret_cast<int*>(tops)[5] = bs->err;
+    bs->ticket = 0;
+    __threadfence_system();
+    reinterpret_cast<volatile unsigned int*>(tops)[6] = seq;     // tops are visible on the host before the sequence number
+  }
+}
+
+// The last block to finish also performs the job of the old finalize kernel (loss, retrieval ratios, asum, error word), unless
+// `finalize` is 0 (row-block mode: lse_finalize_kernel runs once after the last block of rows).
 #ifndef NPAIR_LSE_U
 #define NPAIR_LSE_U 4            // 16-byte loads in flight per lane and array (S, labels)
 #endif
@@ -1420,7 +1475,9 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
                                                        int num_tops, float* __restrict__ tops, float log2_world,
                                                        float* __restrict__ xout /*world scope: this rank's partial tops, else NULL*/,
                                                        int wpr /*warps per row: 1, 2, 4 or 8 (few rows per rank: keep the SMs full)*/,
-                                                       unsigned int seq /*written behind the tops: the host polls it*/) {
+                                                       unsigned int seq /*written behind the tops: the host polls it*/,
+                                                       int row0, int rows /*rows [row0, row0 + rows) of the rank; S holds them from row 0*/,
+                                                       int finalize) {
   const int lane = threadIdx.x & 31;
   __shared__ float s_pA[8], s_pT[8];
   __shared__ int s_pc[8];
@@ -1431,15 +1488,16 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
 #endif
   const int blk = NPAIR_LSE_REV ? static_cast<int>(gridDim.x - 1 - blockIdx.x) : static_cast<int>(blockIdx.x);
   const int wib = threadIdx.x >> 5;
-  const int i = blk * ((blockDim.x >> 5) / wpr) + wib / wpr;
+  const int il = blk * ((blockDim.x >> 5) / wpr) + wib / wpr;  // row of S
+  const int i = row0 + il;                                      // row of the rank
   const int part = wib % wpr;                                   // this warp's column segment of the row
   float A = 0.f, T = 0.f; int c = 0;
   float m2 = 0.f, thr_p = 0.f, thr_n = 0.f, li = 0.f; int cs = 0;
-  if (i < Q) {
+  if (il < rows) {
     // the first block of this warp's segment is requested before anything else: the per-row set-up below (dependent loads of the row
     // statistics, the retrieval cut's expf search) then runs under the DRAM latency instead of in front of it
     constexpr int U = NPAIR_LSE_U;
-    const float* row = S + static_cast<long long>(i) * ldS;
+    const float* row = S + static_cast<long long>(il) * ldS;
     // this warp's segment [c_lo, c_hi) of the row: multiples of 512 columns
     const int seg = ((N + wpr - 1) / wpr + 128 * U - 1) / (128 * U) * (128 * U);
     const int c_lo = min(N, part * seg), c_hi = min(N, c_lo + seg);
@@ -1533,7 +1591,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
       for (int q = 0; q < wpr; ++q) { A += s_pA[wib + q]; T += s_pT[wib + q]; c += s_pc[wib + q]; }
     }
   }
-  if (i < Q && part == 0) {
+  if (il < rows && part == 0) {
     if (lane == 0) {
       ra.A[i] = A; ra.T[i] = T;                                 // T = A + B (.cu:380)
       ra.logv[i] = (A == 0.f || T == 0.f) ? 0.f : logf(A / T);  // .cu:162-169
@@ -1552,6 +1610,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
       rec[1] = make_float4(thr_p, invT - invA, invT, 0.f);
     }
   }
+  if (!finalize) return;
   // ---- grid-level completion: the last block reduces the row results (fixed order -> deterministic) ----
   __shared__ int s_last;
   __threadfence();
@@ -1560,57 +1619,14 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  __shared__ double s_l[8];
-  __shared__ int s_h[3][8];
-  double ls = 0.0; int h[3] = {0, 0, 0};
-  // FU rows per thread and trip, all 4*FU loads issued before the first use: with one row per trip this tail was a chain of 32 L2
-  // latencies at Q = 8192 (~20 us of the row pass).  The per-thread summation order (r ascending) is unchanged.
-  constexpr int FU = 8;
-  for (int r0 = threadIdx.x; r0 < Q; r0 += FU * blockDim.x) {
-    float lv[FU]; int h0[FU], h1[FU], h2[FU];
-#pragma unroll
-    for (int u = 0; u < FU; ++u) {
-      const int r = r0 + u * blockDim.x;
-      const bool ok = r < Q;
-      lv[u] = ok ? __ldcg(&ra.logv[r]) : 0.f;
-      h0[u] = ok ? __ldcg(&ra.hits[r]) : 0; h1[u] = ok ? __ldcg(&ra.hits[Q + r]) : 0; h2[u] = ok ? __ldcg(&ra.hits[2 * Q + r]) : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < FU; ++u) { ls += lv[u]; h[0] += h0[u]; h[1] += h1[u]; h[2] += h2[u]; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    ls += __shfl_xor_sync(0xffffffffu, ls, o);
-    h[0] += __shfl_xor_sync(0xffffffffu, h[0], o); h[1] += __shfl_xor_sync(0xffffffffu, h[1], o); h[2] += __shfl_xor_sync(0xffffffffu, h[2], o);
-  }
-  const int w = threadIdx.x >> 5;
-  if (lane == 0) { s_l[w] = ls; s_h[0][w] = h[0]; s_h[1][w] = h[1]; s_h[2][w] = h[2]; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    ls = 0.0; h[0] = h[1] = h[2] = 0;
-    for (int k = 0; k < (blockDim.x >> 5); ++k) { ls += s_l[k]; h[0] += s_h[0][k]; h[1] += s_h[1][k]; h[2] += s_h[2][k]; }
-    if (xout) {        // world scope: sums only; tops_world_kernel divides by the world's N after the exchange
-      const unsigned long long lb = static_cast<unsigned long long>(__double_as_longlong(ls));
-      xout[0] = __uint_as_float(static_cast<uint32_t>(lb)); xout[1] = __uint_as_float(static_cast<uint32_t>(lb >> 32));
-      xout[2] = __int_as_float(h[0]); xout[3] = __int_as_float(h[1]); xout[4] = __int_as_float(h[2]);
-      xout[5] = bs->asum; xout[6] = __int_as_float(bs->err);
-      bs->ticket = 0;
-      return;
-    }
-    float out[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    out[0] = static_cast<float>(ls) / static_cast<float>(-Q);                       // .cu:384-385
-    for (int t = 1; t <= num_tops - 2 && t <= 3; ++t) out[t] = static_cast<float>(h[t - 1]) / static_cast<float>(Q);   // .cu:205
-    out[num_tops - 1] = bs->asum / static_cast<float>(Q);                           // .cu:400-401 (always the LAST top)
-    for (int t = 0; t < 5; ++t) tops[t] = out[t];
-    reinterpret_cast<int*>(tops)[5] = bs->err;
-    bs->ticket = 0;
-    __threadfence_system();
-    reinterpret_cast<volatile unsigned int*>(tops)[6] = seq;     // tops are visible on the host before the sequence number
-  }
+  lse_finalize_block(Q, ra, bs, num_tops, tops, xout, seq);
 }
-void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, int world, float* xout,
-                     unsigned int seq, cudaStream_t st) {
+__global__ void lse_finalize_kernel(int Q, RowArrays ra, BlockScalars* bs, int num_tops, float* __restrict__ tops, unsigned int seq) {
+  lse_finalize_block(Q, ra, bs, num_tops, tops, nullptr, seq);
+}
+// Launch shape of the row pass, from the rank's row count Q (never from a row block's: the warps per row set the summation order
+// of A and T, the block size that of the finaliser).
+static void lse_shape(int Q, int N, int* wpr_out, int* threads_out) {
   // few rows per rank (anchor sharding over many GPUs): several warps share a row so that every SM still holds ~32 warps
   int wpr = 1;
   while (wpr < 8 && static_cast<long long>(Q) * wpr < 4096 && N / (2 * wpr) >= 512) wpr *= 2;
@@ -1621,21 +1637,29 @@ void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* l
 #ifdef NPAIR_LSE_WPR_FORCE      // tuning builds only
   wpr = NPAIR_LSE_WPR_FORCE;
 #endif
-  if (wpr > 1) {
-    const int rows_per_blk = 8 / wpr;
-    const int grid = (Q + rows_per_blk - 1) / rows_per_blk;
-    lse_rows_kernel<<<grid, 256, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, mp, ra, bs, num_tops, tops_dev,
-                                          xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq);
-    count_launch();
-    return;
-  }
+  *wpr_out = wpr;
+  if (wpr > 1) { *threads_out = 256; return; }
   // 8 warps per block, 4 blocks per SM.  Measured at Q = 8192 (1.73 waves): 7 warps (1.98 waves, less idle tail) is SLOWER
   // (81.3 vs 78.7 us; 6: 83.7, 5: 87.6) -- the pass is latency-bound, more resident warps win.  NPAIR_LSE_WPB overrides.
   int wpb = 8;
   while (wpb > 1 && (Q + wpb - 1) / wpb < 296) wpb >>= 1;     // keep >= 2 blocks per SM when the rank has few rows
-  const int grid = (Q + wpb - 1) / wpb;
-  lse_rows_kernel<<<grid, wpb * 32, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, mp, ra, bs, num_tops, tops_dev,
-                                             xout ? 0.f : log2f(static_cast<float>(world)), xout, 1, seq);
+  *threads_out = wpb * 32;
+}
+void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
+                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, int world, float* xout,
+                     unsigned int seq, int row0, int rows, bool finalize, cudaStream_t st) {
+  int wpr = 1, threads = 256;
+  lse_shape(Q, N, &wpr, &threads);
+  const int rows_per_blk = threads / 32 / wpr;
+  const int grid = (rows + rows_per_blk - 1) / rows_per_blk;
+  lse_rows_kernel<<<grid, threads, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, mp, ra, bs, num_tops, tops_dev,
+                                            xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq, row0, rows, finalize ? 1 : 0);
+  count_launch();
+}
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st) {
+  int wpr = 1, threads = 256;
+  lse_shape(Q, N, &wpr, &threads);
+  lse_finalize_kernel<<<1, threads, 0, st>>>(Q, ra, bs, num_tops, tops_dev, seq);
   count_launch();
 }
 

@@ -105,9 +105,13 @@ void launch_global_select_pass(const float* S, long long ldS, int Q, int N, cons
 // world scope: xall = the ranks' exchanged [2][2048] 64-bit digit counts
 void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
                           uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
+// Row pass over rows [row0, row0 + rows) of the rank (S points at row row0's similarities; lab_rows, self_offset and ra are the
+// rank's).  finalize: the last block also reduces the Q rows' results into the tops; otherwise launch_lse_finalize does, once.
 void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                      int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev /*[5]+err*/,
-                     int world, float* xout /*world scope: 7 floats of partial tops, else NULL*/, unsigned int seq, cudaStream_t st);
+                     int world, float* xout /*world scope: 7 floats of partial tops, else NULL*/, unsigned int seq, int row0, int rows,
+                     bool finalize, cudaStream_t st);
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st);
 // mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-scalar
 // exchange: rs_total = all-gathered [world][5][Q] row scalars)
 enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
