@@ -195,9 +195,14 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == 0) {
+  // Register split as in the fused gradient kernel: the producer warpgroup (warps 0-3, one working thread) keeps 40 registers, the
+  // consumers get 232 for the 128 accumulators plus the epilogue.  Every warp returns to the launch allocation (168 = 64K / 384)
+  // before the tail below, which runs on all 384 threads: the producer warpgroup takes its registers back only once both consumer
+  // warpgroups have given theirs up (named barrier 4), so the increase never waits on registers nobody will release.
+  if (warp < 4) {
     // ===================================== TMA producer =====================================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = worker; tile < num_tiles; tile += num_workers) {
         const int mn = tile / p.splits, split = tile - mn * p.splits;
@@ -217,8 +222,12 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
       }
     }
-  } else if (warp >= 4) {
+    __syncwarp();
+    asm volatile("bar.sync 4, 384;" ::: "memory");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 168;");
+  } else {
     // ===================================== consumers: MMA + epilogue =====================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = warp - 4;                      // consumer warp 0..7
     const int g = cw >> 2, wi = warp & 3;         // warpgroup (64-row half of the tile), warp rank inside it
     // epilogue view (thread = row): 32-row group ew of the tile, and which 32-column chunk of every 64-column pair
@@ -261,10 +270,17 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
 
-      // ---- main loop: this warpgroup's 64 x 256 block, fp32 accumulator in registers ----
+      // ---- main loop: this warpgroup's 64 x 256 block, fp32 accumulator in registers.  One K block of MMAs stays in flight: the
+      //      wait after committing K block kb retires kb - 1, whose stage is then released (a stage is reusable once every consumer
+      //      warp's MMAs on it retired) ----
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      auto release = [&](int st_idx) {
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[st_idx]);
+      };
+      int prev = stage;
       for (int kb = kb0; kb < kb1; ++kb) {
         ptx::mbar_wait(&full_bar[stage], phase);
         const uint32_t a0 = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES) + g * 64 * Cfg::ROW_BYTES;
@@ -282,13 +298,14 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           }
         }
         ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::fence_regs(acc);
-        // smem slot reusable once every consumer warp's MMAs on it retired
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
+        ptx::wgmma_wait<1>();
+        if (kb != kb0) release(prev);
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
+      if (kb1 > kb0) release(prev);
 
       if (EPI == EPI_OUT) {
         // fragments straight to global memory: (row, 2 consecutive columns) per register pair
@@ -424,8 +441,11 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         atomicMax(&p.st_maxall[row], f2ord(maxall));
       }
     }
+    if (STORE && lane == 0) ptx::tma_store_wait<0>();   // bulk stores complete before exit
+    __syncwarp();
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 168;");
+    asm volatile("bar.arrive 4, 384;" ::: "memory");
   }
-  if (STORE && warp >= 4 && lane == 0) ptx::tma_store_wait<0>();   // bulk stores complete before exit
   __syncthreads();
   if (STATS && p.fuse_thr) {
     // every CTA's statistics atomics are out; the last CTA to get here picks the thresholds for the whole block of rows

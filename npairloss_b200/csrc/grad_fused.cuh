@@ -111,25 +111,28 @@ struct RowRec { float m2r, tn, m2, lab, tp, cA; int self_col; };
 // Weight of the pair (row, column m): two exponentials whose arguments already carry the factors 1/T (and 1/world for the
 // transposed term) -- see lse_rows_kernel -- switched off by a -inf argument when the pair is not selected.  Same-label pairs use
 // the positive rule and weights; the self pair and columns beyond N weigh nothing.
-__device__ __forceinline__ float pair_weight(float s, const float4* __restrict__ rec, const RowRec& r, int m, const FusedGradParams& p) {
-  float g;
-  const float4 ca = rec[0];
-  if (ca.w != r.lab) {                           // {m2c, thr_n, m2, label} of the column's row
-    const float key = s * p.sgn_n;               // HARD / RELATIVE_HARD negatives compare -s
-    float e1, e2;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(key <= r.tn ? fmaf(s, NPAIR_LOG2E_F, -r.m2r) : -INFINITY));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(key <= ca.y ? fmaf(s, NPAIR_LOG2E_F, -ca.x) : -INFINITY));
-    g = e1 + e2;
-  } else {
-    const float4 cb = rec[1];                    // {thr_p, cA, cT, -}
-    float e1, e2;                                // same exponential as the forward row pass (fast_exp_m2)
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(s, NPAIR_LOG2E_F, -r.m2)));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(fmaf(s, NPAIR_LOG2E_F, -ca.z)));
-    const float key = s * p.sgn_p;
-    const float w1 = (key <= r.tp) ? e1 * r.cA : 0.f;
-    const float w2 = (key <= cb.x) ? e2 * cb.y : 0.f;
-    g = fmaf(w2, p.inv_world, w1);
-  }
+// Branch-free: the label test selects the two exponentials' arguments and then the result, so the eight weights of a K step form
+// independent straight-line chains that the scheduler interleaves (a branch per weight serialised their shared-memory and MUFU
+// latencies, and with two consumer warps per scheduler nothing else hid them).  Each case performs exactly the operations it would
+// on its own.  The selects are PTX selp: written as C conditionals, the compiler turned them back into branches.
+__device__ __forceinline__ float select_f32(bool c, float a, float b) {
+  float r;
+  asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"(static_cast<int>(c)));
+  return r;
+}
+__device__ __forceinline__ float pair_weight(float s, const float4& ca, const float4& cb, const RowRec& r, int m, const FusedGradParams& p) {
+  // ca = {m2c, thr_n, m2, label}, cb = {thr_p, cA, cT, -} of the column's row
+  const bool same = !(ca.w != r.lab);
+  const float kn = s * p.sgn_n;                  // HARD / RELATIVE_HARD negatives compare -s
+  const float a1 = select_f32(same, fmaf(s, NPAIR_LOG2E_F, -r.m2), select_f32(kn <= r.tn, fmaf(s, NPAIR_LOG2E_F, -r.m2r), -INFINITY));
+  const float a2 = select_f32(same, fmaf(s, NPAIR_LOG2E_F, -ca.z), select_f32(kn <= ca.y, fmaf(s, NPAIR_LOG2E_F, -ca.x), -INFINITY));
+  float e1, e2;                                  // same-label: the forward row pass's exponential (fast_exp_m2)
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(a2));
+  const float kp = s * p.sgn_p;
+  const float w1 = select_f32(kp <= r.tp, e1 * r.cA, 0.f);
+  const float w2 = select_f32(kp <= cb.x, e2 * cb.y, 0.f);
+  const float g = select_f32(same, fmaf(w2, p.inv_world, w1), e1 + e2);
   return (m == r.self_col || m >= p.N) ? 0.f : g;
 }
 
@@ -196,11 +199,45 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
     }
   } else {
     // ===================================== consumers: weights -> wgmma -> drain =====================================
+    // Software pipeline over the 16-wide K steps of a chunk: step i's MMAs run from A buffer i & 1 while the weights of step i + 1
+    // are built into the other one, after wgmma.wait_group 1 has retired step i - 1 (the previous reader of that buffer).  A stage
+    // is released once the last MMA reading it has retired, so a warp holds at most two stages (the one in flight and the one being
+    // built) and the producer keeps STAGES - 2 stages of lead (2 at fp16x2, 1 at bf16x3, 4 at bf16).
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    constexpr int KSTEPS = BK / 16;
+    static_assert(KSTEPS % 2 == 0, "a K block's first step must use A buffer 0");
     const int g = warp >> 2, wi = warp & 3;
     const int c4 = lane & 3;
     const int rl0 = g * 64 + wi * 16 + (lane >> 2);  // tile rows of this thread's fragment: rl0, rl0 + 8
     int stage = 0; uint32_t phase = 0;
+    // A fragment of K step k2 of K block kb (in ring stage `st_idx`): columns 16*k2 + 2*c4 + {0, 1} (t = 0) and + 8 (t = 1),
+    // rows rl0 (h = 0) and rl0 + 8 (h = 1)
+    auto build = [&](uint32_t (&af)[NSPLIT][4], const RowRec (&rr)[2], int st_idx, int kb, int k2) {
+      const uint8_t* s_tile = smem + st_idx * Cfg::STAGE_BYTES + NSPLIT * Cfg::B_PIECE;
+      const float4* crec = reinterpret_cast<const float4*>(s_tile + Cfg::S_TILE);
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        const int k = 16 * k2 + 8 * t + 2 * c4;
+        const int m = kb * BK + k;
+        // records of columns m and m + 1, shared by both rows
+        const float4 ca0 = crec[2 * k], cb0 = crec[2 * k + 1], ca1 = crec[2 * k + 2], cb1 = crec[2 * k + 3];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rl = rl0 + 8 * h;
+          const float2 s2 = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
+          const float w0 = pair_weight(s2.x, ca0, cb0, rr[h], m, p);
+          const float w1 = pair_weight(s2.y, ca1, cb1, rr[h], m + 1, p);
+          uint32_t o[3];
+          split_pair<NSPLIT, BF16>(w0, w1, o);
+#pragma unroll
+          for (int s = 0; s < NSPLIT; ++s) af[s][2 * t + h] = o[s];
+        }
+      }
+    };
+    auto release = [&](int st_idx) {
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty_bar[st_idx]);
+    };
     for (int tile = worker; tile < num_tiles; tile += num_workers) {
       const int mn = tile / p.splits, split = tile - mn * p.splits;
       const int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
@@ -208,55 +245,45 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
       const int ckey = ((p.m_blk0 + m_blk) >> 1) + n_blk + split;
       float* obase = p.splits > 1 ? p.part + static_cast<long long>(split) * p.Q * p.ldo : p.out;
       const float beta = p.splits > 1 ? 0.f : p.beta;
+      RowRec rr[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) rr[h] = load_rowrec(p, m_blk * BM + rl0 + 8 * h);
       float acc[128];
+      uint32_t af[2][NSPLIT][4];
       for (int c0 = kb0, c1; c0 < kb1; c0 = c1) {
         c1 = chunk_end(c0, kb0, kb1, p.chunk_kb, ckey);
+        ptx::mbar_wait(&full_bar[stage], phase);
+        build(af[0], rr, stage, c0, 0);
+        int prev = stage;
         for (int kb = c0; kb < c1; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          uint8_t* st = smem + stage * Cfg::STAGE_BYTES;
-          const uint8_t* s_tile = st + NSPLIT * Cfg::B_PIECE;
-          const float4* crec = reinterpret_cast<const float4*>(s_tile + Cfg::S_TILE);
-          const uint32_t b0 = ptx::smem_u32(st);
+          const int cur = stage;
+          const uint32_t b0 = ptx::smem_u32(smem + cur * Cfg::STAGE_BYTES);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
 #pragma unroll
-          for (int k2 = 0; k2 < BK / 16; ++k2) {
-            // fragment columns 16*k2 + 2*c4 + {0, 1} (t = 0) and + 8 (t = 1), rows rl0 (h = 0) and rl0 + 8 (h = 1)
-            uint32_t af[NSPLIT][4];
-            // row records are re-read (L1) at every step rather than kept in registers next to the 128 accumulators
-            RowRec rr[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) rr[h] = load_rowrec(p, m_blk * BM + rl0 + 8 * h);
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              const int k = 16 * k2 + 8 * t + 2 * c4;
-              const int m = kb * BK + k;
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int rl = rl0 + 8 * h;
-                const float2 s2 = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
-                const float w0 = pair_weight(s2.x, crec + 2 * k, rr[h], m, p);
-                const float w1 = pair_weight(s2.y, crec + 2 * k + 2, rr[h], m + 1, p);
-                uint32_t o[3];
-                split_pair<NSPLIT, BF16>(w0, w1, o);
-#pragma unroll
-                for (int s = 0; s < NSPLIT; ++s) af[s][2 * t + h] = o[s];
-              }
-            }
+          for (int k2 = 0; k2 < KSTEPS; ++k2) {
             ptx::wgmma_fence();
 #pragma unroll
             for (int ps = 0; ps < Cfg::NPASS; ++ps) {
               int sa, sb;
               pass_pieces(NSPLIT, ps, sa, sb);
               const uint64_t bd = ptx::make_kmajor_desc(b0 + sb * Cfg::B_PIECE + k2 * 32, 512u, 2u);   // SWIZZLE_64B, 8 rows = 512 B
-              ptx::wgmma_m64n256k16_rs<BF16>(acc, af[sa], bd, ((kb - c0) | ps | k2) != 0 ? 1u : 0u);
+              ptx::wgmma_m64n256k16_rs<BF16>(acc, af[k2 & 1][sa], bd, ((kb - c0) | ps | k2) != 0 ? 1u : 0u);
             }
             ptx::wgmma_commit();
-            ptx::wgmma_wait<0>();                  // the A registers are rewritten by the next step
-            ptx::fence_regs(acc);
+            ptx::wgmma_wait<1>();                  // the previous step retired: its A buffer is free, and so is its stage
+            if (k2 == 0 && kb != c0) release(prev);
+            if (k2 + 1 < KSTEPS) {
+              build(af[(k2 + 1) & 1], rr, cur, kb, k2 + 1);
+            } else if (kb + 1 < c1) {
+              ptx::mbar_wait(&full_bar[stage], phase);
+              build(af[0], rr, stage, kb + 1, 0);
+            }
           }
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          prev = cur;
         }
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc);
+        release(prev);
         // drain the chunk: first chunk of the tile stores (+ beta * out), later chunks add (fp32 RN)
         const bool first = (c0 == kb0);
 #pragma unroll
