@@ -159,64 +159,63 @@ static inline int bk_of(int prec, int epi) {
 }
 static inline int kcat_mult(int prec) { return prec == PREC_FP16X2 ? 3 : (prec == PREC_BF16X3 ? 6 : 1); }
 
+// A GEMM kernel instantiation with its launch shape.  Its dynamic shared memory exceeds the default limit, so every device that
+// launches it has to allow that much first (allow_smem).
+struct GemmKernel { void (*fn)(CUtensorMap, CUtensorMap, CUtensorMap, GemmParams); int threads, smem; };
+struct FusedKernel { void (*fn)(CUtensorMap, CUtensorMap, FusedGradParams); int threads, smem; };
+template <class K>
+static cudaError_t allow_smem(const K& k) {
+  return k.fn ? cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem) : cudaErrorInvalidValue;
+}
+
 template <int NSPLIT, bool BF16, int EPI, int BK>
-static cudaError_t launch_split_gemm_t(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
+static GemmKernel gemm_t() {
   using Cfg = GemmCfg<NSPLIT, BK, EPI>;
-  auto kern = split_gemm_kernel<NSPLIT, BF16, EPI, BK>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
+  return GemmKernel{split_gemm_kernel<NSPLIT, BF16, EPI, BK>, Cfg::THREADS, Cfg::SMEM_BYTES};
+}
+// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  Only the
+// epilogues the host composes are instantiated.
+template <bool BF16>
+static GemmKernel sim_gemm_t(int epi) {
+  switch (epi) {
+    case EPI_STORE_S | EPI_STATS: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS, 64>();
+    case EPI_STORE_S | EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS | EPI_SYM, 64>();
+    case EPI_STATS: return gemm_t<1, BF16, EPI_STATS, 64>();
+    case EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STATS | EPI_SYM, 64>();
+    case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
+    default: return GemmKernel{nullptr, 0, 0};
   }
+}
+// `epi`: EPI_OUT for the gradient GEMM (A = split gradient weights, B = split transposed features), else a similarity epilogue
+static GemmKernel gemm_kernel(int prec, int epi) {
+  if (epi != EPI_OUT) return prec == PREC_FP16X2 ? sim_gemm_t<false>(epi) : sim_gemm_t<true>(epi);
+  if (prec == PREC_BF16) return gemm_t<1, true, EPI_OUT, 64>();
+  if (prec == PREC_FP16X2) return gemm_t<2, false, EPI_OUT, 32>();
+  return gemm_t<3, true, EPI_OUT, 32>();
+}
+// `sm`: fp32 tensor map of the similarity matrix for EPI_STORE_S's TMA stores (ignored otherwise: pass any valid map)
+static cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
+  const GemmKernel k = gemm_kernel(prec, epi);
+  if (!k.fn) return cudaErrorInvalidValue;
   const int tiles = p.tile_list ? p.num_tiles_list : p.tiles_m * p.tiles_n * p.splits;
-  const int grid = tiles < sms ? tiles : sms;
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(a, b, sm, p);
+  k.fn<<<tiles < sms ? tiles : sms, k.threads, k.smem, st>>>(a, b, sm, p);
   count_launch();
   return cudaGetLastError();
-}
-// `sm`: fp32 tensor map of the similarity matrix for EPI_SIM's TMA stores (ignored by EPI_OUT: pass any valid map)
-// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  `epi`: one of the
-// EPI_SIM* epilogues (gemm_wgmma.cuh).
-template <bool BF16>
-static cudaError_t launch_sim_gemm_t(int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  switch (epi) {
-    case EPI_SIM_SYM: return launch_split_gemm_t<1, BF16, EPI_SIM_SYM, 64>(a, b, sm, p, sms, st);
-    case EPI_SIM_STATS: return launch_split_gemm_t<1, BF16, EPI_SIM_STATS, 64>(a, b, sm, p, sms, st);
-    case EPI_SIM_SYM_STATS: return launch_split_gemm_t<1, BF16, EPI_SIM_SYM_STATS, 64>(a, b, sm, p, sms, st);
-    case EPI_SIM_STORE: return launch_split_gemm_t<1, BF16, EPI_SIM_STORE, 64>(a, b, sm, p, sms, st);
-    default: return launch_split_gemm_t<1, BF16, EPI_SIM, 64>(a, b, sm, p, sms, st);
-  }
-}
-static cudaError_t launch_sim_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  return prec == PREC_FP16X2 ? launch_sim_gemm_t<false>(epi, a, b, sm, p, sms, st) : launch_sim_gemm_t<true>(epi, a, b, sm, p, sms, st);
-}
-// Gradient GEMM: A = split gradient weights, B = split transposed features (EPI_OUT)
-static cudaError_t launch_split_gemm(int prec, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  if (prec == PREC_BF16) return launch_split_gemm_t<1, true, EPI_OUT, 64>(a, b, sm, p, sms, st);
-  if (prec == PREC_FP16X2) return launch_split_gemm_t<2, false, EPI_OUT, 32>(a, b, sm, p, sms, st);
-  return launch_split_gemm_t<3, true, EPI_OUT, 32>(a, b, sm, p, sms, st);
 }
 
 template <int NSPLIT, bool BF16>
-static cudaError_t launch_fused_grad_t(const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
-  using Cfg = FusedCfg<NSPLIT>;
-  auto kern = fused_grad_kernel<NSPLIT, BF16>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  const int tiles = p.tiles_m * p.tiles_n * p.splits;
-  kern<<<tiles < sms ? tiles : sms, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(b, sm, p);
-  count_launch();
-  return cudaGetLastError();
+static FusedKernel fused_t() { return FusedKernel{fused_grad_kernel<NSPLIT, BF16>, FusedCfg<NSPLIT>::THREADS, FusedCfg<NSPLIT>::SMEM_BYTES}; }
+static FusedKernel fused_kernel(int prec) {
+  if (prec == PREC_BF16) return fused_t<1, true>();
+  if (prec == PREC_FP16X2) return fused_t<2, false>();
+  return fused_t<3, true>();
 }
 static cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
-  if (prec == PREC_BF16) return launch_fused_grad_t<1, true>(b, sm, p, sms, st);
-  if (prec == PREC_FP16X2) return launch_fused_grad_t<2, false>(b, sm, p, sms, st);
-  return launch_fused_grad_t<3, true>(b, sm, p, sms, st);
+  const FusedKernel k = fused_kernel(prec);
+  const int tiles = p.tiles_m * p.tiles_n * p.splits;
+  k.fn<<<tiles < sms ? tiles : sms, k.threads, k.smem, st>>>(b, sm, p);
+  count_launch();
+  return cudaGetLastError();
 }
 
 // SIMT cross-check of the same contraction on the same split operands (tests only; NPAIR_GEMM_SIMT_CHECK).
@@ -227,7 +226,8 @@ __device__ __forceinline__ float piece_sum(const uint16_t* base, long long off, 
   return __bfloat162float(__ushort_as_bfloat16(base[off])) + __bfloat162float(__ushort_as_bfloat16(base[ps + off])) +
          __bfloat162float(__ushort_as_bfloat16(base[2 * ps + off]));
 }
-template <int PREC, int EPI>
+// OUT = 1: the gradient GEMM's EPI_OUT epilogue; OUT = 0: the similarity store
+template <int PREC, int OUT>
 __global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restrict__ A, long long lda, long long psA,
                                                         const uint16_t* __restrict__ B, long long ldb, long long psB, int K, GemmParams p) {
   __shared__ float As[16][65], Bs[16][65];
@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restri
     for (int j = 0; j < 4; ++j) {
       const int col = n0 + tx * 4 + j;
       if (col >= p.Nn) continue;
-      if (EPI == EPI_SIM) p.S[static_cast<long long>(row) * p.ldS + col] = acc[i][j] * inv * inv;
+      if (!OUT) p.S[static_cast<long long>(row) * p.ldS + col] = acc[i][j] * inv * inv;
       else {
         float* d = p.out + static_cast<long long>(row) * p.ldo + col;
         float o = p.alpha * inv * acc[i][j];
@@ -271,13 +271,14 @@ __global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restri
     }
   }
 }
+// `epi`: EPI_OUT, or EPI_STORE_S for the similarity matrix
 static cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long long lda, long long psA, const uint16_t* B, long long ldb,
                                     long long psB, int K, const GemmParams& p, cudaStream_t st) {
   dim3 grid((p.Nn + 63) / 64, (p.M + 63) / 64);
 #define NPAIR_SIMT(P)                                                                                   \
   do {                                                                                                  \
-    if (epi == EPI_SIM) simt_gemm_kernel<P, EPI_SIM><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p); \
-    else simt_gemm_kernel<P, EPI_OUT><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);                \
+    if (epi == EPI_OUT) simt_gemm_kernel<P, 1><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);   \
+    else simt_gemm_kernel<P, 0><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);                  \
   } while (0)
   if (prec == PREC_BF16) NPAIR_SIMT(PREC_BF16);
   else if (prec == PREC_FP16X2) NPAIR_SIMT(PREC_FP16X2);
@@ -417,6 +418,13 @@ static int sim_block_rows(const npair_config& c) {
   return h < c.Q ? static_cast<int>(h) : 0;
 }
 
+// The sides of `region` (NPAIR_LOCAL / NPAIR_GLOBAL) that need a radix select: bit 0 AP, bit 1 AN.  A RELATIVE_* side needs one
+// unless its SN picks the list's maximum (sn_is_max), which the threshold pick already has.
+static int select_mask(const npair_config& c, int region) {
+  return (c.ap_region == region && is_rel(c.ap_method) && !sn_is_max(c.identsn) ? 1 : 0) |
+         (c.an_region == region && is_rel(c.an_method) && !sn_is_max(c.diffsn) ? 2 : 0);
+}
+
 // device buffers of a context
 enum { B_XTOT, B_LABTOT, B_YNORM, B_DY, B_INV_NORM, B_S, B_XS, B_XST, B_XCAT_A, B_XCAT_B, B_H, B_XLT, B_HT, B_OUT2, B_RS_TOTAL,
        B_PART, B_ROWS, B_BS, B_PARTIAL, B_GHIST, B_GCAND, B_SYM_TILES, B_XCH_SRC, B_XCH_ALL, B_P2P_REGION, B_P2P_TICKET, B_P2P_PEERS,
@@ -435,8 +443,12 @@ struct Plan {
   int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
   SplitK grad_split;             // and its split-K
   int n_sym_tiles;
-  int blk_rows;                  // row-block similarity mode: rows of S kept in device memory (0: all Q rows, S materialised)
-  int s_rows;                    // rows of the S buffer
+  int s_rows;                    // rows of the S buffer: all Q (S materialised), or one block in row-block similarity mode
+  int n_blocks;                  // blocks of s_rows rows that the row pass and the fused gradient walk; 1: S materialised
+  int sweep_epi;                 // the forward's similarity sweep: statistics, + symmetric tiles, + stores to S if there is one block
+  bool fuse_thr;                 // the threshold pick runs in the sweep's last CTA (not in world scope: it needs the world's statistics)
+  bool wscope;                   // world-scope mode: global_scope at world > 1
+  int lsel_mask, gsel_mask;      // radix selects (select_mask) of the LOCAL / GLOBAL region
   bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
   XchgLayout xl;
   size_t bytes[B_COUNT];
@@ -448,10 +460,15 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const long long Q = cfg.Q, D = cfg.D, N = Q * W;
   const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
   p.N = static_cast<int>(N);
-  p.nsplit = nsplit_of_prec(prec); p.bk_sim = bk_of(prec, EPI_SIM); p.bk_grad = bk_of(prec, EPI_OUT);
+  p.nsplit = nsplit_of_prec(prec); p.bk_sim = bk_of(prec, EPI_STORE_S); p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
-  p.blk_rows = sim_block_rows(cfg);
-  p.s_rows = p.blk_rows ? p.blk_rows : cfg.Q;
+  const int blk_rows = sim_block_rows(cfg);
+  p.s_rows = blk_rows ? blk_rows : cfg.Q;
+  p.n_blocks = (cfg.Q + p.s_rows - 1) / p.s_rows;
+  p.wscope = cfg.global_scope && multi;
+  p.fuse_thr = tc && !p.wscope;
+  p.lsel_mask = select_mask(cfg, NPAIR_LOCAL);
+  p.gsel_mask = select_mask(cfg, NPAIR_GLOBAL);
   // The row-record exchange needs S[j][m] on rank r to equal S[m][j] on the rank that owns row m BIT FOR BIT, i.e. a tensor-core
   // MMA whose result does not change when the operand roles are swapped; without one the reference's reduce-scatter form is used.
   p.bwd_mode = !multi ? NPAIR_BWDMODE_SINGLE
@@ -459,9 +476,9 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const bool rs = p.bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER;
   p.fused_grad = tc && !rs && !(cfg.flags & NPAIR_FLAG_NO_FUSED_GRAD);
   p.cat = tc && prec != PREC_BF16;
-  // GLOBAL relative select with a general SN: candidate lists of the chosen first-digit bucket (1/8 of the block, at most
-  // 32 M entries per side; a bigger bucket -- heavily tied data -- takes the three-sweep path)
-  if ((is_rel(cfg.ap_method) && cfg.ap_region == NPAIR_GLOBAL) || (is_rel(cfg.an_method) && cfg.an_region == NPAIR_GLOBAL)) {
+  // GLOBAL radix select: candidate lists of the chosen first-digit bucket (1/8 of the block, at most 32 M entries per side; a
+  // bigger bucket -- heavily tied data -- takes the three-sweep path)
+  if (p.gsel_mask) {
     const long long cap = Q * N / 8 + 4096;
     p.gcand_cap = static_cast<unsigned int>(cap < (32ll << 20) ? cap : (32ll << 20));
   }
@@ -472,10 +489,10 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const int tiles = static_cast<int>(((Q + 127) / 128) * ((D + 255) / 256));
   p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
   if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_list(cfg.Q, p.N).size());
+  p.sweep_epi = EPI_STATS | (p.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
   p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
   p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
-  const bool wscope = cfg.global_scope && multi;
-  if (p.want_p2p_feat || p.want_p2p_rec) p.xl = xchg_layout(cfg.Q, cfg.D, W, wscope);
+  if (p.want_p2p_feat || p.want_p2p_rec) p.xl = xchg_layout(cfg.Q, cfg.D, W, p.wscope);
 
   size_t* b = p.bytes;
   const size_t f = sizeof(float), ns = p.nsplit;
@@ -495,7 +512,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   b[B_GHIST] = sizeof(unsigned long long) * 4096;
   b[B_GCAND] = sizeof(uint32_t) * 2ull * p.gcand_cap;
   b[B_SYM_TILES] = sizeof(int2) * p.n_sym_tiles;
-  if (wscope) { b[B_XCH_SRC] = f * NPAIR_XCH_FLOATS; b[B_XCH_ALL] = f * NPAIR_XCH_FLOATS * W; }   // the latter for NCCL
+  if (p.wscope) { b[B_XCH_SRC] = f * NPAIR_XCH_FLOATS; b[B_XCH_ALL] = f * NPAIR_XCH_FLOATS * W; }   // the latter for NCCL
   if (p.want_p2p_feat || p.want_p2p_rec) {
     b[B_P2P_REGION] = f * p.xl.floats; b[B_P2P_TICKET] = sizeof(unsigned int); b[B_P2P_PEERS] = sizeof(float*) * W;
   }
@@ -609,9 +626,7 @@ static int validate(const npair_config* c, std::string* err) {
       *err = "row-block similarity mode needs the tensor-core backend, the fused gradient kernel and bwd_exchange AUTO"; return NPAIR_E_ARG;
     }
     if (c->global_scope) { *err = "row-block similarity mode does not support global_scope"; return NPAIR_E_ARG; }
-    const bool gsel_ap = c->ap_region == NPAIR_GLOBAL && is_rel(c->ap_method) && !sn_is_max(c->identsn);
-    const bool gsel_an = c->an_region == NPAIR_GLOBAL && is_rel(c->an_method) && !sn_is_max(c->diffsn);
-    if (gsel_ap || gsel_an) {
+    if (select_mask(*c, NPAIR_GLOBAL)) {
       *err = "row-block similarity mode: a GLOBAL RELATIVE_* side needs SN >= 0 with floor(SN) = 0 (its general-SN select sweeps the whole block)";
       return NPAIR_E_ARG;
     }
@@ -800,8 +815,13 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   CREATE_TRY(cudaHostAlloc(&c->tops_pinned, 64, cudaHostAllocMapped));
   memset(c->tops_pinned, 0, 64);
   CREATE_TRY(cudaHostGetDevicePointer(&c->tops_dev, c->tops_pinned, 0));
-  // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
+  // the dynamic shared memory of the kernels this context launches, allowed on its device
+  if (c->lsel_mask) CREATE_TRY(allow_local_select_smem());
   if (cfg->gemm_backend == NPAIR_GEMM_TCGEN05) {
+    CREATE_TRY(allow_smem(gemm_kernel(c->prec, c->sweep_epi)));
+    if (c->n_blocks > 1) CREATE_TRY(allow_smem(gemm_kernel(c->prec, EPI_STORE_S)));
+    CREATE_TRY(c->fused_grad ? allow_smem(fused_kernel(c->prec)) : allow_smem(gemm_kernel(c->prec, EPI_OUT)));
+    // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
     std::string te;
     const int bks = c->bk_sim, bkg = c->bk_grad;
     bool ok = true;
@@ -876,7 +896,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     // (no peer access between some pair of GPUs: the NCCL paths are used; every rank takes the same decision only if the
     // topology is symmetric, which holds on an NVSwitch box -- a mixed outcome is reported by the first exchange's timeout)
   }
-  if (cfg->global_scope && c->world > 1 && !c->comm) {
+  if (c->wscope && !c->comm) {
     g_create_err = "global_scope with world > 1 needs a communicator (the world-scope reductions are internal)"; npair_destroy(c); return NPAIR_E_ARG;
   }
 #undef CREATE_TRY
@@ -1020,20 +1040,36 @@ static RowArrays rows_from(const RowArrays& ra, int r0) {
   return v;
 }
 
-// Row-block similarity mode: rows [r0, r0 + blk_rows) of the rank's S into the S buffer (full tiles, store only).  The similarity GEMM is
-// bitwise deterministic and symmetric, so these are the bits the materialised path holds in those rows.
-static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
-  if (c->s_block_row0 == r0) return cudaSuccess;
-  const int rows = c->Q - r0 < c->blk_rows ? c->Q - r0 : c->blk_rows;
+// The similarity GEMM over rows [r0, r0 + rows) of the rank's S through the epilogue `epi` (gemm_wgmma.cuh)
+static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_t st) {
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.M = rows; gp.Nn = c->N; gp.a_row0 = r0;
   gp.num_kblocks = static_cast<int>(c->cat ? kcat_mult(c->prec) * c->Dp / 64 : (c->D + c->bk_sim - 1) / c->bk_sim);
   gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (c->N + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
   gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
-  const cudaError_t e = c->cat ? launch_sim_gemm(c->prec, EPI_SIM_STORE, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st)
-                               : launch_sim_gemm(c->prec, EPI_SIM_STORE, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
+  if (epi & EPI_SYM) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
+  if (epi & EPI_STATS) {
+    gp.lab_rows = c->cur_label; gp.lab_cols = c->lab_total; gp.self_offset = c->rank * c->Q;
+    gp.st_minw = c->ra.st_minw; gp.st_maxw = c->ra.st_maxw; gp.st_maxb = c->ra.st_maxb; gp.st_maxall = c->ra.st_maxall; gp.cnt_same = c->ra.cnt_same;
+    gp.fuse_thr = c->fuse_thr ? 1 : 0; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
+  }
+  return c->cat ? launch_gemm(c->prec, epi, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st)
+                : launch_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
+}
+
+// Rows [r0, r0 + s_rows) of the rank's S into the S buffer, unless it holds them already (a materialised S always does): full tiles,
+// store only.  The similarity GEMM is bitwise deterministic and symmetric, so these are the bits the materialised path holds in those rows.
+static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
+  if (c->s_block_row0 == r0) return cudaSuccess;
+  const cudaError_t e = sim_gemm(c, EPI_STORE_S, r0, c->Q - r0 < c->s_rows ? c->Q - r0 : c->s_rows, st);
   c->s_block_row0 = e == cudaSuccess ? r0 : -1;
   return e;
+}
+
+// LOCAL relative selects of rows [r0, r0 + rows), which the S buffer holds
+static void local_select(npair_ctx* c, int r0, int rows, cudaStream_t st) {
+  launch_local_select(c->S, c->ldS, rows, c->N, c->cur_label + r0, c->lab_total, c->rank * c->Q + r0, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn,
+                      rows_from(c->ra, r0), c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
 }
 
 static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st) {
@@ -1048,88 +1084,59 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
                        c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
     launch_split(c->x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
   }
-  // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) ----
-  GemmParams gp; memset(&gp, 0, sizeof(gp));
-  gp.M = Q; gp.Nn = N; gp.num_kblocks = static_cast<int>((D + c->bk_sim - 1) / c->bk_sim);
-  gp.tiles_m = (Q + 127) / 128; gp.tiles_n = (N + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
-  gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
-  gp.lab_rows = d_label; gp.lab_cols = c->lab_total; gp.self_offset = self_off;
-  gp.st_minw = c->ra.st_minw; gp.st_maxw = c->ra.st_maxw; gp.st_maxb = c->ra.st_maxb; gp.st_maxall = c->ra.st_maxall; gp.cnt_same = c->ra.cnt_same;
-  // the threshold pick rides in the similarity kernel's last CTA unless its result has to be exchanged first (world scope)
-  const bool fuse_thr = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05 && !(c->cfg.global_scope && c->world > 1);
-  gp.fuse_thr = fuse_thr ? 1 : 0; gp.ra = c->ra; gp.mp = mp; gp.bs = c->bs;
+  // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) over all Q rows; S is stored
+  //      only when it is materialised, and is then block 0 of the row pass ----
+  c->s_block_row0 = c->n_blocks == 1 ? 0 : -1;
   if (c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05) {
     PhaseTimer pt(c, 2, st);
-    // row-block mode: the same sweep without the stores (S is recomputed block by block below)
-    const int epi = c->sym_tiles ? (c->blk_rows ? EPI_SIM_SYM_STATS : EPI_SIM_SYM) : (c->blk_rows ? EPI_SIM_STATS : EPI_SIM);
-    c->s_block_row0 = -1;
-    if (c->sym_tiles) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
-    if (c->cat) {
-      gp.num_kblocks = static_cast<int>(kcat_mult(c->prec) * c->Dp / 64); gp.kb_per_split = gp.num_kblocks;
-      CUDA_TRY(c, launch_sim_gemm(c->prec, epi, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st));
-    } else
-      CUDA_TRY(c, launch_sim_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st));
+    CUDA_TRY(c, sim_gemm(c, c->sweep_epi, 0, Q, st));
   } else {
-    CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_SIM, c->Xs + static_cast<long long>(self_off) * c->Dp, c->Dp, static_cast<long long>(N) * c->Dp,
+    GemmParams gp; memset(&gp, 0, sizeof(gp));
+    gp.M = Q; gp.Nn = N; gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
+    CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_STORE_S, c->Xs + static_cast<long long>(self_off) * c->Dp, c->Dp, static_cast<long long>(N) * c->Dp,
                                  c->Xs, c->Dp, static_cast<long long>(N) * c->Dp, D, gp, st));
     launch_row_stats_ref(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, c->ra, st);
   }
   // ---- thresholds (.cu:275-337) ----
   {
-  PhaseTimer pt(c, 3, st);
-  const bool wscope = c->cfg.global_scope && c->world > 1;      // world == 1: the block IS the world
-  if (!fuse_thr) launch_thresholds(c->ra, Q, N, mp, c->bs, c->partial, wscope ? c->xch_src : nullptr, st);
-  if (wscope) {
-    const float* all = nullptr;
-    const int rc = xchg_small(c, c->xch_src, 8, &all, st);
-    if (rc != NPAIR_OK) return rc;
-    launch_thresholds_world(all, NPAIR_XCH_FLOATS, c->world, N, mp, c->bs, st);
-  }
-  {
-    // general relative SN: radix selects; both sides of a region share one sweep of S
-    int local_mask = 0, global_mask = 0;
-    if (is_rel(mp.ap_method) && !sn_is_max(mp.identsn)) (mp.ap_region == NPAIR_LOCAL ? local_mask : global_mask) |= 1;
-    if (is_rel(mp.an_method) && !sn_is_max(mp.diffsn)) (mp.an_region == NPAIR_LOCAL ? local_mask : global_mask) |= 2;
-    if (global_mask) {
+    PhaseTimer pt(c, 3, st);
+    if (!c->fuse_thr) launch_thresholds(c->ra, Q, N, mp, c->bs, c->partial, c->wscope ? c->xch_src : nullptr, st);
+    if (c->wscope) {
+      const float* all = nullptr;
+      const int rc = xchg_small(c, c->xch_src, 8, &all, st);
+      if (rc != NPAIR_OK) return rc;
+      launch_thresholds_world(all, NPAIR_XCH_FLOATS, c->world, N, mp, c->bs, st);
+    }
+    // general relative SN: radix selects; both sides of a region share one sweep of S.  GLOBAL selects need the whole S (one block,
+    // validate()); LOCAL selects of row blocks run in the row pass, block by block
+    if (c->gsel_mask) {
       for (int pass = 0; pass < 3; ++pass) {
-        launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, global_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
-                                  wscope ? 1 : 0, c->bs, c->sms, st);
-        if (wscope) {
+        launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, c->gsel_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
+                                  c->wscope ? 1 : 0, c->bs, c->sms, st);
+        if (c->wscope) {
           const float* all = nullptr;
           const int rc = xchg_small(c, reinterpret_cast<const float*>(c->ghist), NPAIR_XCH_FLOATS, &all, st);
           if (rc != NPAIR_OK) return rc;
-          launch_global_decide(all, NPAIR_XCH_FLOATS, c->world, global_mask, pass, c->ra, Q, c->ghist, c->gcand, c->gcand_cap, c->bs, st);
+          launch_global_decide(all, NPAIR_XCH_FLOATS, c->world, c->gsel_mask, pass, c->ra, Q, c->ghist, c->gcand, c->gcand_cap, c->bs, st);
         }
       }
     }
-    if (local_mask && !c->blk_rows) launch_local_select(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, local_mask, mp.identsn, mp.diffsn, c->ra, c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
+    if (c->lsel_mask && c->n_blocks == 1) local_select(c, 0, Q, st);
   }
-  }
-  // ---- selection + counts + exp + masked sums + log + retrieval in one pass (.cu:343-398) ----
-  if (c->blk_rows) {
-    // row-block mode: per block of rows, recompute S, the LOCAL relative selects, the row pass; then the tops over all Q rows
+  // ---- selection + counts + exp + masked sums + log + retrieval in one pass (.cu:343-398), per block of rows of S ----
+  {
     PhaseTimer pt(c, 4, st);
-    int local_mask = 0;
-    if (is_rel(mp.ap_method) && !sn_is_max(mp.identsn)) local_mask |= 1;     // GLOBAL general-SN selects are refused by validate()
-    if (is_rel(mp.an_method) && !sn_is_max(mp.diffsn)) local_mask |= 2;
     ++c->tops_seq;
-    for (int r0 = 0; r0 < Q; r0 += c->blk_rows) {
-      const int rows = Q - r0 < c->blk_rows ? Q - r0 : c->blk_rows;
+    for (int r0 = 0; r0 < Q; r0 += c->s_rows) {
+      const int rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
-      if (local_mask)
-        launch_local_select(c->S, c->ldS, rows, N, d_label + r0, c->lab_total, self_off + r0, local_mask, mp.identsn, mp.diffsn, rows_from(c->ra, r0),
-                            c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
+      if (c->lsel_mask && c->n_blocks > 1) local_select(c, r0, rows, st);
+      // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
       launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
-                      nullptr, c->tops_seq, r0, rows, false, st);
+                      c->wscope ? c->xch_src : nullptr, c->tops_seq, r0, rows, c->n_blocks == 1, st);
     }
-    launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
-  } else {
-    PhaseTimer pt(c, 4, st);
-    const bool wscope = c->cfg.global_scope && c->world > 1;
-    ++c->tops_seq;
-    launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
-                    wscope ? c->xch_src : nullptr, c->tops_seq, 0, Q, true, st);
-    if (wscope) {       // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
+    if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
+    if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
       const float* all = nullptr;
       const int rc = xchg_small(c, c->xch_src, 8, &all, st);
       if (rc != NPAIR_OK) return rc;
@@ -1244,10 +1251,9 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   const int self_off = c->rank * Q;
-  const bool wscope = c->cfg.global_scope && c->world > 1;
   // loss_weight / dot_normalizer (.cu:427,448); world scope: the normaliser is the world's batch and the transposed term is not
   // divided by the world size, i.e. exactly what a single rank holding the whole batch computes
-  const float lw_over_q = loss_weight / static_cast<float>(wscope ? N : Q);
+  const float lw_over_q = loss_weight / static_cast<float>(c->wscope ? N : Q);
   const bool tc = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
   const float* rs_total = nullptr;
   int bw_mode = BW_SYM;
@@ -1273,36 +1279,28 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   if (tc && c->fused_grad) {
     // weights are produced inside the gradient GEMM: no H in HBM
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));
-    fp.Q = Q; fp.N = N; fp.D = D; fp.num_kblocks = c->grad_kblocks;
-    fp.tiles_m = (Q + 127) / 128; fp.tiles_n = (D + 255) / 256;
-    fp.rowrec = c->ra.rowscal; fp.colrec = rs_total ? rs_total : c->ra.rowscal;
-    fp.self_offset = self_off; fp.inv_world = wscope ? 1.f : 1.f / static_cast<float>(c->world);
-    fp.log2_world = wscope ? 0.f : log2f(static_cast<float>(c->world));
+    fp.N = N; fp.D = D; fp.num_kblocks = c->grad_kblocks;
+    fp.tiles_n = (D + 255) / 256;
+    fp.colrec = rs_total ? rs_total : c->ra.rowscal;
+    fp.inv_world = c->wscope ? 1.f : 1.f / static_cast<float>(c->world);
+    fp.log2_world = c->wscope ? 0.f : log2f(static_cast<float>(c->world));
     fp.sgn_p = (mp.ap_method == M_EASY || mp.ap_method == M_RELATIVE_EASY) ? -1.f : 1.f;
     fp.sgn_n = (mp.an_method == M_HARD || mp.an_method == M_RELATIVE_HARD) ? -1.f : 1.f;
-    fp.out = d_diff; fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
+    fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
     fp.part = c->part; fp.splits = c->grad_split.splits; fp.kb_per_split = c->grad_split.kb_per_split;
     fp.chunk_kb = c->grad_chunk_kb;
-    if (c->blk_rows) {
-      // row-block mode: per block of rows (the one the forward left in the buffer first), recompute S, then the gradient rows.  The
-      // split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output bit is the materialised path's
-      PhaseTimer pt(c, 6, st);
-      const int nblk = (Q + c->blk_rows - 1) / c->blk_rows;
-      const int first = c->s_block_row0 >= 0 ? c->s_block_row0 / c->blk_rows : 0;
-      for (int k = 0; k < nblk; ++k) {
-        const int bi = (first + k) % nblk;
-        const int r0 = bi * c->blk_rows, rows = Q - r0 < c->blk_rows ? Q - r0 : c->blk_rows;
-        CUDA_TRY(c, recompute_sim_block(c, r0, st));
-        FusedGradParams fb = fp;
-        fb.Q = rows; fb.tiles_m = (rows + 127) / 128; fb.m_blk0 = r0 / 128;
-        fb.rowrec = c->ra.rowscal + 8ll * r0; fb.self_offset = self_off + r0; fb.out = d_diff + static_cast<long long>(r0) * D;
-        CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fb, c->sms, st));
-        if (fb.splits > 1) reduce_splits(c, fb.splits, rows, fb.out, 0.f, st);
-      }
-    } else {
-      PhaseTimer pt(c, 6, st);
+    // per block of rows of S, starting with the one the forward left in the buffer (a materialised S is the one block): recompute it,
+    // then its gradient rows.  The split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output
+    // bit is the materialised path's
+    PhaseTimer pt(c, 6, st);
+    const int first = c->s_block_row0 >= 0 ? c->s_block_row0 / c->s_rows : 0;
+    for (int k = 0; k < c->n_blocks; ++k) {
+      const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
+      CUDA_TRY(c, recompute_sim_block(c, r0, st));
+      fp.Q = rows; fp.tiles_m = (rows + 127) / 128; fp.m_blk0 = r0 / 128;
+      fp.rowrec = c->ra.rowscal + 8ll * r0; fp.self_offset = self_off + r0; fp.out = d_diff + static_cast<long long>(r0) * D;
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
-      if (fp.splits > 1) reduce_splits(c, fp.splits, Q, d_diff, 0.f, st);
+      if (fp.splits > 1) reduce_splits(c, fp.splits, rows, fp.out, 0.f, st);
     }
     CUDA_TRY(c, cudaGetLastError());
     return NPAIR_OK;
@@ -1321,7 +1319,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     gp.out = d_total_ext ? d_total_ext : c->OUT2; gp.ldo = D; gp.alpha = 0.5f * (1.f / static_cast<float>(c->world)) * lw_over_q; gp.beta = 0.f;
     {
       PhaseTimer pt(c, 7, st);
-      if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, c->tm_b2A, c->tm_b2B, c->tm_S, gp, c->sms, st));
+      if (tc) CUDA_TRY(c, launch_gemm(c->prec, EPI_OUT,c->tm_b2A, c->tm_b2B, c->tm_S, gp, c->sms, st));
       else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->HT, c->Qp, static_cast<long long>(N) * c->Qp, c->XlT, c->Qp, static_cast<long long>(D) * c->Qp, Q, gp, st));
     }
     if (!d_total_ext) {
@@ -1338,7 +1336,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   gp.splits = c->grad_split.splits; gp.kb_per_split = c->grad_split.kb_per_split; gp.part = c->part;
   {
     PhaseTimer pt(c, 6, st);
-    if (tc) CUDA_TRY(c, launch_split_gemm(c->prec, c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
+    if (tc) CUDA_TRY(c, launch_gemm(c->prec, EPI_OUT,c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
     else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->H, c->Np, static_cast<long long>(Q) * c->Np, c->XsT, c->Np, static_cast<long long>(D) * c->Np, N, gp, st));
     if (gp.splits > 1) reduce_splits(c, gp.splits, Q, d_diff, gp.beta, st);
   }
@@ -1391,7 +1389,7 @@ int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
   CUDA_TRY(c, cudaStreamSynchronize(c->last_stream));
   const int Q = c->Q, N = c->N;
   if (which == 0) {
-    if (c->blk_rows) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
+    if (c->n_blocks > 1) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
     if (n < static_cast<size_t>(Q) * N) { c->err = "buffer too small"; return NPAIR_E_ARG; }
     CUDA_TRY(c, cudaMemcpy2D(dst, sizeof(float) * N, c->S, sizeof(float) * c->ldS, sizeof(float) * N, Q, cudaMemcpyDeviceToHost));
     return NPAIR_OK;
@@ -1517,7 +1515,8 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
       CUtensorMap ta, tb; std::string te;
       if (!make_tmap_pieces(&ta, As, K, M, ns, Kp, static_cast<long long>(M) * Kp, bk, 128, &te) ||
           !make_tmap_pieces(&tb, Bs, K, Nn, ns, Kp, static_cast<long long>(Nn) * Kp, bk, 256, &te)) { g_create_err = te; rc = NPAIR_E_CUDA; goto done; }
-      DG_TRY(launch_split_gemm(precision, ta, tb, ta, gp, sms, st));
+      DG_TRY(allow_smem(gemm_kernel(precision, EPI_OUT)));
+      DG_TRY(launch_gemm(precision, EPI_OUT, ta, tb, ta, gp, sms, st));
     } else {
       DG_TRY(launch_simt_gemm(precision, EPI_OUT, As, Kp, static_cast<long long>(M) * Kp, Bs, Kp, static_cast<long long>(Nn) * Kp, K, gp, st));
     }

@@ -12,7 +12,7 @@
 // swizzled smem ring); warps 4-11 two consumer warpgroups, each issuing wgmma.m64n256k16 for 64 rows of the tile and running the
 // fused epilogue (similarity store + row statistics, or a scaled store of a gradient tile) on its register accumulator.
 // Replaces the reference's cublasSgemm calls: sim GEMM npair_multi_class_loss.cu:218 and the six backward
-// GEMMs .cu:448-460; the EPI_SIM epilogue also replaces GetLabelDiffMtx (.cu:44-66) and the host statistics loop
+// GEMMs .cu:448-460; the EPI_STATS epilogue also replaces GetLabelDiffMtx (.cu:44-66) and the host statistics loop
 // (.cu:225-265: min_within / max_between / max_all) -- they are computed while the tile is in registers.
 #pragma once
 #include <cuda.h>
@@ -26,33 +26,29 @@
 
 namespace npair {
 
-// EPI_SIM     : similarity tile -> S + fused row statistics (any world size)
 // EPI_OUT     : alpha * acc (+ beta * out) gradient tile
-// EPI_SIM_SYM : world == 1 only.  S = X X^T is symmetric, so only tiles that touch the upper triangle are computed
+// A similarity epilogue is an OR of three bits:
+// EPI_STORE_S : the tile goes to S.  Without EPI_STATS this is the store-only recompute of a row block [a_row0, a_row0 + M) of S
+//               into a buffer of M rows (row-block similarity mode, DESIGN 4.2)
+// EPI_STATS   : fused row statistics, and the threshold pick in the last CTA (fuse_thr)
+// EPI_SYM     : world == 1 only.  S = X X^T is symmetric, so only tiles that touch the upper triangle are computed
 //               (tile list from the host, ~52 % of the tiles); every strictly-upper 128-column block is also written
-//               MIRRORED (second TMA store) and contributes COLUMN statistics (warp redux) to the rows it mirrors into.
-//               S comes out bitwise symmetric, which the backward weight builder relies on.
-// Row-block similarity mode (S is never materialised whole, see DESIGN 4.2):
-// EPI_SIM_STATS     : EPI_SIM without the stores to S: fused row statistics (and threshold pick) only
-// EPI_SIM_SYM_STATS : EPI_SIM_SYM without the stores to S; mirrored blocks still go through the staging tile for their column statistics
-// EPI_SIM_STORE     : store-only recompute of a row block [a_row0, a_row0 + M) of S into a buffer of M rows; no statistics
-enum { EPI_SIM = 0, EPI_OUT = 1, EPI_SIM_SYM = 2, EPI_SIM_STATS = 3, EPI_SIM_SYM_STATS = 4, EPI_SIM_STORE = 5 };
-__host__ __device__ constexpr bool epi_sym(int e) { return e == EPI_SIM_SYM || e == EPI_SIM_SYM_STATS; }
-__host__ __device__ constexpr bool epi_stores_s(int e) { return e == EPI_SIM || e == EPI_SIM_SYM || e == EPI_SIM_STORE; }
-__host__ __device__ constexpr bool epi_stats(int e) { return e != EPI_OUT && e != EPI_SIM_STORE; }
+//               MIRRORED (second TMA store, with EPI_STORE_S) and contributes COLUMN statistics (warp redux) to the rows it
+//               mirrors into.  S comes out bitwise symmetric, which the backward weight builder relies on.
+enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32 };
 
 struct GemmParams {
   int M, Nn;           // logical output extent
   int num_kblocks;     // K_pad / BK
   int tiles_m, tiles_n;
-  const int2* tile_list;      // optional explicit (m_blk, n_blk) list (EPI_SIM_SYM); tiles_m*tiles_n entries are then ignored
+  const int2* tile_list;      // optional explicit (m_blk, n_blk) list (EPI_SYM); tiles_m*tiles_n entries are then ignored
   int num_tiles_list;
   int splits, kb_per_split;   // split-K (EPI_OUT only): tile = (m_blk*tiles_n + n_blk)*splits + split, k-blocks [split*kb_per_split, ...)
   float* part;                // splits > 1: partial products [split][M][ldo]; a reduce kernel sums them in fixed order
-  // ---- EPI_SIM ----
+  // ---- similarity epilogues ----
   float* S;            // [M x ldS] fp32 similarities
   long long ldS;       // multiple of 32
-  const float* dev_scale;  // device scalar: inverse operand pre-scale (power of two) or NULL.  EPI_SIM multiplies the
+  const float* dev_scale;  // device scalar: inverse operand pre-scale (power of two) or NULL.  A similarity epilogue multiplies the
                            // accumulators by its square (both operands were pre-scaled), EPI_OUT multiplies alpha by it
   const float* lab_rows;   // [M]  labels of this rank's rows
   const float* lab_cols;   // [Nn] labels of all columns
@@ -71,7 +67,7 @@ struct GemmParams {
   float* out;          // [M x ldo]
   long long ldo;
   float alpha, beta;   // out = alpha*acc + beta*out
-  // ---- EPI_SIM_STORE ----
+  // ---- EPI_STORE_S without EPI_STATS ----
   int a_row0;          // row of the A operand (and of the rank's S) that output row 0 stands for; a multiple of 128
 };
 
@@ -165,7 +161,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   using Cfg = GemmCfg<NSPLIT, BK_, EPI>;
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
-  constexpr bool SYM = epi_sym(EPI), STORE = epi_stores_s(EPI), STATS = epi_stats(EPI);
+  constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS;
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer in the shared address space (offset arithmetic, no integer round trip): LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -174,8 +170,8 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint8_t* aux = store_stage + Cfg::STORE_STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);            // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                           // [STAGES]
-  float* s_lab = reinterpret_cast<float*>(aux + 256);                // [256] column labels of the current tile (EPI_SIM*)
-  float* s_labr = reinterpret_cast<float*>(aux + 256 + 1024);        // [128] row labels of the current tile (EPI_SIM_SYM)
+  float* s_lab = reinterpret_cast<float*>(aux + 256);                // [256] column labels of the current tile (EPI_STATS)
+  float* s_labr = reinterpret_cast<float*>(aux + 256 + 1024);        // [128] row labels of the current tile (EPI_SYM)
   float2* s_rng = reinterpret_cast<float2*>(aux + 256 + 1024 + 512); // [8] {min, max} label of each 32-column chunk, [8..12) of each 32-row group
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -215,7 +211,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s) {
-            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, &full_bar[stage], kb * BK, m_blk * BM + (EPI == EPI_SIM_STORE ? p.a_row0 : 0), s);
+            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, &full_bar[stage], kb * BK, m_blk * BM + (STORE && !STATS ? p.a_row0 : 0), s);
             ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, &full_bar[stage], kb * BK, n_blk * BN, s);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -357,7 +353,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
         const int ch = 2 * cp + half;                     // 32-column chunk of the tile
         const int col0 = col_base + ch * 32;
-        const int cb = col0 >> 7;                          // 128-wide column block (EPI_SIM_SYM bookkeeping)
+        const int cb = col0 >> 7;                          // 128-wide column block (EPI_SYM bookkeeping)
         // lower-triangle half of a straddling tile: produced by mirroring
         if ((SYM && cb < m_blk) || col0 >= p.Nn) continue;
         float v[32];

@@ -1091,6 +1091,10 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     __syncthreads();
   }
 }
+static constexpr int LSEL_SMEM = static_cast<int>(sizeof(LselWarp)) * NPAIR_LSEL_WARPS;
+cudaError_t allow_local_select_smem() {
+  return cudaFuncSetAttribute(local_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LSEL_SMEM);
+}
 void launch_local_select(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                          int self_offset, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st) {
   if (!force_warp_kernel && N <= NPAIR_LSB_THREADS * NPAIR_LSB_VPT * 4 && (reinterpret_cast<uintptr_t>(lab_cols) & 15) == 0 && (ldS & 3) == 0) {
@@ -1099,14 +1103,11 @@ void launch_local_select(const float* S, long long ldS, int Q, int N, const floa
     count_launch();
     return;
   }
-  const int smem = static_cast<int>(sizeof(LselWarp)) * NPAIR_LSEL_WARPS;
-  static bool attr_set = false;
-  if (!attr_set) { cudaFuncSetAttribute(local_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_set = true; }
-  const int per_sm = (227 * 1024) / (smem + 1024);
+  const int per_sm = (227 * 1024) / (LSEL_SMEM + 1024);
   int grid = sms * (per_sm < 1 ? 1 : per_sm);
   const int need = (Q + NPAIR_LSEL_WARPS - 1) / NPAIR_LSEL_WARPS;
   if (grid > need) grid = need;
-  local_select_kernel<<<grid, 32 * NPAIR_LSEL_WARPS, smem, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, side_mask, sn_ap, sn_an, ra, bs);
+  local_select_kernel<<<grid, 32 * NPAIR_LSEL_WARPS, LSEL_SMEM, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, side_mask, sn_ap, sn_an, ra, bs);
   count_launch();
 }
 
@@ -1702,7 +1703,7 @@ __device__ __forceinline__ void store_quad(uint16_t* __restrict__ base, long lon
 // 64 x 64 tiles, 256 threads; thread (tr = t/16, tc = t%16) owns the 4 x 4 micro-tile rows 4tr.., columns 4tc.. :
 // one 16-byte load per row of the micro-tile, one 8-byte store per row and operand piece -- every request covers whole
 // sectors, nothing is transposed.
-// SYM (world == 1): the similarity GEMM wrote a bitwise symmetric S (EPI_SIM_SYM), so
+// SYM (world == 1): the similarity GEMM wrote a bitwise symmetric S (EPI_SYM), so
 //     H[j][m] = g'(S[j][m]; row j) + g'(S[j][m]; row m)                       (= G + G^T, .cu:448-497 folded)
 //   needs only the row scalars of BOTH indices, which are local when world == 1.
 // !SYM (world > 1): H[j][m] = g'(j,m) and the transposed copy HT[m][j] (micro-tile transposed in registers).

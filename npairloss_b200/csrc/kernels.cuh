@@ -99,6 +99,8 @@ void launch_tops_world(const float* xall, int xstride, int world, long long N, i
 // side_mask: bit 0 = AP threshold over the same-label list, bit 1 = AN threshold over the diff-label list
 void launch_local_select(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                          int self_offset, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
+// lets the current device launch the one-warp-per-row local select with its dynamic shared memory (above the default limit)
+cudaError_t allow_local_select_smem();
 void launch_global_select_pass(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                                int self_offset, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
                                uint32_t* cand /*[2][cand_cap]*/, unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st);

@@ -92,9 +92,13 @@ def test_workspace_counts_the_materialised_gradient_weights():
 
 @pytest.mark.parametrize("side", ["ap", "an"])
 def test_workspace_counts_the_global_select_candidates_on_every_backend(side):
-    """A GLOBAL RELATIVE_* side needs two candidate lists of cap 4-byte entries, whichever GEMM backend computes S."""
+    """A GLOBAL RELATIVE_* side with a general SN needs two candidate lists of cap 4-byte entries, whichever GEMM backend
+    computes S.  With SN = -0.0 (the usage block's) its threshold is the list's maximum, no select runs and nothing is added."""
     Q, D = 1024, 256
     cap = min(Q * Q // 8 + 4096, 32 << 20)
-    base = dict(gemm_backend=capi.GEMM_SIMT_CHECK)
-    rel = dict(base, **{f"{side}_region": capi.GLOBAL, f"{side}_method": capi.RELATIVE_HARD})
-    assert _workspace(Q, D, **rel) - _workspace(Q, D, **base) == 8 * cap
+    for backend in (capi.GEMM_TCGEN05, capi.GEMM_SIMT_CHECK):
+        base = dict(gemm_backend=backend)
+        rel = dict(base, **{f"{side}_region": capi.GLOBAL, f"{side}_method": capi.RELATIVE_HARD})
+        closed_form = dict(rel, **{"identsn" if side == "ap" else "diffsn": -0.0})
+        assert _workspace(Q, D, **rel) - _workspace(Q, D, **base) == 8 * cap, backend
+        assert _workspace(Q, D, **closed_form) == _workspace(Q, D, **base), backend
