@@ -151,13 +151,11 @@ static bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int 
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM launchers
-static inline int nsplit_of_prec(int prec) { return prec == PREC_BF16 ? 1 : (prec == PREC_FP16X2 ? 2 : 3); }
 // K-block per (operand format, GEMM role); see GemmCfg
-static inline int bk_of(int prec, int epi) {
+static constexpr int bk_of(int prec, int epi) {
   if (epi != EPI_OUT) return 64;                 // similarity GEMM: single pass, 64-element K blocks
   return prec == PREC_BF16 ? 64 : 32;
 }
-static inline int kcat_mult(int prec) { return prec == PREC_FP16X2 ? 3 : (prec == PREC_BF16X3 ? 6 : 1); }
 
 // A GEMM kernel instantiation with its launch shape.  Its dynamic shared memory exceeds the default limit, so every device that
 // launches it has to allow that much first (allow_smem).
@@ -188,10 +186,10 @@ static GemmKernel sim_gemm_t(int epi) {
 }
 // `epi`: EPI_OUT for the gradient GEMM (A = split gradient weights, B = split transposed features), else a similarity epilogue
 static GemmKernel gemm_kernel(int prec, int epi) {
-  if (epi != EPI_OUT) return prec == PREC_FP16X2 ? sim_gemm_t<false>(epi) : sim_gemm_t<true>(epi);
-  if (prec == PREC_BF16) return gemm_t<1, true, EPI_OUT, 64>();
-  if (prec == PREC_FP16X2) return gemm_t<2, false, EPI_OUT, 32>();
-  return gemm_t<3, true, EPI_OUT, 32>();
+  return with_prec(prec, [epi](auto P) {
+    constexpr SplitFormat f = SPLIT_FORMATS[P];
+    return epi != EPI_OUT ? sim_gemm_t<f.bf16>(epi) : gemm_t<f.pieces, f.bf16, EPI_OUT, bk_of(P, EPI_OUT)>();
+  });
 }
 // `sm`: fp32 tensor map of the similarity matrix for EPI_STORE_S's TMA stores (ignored otherwise: pass any valid map)
 static cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
@@ -203,12 +201,11 @@ static cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CU
   return cudaGetLastError();
 }
 
-template <int NSPLIT, bool BF16>
-static FusedKernel fused_t() { return FusedKernel{fused_grad_kernel<NSPLIT, BF16>, FusedCfg<NSPLIT>::THREADS, FusedCfg<NSPLIT>::SMEM_BYTES}; }
 static FusedKernel fused_kernel(int prec) {
-  if (prec == PREC_BF16) return fused_t<1, true>();
-  if (prec == PREC_FP16X2) return fused_t<2, false>();
-  return fused_t<3, true>();
+  return with_prec(prec, [](auto P) {
+    constexpr SplitFormat f = SPLIT_FORMATS[P];
+    return FusedKernel{fused_grad_kernel<f.pieces, f.bf16>, FusedCfg<f.pieces>::THREADS, FusedCfg<f.pieces>::SMEM_BYTES};
+  });
 }
 static cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
   const FusedKernel k = fused_kernel(prec);
@@ -275,16 +272,11 @@ __global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restri
 static cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long long lda, long long psA, const uint16_t* B, long long ldb,
                                     long long psB, int K, const GemmParams& p, cudaStream_t st) {
   dim3 grid((p.Nn + 63) / 64, (p.M + 63) / 64);
-#define NPAIR_SIMT(P)                                                                                   \
-  do {                                                                                                  \
-    if (epi == EPI_OUT) simt_gemm_kernel<P, 1><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);   \
-    else simt_gemm_kernel<P, 0><<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);                  \
-  } while (0)
-  if (prec == PREC_BF16) NPAIR_SIMT(PREC_BF16);
-  else if (prec == PREC_FP16X2) NPAIR_SIMT(PREC_FP16X2);
-  else NPAIR_SIMT(PREC_BF16X3);
+  with_prec(prec, [&](auto P) {
+    auto kernel = epi == EPI_OUT ? simt_gemm_kernel<P, 1> : simt_gemm_kernel<P, 0>;
+    kernel<<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);
+  });
   count_launch();
-#undef NPAIR_SIMT
   return cudaGetLastError();
 }
 
@@ -380,7 +372,7 @@ using namespace npair;
 
 // ------------------------------------------------------------------------------------------------ buffer plan
 // One rank's peer-memory exchange region, in floats.  Each part is double-buffered by the step parity and holds every rank's rows:
-//     X[2][N][D] | LAB[2][N rounded up to 4] | REC[2][N][8] | XCH[2][world][NPAIR_XCH_FLOATS] (world scope) | FLAGS[3 kinds][2][world] uint32
+//     X[2][N][D] | LAB[2][N rounded up to 4] | REC[2][N] RowRecord | XCH[2][world][NPAIR_XCH_FLOATS] (world scope) | FLAGS[3 kinds][2][world] uint32
 enum { XP_X, XP_LAB, XP_REC, XP_XCH, XP_COUNT };
 struct XchgLayout {
   long long base[XP_COUNT], par_stride[XP_COUNT], rank_stride[XP_COUNT], flags, floats;
@@ -388,8 +380,8 @@ struct XchgLayout {
 };
 static XchgLayout xchg_layout(int Q, int D, int world, bool world_scope) {
   const long long N = static_cast<long long>(Q) * world;
-  const long long rank_floats[XP_COUNT] = {static_cast<long long>(Q) * D, Q, 8ll * Q, world_scope ? NPAIR_XCH_FLOATS : 0};
-  const long long par_floats[XP_COUNT] = {N * D, round_up(N, 4), 8 * N, world * rank_floats[XP_XCH]};
+  const long long rank_floats[XP_COUNT] = {static_cast<long long>(Q) * D, Q, ROW_RECORD_FLOATS * Q, world_scope ? NPAIR_XCH_FLOATS : 0};
+  const long long par_floats[XP_COUNT] = {N * D, round_up(N, 4), ROW_RECORD_FLOATS * N, world * rank_floats[XP_XCH]};
   XchgLayout l;
   long long o = 0;
   for (int p = 0; p < XP_COUNT; ++p) { l.base[p] = o; l.par_stride[p] = par_floats[p]; l.rank_stride[p] = rank_floats[p]; o += 2 * par_floats[p]; }
@@ -460,7 +452,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const long long Q = cfg.Q, D = cfg.D, N = Q * W;
   const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
   p.N = static_cast<int>(N);
-  p.nsplit = nsplit_of_prec(prec); p.bk_sim = bk_of(prec, EPI_STORE_S); p.bk_grad = bk_of(prec, EPI_OUT);
+  p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_sim = bk_of(prec, EPI_STORE_S); p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
   const int blk_rows = sim_block_rows(cfg);
   p.s_rows = blk_rows ? blk_rows : cfg.Q;
@@ -501,12 +493,12 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   b[B_S] = f * p.s_rows * p.ldS;
   if (!p.cat) b[B_XS] = 2 * ns * N * p.Dp;                                      // operand pieces [ns][N][Dp]
   b[B_XST] = 2 * ns * D * p.Np;                                                 // transposed pieces [ns][D][Np]
-  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * kcat_mult(prec) * p.Dp;        // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * mma_passes(ns) * p.Dp;        // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
   if (!p.fused_grad) b[B_H] = 2 * ns * Q * p.Np;                                // materialised gradient weights
   if (rs) { b[B_XLT] = 2 * ns * D * p.Qp; b[B_HT] = 2 * ns * N * p.Qp; b[B_OUT2] = f * N * D; }
-  if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = f * 8 * N;        // gathered row records
+  if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = sizeof(RowRecord) * N;   // gathered row records
   if (p.grad_split.splits > 1) b[B_PART] = f * p.grad_split.splits * Q * D;     // split-K partial products
-  b[B_ROWS] = 4 * 21 * Q + 64;   // 13 row arrays of Q 4-byte words (RowArrays) + the 32-byte aligned [Q][8] row records
+  b[B_ROWS] = (4 * 13 + sizeof(RowRecord)) * Q + 64;   // 13 row arrays of Q 4-byte words (RowArrays) + the 32-byte aligned row records
   b[B_BS] = sizeof(BlockScalars);
   b[B_PARTIAL] = f * 2048;
   b[B_GHIST] = sizeof(unsigned long long) * 4096;
@@ -540,7 +532,7 @@ struct npair_ctx : Plan {
   uint16_t *Xs = nullptr, *XsT = nullptr, *XlT = nullptr, *H = nullptr, *HT = nullptr;
   float* OUT2 = nullptr;         // world > 1: N x D transposed-term product before the reduce-scatter
   uint16_t *XcatA = nullptr, *XcatB = nullptr;   // K-concatenated operands [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
-  float* rs_total = nullptr;     // row-scalar mode: all-gathered [N][8] row records
+  RowRecord* rs_total = nullptr;   // row-scalar mode: the world's N row records, all-gathered
   CUtensorMap tm_catA, tm_catB;
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
@@ -806,7 +798,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     ra.A = reinterpret_cast<float*>(w); w += Q; ra.T = reinterpret_cast<float*>(w); w += Q; ra.logv = reinterpret_cast<float*>(w); w += Q;
     ra.hits = reinterpret_cast<int*>(w); w += 3 * Q;
     w = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(w) + 31) & ~static_cast<uintptr_t>(31));
-    ra.rowscal = reinterpret_cast<float*>(w); w += 8ll * Q;
+    ra.rowrec = reinterpret_cast<RowRecord*>(w);
   }
   if (c->sym_tiles) {
     const std::vector<int2> tl = sym_tile_list(Q, N);
@@ -838,7 +830,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, &te, 128);
     }
     if (c->XcatA) {       // bitwise-symmetric similarity: one pass over K_cat = 3*Dp (fp16x2) / 6*Dp (bf16x3)
-      const long long kc = kcat_mult(c->prec) * c->Dp;
+      const long long kc = mma_passes(ns) * c->Dp;
       ok = ok && make_tmap_pieces(&c->tm_catA, c->XcatA + static_cast<long long>(c->rank) * Q * kc, static_cast<int>(kc), Q, 1, kc, static_cast<long long>(N) * kc, 64, 128, &te);
       ok = ok && make_tmap_pieces(&c->tm_catB, c->XcatB, static_cast<int>(kc), N, 1, kc, static_cast<long long>(N) * kc, 64, 256, &te);
     }
@@ -1036,7 +1028,7 @@ static RowArrays rows_from(const RowArrays& ra, int r0) {
   v.st_minw += r0; v.st_maxw += r0; v.st_maxb += r0; v.st_maxall += r0; v.cnt_same += r0;
   v.posi_thr += r0; v.nega_thr += r0; v.A += r0; v.T += r0; v.logv += r0;
   v.hits = nullptr;
-  v.rowscal += 8ll * r0;
+  v.rowrec += r0;
   return v;
 }
 
@@ -1044,7 +1036,7 @@ static RowArrays rows_from(const RowArrays& ra, int r0) {
 static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_t st) {
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.M = rows; gp.Nn = c->N; gp.a_row0 = r0;
-  gp.num_kblocks = static_cast<int>(c->cat ? kcat_mult(c->prec) * c->Dp / 64 : (c->D + c->bk_sim - 1) / c->bk_sim);
+  gp.num_kblocks = static_cast<int>(c->cat ? mma_passes(c->nsplit) * c->Dp / 64 : (c->D + c->bk_sim - 1) / c->bk_sim);
   gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (c->N + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
   gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
   if (epi & EPI_SYM) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
@@ -1148,7 +1140,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
     // peer-memory exchange: push this rank's 32-byte row records to every rank now; the backward only waits for the flags
     PhaseTimer pt(c, 8, st);
     const uint32_t ep = ++c->p2p_rec_epoch;
-    p2p_push(c, XCHG_RECORDS, ep, grid_for(2ll * Q, 64), c->ra.rowscal, 8ll * Q, XP_REC, nullptr, 0, XP_REC, st);
+    p2p_push(c, XCHG_RECORDS, ep, grid_for(2ll * Q, 64), reinterpret_cast<const float*>(c->ra.rowrec), ROW_RECORD_FLOATS * Q, XP_REC,
+             nullptr, 0, XP_REC, st);
   }
   CUDA_TRY(c, cudaGetLastError());
   if (c->defer_sync) return NPAIR_OK;              // npair_forward_backward enqueues the backward first, then waits once
@@ -1157,9 +1150,9 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   return rc;
 }
 
-static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const float* d_rs_ext, cudaStream_t st);
+static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
 // Backward_gpu (+ the projection of the fused L2Normalize producer: the kernels produce d loss / d y, the caller gets d loss / d x)
-static int backward_impl(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const float* d_rs_ext, cudaStream_t st) {
+static int backward_impl(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
   if (!c->cfg.normalize_input) return backward_core(c, loss_weight, d_diff, d_total_ext, d_rs_ext, st);
   if (d_total_ext) { c->err = "normalize_input: the partial (pre-all-reduce) backward is not available, its sum over ranks would have to be projected"; return NPAIR_E_STATE; }
   const int rc = backward_core(c, loss_weight, c->dY, nullptr, d_rs_ext, st);
@@ -1225,7 +1218,7 @@ int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
   if (!c || !d_out) return NPAIR_E_ARG;
   if (!c->fwd_done) { c->err = "npair_row_scalars called without a successful forward"; return NPAIR_E_STATE; }
   CUDA_TRY(c, cudaSetDevice(c->device));
-  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowscal, sizeof(float) * 8ull * c->Q, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowrec, sizeof(RowRecord) * c->Q, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return NPAIR_OK;
 }
 
@@ -1237,7 +1230,7 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
   c->last_stream = st;
-  return backward_impl(c, loss_weight, d_diff, nullptr, d_rs_total, st);
+  return backward_impl(c, loss_weight, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), st);
 }
 
 // d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
@@ -1247,7 +1240,7 @@ static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, flo
   count_launch();
 }
 
-static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const float* d_rs_ext, cudaStream_t st) {
+static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   const int self_off = c->rank * Q;
@@ -1255,7 +1248,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   // divided by the world size, i.e. exactly what a single rank holding the whole batch computes
   const float lw_over_q = loss_weight / static_cast<float>(c->wscope ? N : Q);
   const bool tc = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
-  const float* rs_total = nullptr;
+  const RowRecord* rs_total = nullptr;
   int bw_mode = BW_SYM;
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) {
     bw_mode = BW_ROWSCAL;
@@ -1263,13 +1256,13 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     else {
       if (c->p2p_rec && !c->ext_gathered) {
         PhaseTimer pt(c, 8, st);
-        rs_total = p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st);
+        rs_total = reinterpret_cast<const RowRecord*>(p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st));
       } else if (!c->rs_gathered) {
-        // the only backward exchange: 8*Q floats per rank (replaces the N x D MPI_Allreduce of .cu:462-489)
+        // the only backward exchange: Q row records per rank (replaces the N x D MPI_Allreduce of .cu:462-489)
         if (!c->comm) { c->err = "no communicator: use npair_backward_gathered with externally gathered row records"; return NPAIR_E_STATE; }
         PhaseTimer pt(c, 8, st);
         NcclApi* api = nccl_api();
-        int r = api->AllGather(c->ra.rowscal, c->rs_total, 8ull * Q, NCCL_FLOAT32, c->comm, st);
+        int r = api->AllGather(c->ra.rowrec, c->rs_total, ROW_RECORD_FLOATS * Q, NCCL_FLOAT32, c->comm, st);
         if (r != 0) { c->err = fmt("ncclAllGather(row records): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
         c->rs_gathered = true;
         rs_total = c->rs_total;
@@ -1281,11 +1274,10 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));
     fp.N = N; fp.D = D; fp.num_kblocks = c->grad_kblocks;
     fp.tiles_n = (D + 255) / 256;
-    fp.colrec = rs_total ? rs_total : c->ra.rowscal;
+    fp.colrec = rs_total ? rs_total : c->ra.rowrec;
     fp.inv_world = c->wscope ? 1.f : 1.f / static_cast<float>(c->world);
     fp.log2_world = c->wscope ? 0.f : log2f(static_cast<float>(c->world));
-    fp.sgn_p = (mp.ap_method == M_EASY || mp.ap_method == M_RELATIVE_EASY) ? -1.f : 1.f;
-    fp.sgn_n = (mp.an_method == M_HARD || mp.an_method == M_RELATIVE_HARD) ? -1.f : 1.f;
+    fp.sgn_p = ap_sign(mp.ap_method); fp.sgn_n = an_sign(mp.an_method);
     fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
     fp.part = c->part; fp.splits = c->grad_split.splits; fp.kb_per_split = c->grad_split.kb_per_split;
     fp.chunk_kb = c->grad_chunk_kb;
@@ -1298,7 +1290,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
       const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
       fp.Q = rows; fp.tiles_m = (rows + 127) / 128; fp.m_blk0 = r0 / 128;
-      fp.rowrec = c->ra.rowscal + 8ll * r0; fp.self_offset = self_off + r0; fp.out = d_diff + static_cast<long long>(r0) * D;
+      fp.rowrec = c->ra.rowrec + r0; fp.self_offset = self_off + r0; fp.out = d_diff + static_cast<long long>(r0) * D;
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
       if (fp.splits > 1) reduce_splits(c, fp.splits, rows, fp.out, 0.f, st);
     }
@@ -1470,7 +1462,7 @@ int npair_debug_mma_symmetric(int precision) {
 int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const float* dA, const float* dB, float* dC, void* stream) {
   if (M < 1 || Nn < 1 || K < 1 || !dA || !dB || !dC || precision < 0 || precision > 2) { g_create_err = "bad argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int ns = nsplit_of_prec(precision), bk = bk_of(precision, EPI_OUT);
+  const int ns = SPLIT_FORMATS[precision].pieces, bk = bk_of(precision, EPI_OUT);
   const long long Kp = round_up(K, 64);
   uint16_t *As = nullptr, *Bs = nullptr, *dummyT = nullptr;
   BlockScalars* bs = nullptr; float* partial = nullptr;
@@ -1485,32 +1477,30 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
     DG_TRY(cudaMalloc(&dummyT, 2ull * ns * K * tmax));
     DG_TRY(cudaMalloc(&bs, sizeof(BlockScalars))); DG_TRY(cudaMemset(bs, 0, sizeof(BlockScalars)));
     DG_TRY(cudaMalloc(&partial, sizeof(float) * 2048));
-    // one common power-of-two scale over both operands (the layer multiplies X by X^T, i.e. a single matrix)
-    launch_absmax_asum(dA, static_cast<long long>(M) * K, dA, static_cast<long long>(M) * K, partial, bs, precision == PREC_FP16X2, st);
-    float sA = 1.f, sB = 1.f;
+    // one common power-of-two scale over both operands (the layer multiplies X by X^T, i.e. a single matrix), from max|A| and
+    // max|B| as the step's operand preparation finds them (no rows: nothing else is touched)
+    float sc[2] = {1.f, 1.f};                  // x_scale, x_inv_scale
     if (precision == PREC_FP16X2) {
+      const float* op[2] = {dA, dB};
+      const long long n[2] = {static_cast<long long>(M) * K, static_cast<long long>(Nn) * K};
+      float mx[2] = {0.f, 0.f};
+      for (int i = 0; i < 2; ++i) {
+        launch_prep_reduce(op[i], n[i], op[i], n[i], partial, 1, RowArrays{}, 0, bs, st);
+        DG_TRY(cudaMemcpyAsync(&mx[i], &bs->x_absmax, 4, cudaMemcpyDeviceToHost, st));
+      }
       DG_TRY(cudaStreamSynchronize(st));
-      float mA = 0.f, mB = 0.f;
-      DG_TRY(cudaMemcpy(&mA, &bs->x_absmax, 4, cudaMemcpyDeviceToHost));
-      launch_absmax_asum(dB, static_cast<long long>(Nn) * K, dB, static_cast<long long>(Nn) * K, partial, bs, 1, st);
-      DG_TRY(cudaStreamSynchronize(st));
-      DG_TRY(cudaMemcpy(&mB, &bs->x_absmax, 4, cudaMemcpyDeviceToHost));
-      const float mx = mA > mB ? mA : mB;
-      int e = 0; if (mx > 0.f) frexpf(mx, &e);
-      sA = ldexpf(1.f, -e); sB = ldexpf(1.f, e);
-      float sc[2] = {sA, sB};
-      DG_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
-    } else {
-      float sc[2] = {1.f, 1.f};
-      DG_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
+      const float m = mx[0] > mx[1] ? mx[0] : mx[1];
+      int e = 0; if (m > 0.f) frexpf(m, &e);
+      sc[0] = ldexpf(1.f, -e); sc[1] = ldexpf(1.f, e);
     }
+    DG_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
     launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
     launch_split(dB, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
     GemmParams gp; memset(&gp, 0, sizeof(gp));
     gp.M = M; gp.Nn = Nn; gp.num_kblocks = (K + bk - 1) / bk; gp.tiles_m = (M + 127) / 128; gp.tiles_n = (Nn + 255) / 256;
     gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
     // EPI_OUT applies the inverse scale once; both operands were scaled -> fold the second factor into alpha
-    gp.alpha = sB; gp.dev_scale = &bs->x_inv_scale;
+    gp.alpha = sc[1]; gp.dev_scale = &bs->x_inv_scale;
     if (backend == NPAIR_GEMM_TCGEN05) {
       CUtensorMap ta, tb; std::string te;
       if (!make_tmap_pieces(&ta, As, K, M, ns, Kp, static_cast<long long>(M) * Kp, bk, 128, &te) ||

@@ -85,7 +85,7 @@ struct GemmCfg {
   static constexpr int A_PIECE = BM * ROW_BYTES;
   static constexpr int B_PIECE = BN * ROW_BYTES;
   static constexpr int STAGE_BYTES = NSPLIT * (A_PIECE + B_PIECE);
-  static constexpr int NPASS = (NSPLIT == 1) ? 1 : (NSPLIT == 2 ? 3 : 6);
+  static constexpr int NPASS = mma_passes(NSPLIT);
   static constexpr int ACC_STAGE_BYTES = (EPI != EPI_OUT) ? 2 * 64 * 64 * 4 : 0;
   static constexpr int STORE_STAGE_BYTES = (EPI != EPI_OUT) ? 8 * 4096 : 0;
   static constexpr int SMEM_AUX = 2048;                       // barriers + column labels

@@ -21,8 +21,6 @@
 
 namespace npair {
 
-#define NPAIR_LOG2E_F 1.4426950408889634f
-
 struct FusedGradParams {
   int Q, N, D;
   int num_kblocks;              // ceil(N / 32)
@@ -31,8 +29,8 @@ struct FusedGradParams {
   int chunk_kb;                 // accumulation chunk in K blocks (0 = the whole K range in one accumulator), see below
   float* part;                  // split-K partials [split][Q][ldo]
   const float* S;               // only for address checks; tiles come through the tensor map
-  const float* rowrec;          // [Q][8]  this rank's row records {m2c, thr_n, m2, label | thr_p, cA, cT, 0} (lse_rows_kernel)
-  const float* colrec;          // [N][8]  records of every column's row (== rowrec when world == 1)
+  const RowRecord* rowrec;      // [Q] this rank's row records
+  const RowRecord* colrec;      // [N] records of every column's row (== rowrec when world == 1)
   int self_offset;              // global column of local row 0
   float inv_world, log2_world;
   float sgn_p, sgn_n;           // +-1: direction of the same-/diff-label selection compare
@@ -48,9 +46,9 @@ struct FusedCfg {
   static constexpr int BM = 128, BN = 256, BK = 32;
   static constexpr int B_PIECE = BN * 64;                 // 64-byte rows (32 x 2-byte), SWIZZLE_64B
   static constexpr int S_TILE = BM * 128;                 // 128-byte rows (32 x fp32), SWIZZLE_128B
-  static constexpr int CREC = BK * 32;                    // 32 column records of 32 bytes
+  static constexpr int CREC = BK * sizeof(RowRecord);     // the K block's column records
   static constexpr int STAGE_BYTES = NSPLIT * B_PIECE + S_TILE + CREC;
-  static constexpr int NPASS = (NSPLIT == 1) ? 1 : (NSPLIT == 2 ? 3 : 6);
+  static constexpr int NPASS = mma_passes(NSPLIT);
   static constexpr int STAGES_FIT = (227 * 1024 - 2048) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*barriers*/ + 1024 /*alignment*/;
@@ -120,18 +118,18 @@ __device__ __forceinline__ float select_f32(bool c, float a, float b) {
   asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"(static_cast<int>(c)));
   return r;
 }
-__device__ __forceinline__ float pair_weight(float s, const float4& ca, const float4& cb, const RowRec& r, int m, const FusedGradParams& p) {
-  // ca = {m2c, thr_n, m2, label}, cb = {thr_p, cA, cT, -} of the column's row
-  const bool same = !(ca.w != r.lab);
+__device__ __forceinline__ float pair_weight(float s, const RowRecord& c, const RowRec& r, int m, const FusedGradParams& p) {
+  // c: the record of the column's row
+  const bool same = !(c.label() != r.lab);
   const float kn = s * p.sgn_n;                  // HARD / RELATIVE_HARD negatives compare -s
-  const float a1 = select_f32(same, fmaf(s, NPAIR_LOG2E_F, -r.m2), select_f32(kn <= r.tn, fmaf(s, NPAIR_LOG2E_F, -r.m2r), -INFINITY));
-  const float a2 = select_f32(same, fmaf(s, NPAIR_LOG2E_F, -ca.z), select_f32(kn <= ca.y, fmaf(s, NPAIR_LOG2E_F, -ca.x), -INFINITY));
+  const float a1 = select_f32(same, fmaf(s, LOG2E, -r.m2), select_f32(kn <= r.tn, fmaf(s, LOG2E, -r.m2r), -INFINITY));
+  const float a2 = select_f32(same, fmaf(s, LOG2E, -c.m2()), select_f32(kn <= c.thr_n(), fmaf(s, LOG2E, -c.m2c()), -INFINITY));
   float e1, e2;                                  // same-label: the forward row pass's exponential (fast_exp_m2)
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(a2));
   const float kp = s * p.sgn_p;
   const float w1 = select_f32(kp <= r.tp, e1 * r.cA, 0.f);
-  const float w2 = select_f32(kp <= cb.x, e2 * cb.y, 0.f);
+  const float w2 = select_f32(kp <= c.thr_p(), e2 * c.cA(), 0.f);
   const float g = select_f32(same, fmaf(w2, p.inv_world, w1), e1 + e2);
   return (m == r.self_col || m >= p.N) ? 0.f : g;
 }
@@ -141,9 +139,8 @@ __device__ __forceinline__ RowRec load_rowrec(const FusedGradParams& p, int row)
   r.m2 = 0.f; r.m2r = INFINITY; r.tp = -INFINITY; r.tn = -INFINITY; r.cA = 0.f; r.lab = 0.f;
   r.self_col = row + p.self_offset;
   if (row < p.Q) {
-    const float4 a = *reinterpret_cast<const float4*>(p.rowrec + 8ll * row);
-    const float4 b = *reinterpret_cast<const float4*>(p.rowrec + 8ll * row + 4);
-    r.m2r = a.x - p.log2_world; r.tn = a.y; r.m2 = a.z; r.lab = a.w; r.tp = b.x; r.cA = b.y;   // the row term carries no 1/world
+    const RowRecord c = p.rowrec[row];
+    r.m2r = c.m2c() - p.log2_world; r.tn = c.thr_n(); r.m2 = c.m2(); r.lab = c.label(); r.tp = c.thr_p(); r.cA = c.cA();   // the row term carries no 1/world
   }
   return r;
 }
@@ -185,14 +182,14 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
         for (int kb = kb0; kb < kb1; ++kb) {
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
           const int m0 = kb * BK;
-          const uint32_t crec_bytes = static_cast<uint32_t>(min(BK, p.N - m0)) * 32u;
+          const uint32_t crec_bytes = static_cast<uint32_t>(min(BK, p.N - m0)) * static_cast<uint32_t>(sizeof(RowRecord));
           uint8_t* st = smem + stage * Cfg::STAGE_BYTES;
           ptx::mbar_arrive_expect_tx(&full_bar[stage], NSPLIT * Cfg::B_PIECE + Cfg::S_TILE + crec_bytes);
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s)
             ptx::tma_load_3d(st + s * Cfg::B_PIECE, &tmapB, &full_bar[stage], m0, n_blk * BN, s);
           ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE, &tmapS, &full_bar[stage], m0, m_blk * BM);
-          bulk_copy_g2s(st + NSPLIT * Cfg::B_PIECE + Cfg::S_TILE, p.colrec + 8ll * m0, crec_bytes, &full_bar[stage]);
+          bulk_copy_g2s(st + NSPLIT * Cfg::B_PIECE + Cfg::S_TILE, p.colrec + m0, crec_bytes, &full_bar[stage]);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -214,19 +211,19 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
     // rows rl0 (h = 0) and rl0 + 8 (h = 1)
     auto build = [&](uint32_t (&af)[NSPLIT][4], const RowRec (&rr)[2], int st_idx, int kb, int k2) {
       const uint8_t* s_tile = smem + st_idx * Cfg::STAGE_BYTES + NSPLIT * Cfg::B_PIECE;
-      const float4* crec = reinterpret_cast<const float4*>(s_tile + Cfg::S_TILE);
+      const RowRecord* crec = reinterpret_cast<const RowRecord*>(s_tile + Cfg::S_TILE);
 #pragma unroll
       for (int t = 0; t < 2; ++t) {
         const int k = 16 * k2 + 8 * t + 2 * c4;
         const int m = kb * BK + k;
         // records of columns m and m + 1, shared by both rows
-        const float4 ca0 = crec[2 * k], cb0 = crec[2 * k + 1], ca1 = crec[2 * k + 2], cb1 = crec[2 * k + 3];
+        const RowRecord c0 = RowRecord::load(crec, k), c1 = RowRecord::load(crec, k + 1);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int rl = rl0 + 8 * h;
           const float2 s2 = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
-          const float w0 = pair_weight(s2.x, ca0, cb0, rr[h], m, p);
-          const float w1 = pair_weight(s2.y, ca1, cb1, rr[h], m + 1, p);
+          const float w0 = pair_weight(s2.x, c0, rr[h], m, p);
+          const float w1 = pair_weight(s2.y, c1, rr[h], m + 1, p);
           uint32_t o[3];
           split_pair<NSPLIT, BF16>(w0, w1, o);
 #pragma unroll

@@ -55,67 +55,15 @@ __device__ __forceinline__ void split3(float v, uint16_t& p0, uint16_t& p1, uint
     p0 = __bfloat16_as_ushort(h); p1 = __bfloat16_as_ushort(m); p2 = __bfloat16_as_ushort(__float2bfloat16_rn(r2));
   }
 }
-__host__ __device__ inline int nsplit_of(int prec) { return prec == PREC_BF16 ? 1 : (prec == PREC_FP16X2 ? 2 : 3); }
 
-// exp(x) for x <= 0 as one FMUL + MUFU.EX2 (relative error ~ (2 + 1.44|x|) ulp: 3e-7 for the |x| <= 2 of unit-norm
-// embeddings, 1e-5 only beyond |x| ~ 80 where the terms are ~1e-35 anyway).  Cheap enough to evaluate for EVERY pair,
-// which keeps the row pass and the weight builder branch-free (the reference's expf, .cu:131, under a selection branch
-// costs ~20 instructions per divergent hit).  The same function is used forward and backward, so W = e / A stays consistent.
-__device__ __forceinline__ float fast_exp(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x * 1.4426950408889634f));
-  return y;
-}
-#define NPAIR_LOG2E 1.4426950408889634f
-// exp(s - max) with the row constant pre-multiplied: m2 = max * log2(e)  ->  one FFMA + one MUFU.EX2
+// exp(s - max) with the row constant pre-multiplied, m2 = max * log2(e): one FFMA + one MUFU.EX2 (relative error ~ (2 + 1.44|x|)
+// ulp: 3e-7 for the |x| <= 2 of unit-norm embeddings).  Cheap enough to evaluate for EVERY pair, which keeps the row pass and the
+// weight builder branch-free (the reference's expf, .cu:131, under a selection branch costs ~20 instructions per divergent hit).
+// The same exponential is used forward and backward, so W = e / A stays consistent.
 __device__ __forceinline__ float fast_exp_m2(float sv, float m2) {
   float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(fmaf(sv, NPAIR_LOG2E, -m2)));
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(fmaf(sv, LOG2E, -m2)));
   return y;
-}
-
-// Every selection rule of .cu:79-120 is rewritten as ONE compare  sgn*s <= thr'  with a per-row transformed threshold:
-//   s <  t  <=>   s <= nextbelow(t)         s <= t  <=>   s <= t
-//   s >= t  <=>  -s <= -t                   s >  t  <=>  -s <= nextbelow(-t)          ALL  <=>  s <= +inf
-// (exact for every float incl. +-0 and the -FLT_MAX / FLT_MAX sentinels; NaN compares false on both sides).
-__host__ __device__ __forceinline__ float ap_sign(int m) { return (m == M_EASY || m == M_RELATIVE_EASY) ? -1.f : 1.f; }
-__host__ __device__ __forceinline__ float an_sign(int m) { return (m == M_HARD || m == M_RELATIVE_HARD) ? -1.f : 1.f; }
-__device__ __forceinline__ float ap_thr(float t, int m) {     // same-label rule on t = posi_thr + margin_ident
-  switch (m) {
-    case M_HARD: return nextafterf(t, -INFINITY);            // s <  t
-    case M_EASY: return -t;                                  // s >= t
-    case M_RAND: return INFINITY;
-    case M_RELATIVE_HARD: return t;                          // s <= t
-    default: return -t;                                      // RELATIVE_EASY: s >= t
-  }
-}
-__device__ __forceinline__ float an_thr(float t, int m) {     // diff-label rule on t = nega_thr + margin_diff
-  switch (m) {
-    case M_HARD: return nextafterf(-t, -INFINITY);           // s >  t
-    case M_EASY: return t;                                   // s <= t
-    case M_RAND: return INFINITY;
-    case M_RELATIVE_HARD: return -t;                         // s >= t
-    default: return t;                                       // RELATIVE_EASY: s <= t
-  }
-}
-
-__device__ __forceinline__ bool sel_ap(float s, float tp, int m) {   // .cu:79-98
-  switch (m) {
-    case M_HARD: return s < tp;
-    case M_EASY: return s >= tp;
-    case M_RAND: return true;
-    case M_RELATIVE_HARD: return s <= tp;
-    default: return s >= tp;
-  }
-}
-__device__ __forceinline__ bool sel_an(float s, float tn, int m) {   // .cu:100-119
-  switch (m) {
-    case M_HARD: return s > tn;
-    case M_EASY: return s <= tn;
-    case M_RAND: return true;
-    case M_RELATIVE_HARD: return s >= tn;
-    default: return s <= tn;
-  }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -228,59 +176,6 @@ void launch_prep_reduce(const float* x_local, long long n_local, const float* x_
   count_launch();
 }
 
-__global__ void absmax_asum_partial_kernel(const float* __restrict__ xl, long long nl, const float* __restrict__ xt, long long ntot,
-                                           float* __restrict__ partial, int want_scale) {
-  __shared__ float s_sum[32], s_max[32];
-  float sum = 0.f, mx = 0.f;
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nl; i += stride) sum += fabsf(xl[i]);
-  if (want_scale)
-    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < ntot; i += stride) mx = fmaxf(mx, fabsf(xt[i]));
-  sum = warp_sum(sum); mx = warp_max(mx);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { s_sum[w] = sum; s_max[w] = mx; }
-  __syncthreads();
-  if (w == 0) {
-    sum = (l < (blockDim.x >> 5)) ? s_sum[l] : 0.f;
-    mx = (l < (blockDim.x >> 5)) ? s_max[l] : 0.f;
-    sum = warp_sum(sum); mx = warp_max(mx);
-    if (l == 0) { partial[blockIdx.x] = sum; partial[1024 + blockIdx.x] = mx; }
-  }
-}
-__global__ void absmax_asum_final_kernel(const float* __restrict__ partial, int nb, BlockScalars* bs, int want_scale) {
-  __shared__ double s_sum[32];
-  __shared__ float s_max[32];
-  double sum = 0.0; float mx = 0.f;
-  for (int b = threadIdx.x; b < nb; b += blockDim.x) { sum += partial[b]; mx = fmaxf(mx, partial[1024 + b]); }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { sum += __shfl_xor_sync(0xffffffffu, sum, o); mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o)); }
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { s_sum[w] = sum; s_max[w] = mx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    sum = 0.0; mx = 0.f;
-    for (int k = 0; k < (blockDim.x >> 5); ++k) { sum += s_sum[k]; mx = fmaxf(mx, s_max[k]); }
-    bs->asum = static_cast<float>(sum);
-    bs->x_absmax = mx;
-    float sc = 1.f, inv = 1.f;
-    if (want_scale && mx > 0.f && isfinite(mx)) {
-      int e; frexpf(mx, &e);                 // mx = m * 2^e, m in [0.5,1)
-      sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e);
-    }
-    bs->x_scale = sc; bs->x_inv_scale = inv;
-  }
-}
-void launch_absmax_asum(const float* x_local, long long n_local, const float* x_total, long long n_total,
-                        float* partial, BlockScalars* bs, int want_scale, cudaStream_t st) {
-  long long nmax = n_local > n_total ? n_local : n_total;
-  int nb = static_cast<int>((nmax + 256 * 8 - 1) / (256 * 8));
-  if (nb < 1) nb = 1; if (nb > 1024) nb = 1024;
-  absmax_asum_partial_kernel<<<nb, 256, 0, st>>>(x_local, n_local, x_total, n_total, partial, want_scale);
-  count_launch();
-  absmax_asum_final_kernel<<<1, 256, 0, st>>>(partial, nb, bs, want_scale);
-  count_launch();
-}
-
 // --------------------------------------------------------------------------------------------
 // operand split: x_total fp32 [N x D] -> Xs[s][N][ldXs] (K-major for the similarity GEMM) and the transposed
 // XsT[s][D][ldXsT] (K-major for the gradient GEMM whose K is the sample index); XlT = local columns only.
@@ -316,7 +211,7 @@ __device__ __forceinline__ void split_tile(const SplitArgs& a, float sc, int til
   uint16_t* __restrict__ Xs = a.Xs; const long long ldXs = a.ldXs; uint16_t* __restrict__ XsT = a.XsT; const long long ldXsT = a.ldXsT;
   uint16_t* __restrict__ XlT = a.XlT; const long long ldXlT = a.ldXlT; const int row0 = a.row0, Q = a.Q;
   uint16_t* __restrict__ XcatA = a.XcatA; uint16_t* __restrict__ XcatB = a.XcatB; const long long Dp = a.Dp;
-  constexpr int NS = (PREC == PREC_BF16) ? 1 : (PREC == PREC_FP16X2 ? 2 : 3);
+  constexpr int NS = SPLIT_FORMATS[PREC].pieces;
   __shared__ __align__(16) uint16_t tile2[2][NS][64][40];  // [buffer][piece][d][n], row padded to 80 bytes (16-byte aligned, spreads banks)
   uint16_t (*tile)[64][40] = tile2[buf];
   const int n0 = tile_n * 32, d0 = tile_d * 64;
@@ -348,7 +243,7 @@ __device__ __forceinline__ void split_tile(const SplitArgs& a, float sc, int til
     // permutes the products inside an instruction, whose sum is order-invariant (measured: tests/diag_mma_symmetry.py),
     // so S[j][m] == S[m][j] bit for bit, on one rank and across ranks.
     if (PREC != PREC_BF16 && XcatA) {
-      const long long kcat = (PREC == PREC_FP16X2 ? 3 : 6) * Dp;
+      const long long kcat = mma_passes(NS) * Dp;
       uint16_t* ra = XcatA + static_cast<long long>(n) * kcat;
       uint16_t* rb = XcatB + static_cast<long long>(n) * kcat;
       const bool local = (n >= row0 && n < row0 + Q);        // only the rank's own rows are ever an A operand
@@ -403,9 +298,7 @@ void launch_split(const float* x_total, int N, int D, int prec, const BlockScala
                   uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st) {
   dim3 grid((D + 63) / 64, (N + 31) / 32);
   const SplitArgs a{x_total, N, D, Xs, ldXs, XsT, ldXsT, XlT, ldXlT, row0_local, Q, XcatA, XcatB, Dp};
-  if (prec == PREC_BF16) split_kernel<PREC_BF16><<<grid, 256, 0, st>>>(a, bs);
-  else if (prec == PREC_FP16X2) split_kernel<PREC_FP16X2><<<grid, 256, 0, st>>>(a, bs);
-  else split_kernel<PREC_BF16X3><<<grid, 256, 0, st>>>(a, bs);
+  with_prec(prec, [&](auto P) { split_kernel<P><<<grid, 256, 0, st>>>(a, bs); });
   count_launch();
 }
 
@@ -461,14 +354,7 @@ __global__ void __launch_bounds__(256) thresholds_kernel(RowArrays ra, int Q, in
     const float r_mn = ord2f(ra.st_minw[i]), r_mxw = ord2f(ra.st_maxw[i]), r_mxb = ord2f(ra.st_maxb[i]);
     ns += static_cast<unsigned long long>(cs);
     mn = fminf(mn, r_mn); mxw = fmaxf(mxw, r_mxw); mxb = fmaxf(mxb, r_mxb);
-    if (mp.ap_region == REGION_LOCAL) {
-      if (!is_rel(mp.ap_method)) ra.posi_thr[i] = r_mxb;                                                   // .cu:279
-      else if (sn_is_max(mp.identsn)) { if (cs == 0) atomicOr(&s_err, DERR_EMPTY_LIST); ra.posi_thr[i] = clamp_thr(r_mxw); }
-    }
-    if (mp.an_region == REGION_LOCAL) {
-      if (!is_rel(mp.an_method)) ra.nega_thr[i] = r_mn;                                                    // .cu:310
-      else if (sn_is_max(mp.diffsn)) { if (N - 1 - cs == 0) atomicOr(&s_err, DERR_EMPTY_LIST); ra.nega_thr[i] = clamp_thr(r_mxb); }
-    }
+    local_thresholds(ra, mp, i, N, cs, r_mn, r_mxw, r_mxb, &s_err);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ns += __shfl_xor_sync(0xffffffffu, ns, o);
@@ -1515,7 +1401,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
     li = lab_rows[i];
     const int self_col = i + self_offset;
     const float max_all = ord2f(ra.st_maxall[i]);
-    m2 = max_all * NPAIR_LOG2E;
+    m2 = max_all * LOG2E;
     // GLOBAL-region thresholds are block-wide scalars (thresholds_kernel / global_pick_kernel); LOCAL ones are per row
     const float posi = mp.ap_region == REGION_GLOBAL ? bs->posi_global : ra.posi_thr[i];
     const float nega = mp.an_region == REGION_GLOBAL ? bs->nega_global : ra.nega_thr[i];
@@ -1602,13 +1488,8 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
       ra.hits[2 * Q + i] = (cs > 0 && c <= min(10, lim)) ? 1 : 0;
       const float invA = A == 0.f ? 0.f : 1.f / A;              // Get_Query_Diff_Part zero rules (.cu:410-415)
       const float invT = T == 0.f ? 0.f : 1.f / T;
-      // first 16 bytes = all a diff-label pair needs.  Its backward weight exp(s - max) / T / world is evaluated by the gradient
-      // kernel as ONE exponential 2^(s*log2(e) - m2c) with m2c = max*log2(e) + log2(T) + log2(world) (T == 0: +inf, weight 0):
-      // {m2c, an_thr-transformed threshold, max*log2(e), label}; second 16 bytes = the same-label rule and the plain factors:
-      // {ap_thr threshold, weight 1/T - 1/A, 1/T, 0}
-      float4* rec = reinterpret_cast<float4*>(ra.rowscal + 8ll * i);
-      rec[0] = make_float4(T == 0.f ? INFINITY : m2 + log2f(T) + log2_world, thr_n, m2, li);
-      rec[1] = make_float4(thr_p, invT - invA, invT, 0.f);
+      const float cA = invT - invA;
+      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + log2_world, thr_n, m2, li, thr_p, cA, invT);
     }
   }
   if (!finalize) return;
@@ -1674,6 +1555,12 @@ void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_t
 //                 local = H . X_total ,  total = HT . X_local , then reduce-scatter and blend (.cu:462-497)
 // --------------------------------------------------------------------------------------------
 struct RowScal { float maxall, tp, tn, cA, cT, lab; };   // maxall: max_all*log2e; tp/tn: ap_thr / an_thr transformed thresholds
+// A row's scalars from its record, the weight factors scaled by w.  No record (no such row): the thresholds -inf select nothing.
+__device__ __forceinline__ RowScal row_scal(const RowRecord* rec, float w) {
+  if (!rec) return RowScal{0.f, -INFINITY, -INFINITY, 0.f, 0.f, 0.f};
+  const RowRecord r = *rec;
+  return RowScal{r.m2(), r.thr_p(), r.thr_n(), r.cA() * w, r.cT() * w, r.label()};
+}
 
 // r.maxall holds max_all * log2(e) (see lse_rows_kernel)
 __device__ __forceinline__ float gprime(float sv, bool same, const RowScal& r, float sgn_p, float sgn_n) {
@@ -1685,7 +1572,7 @@ __device__ __forceinline__ float gprime(float sv, bool same, const RowScal& r, f
 // four consecutive weights -> NS pieces, one 8-byte store per piece
 template <int PREC>
 __device__ __forceinline__ void store_quad(uint16_t* __restrict__ base, long long piece_stride, long long off, const float g[4]) {
-  constexpr int NS = (PREC == PREC_BF16) ? 1 : (PREC == PREC_FP16X2 ? 2 : 3);
+  constexpr int NS = SPLIT_FORMATS[PREC].pieces;
   if (g[0] == 0.f && g[1] == 0.f && g[2] == 0.f && g[3] == 0.f) {          // the common case under margin mining
 #pragma unroll
     for (int s = 0; s < NS; ++s) *reinterpret_cast<uint2*>(base + s * piece_stride + off) = make_uint2(0u, 0u);
@@ -1713,7 +1600,7 @@ __device__ __forceinline__ void store_quad(uint16_t* __restrict__ base, long lon
 template <int PREC, int MODE>
 __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
                                                             const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
-                                                            int self_offset, float inv_world, const float* __restrict__ rs_total,
+                                                            int self_offset, float inv_world, const RowRecord* __restrict__ rs_total,
                                                             MiningParams mp, RowArrays ra,
                                                             uint16_t* __restrict__ H, long long ldH, uint16_t* __restrict__ HT, long long ldHT) {
   constexpr bool SYM = (MODE != BW_SPLIT);      // both symmetric modes add the row-m term
@@ -1724,22 +1611,18 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
   const int t = threadIdx.x, tr = t >> 4, tc = t & 15;
   const float sgn_p = ap_sign(mp.ap_method), sgn_n = an_sign(mp.an_method);
   if (t < TS) {
-    const int j = a0 + t;
-    RowScal r = {0.f, -INFINITY, -INFINITY, 0.f, 0.f, 0.f};
-    if (j < Q) { const float* b = ra.rowscal + 8ll * j; r.maxall = b[2]; r.tn = b[1]; r.cT = b[6]; r.lab = b[3]; r.tp = b[4]; r.cA = b[5]; }
-    sc_a[t] = r;
+    sc_a[t] = row_scal(a0 + t < Q ? ra.rowrec + a0 + t : nullptr, 1.f);
   } else if (t < 2 * TS) {
     const int mm = t - TS, m = b0 + mm;
-    RowScal r = {0.f, -INFINITY, -INFINITY, 0.f, 0.f, 0.f};
     if (MODE == BW_SYM) {   // world == 1: column m is also a local row
-      if (m < Q) { const float* b = ra.rowscal + 8ll * m; r.maxall = b[2]; r.tn = b[1]; r.cT = b[6]; r.lab = b[3]; r.tp = b[4]; r.cA = b[5]; }
-    } else if (MODE == BW_ROWSCAL) {   // all-gathered [N][8] row records; the 1/world of .cu:474 folded into the weights
-      if (m < N) {
-        const float* b = rs_total + 8ll * m;
-        r.maxall = b[2]; r.tn = b[1]; r.cT = b[6] * inv_world; r.lab = b[3]; r.tp = b[4]; r.cA = b[5] * inv_world;
-      }
-    } else if (m < N) r.lab = lab_cols[m];
-    sc_b[mm] = r;
+      sc_b[mm] = row_scal(m < Q ? ra.rowrec + m : nullptr, 1.f);
+    } else if (MODE == BW_ROWSCAL) {   // the world's records; the 1/world of .cu:474 folded into the weights
+      sc_b[mm] = row_scal(m < N ? rs_total + m : nullptr, inv_world);
+    } else {
+      RowScal r = row_scal(nullptr, 1.f);
+      if (m < N) r.lab = lab_cols[m];
+      sc_b[mm] = r;
+    }
   }
   __syncthreads();
   const int ja0 = a0 + 4 * tr, mb0 = b0 + 4 * tc;       // my rows of block a, my columns of block b
@@ -1783,23 +1666,16 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
   }
 }
 void launch_build_weights(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, int world, int mode, const float* rs_total, MiningParams mp, RowArrays ra, int prec,
+                          int self_offset, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH, uint16_t* HT, long long ldHT, cudaStream_t st) {
   dim3 grid((N + 63) / 64, (Q + 63) / 64);
   const float inv_world = 1.f / static_cast<float>(world);
-#define NPAIR_BW_ARGS S, ldS, Q, N, lab_rows, lab_cols, self_offset, inv_world, rs_total, mp, ra, H, ldH, HT, ldHT
-#define NPAIR_LAUNCH_BW(P)                                                                            \
-  do {                                                                                                \
-    if (mode == BW_SYM) build_weights_kernel<P, BW_SYM><<<grid, 256, 0, st>>>(NPAIR_BW_ARGS);         \
-    else if (mode == BW_ROWSCAL) build_weights_kernel<P, BW_ROWSCAL><<<grid, 256, 0, st>>>(NPAIR_BW_ARGS); \
-    else build_weights_kernel<P, BW_SPLIT><<<grid, 256, 0, st>>>(NPAIR_BW_ARGS);                      \
-  } while (0)
-  if (prec == PREC_BF16) NPAIR_LAUNCH_BW(PREC_BF16);
-  else if (prec == PREC_FP16X2) NPAIR_LAUNCH_BW(PREC_FP16X2);
-  else NPAIR_LAUNCH_BW(PREC_BF16X3);
+  with_prec(prec, [&](auto P) {
+    auto kernel = mode == BW_SYM ? build_weights_kernel<P, BW_SYM> : mode == BW_ROWSCAL ? build_weights_kernel<P, BW_ROWSCAL>
+                                                                                        : build_weights_kernel<P, BW_SPLIT>;
+    kernel<<<grid, 256, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, inv_world, rs_total, mp, ra, H, ldH, HT, ldHT);
+  });
   count_launch();
-#undef NPAIR_LAUNCH_BW
-#undef NPAIR_BW_ARGS
 }
 
 // --------------------------------------------------------------------------------------------

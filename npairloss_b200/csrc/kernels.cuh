@@ -3,6 +3,8 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cmath>
+#include <type_traits>
 
 namespace npair {
 
@@ -13,8 +15,79 @@ enum { M_HARD = 0, M_EASY = 1, M_RAND = 2, M_RELATIVE_HARD = 3, M_RELATIVE_EASY 
 // device error bits (the reference has undefined behaviour in these cases: SURVEY.md 9.4 Q5)
 enum { DERR_EMPTY_LIST = 1, DERR_POS_RANGE = 2 };
 
-// operand split formats (see gemm_wgmma.cuh)
+constexpr float LOG2E = 1.4426950408889634f;
+
+// Operand split formats (gemm_wgmma.cuh): an fp32 value is stored as `pieces` 2-byte pieces whose sum reproduces it.
 enum { PREC_BF16X3 = 0, PREC_BF16 = 1, PREC_FP16X2 = 2 };
+struct SplitFormat {
+  int pieces;   // 2-byte pieces per value, largest first
+  bool bf16;    // element type of the pieces: bf16, else fp16
+};
+constexpr SplitFormat SPLIT_FORMATS[3] = {{3, true} /*PREC_BF16X3*/, {1, true} /*PREC_BF16*/, {2, false} /*PREC_FP16X2*/};
+// MMA passes of a product of two operands of `pieces` pieces: one per piece pair (a, b) with a + b < pieces, in the order of
+// pass_pieces.  The K-concatenated operands of the bitwise-symmetric similarity GEMM hold one Dp-long segment per pass (split_tile),
+// so their K extent is mma_passes(pieces) * Dp.
+__host__ __device__ constexpr int mma_passes(int pieces) { return pieces * (pieces + 1) / 2; }
+// Calls f(std::integral_constant<int, PREC>()) for the runtime format `prec`: where a kernel instantiation is chosen by format.
+template <class F>
+inline decltype(auto) with_prec(int prec, F&& f) {
+  if (prec == PREC_BF16) return f(std::integral_constant<int, PREC_BF16>());
+  if (prec == PREC_FP16X2) return f(std::integral_constant<int, PREC_FP16X2>());
+  return f(std::integral_constant<int, PREC_BF16X3>());
+}
+
+// Every selection rule of .cu:79-120 is rewritten as ONE compare  sgn*s <= thr'  with a per-row transformed threshold:
+//   s <  t  <=>   s <= nextbelow(t)         s <= t  <=>   s <= t
+//   s >= t  <=>  -s <= -t                   s >  t  <=>  -s <= nextbelow(-t)          ALL  <=>  s <= +inf
+// (exact for every float incl. +-0 and the -FLT_MAX / FLT_MAX sentinels; NaN compares false on both sides).
+__host__ __device__ __forceinline__ float ap_sign(int m) { return (m == M_EASY || m == M_RELATIVE_EASY) ? -1.f : 1.f; }
+__host__ __device__ __forceinline__ float an_sign(int m) { return (m == M_HARD || m == M_RELATIVE_HARD) ? -1.f : 1.f; }
+__device__ __forceinline__ float ap_thr(float t, int m) {     // same-label rule on t = posi_thr + margin_ident
+  switch (m) {
+    case M_HARD: return nextafterf(t, -INFINITY);            // s <  t
+    case M_EASY: return -t;                                  // s >= t
+    case M_RAND: return INFINITY;
+    case M_RELATIVE_HARD: return t;                          // s <= t
+    default: return -t;                                      // RELATIVE_EASY: s >= t
+  }
+}
+__device__ __forceinline__ float an_thr(float t, int m) {     // diff-label rule on t = nega_thr + margin_diff
+  switch (m) {
+    case M_HARD: return nextafterf(-t, -INFINITY);           // s >  t
+    case M_EASY: return t;                                   // s <= t
+    case M_RAND: return INFINITY;
+    case M_RELATIVE_HARD: return -t;                         // s >= t
+    default: return t;                                       // RELATIVE_EASY: s <= t
+  }
+}
+
+// What the backward needs of one row, written by the forward row pass (lse_rows_kernel).  It crosses GPUs as raw bytes (peer-memory
+// pushes, the NCCL all-gather, npair_row_scalars / npair_backward_gathered), so this is the one description of its layout.  The two
+// 16-byte halves are loaded and stored as vectors; the first holds all that a diff-label pair needs.
+//   m2     max_all * log2(e), the row's exponent offset
+//   m2c    m2 + log2(T) + log2(world) (+inf when T == 0): a diff-label weight exp(s - max) / T / world is ONE exponential 2^(s*log2(e) - m2c)
+//   thr_n  the an_thr-transformed diff-label threshold;  thr_p  the ap_thr-transformed same-label threshold
+//   cA     same-label weight factor 1/T - 1/A;  cT  diff-label weight factor 1/T
+struct RowRecord {
+  float4 lo, hi;   // {m2c, thr_n, m2, label}, {thr_p, cA, cT, 0}
+  __host__ __device__ static RowRecord make(float m2c, float thr_n, float m2, float label, float thr_p, float cA, float cT) {
+    return RowRecord{make_float4(m2c, thr_n, m2, label), make_float4(thr_p, cA, cT, 0.f)};
+  }
+  // records[k] addressed in 16-byte halves (the gradient kernel's shared-memory reads are scheduled for this address arithmetic)
+  __host__ __device__ static RowRecord load(const RowRecord* records, int k) {
+    const float4* h = reinterpret_cast<const float4*>(records);
+    return RowRecord{h[2 * k], h[2 * k + 1]};
+  }
+  __host__ __device__ float m2c() const { return lo.x; }
+  __host__ __device__ float thr_n() const { return lo.y; }
+  __host__ __device__ float m2() const { return lo.z; }
+  __host__ __device__ float label() const { return lo.w; }
+  __host__ __device__ float thr_p() const { return hi.x; }
+  __host__ __device__ float cA() const { return hi.y; }
+  __host__ __device__ float cT() const { return hi.z; }
+};
+static_assert(sizeof(RowRecord) == 32, "row records are exchanged as 32 raw bytes");
+constexpr long long ROW_RECORD_FLOATS = sizeof(RowRecord) / sizeof(float);   // exchanges count floats
 
 // Global (per-rank-block) scalars living in device memory.
 struct BlockScalars {
@@ -53,9 +126,7 @@ struct RowArrays {
   // forward row results
   float *A, *T, *logv;
   int* hits;                 // [3][Q] retrieval hit flags for k=1,5,10
-  // row scalars consumed by the backward: [Q][8] floats {m2c, thr_n', max_all*log2e, label | thr_p', cA, cT, 0} (see lse_rows_kernel)
-  // (one 32-byte record per row: all-gathered as is when world > 1, bulk-copied per K block by the fused gradient kernel)
-  float* rowscal;
+  RowRecord* rowrec;         // [Q] what the backward needs of each row
 };
 
 // order-preserving float <-> uint32 map so atomicMin/atomicMax work on floats of either sign
@@ -82,8 +153,6 @@ extern unsigned long long g_kernel_launches;
 inline void count_launch(int n = 1) { g_kernel_launches += static_cast<unsigned long long>(n); }
 
 // launchers (kernels.cu)
-void launch_absmax_asum(const float* x_local, long long n_local, const float* x_total, long long n_total,
-                        float* partial /*[2*1024]*/, BlockScalars* bs, int want_scale, cudaStream_t st);
 void launch_prep_reduce(const float* x_local, long long n_local, const float* x_total, long long n_total, float* partial /*[2*1024]*/,
                         int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st);
 void launch_split(const float* x_total, int N, int D, int prec, const BlockScalars* bs,
@@ -114,11 +183,11 @@ void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* l
                      int world, float* xout /*world scope: 7 floats of partial tops, else NULL*/, unsigned int seq, int row0, int rows,
                      bool finalize, cudaStream_t st);
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st);
-// mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-scalar
-// exchange: rs_total = all-gathered [world][5][Q] row scalars)
+// mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-record
+// exchange: rs_total = the world's N records, all-gathered)
 enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
 void launch_build_weights(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, int world, int mode, const float* rs_total, MiningParams mp, RowArrays ra, int prec,
+                          int self_offset, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH /*Np*/, uint16_t* HT, long long ldHT /*Qp*/, cudaStream_t st);
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);

@@ -27,6 +27,20 @@ __device__ __forceinline__ float clamp_thr(float v) { return v >= 0.f ? v : -FLT
 __host__ __device__ __forceinline__ bool is_rel(int m) { return m == M_RELATIVE_HARD || m == M_RELATIVE_EASY; }
 __host__ __device__ inline bool sn_is_max(float sn) { return sn >= 0.f && static_cast<int>(sn) == 0; }   // pos = size-1
 
+// The LOCAL-region thresholds of row i that are closed forms of its statistics (cs same-label pairs, min / max same-label and max
+// diff-label similarity); a relative rule with any other SN is left to the radix select.  An empty list sets DERR_EMPTY_LIST in *err.
+__device__ __forceinline__ void local_thresholds(const RowArrays& ra, const MiningParams& mp, int i, int N, int cs, float r_mn, float r_mxw,
+                                                 float r_mxb, int* err) {
+  if (mp.ap_region == REGION_LOCAL) {
+    if (!is_rel(mp.ap_method)) ra.posi_thr[i] = r_mxb;                                                   // .cu:279
+    else if (sn_is_max(mp.identsn)) { if (cs == 0) atomicOr(err, DERR_EMPTY_LIST); ra.posi_thr[i] = clamp_thr(r_mxw); }
+  }
+  if (mp.an_region == REGION_LOCAL) {
+    if (!is_rel(mp.an_method)) ra.nega_thr[i] = r_mn;                                                    // .cu:310
+    else if (sn_is_max(mp.diffsn)) { if (N - 1 - cs == 0) atomicOr(err, DERR_EMPTY_LIST); ra.nega_thr[i] = clamp_thr(r_mxb); }
+  }
+}
+
 // Block-wide (or, world scope, world-wide) sizes / extrema -> GLOBAL-region thresholds and the arming of the radix selects (.cu:292-337)
 __device__ inline void finish_thresholds(unsigned long long n_same, unsigned long long n_diff, float gmin_w, float gmax_w, float gmax_b, int err,
                                   const MiningParams& mp, BlockScalars* bs) {
@@ -87,14 +101,7 @@ __device__ inline void thresholds_one_block(RowArrays ra, int Q, int N, const Mi
       const float r_mn = ord2f(a_[u]), r_mxw = ord2f(b_[u]), r_mxb = ord2f(c_[u]);
       ns += static_cast<unsigned long long>(cs);
       mn = fminf(mn, r_mn); mxw = fmaxf(mxw, r_mxw); mxb = fmaxf(mxb, r_mxb);
-      if (mp.ap_region == REGION_LOCAL) {
-        if (!is_rel(mp.ap_method)) ra.posi_thr[i] = r_mxb;                                                   // .cu:279
-        else if (sn_is_max(mp.identsn)) { if (cs == 0) atomicOr(s_err, DERR_EMPTY_LIST); ra.posi_thr[i] = clamp_thr(r_mxw); }
-      }
-      if (mp.an_region == REGION_LOCAL) {
-        if (!is_rel(mp.an_method)) ra.nega_thr[i] = r_mn;                                                    // .cu:310
-        else if (sn_is_max(mp.diffsn)) { if (N - 1 - cs == 0) atomicOr(s_err, DERR_EMPTY_LIST); ra.nega_thr[i] = clamp_thr(r_mxb); }
-      }
+      local_thresholds(ra, mp, i, N, cs, r_mn, r_mxw, r_mxb, s_err);
     }
   }
 #pragma unroll
