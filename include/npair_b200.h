@@ -217,6 +217,43 @@ int npair_debug_mma_symmetric(int precision);
 int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const float* d_A, const float* d_B, float* d_C,
                      void* stream);
 
+/* ---- retrieval evaluation, not part of the reference layer (DESIGN 8) ----
+ * Recall@K of a whole embedding set on the tensor cores, without ever storing the nq x ng similarity matrix.  For query i with label
+ * l_i and the library's similarity s_ij in operand format `precision` (NPAIR_PREC_*), over gallery rows j other than query i's own:
+ *   p*_i   = max of s_ij over gallery rows with label l_i (undefined when there is none)
+ *   rank_i = #{ j != self(i) : s_ij >= p*_i }   (0 when p*_i is undefined, else >= 1: ties count against the positive)
+ *   Recall@K = #{ i : 1 <= rank_i <= K } / nq
+ * Two sweeps of the similarity GEMM: one for p* (the layer's statistics epilogue), one counting the columns that reach it.  Both
+ * sweeps use the same tile geometry and the GEMM is bitwise deterministic, so the ranks are the same bits on every call.  Inputs are
+ * used as given (for cosine similarity, call npair_l2normalize_forward first).  Memory is O((nq + ng) * D).
+ * self_offset: -1 when queries and gallery are disjoint; k >= 0 when query i is gallery row k + i.  When the query and gallery
+ * pointers (features and labels) are the same and self_offset = 0 (self-retrieval over the whole set), only the similarity tiles
+ * that touch the upper triangle are computed.  An evaluator, like a layer context, is not re-entrant. */
+typedef struct npair_eval npair_eval;
+/* Device memory an evaluator of this capacity allocates: the two K-concatenated operands, (max_queries + max_gallery) * D * 2 bytes
+ * times 1 / 3 / 6 (bf16 / fp16x2 / bf16x3), 20 bytes per query and 8 bytes per symmetric 128 x 256 tile.  0 for invalid arguments. */
+size_t npair_eval_workspace_bytes(int32_t max_queries, int32_t max_gallery, int32_t D, int32_t precision);
+/* device = -1: the current device.  NPAIR_E_ARG for invalid arguments, NPAIR_E_CUDA without an sm_90 device (no CPU fallback). */
+int npair_eval_create(int32_t max_queries, int32_t max_gallery, int32_t D, int32_t precision, int32_t device, npair_eval** out);
+void npair_eval_destroy(npair_eval* ev);
+const char* npair_eval_last_error(const npair_eval* ev);   /* ev may be NULL: last npair_eval_create error of this thread */
+/* One call.  d_query nq x D and d_qlabel[nq], d_gallery ng x D and d_glabel[ng] (fp32, row-major, on the evaluator's device), with
+ * 1 <= nq <= max_queries, 1 <= ng <= max_gallery, self_offset = -1 or 0 <= self_offset <= ng - nq.  Writes d_rank[nq] (int32);
+ * asynchronous on `stream`. */
+int npair_eval_rank(npair_eval* ev, const float* d_query, const float* d_qlabel, int32_t nq, const float* d_gallery, const float* d_glabel,
+                    int32_t ng, int32_t self_offset, int32_t* d_rank, void* stream);
+/* Two-phase form for a gallery sharded across GPUs or calls (the library does no collective, as with npair_forward_gathered).  The
+ * gallery shard holds global gallery rows [gallery_row0, gallery_row0 + ng); self_offset is global (-1: disjoint).  absmax >= 0 is
+ * max|x| over the queries and the WHOLE gallery, so that every shard splits its operands identically.
+ *   phase 1: d_best[nq] = each query's best positive on this shard, or -inf.       The caller max-reduces the shards' d_best.
+ *   phase 2: d_count[nq] = #{ columns of this shard >= d_cut[i] }, self excluded;  The caller sum-reduces the shards' d_count:
+ *            0 for a row whose cut is -inf.                                        that is rank. */
+int npair_eval_best_positive(npair_eval* ev, const float* d_query, const float* d_qlabel, int32_t nq, const float* d_gallery,
+                             const float* d_glabel, int32_t ng, int32_t self_offset, int32_t gallery_row0, float absmax, float* d_best,
+                             void* stream);
+int npair_eval_count(npair_eval* ev, const float* d_query, int32_t nq, const float* d_gallery, int32_t ng, int32_t self_offset,
+                     int32_t gallery_row0, float absmax, const float* d_cut, int32_t* d_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -41,7 +41,10 @@ def sim_block_flags(rows: int) -> int:
 
 EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_id", "npair_create", "npair_create_with_comm",
            "npair_destroy", "npair_forward", "npair_backward", "npair_forward_backward", "npair_forward_gathered", "npair_backward_partial", "npair_bwd_exchange_mode", "npair_row_scalars", "npair_backward_gathered", "npair_profile_enable", "npair_profile_read", "npair_kernel_launches", "npair_util_f64_to_f32", "npair_util_f32_to_f64", "npair_last_error", "npair_version", "npair_debug_read",
-           "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward"]
+           "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
+           # retrieval evaluation (not part of the reference layer)
+           "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
+           "npair_eval_best_positive", "npair_eval_count"]
 
 _LIB = None
 
@@ -92,6 +95,17 @@ def lib():
         L.npair_debug_gemm.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
         L.npair_l2normalize_forward.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
         L.npair_l2normalize_backward.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp]
+        i32 = C.c_int32
+        L.npair_eval_workspace_bytes.argtypes = [i32, i32, i32, i32]
+        L.npair_eval_workspace_bytes.restype = C.c_size_t
+        L.npair_eval_create.argtypes = [i32, i32, i32, i32, i32, C.POINTER(vp)]
+        L.npair_eval_destroy.argtypes = [vp]
+        L.npair_eval_destroy.restype = None
+        L.npair_eval_last_error.argtypes = [vp]
+        L.npair_eval_last_error.restype = C.c_char_p
+        L.npair_eval_rank.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, vp]
+        L.npair_eval_best_positive.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, i32, C.c_float, vp, vp]
+        L.npair_eval_count.argtypes = [vp, vp, i32, vp, i32, i32, i32, C.c_float, vp, vp, vp]
         _LIB = L
     return _LIB
 
@@ -215,6 +229,75 @@ class Context:
         out = np.zeros(n, dtype=np.float32)
         self._check(lib().npair_debug_read(self._h, which, out.ctypes.data_as(C.POINTER(C.c_float)), n))
         return out
+
+
+def eval_workspace_bytes(max_queries: int, max_gallery: int, D: int, precision: int = PREC_FP32_FP16X2) -> int:
+    """Device bytes an Evaluator of this capacity allocates (0 for invalid arguments)."""
+    return int(lib().npair_eval_workspace_bytes(max_queries, max_gallery, D, precision))
+
+
+class Evaluator:
+    """Retrieval evaluation (include/npair_b200.h, DESIGN 8): the rank of every query's best positive among the gallery, computed on
+    the tensor cores without storing the similarity matrix.  Takes contiguous CUDA fp32 tensors; results are int32 / fp32 CUDA
+    tensors, produced asynchronously on the current stream."""
+
+    def __init__(self, max_queries: int, max_gallery: int, D: int, precision: int = PREC_FP32_FP16X2, device: int = -1):
+        L = lib()
+        self.max_queries, self.max_gallery, self.D, self.precision = max_queries, max_gallery, D, precision
+        self._h = C.c_void_p()
+        rc = L.npair_eval_create(max_queries, max_gallery, D, precision, device, C.byref(self._h))
+        if rc:
+            raise NpairError(rc, L.npair_eval_last_error(None).decode())
+
+    def close(self):
+        if self._h:
+            lib().npair_eval_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, rc):
+        if rc:
+            raise NpairError(rc, lib().npair_eval_last_error(self._h).decode())
+
+    @staticmethod
+    def _arg(t, dim):
+        import torch
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == dim):
+            raise TypeError("expected a contiguous CUDA float32 tensor of %d dimension(s)" % dim)
+        return t.data_ptr()
+
+    def rank(self, query, qlabel, gallery, glabel, self_offset=-1):
+        """int32 rank[nq] (npair_eval_rank)."""
+        import torch
+        rank = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
+        self._check(lib().npair_eval_rank(self._h, self._arg(query, 2), self._arg(qlabel, 1), query.shape[0], self._arg(gallery, 2),
+                                          self._arg(glabel, 1), gallery.shape[0], self_offset, rank.data_ptr(),
+                                          torch.cuda.current_stream().cuda_stream))
+        return rank
+
+    def best_positive(self, query, qlabel, gallery, glabel, absmax, self_offset=-1, gallery_row0=0):
+        """Phase 1 on one gallery shard: fp32 best[nq], -inf where the shard holds no positive."""
+        import torch
+        best = torch.empty(query.shape[0], dtype=torch.float32, device=query.device)
+        self._check(lib().npair_eval_best_positive(self._h, self._arg(query, 2), self._arg(qlabel, 1), query.shape[0],
+                                                   self._arg(gallery, 2), self._arg(glabel, 1), gallery.shape[0], self_offset,
+                                                   gallery_row0, C.c_float(absmax), best.data_ptr(),
+                                                   torch.cuda.current_stream().cuda_stream))
+        return best
+
+    def count(self, query, gallery, cut, absmax, self_offset=-1, gallery_row0=0):
+        """Phase 2 on one gallery shard: int32 count[nq] of the shard's columns >= cut (0 where cut is -inf)."""
+        import torch
+        count = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
+        self._check(lib().npair_eval_count(self._h, self._arg(query, 2), query.shape[0], self._arg(gallery, 2), gallery.shape[0],
+                                           self_offset, gallery_row0, C.c_float(absmax), self._arg(cut, 1), count.data_ptr(),
+                                           torch.cuda.current_stream().cuda_stream))
+        return count
 
 
 def debug_gemm(precision, backend, A, B):

@@ -181,6 +181,8 @@ static GemmKernel sim_gemm_t(int epi) {
     case EPI_STATS: return gemm_t<1, BF16, EPI_STATS, 64>();
     case EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STATS | EPI_SYM, 64>();
     case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
+    case EPI_COUNT: return gemm_t<1, BF16, EPI_COUNT, 64>();                       // retrieval evaluation
+    case EPI_COUNT | EPI_SYM: return gemm_t<1, BF16, EPI_COUNT | EPI_SYM, 64>();
     default: return GemmKernel{nullptr, 0, 0};
   }
 }
@@ -1516,6 +1518,252 @@ done:
   cudaFree(As); cudaFree(Bs); cudaFree(dummyT); cudaFree(bs); cudaFree(partial);
 #undef DG_TRY
   return rc;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ retrieval evaluation (DESIGN 8)
+// Not part of the reference layer.  Queries go to the A format and gallery rows to the B format of the K-concatenated operands, so the
+// similarity GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
+enum { E_CAT_A, E_CAT_B, E_ROWS, E_BS, E_SYM_TILES, E_COUNT_BUFS };
+static constexpr int EVAL_ROW_WORDS = 5;        // EvalRows: four ordered-uint statistics and the same-label count per query
+static constexpr int EVAL_NO_SELF = -(1 << 30); // a self offset that matches no column (rows and columns stay below 2^30)
+
+struct EvalPlan {
+  int max_q, max_g, D, prec;
+  long long Dp, kcat;           // padded feature extent, K extent of the concatenated operands (mma_passes * Dp)
+  int n_sym_tiles;              // tile-list capacity: self-retrieval over min(max_q, max_g) rows
+  size_t bytes[E_COUNT_BUFS];
+};
+
+static int eval_validate(long long max_q, long long max_g, long long D, int prec, std::string* err) {
+  if (max_q < 1 || max_g < 1 || D < 1) { *err = "max_queries, max_gallery and D must be >= 1"; return NPAIR_E_ARG; }
+  if (max_q >= (1 << 30) || max_g >= (1 << 30) || D >= (1 << 24)) { *err = "max_queries and max_gallery must be < 2^30, D < 2^24"; return NPAIR_E_ARG; }
+  if (prec < 0 || prec > 2) { *err = "bad precision"; return NPAIR_E_ARG; }
+  return NPAIR_OK;
+}
+
+static EvalPlan eval_plan_of(int max_q, int max_g, int D, int prec) {
+  EvalPlan p{};
+  p.max_q = max_q; p.max_g = max_g; p.D = D; p.prec = prec;
+  p.Dp = round_up(D, 64);
+  p.kcat = mma_passes(SPLIT_FORMATS[prec].pieces) * p.Dp;
+  const int n = max_q < max_g ? max_q : max_g;
+  const long long tm = (n + 127) / 128, tn = (n + 255) / 256;
+  for (long long mb = 0; mb < tm; ++mb) p.n_sym_tiles += static_cast<int>(tn - mb / 2);   // sym_tile_list(n, n).size()
+  size_t* b = p.bytes;
+  b[E_CAT_A] = 2ull * max_q * p.kcat;
+  b[E_CAT_B] = 2ull * max_g * p.kcat;
+  b[E_ROWS] = 4ull * EVAL_ROW_WORDS * max_q + 16;     // + the absmax word
+  b[E_BS] = sizeof(BlockScalars);
+  b[E_SYM_TILES] = sizeof(int2) * p.n_sym_tiles;
+  return p;
+}
+
+struct npair_eval : EvalPlan {
+  int device = -1, sms = 0;
+  uint16_t *catA = nullptr, *catB = nullptr;
+  void* rows = nullptr;
+  EvalRows er{};
+  unsigned int* absmax_bits = nullptr;
+  BlockScalars* bs = nullptr;
+  int2* sym_tiles = nullptr;
+  int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
+  std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
+  std::string err;
+};
+
+extern "C" {
+
+size_t npair_eval_workspace_bytes(int32_t max_q, int32_t max_g, int32_t D, int32_t prec) {
+  std::string e;
+  if (eval_validate(max_q, max_g, D, prec, &e) != NPAIR_OK) return 0;
+  const EvalPlan p = eval_plan_of(max_q, max_g, D, prec);
+  size_t total = 0;
+  for (size_t b : p.bytes) total += b;
+  return total;
+}
+
+const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
+
+void npair_eval_destroy(npair_eval* ev) {
+  if (!ev) return;
+  if (ev->device >= 0) cudaSetDevice(ev->device);
+  cudaFree(ev->catA); cudaFree(ev->catB); cudaFree(ev->rows); cudaFree(ev->bs); cudaFree(ev->sym_tiles);
+  delete ev;
+}
+
+int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int32_t device, npair_eval** out) {
+  if (!out) { g_create_err = "null out"; return NPAIR_E_ARG; }
+  *out = nullptr;
+  const int rc = eval_validate(max_q, max_g, D, prec, &g_create_err);
+  if (rc != NPAIR_OK) return rc;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) {
+    g_create_err = "no CUDA device: libnpair_b200 has no CPU fallback (the oracle under oracle/ is test-only)";
+    return NPAIR_E_CUDA;
+  }
+  npair_eval* ev = new npair_eval();
+  static_cast<EvalPlan&>(*ev) = eval_plan_of(max_q, max_g, D, prec);
+#define EVAL_CREATE_TRY(call)                                                                             \
+  do {                                                                                                    \
+    cudaError_t e__ = (call);                                                                             \
+    if (e__ != cudaSuccess) {                                                                             \
+      g_create_err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);     \
+      npair_eval_destroy(ev); return NPAIR_E_CUDA;                                                        \
+    }                                                                                                     \
+  } while (0)
+  if (device >= 0) EVAL_CREATE_TRY(cudaSetDevice(device));
+  EVAL_CREATE_TRY(cudaGetDevice(&ev->device));
+  cudaDeviceProp prop;
+  EVAL_CREATE_TRY(cudaGetDeviceProperties(&prop, ev->device));
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_err = fmt("device %d is sm_%d%d; this library contains sm_90a code only", ev->device, prop.major, prop.minor);
+    npair_eval_destroy(ev); return NPAIR_E_CUDA;
+  }
+  ev->sms = prop.multiProcessorCount;
+  const size_t* b = ev->bytes;
+  EVAL_CREATE_TRY(dev_alloc(&ev->catA, b[E_CAT_A], false));
+  EVAL_CREATE_TRY(dev_alloc(&ev->catB, b[E_CAT_B], false));
+  EVAL_CREATE_TRY(dev_alloc(&ev->rows, b[E_ROWS], true));
+  EVAL_CREATE_TRY(dev_alloc(&ev->bs, b[E_BS], true));
+  EVAL_CREATE_TRY(dev_alloc(&ev->sym_tiles, b[E_SYM_TILES], false));
+  uint32_t* w = static_cast<uint32_t*>(ev->rows);
+  ev->er.st_minw = w; w += max_q; ev->er.st_maxw = w; w += max_q; ev->er.st_maxb = w; w += max_q; ev->er.st_maxall = w; w += max_q;
+  ev->er.cnt_same = reinterpret_cast<int*>(w); w += max_q;
+  ev->absmax_bits = w;
+  const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM};
+  for (int epi : epis) EVAL_CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
+#undef EVAL_CREATE_TRY
+  *out = ev;
+  return NPAIR_OK;
+}
+
+}  // extern "C"
+
+// Arguments shared by the three calls.  self_offset is global, the shard holds gallery rows [gallery_row0, gallery_row0 + ng).
+static int eval_check(npair_eval* ev, const float* q, int nq, const float* g, int ng, int self_offset, int gallery_row0, float absmax,
+                      bool whole_gallery) {
+  if (!q || !g) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (nq < 1 || ng < 1) { ev->err = "nq and ng must be >= 1"; return NPAIR_E_ARG; }
+  if (nq > ev->max_q || ng > ev->max_g) { ev->err = fmt("nq = %d, ng = %d exceed the evaluator's capacity (%d, %d)", nq, ng, ev->max_q, ev->max_g); return NPAIR_E_ARG; }
+  if (self_offset < -1) { ev->err = "self_offset must be -1 (disjoint sets) or >= 0"; return NPAIR_E_ARG; }
+  if (whole_gallery && self_offset >= 0 && static_cast<long long>(self_offset) + nq > ng) { ev->err = "self_offset + nq exceeds ng"; return NPAIR_E_ARG; }
+  if (gallery_row0 < 0) { ev->err = "gallery_row0 must be >= 0"; return NPAIR_E_ARG; }
+  if (!(absmax >= 0.f) && !whole_gallery) { ev->err = "absmax must be max|x| over the queries and the whole gallery (>= 0)"; return NPAIR_E_ARG; }
+  if (!std::isfinite(absmax) && !whole_gallery) { ev->err = "absmax must be finite"; return NPAIR_E_ARG; }
+  return NPAIR_OK;
+}
+
+// Self column of query 0 inside the shard (EVAL_NO_SELF: none), and whether the sweeps use the symmetric tile list: the query set is
+// the whole gallery shard, as one buffer, with every query its own row
+static int eval_self_col(int self_offset, int gallery_row0) { return self_offset < 0 ? EVAL_NO_SELF : self_offset - gallery_row0; }
+static bool eval_sym(const float* q, int nq, const float* g, int ng, int self_col) { return q == g && nq == ng && self_col == 0; }
+
+// Operand preparation: the statistics reset, the pre-scale (from max|x| over both sets unless the caller gives it) and both operands
+static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, int ng, float absmax, bool sym, cudaStream_t st) {
+  const long long D = ev->D;
+  unsigned int* amx = nullptr;
+  if (absmax < 0.f && ev->prec == PREC_FP16X2) {
+    amx = ev->absmax_bits;
+    CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
+  }
+  launch_eval_prep(q, nq * D, sym ? nullptr : g, ng * D, amx, ev->er, nq, ev->sms, st);
+  launch_eval_split(q, nq, ev->D, ev->Dp, ev->prec, 0, absmax, amx, ev->bs, ev->catA, st);
+  launch_eval_split(g, ng, ev->D, ev->Dp, ev->prec, 1, absmax, amx, ev->bs, ev->catB, st);
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+// One sweep of the similarity GEMM over the prepared operands: EPI_STATS (labels) or EPI_COUNT (cut, count), + EPI_SYM when `sym`
+static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, const float* ql, const float* gl, const float* cut, int32_t* count,
+                      bool sym, cudaStream_t st) {
+  GemmParams gp; memset(&gp, 0, sizeof(gp));
+  gp.M = nq; gp.Nn = ng;
+  gp.num_kblocks = static_cast<int>(ev->kcat / 64);
+  gp.tiles_m = (nq + 127) / 128; gp.tiles_n = (ng + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+  gp.dev_scale = &ev->bs->x_inv_scale;
+  gp.self_offset = self_col;
+  if (sym) {
+    if (ev->sym_n != nq) {
+      ev->sym_host = sym_tile_list(nq, nq);
+      CUDA_TRY(ev, cudaMemcpyAsync(ev->sym_tiles, ev->sym_host.data(), sizeof(int2) * ev->sym_host.size(), cudaMemcpyHostToDevice, st));
+      ev->sym_n = nq;
+    }
+    epi |= EPI_SYM;
+    gp.tile_list = ev->sym_tiles; gp.num_tiles_list = static_cast<int>(ev->sym_host.size());
+  }
+  if (epi & EPI_STATS) {
+    gp.lab_rows = ql; gp.lab_cols = gl;
+    gp.st_minw = ev->er.st_minw; gp.st_maxw = ev->er.st_maxw; gp.st_maxb = ev->er.st_maxb; gp.st_maxall = ev->er.st_maxall;
+    gp.cnt_same = ev->er.cnt_same;
+  } else {
+    gp.cut = cut; gp.count = count;
+  }
+  CUtensorMap ta, tb;
+  std::string te;
+  if (!make_tmap_pieces(&ta, ev->catA, static_cast<int>(ev->kcat), nq, 1, ev->kcat, static_cast<long long>(nq) * ev->kcat, 64, 128, &te) ||
+      !make_tmap_pieces(&tb, ev->catB, static_cast<int>(ev->kcat), ng, 1, ev->kcat, static_cast<long long>(ng) * ev->kcat, 64, 256, &te)) {
+    ev->err = te; return NPAIR_E_CUDA;
+  }
+  CUDA_TRY(ev, launch_gemm(ev->prec, epi, ta, tb, ta, gp, ev->sms, st));
+  return NPAIR_OK;
+}
+
+extern "C" {
+
+int npair_eval_rank(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng, int32_t self_offset,
+                    int32_t* d_rank, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
+  if (rc != NPAIR_OK) return rc;
+  if (!ql || !gl || !d_rank) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(ev, cudaSetDevice(ev->device));
+  const int self_col = eval_self_col(self_offset, 0);
+  const bool sym = eval_sym(q, nq, g, ng, self_col);
+  float* cut = reinterpret_cast<float*>(ev->er.st_minw);   // p* overwrites a statistic sweep 2 does not read
+  if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
+  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
+  launch_eval_best(ev->er, nq, cut, st);
+  CUDA_TRY(ev, cudaMemsetAsync(d_rank, 0, sizeof(int32_t) * nq, st));
+  if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, cut, d_rank, sym, st)) != NPAIR_OK) return rc;
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+int npair_eval_best_positive(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng,
+                             int32_t self_offset, int32_t gallery_row0, float absmax, float* d_best, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
+  if (rc != NPAIR_OK) return rc;
+  if (!ql || !gl || !d_best) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(ev, cudaSetDevice(ev->device));
+  const int self_col = eval_self_col(self_offset, gallery_row0);
+  const bool sym = eval_sym(q, nq, g, ng, self_col);
+  if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
+  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
+  launch_eval_best(ev->er, nq, d_best, st);
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g, int32_t ng, int32_t self_offset, int32_t gallery_row0,
+                     float absmax, const float* d_cut, int32_t* d_count, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
+  if (rc != NPAIR_OK) return rc;
+  if (!d_cut || !d_count) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(ev, cudaSetDevice(ev->device));
+  const int self_col = eval_self_col(self_offset, gallery_row0);
+  const bool sym = eval_sym(q, nq, g, ng, self_col);
+  if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
+  CUDA_TRY(ev, cudaMemsetAsync(d_count, 0, sizeof(int32_t) * nq, st));
+  if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, d_cut, d_count, sym, st)) != NPAIR_OK) return rc;
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
 }
 
 }  // extern "C"

@@ -35,7 +35,10 @@ namespace npair {
 //               (tile list from the host, ~52 % of the tiles); every strictly-upper 128-column block is also written
 //               MIRRORED (second TMA store, with EPI_STORE_S) and contributes COLUMN statistics (warp redux) to the rows it
 //               mirrors into.  S comes out bitwise symmetric, which the backward weight builder relies on.
-enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32 };
+// EPI_COUNT   : retrieval evaluation, not the layer (DESIGN 8).  Per row, the number of valid non-self columns with s >= cut[row]
+//               (a cut of -inf or NaN counts nothing), one atomicAdd per row and tile into count[row]; with EPI_SYM a mirrored block
+//               also counts, for each column gc, its entries against cut[gc].  Used without EPI_STATS and EPI_STORE_S.
+enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64 };
 
 struct GemmParams {
   int M, Nn;           // logical output extent
@@ -69,6 +72,9 @@ struct GemmParams {
   float alpha, beta;   // out = alpha*acc + beta*out
   // ---- EPI_STORE_S without EPI_STATS ----
   int a_row0;          // row of the A operand (and of the rank's S) that output row 0 stands for; a multiple of 128
+  // ---- EPI_COUNT (self_offset as for EPI_STATS) ----
+  const float* cut;    // [M] per-row cut
+  int* count;          // [M] counts, pre-initialised
 };
 
 // BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
@@ -154,6 +160,22 @@ __device__ __forceinline__ float max32(const float (&v)[32]) {
   return fmaxf(fmaxf(fmaxf(m[0], m[1]), fmaxf(m[2], m[3])), fmaxf(fmaxf(m[4], m[5]), fmaxf(m[6], m[7])));
 }
 
+// EPI_COUNT: how many of 32 consecutive similarities reach `cut`.  fast: all 32 are valid; otherwise entry c is valid iff
+// idx0 + c < limit and idx0 + c != self_idx.
+__device__ __forceinline__ int count32(const float (&v)[32], float cut, bool fast, int idx0, int limit, int self_idx) {
+  int n = 0;
+  if (fast) {
+#pragma unroll
+    for (int c = 0; c < 32; ++c) n += (v[c] >= cut) ? 1 : 0;
+  } else {
+#pragma unroll
+    for (int c = 0; c < 32; ++c) n += (idx0 + c < limit && idx0 + c != self_idx && v[c] >= cut) ? 1 : 0;
+  }
+  return n;
+}
+// A row without a best positive has cut -inf and must count nothing: NaN compares false with everything
+__device__ __forceinline__ float count_cut(float c) { return c == -INFINITY ? __int_as_float(0x7fffffff) : c; }
+
 template <int NSPLIT, bool BF16, int EPI, int BK_>
 __global__ void __launch_bounds__(384, 1)
 split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
@@ -161,7 +183,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   using Cfg = GemmCfg<NSPLIT, BK_, EPI>;
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
-  constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS;
+  constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS, COUNT = EPI & EPI_COUNT;
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer in the shared address space (offset arithmetic, no integer round trip): LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -334,6 +356,9 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       int cnt = 0;
       const int self_col = row + p.self_offset;
       const int srow = (wi & 1) * 32 + lane;       // staging row read back by this thread
+      float cut_i = 0.f;
+      int cnt_ge = 0;
+      if (COUNT && row < p.M) cut_i = count_cut(p.cut[row]);
 #pragma unroll
       for (int cp = 0; cp < 4; ++cp) {
         asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");   // the warpgroup's previous reads of the staging tile are done
@@ -357,7 +382,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         // lower-triangle half of a straddling tile: produced by mirroring
         if ((SYM && cb < m_blk) || col0 >= p.Nn) continue;
         float v[32];
-        if (STATS) {
+        if (STATS || COUNT) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
@@ -388,6 +413,8 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             stats32(v, s_lab + ch * 32, lab_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col,
                     minw, maxw, maxb, cnt);
         }
+        if (COUNT && row < p.M)
+          cnt_ge += count32(v, cut_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col);
         if (SYM && cb > m_blk && m_blk * BM + ew * 32 < p.M) {
           // ---- mirrored store: staging row c holds S[col0 + c][rows of this warp]; box lands at (x = row block, y = col0) ----
           if (STORE && lane == 0) ptx::tma_store_wait_read<0>();   // this warp's previous box has been read out of smem
@@ -413,7 +440,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           const float lab_c = s_lab[ch * 32 + lane];
           const float2 rr = s_rng[8 + ew];
           const bool plain = __all_sync(0xffffffffu, gc >= p.Nn || lab_c < rr.x || lab_c > rr.y) && r0 + 32 <= p.M;
-          if (gc < p.Nn) {
+          if (STATS && gc < p.Nn) {
             if (plain) t_maxb = max32(vt);
             else stats32(vt, s_labr + ew * 32, lab_c, r0 + 32 <= p.M, r0, p.M, -1, t_minw, t_maxw, t_maxb, t_cnt);
             if (t_cnt) {
@@ -424,8 +451,14 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             atomicMax(&p.st_maxb[gc], f2ord(t_maxb));
             atomicMax(&p.st_maxall[gc], f2ord(fmaxf(t_maxw, t_maxb)));
           }
+          // mirrored count: the rows of this warp lie in a 128-row block left of column block cb, so none is gc's self pair
+          if (COUNT && gc < p.Nn) {
+            const int t_ge = count32(vt, count_cut(p.cut[gc]), r0 + 32 <= p.M, r0, p.M, -1);
+            if (t_ge) atomicAdd(&p.count[gc], t_ge);
+          }
         }
       }
+      if (COUNT && row < p.M && cnt_ge) atomicAdd(&p.count[row], cnt_ge);
       if (STATS && row < p.M) {
         maxall = fmaxf(maxw, maxb);                       // every valid column is either same- or diff-label
         if (cnt) {

@@ -1759,4 +1759,102 @@ void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, i
   count_launch();
 }
 
+// --------------------------------------------------------------------------------------------
+// retrieval evaluation (DESIGN 8; not part of the reference layer): operand preparation of two matrices and the best-positive cut
+// --------------------------------------------------------------------------------------------
+// max|x| over the queries and the gallery (g == NULL: the gallery is the query set) into *absmax_bits, which is pre-zeroed (the bits
+// of non-negative floats order like the floats; NaN is skipped by fmaxf), and the reset of the per-query statistics.
+__global__ void __launch_bounds__(256) eval_prep_kernel(const float* __restrict__ q, long long nq_el, const float* __restrict__ g, long long ng_el,
+                                                        unsigned int* absmax_bits, EvalRows er, int nq) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (absmax_bits) {
+    float mx = 0.f;
+    for (long long i = t0; i < nq_el; i += stride) mx = fmaxf(mx, fabsf(__ldg(q + i)));
+    if (g) for (long long i = t0; i < ng_el; i += stride) mx = fmaxf(mx, fabsf(__ldg(g + i)));
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(absmax_bits, __float_as_uint(mx));
+  }
+  for (long long i = t0; i < nq; i += stride) {
+    er.st_minw[i] = f2ord(FLT_MAX); er.st_maxw[i] = f2ord(-FLT_MAX);
+    er.st_maxb[i] = f2ord(-FLT_MAX); er.st_maxall[i] = f2ord(-FLT_MAX);
+    er.cnt_same[i] = 0;
+  }
+}
+void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, EvalRows er, int nq,
+                      int sms, cudaStream_t st) {
+  const long long work = absmax_bits ? (nq_el > ng_el ? nq_el : ng_el) / 16 : nq;   // threads: ~16 elements each
+  long long nb = (work + 255) / 256;
+  nb = nb < 1 ? 1 : (nb > 8 * sms ? 8 * sms : nb);
+  eval_prep_kernel<<<static_cast<int>(nb), 256, 0, st>>>(q, nq_el, g, ng_el, absmax_bits, er, nq);
+  count_launch();
+}
+
+// Rows of x to one side of the K-concatenated operands of the similarity GEMM, in split_tile's layout (side_b = 0: the A format of
+// the queries, 1: the B format of the gallery; PREC_BF16 has one segment, the same on both sides).  Thread = 8 features of one row.
+// The pre-scale is the layer's rule applied to max|x| over both sets: `absmax` when the caller gives it (>= 0), else *absmax_bits.
+template <int PREC>
+__global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict__ x, int rows, int D, long long Dp, int side_b, float absmax,
+                                                         const unsigned int* __restrict__ absmax_bits, BlockScalars* bs,
+                                                         uint16_t* __restrict__ out) {
+  constexpr int NS = SPLIT_FORMATS[PREC].pieces;
+  float sc = 1.f, inv = 1.f;
+  if (PREC == PREC_FP16X2) {
+    const float mx = absmax >= 0.f ? absmax : __uint_as_float(*absmax_bits);
+    if (mx > 0.f && isfinite(mx)) { int e; frexpf(mx, &e); sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e); }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0 && !side_b) { bs->x_scale = sc; bs->x_inv_scale = inv; }
+  const long long groups = Dp / 8, i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= rows * groups) return;
+  const long long n = i / groups;
+  const int d = static_cast<int>(i - n * groups) * 8;
+  const float* xr = x + n * D;
+  float v[8];
+  if (d + 7 < D && (D & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const float4 a4 = __ldg(reinterpret_cast<const float4*>(xr + d)), b4 = __ldg(reinterpret_cast<const float4*>(xr + d + 4));
+    v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = d + e < D ? __ldg(xr + d + e) : 0.f;
+  }
+  uint16_t p[8][3];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split3<PREC>(v[e] * sc, p[e][0], p[e][1], p[e][2]);
+  uint4 pk[3];
+#pragma unroll
+  for (int s = 0; s < 3; ++s)
+    pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
+                       p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
+  uint16_t* r = out + n * (mma_passes(NS) * Dp);
+  *reinterpret_cast<uint4*>(r + d) = pk[0];
+  if (PREC == PREC_FP16X2) {            // A = [ hi | hi(8) lo(8) ... ]   B = [ hi | lo(8) hi(8) ... ]
+    *reinterpret_cast<uint4*>(r + Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(r + Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+  } else if (PREC == PREC_BF16X3) {     // A = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]
+    *reinterpret_cast<uint4*>(r + Dp + d) = pk[1];
+    *reinterpret_cast<uint4*>(r + 2 * Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(r + 2 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+    *reinterpret_cast<uint4*>(r + 4 * Dp + 2 * d) = side_b ? pk[2] : pk[0];
+    *reinterpret_cast<uint4*>(r + 4 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[2];
+  }
+}
+void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
+                       BlockScalars* bs, uint16_t* out, cudaStream_t st) {
+  const long long work = static_cast<long long>(rows) * (Dp / 8);
+  with_prec(prec, [&](auto P) {
+    eval_split_kernel<P><<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(x, rows, D, Dp, side_b, absmax, absmax_bits, bs, out);
+  });
+  count_launch();
+}
+
+// Best positive of each query from the statistics sweep: max over same-label non-self gallery rows, -inf when there is none
+__global__ void eval_best_kernel(EvalRows er, int nq, float* __restrict__ best) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nq) best[i] = er.cnt_same[i] > 0 ? ord2f(er.st_maxw[i]) : -INFINITY;
+}
+void launch_eval_best(EvalRows er, int nq, float* best, cudaStream_t st) {
+  eval_best_kernel<<<(nq + 255) / 256, 256, 0, st>>>(er, nq, best);
+  count_launch();
+}
+
 }  // namespace npair

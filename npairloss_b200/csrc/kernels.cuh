@@ -192,4 +192,20 @@ void launch_build_weights(const float* S, long long ldS, int Q, int N, const flo
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);
 
+// Retrieval evaluation (DESIGN 8): the per-query statistics of the similarity GEMM's EPI_STATS epilogue
+struct EvalRows {
+  uint32_t *st_minw, *st_maxw, *st_maxb, *st_maxall;   // ordered-uint encoded
+  int* cnt_same;
+};
+// max|x| over queries and gallery (g == NULL: the query set is the gallery) into the pre-zeroed *absmax_bits (NULL: no reduction),
+// and the reset of the nq queries' statistics
+void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, EvalRows er, int nq,
+                      int sms, cudaStream_t st);
+// rows x D fp32 -> the A (side_b = 0) or B (side_b = 1) format of the K-concatenated operands [rows][mma_passes * Dp], pre-scaled by
+// the power of two of `absmax` (>= 0) or of *absmax_bits; the side-A launch also stores the scale in bs
+void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
+                       BlockScalars* bs, uint16_t* out, cudaStream_t st);
+// best[i] = max same-label non-self similarity of query i, -inf when there is none
+void launch_eval_best(EvalRows er, int nq, float* best, cudaStream_t st);
+
 }  // namespace npair

@@ -85,3 +85,39 @@ class NPairLoss(torch.nn.Module):
         label = label.to(torch.float32).contiguous()          # labels are stored as Dtype in the reference (bottom[1])
         loss, tops = _NPairFunction.apply(feat2, label, self)
         return loss, tops
+
+
+def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), precision=capi.PREC_FP32_FP16X2, self_offset=None):
+    """Recall@K of a whole embedding set (DESIGN 8; not part of the reference layer): query i is a hit at K when its best positive --
+    the most similar gallery row of its label, itself excluded -- is among its K nearest gallery rows, ties counting against it.
+
+    gallery=None: self-retrieval, every query against all the others.  Otherwise query/gallery with disjoint sets, or, with
+    `self_offset` = k, queries that are gallery rows k, k+1, ...  Takes CUDA fp32 embeddings as given (L2-normalise them first for
+    cosine similarity); labels of any numeric dtype.  Returns ({K: recall}, rank) with rank the int32 CUDA tensor of the best
+    positive's rank per query (0: the query has no positive)."""
+    if not query.is_cuda or query.dtype != torch.float32:
+        raise TypeError("recall_at_k takes CUDA float32 embeddings (there is no CPU path)")
+    q = query.reshape(query.shape[0], -1).contiguous()
+    ql = qlabel.to(device=q.device, dtype=torch.float32).contiguous()
+    if gallery is None:
+        if glabel is not None:
+            raise ValueError("glabel without gallery")
+        g, gl, off = q, ql, 0 if self_offset is None else self_offset
+    else:
+        if glabel is None:
+            raise ValueError("gallery without glabel")
+        if not gallery.is_cuda or gallery.dtype != torch.float32:
+            raise TypeError("recall_at_k takes CUDA float32 embeddings (there is no CPU path)")
+        g = gallery.reshape(gallery.shape[0], -1).contiguous()
+        gl = glabel.to(device=q.device, dtype=torch.float32).contiguous()
+        off = -1 if self_offset is None else self_offset
+    if g.shape[1] != q.shape[1]:
+        raise ValueError("query and gallery dimensions differ")
+    ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
+    try:
+        rank = ev.rank(q, ql, g, gl, off)
+        hits = {int(k): ((rank >= 1) & (rank <= int(k))).sum() for k in ks}
+        nq = q.shape[0]
+        return {k: int(v) / nq for k, v in hits.items()}, rank
+    finally:
+        ev.close()
