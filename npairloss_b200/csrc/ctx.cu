@@ -136,6 +136,14 @@ static bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int row
   return true;
 }
 
+// The similarity GEMM's operand maps over K-concatenated rows of kcat elements (split_kernel): `a` over rows_a rows from A (128-row
+// boxes), `b` over rows_b rows from B (256-row boxes), both in 64-element K blocks
+static bool make_tmap_kcat(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, long long kcat,
+                           std::string* err) {
+  return make_tmap_pieces(a, A, static_cast<int>(kcat), rows_a, 1, kcat, rows_a * kcat, 64, 128, err) &&
+         make_tmap_pieces(b, B, static_cast<int>(kcat), rows_b, 1, kcat, rows_b * kcat, 64, 256, err);
+}
+
 // 2-D fp32 map over the similarity matrix [rows x ld], inner extent `cols`, box {32, 32}, 128B swizzle (TMA stores)
 static bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int rows, long long ld_elems, std::string* err, int box_rows = 32) {
   auto fn = tmap_encode_fn();
@@ -404,6 +412,30 @@ static std::vector<int2> sym_tile_list(int Q, int N) {
     for (int nb = mb / 2; nb < tn; ++nb) tl.push_back(make_int2(mb, nb));
   return tl;
 }
+// sym_tile_list(Q, N).size()
+static long long sym_tile_count(int Q, int N) {
+  const int tm = (Q + 127) / 128, tn = (N + 255) / 256;
+  long long n = 0;
+  for (int mb = 0; mb < tm; ++mb) n += mb / 2 < tn ? tn - mb / 2 : 0;
+  return n;
+}
+
+// A sweep of the similarity GEMM over rows x cols of the K-concatenated operands of K extent kcat (make_tmap_kcat): 128 x 256 tiles
+// of 64-element K blocks, no split-K, the accumulators scaled by the square of *inv_scale; under EPI_SYM only the tiles of
+// `sym_tiles`, and under EPI_STATS the per-row statistics of `ra`
+static GemmParams sim_sweep(int epi, int rows, int cols, long long kcat, const float* inv_scale, const int2* sym_tiles, int n_sym_tiles,
+                            const RowArrays& ra) {
+  GemmParams gp; memset(&gp, 0, sizeof(gp));
+  gp.M = rows; gp.Nn = cols;
+  gp.num_kblocks = static_cast<int>(kcat / 64);
+  gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (cols + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+  gp.dev_scale = inv_scale;
+  if (epi & EPI_SYM) { gp.tile_list = sym_tiles; gp.num_tiles_list = n_sym_tiles; }
+  if (epi & EPI_STATS) {
+    gp.st_minw = ra.st_minw; gp.st_maxw = ra.st_maxw; gp.st_maxb = ra.st_maxb; gp.st_maxall = ra.st_maxall; gp.cnt_same = ra.cnt_same;
+  }
+  return gp;
+}
 
 // Row-block similarity mode (NPAIR_SIM_BLOCK_ROWS): the block height in rows, a multiple of 128; 0 when the mode is off or the
 // height reaches Q (the materialised path)
@@ -427,8 +459,9 @@ enum { B_XTOT, B_LABTOT, B_YNORM, B_DY, B_INV_NORM, B_S, B_XS, B_XST, B_XCAT_A, 
 // What a context decides from its configuration and two device facts, and the byte size of every device buffer it allocates
 // (0: not allocated).  The peer-memory exchange buffers are sized as if the context had a communicator and peer access.
 struct Plan {
-  int N, nsplit, bk_sim, bk_grad;
+  int N, nsplit, bk_grad;
   long long Dp, Np, Qp, ldS;     // padded feature / all-rows / local-rows extents of the operand pieces, row stride of S
+  long long kcat;                // K extent of the similarity GEMM's operands: mma_passes(nsplit) * Dp (PREC_BF16: Xs, one piece)
   int bwd_mode;                  // NPAIR_BWDMODE_*
   bool fused_grad;               // the gradient weights are produced inside the gradient GEMM: no H in HBM
   bool cat;                      // the similarity GEMM reads the K-concatenated operands XcatA / XcatB, not Xs
@@ -454,8 +487,9 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   const long long Q = cfg.Q, D = cfg.D, N = Q * W;
   const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
   p.N = static_cast<int>(N);
-  p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_sim = bk_of(prec, EPI_STORE_S); p.bk_grad = bk_of(prec, EPI_OUT);
+  p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
+  p.kcat = mma_passes(p.nsplit) * p.Dp;
   const int blk_rows = sim_block_rows(cfg);
   p.s_rows = blk_rows ? blk_rows : cfg.Q;
   p.n_blocks = (cfg.Q + p.s_rows - 1) / p.s_rows;
@@ -482,7 +516,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
   const int tiles = static_cast<int>(((Q + 127) / 128) * ((D + 255) / 256));
   p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
-  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_list(cfg.Q, p.N).size());
+  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, p.N));
   p.sweep_epi = EPI_STATS | (p.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
   p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
   p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
@@ -495,7 +529,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   b[B_S] = f * p.s_rows * p.ldS;
   if (!p.cat) b[B_XS] = 2 * ns * N * p.Dp;                                      // operand pieces [ns][N][Dp]
   b[B_XST] = 2 * ns * D * p.Np;                                                 // transposed pieces [ns][D][Np]
-  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * mma_passes(ns) * p.Dp;        // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * p.kcat;                         // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
   if (!p.fused_grad) b[B_H] = 2 * ns * Q * p.Np;                                // materialised gradient weights
   if (rs) { b[B_XLT] = 2 * ns * D * p.Qp; b[B_HT] = 2 * ns * N * p.Qp; b[B_OUT2] = f * N * D; }
   if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = sizeof(RowRecord) * N;   // gathered row records
@@ -535,7 +569,6 @@ struct npair_ctx : Plan {
   float* OUT2 = nullptr;         // world > 1: N x D transposed-term product before the reduce-scatter
   uint16_t *XcatA = nullptr, *XcatB = nullptr;   // K-concatenated operands [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
   RowRecord* rs_total = nullptr;   // row-scalar mode: the world's N row records, all-gathered
-  CUtensorMap tm_catA, tm_catB;
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
   bool rs_gathered = false;
@@ -563,7 +596,7 @@ struct npair_ctx : Plan {
   float* tops_pinned = nullptr;  // host-mapped: 5 tops + err(int) + sequence number of the forward that wrote them
   unsigned int tops_seq = 0;
   float* tops_dev = nullptr;
-  CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;
+  CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_kcat)
   // nccl
   void* comm = nullptr; bool own_comm = false;
   // per-step state
@@ -598,6 +631,35 @@ struct PhaseTimer {
       return NPAIR_E_CUDA;                                                                               \
     }                                                                                                    \
   } while (0)
+// The same while a context or an evaluator is created, before it exists for npair_last_error: the message goes to g_create_err.  The
+// object under construction is held by a unique_ptr, which releases it on the early return.
+#define CREATE_TRY(call)                                                                                 \
+  do {                                                                                                   \
+    cudaError_t e__ = (call);                                                                            \
+    if (e__ != cudaSuccess) {                                                                            \
+      g_create_err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);    \
+      return NPAIR_E_CUDA;                                                                               \
+    }                                                                                                    \
+  } while (0)
+
+// Makes `device` (< 0: the current one) current for a new context or evaluator, which needs an sm_90 device; its id and SM count
+static int open_device(int device, int* dev, int* sms) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) {
+    g_create_err = "no CUDA device: libnpair_b200 has no CPU fallback (the oracle under oracle/ is test-only)";
+    return NPAIR_E_CUDA;
+  }
+  if (device >= 0) CREATE_TRY(cudaSetDevice(device));
+  CREATE_TRY(cudaGetDevice(dev));
+  cudaDeviceProp prop;
+  CREATE_TRY(cudaGetDeviceProperties(&prop, *dev));
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_err = fmt("device %d is sm_%d%d; this library contains sm_90a code only", *dev, prop.major, prop.minor);
+    return NPAIR_E_CUDA;
+  }
+  *sms = prop.multiProcessorCount;
+  return NPAIR_OK;
+}
 
 static int validate(const npair_config* c, std::string* err) {
   if (!c) { *err = "null config"; return NPAIR_E_ARG; }
@@ -729,30 +791,11 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   std::string e;
   int rc = validate(cfg, &e);
   if (rc != NPAIR_OK) { g_create_err = e; return rc; }
-  npair_ctx* c = new npair_ctx();
-  c->cfg = *cfg;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) {
-    g_create_err = "no CUDA device: libnpair_b200 has no CPU fallback (the oracle under oracle/ is test-only)";
-    delete c; return NPAIR_E_CUDA;
-  }
-#define CREATE_TRY(call)                                                                                  \
-  do {                                                                                                    \
-    cudaError_t e__ = (call);                                                                             \
-    if (e__ != cudaSuccess) {                                                                             \
-      g_create_err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);     \
-      npair_destroy(c); return NPAIR_E_CUDA;                                                              \
-    }                                                                                                     \
-  } while (0)
-  if (cfg->device >= 0) CREATE_TRY(cudaSetDevice(cfg->device));
-  CREATE_TRY(cudaGetDevice(&c->device));
-  cudaDeviceProp prop;
-  CREATE_TRY(cudaGetDeviceProperties(&prop, c->device));
-  if (prop.major != 9 || prop.minor != 0) {
-    g_create_err = fmt("device %d is sm_%d%d; this library contains sm_90a code only", c->device, prop.major, prop.minor);
-    npair_destroy(c); return NPAIR_E_CUDA;
-  }
-  c->sms = prop.multiProcessorCount;
+  int device = -1, sms = 0;
+  if ((rc = open_device(cfg->device, &device, &sms)) != NPAIR_OK) return rc;
+  std::unique_ptr<npair_ctx, void (*)(npair_ctx*)> made(new npair_ctx(), npair_destroy);   // until it is handed out
+  npair_ctx* c = made.get();
+  c->cfg = *cfg; c->device = device; c->sms = sms;
   // only the multi-rank row-record backward on the tensor cores and the row-block similarity mode depend on the check, which itself
   // creates a single-rank context
   const bool blocks = sim_block_rows(*cfg) > 0;
@@ -761,7 +804,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   if (blocks && !sym) {
     g_create_err = "row-block similarity mode: the similarity GEMM is not bitwise symmetric on this device, so a recomputed block of S "
                    "would not match the rows the statistics were taken from";
-    npair_destroy(c); return NPAIR_E_ARG;
+    return NPAIR_E_ARG;
   }
   static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym);
   c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
@@ -817,12 +860,11 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     CREATE_TRY(c->fused_grad ? allow_smem(fused_kernel(c->prec)) : allow_smem(gemm_kernel(c->prec, EPI_OUT)));
     // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
     std::string te;
-    const int bks = c->bk_sim, bkg = c->bk_grad;
-    bool ok = true;
-    if (c->Xs) {          // similarity: A = local rows of Xs, B = all rows of Xs; K = D
-      ok = ok && make_tmap_pieces(&c->tm_simA, c->Xs + static_cast<long long>(c->rank) * Q * c->Dp, D, Q, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 128, &te);
-      ok = ok && make_tmap_pieces(&c->tm_simB, c->Xs, D, N, ns, c->Dp, static_cast<long long>(N) * c->Dp, bks, 256, &te);
-    }
+    const int bkg = c->bk_grad;
+    // similarity: A = the rank's rows, B = all rows of the K-concatenated operands (PREC_BF16: Xs, whose one piece is that format)
+    const uint16_t* catA = c->cat ? c->XcatA : c->Xs;
+    const uint16_t* catB = c->cat ? c->XcatB : c->Xs;
+    bool ok = make_tmap_kcat(&c->tm_simA, &c->tm_simB, catA +static_cast<long long>(c->rank) * Q * c->kcat, Q, catB, N, c->kcat, &te);
     ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, c->s_rows, c->ldS, &te);
     // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
     if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, &te);
@@ -831,25 +873,20 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       ok = ok && make_tmap_pieces(&c->tm_fB, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, &te);
       ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, &te, 128);
     }
-    if (c->XcatA) {       // bitwise-symmetric similarity: one pass over K_cat = 3*Dp (fp16x2) / 6*Dp (bf16x3)
-      const long long kc = mma_passes(ns) * c->Dp;
-      ok = ok && make_tmap_pieces(&c->tm_catA, c->XcatA + static_cast<long long>(c->rank) * Q * kc, static_cast<int>(kc), Q, 1, kc, static_cast<long long>(N) * kc, 64, 128, &te);
-      ok = ok && make_tmap_pieces(&c->tm_catB, c->XcatB, static_cast<int>(kc), N, 1, kc, static_cast<long long>(N) * kc, 64, 256, &te);
-    }
     if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) {   // gradient 2: A = HT [N x Q], B = XlT [D x Q]; K = Q
       ok = ok && make_tmap_pieces(&c->tm_b2A, c->HT, Q, N, ns, c->Qp, static_cast<long long>(N) * c->Qp, bkg, 128, &te);
       ok = ok && make_tmap_pieces(&c->tm_b2B, c->XlT, Q, D, ns, c->Qp, static_cast<long long>(D) * c->Qp, bkg, 256, &te);
     }
-    if (!ok) { g_create_err = te; npair_destroy(c); return NPAIR_E_CUDA; }
+    if (!ok) { g_create_err = te; return NPAIR_E_CUDA; }
   }
   // ---- NCCL ----
   if (c->world > 1 && (id128 || ext_comm)) {
     NcclApi* api = nccl_api();
-    if (!api->h || !api->err.empty()) { g_create_err = api->err; npair_destroy(c); return NPAIR_E_NCCL; }
+    if (!api->h || !api->err.empty()) { g_create_err = api->err; return NPAIR_E_NCCL; }
     if (ext_comm) { c->comm = ext_comm; c->own_comm = false; }
     else {
       std::string ce;
-      if (acquire_comm(id128, c->world, c->rank, &c->comm, &ce) != 0) { g_create_err = ce; c->comm = nullptr; npair_destroy(c); return NPAIR_E_NCCL; }
+      if (acquire_comm(id128, c->world, c->rank, &c->comm, &ce) != 0) { g_create_err = ce; c->comm = nullptr; return NPAIR_E_NCCL; }
       c->own_comm = true;
     }
   }
@@ -869,7 +906,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     CREATE_TRY(cudaMemcpy(d_mine, &mine, 64, cudaMemcpyHostToDevice));
     CREATE_TRY(cudaDeviceSynchronize());                       // the memset above has landed before any peer can write into the region
     int r = api->AllGather(d_mine, d_all, 16, NCCL_FLOAT32, c->comm, nullptr);
-    if (r != 0) { g_create_err = fmt("ncclAllGather(ipc handles): %s", api->GetErrorString(r)); npair_destroy(c); return NPAIR_E_NCCL; }
+    if (r != 0) { g_create_err = fmt("ncclAllGather(ipc handles): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
     CREATE_TRY(cudaStreamSynchronize(nullptr));
     std::vector<cudaIpcMemHandle_t> all(W);
     CREATE_TRY(cudaMemcpy(all.data(), d_all, 64ull * W, cudaMemcpyDeviceToHost));
@@ -891,10 +928,9 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     // topology is symmetric, which holds on an NVSwitch box -- a mixed outcome is reported by the first exchange's timeout)
   }
   if (c->wscope && !c->comm) {
-    g_create_err = "global_scope with world > 1 needs a communicator (the world-scope reductions are internal)"; npair_destroy(c); return NPAIR_E_ARG;
+    g_create_err = "global_scope with world > 1 needs a communicator (the world-scope reductions are internal)"; return NPAIR_E_ARG;
   }
-#undef CREATE_TRY
-  *out = c;
+  *out = made.release();
   return NPAIR_OK;
 }
 
@@ -1036,19 +1072,13 @@ static RowArrays rows_from(const RowArrays& ra, int r0) {
 
 // The similarity GEMM over rows [r0, r0 + rows) of the rank's S through the epilogue `epi` (gemm_wgmma.cuh)
 static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_t st) {
-  GemmParams gp; memset(&gp, 0, sizeof(gp));
-  gp.M = rows; gp.Nn = c->N; gp.a_row0 = r0;
-  gp.num_kblocks = static_cast<int>(c->cat ? mma_passes(c->nsplit) * c->Dp / 64 : (c->D + c->bk_sim - 1) / c->bk_sim);
-  gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (c->N + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
-  gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
-  if (epi & EPI_SYM) { gp.tile_list = c->sym_tiles; gp.num_tiles_list = c->n_sym_tiles; }
+  GemmParams gp = sim_sweep(epi, rows, c->N, c->kcat, &c->bs->x_inv_scale, c->sym_tiles, c->n_sym_tiles, c->ra);
+  gp.a_row0 = r0; gp.S = c->S; gp.ldS = c->ldS;
   if (epi & EPI_STATS) {
     gp.lab_rows = c->cur_label; gp.lab_cols = c->lab_total; gp.self_offset = c->rank * c->Q;
-    gp.st_minw = c->ra.st_minw; gp.st_maxw = c->ra.st_maxw; gp.st_maxb = c->ra.st_maxb; gp.st_maxall = c->ra.st_maxall; gp.cnt_same = c->ra.cnt_same;
     gp.fuse_thr = c->fuse_thr ? 1 : 0; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
   }
-  return c->cat ? launch_gemm(c->prec, epi, c->tm_catA, c->tm_catB, c->tm_S, gp, c->sms, st)
-                : launch_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
+  return launch_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
 }
 
 // Rows [r0, r0 + s_rows) of the rank's S into the S buffer, unless it holds them already (a materialised S always does): full tiles,
@@ -1491,9 +1521,8 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
         DG_TRY(cudaMemcpyAsync(&mx[i], &bs->x_absmax, 4, cudaMemcpyDeviceToHost, st));
       }
       DG_TRY(cudaStreamSynchronize(st));
-      const float m = mx[0] > mx[1] ? mx[0] : mx[1];
-      int e = 0; if (m > 0.f) frexpf(m, &e);
-      sc[0] = ldexpf(1.f, -e); sc[1] = ldexpf(1.f, e);
+      const PreScale ps = pre_scale(mx[0] > mx[1] ? mx[0] : mx[1]);
+      sc[0] = ps.scale; sc[1] = ps.inv;
     }
     DG_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
     launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
@@ -1526,7 +1555,7 @@ done:
 // Not part of the reference layer.  Queries go to the A format and gallery rows to the B format of the K-concatenated operands, so the
 // similarity GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
 enum { E_CAT_A, E_CAT_B, E_ROWS, E_BS, E_SYM_TILES, E_COUNT_BUFS };
-static constexpr int EVAL_ROW_WORDS = 5;        // EvalRows: four ordered-uint statistics and the same-label count per query
+static constexpr int EVAL_ROW_WORDS = 5;        // the statistics of RowArrays: four ordered-uint statistics and the same-label count per query
 static constexpr int EVAL_NO_SELF = -(1 << 30); // a self offset that matches no column (rows and columns stay below 2^30)
 
 struct EvalPlan {
@@ -1549,8 +1578,7 @@ static EvalPlan eval_plan_of(int max_q, int max_g, int D, int prec) {
   p.Dp = round_up(D, 64);
   p.kcat = mma_passes(SPLIT_FORMATS[prec].pieces) * p.Dp;
   const int n = max_q < max_g ? max_q : max_g;
-  const long long tm = (n + 127) / 128, tn = (n + 255) / 256;
-  for (long long mb = 0; mb < tm; ++mb) p.n_sym_tiles += static_cast<int>(tn - mb / 2);   // sym_tile_list(n, n).size()
+  p.n_sym_tiles = static_cast<int>(sym_tile_count(n, n));
   size_t* b = p.bytes;
   b[E_CAT_A] = 2ull * max_q * p.kcat;
   b[E_CAT_B] = 2ull * max_g * p.kcat;
@@ -1564,7 +1592,7 @@ struct npair_eval : EvalPlan {
   int device = -1, sms = 0;
   uint16_t *catA = nullptr, *catB = nullptr;
   void* rows = nullptr;
-  EvalRows er{};
+  RowArrays ra{};                 // only the statistics (EVAL_ROW_WORDS)
   unsigned int* absmax_bits = nullptr;
   BlockScalars* bs = nullptr;
   int2* sym_tiles = nullptr;
@@ -1596,46 +1624,27 @@ void npair_eval_destroy(npair_eval* ev) {
 int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int32_t device, npair_eval** out) {
   if (!out) { g_create_err = "null out"; return NPAIR_E_ARG; }
   *out = nullptr;
-  const int rc = eval_validate(max_q, max_g, D, prec, &g_create_err);
+  int rc = eval_validate(max_q, max_g, D, prec, &g_create_err);
   if (rc != NPAIR_OK) return rc;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) {
-    g_create_err = "no CUDA device: libnpair_b200 has no CPU fallback (the oracle under oracle/ is test-only)";
-    return NPAIR_E_CUDA;
-  }
-  npair_eval* ev = new npair_eval();
+  int dev = -1, sms = 0;
+  if ((rc = open_device(device, &dev, &sms)) != NPAIR_OK) return rc;
+  std::unique_ptr<npair_eval, void (*)(npair_eval*)> made(new npair_eval(), npair_eval_destroy);   // until it is handed out
+  npair_eval* ev = made.get();
   static_cast<EvalPlan&>(*ev) = eval_plan_of(max_q, max_g, D, prec);
-#define EVAL_CREATE_TRY(call)                                                                             \
-  do {                                                                                                    \
-    cudaError_t e__ = (call);                                                                             \
-    if (e__ != cudaSuccess) {                                                                             \
-      g_create_err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);     \
-      npair_eval_destroy(ev); return NPAIR_E_CUDA;                                                        \
-    }                                                                                                     \
-  } while (0)
-  if (device >= 0) EVAL_CREATE_TRY(cudaSetDevice(device));
-  EVAL_CREATE_TRY(cudaGetDevice(&ev->device));
-  cudaDeviceProp prop;
-  EVAL_CREATE_TRY(cudaGetDeviceProperties(&prop, ev->device));
-  if (prop.major != 9 || prop.minor != 0) {
-    g_create_err = fmt("device %d is sm_%d%d; this library contains sm_90a code only", ev->device, prop.major, prop.minor);
-    npair_eval_destroy(ev); return NPAIR_E_CUDA;
-  }
-  ev->sms = prop.multiProcessorCount;
+  ev->device = dev; ev->sms = sms;
   const size_t* b = ev->bytes;
-  EVAL_CREATE_TRY(dev_alloc(&ev->catA, b[E_CAT_A], false));
-  EVAL_CREATE_TRY(dev_alloc(&ev->catB, b[E_CAT_B], false));
-  EVAL_CREATE_TRY(dev_alloc(&ev->rows, b[E_ROWS], true));
-  EVAL_CREATE_TRY(dev_alloc(&ev->bs, b[E_BS], true));
-  EVAL_CREATE_TRY(dev_alloc(&ev->sym_tiles, b[E_SYM_TILES], false));
+  CREATE_TRY(dev_alloc(&ev->catA, b[E_CAT_A], false));
+  CREATE_TRY(dev_alloc(&ev->catB, b[E_CAT_B], false));
+  CREATE_TRY(dev_alloc(&ev->rows, b[E_ROWS], true));
+  CREATE_TRY(dev_alloc(&ev->bs, b[E_BS], true));
+  CREATE_TRY(dev_alloc(&ev->sym_tiles, b[E_SYM_TILES], false));
   uint32_t* w = static_cast<uint32_t*>(ev->rows);
-  ev->er.st_minw = w; w += max_q; ev->er.st_maxw = w; w += max_q; ev->er.st_maxb = w; w += max_q; ev->er.st_maxall = w; w += max_q;
-  ev->er.cnt_same = reinterpret_cast<int*>(w); w += max_q;
+  ev->ra.st_minw = w; w += max_q; ev->ra.st_maxw = w; w += max_q; ev->ra.st_maxb = w; w += max_q; ev->ra.st_maxall = w; w += max_q;
+  ev->ra.cnt_same = reinterpret_cast<int*>(w); w += max_q;
   ev->absmax_bits = w;
   const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM};
-  for (int epi : epis) EVAL_CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
-#undef EVAL_CREATE_TRY
-  *out = ev;
+  for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
+  *out = made.release();
   return NPAIR_OK;
 }
 
@@ -1668,7 +1677,7 @@ static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, 
     amx = ev->absmax_bits;
     CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
   }
-  launch_eval_prep(q, nq * D, sym ? nullptr : g, ng * D, amx, ev->er, nq, ev->sms, st);
+  launch_eval_prep(q, nq * D, sym ? nullptr : g, ng * D, amx, ev->ra, nq, ev->sms, st);
   launch_eval_split(q, nq, ev->D, ev->Dp, ev->prec, 0, absmax, amx, ev->bs, ev->catA, st);
   launch_eval_split(g, ng, ev->D, ev->Dp, ev->prec, 1, absmax, amx, ev->bs, ev->catB, st);
   CUDA_TRY(ev, cudaGetLastError());
@@ -1678,12 +1687,6 @@ static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, 
 // One sweep of the similarity GEMM over the prepared operands: EPI_STATS (labels) or EPI_COUNT (cut, count), + EPI_SYM when `sym`
 static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, const float* ql, const float* gl, const float* cut, int32_t* count,
                       bool sym, cudaStream_t st) {
-  GemmParams gp; memset(&gp, 0, sizeof(gp));
-  gp.M = nq; gp.Nn = ng;
-  gp.num_kblocks = static_cast<int>(ev->kcat / 64);
-  gp.tiles_m = (nq + 127) / 128; gp.tiles_n = (ng + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
-  gp.dev_scale = &ev->bs->x_inv_scale;
-  gp.self_offset = self_col;
   if (sym) {
     if (ev->sym_n != nq) {
       ev->sym_host = sym_tile_list(nq, nq);
@@ -1691,21 +1694,14 @@ static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, con
       ev->sym_n = nq;
     }
     epi |= EPI_SYM;
-    gp.tile_list = ev->sym_tiles; gp.num_tiles_list = static_cast<int>(ev->sym_host.size());
   }
-  if (epi & EPI_STATS) {
-    gp.lab_rows = ql; gp.lab_cols = gl;
-    gp.st_minw = ev->er.st_minw; gp.st_maxw = ev->er.st_maxw; gp.st_maxb = ev->er.st_maxb; gp.st_maxall = ev->er.st_maxall;
-    gp.cnt_same = ev->er.cnt_same;
-  } else {
-    gp.cut = cut; gp.count = count;
-  }
+  GemmParams gp = sim_sweep(epi, nq, ng, ev->kcat, &ev->bs->x_inv_scale, ev->sym_tiles, static_cast<int>(ev->sym_host.size()), ev->ra);
+  gp.self_offset = self_col;
+  if (epi & EPI_STATS) { gp.lab_rows = ql; gp.lab_cols = gl; }
+  else { gp.cut = cut; gp.count = count; }
   CUtensorMap ta, tb;
   std::string te;
-  if (!make_tmap_pieces(&ta, ev->catA, static_cast<int>(ev->kcat), nq, 1, ev->kcat, static_cast<long long>(nq) * ev->kcat, 64, 128, &te) ||
-      !make_tmap_pieces(&tb, ev->catB, static_cast<int>(ev->kcat), ng, 1, ev->kcat, static_cast<long long>(ng) * ev->kcat, 64, 256, &te)) {
-    ev->err = te; return NPAIR_E_CUDA;
-  }
+  if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
   CUDA_TRY(ev, launch_gemm(ev->prec, epi, ta, tb, ta, gp, ev->sms, st));
   return NPAIR_OK;
 }
@@ -1722,10 +1718,10 @@ int npair_eval_rank(npair_eval* ev, const float* q, const float* ql, int32_t nq,
   CUDA_TRY(ev, cudaSetDevice(ev->device));
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
-  float* cut = reinterpret_cast<float*>(ev->er.st_minw);   // p* overwrites a statistic sweep 2 does not read
+  float* cut = reinterpret_cast<float*>(ev->ra.st_minw);   // p* overwrites a statistic sweep 2 does not read
   if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
   if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_best(ev->er, nq, cut, st);
+  launch_eval_best(ev->ra, nq, cut, st);
   CUDA_TRY(ev, cudaMemsetAsync(d_rank, 0, sizeof(int32_t) * nq, st));
   if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, cut, d_rank, sym, st)) != NPAIR_OK) return rc;
   CUDA_TRY(ev, cudaGetLastError());
@@ -1744,7 +1740,7 @@ int npair_eval_best_positive(npair_eval* ev, const float* q, const float* ql, in
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
   if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_best(ev->er, nq, d_best, st);
+  launch_eval_best(ev->ra, nq, d_best, st);
   CUDA_TRY(ev, cudaGetLastError());
   return NPAIR_OK;
 }

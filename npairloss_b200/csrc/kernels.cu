@@ -55,6 +55,46 @@ __device__ __forceinline__ void split3(float v, uint16_t& p0, uint16_t& p1, uint
     p0 = __bfloat16_as_ushort(h); p1 = __bfloat16_as_ushort(m); p2 = __bfloat16_as_ushort(__float2bfloat16_rn(r2));
   }
 }
+// Eight consecutive features v, times the pre-scale sc, as pieces: p[e][s] is piece s of feature e, pk[s] the eight pieces s packed into
+// one 16-byte group (only the format's pieces are packed)
+template <int PREC>
+__device__ __forceinline__ void split8(const float (&v)[8], float sc, uint16_t (&p)[8][3], uint4 (&pk)[3]) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split3<PREC>(v[e] * sc, p[e][0], p[e][1], p[e][2]);
+#pragma unroll
+  for (int s = 0; s < SPLIT_FORMATS[PREC].pieces; ++s)
+    pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
+                       p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
+}
+// The packed pieces pk of features [d, d + 8) into one row of the K-concatenated operands of the bitwise-symmetric similarity GEMM,
+// in the A (side_b = false) or B format; one Dp-long segment per MMA pass:
+//   bf16   : A row = B row = [ hi ]                                                                                       K_cat = Dp
+//   fp16x2 : A row = [ hi | hi(8) lo(8) ... ]                         B row = [ hi | lo(8) hi(8) ... ]                  K_cat = 3*Dp
+//   bf16x3 : A row = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B row = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]   K_cat = 6*Dp
+// ONE K=16 MMA then sums 8 products p_j*q_m and the 8 mirrored products q_j*p_m: swapping the operand roles only
+// permutes the products inside an instruction, whose sum is order-invariant (measured: tests/diag_mma_symmetry.py),
+// so S[j][m] == S[m][j] bit for bit, on one rank and across ranks.
+template <int PREC>
+__device__ __forceinline__ void store_kcat_row(uint16_t* row, long long Dp, int d, const uint4 (&pk)[3], bool side_b) {
+  *reinterpret_cast<uint4*>(row + d) = pk[0];
+  if (PREC == PREC_FP16X2) {
+    *reinterpret_cast<uint4*>(row + Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(row + Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+  } else if (PREC == PREC_BF16X3) {
+    *reinterpret_cast<uint4*>(row + Dp + d) = pk[1];
+    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d) = side_b ? pk[2] : pk[0];
+    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[2];
+  }
+}
+
+// Row i's statistics before a similarity sweep accumulates into them (caffe_set of the stat blobs, .cu:230-236)
+__device__ __forceinline__ void reset_row_stats(const RowArrays& ra, long long i) {
+  ra.st_minw[i] = f2ord(FLT_MAX); ra.st_maxw[i] = f2ord(-FLT_MAX);
+  ra.st_maxb[i] = f2ord(-FLT_MAX); ra.st_maxall[i] = f2ord(-FLT_MAX);
+  ra.cnt_same[i] = 0;
+}
 
 // exp(s - max) with the row constant pre-multiplied, m2 = max * log2(e): one FFMA + one MUFU.EX2 (relative error ~ (2 + 1.44|x|)
 // ulp: 3e-7 for the |x| <= 2 of unit-norm embeddings).  Cheap enough to evaluate for EVERY pair, which keeps the row pass and the
@@ -120,11 +160,7 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
       for (long long i = t0; i < ntot; i += stride) mx = fmaxf(mx, fabsf(xt[i]));
     }
   }
-  for (long long i = t0; i < Q; i += stride) {                  // caffe_set of the stat blobs, .cu:230-236
-    ra.st_minw[i] = f2ord(FLT_MAX); ra.st_maxw[i] = f2ord(-FLT_MAX);
-    ra.st_maxb[i] = f2ord(-FLT_MAX); ra.st_maxall[i] = f2ord(-FLT_MAX);
-    ra.cnt_same[i] = 0;
-  }
+  for (long long i = t0; i < Q; i += stride) reset_row_stats(ra, i);
   sum = warp_sum(sum); mx = warp_max(mx);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   if (l == 0) { s_sum[w] = sum; s_max[w] = mx; }
@@ -152,10 +188,7 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
     bs->asum = static_cast<float>(dsum);
     bs->x_absmax = mx;
     float sc = 1.f, inv = 1.f;
-    if (want_scale && mx > 0.f && isfinite(mx)) {
-      int e; frexpf(mx, &e);                 // mx = m * 2^e, m in [0.5,1)
-      sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e);
-    }
+    if (want_scale) { const PreScale ps = pre_scale(mx); sc = ps.scale; inv = ps.inv; }
     bs->x_scale = sc; bs->x_inv_scale = inv;
     bs->err = 0; bs->ticket = 0; bs->ticket2 = 0; bs->ticket0 = 0; bs->ticket3 = 0; bs->sel_active[0] = 0; bs->sel_active[1] = 0;
     bs->cand_n[0] = 0; bs->cand_n[1] = 0;
@@ -218,50 +251,27 @@ __device__ __forceinline__ void split_tile(const SplitArgs& a, float sc, int til
   const int t = threadIdx.x, nl = t >> 3, dg = t & 7;
   const int n = n0 + nl, d = d0 + 8 * dg;
   uint16_t p[8][3];
-  const bool rowok = n < N;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) split3<PREC>(v[e] * sc, p[e][0], p[e][1], p[e][2]);
   uint4 pk[3];
+  const bool rowok = n < N;
+  split8<PREC>(v, sc, p, pk);
 #pragma unroll
-  for (int s = 0; s < NS; ++s) {
-    pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
-                       p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
+  for (int s = 0; s < NS; ++s)
 #pragma unroll
     for (int e = 0; e < 8; ++e) tile[s][8 * dg + e][nl] = p[e][s];
-  }
   // every destination row is padded to a multiple of 64 elements (Dp), so whole 16-byte groups can be stored even when
-  // D is ragged: the excess elements are zeros (v = 0 above) and lie beyond the TMA extent anyway
+  // D is ragged: the excess elements are zeros (v = 0 above), which is what the similarity GEMM reads past D (its K extent is Dp
+  // per segment) and which lies beyond the TMA extent of every other map
   if (rowok && d < Dp) {
     const long long ps = static_cast<long long>(N) * ldXs;
     if (Xs)      // NULL when the similarity GEMM reads the K-concatenated operands below
 #pragma unroll
       for (int s = 0; s < NS; ++s) *reinterpret_cast<uint4*>(Xs + s * ps + static_cast<long long>(n) * ldXs + d) = pk[s];
-    // K-concatenated operands of the bitwise-symmetric similarity GEMM (one MMA pass over K_cat):
-    //   fp16x2 : A row = [ hi | hi(8) lo(8) ... ]                         B row = [ hi | lo(8) hi(8) ... ]                  K_cat = 3*Dp
-    //   bf16x3 : A row = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B row = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]   K_cat = 6*Dp
-    // ONE K=16 MMA then sums 8 products p_j*q_m and the 8 mirrored products q_j*p_m: swapping the operand roles only
-    // permutes the products inside an instruction, whose sum is order-invariant (measured: tests/diag_mma_symmetry.py),
-    // so S[j][m] == S[m][j] bit for bit, on one rank and across ranks.
+    // K-concatenated operands of the bitwise-symmetric similarity GEMM: every row in the B format, and the rank's own rows, the only
+    // ones that are ever an A operand, also in the A format
     if (PREC != PREC_BF16 && XcatA) {
       const long long kcat = mma_passes(NS) * Dp;
-      uint16_t* ra = XcatA + static_cast<long long>(n) * kcat;
-      uint16_t* rb = XcatB + static_cast<long long>(n) * kcat;
-      const bool local = (n >= row0 && n < row0 + Q);        // only the rank's own rows are ever an A operand
-      *reinterpret_cast<uint4*>(rb + d) = pk[0];
-      if (local) *reinterpret_cast<uint4*>(ra + d) = pk[0];
-      if (PREC == PREC_FP16X2) {
-        *reinterpret_cast<uint4*>(rb + Dp + 2 * d) = pk[1]; *reinterpret_cast<uint4*>(rb + Dp + 2 * d + 8) = pk[0];
-        if (local) { *reinterpret_cast<uint4*>(ra + Dp + 2 * d) = pk[0]; *reinterpret_cast<uint4*>(ra + Dp + 2 * d + 8) = pk[1]; }
-      } else {
-        *reinterpret_cast<uint4*>(rb + Dp + d) = pk[1];
-        *reinterpret_cast<uint4*>(rb + 2 * Dp + 2 * d) = pk[1]; *reinterpret_cast<uint4*>(rb + 2 * Dp + 2 * d + 8) = pk[0];
-        *reinterpret_cast<uint4*>(rb + 4 * Dp + 2 * d) = pk[2]; *reinterpret_cast<uint4*>(rb + 4 * Dp + 2 * d + 8) = pk[0];
-        if (local) {
-          *reinterpret_cast<uint4*>(ra + Dp + d) = pk[1];
-          *reinterpret_cast<uint4*>(ra + 2 * Dp + 2 * d) = pk[0]; *reinterpret_cast<uint4*>(ra + 2 * Dp + 2 * d + 8) = pk[1];
-          *reinterpret_cast<uint4*>(ra + 4 * Dp + 2 * d) = pk[0]; *reinterpret_cast<uint4*>(ra + 4 * Dp + 2 * d + 8) = pk[2];
-        }
-      }
+      store_kcat_row<PREC>(XcatB + static_cast<long long>(n) * kcat, Dp, d, pk, true);
+      if (n >= row0 && n < row0 + Q) store_kcat_row<PREC>(XcatA + static_cast<long long>(n) * kcat, Dp, d, pk, false);
     }
   }
   __syncthreads();
@@ -1765,7 +1775,7 @@ void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, i
 // max|x| over the queries and the gallery (g == NULL: the gallery is the query set) into *absmax_bits, which is pre-zeroed (the bits
 // of non-negative floats order like the floats; NaN is skipped by fmaxf), and the reset of the per-query statistics.
 __global__ void __launch_bounds__(256) eval_prep_kernel(const float* __restrict__ q, long long nq_el, const float* __restrict__ g, long long ng_el,
-                                                        unsigned int* absmax_bits, EvalRows er, int nq) {
+                                                        unsigned int* absmax_bits, RowArrays ra, int nq) {
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (absmax_bits) {
@@ -1775,35 +1785,28 @@ __global__ void __launch_bounds__(256) eval_prep_kernel(const float* __restrict_
     mx = warp_max(mx);
     if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(absmax_bits, __float_as_uint(mx));
   }
-  for (long long i = t0; i < nq; i += stride) {
-    er.st_minw[i] = f2ord(FLT_MAX); er.st_maxw[i] = f2ord(-FLT_MAX);
-    er.st_maxb[i] = f2ord(-FLT_MAX); er.st_maxall[i] = f2ord(-FLT_MAX);
-    er.cnt_same[i] = 0;
-  }
+  for (long long i = t0; i < nq; i += stride) reset_row_stats(ra, i);
 }
-void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, EvalRows er, int nq,
+void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, RowArrays ra, int nq,
                       int sms, cudaStream_t st) {
   const long long work = absmax_bits ? (nq_el > ng_el ? nq_el : ng_el) / 16 : nq;   // threads: ~16 elements each
   long long nb = (work + 255) / 256;
   nb = nb < 1 ? 1 : (nb > 8 * sms ? 8 * sms : nb);
-  eval_prep_kernel<<<static_cast<int>(nb), 256, 0, st>>>(q, nq_el, g, ng_el, absmax_bits, er, nq);
+  eval_prep_kernel<<<static_cast<int>(nb), 256, 0, st>>>(q, nq_el, g, ng_el, absmax_bits, ra, nq);
   count_launch();
 }
 
-// Rows of x to one side of the K-concatenated operands of the similarity GEMM, in split_tile's layout (side_b = 0: the A format of
-// the queries, 1: the B format of the gallery; PREC_BF16 has one segment, the same on both sides).  Thread = 8 features of one row.
-// The pre-scale is the layer's rule applied to max|x| over both sets: `absmax` when the caller gives it (>= 0), else *absmax_bits.
+// Rows of x to one side of the K-concatenated operands of the similarity GEMM (side_b = 0: the A format of the queries, 1: the B format
+// of the gallery), through the layer's store_kcat_row.  Thread = 8 features of one row.  The pre-scale is the layer's rule applied to
+// max|x| over both sets: `absmax` when the caller gives it (>= 0), else *absmax_bits.
 template <int PREC>
 __global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict__ x, int rows, int D, long long Dp, int side_b, float absmax,
                                                          const unsigned int* __restrict__ absmax_bits, BlockScalars* bs,
                                                          uint16_t* __restrict__ out) {
   constexpr int NS = SPLIT_FORMATS[PREC].pieces;
-  float sc = 1.f, inv = 1.f;
-  if (PREC == PREC_FP16X2) {
-    const float mx = absmax >= 0.f ? absmax : __uint_as_float(*absmax_bits);
-    if (mx > 0.f && isfinite(mx)) { int e; frexpf(mx, &e); sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e); }
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && !side_b) { bs->x_scale = sc; bs->x_inv_scale = inv; }
+  PreScale ps{1.f, 1.f};
+  if (PREC == PREC_FP16X2) ps = pre_scale(absmax >= 0.f ? absmax : __uint_as_float(*absmax_bits));
+  if (blockIdx.x == 0 && threadIdx.x == 0 && !side_b) { bs->x_scale = ps.scale; bs->x_inv_scale = ps.inv; }
   const long long groups = Dp / 8, i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= rows * groups) return;
   const long long n = i / groups;
@@ -1818,25 +1821,9 @@ __global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict
     for (int e = 0; e < 8; ++e) v[e] = d + e < D ? __ldg(xr + d + e) : 0.f;
   }
   uint16_t p[8][3];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) split3<PREC>(v[e] * sc, p[e][0], p[e][1], p[e][2]);
   uint4 pk[3];
-#pragma unroll
-  for (int s = 0; s < 3; ++s)
-    pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
-                       p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
-  uint16_t* r = out + n * (mma_passes(NS) * Dp);
-  *reinterpret_cast<uint4*>(r + d) = pk[0];
-  if (PREC == PREC_FP16X2) {            // A = [ hi | hi(8) lo(8) ... ]   B = [ hi | lo(8) hi(8) ... ]
-    *reinterpret_cast<uint4*>(r + Dp + 2 * d) = side_b ? pk[1] : pk[0];
-    *reinterpret_cast<uint4*>(r + Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
-  } else if (PREC == PREC_BF16X3) {     // A = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]
-    *reinterpret_cast<uint4*>(r + Dp + d) = pk[1];
-    *reinterpret_cast<uint4*>(r + 2 * Dp + 2 * d) = side_b ? pk[1] : pk[0];
-    *reinterpret_cast<uint4*>(r + 2 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
-    *reinterpret_cast<uint4*>(r + 4 * Dp + 2 * d) = side_b ? pk[2] : pk[0];
-    *reinterpret_cast<uint4*>(r + 4 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[2];
-  }
+  split8<PREC>(v, ps.scale, p, pk);
+  store_kcat_row<PREC>(out + n * (mma_passes(NS) * Dp), Dp, d, pk, side_b);
 }
 void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
                        BlockScalars* bs, uint16_t* out, cudaStream_t st) {
@@ -1848,12 +1835,12 @@ void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, 
 }
 
 // Best positive of each query from the statistics sweep: max over same-label non-self gallery rows, -inf when there is none
-__global__ void eval_best_kernel(EvalRows er, int nq, float* __restrict__ best) {
+__global__ void eval_best_kernel(RowArrays ra, int nq, float* __restrict__ best) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nq) best[i] = er.cnt_same[i] > 0 ? ord2f(er.st_maxw[i]) : -INFINITY;
+  if (i < nq) best[i] = ra.cnt_same[i] > 0 ? ord2f(ra.st_maxw[i]) : -INFINITY;
 }
-void launch_eval_best(EvalRows er, int nq, float* best, cudaStream_t st) {
-  eval_best_kernel<<<(nq + 255) / 256, 256, 0, st>>>(er, nq, best);
+void launch_eval_best(RowArrays ra, int nq, float* best, cudaStream_t st) {
+  eval_best_kernel<<<(nq + 255) / 256, 256, 0, st>>>(ra, nq, best);
   count_launch();
 }
 

@@ -109,8 +109,20 @@ struct BlockScalars {
   unsigned int ticket3;                    // block-completion counter of the GLOBAL select kernels
   float asum;                              // sum |x| over the local features (.cu:400)
   float x_absmax;                          // max |x| over x_total (operand pre-scale for PREC_FP16X2)
-  float x_scale, x_inv_scale;              // power of two s.t. max|x*scale| in [0.5,1]; 1 for other precisions
+  float x_scale, x_inv_scale;              // pre_scale(x_absmax) for PREC_FP16X2; 1 for other precisions
 };
+
+// The operand pre-scale of a set whose largest |x| is `absmax`: a power of two with max|x * scale| in [0.5, 1), so the split is exact
+// and the inverse undoes it exactly; 1 when absmax is 0 or not finite
+struct PreScale { float scale, inv; };
+__host__ __device__ inline PreScale pre_scale(float absmax) {
+  float sc = 1.f, inv = 1.f;
+  if (absmax > 0.f && isfinite(absmax)) {
+    int e; frexpf(absmax, &e);                 // absmax = m * 2^e, m in [0.5,1)
+    sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e);
+  }
+  return PreScale{sc, inv};
+}
 
 struct MiningParams {
   int ap_region, ap_method, an_region, an_method;
@@ -192,20 +204,16 @@ void launch_build_weights(const float* S, long long ldS, int Q, int N, const flo
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);
 
-// Retrieval evaluation (DESIGN 8): the per-query statistics of the similarity GEMM's EPI_STATS epilogue
-struct EvalRows {
-  uint32_t *st_minw, *st_maxw, *st_maxb, *st_maxall;   // ordered-uint encoded
-  int* cnt_same;
-};
+// Retrieval evaluation (DESIGN 8).  `ra` holds only the per-query statistics of the similarity GEMM's EPI_STATS epilogue (st_*, cnt_same).
 // max|x| over queries and gallery (g == NULL: the query set is the gallery) into the pre-zeroed *absmax_bits (NULL: no reduction),
 // and the reset of the nq queries' statistics
-void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, EvalRows er, int nq,
+void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, RowArrays ra, int nq,
                       int sms, cudaStream_t st);
 // rows x D fp32 -> the A (side_b = 0) or B (side_b = 1) format of the K-concatenated operands [rows][mma_passes * Dp], pre-scaled by
-// the power of two of `absmax` (>= 0) or of *absmax_bits; the side-A launch also stores the scale in bs
+// pre_scale of `absmax` (>= 0) or of *absmax_bits; the side-A launch also stores the scale in bs
 void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
                        BlockScalars* bs, uint16_t* out, cudaStream_t st);
 // best[i] = max same-label non-self similarity of query i, -inf when there is none
-void launch_eval_best(EvalRows er, int nq, float* best, cudaStream_t st);
+void launch_eval_best(RowArrays ra, int nq, float* best, cudaStream_t st);
 
 }  // namespace npair

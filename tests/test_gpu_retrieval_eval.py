@@ -1,6 +1,6 @@
 """Retrieval evaluation on the GPU (DESIGN 8): the ranks of the best positives against exact and fp64 brute force, symmetric tiles
-against full tiles, the two-phase sharded form against the one call, agreement with the layer's retrieval tops, and a set whose
-similarity matrix would not fit in HBM."""
+against full tiles, the two-phase sharded form against the one call, the best positives and ranks against the layer's own
+similarities, agreement with the layer's retrieval tops, and a set whose similarity matrix would not fit in HBM."""
 import numpy as np
 import pytest
 
@@ -139,6 +139,34 @@ def test_sharded_gallery_equals_one_call(prec):
         torch.cuda.synchronize()
         assert torch.equal(count.int(), one), (off, (count.int() != one).sum().item())
     ev.close()
+
+
+@pytest.mark.parametrize("prec", PRECS)
+def test_sees_the_layers_similarities(prec):
+    """The evaluator splits and pre-scales its operands exactly as the layer does: p* and the ranks taken from the layer's own fp32 S
+    (world 1, S materialised) come out bit for bit.  Random unit rows at a ragged D, so every lo / mid piece is non-zero."""
+    from npairloss_b200 import capi
+    rng = np.random.default_rng(20171233 + prec)
+    n, D = 1000, 100
+    x = rng.standard_normal((n, D)).astype(np.float32)
+    x /= np.linalg.norm(x, axis=1, keepdims=True)
+    lab = rng.integers(0, n // 3, size=n).astype(np.float32)           # about 3 rows per label, some without a positive
+    xt, lt = _cuda(x), _cuda(lab)
+    ctx = capi.Context(capi.make_config(n, D, sim_precision=prec))
+    ctx.forward(xt, lt)
+    S = ctx.debug_read(0, n * n).reshape(n, n)
+    ctx.close()
+    not_self = ~np.eye(n, dtype=bool)
+    same = (lab[:, None] == lab[None, :]) & not_self
+    p = np.where(same, S, np.float32(-np.inf)).max(1)
+    want = np.where(p > -np.inf, ((S >= p[:, None]) & not_self).sum(1), 0)
+    assert (p == -np.inf).sum() >= 5
+    ev = capi.Evaluator(n, n, D, prec)
+    best = ev.best_positive(xt, lt, xt, lt, float(np.abs(x).max()), 0).cpu().numpy()
+    rank = ev.rank(xt, lt, xt, lt, 0).cpu().numpy()
+    ev.close()
+    np.testing.assert_array_equal(best.view(np.uint32), p.view(np.uint32))
+    np.testing.assert_array_equal(rank, want)
 
 
 def test_agrees_with_layer_tops():
