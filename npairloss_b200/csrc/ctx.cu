@@ -159,6 +159,8 @@ static bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int 
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM launchers
+static int gemm_grid(const TileSched& ts, int sms) { return ts.num_tiles() < sms ? ts.num_tiles() : sms; }   // one CTA per tile, at most one per SM
+
 // K-block per (operand format, GEMM role); see GemmCfg
 static constexpr int bk_of(int prec, int epi) {
   if (epi != EPI_OUT) return 64;                 // similarity GEMM: single pass, 64-element K blocks
@@ -205,8 +207,7 @@ static GemmKernel gemm_kernel(int prec, int epi) {
 static cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
   const GemmKernel k = gemm_kernel(prec, epi);
   if (!k.fn) return cudaErrorInvalidValue;
-  const int tiles = p.tile_list ? p.num_tiles_list : p.tiles_m * p.tiles_n * p.splits;
-  k.fn<<<tiles < sms ? tiles : sms, k.threads, k.smem, st>>>(a, b, sm, p);
+  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(a, b, sm, p);
   count_launch();
   return cudaGetLastError();
 }
@@ -219,8 +220,7 @@ static FusedKernel fused_kernel(int prec) {
 }
 static cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
   const FusedKernel k = fused_kernel(prec);
-  const int tiles = p.tiles_m * p.tiles_n * p.splits;
-  k.fn<<<tiles < sms ? tiles : sms, k.threads, k.smem, st>>>(b, sm, p);
+  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(b, sm, p);
   count_launch();
   return cudaGetLastError();
 }
@@ -363,6 +363,14 @@ static SplitK split_k(int num_kblocks, int tiles, int sms, int min_kb) {
   return SplitK{(num_kblocks + kpb - 1) / kpb, kpb};                    // no empty split
 }
 
+// The tile schedule of either GEMM kernel over a rows x cols output and num_kblocks K blocks, split-K `sk` (default: none)
+using TileShape = GemmCfg<1, 64, EPI_OUT>;
+static_assert(TileShape::BM == FusedCfg<1>::BM && TileShape::BN == FusedCfg<1>::BN, "both GEMM kernels share one tile shape");
+static TileSched tile_sched(int rows, int cols, int num_kblocks, SplitK sk) {
+  return TileSched{num_kblocks, (rows + TileShape::BM - 1) / TileShape::BM, (cols + TileShape::BN - 1) / TileShape::BN, nullptr, 0, sk.splits, sk.kb_per_split};
+}
+static TileSched tile_sched(int rows, int cols, int num_kblocks) { return tile_sched(rows, cols, num_kblocks, SplitK{1, num_kblocks}); }
+
 // blocks of 256 threads for `work` items: at least one, at most max_blocks
 static inline int grid_for(long long work, int max_blocks) {
   const long long nb = (work + 255) / 256;
@@ -407,16 +415,16 @@ static inline int xchg_flag(int kind, int par, int world, int rank) { return (2 
 // 128-row block's diagonal or beyond
 static std::vector<int2> sym_tile_list(int Q, int N) {
   std::vector<int2> tl;
-  const int tm = (Q + 127) / 128, tn = (N + 255) / 256;
-  for (int mb = 0; mb < tm; ++mb)
-    for (int nb = mb / 2; nb < tn; ++nb) tl.push_back(make_int2(mb, nb));
+  const TileSched ts = tile_sched(Q, N, 0);
+  for (int mb = 0; mb < ts.tiles_m; ++mb)
+    for (int nb = mb / 2; nb < ts.tiles_n; ++nb) tl.push_back(make_int2(mb, nb));
   return tl;
 }
 // sym_tile_list(Q, N).size()
 static long long sym_tile_count(int Q, int N) {
-  const int tm = (Q + 127) / 128, tn = (N + 255) / 256;
+  const TileSched ts = tile_sched(Q, N, 0);
   long long n = 0;
-  for (int mb = 0; mb < tm; ++mb) n += mb / 2 < tn ? tn - mb / 2 : 0;
+  for (int mb = 0; mb < ts.tiles_m; ++mb) n += mb / 2 < ts.tiles_n ? ts.tiles_n - mb / 2 : 0;
   return n;
 }
 
@@ -427,10 +435,9 @@ static GemmParams sim_sweep(int epi, int rows, int cols, long long kcat, const f
                             const RowArrays& ra) {
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.M = rows; gp.Nn = cols;
-  gp.num_kblocks = static_cast<int>(kcat / 64);
-  gp.tiles_m = (rows + 127) / 128; gp.tiles_n = (cols + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+  gp.ts = tile_sched(rows, cols, static_cast<int>(kcat / 64));
   gp.dev_scale = inv_scale;
-  if (epi & EPI_SYM) { gp.tile_list = sym_tiles; gp.num_tiles_list = n_sym_tiles; }
+  if (epi & EPI_SYM) { gp.ts.tile_list = sym_tiles; gp.ts.num_tiles_list = n_sym_tiles; }
   if (epi & EPI_STATS) {
     gp.st_minw = ra.st_minw; gp.st_maxw = ra.st_maxw; gp.st_maxb = ra.st_maxb; gp.st_maxall = ra.st_maxall; gp.cnt_same = ra.cnt_same;
   }
@@ -514,7 +521,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.grad_chunk_kb = cfg.grad_chunk_cols > 0 ? (cfg.grad_chunk_cols + 31) / 32 : (cfg.grad_chunk_cols < 0 ? 0 : 64);
   // the fused kernel walks K in 32-column blocks and keeps >= 8 of them (256 columns) per split; the split GEMM keeps >= 4
   p.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
-  const int tiles = static_cast<int>(((Q + 127) / 128) * ((D + 255) / 256));
+  const int tiles = tile_sched(cfg.Q, cfg.D, p.grad_kblocks).num_tiles();
   p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
   if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, p.N));
   p.sweep_epi = EPI_STATS | (p.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
@@ -533,7 +540,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   if (!p.fused_grad) b[B_H] = 2 * ns * Q * p.Np;                                // materialised gradient weights
   if (rs) { b[B_XLT] = 2 * ns * D * p.Qp; b[B_HT] = 2 * ns * N * p.Qp; b[B_OUT2] = f * N * D; }
   if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = sizeof(RowRecord) * N;   // gathered row records
-  if (p.grad_split.splits > 1) b[B_PART] = f * p.grad_split.splits * Q * D;     // split-K partial products
+  if (p.grad_split.splits > 1) b[B_PART] = f * split_part(p.grad_split.splits, cfg.Q, D);   // split-K partial products
   b[B_ROWS] = (4 * 13 + sizeof(RowRecord)) * Q + 64;   // 13 row arrays of Q 4-byte words (RowArrays) + the 32-byte aligned row records
   b[B_BS] = sizeof(BlockScalars);
   b[B_PARTIAL] = f * 2048;
@@ -1267,7 +1274,7 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
 
 // d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
 static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, float beta, cudaStream_t st) {
-  const long long n = static_cast<long long>(rows) * c->D;
+  const long long n = split_part(1, rows, c->D);                       // one slice; the kernel takes it as the slice stride
   splitk_reduce_kernel<<<grid_for(n / 4, 8 * c->sms), 256, 0, st>>>(c->part, splits, n, d_diff, beta);
   count_launch();
 }
@@ -1304,14 +1311,13 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   if (tc && c->fused_grad) {
     // weights are produced inside the gradient GEMM: no H in HBM
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));
-    fp.N = N; fp.D = D; fp.num_kblocks = c->grad_kblocks;
-    fp.tiles_n = (D + 255) / 256;
+    fp.N = N; fp.D = D;
     fp.colrec = rs_total ? rs_total : c->ra.rowrec;
     fp.inv_world = c->wscope ? 1.f : 1.f / static_cast<float>(c->world);
     fp.log2_world = c->wscope ? 0.f : log2f(static_cast<float>(c->world));
     fp.sgn_p = ap_sign(mp.ap_method); fp.sgn_n = an_sign(mp.an_method);
     fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
-    fp.part = c->part; fp.splits = c->grad_split.splits; fp.kb_per_split = c->grad_split.kb_per_split;
+    fp.part = c->part;
     fp.chunk_kb = c->grad_chunk_kb;
     // per block of rows of S, starting with the one the forward left in the buffer (a materialised S is the one block): recompute it,
     // then its gradient rows.  The split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output
@@ -1321,10 +1327,10 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     for (int k = 0; k < c->n_blocks; ++k) {
       const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
-      fp.Q = rows; fp.tiles_m = (rows + 127) / 128; fp.m_blk0 = r0 / 128;
+      fp.Q = rows; fp.ts = tile_sched(rows, D, c->grad_kblocks, c->grad_split); fp.m_blk0 = r0 / TileShape::BM;
       fp.rowrec = c->ra.rowrec + r0; fp.self_offset = self_off + r0; fp.out = d_diff + static_cast<long long>(r0) * D;
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
-      if (fp.splits > 1) reduce_splits(c, fp.splits, rows, fp.out, 0.f, st);
+      if (fp.ts.splits > 1) reduce_splits(c, fp.ts.splits, rows, fp.out, 0.f, st);
     }
     CUDA_TRY(c, cudaGetLastError());
     return NPAIR_OK;
@@ -1338,8 +1344,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   const bool rs_path = c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER;
   if (rs_path) {
     // total = (1/2)(1/k)(lw/Q) * G^T . X_local  (N x D)  -> reduce-scatter (== all-reduce + own slice, .cu:462-497)
-    gp.M = N; gp.Nn = D; gp.num_kblocks = static_cast<int>((Q + c->bk_grad - 1) / c->bk_grad);
-    gp.tiles_m = (N + 127) / 128; gp.tiles_n = (D + 255) / 256; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+    gp.M = N; gp.Nn = D; gp.ts = tile_sched(N, D, (Q + c->bk_grad - 1) / c->bk_grad);
     gp.out = d_total_ext ? d_total_ext : c->OUT2; gp.ldo = D; gp.alpha = 0.5f * (1.f / static_cast<float>(c->world)) * lw_over_q; gp.beta = 0.f;
     {
       PhaseTimer pt(c, 7, st);
@@ -1354,15 +1359,14 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     }
   }
   // d_diff = (1/2)(lw/Q) * H . X_total  (H = G + G^T/world in the symmetric modes; accumulated onto the scattered term otherwise)
-  gp.M = Q; gp.Nn = D; gp.num_kblocks = c->grad_kblocks;
-  gp.tiles_m = (Q + 127) / 128; gp.tiles_n = (D + 255) / 256;
+  gp.M = Q; gp.Nn = D; gp.ts = tile_sched(Q, D, c->grad_kblocks, c->grad_split);
   gp.out = d_diff; gp.ldo = D; gp.alpha = 0.5f * lw_over_q; gp.beta = (rs_path && !d_total_ext) ? 1.f : 0.f;
-  gp.splits = c->grad_split.splits; gp.kb_per_split = c->grad_split.kb_per_split; gp.part = c->part;
+  gp.part = c->part;
   {
     PhaseTimer pt(c, 6, st);
     if (tc) CUDA_TRY(c, launch_gemm(c->prec, EPI_OUT,c->tm_b1A, c->tm_b1B, c->tm_S, gp, c->sms, st));
     else CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_OUT, c->H, c->Np, static_cast<long long>(Q) * c->Np, c->XsT, c->Np, static_cast<long long>(D) * c->Np, N, gp, st));
-    if (gp.splits > 1) reduce_splits(c, gp.splits, Q, d_diff, gp.beta, st);
+    if (gp.ts.splits > 1) reduce_splits(c, gp.ts.splits, Q, d_diff, gp.beta, st);
   }
   CUDA_TRY(c, cudaGetLastError());
   return NPAIR_OK;
@@ -1528,8 +1532,8 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
     launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
     launch_split(dB, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
     GemmParams gp; memset(&gp, 0, sizeof(gp));
-    gp.M = M; gp.Nn = Nn; gp.num_kblocks = (K + bk - 1) / bk; gp.tiles_m = (M + 127) / 128; gp.tiles_n = (Nn + 255) / 256;
-    gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f; gp.splits = 1; gp.kb_per_split = gp.num_kblocks;
+    gp.M = M; gp.Nn = Nn; gp.ts = tile_sched(M, Nn, (K + bk - 1) / bk);
+    gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f;
     // EPI_OUT applies the inverse scale once; both operands were scaled -> fold the second factor into alpha
     gp.alpha = sc[1]; gp.dev_scale = &bs->x_inv_scale;
     if (backend == NPAIR_GEMM_TCGEN05) {

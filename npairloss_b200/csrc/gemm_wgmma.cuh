@@ -40,14 +40,31 @@ namespace npair {
 //               also counts, for each column gc, its entries against cut[gc].  Used without EPI_STATS and EPI_STORE_S.
 enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64 };
 
+// Persistent tile schedule of both wgmma GEMMs (host: tile_sched, ctx.cu).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
+// output tile (m_blk, n_blk) or tile_list[t], K blocks [kb0, kb1) of split-K slice `split`.  split moves fastest, then n_blk, m_blk.
+struct Tile { int m_blk, n_blk, split, kb0, kb1; };
+struct TileSched {
+  int num_kblocks;            // K extent in K blocks
+  int tiles_m, tiles_n;       // row and column tiles of the output
+  const int2* tile_list;      // optional explicit (m_blk, n_blk) list; tiles_m*tiles_n entries are then ignored
+  int num_tiles_list;
+  int splits, kb_per_split;   // split-K: slice s covers K blocks [s*kb_per_split, min(num_kblocks, (s+1)*kb_per_split))
+  __host__ __device__ int num_tiles() const { return tile_list ? num_tiles_list : tiles_m * tiles_n * splits; }
+  __device__ __forceinline__ Tile at(int tile) const {
+    const int mn = tile / splits, split = tile - mn * splits, kb0 = split * kb_per_split;
+    int m_blk = mn / tiles_n, n_blk = mn % tiles_n;
+    if (tile_list) { const int2 tl = tile_list[tile]; m_blk = tl.x; n_blk = tl.y; }
+    return Tile{m_blk, n_blk, split, kb0, min(num_kblocks, kb0 + kb_per_split)};
+  }
+};
+
+// Offset in floats of split-K slice `split` in the partial products [split][rows][ldo]
+__host__ __device__ __forceinline__ long long split_part(int split, int rows, long long ldo) { return static_cast<long long>(split) * rows * ldo; }
+
 struct GemmParams {
   int M, Nn;           // logical output extent
-  int num_kblocks;     // K_pad / BK
-  int tiles_m, tiles_n;
-  const int2* tile_list;      // optional explicit (m_blk, n_blk) list (EPI_SYM); tiles_m*tiles_n entries are then ignored
-  int num_tiles_list;
-  int splits, kb_per_split;   // split-K (EPI_OUT only): tile = (m_blk*tiles_n + n_blk)*splits + split, k-blocks [split*kb_per_split, ...)
-  float* part;                // splits > 1: partial products [split][M][ldo]; a reduce kernel sums them in fixed order
+  TileSched ts;        // split-K: EPI_OUT only; tile list: EPI_SYM only
+  float* part;         // splits > 1: partial products [split][M][ldo] (split_part); a reduce kernel sums them in fixed order
   // ---- similarity epilogues ----
   float* S;            // [M x ldS] fp32 similarities
   long long ldS;       // multiple of 32
@@ -101,6 +118,28 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_STAGE_BYTES + STORE_STAGE_BYTES + SMEM_AUX + 1024 /*alignment slack*/;
   static constexpr int THREADS = 384;                         // producer warpgroup + 2 consumer warpgroups
   static_assert(STAGES >= 2 && 16 * STAGES <= 192, "operand ring");
+};
+
+// The operand ring of both GEMM kernels: per stage a `full` barrier (the producer's arrival + the TMA bytes) and an `empty` barrier
+// (one arrival per consumer warp).  The producer thread and every consumer thread walk the stages with their own (stage, phase).
+template <int STAGES>
+struct StageRing {
+  uint64_t *full, *empty;      // [STAGES] each, empty right after full
+  int stage = 0; uint32_t phase = 0;
+  __device__ explicit StageRing(uint8_t* bars) : full(reinterpret_cast<uint64_t*>(bars)), empty(full + STAGES) {}
+  __device__ void init() const {       // one thread, before the __syncthreads that publishes the barriers
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
+    ptx::fence_mbar_init();
+  }
+  // producer: wait until the consumers released the stage, expect `bytes` on its full barrier and return it for the loads
+  __device__ uint64_t* produce(uint32_t bytes) const {
+    ptx::mbar_wait(&empty[stage], phase ^ 1);
+    ptx::mbar_arrive_expect_tx(&full[stage], bytes);
+    return &full[stage];
+  }
+  __device__ void wait_full() const { ptx::mbar_wait(&full[stage], phase); }
+  __device__ void release(int st, int lane) const { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty[st]); }   // MMAs on st retired
+  __device__ void advance() { if (++stage == STAGES) { stage = 0; phase ^= 1; } }
 };
 
 __device__ __forceinline__ void pass_pieces(int nsplit, int p, int& sa, int& sb) {
@@ -190,14 +229,12 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint8_t* acc_stage = smem + STAGES * Cfg::STAGE_BYTES;            // [2 warpgroups][64 rows][16 x 16 B], chunk ^ (row & 7)
   uint8_t* store_stage = acc_stage + Cfg::ACC_STAGE_BYTES;          // [8 warps][32 rows][128 B], 128B-swizzled
   uint8_t* aux = store_stage + Cfg::STORE_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);            // [STAGES]
-  uint64_t* empty_bar = full_bar + STAGES;                           // [STAGES]
   float* s_lab = reinterpret_cast<float*>(aux + 256);                // [256] column labels of the current tile (EPI_STATS)
   float* s_labr = reinterpret_cast<float*>(aux + 256 + 1024);        // [128] row labels of the current tile (EPI_SYM)
   float2* s_rng = reinterpret_cast<float2*>(aux + 256 + 1024 + 512); // [8] {min, max} label of each 32-column chunk, [8..12) of each 32-row group
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = p.tile_list ? p.num_tiles_list : p.tiles_m * p.tiles_n * p.splits;
+  const int num_tiles = p.ts.num_tiles();
   const float inv_scale = p.dev_scale ? *p.dev_scale : 1.f;
   const float out_scale = (EPI != EPI_OUT) ? inv_scale * inv_scale : 1.f;
   const float alpha = p.alpha * inv_scale;
@@ -207,10 +244,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     ptx::prefetch_tmap(&tmapB);
     if (STORE) ptx::prefetch_tmap(&tmapS);
   }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }
-    ptx::fence_mbar_init();
-  }
+  if (warp == 1 && lane == 0) StageRing<STAGES>(aux).init();     // barriers: aux[0, 16 * STAGES)
   __syncthreads();
 
   // Register split as in the fused gradient kernel: the producer warpgroup (warps 0-3, one working thread) keeps 40 registers, the
@@ -221,22 +255,18 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     // ===================================== TMA producer =====================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0 && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      StageRing<STAGES> ring(aux);
       for (int tile = worker; tile < num_tiles; tile += num_workers) {
-        const int mn = tile / p.splits, split = tile - mn * p.splits;
-        int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
-        if (p.tile_list) { const int2 tl = p.tile_list[tile]; m_blk = tl.x; n_blk = tl.y; }
-        const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kblocks, kb0 + p.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* st = smem + stage * Cfg::STAGE_BYTES;
-          ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+        const Tile t = p.ts.at(tile);
+        for (int kb = t.kb0; kb < t.kb1; ++kb) {
+          uint64_t* full = ring.produce(Cfg::STAGE_BYTES);
+          uint8_t* st = smem + ring.stage * Cfg::STAGE_BYTES;
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s) {
-            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, &full_bar[stage], kb * BK, m_blk * BM + (STORE && !STATS ? p.a_row0 : 0), s);
-            ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, &full_bar[stage], kb * BK, n_blk * BN, s);
+            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, full, kb * BK, t.m_blk * BM + (STORE && !STATS ? p.a_row0 : 0), s);
+            ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, full, kb * BK, t.n_blk * BN, s);
           }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          ring.advance();
         }
       }
     }
@@ -254,14 +284,11 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     const int et = threadIdx.x - 128;            // 0..255
     uint8_t* const accs = acc_stage + g * (64 * 256);
     uint8_t* const stg = store_stage + cw * 4096;
-    int stage = 0; uint32_t phase = 0;
+    StageRing<STAGES> ring(aux);
     for (int tile = worker; tile < num_tiles; tile += num_workers) {
-      const int mn = tile / p.splits, split = tile - mn * p.splits;
-      int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
-      if (p.tile_list) { const int2 tl = p.tile_list[tile]; m_blk = tl.x; n_blk = tl.y; }
-      const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kblocks, kb0 + p.kb_per_split);
-      const int row = m_blk * BM + ew * 32 + lane;
-      const int col_base = n_blk * BN;
+      const Tile t = p.ts.at(tile);
+      const int row = t.m_blk * BM + ew * 32 + lane;
+      const int col_base = t.n_blk * BN;
       float lab_i = 0.f;
       if (STATS) {
         asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers are done with s_lab
@@ -294,15 +321,11 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      auto release = [&](int st_idx) {
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty_bar[st_idx]);
-      };
-      int prev = stage;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase);
-        const uint32_t a0 = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES) + g * 64 * Cfg::ROW_BYTES;
-        const uint32_t b0 = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES) + NSPLIT * Cfg::A_PIECE;
+      int prev = ring.stage;
+      for (int kb = t.kb0; kb < t.kb1; ++kb) {
+        ring.wait_full();
+        const uint32_t a0 = ptx::smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + g * 64 * Cfg::ROW_BYTES;
+        const uint32_t b0 = ptx::smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + NSPLIT * Cfg::A_PIECE;
         ptx::wgmma_fence();
 #pragma unroll
         for (int ps = 0; ps < Cfg::NPASS; ++ps) {
@@ -317,19 +340,19 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         ptx::wgmma_commit();
         ptx::wgmma_wait<1>();
-        if (kb != kb0) release(prev);
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (kb != t.kb0) ring.release(prev, lane);
+        prev = ring.stage;
+        ring.advance();
       }
       ptx::wgmma_wait<0>();
       ptx::fence_regs(acc);
-      if (kb1 > kb0) release(prev);
+      if (t.kb1 > t.kb0) ring.release(prev, lane);
 
       if (EPI == EPI_OUT) {
         // fragments straight to global memory: (row, 2 consecutive columns) per register pair
-        float* obase = p.splits > 1 ? p.part + static_cast<long long>(split) * p.M * p.ldo : p.out;
-        const float beta = p.splits > 1 ? 0.f : p.beta;
-        const int rbase = m_blk * BM + g * 64 + wi * 16 + (lane >> 2);
+        float* obase = p.ts.splits > 1 ? p.part + split_part(t.split, p.M, p.ldo) : p.out;
+        const float beta = p.ts.splits > 1 ? 0.f : p.beta;
+        const int rbase = t.m_blk * BM + g * 64 + wi * 16 + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           const int col = col_base + 8 * j + 2 * (lane & 3);
@@ -380,7 +403,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         const int col0 = col_base + ch * 32;
         const int cb = col0 >> 7;                          // 128-wide column block (EPI_SYM bookkeeping)
         // lower-triangle half of a straddling tile: produced by mirroring
-        if ((SYM && cb < m_blk) || col0 >= p.Nn) continue;
+        if ((SYM && cb < t.m_blk) || col0 >= p.Nn) continue;
         float v[32];
         if (STATS || COUNT) {
 #pragma unroll
@@ -396,7 +419,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int rr = 4 * i + (lane >> 3);
-            const int grow = m_blk * BM + ew * 32 + rr;
+            const int grow = t.m_blk * BM + ew * 32 + rr;
             const int sr = (wi & 1) * 32 + rr;
             float4 o = *reinterpret_cast<const float4*>(accs + sr * 256 + (((half * 8 + cq) ^ (sr & 7)) << 4));
             o.x *= out_scale; o.y *= out_scale; o.z *= out_scale; o.w *= out_scale;
@@ -415,7 +438,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         if (COUNT && row < p.M)
           cnt_ge += count32(v, cut_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col);
-        if (SYM && cb > m_blk && m_blk * BM + ew * 32 < p.M) {
+        if (SYM && cb > t.m_blk && t.m_blk * BM + ew * 32 < p.M) {
           // ---- mirrored store: staging row c holds S[col0 + c][rows of this warp]; box lands at (x = row block, y = col0) ----
           if (STORE && lane == 0) ptx::tma_store_wait_read<0>();   // this warp's previous box has been read out of smem
           __syncwarp();
@@ -424,7 +447,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             *reinterpret_cast<float*>(stg + c * 128 + ((((lane >> 2) ^ (c & 7))) << 4) + ((lane & 3) << 2)) = v[c];
           if (STORE) ptx::fence_proxy_async_smem();
           __syncwarp();
-          if (STORE && lane == 0) { ptx::tma_store_2d(&tmapS, stg, m_blk * BM + ew * 32, col0); ptx::tma_store_commit(); }
+          if (STORE && lane == 0) { ptx::tma_store_2d(&tmapS, stg, t.m_blk * BM + ew * 32, col0); ptx::tma_store_commit(); }
           // ---- mirrored statistics: the staging tile is the transposed chunk, so lane L reads back ROW gc = col0 + L of the
           //      symmetric matrix (32 entries against this warp's 32 row labels) and reuses the per-thread statistics ----
           const int gc = col0 + lane;
@@ -436,7 +459,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           }
           float t_minw = FLT_MAX, t_maxw = -FLT_MAX, t_maxb = -FLT_MAX;
           int t_cnt = 0;
-          const int r0 = m_blk * BM + ew * 32;
+          const int r0 = t.m_blk * BM + ew * 32;
           const float lab_c = s_lab[ch * 32 + lane];
           const float2 rr = s_rng[8 + ew];
           const bool plain = __all_sync(0xffffffffu, gc >= p.Nn || lab_c < rr.x || lab_c > rr.y) && r0 + 32 <= p.M;

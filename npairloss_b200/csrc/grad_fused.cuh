@@ -23,11 +23,9 @@ namespace npair {
 
 struct FusedGradParams {
   int Q, N, D;
-  int num_kblocks;              // ceil(N / 32)
-  int tiles_m, tiles_n;         // 128-row blocks, 256-column tiles of D
-  int splits, kb_per_split;     // split-K over the sample index (few row blocks when Q = B / world is small)
+  TileSched ts;                 // Q x D output, ceil(N / 32) K blocks; split-K over the sample index (few row blocks when Q = B / world is small)
   int chunk_kb;                 // accumulation chunk in K blocks (0 = the whole K range in one accumulator), see below
-  float* part;                  // split-K partials [split][Q][ldo]
+  float* part;                  // split-K partials (split_part)
   const float* S;               // only for address checks; tiles come through the tensor map
   const RowRecord* rowrec;      // [Q] this rank's row records
   const RowRecord* colrec;      // [N] records of every column's row (== rowrec when world == 1)
@@ -153,19 +151,16 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);            // [STAGES] TMA bytes landed (B, S tile, column records)
-  uint64_t* empty_bar = full_bar + STAGES;                           // [STAGES] every consumer warp is done with the stage
+  StageRing<STAGES> ring(smem + STAGES * Cfg::STAGE_BYTES);          // a stage: B pieces, S tile, column records
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = p.tiles_m * p.tiles_n * p.splits;
+  const int num_tiles = p.ts.num_tiles();
   const float inv_scale = p.dev_scale ? *p.dev_scale : 1.f;
   const float alpha = p.alpha * inv_scale;
 
   if (warp == 8 && lane == 0) {
     ptx::prefetch_tmap(&tmapB); ptx::prefetch_tmap(&tmapS);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 8); }
-    ptx::fence_mbar_init();
+    ring.init();
   }
   __syncthreads();
 
@@ -174,23 +169,19 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
     // the producer warpgroup hands its registers to the consumers (128 accumulators + the weight builder per thread)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 8 && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
       for (int tile = worker; tile < num_tiles; tile += num_workers) {
-        const int mn = tile / p.splits, split = tile - mn * p.splits;
-        const int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
-        const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kblocks, kb0 + p.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+        const Tile t = p.ts.at(tile);
+        for (int kb = t.kb0; kb < t.kb1; ++kb) {
           const int m0 = kb * BK;
           const uint32_t crec_bytes = static_cast<uint32_t>(min(BK, p.N - m0)) * static_cast<uint32_t>(sizeof(RowRecord));
-          uint8_t* st = smem + stage * Cfg::STAGE_BYTES;
-          ptx::mbar_arrive_expect_tx(&full_bar[stage], NSPLIT * Cfg::B_PIECE + Cfg::S_TILE + crec_bytes);
+          uint64_t* full = ring.produce(NSPLIT * Cfg::B_PIECE + Cfg::S_TILE + crec_bytes);
+          uint8_t* st = smem + ring.stage * Cfg::STAGE_BYTES;
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s)
-            ptx::tma_load_3d(st + s * Cfg::B_PIECE, &tmapB, &full_bar[stage], m0, n_blk * BN, s);
-          ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE, &tmapS, &full_bar[stage], m0, m_blk * BM);
-          bulk_copy_g2s(st + NSPLIT * Cfg::B_PIECE + Cfg::S_TILE, p.colrec + m0, crec_bytes, &full_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            ptx::tma_load_3d(st + s * Cfg::B_PIECE, &tmapB, full, m0, t.n_blk * BN, s);
+          ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE, &tmapS, full, m0, t.m_blk * BM);
+          bulk_copy_g2s(st + NSPLIT * Cfg::B_PIECE + Cfg::S_TILE, p.colrec + m0, crec_bytes, full);
+          ring.advance();
         }
       }
     }
@@ -206,7 +197,6 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
     const int g = warp >> 2, wi = warp & 3;
     const int c4 = lane & 3;
     const int rl0 = g * 64 + wi * 16 + (lane >> 2);  // tile rows of this thread's fragment: rl0, rl0 + 8
-    int stage = 0; uint32_t phase = 0;
     // A fragment of K step k2 of K block kb (in ring stage `st_idx`): columns 16*k2 + 2*c4 + {0, 1} (t = 0) and + 8 (t = 1),
     // rows rl0 (h = 0) and rl0 + 8 (h = 1)
     auto build = [&](uint32_t (&af)[NSPLIT][4], const RowRec (&rr)[2], int st_idx, int kb, int k2) {
@@ -231,31 +221,25 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
         }
       }
     };
-    auto release = [&](int st_idx) {
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&empty_bar[st_idx]);
-    };
     for (int tile = worker; tile < num_tiles; tile += num_workers) {
-      const int mn = tile / p.splits, split = tile - mn * p.splits;
-      const int m_blk = mn / p.tiles_n, n_blk = mn % p.tiles_n;
-      const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kblocks, kb0 + p.kb_per_split);
-      const int ckey = ((p.m_blk0 + m_blk) >> 1) + n_blk + split;
-      float* obase = p.splits > 1 ? p.part + static_cast<long long>(split) * p.Q * p.ldo : p.out;
-      const float beta = p.splits > 1 ? 0.f : p.beta;
+      const Tile t = p.ts.at(tile);
+      const int ckey = ((p.m_blk0 + t.m_blk) >> 1) + t.n_blk + t.split;
+      float* obase = p.ts.splits > 1 ? p.part + split_part(t.split, p.Q, p.ldo) : p.out;
+      const float beta = p.ts.splits > 1 ? 0.f : p.beta;
       RowRec rr[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) rr[h] = load_rowrec(p, m_blk * BM + rl0 + 8 * h);
+      for (int h = 0; h < 2; ++h) rr[h] = load_rowrec(p, t.m_blk * BM + rl0 + 8 * h);
       float acc[128];
       uint32_t af[2][NSPLIT][4];
-      for (int c0 = kb0, c1; c0 < kb1; c0 = c1) {
-        c1 = chunk_end(c0, kb0, kb1, p.chunk_kb, ckey);
-        ptx::mbar_wait(&full_bar[stage], phase);
-        build(af[0], rr, stage, c0, 0);
-        int prev = stage;
+      for (int c0 = t.kb0, c1; c0 < t.kb1; c0 = c1) {
+        c1 = chunk_end(c0, t.kb0, t.kb1, p.chunk_kb, ckey);
+        ring.wait_full();
+        build(af[0], rr, ring.stage, c0, 0);
+        int prev = ring.stage;
         for (int kb = c0; kb < c1; ++kb) {
-          const int cur = stage;
+          const int cur = ring.stage;
           const uint32_t b0 = ptx::smem_u32(smem + cur * Cfg::STAGE_BYTES);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          ring.advance();
 #pragma unroll
           for (int k2 = 0; k2 < KSTEPS; ++k2) {
             ptx::wgmma_fence();
@@ -268,27 +252,27 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
             }
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>();                  // the previous step retired: its A buffer is free, and so is its stage
-            if (k2 == 0 && kb != c0) release(prev);
+            if (k2 == 0 && kb != c0) ring.release(prev, lane);
             if (k2 + 1 < KSTEPS) {
               build(af[(k2 + 1) & 1], rr, cur, kb, k2 + 1);
             } else if (kb + 1 < c1) {
-              ptx::mbar_wait(&full_bar[stage], phase);
-              build(af[0], rr, stage, kb + 1, 0);
+              ring.wait_full();
+              build(af[0], rr, ring.stage, kb + 1, 0);
             }
           }
           prev = cur;
         }
         ptx::wgmma_wait<0>();
         ptx::fence_regs(acc);
-        release(prev);
+        ring.release(prev, lane);
         // drain the chunk: first chunk of the tile stores (+ beta * out), later chunks add (fp32 RN)
-        const bool first = (c0 == kb0);
+        const bool first = (c0 == t.kb0);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          const int col = n_blk * BN + 8 * j + 2 * c4;
+          const int col = t.n_blk * BN + 8 * j + 2 * c4;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int row = m_blk * BM + rl0 + 8 * h;
+            const int row = t.m_blk * BM + rl0 + 8 * h;
             if (row >= p.Q || col >= p.D) continue;
             float* dst = obase + static_cast<long long>(row) * p.ldo + col;
             float o0 = alpha * acc[4 * j + 2 * h], o1 = alpha * acc[4 * j + 2 * h + 1];
