@@ -253,6 +253,26 @@ int npair_eval_best_positive(npair_eval* ev, const float* d_query, const float* 
                              void* stream);
 int npair_eval_count(npair_eval* ev, const float* d_query, int32_t nq, const float* d_gallery, int32_t ng, int32_t self_offset,
                      int32_t gallery_row0, float absmax, const float* d_cut, int32_t* d_count, void* stream);
+/* MAP@R and R-Precision (Musgrave et al., "A Metric Learning Reality Check", 2020), with the conventions of npair_eval_rank:
+ *   R_i      = #{ j != self(i) : l_j = l_i }  (labels compared as floats), and query i's positives sorted p_1 >= p_2 >= ... >= p_R
+ *   pos_k    = k + #{ negatives j : s_ij >= p_k }   (a negative that ties a positive is placed before it)
+ *   R-Precision_i = #{ k : pos_k <= R_i } / R_i,     MAP@R_i = (1/R_i) * sum over { k : pos_k <= R_i } of k / pos_k
+ * in fp64, summed in ascending k and divided by R_i last; both are NaN for R_i = 0.  Without ties these are the usual definitions.
+ * Arguments as for npair_eval_rank; writes d_map_r[nq] and d_r_precision[nq] (double) and, unless NULL, d_R[nq] and d_rank[nq] (int32),
+ * where d_rank is bit for bit npair_eval_rank's rank, so the one call also gives Recall@K.
+ * Three sweeps of the similarity GEMM (R_i; the positives; the negatives bucketed among them), a per-query sort and a finishing pass.
+ * The call synchronises with the host ONCE, after the first sweep, to read sum R_i; the rest is asynchronous on `stream`.
+ * Device memory: on top of the workspace, npair_eval_map_at_r_bytes(nq, sum R_i), grown on demand, kept by the evaluator and freed by
+ * npair_eval_destroy (growing it waits for the device).  sum R_i is quadratic in the rows per label: a set with few labels needs
+ * about 8 * n^2 / labels bytes, and NPAIR_E_CUDA with the byte count is returned when it cannot be allocated.
+ * A query whose second sweep finds more positives than the first counted (which their shared pair predicate rules out) never writes
+ * outside its segment: its results are NaN and the next call on the evaluator returns NPAIR_E_CUDA. */
+int npair_eval_map_at_r(npair_eval* ev, const float* d_query, const float* d_qlabel, int32_t nq, const float* d_gallery,
+                        const float* d_glabel, int32_t ng, int32_t self_offset, double* d_map_r, double* d_r_precision,
+                        int32_t* d_R /* may be NULL */, int32_t* d_rank /* may be NULL */, void* stream);
+/* Device memory npair_eval_map_at_r adds on top of the workspace for nq queries with sum_r = sum R_i positive pairs:
+ * 12 bytes per query, 8 bytes per positive pair and 24 bytes.  0 for nq < 1 or sum_r < 0. */
+size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r);
 
 #ifdef __cplusplus
 }

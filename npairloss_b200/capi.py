@@ -44,7 +44,7 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
-           "npair_eval_best_positive", "npair_eval_count"]
+           "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes"]
 
 _LIB = None
 
@@ -106,6 +106,9 @@ def lib():
         L.npair_eval_rank.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, vp]
         L.npair_eval_best_positive.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, i32, C.c_float, vp, vp]
         L.npair_eval_count.argtypes = [vp, vp, i32, vp, i32, i32, i32, C.c_float, vp, vp, vp]
+        L.npair_eval_map_at_r.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp]
+        L.npair_eval_map_at_r_bytes.argtypes = [i32, C.c_int64]
+        L.npair_eval_map_at_r_bytes.restype = C.c_size_t
         _LIB = L
     return _LIB
 
@@ -236,6 +239,11 @@ def eval_workspace_bytes(max_queries: int, max_gallery: int, D: int, precision: 
     return int(lib().npair_eval_workspace_bytes(max_queries, max_gallery, D, precision))
 
 
+def eval_map_at_r_bytes(nq: int, sum_r: int) -> int:
+    """Device bytes Evaluator.map_at_r adds on top of the workspace for nq queries with sum_r positive pairs in all (0 if invalid)."""
+    return int(lib().npair_eval_map_at_r_bytes(nq, sum_r))
+
+
 class Evaluator:
     """Retrieval evaluation (include/npair_b200.h, DESIGN 8): the rank of every query's best positive among the gallery, computed on
     the tensor cores without storing the similarity matrix.  Takes contiguous CUDA fp32 tensors; results are int32 / fp32 CUDA
@@ -298,6 +306,20 @@ class Evaluator:
                                            self_offset, gallery_row0, C.c_float(absmax), self._arg(cut, 1), count.data_ptr(),
                                            torch.cuda.current_stream().cuda_stream))
         return count
+
+    def map_at_r(self, query, qlabel, gallery, glabel, self_offset=-1):
+        """npair_eval_map_at_r: fp64 map_r[nq] and r_precision[nq] (NaN where a query has no positive), int32 R[nq] and rank[nq]
+        (rank as Evaluator.rank).  Synchronises with the host once, to size its positive-pair buffer."""
+        import torch
+        nq, dev = query.shape[0], query.device
+        map_r = torch.empty(nq, dtype=torch.float64, device=dev)
+        r_prec = torch.empty(nq, dtype=torch.float64, device=dev)
+        R = torch.empty(nq, dtype=torch.int32, device=dev)
+        rank = torch.empty(nq, dtype=torch.int32, device=dev)
+        self._check(lib().npair_eval_map_at_r(self._h, self._arg(query, 2), self._arg(qlabel, 1), nq, self._arg(gallery, 2),
+                                              self._arg(glabel, 1), gallery.shape[0], self_offset, map_r.data_ptr(), r_prec.data_ptr(),
+                                              R.data_ptr(), rank.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        return {"map_r": map_r, "r_precision": r_prec, "R": R, "rank": rank}
 
 
 def debug_gemm(precision, backend, A, B):

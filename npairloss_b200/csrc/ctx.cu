@@ -193,6 +193,10 @@ static GemmKernel sim_gemm_t(int epi) {
     case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
     case EPI_COUNT: return gemm_t<1, BF16, EPI_COUNT, 64>();                       // retrieval evaluation
     case EPI_COUNT | EPI_SYM: return gemm_t<1, BF16, EPI_COUNT | EPI_SYM, 64>();
+    case EPI_GATHER: return gemm_t<1, BF16, EPI_GATHER, 64>();                     // MAP@R evaluation
+    case EPI_GATHER | EPI_SYM: return gemm_t<1, BF16, EPI_GATHER | EPI_SYM, 64>();
+    case EPI_BUCKET: return gemm_t<1, BF16, EPI_BUCKET, 64>();
+    case EPI_BUCKET | EPI_SYM: return gemm_t<1, BF16, EPI_BUCKET | EPI_SYM, 64>();
     default: return GemmKernel{nullptr, 0, 0};
   }
 }
@@ -1602,8 +1606,34 @@ struct npair_eval : EvalPlan {
   int2* sym_tiles = nullptr;
   int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
   std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
+  // MAP@R (npair_eval_map_at_r), grown on demand and kept: per query the segment offsets and gather counters, per positive pair the
+  // positive and its bucket counter (map_at_r_bytes)
+  void* map_rows = nullptr;
+  size_t map_rows_bytes = 0;
+  void* map_pairs = nullptr;
+  size_t map_pairs_bytes = 0;
   std::string err;
 };
+
+// Device memory of npair_eval_map_at_r beyond the workspace, in the two parts it is allocated in: per query the nq + 1 segment offsets,
+// the gather counter and the {sum R, error bits} word pair; per positive pair the value and the histogram word
+static size_t map_rows_bytes(long long nq) { return 8ull * (nq + 1) + 4ull * nq + 16; }
+static size_t map_pairs_bytes(long long sum_r) { return 8ull * sum_r; }
+
+// Grows *buf to at least `bytes` (freeing the old one: cudaFree waits for the device)
+static int eval_grow(npair_eval* ev, void** buf, size_t* have, size_t bytes, const char* what) {
+  if (bytes <= *have) return NPAIR_OK;
+  cudaFree(*buf);
+  *buf = nullptr; *have = 0;
+  if (cudaMalloc(buf, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    *buf = nullptr;
+    ev->err = fmt("cannot allocate %zu bytes for the MAP@R %s", bytes, what);
+    return NPAIR_E_CUDA;
+  }
+  *have = bytes;
+  return NPAIR_OK;
+}
 
 extern "C" {
 
@@ -1616,12 +1646,18 @@ size_t npair_eval_workspace_bytes(int32_t max_q, int32_t max_g, int32_t D, int32
   return total;
 }
 
+size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r) {
+  if (nq < 1 || sum_r < 0) return 0;
+  return map_rows_bytes(nq) + map_pairs_bytes(sum_r);
+}
+
 const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
 
 void npair_eval_destroy(npair_eval* ev) {
   if (!ev) return;
   if (ev->device >= 0) cudaSetDevice(ev->device);
   cudaFree(ev->catA); cudaFree(ev->catB); cudaFree(ev->rows); cudaFree(ev->bs); cudaFree(ev->sym_tiles);
+  cudaFree(ev->map_rows); cudaFree(ev->map_pairs);
   delete ev;
 }
 
@@ -1646,7 +1682,8 @@ int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int
   ev->ra.st_minw = w; w += max_q; ev->ra.st_maxw = w; w += max_q; ev->ra.st_maxb = w; w += max_q; ev->ra.st_maxall = w; w += max_q;
   ev->ra.cnt_same = reinterpret_cast<int*>(w); w += max_q;
   ev->absmax_bits = w;
-  const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM};
+  const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
+                      EPI_BUCKET | EPI_SYM};
   for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
   *out = made.release();
   return NPAIR_OK;
@@ -1688,9 +1725,10 @@ static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, 
   return NPAIR_OK;
 }
 
-// One sweep of the similarity GEMM over the prepared operands: EPI_STATS (labels) or EPI_COUNT (cut, count), + EPI_SYM when `sym`
+// One sweep of the similarity GEMM over the prepared operands: EPI_STATS, EPI_GATHER or EPI_BUCKET (labels, and `map` for the MAP@R
+// sweeps) or EPI_COUNT (cut, count), + EPI_SYM when `sym`
 static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, const float* ql, const float* gl, const float* cut, int32_t* count,
-                      bool sym, cudaStream_t st) {
+                      bool sym, cudaStream_t st, const GemmParams* map = nullptr) {
   if (sym) {
     if (ev->sym_n != nq) {
       ev->sym_host = sym_tile_list(nq, nq);
@@ -1701,8 +1739,9 @@ static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, con
   }
   GemmParams gp = sim_sweep(epi, nq, ng, ev->kcat, &ev->bs->x_inv_scale, ev->sym_tiles, static_cast<int>(ev->sym_host.size()), ev->ra);
   gp.self_offset = self_col;
-  if (epi & EPI_STATS) { gp.lab_rows = ql; gp.lab_cols = gl; }
+  if (epi & (EPI_STATS | EPI_GATHER | EPI_BUCKET)) { gp.lab_rows = ql; gp.lab_cols = gl; }
   else { gp.cut = cut; gp.count = count; }
+  if (map) { gp.cnt_same = ev->ra.cnt_same; gp.bs = ev->bs; gp.seg = map->seg; gp.fill = map->fill; gp.pos = map->pos; gp.hist = map->hist; }
   CUtensorMap ta, tb;
   std::string te;
   if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
@@ -1762,6 +1801,58 @@ int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g,
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
   CUDA_TRY(ev, cudaMemsetAsync(d_count, 0, sizeof(int32_t) * nq, st));
   if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, d_cut, d_count, sym, st)) != NPAIR_OK) return rc;
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+// MAP@R in three sweeps over the same prepared operands and tile geometry (DESIGN 8): the statistics sweep gives R_i, EPI_GATHER
+// collects every query's positives into its segment, a sort orders each segment, and EPI_BUCKET places every negative that reaches the
+// query's smallest positive among them.  The gather writes its unordered positives into the histogram words, which the sort reads and
+// which are then cleared for the bucket sweep: 8 bytes per positive pair in all.
+int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng,
+                        int32_t self_offset, double* d_map_r, double* d_r_precision, int32_t* d_R, int32_t* d_rank, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
+  if (rc != NPAIR_OK) return rc;
+  if (!ql || !gl || !d_map_r || !d_r_precision) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(ev, cudaSetDevice(ev->device));
+  const int self_col = eval_self_col(self_offset, 0);
+  const bool sym = eval_sym(q, nq, g, ng, self_col);
+  if ((rc = eval_grow(ev, &ev->map_rows, &ev->map_rows_bytes, map_rows_bytes(nq), "per-query offsets")) != NPAIR_OK) return rc;
+  long long* seg = static_cast<long long*>(ev->map_rows);                          // [nq + 1]
+  unsigned long long* sum_err = reinterpret_cast<unsigned long long*>(seg + nq + 1);  // {sum R_i, error bits}
+  int* fill = reinterpret_cast<int*>(sum_err + 2);                                    // [nq]
+  const int* R = ev->ra.cnt_same;
+  // sweep 1: R_i, and the one host synchronisation, for sum R_i
+  if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
+  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
+  launch_eval_seg_scan(R, nq, seg, ev->bs, sum_err, st);
+  unsigned long long h[2] = {0, 0};
+  CUDA_TRY(ev, cudaMemcpyAsync(h, sum_err, sizeof(h), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ev, cudaStreamSynchronize(st));
+  if (h[1] & DERR_GATHER_SLOT) {
+    ev->err = "an earlier npair_eval_map_at_r on this evaluator gathered more positives for a query than its statistics sweep counted "
+              "(that query's results were NaN)";
+    return NPAIR_E_CUDA;
+  }
+  const long long sum_r = static_cast<long long>(h[0]);
+  if ((rc = eval_grow(ev, &ev->map_pairs, &ev->map_pairs_bytes, map_pairs_bytes(sum_r), "positive pairs")) != NPAIR_OK) return rc;
+  float* pos = static_cast<float*>(ev->map_pairs);
+  unsigned int* hist = reinterpret_cast<unsigned int*>(pos + sum_r);
+  CUDA_TRY(ev, cudaMemsetAsync(fill, 0, sizeof(int) * nq, st));
+  if (sum_r > 0) {
+    GemmParams mp{};
+    // sweep 2: the positives, unordered, into the histogram words; then sorted into pos
+    mp.seg = seg; mp.fill = fill; mp.pos = reinterpret_cast<float*>(hist);
+    if ((rc = eval_sweep(ev, EPI_GATHER, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
+    launch_eval_seg_sort(R, seg, nq, reinterpret_cast<const float*>(hist), pos, st);
+    CUDA_TRY(ev, cudaMemsetAsync(hist, 0, sizeof(unsigned int) * sum_r, st));
+    // sweep 3: the buckets
+    mp.pos = pos; mp.hist = hist;
+    if ((rc = eval_sweep(ev, EPI_BUCKET, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
+  }
+  launch_eval_map_finish(R, seg, fill, pos, hist, nq, d_map_r, d_r_precision, d_R, d_rank, st);
   CUDA_TRY(ev, cudaGetLastError());
   return NPAIR_OK;
 }

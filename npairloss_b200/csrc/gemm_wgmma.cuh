@@ -38,7 +38,11 @@ namespace npair {
 // EPI_COUNT   : retrieval evaluation, not the layer (DESIGN 8).  Per row, the number of valid non-self columns with s >= cut[row]
 //               (a cut of -inf or NaN counts nothing), one atomicAdd per row and tile into count[row]; with EPI_SYM a mirrored block
 //               also counts, for each column gc, its entries against cut[gc].  Used without EPI_STATS and EPI_STORE_S.
-enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64 };
+// EPI_GATHER  : MAP@R evaluation (DESIGN 8).  Every positive pair of row i (the predicate of cnt_same) is written to row i's segment
+//               of `pos`, in atomic order; with EPI_SYM a mirrored block gathers for each column gc.  Used alone (+ EPI_SYM).
+// EPI_BUCKET  : MAP@R evaluation.  For every negative pair s of row i with s >= the row's smallest positive, hist[seg[i] + b] += 1 with
+//               b = #{k : p_k > s} over the row's positives sorted descending; with EPI_SYM also for each mirrored column gc.
+enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64, EPI_GATHER = 128, EPI_BUCKET = 256 };
 
 // Persistent tile schedule of both wgmma GEMMs (host: tile_sched, ctx.cu).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
 // output tile (m_blk, n_blk) or tile_list[t], K blocks [kb0, kb1) of split-K slice `split`.  split moves fastest, then n_blk, m_blk.
@@ -92,6 +96,11 @@ struct GemmParams {
   // ---- EPI_COUNT (self_offset as for EPI_STATS) ----
   const float* cut;    // [M] per-row cut
   int* count;          // [M] counts, pre-initialised
+  // ---- EPI_GATHER / EPI_BUCKET (labels and self_offset as for EPI_STATS; cnt_same = R_i, read only; bs->err for the slot guard) ----
+  const long long* seg;    // [M] first slot of row i's segment in pos / hist: the exclusive scan of cnt_same
+  int* fill;               // [M] EPI_GATHER: positives claimed so far, pre-zeroed
+  float* pos;              // EPI_GATHER: row i's positives, unordered; EPI_BUCKET: the same sorted descending
+  unsigned int* hist;      // EPI_BUCKET: per-row bucket counts, pre-zeroed
 };
 
 // BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
@@ -152,6 +161,12 @@ __device__ __forceinline__ void pass_pieces(int nsplit, int p, int& sa, int& sb)
   sa = A[p]; sb = B[p];
 }
 
+// The pair predicate of every similarity epilogue that looks at labels: column idx of a row is a pair iff it lies inside the gallery
+// and is not the row's own column (fast: the caller knows this holds for the whole chunk), and a pair is a positive iff the labels
+// compare equal as floats.  stats32's cnt_same and EPI_GATHER's hits both use it, so they cannot disagree.
+__device__ __forceinline__ bool pair_valid(bool fast, int idx, int limit, int self_idx) { return fast || (idx < limit && idx != self_idx); }
+__device__ __forceinline__ bool same_label(float lab_c, float lab_i) { return lab_c == lab_i; }
+
 // Per-thread statistics of 32 consecutive similarities against 32 labels staged in shared memory.
 // fast: no bounds / self-pair checks, branch-free (predicated).  Otherwise entry c is valid iff idx0 + c < limit and
 // idx0 + c != self_idx.
@@ -170,6 +185,7 @@ __device__ __forceinline__ void stats32(const float (&v)[32], const float* __res
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const float x = v[4 * q + e];
+        // same_label written out: the call compiles this loop to other (equivalent) machine code
         if (ll[e] == lab_i) { mnw[e] = fminf(mnw[e], x); mxw[e] = fmaxf(mxw[e], x); ++cn[e]; }
         else mxb[e] = fmaxf(mxb[e], x);
       }
@@ -181,9 +197,8 @@ __device__ __forceinline__ void stats32(const float (&v)[32], const float* __res
   } else {
 #pragma unroll
     for (int c = 0; c < 32; ++c) {
-      const int idx = idx0 + c;
-      const bool valid = (idx < limit) && (idx != self_idx);
-      const bool same = (lab[c] == lab_i);
+      const bool valid = pair_valid(false, idx0 + c, limit, self_idx);
+      const bool same = same_label(lab[c], lab_i);
       if (valid && same) { minw = fminf(minw, v[c]); maxw = fmaxf(maxw, v[c]); ++cnt; }
       if (valid && !same) maxb = fmaxf(maxb, v[c]);
     }
@@ -215,6 +230,62 @@ __device__ __forceinline__ int count32(const float (&v)[32], float cut, bool fas
 // A row without a best positive has cut -inf and must count nothing: NaN compares false with everything
 __device__ __forceinline__ float count_cut(float c) { return c == -INFINITY ? __int_as_float(0x7fffffff) : c; }
 
+// EPI_GATHER: bit c set iff entry c of 32 consecutive columns is a positive pair of the row (pair_valid && same_label)
+__device__ __forceinline__ uint32_t positives32(const float* __restrict__ lab, float lab_i, bool fast, int idx0, int limit, int self_idx) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) m |= (pair_valid(fast, idx0 + c, limit, self_idx) && same_label(lab[c], lab_i)) ? 1u << c : 0u;
+  return m;
+}
+// EPI_GATHER: appends the entries `hits` of a chunk (value of entry c: val(c)) to the row's segment [seg, seg + R) of pos.  One atomic
+// claims the slots; a slot past R_i (cnt_same and the gather disagree) is not written but flagged in *err.
+template <class Val>
+__device__ __forceinline__ void gather_hits(uint32_t hits, Val val, int* fill, long long seg, int R, float* pos, int* err) {
+  if (!hits) return;
+  int slot = atomicAdd(fill, __popc(hits));
+  for (; hits; hits &= hits - 1, ++slot) {
+    const float s = val(__ffs(hits) - 1);
+    if (slot < R) pos[seg + slot] = s;
+    else atomicOr(err, DERR_GATHER_SLOT);
+  }
+}
+// EPI_BUCKET: bit c of the result set iff entry c is a negative pair of the row with s >= cut (the row's smallest positive p_R, NaN for
+// a row without positives); bit c of *above also iff s >= p1 (the row's largest positive), where b = 0 needs no search
+__device__ __forceinline__ uint32_t negatives32(const float (&v)[32], float cut, float p1, const float* __restrict__ lab, float lab_i, bool fast,
+                                                int idx0, int limit, int self_idx, uint32_t* above) {
+  uint32_t m = 0, a = 0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) {
+    const bool neg = v[c] >= cut && pair_valid(fast, idx0 + c, limit, self_idx) && !same_label(lab[c], lab_i);
+    m |= neg ? 1u << c : 0u;
+    a |= (neg && v[c] >= p1) ? 1u << c : 0u;
+  }
+  *above = a;
+  return m;
+}
+// EPI_BUCKET: entries `cand` with p_R <= s < p_1 of a row whose R >= 2 positives p[0..R) are sorted descending: b = #{k : p_k > s} by a
+// binary search over [1, R - 1] (p[0] > s >= p[R - 1]), one atomic per run of equal buckets
+template <class Val>
+__device__ __forceinline__ void bucket_search(uint32_t cand, Val val, const float* __restrict__ p, int R, unsigned int* hist) {
+  int run_b = -1;
+  unsigned int run = 0;
+  for (; cand; cand &= cand - 1) {
+    const float s = val(__ffs(cand) - 1);
+    int lo = 1, hi = R - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (p[mid] > s) lo = mid + 1;
+      else hi = mid;
+    }
+    if (lo != run_b) {
+      if (run) atomicAdd(&hist[run_b], run);
+      run_b = lo; run = 0;
+    }
+    ++run;
+  }
+  if (run) atomicAdd(&hist[run_b], run);
+}
+
 template <int NSPLIT, bool BF16, int EPI, int BK_>
 __global__ void __launch_bounds__(384, 1)
 split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
@@ -223,6 +294,8 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
   constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS, COUNT = EPI & EPI_COUNT;
+  constexpr bool GATHER = EPI & EPI_GATHER, BUCKET = EPI & EPI_BUCKET;
+  constexpr bool LABELS = STATS || GATHER || BUCKET;              // the epilogue needs the tile's labels
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer in the shared address space (offset arithmetic, no integer round trip): LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -290,7 +363,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       const int row = t.m_blk * BM + ew * 32 + lane;
       const int col_base = t.n_blk * BN;
       float lab_i = 0.f;
-      if (STATS) {
+      if (LABELS) {
         asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers are done with s_lab
         s_lab[et] = (col_base + et < p.Nn) ? p.lab_cols[col_base + et] : 0.f;
         if (row < p.M) lab_i = p.lab_rows[row];
@@ -382,6 +455,18 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       float cut_i = 0.f;
       int cnt_ge = 0;
       if (COUNT && row < p.M) cut_i = count_cut(p.cut[row]);
+      // EPI_GATHER / EPI_BUCKET: the row's segment and R_i; EPI_BUCKET: its largest and smallest positive (NaN bounds for a row without
+      // positives, which no similarity reaches), and the count of its b = 0 negatives over the tile
+      long long seg_i = 0;
+      int R_i = 0, above_i = 0;
+      float p1_i = 0.f, pR_i = 0.f;
+      if constexpr (GATHER || BUCKET) {
+        if (row < p.M) { seg_i = p.seg[row]; R_i = p.cnt_same[row]; }
+      }
+      if constexpr (BUCKET) {
+        p1_i = count_cut(R_i ? p.pos[seg_i] : -INFINITY);
+        pR_i = count_cut(R_i ? p.pos[seg_i + R_i - 1] : -INFINITY);
+      }
 #pragma unroll
       for (int cp = 0; cp < 4; ++cp) {
         asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");   // the warpgroup's previous reads of the staging tile are done
@@ -405,7 +490,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         // lower-triangle half of a straddling tile: produced by mirroring
         if ((SYM && cb < t.m_blk) || col0 >= p.Nn) continue;
         float v[32];
-        if (STATS || COUNT) {
+        if (STATS || COUNT || GATHER || BUCKET) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
@@ -438,6 +523,28 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         if (COUNT && row < p.M)
           cnt_ge += count32(v, cut_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col);
+        if constexpr (GATHER || BUCKET) {
+          const bool fast = col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32);
+          // entry c of this thread's chunk, bit for bit the v[c] above, read back from the staging tile by a runtime index
+          const auto staged = [&](int c) {
+            return *reinterpret_cast<const float*>(accs + srow * 256 + (((half * 8 + (c >> 2)) ^ (srow & 7)) << 4) + (c & 3) * 4) * out_scale;
+          };
+          if constexpr (GATHER) {
+            // the warp-uniform label-range skip of EPI_STATS: a chunk without a same-label column for any row of the warp
+            const float2 rg = s_rng[ch];
+            const bool none = __all_sync(0xffffffffu, row >= p.M || lab_i < rg.x || lab_i > rg.y) && col0 + 32 <= p.Nn;
+            if (!none && row < p.M)
+              gather_hits(positives32(s_lab + ch * 32, lab_i, fast, col0, p.Nn, self_col), staged, &p.fill[row], seg_i, R_i, p.pos, &p.bs->err);
+          }
+          if constexpr (BUCKET) {
+            if (row < p.M && max32(v) >= pR_i) {
+              uint32_t above;
+              const uint32_t neg = negatives32(v, pR_i, p1_i, s_lab + ch * 32, lab_i, fast, col0, p.Nn, self_col, &above);
+              above_i += __popc(above);
+              bucket_search(neg & ~above, staged, p.pos + seg_i, R_i, p.hist + seg_i);
+            }
+          }
+        }
         if (SYM && cb > t.m_blk && t.m_blk * BM + ew * 32 < p.M) {
           // ---- mirrored store: staging row c holds S[col0 + c][rows of this warp]; box lands at (x = row block, y = col0) ----
           if (STORE && lane == 0) ptx::tma_store_wait_read<0>();   // this warp's previous box has been read out of smem
@@ -479,9 +586,36 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             const int t_ge = count32(vt, count_cut(p.cut[gc]), r0 + 32 <= p.M, r0, p.M, -1);
             if (t_ge) atomicAdd(&p.count[gc], t_ge);
           }
+          // mirrored gather and buckets for row gc, against this warp's rows (none of them gc's self pair), as the statistics above
+          if constexpr (GATHER || BUCKET) {
+            const auto staged_t = [stg, lane](int c) {
+              return *reinterpret_cast<const float*>(stg + lane * 128 + (((c >> 2) ^ (lane & 7)) << 4) + (c & 3) * 4);
+            };
+            if constexpr (GATHER) {
+              if (!plain && gc < p.Nn)
+                gather_hits(positives32(s_labr + ew * 32, lab_c, r0 + 32 <= p.M, r0, p.M, -1), staged_t, &p.fill[gc], p.seg[gc],
+                            p.cnt_same[gc], p.pos, &p.bs->err);
+            }
+            if constexpr (BUCKET) {
+              const int R_g = gc < p.Nn ? p.cnt_same[gc] : 0;
+              if (R_g) {
+                const long long seg_g = p.seg[gc];
+                const float p1 = p.pos[seg_g], pR = p.pos[seg_g + R_g - 1];
+                if (max32(vt) >= pR) {
+                  uint32_t above;
+                  const uint32_t neg = negatives32(vt, pR, p1, s_labr + ew * 32, lab_c, r0 + 32 <= p.M, r0, p.M, -1, &above);
+                  if (above) atomicAdd(&p.hist[seg_g], static_cast<unsigned int>(__popc(above)));
+                  bucket_search(neg & ~above, staged_t, p.pos + seg_g, R_g, p.hist + seg_g);
+                }
+              }
+            }
+          }
         }
       }
       if (COUNT && row < p.M && cnt_ge) atomicAdd(&p.count[row], cnt_ge);
+      if constexpr (BUCKET) {
+        if (above_i) atomicAdd(&p.hist[seg_i], static_cast<unsigned int>(above_i));
+      }
       if (STATS && row < p.M) {
         maxall = fmaxf(maxw, maxb);                       // every valid column is either same- or diff-label
         if (cnt) {

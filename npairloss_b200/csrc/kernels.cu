@@ -1844,4 +1844,116 @@ void launch_eval_best(RowArrays ra, int nq, float* best, cudaStream_t st) {
   count_launch();
 }
 
+// MAP@R: 64-bit segment offsets of the queries' positives, by one block.  Thread t sums a contiguous run of counts, the block scans
+// the runs, and each thread writes its run's offsets.
+__global__ void __launch_bounds__(1024) eval_seg_scan_kernel(const int* __restrict__ cnt, int nq, long long* __restrict__ seg, BlockScalars* bs,
+                                                             unsigned long long* __restrict__ sum_err) {
+  __shared__ long long s_warp[32];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int per = (nq + 1023) / 1024, i0 = min(nq, t * per), i1 = min(nq, i0 + per);
+  long long run = 0;
+  for (int i = i0; i < i1; ++i) run += cnt[i];
+  long long incl = run;                                      // inclusive scan: across the warp, then across the warps
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) s_warp[w] = incl;
+  __syncthreads();
+  if (w == 0) {
+    long long x = s_warp[lane], xi = x;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, xi, o);
+      if (lane >= o) xi += y;
+    }
+    s_warp[lane] = xi - x;                                   // exclusive prefix of each warp
+  }
+  __syncthreads();
+  long long off = s_warp[w] + incl - run;
+  for (int i = i0; i < i1; ++i) { seg[i] = off; off += cnt[i]; }
+  if (t == 1023) {
+    seg[nq] = off;
+    sum_err[0] = static_cast<unsigned long long>(off);
+    sum_err[1] = static_cast<unsigned long long>(bs->err);
+    bs->err = 0;
+  }
+}
+void launch_eval_seg_scan(const int* cnt, int nq, long long* seg, BlockScalars* bs, unsigned long long* sum_err, cudaStream_t st) {
+  eval_seg_scan_kernel<<<1, 1024, 0, st>>>(cnt, nq, seg, bs, sum_err);
+  count_launch();
+}
+
+// One warp per query: the rank of each positive in its segment is the number of larger keys plus the number of equal keys before it,
+// so every key lands on its own slot.  O(R_i^2 / 32) per query; the segments of metric-learning sets are short.
+__global__ void __launch_bounds__(256) eval_seg_sort_kernel(const int* __restrict__ cnt, const long long* __restrict__ seg, int nq,
+                                                            const float* __restrict__ src, float* __restrict__ dst) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= nq) return;
+  const int R = cnt[i];
+  const float* s = src + seg[i];
+  float* d = dst + seg[i];
+  for (int a = 0; a < R; a += 32) {
+    const int k = a + lane;
+    const uint32_t mine = k < R ? f2ord(s[k]) : 0u;
+    int r = 0;
+    for (int b = 0; b < R; b += 32) {
+      const uint32_t other = b + lane < R ? f2ord(s[b + lane]) : 0u;
+      const int n = min(32, R - b);
+      for (int j = 0; j < n; ++j) {
+        const uint32_t o = __shfl_sync(0xffffffffu, other, j);
+        r += (o > mine || (o == mine && b + j < k)) ? 1 : 0;
+      }
+    }
+    if (k < R) d[r] = ord2f(mine);
+  }
+}
+void launch_eval_seg_sort(const int* cnt, const long long* seg, int nq, const float* src, float* dst, cudaStream_t st) {
+  eval_seg_sort_kernel<<<(nq + 7) / 8, 256, 0, st>>>(cnt, seg, nq, src, dst);
+  count_launch();
+}
+
+// One thread per query, k = 1..R ascending: neg_ge(k) = sum of hist[b < k], pos_k = k + neg_ge(k).  fp64, summed in ascending k and
+// divided by R last, so a host loop in the same order gives the same bits.  rank = c_1 + neg_ge(1), c_1 = #{k : p_k = p_1}: the rank
+// of npair_eval_rank.
+__global__ void __launch_bounds__(256) eval_map_finish_kernel(const int* __restrict__ cnt, const long long* __restrict__ seg,
+                                                              const int* __restrict__ fill, const float* __restrict__ pos,
+                                                              const unsigned int* __restrict__ hist, int nq, double* __restrict__ map_r,
+                                                              double* __restrict__ r_precision, int* __restrict__ R_out, int* __restrict__ rank) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nq) return;
+  const int R = cnt[i];
+  double m = __longlong_as_double(0x7ff8000000000000ll), rp = m;
+  int rk = 0;
+  if (R > 0 && fill[i] == R) {
+    const float* p = pos + seg[i];
+    const unsigned int* h = hist + seg[i];
+    int c1 = 1;
+    while (c1 < R && p[c1] == p[0]) ++c1;
+    rk = c1 + static_cast<int>(h[0]);
+    double sum = 0.0;
+    long long neg_ge = 0;
+    int hits = 0;
+    for (int k = 1; k <= R; ++k) {
+      neg_ge += h[k - 1];
+      const long long pk = k + neg_ge;
+      if (pk > R) break;                                     // pos_k only grows with k
+      sum += static_cast<double>(k) / static_cast<double>(pk);
+      ++hits;
+    }
+    m = sum / R;
+    rp = static_cast<double>(hits) / R;
+  }
+  map_r[i] = m;
+  r_precision[i] = rp;
+  if (R_out) R_out[i] = R;
+  if (rank) rank[i] = rk;
+}
+void launch_eval_map_finish(const int* cnt, const long long* seg, const int* fill, const float* pos, const unsigned int* hist, int nq,
+                            double* map_r, double* r_precision, int* R_out, int* rank, cudaStream_t st) {
+  eval_map_finish_kernel<<<(nq + 255) / 256, 256, 0, st>>>(cnt, seg, fill, pos, hist, nq, map_r, r_precision, R_out, rank);
+  count_launch();
+}
+
 }  // namespace npair

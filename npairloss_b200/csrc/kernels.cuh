@@ -14,6 +14,8 @@ enum { M_HARD = 0, M_EASY = 1, M_RAND = 2, M_RELATIVE_HARD = 3, M_RELATIVE_EASY 
 
 // device error bits (the reference has undefined behaviour in these cases: SURVEY.md 9.4 Q5)
 enum { DERR_EMPTY_LIST = 1, DERR_POS_RANGE = 2 };
+// retrieval evaluation: the MAP@R gather found more positives in a row than the statistics sweep counted
+enum { DERR_GATHER_SLOT = 4 };
 
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -215,5 +217,14 @@ void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, 
                        BlockScalars* bs, uint16_t* out, cudaStream_t st);
 // best[i] = max same-label non-self similarity of query i, -inf when there is none
 void launch_eval_best(RowArrays ra, int nq, float* best, cudaStream_t st);
+// MAP@R (npair_eval_map_at_r).  seg[0..nq] = exclusive scan of R_i = cnt[i] (seg[nq] = sum R_i), and sum_err = {sum R_i, the error
+// bits of bs}, whose bits it then clears
+void launch_eval_seg_scan(const int* cnt, int nq, long long* seg, BlockScalars* bs, unsigned long long* sum_err, cudaStream_t st);
+// dst = each query's segment of src sorted descending (ordered-uint keys, so the order is a total one and does not depend on src's)
+void launch_eval_seg_sort(const int* cnt, const long long* seg, int nq, const float* src, float* dst, cudaStream_t st);
+// MAP@R_i, R-Precision_i (NaN for R_i = 0 or a row whose gather count `fill` differs from R_i), optionally R_i and the best
+// positive's rank, from the sorted positives and the bucket counts
+void launch_eval_map_finish(const int* cnt, const long long* seg, const int* fill, const float* pos, const unsigned int* hist, int nq,
+                            double* map_r, double* r_precision, int* R_out, int* rank, cudaStream_t st);
 
 }  // namespace npair

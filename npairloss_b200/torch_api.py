@@ -95,8 +95,51 @@ def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), preci
     `self_offset` = k, queries that are gallery rows k, k+1, ...  Takes CUDA fp32 embeddings as given (L2-normalise them first for
     cosine similarity); labels of any numeric dtype.  Returns ({K: recall}, rank) with rank the int32 CUDA tensor of the best
     positive's rank per query (0: the query has no positive)."""
+    q, ql, g, gl, off = _retrieval_sets("recall_at_k", query, qlabel, gallery, glabel, self_offset)
+    ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
+    try:
+        rank = ev.rank(q, ql, g, gl, off)
+        hits = {int(k): ((rank >= 1) & (rank <= int(k))).sum() for k in ks}
+        nq = q.shape[0]
+        return {k: int(v) / nq for k, v in hits.items()}, rank
+    finally:
+        ev.close()
+
+
+def retrieval_metrics(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), precision=capi.PREC_FP32_FP16X2, self_offset=None):
+    """MAP@R, R-Precision and Recall@K of a whole embedding set in one evaluator call (DESIGN 8; not part of the reference layer).
+
+    Sets, labels and ties as in recall_at_k.  Query i has R_i positives (gallery rows of its label, itself excluded); MAP@R_i and
+    R-Precision_i look at where each of them lands among its R_i nearest gallery rows, a negative that ties a positive placed before it.
+    Returns ({"map@r": mean MAP@R, "r_precision": mean R-Precision, "recall@K": Recall@K for each K in ks, "no_positive": n},
+    per_query) with per_query the CUDA tensors "map_r" and "r_precision" (fp64, NaN where R_i = 0), "R" and "rank" (int32, rank as in
+    recall_at_k).
+
+    The MAP@R and R-Precision means are taken over the queries with R_i >= 1 only, and "no_positive" is the number of queries left out
+    (NaN means when every query is).  recall_at_k and "recall@K" instead count a query without a positive as a miss, over all nq."""
+    q, ql, g, gl, off = _retrieval_sets("retrieval_metrics", query, qlabel, gallery, glabel, self_offset)
+    ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
+    try:
+        per_query = ev.map_at_r(q, ql, g, gl, off)
+    finally:
+        ev.close()
+    nq, R, rank = q.shape[0], per_query["R"], per_query["rank"]
+    has = R > 0
+    n_has = int(has.sum())
+    nan = float("nan")
+    out = {"map@r": float(per_query["map_r"][has].mean()) if n_has else nan,
+           "r_precision": float(per_query["r_precision"][has].mean()) if n_has else nan}
+    for k in ks:
+        out[f"recall@{int(k)}"] = int(((rank >= 1) & (rank <= int(k))).sum()) / nq
+    out["no_positive"] = nq - n_has
+    return out, per_query
+
+
+def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
+    """(query, query labels, gallery, gallery labels, self_offset) as the evaluator takes them: contiguous 2-D CUDA fp32 rows, fp32
+    labels; gallery=None is self-retrieval."""
     if not query.is_cuda or query.dtype != torch.float32:
-        raise TypeError("recall_at_k takes CUDA float32 embeddings (there is no CPU path)")
+        raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
     q = query.reshape(query.shape[0], -1).contiguous()
     ql = qlabel.to(device=q.device, dtype=torch.float32).contiguous()
     if gallery is None:
@@ -107,17 +150,10 @@ def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), preci
         if glabel is None:
             raise ValueError("gallery without glabel")
         if not gallery.is_cuda or gallery.dtype != torch.float32:
-            raise TypeError("recall_at_k takes CUDA float32 embeddings (there is no CPU path)")
+            raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
         g = gallery.reshape(gallery.shape[0], -1).contiguous()
         gl = glabel.to(device=q.device, dtype=torch.float32).contiguous()
         off = -1 if self_offset is None else self_offset
     if g.shape[1] != q.shape[1]:
         raise ValueError("query and gallery dimensions differ")
-    ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
-    try:
-        rank = ev.rank(q, ql, g, gl, off)
-        hits = {int(k): ((rank >= 1) & (rank <= int(k))).sum() for k in ks}
-        nq = q.shape[0]
-        return {k: int(v) / nq for k, v in hits.items()}, rank
-    finally:
-        ev.close()
+    return q, ql, g, gl, off

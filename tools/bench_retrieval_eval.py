@@ -7,14 +7,19 @@ Shapes: "sop" = self-retrieval over 60502 x 512 (Stanford Online Products' test 
 gallery of 12612, D = 512 (In-Shop).  Inputs are random unit vectors with about 5 rows per label, made on the device from a fixed seed.
 For every shape and format: --warmup untimed calls, then --repeats timed rounds of each of the three calls with CUDA events (L2 not
 flushed): phase 1 alone (operand preparation + the best-positive sweep), phase 2 alone (operand preparation + the count sweep) and
-the one-call rank.  Prints one JSON line per (shape, format) with median milliseconds, the algorithmic rate 2 * nq * ng * D per sweep
-over the phase times, and the card's name, power limit and median SM clock sampled during the timed rounds.  Writes nothing.
+the one-call rank, and the one-call MAP@R (`map_at_r`: operand preparation + three sweeps + sort + finish).  A separate, untimed
+torch.profiler run of one map_at_r call gives the device time of each of its three sweeps (statistics, gather, bucket) and of its other
+kernels, and a fp32 torch matmul over --sample queries gives the fraction of the entries that take the bucket sweep's search path
+(p_R <= s < p_1 for a negative s).  Prints one JSON line per (shape, format) with median milliseconds, the algorithmic rate
+2 * nq * ng * D per sweep over the phase times, and the card's name, power limit and median SM clock sampled during the timed rounds.
+Writes nothing.
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
+import re
 import statistics
 import subprocess
 import sys
@@ -67,12 +72,52 @@ class ClockSampler:
         return statistics.median(self.samples) if self.samples else None
 
 
+def sweep_times(f):
+    """Device milliseconds of each similarity sweep of one call of f (by epilogue) and of everything else, from torch.profiler."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    names = {16: "stats", 128: "gather", 256: "bucket", 64: "count"}
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        f()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        m = re.search(r"split_gemm_kernel<\d+, \w+, (\d+), \d+>", e.key)
+        if m:
+            key = names.get(int(m.group(1)) & ~32, "other_gemm")
+        elif "npair::" in e.key:
+            key = "other_kernels"
+        elif e.key.startswith("Memset"):
+            key = "memset"
+        else:
+            continue
+        out[key] = out.get(key, 0.0) + e.self_device_time_total / 1e3
+    return {k: round(v, 4) for k, v in out.items()}
+
+
+def search_fraction(q, ql, g, gl, off, sample):
+    """Share of the valid (query, gallery) entries of `sample` queries that are negatives with p_R <= s < p_1 (fp32 torch matmul)."""
+    import torch
+    idx = torch.linspace(0, q.shape[0] - 1, min(sample, q.shape[0]), device=q.device).long()
+    S = q[idx] @ g.T
+    same = ql[idx, None] == gl[None, :]
+    valid = torch.ones_like(same)
+    if off >= 0:
+        valid[torch.arange(len(idx), device=q.device), off + idx] = False
+    p1 = torch.where(same & valid, S, torch.full_like(S, -float("inf"))).max(1).values
+    pR = torch.where(same & valid, S, torch.full_like(S, float("inf"))).min(1).values
+    neg = ~same & valid
+    srch = neg & (S >= pR[:, None]) & (S < p1[:, None])
+    return float(srch.sum()) / float(valid.sum())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", nargs="+", default=["sop", "inshop"], choices=sorted(SHAPES))
     ap.add_argument("--precisions", nargs="+", default=["fp16x2", "bf16x3"], choices=sorted(PRECS))
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--sample", type=int, default=2048, help="queries sampled for the search-path fraction")
     args = ap.parse_args()
 
     import torch
@@ -100,7 +145,8 @@ def main():
             cut = ev.best_positive(q, ql, g, gl, absmax, off, 0)
             calls = {"best_positive": lambda: ev.best_positive(q, ql, g, gl, absmax, off, 0),
                      "count": lambda: ev.count(q, g, cut, absmax, off, 0),
-                     "rank": lambda: ev.rank(q, ql, g, gl, off)}
+                     "rank": lambda: ev.rank(q, ql, g, gl, off),
+                     "map_at_r": lambda: ev.map_at_r(q, ql, g, gl, off)}
             for _ in range(args.warmup):
                 for f in calls.values():
                     f()
@@ -117,7 +163,13 @@ def main():
                         ms[k].append(e0.elapsed_time(e1))
             rank = ev.rank(q, ql, g, gl, off)
             r1 = float(((rank >= 1) & (rank <= 1)).float().mean())
+            mp = ev.map_at_r(q, ql, g, gl, off)
+            has = mp["R"] > 0
+            map_r = float(mp["map_r"][has].mean())
+            sum_r = int(mp["R"].long().sum())
+            sweeps = sweep_times(lambda: ev.map_at_r(q, ql, g, gl, off))
             ev.close()
+            frac = search_fraction(q, ql, g, gl, off, args.sample)
             flop = 2.0 * nq * ng * D
             med = {k: statistics.median(v) for k, v in ms.items()}
             print(json.dumps({"shape": shape, "nq": nq, "ng": ng, "D": D, "precision": pname,
@@ -125,7 +177,9 @@ def main():
                               "ms_median": {k: round(v, 4) for k, v in med.items()},
                               "ms_all": {k: [round(x, 4) for x in v] for k, v in ms.items()},
                               "algorithmic_tflops_per_sweep": {k: round(flop / (med[k] * 1e-3) / 1e12, 1) for k in ("best_positive", "count")},
-                              "recall_at_1": round(r1, 5),
+                              "recall_at_1": round(r1, 5), "map_at_r": round(map_r, 5),
+                              "map_at_r_device_ms_by_kernel": sweeps, "search_path_fraction_sampled": round(frac, 5),
+                              "map_at_r_extra_bytes": capi.eval_map_at_r_bytes(nq, sum_r),
                               "workspace_bytes": capi.eval_workspace_bytes(nq, ng, D, PRECS[pname]),
                               "card": name, "sm_clock_mhz_median": clk.median()}), flush=True)
 
