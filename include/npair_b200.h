@@ -273,6 +273,29 @@ int npair_eval_map_at_r(npair_eval* ev, const float* d_query, const float* d_qla
 /* Device memory npair_eval_map_at_r adds on top of the workspace for nq queries with sum_r = sum R_i positive pairs:
  * 12 bytes per query, 8 bytes per positive pair and 24 bytes.  0 for nq < 1 or sum_r < 0. */
 size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r);
+/* Lloyd's k-means of n points (rows of d_x, n x D fp32) into k clusters, on the evaluator's operands: the points take the query side
+ * (n <= max_queries), the centroids the gallery side (k <= max_gallery), 1 <= k <= n.  init_rows_host: k HOST row indices in [0, n)
+ * (duplicates allowed); centroid c starts as row init_rows_host[c].  max_iter >= 1 is the maximum number of assignment sweeps.
+ * Writes d_assign[n] (int32), d_centroids[k x D] (the centroids that d_assign was computed against), *d_inertia (fp64, may be NULL),
+ * and stats_host[3] = {assignment sweeps run, assignments changed by the last sweep (n for the first), empty clusters}.
+ * Synchronises with the host once per iteration; everything else is asynchronous on `stream`.
+ * Iteration t (DESIGN 8.2):
+ *   1. the centroids C_t are split into the B format;
+ *   2. a_i = argmax_c ( s_ic - 0.5 ||mu_c||^2 ), s_ic the library's similarity in `precision`, ties to the LOWEST c; the bias is
+ *      computed in fp32 from the fp32 centroid;
+ *   3. stop if t > 0 and no assignment changed, or if t + 1 = max_iter;
+ *   4. else C_{t+1} = the members' means by the fixed-point rule below; an EMPTY cluster keeps its centroid.
+ * sigma = the pre-scale of max|x| over the points (a power of two with max|x * sigma| in [0.5, 1)), in every format.  Each member adds
+ * q_id = rint(x_id * sigma * 2^32) to the int64 sum S_c[d] (64-bit integer atomics: exact, and independent of their order), and
+ * mu_c[d] = (float)( ldexp((double)S_c[d] / count_c, -32) * (1 / sigma) ).  Inertia = sum_i ||x_i - mu_{a_i}||^2 in fp64 from the fp32
+ * values, in a fixed order.  Every output has the same bits on every call and on a fresh evaluator.
+ * NPAIR_E_ARG (checked on the host) for a capacity, k > n, init row, max_iter < 1 or null pointer error; NPAIR_E_CUDA when a point
+ * finds no centroid with a finite score (NaN or infinite input). */
+int npair_eval_kmeans(npair_eval* ev, const float* d_x, int32_t n, int32_t k, const int32_t* init_rows_host, int32_t max_iter,
+                      float* d_centroids, int32_t* d_assign, double* d_inertia, int32_t stats_host[3], void* stream);
+/* Device memory npair_eval_kmeans adds on top of the workspace (grown on demand, kept until npair_eval_destroy): 8 * k * D + 8 * n +
+ * 12 * k + 2064 bytes.  0 for bad arguments (n, k or D < 1, k > n). */
+size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D);
 
 #ifdef __cplusplus
 }

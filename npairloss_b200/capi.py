@@ -44,7 +44,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
-           "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes"]
+           "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
+           "npair_eval_kmeans", "npair_eval_kmeans_bytes"]
 
 _LIB = None
 
@@ -109,6 +110,9 @@ def lib():
         L.npair_eval_map_at_r.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp]
         L.npair_eval_map_at_r_bytes.argtypes = [i32, C.c_int64]
         L.npair_eval_map_at_r_bytes.restype = C.c_size_t
+        L.npair_eval_kmeans.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, vp]
+        L.npair_eval_kmeans_bytes.argtypes = [i32, i32, i32]
+        L.npair_eval_kmeans_bytes.restype = C.c_size_t
         _LIB = L
     return _LIB
 
@@ -244,6 +248,11 @@ def eval_map_at_r_bytes(nq: int, sum_r: int) -> int:
     return int(lib().npair_eval_map_at_r_bytes(nq, sum_r))
 
 
+def eval_kmeans_bytes(n: int, k: int, D: int) -> int:
+    """Device bytes Evaluator.kmeans adds on top of the workspace for n points of dimension D in k clusters (0 if invalid)."""
+    return int(lib().npair_eval_kmeans_bytes(n, k, D))
+
+
 class Evaluator:
     """Retrieval evaluation (include/npair_b200.h, DESIGN 8): the rank of every query's best positive among the gallery, computed on
     the tensor cores without storing the similarity matrix.  Takes contiguous CUDA fp32 tensors; results are int32 / fp32 CUDA
@@ -320,6 +329,26 @@ class Evaluator:
                                               self._arg(glabel, 1), gallery.shape[0], self_offset, map_r.data_ptr(), r_prec.data_ptr(),
                                               R.data_ptr(), rank.data_ptr(), torch.cuda.current_stream().cuda_stream))
         return {"map_r": map_r, "r_precision": r_prec, "R": R, "rank": rank}
+
+    def kmeans(self, x, k, init_rows, max_iter):
+        """npair_eval_kmeans (DESIGN 8.2): Lloyd's k-means of the rows of x into k clusters, centroid c starting as row init_rows[c].
+        Returns {"assign": int32[n], "centroids": fp32[k, D] (those assign was computed against), "inertia": fp64 scalar tensor,
+        "iterations": sweeps run, "changed": assignments the last sweep changed, "empty": empty clusters}.  Synchronises with the host
+        once per iteration."""
+        import torch
+        n, dev = x.shape[0], x.device
+        init_rows = [int(r) for r in init_rows]
+        if len(init_rows) != int(k):
+            raise ValueError("init_rows must hold k row indices")
+        rows = (C.c_int32 * int(k))(*init_rows)
+        centroids = torch.empty(int(k), self.D, dtype=torch.float32, device=dev)
+        assign = torch.empty(n, dtype=torch.int32, device=dev)
+        inertia = torch.empty((), dtype=torch.float64, device=dev)
+        stats = (C.c_int32 * 3)()
+        self._check(lib().npair_eval_kmeans(self._h, self._arg(x, 2), n, int(k), rows, int(max_iter), centroids.data_ptr(),
+                                            assign.data_ptr(), inertia.data_ptr(), stats, torch.cuda.current_stream().cuda_stream))
+        return {"assign": assign, "centroids": centroids, "inertia": inertia, "iterations": stats[0], "changed": stats[1],
+                "empty": stats[2]}
 
 
 def debug_gemm(precision, backend, A, B):

@@ -197,6 +197,7 @@ static GemmKernel sim_gemm_t(int epi) {
     case EPI_GATHER | EPI_SYM: return gemm_t<1, BF16, EPI_GATHER | EPI_SYM, 64>();
     case EPI_BUCKET: return gemm_t<1, BF16, EPI_BUCKET, 64>();
     case EPI_BUCKET | EPI_SYM: return gemm_t<1, BF16, EPI_BUCKET | EPI_SYM, 64>();
+    case EPI_ARGMAX: return gemm_t<1, BF16, EPI_ARGMAX, 64>();                     // k-means assignment
     default: return GemmKernel{nullptr, 0, 0};
   }
 }
@@ -1612,6 +1613,9 @@ struct npair_eval : EvalPlan {
   size_t map_rows_bytes = 0;
   void* map_pairs = nullptr;
   size_t map_pairs_bytes = 0;
+  // k-means (npair_eval_kmeans), grown on demand and kept (kmeans_bytes)
+  void* km = nullptr;
+  size_t km_bytes = 0;
   std::string err;
 };
 
@@ -1619,8 +1623,13 @@ struct npair_eval : EvalPlan {
 // the gather counter and the {sum R, error bits} word pair; per positive pair the value and the histogram word
 static size_t map_rows_bytes(long long nq) { return 8ull * (nq + 1) + 4ull * nq + 16; }
 static size_t map_pairs_bytes(long long sum_r) { return 8ull * sum_r; }
+// Device memory of npair_eval_kmeans beyond the workspace, in the order it is carved: the int64 sums [k][D], the argmax keys [n], the
+// inertia partials, then the counts [k], the biases [k], the initial rows [k] and the KmeansWords
+static size_t kmeans_bytes(long long n, long long k, long long D) {
+  return 8ull * k * D + 8ull * n + 8ull * KM_INERTIA_BLOCKS + 12ull * k + sizeof(KmeansWords);
+}
 
-// Grows *buf to at least `bytes` (freeing the old one: cudaFree waits for the device)
+// Grows *buf to at least `bytes` (freeing the old one: cudaFree waits for the device); `what` names the buffer in the error text
 static int eval_grow(npair_eval* ev, void** buf, size_t* have, size_t bytes, const char* what) {
   if (bytes <= *have) return NPAIR_OK;
   cudaFree(*buf);
@@ -1628,7 +1637,7 @@ static int eval_grow(npair_eval* ev, void** buf, size_t* have, size_t bytes, con
   if (cudaMalloc(buf, bytes) != cudaSuccess) {
     cudaGetLastError();
     *buf = nullptr;
-    ev->err = fmt("cannot allocate %zu bytes for the MAP@R %s", bytes, what);
+    ev->err = fmt("cannot allocate %zu bytes for %s", bytes, what);
     return NPAIR_E_CUDA;
   }
   *have = bytes;
@@ -1651,13 +1660,18 @@ size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r) {
   return map_rows_bytes(nq) + map_pairs_bytes(sum_r);
 }
 
+size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
+  if (n < 1 || k < 1 || D < 1 || k > n) return 0;
+  return kmeans_bytes(n, k, D);
+}
+
 const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
 
 void npair_eval_destroy(npair_eval* ev) {
   if (!ev) return;
   if (ev->device >= 0) cudaSetDevice(ev->device);
   cudaFree(ev->catA); cudaFree(ev->catB); cudaFree(ev->rows); cudaFree(ev->bs); cudaFree(ev->sym_tiles);
-  cudaFree(ev->map_rows); cudaFree(ev->map_pairs);
+  cudaFree(ev->map_rows); cudaFree(ev->map_pairs); cudaFree(ev->km);
   delete ev;
 }
 
@@ -1683,7 +1697,7 @@ int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int
   ev->ra.cnt_same = reinterpret_cast<int*>(w); w += max_q;
   ev->absmax_bits = w;
   const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
-                      EPI_BUCKET | EPI_SYM};
+                      EPI_BUCKET | EPI_SYM, EPI_ARGMAX};
   for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
   *out = made.release();
   return NPAIR_OK;
@@ -1726,7 +1740,7 @@ static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, 
 }
 
 // One sweep of the similarity GEMM over the prepared operands: EPI_STATS, EPI_GATHER or EPI_BUCKET (labels, and `map` for the MAP@R
-// sweeps) or EPI_COUNT (cut, count), + EPI_SYM when `sym`
+// sweeps), EPI_COUNT (cut, count) or EPI_ARGMAX (`map`'s col_bias and best), + EPI_SYM when `sym`
 static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, const float* ql, const float* gl, const float* cut, int32_t* count,
                       bool sym, cudaStream_t st, const GemmParams* map = nullptr) {
   if (sym) {
@@ -1741,7 +1755,10 @@ static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, con
   gp.self_offset = self_col;
   if (epi & (EPI_STATS | EPI_GATHER | EPI_BUCKET)) { gp.lab_rows = ql; gp.lab_cols = gl; }
   else { gp.cut = cut; gp.count = count; }
-  if (map) { gp.cnt_same = ev->ra.cnt_same; gp.bs = ev->bs; gp.seg = map->seg; gp.fill = map->fill; gp.pos = map->pos; gp.hist = map->hist; }
+  if (map) {
+    gp.cnt_same = ev->ra.cnt_same; gp.bs = ev->bs; gp.seg = map->seg; gp.fill = map->fill; gp.pos = map->pos; gp.hist = map->hist;
+    gp.col_bias = map->col_bias; gp.best = map->best;
+  }
   CUtensorMap ta, tb;
   std::string te;
   if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
@@ -1819,7 +1836,7 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
   CUDA_TRY(ev, cudaSetDevice(ev->device));
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
-  if ((rc = eval_grow(ev, &ev->map_rows, &ev->map_rows_bytes, map_rows_bytes(nq), "per-query offsets")) != NPAIR_OK) return rc;
+  if ((rc = eval_grow(ev, &ev->map_rows, &ev->map_rows_bytes, map_rows_bytes(nq), "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
   long long* seg = static_cast<long long*>(ev->map_rows);                          // [nq + 1]
   unsigned long long* sum_err = reinterpret_cast<unsigned long long*>(seg + nq + 1);  // {sum R_i, error bits}
   int* fill = reinterpret_cast<int*>(sum_err + 2);                                    // [nq]
@@ -1837,7 +1854,7 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
     return NPAIR_E_CUDA;
   }
   const long long sum_r = static_cast<long long>(h[0]);
-  if ((rc = eval_grow(ev, &ev->map_pairs, &ev->map_pairs_bytes, map_pairs_bytes(sum_r), "positive pairs")) != NPAIR_OK) return rc;
+  if ((rc = eval_grow(ev, &ev->map_pairs, &ev->map_pairs_bytes, map_pairs_bytes(sum_r), "the MAP@R positive pairs")) != NPAIR_OK) return rc;
   float* pos = static_cast<float*>(ev->map_pairs);
   unsigned int* hist = reinterpret_cast<unsigned int*>(pos + sum_r);
   CUDA_TRY(ev, cudaMemsetAsync(fill, 0, sizeof(int) * nq, st));
@@ -1854,6 +1871,71 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
   }
   launch_eval_map_finish(R, seg, fill, pos, hist, nq, d_map_r, d_r_precision, d_R, d_rank, st);
   CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+// Lloyd's k-means on the evaluator's operands (DESIGN 8.2): the points are split once into the A format, with the pre-scale sigma of
+// max|x|, which also bounds every centroid (a mean lies in its members' convex hull); each iteration splits the centroids into the B
+// format with the same sigma, sweeps EPI_ARGMAX against their biases 0.5 ||mu||^2, decodes the keys while adding the members'
+// fixed-point features into int64 sums, reads back {changed, err} and, unless it stops, replaces each non-empty centroid by its mean.
+int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, const int32_t* init_rows, int32_t max_iter, float* d_centroids,
+                      int32_t* d_assign, double* d_inertia, int32_t stats[3], void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  if (!x || !init_rows || !d_centroids || !d_assign || !stats) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (n < 1 || k < 1 || k > n) { ev->err = fmt("k-means needs 1 <= k <= n (n = %d, k = %d)", n, k); return NPAIR_E_ARG; }
+  if (n > ev->max_q || k > ev->max_g) {
+    ev->err = fmt("n = %d points, k = %d centroids exceed the evaluator's capacity (%d, %d)", n, k, ev->max_q, ev->max_g);
+    return NPAIR_E_ARG;
+  }
+  if (max_iter < 1) { ev->err = "max_iter must be >= 1"; return NPAIR_E_ARG; }
+  for (int c = 0; c < k; ++c)
+    if (init_rows[c] < 0 || init_rows[c] >= n) { ev->err = fmt("init_rows[%d] = %d is not a row of x", c, init_rows[c]); return NPAIR_E_ARG; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(ev, cudaSetDevice(ev->device));
+  int rc;
+  if ((rc = eval_grow(ev, &ev->km, &ev->km_bytes, kmeans_bytes(n, k, ev->D), "the k-means buffers")) != NPAIR_OK) return rc;
+  const long long D = ev->D;
+  long long* sums = static_cast<long long*>(ev->km);                                  // [k][D]
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(sums + k * D);     // [n]
+  double* partial = reinterpret_cast<double*>(keys + n);                              // [KM_INERTIA_BLOCKS]
+  int* counts = reinterpret_cast<int*>(partial + KM_INERTIA_BLOCKS);                  // [k]
+  float* bias = reinterpret_cast<float*>(counts + k);                                 // [k]
+  int* rows = reinterpret_cast<int*>(bias + k);                                       // [k]
+  KmeansWords* words = reinterpret_cast<KmeansWords*>(rows + k);
+  unsigned int* amx = ev->absmax_bits;
+  CUDA_TRY(ev, cudaMemcpyAsync(rows, init_rows, sizeof(int) * k, cudaMemcpyHostToDevice, st));
+  // the points, once: max|x| in every format (the update's fixed-point scale), then the A operand
+  CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
+  launch_eval_prep(x, n * D, nullptr, 0, amx, ev->ra, 0, ev->sms, st);
+  launch_eval_split(x, n, ev->D, ev->Dp, ev->prec, 0, -1.f, amx, ev->bs, ev->catA, st);
+  launch_km_gather(x, ev->D, rows, k, d_centroids, st);
+  CUDA_TRY(ev, cudaMemsetAsync(d_assign, 0xFF, sizeof(int32_t) * n, st));   // -1: every point of the first sweep changes
+  CUDA_TRY(ev, cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * n, st));
+  CUDA_TRY(ev, cudaMemsetAsync(sums, 0, sizeof(long long) * k * D, st));     // a call that stopped on convergence leaves them set
+  GemmParams am{};
+  am.col_bias = bias; am.best = keys;
+  KmeansWords h{};
+  int t = 0;
+  for (;; ++t) {
+    const bool last = t + 1 == max_iter;
+    launch_eval_split(d_centroids, k, ev->D, ev->Dp, ev->prec, 1, -1.f, amx, ev->bs, ev->catB, st);
+    launch_km_bias(d_centroids, k, ev->D, bias, counts, words, st);
+    if ((rc = eval_sweep(ev, EPI_ARGMAX, n, k, EVAL_NO_SELF, nullptr, nullptr, nullptr, nullptr, false, st, &am)) != NPAIR_OK) return rc;
+    launch_km_assign(keys, x, n, ev->D, amx, k, d_assign, counts, sums, !last, words, st);
+    CUDA_TRY(ev, cudaMemcpyAsync(&h, words, sizeof(h), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ev, cudaStreamSynchronize(st));
+    if (h.err & DERR_KMEANS_NO_ARGMAX) {
+      ev->err = "a point has no centroid with a finite score: x or a centroid holds NaN or infinity";
+      return NPAIR_E_CUDA;
+    }
+    if ((t > 0 && h.changed == 0) || last) break;
+    launch_km_update(sums, counts, amx, k, ev->D, d_centroids, st);
+  }
+  if (d_inertia) launch_km_inertia(x, d_centroids, d_assign, n, ev->D, partial, d_inertia, st);
+  CUDA_TRY(ev, cudaGetLastError());
+  stats[0] = t + 1;
+  stats[1] = static_cast<int32_t>(h.changed);
+  stats[2] = k - static_cast<int32_t>(h.nonempty);
   return NPAIR_OK;
 }
 

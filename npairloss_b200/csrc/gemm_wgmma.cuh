@@ -42,7 +42,10 @@ namespace npair {
 //               of `pos`, in atomic order; with EPI_SYM a mirrored block gathers for each column gc.  Used alone (+ EPI_SYM).
 // EPI_BUCKET  : MAP@R evaluation.  For every negative pair s of row i with s >= the row's smallest positive, hist[seg[i] + b] += 1 with
 //               b = #{k : p_k > s} over the row's positives sorted descending; with EPI_SYM also for each mirrored column gc.
-enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64, EPI_GATHER = 128, EPI_BUCKET = 256 };
+// EPI_ARGMAX  : k-means assignment (DESIGN 8.2).  Per row, the column c < Nn with the largest s - col_bias[c], the lowest such c on
+//               ties, as one 64-bit atomicMax per row and thread into best[row] of the key (f2ord(score) << 32) | (0xFFFFFFFF - c),
+//               which is independent of the tile order.  No self exclusion, no labels.  Used alone, with full tiles (no EPI_SYM).
+enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64, EPI_GATHER = 128, EPI_BUCKET = 256, EPI_ARGMAX = 512 };
 
 // Persistent tile schedule of both wgmma GEMMs (host: tile_sched, ctx.cu).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
 // output tile (m_blk, n_blk) or tile_list[t], K blocks [kb0, kb1) of split-K slice `split`.  split moves fastest, then n_blk, m_blk.
@@ -101,6 +104,9 @@ struct GemmParams {
   int* fill;               // [M] EPI_GATHER: positives claimed so far, pre-zeroed
   float* pos;              // EPI_GATHER: row i's positives, unordered; EPI_BUCKET: the same sorted descending
   unsigned int* hist;      // EPI_BUCKET: per-row bucket counts, pre-zeroed
+  // ---- EPI_ARGMAX ----
+  const float* col_bias;          // [Nn] subtracted from column c's similarities
+  unsigned long long* best;       // [M] argmax keys, pre-zeroed
 };
 
 // BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
@@ -286,6 +292,16 @@ __device__ __forceinline__ void bucket_search(uint32_t cand, Val val, const floa
   if (run) atomicAdd(&hist[run_b], run);
 }
 
+// EPI_ARGMAX: the largest s - bias[c] over the first `valid` of 32 consecutive columns (idx0 + c) into (best, col), keeping the earlier
+// column on ties; NaN scores never win
+__device__ __forceinline__ void argmax32(const float (&v)[32], const float* __restrict__ bias, int idx0, int valid, float& best, int& col) {
+#pragma unroll
+  for (int c = 0; c < 32; ++c) {
+    const float s = v[c] - bias[c];
+    if (c < valid && s > best) { best = s; col = idx0 + c; }
+  }
+}
+
 template <int NSPLIT, bool BF16, int EPI, int BK_>
 __global__ void __launch_bounds__(384, 1)
 split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
@@ -294,15 +310,17 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
   constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS, COUNT = EPI & EPI_COUNT;
-  constexpr bool GATHER = EPI & EPI_GATHER, BUCKET = EPI & EPI_BUCKET;
+  constexpr bool GATHER = EPI & EPI_GATHER, BUCKET = EPI & EPI_BUCKET, ARGMAX = EPI & EPI_ARGMAX;
   constexpr bool LABELS = STATS || GATHER || BUCKET;              // the epilogue needs the tile's labels
+  static_assert(!ARGMAX || EPI == EPI_ARGMAX, "EPI_ARGMAX is used alone, with full tiles");
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer in the shared address space (offset arithmetic, no integer round trip): LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* acc_stage = smem + STAGES * Cfg::STAGE_BYTES;            // [2 warpgroups][64 rows][16 x 16 B], chunk ^ (row & 7)
   uint8_t* store_stage = acc_stage + Cfg::ACC_STAGE_BYTES;          // [8 warps][32 rows][128 B], 128B-swizzled
   uint8_t* aux = store_stage + Cfg::STORE_STAGE_BYTES;
-  float* s_lab = reinterpret_cast<float*>(aux + 256);                // [256] column labels of the current tile (EPI_STATS)
+  float* s_lab = reinterpret_cast<float*>(aux + 256);                // [256] column labels of the current tile (EPI_STATS), or its
+                                                                     // column biases (EPI_ARGMAX)
   float* s_labr = reinterpret_cast<float*>(aux + 256 + 1024);        // [128] row labels of the current tile (EPI_SYM)
   float2* s_rng = reinterpret_cast<float2*>(aux + 256 + 1024 + 512); // [8] {min, max} label of each 32-column chunk, [8..12) of each 32-row group
 
@@ -387,6 +405,11 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
+      if constexpr (ARGMAX) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers are done with the biases
+        s_lab[et] = (col_base + et < p.Nn) ? p.col_bias[col_base + et] : 0.f;
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
 
       // ---- main loop: this warpgroup's 64 x 256 block, fp32 accumulator in registers.  One K block of MMAs stays in flight: the
       //      wait after committing K block kb retires kb - 1, whose stage is then released (a stage is reusable once every consumer
@@ -467,6 +490,9 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         p1_i = count_cut(R_i ? p.pos[seg_i] : -INFINITY);
         pR_i = count_cut(R_i ? p.pos[seg_i + R_i - 1] : -INFINITY);
       }
+      // EPI_ARGMAX: the row's best score and column over this thread's chunks of the tile (-1: none yet)
+      float arg_s = -INFINITY;
+      int arg_c = -1;
 #pragma unroll
       for (int cp = 0; cp < 4; ++cp) {
         asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");   // the warpgroup's previous reads of the staging tile are done
@@ -490,7 +516,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         // lower-triangle half of a straddling tile: produced by mirroring
         if ((SYM && cb < t.m_blk) || col0 >= p.Nn) continue;
         float v[32];
-        if (STATS || COUNT || GATHER || BUCKET) {
+        if (STATS || COUNT || GATHER || BUCKET || ARGMAX) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
@@ -520,6 +546,9 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           } else if (row < p.M)
             stats32(v, s_lab + ch * 32, lab_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col,
                     minw, maxw, maxb, cnt);
+        }
+        if constexpr (ARGMAX) {
+          if (row < p.M) argmax32(v, s_lab + ch * 32, col0, p.Nn - col0, arg_s, arg_c);
         }
         if (COUNT && row < p.M)
           cnt_ge += count32(v, cut_i, col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32), col0, p.Nn, self_col);
@@ -615,6 +644,10 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       if (COUNT && row < p.M && cnt_ge) atomicAdd(&p.count[row], cnt_ge);
       if constexpr (BUCKET) {
         if (above_i) atomicAdd(&p.hist[seg_i], static_cast<unsigned int>(above_i));
+      }
+      if constexpr (ARGMAX) {
+        if (row < p.M && arg_c >= 0)
+          atomicMax(&p.best[row], (static_cast<unsigned long long>(f2ord(arg_s)) << 32) | (0xFFFFFFFFu - static_cast<uint32_t>(arg_c)));
       }
       if (STATS && row < p.M) {
         maxall = fmaxf(maxw, maxb);                       // every valid column is either same- or diff-label

@@ -1956,4 +1956,135 @@ void launch_eval_map_finish(const int* cnt, const long long* seg, const int* fil
   count_launch();
 }
 
+// --------------------------------------------------------------------------------------------
+// k-means (npair_eval_kmeans, DESIGN 8.2): everything around the EPI_ARGMAX sweep
+// --------------------------------------------------------------------------------------------
+// Centroid c = row rows[c] of x.  Thread = one feature of one centroid.
+__global__ void __launch_bounds__(256) km_gather_kernel(const float* __restrict__ x, int D, const int* __restrict__ rows, int k,
+                                                        float* __restrict__ C) {
+  const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<long long>(k) * D) return;
+  const long long c = e / D;
+  C[e] = x[static_cast<long long>(rows[c]) * D + (e - c * D)];
+}
+void launch_km_gather(const float* x, int D, const int* rows, int k, float* C, cudaStream_t st) {
+  const long long work = static_cast<long long>(k) * D;
+  km_gather_kernel<<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(x, D, rows, k, C);
+  count_launch();
+}
+
+// One warp per centroid: bias[c] = 0.5f * ||C_c||^2 in fp32 (per-lane fmaf chains over d = lane mod 32, then the warp tree), and the
+// iteration's reset of counts[c]; thread 0 also clears the {changed, err, nonempty} words.
+__global__ void __launch_bounds__(256) km_bias_kernel(const float* __restrict__ C, int k, int D, float* __restrict__ bias,
+                                                      int* __restrict__ counts, KmeansWords* words) {
+  const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *words = KmeansWords{0u, 0u, 0u, 0u};
+  if (c >= k) return;
+  const float* r = C + static_cast<long long>(c) * D;
+  float s = 0.f;
+  for (int d = lane; d < D; d += 32) s = fmaf(r[d], r[d], s);
+  s = warp_sum(s);
+  if (lane == 0) { bias[c] = 0.5f * s; counts[c] = 0; }
+}
+void launch_km_bias(const float* C, int k, int D, float* bias, int* counts, KmeansWords* words, cudaStream_t st) {
+  km_bias_kernel<<<(k + 7) / 8, 256, 0, st>>>(C, k, D, bias, counts, words);
+  count_launch();
+}
+
+// One warp per point: decode and clear its argmax key, count a changed assignment and a cluster's first member, and (accumulate)
+// add the point's fixed-point features q = rint(x * sigma * 2^32) to its cluster's int64 sums.  Integer atomics: the sums do not
+// depend on the order the points arrive in.
+__global__ void __launch_bounds__(256) km_assign_kernel(unsigned long long* __restrict__ best, const float* __restrict__ x, int n, int D,
+                                                        const unsigned int* __restrict__ absmax_bits, int k, int* __restrict__ assign,
+                                                        int* __restrict__ counts, long long* __restrict__ sums, int accumulate,
+                                                        KmeansWords* words) {
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  bool changed = false, first = false;
+  if (i < n) {
+    unsigned int a = 0;
+    if (lane == 0) {
+      const unsigned long long key = best[i];
+      best[i] = 0;
+      a = 0xFFFFFFFFu - static_cast<unsigned int>(key);
+      if (key == 0 || a >= static_cast<unsigned int>(k)) { a = 0; atomicOr(&words->err, static_cast<unsigned int>(DERR_KMEANS_NO_ARGMAX)); }
+      changed = assign[i] != static_cast<int>(a);
+      assign[i] = static_cast<int>(a);
+      first = atomicAdd(&counts[a], 1) == 0;
+    }
+    a = __shfl_sync(0xffffffffu, a, 0);
+    if (accumulate) {
+      const float sigma = pre_scale(__uint_as_float(*absmax_bits)).scale;
+      const float* xr = x + static_cast<long long>(i) * D;
+      unsigned long long* sr = reinterpret_cast<unsigned long long*>(sums + static_cast<long long>(a) * D);
+      for (int d = lane; d < D; d += 32)    // x * sigma in (-1, 1) and the scaling by 2^32 are exact; one rounding, to nearest even
+        atomicAdd(&sr[d], static_cast<unsigned long long>(__float2ll_rn((__ldg(xr + d) * sigma) * 4294967296.f)));
+    }
+  }
+  const int n_changed = __syncthreads_count(changed), n_first = __syncthreads_count(first);
+  if (threadIdx.x == 0) {
+    if (n_changed) atomicAdd(&words->changed, static_cast<unsigned int>(n_changed));
+    if (n_first) atomicAdd(&words->nonempty, static_cast<unsigned int>(n_first));
+  }
+}
+void launch_km_assign(unsigned long long* best, const float* x, int n, int D, const unsigned int* absmax_bits, int k, int* assign,
+                      int* counts, long long* sums, bool accumulate, KmeansWords* words, cudaStream_t st) {
+  km_assign_kernel<<<(n + 7) / 8, 256, 0, st>>>(best, x, n, D, absmax_bits, k, assign, counts, sums, accumulate ? 1 : 0, words);
+  count_launch();
+}
+
+// Thread = one feature of one centroid: the mean of a non-empty cluster, (float)(ldexp((double)sum / count, -32) * (1 / sigma)), every
+// step exactly rounded so a host loop in fp64 gives the same bits; an empty cluster keeps its centroid.  Clears the sums.
+__global__ void __launch_bounds__(256) km_update_kernel(long long* __restrict__ sums, const int* __restrict__ counts,
+                                                        const unsigned int* __restrict__ absmax_bits, int k, int D, float* __restrict__ C) {
+  const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<long long>(k) * D) return;
+  const int cnt = counts[e / D];
+  if (cnt > 0) {
+    const double inv = pre_scale(__uint_as_float(*absmax_bits)).inv;
+    C[e] = static_cast<float>(ldexp(static_cast<double>(sums[e]) / static_cast<double>(cnt), -32) * inv);
+    sums[e] = 0;
+  }
+}
+void launch_km_update(long long* sums, const int* counts, const unsigned int* absmax_bits, int k, int D, float* C, cudaStream_t st) {
+  const long long work = static_cast<long long>(k) * D;
+  km_update_kernel<<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(sums, counts, absmax_bits, k, D, C);
+  count_launch();
+}
+
+// Inertia in fp64 in a fixed order: warp w of the fixed grid takes points w, w + KM_INERTIA_BLOCKS * 8, ..., each lane its features
+// d = lane mod 32; the warp tree, the block's warps in order, then one thread over the blocks in order.
+__global__ void __launch_bounds__(256) km_inertia_kernel(const float* __restrict__ x, const float* __restrict__ C,
+                                                         const int* __restrict__ assign, int n, int D, double* __restrict__ partial) {
+  __shared__ double s_w[8];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double s = 0.0;
+  for (int i = blockIdx.x * 8 + w; i < n; i += KM_INERTIA_BLOCKS * 8) {
+    const float* xr = x + static_cast<long long>(i) * D;
+    const float* cr = C + static_cast<long long>(assign[i]) * D;
+    for (int d = lane; d < D; d += 32) {
+      const double e = static_cast<double>(xr[d]) - static_cast<double>(cr[d]);
+      s = fma(e, e, s);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) s_w[w] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int j = 0; j < 8; ++j) b += s_w[j];
+    partial[blockIdx.x] = b;
+  }
+}
+__global__ void km_inertia_finish_kernel(const double* __restrict__ partial, double* __restrict__ out) {
+  double s = 0.0;
+  for (int b = 0; b < KM_INERTIA_BLOCKS; ++b) s += partial[b];
+  *out = s;
+}
+void launch_km_inertia(const float* x, const float* C, const int* assign, int n, int D, double* partial, double* out, cudaStream_t st) {
+  km_inertia_kernel<<<KM_INERTIA_BLOCKS, 256, 0, st>>>(x, C, assign, n, D, partial);
+  km_inertia_finish_kernel<<<1, 1, 0, st>>>(partial, out);
+  count_launch(2);
+}
+
 }  // namespace npair

@@ -16,6 +16,8 @@ enum { M_HARD = 0, M_EASY = 1, M_RAND = 2, M_RELATIVE_HARD = 3, M_RELATIVE_EASY 
 enum { DERR_EMPTY_LIST = 1, DERR_POS_RANGE = 2 };
 // retrieval evaluation: the MAP@R gather found more positives in a row than the statistics sweep counted
 enum { DERR_GATHER_SLOT = 4 };
+// k-means: a point's assignment sweep found no column with a score above -inf (a NaN or infinite input)
+enum { DERR_KMEANS_NO_ARGMAX = 8 };
 
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -226,5 +228,21 @@ void launch_eval_seg_sort(const int* cnt, const long long* seg, int nq, const fl
 // positive's rank, from the sorted positives and the bucket counts
 void launch_eval_map_finish(const int* cnt, const long long* seg, const int* fill, const float* pos, const unsigned int* hist, int nq,
                             double* map_r, double* r_precision, int* R_out, int* rank, cudaStream_t st);
+// k-means (npair_eval_kmeans, DESIGN 8.2).  sigma = pre_scale(max|x|).scale of the points, read from *absmax_bits.
+// What each assignment sweep reports back to the host: assignments that changed, error bits, clusters that have a member
+struct KmeansWords { unsigned int changed, err, nonempty, pad; };
+constexpr int KM_INERTIA_BLOCKS = 256;          // fixed grid of the inertia reduction: its order does not depend on the device
+// C[c] = x[rows[c]] (k x D)
+void launch_km_gather(const float* x, int D, const int* rows, int k, float* C, cudaStream_t st);
+// bias[c] = 0.5f * ||C_c||^2 in fp32; also zeroes counts[0..k) and *words
+void launch_km_bias(const float* C, int k, int D, float* bias, int* counts, KmeansWords* words, cudaStream_t st);
+// assign[i] = the column of the EPI_ARGMAX key best[i] (then zeroed); counts[a] += 1, words->changed / nonempty / err; accumulate:
+// sums[a][d] += rint(x[i][d] * sigma * 2^32) in int64
+void launch_km_assign(unsigned long long* best, const float* x, int n, int D, const unsigned int* absmax_bits, int k, int* assign,
+                      int* counts, long long* sums, bool accumulate, KmeansWords* words, cudaStream_t st);
+// C[c] = the fixed-point mean of cluster c where counts[c] > 0 (else unchanged); zeroes the sums
+void launch_km_update(long long* sums, const int* counts, const unsigned int* absmax_bits, int k, int D, float* C, cudaStream_t st);
+// *out = sum_i ||x_i - C[assign[i]]||^2 in fp64, in a fixed order (partial: KM_INERTIA_BLOCKS doubles of scratch)
+void launch_km_inertia(const float* x, const float* C, const int* assign, int n, int D, double* partial, double* out, cudaStream_t st);
 
 }  // namespace npair

@@ -135,6 +135,70 @@ def retrieval_metrics(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8),
     return out, per_query
 
 
+def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi.PREC_FP32_FP16X2):
+    """NMI and F1 of a k-means clustering of a whole embedding set, the clustering half of the metric-learning protocol (Sohn 2016;
+    Song et al. 2016), with Lloyd's k-means on the tensor cores (Evaluator.kmeans, DESIGN 8.2; not part of the reference layer).
+
+    Takes CUDA fp32 embeddings as given (L2-normalise them first for cosine geometry) and labels of any numeric dtype, compared as
+    floats.  k=None: the number of distinct labels.  Centroid c starts as row init[c] of
+    init = torch.randperm(n, generator=torch.Generator().manual_seed(seed))[:k], so the same seed gives the same result; there is
+    one run, no restarts.  Returns ({"nmi", "f1", "inertia", "iterations", "converged", "empty_clusters"}, assign, centroids) with
+    the scores of clustering_scores, "converged" whether the last sweep changed no assignment, and assign / centroids CUDA tensors."""
+    x, lab, _, _, _ = _retrieval_sets("clustering_metrics", emb, labels, None, None, None)
+    n, D = x.shape
+    if k is None:
+        k = int(torch.unique(lab).numel())
+    k = int(k)
+    if not 1 <= k <= n:
+        raise ValueError(f"clustering_metrics needs 1 <= k <= n (n = {n}, k = {k})")
+    init = torch.randperm(n, generator=torch.Generator().manual_seed(int(seed)))[:k].tolist()
+    ev = capi.Evaluator(n, k, D, precision, x.device.index or 0)
+    try:
+        res = ev.kmeans(x, k, init, max_iter)
+    finally:
+        ev.close()
+    nmi, f1 = clustering_scores(lab, res["assign"])
+    out = {"nmi": nmi, "f1": f1, "inertia": float(res["inertia"]), "iterations": res["iterations"],
+           "converged": res["changed"] == 0, "empty_clusters": res["empty"]}
+    return out, res["assign"], res["centroids"]
+
+
+def clustering_scores(labels, assign):
+    """(NMI, F1) of the clustering `assign` against `labels` (compared as floats), by fp64 / int64 bookkeeping over the non-zero
+    cells of the contingency table, on the tensors' device.
+      NMI = 2 I(Y;C) / (H(Y) + H(C)), natural log, over the non-empty clusters; 1.0 when both entropies are 0.
+      F1  = pairwise: TP = sum over cells of C(n_lc, 2), precision = TP / sum_c C(n_c, 2), recall = TP / sum_l C(n_l, 2); a 0/0 term
+            counts as 0, and F1 = 0 when precision + recall = 0.
+    Each entropy and the mutual information sum their terms in ascending order, so a perfect clustering gives exactly 1.0."""
+    lab = labels.reshape(-1).to(torch.float32)
+    a = assign.reshape(-1).to(device=lab.device, dtype=torch.int64)
+    if lab.numel() != a.numel():
+        raise ValueError("labels and assign differ in length")
+    n = lab.numel()
+    _, y = torch.unique(lab, return_inverse=True)
+    _, c = torch.unique(a, return_inverse=True)                   # the non-empty clusters, renumbered
+    n_c_ids = int(c.max()) + 1
+    cells, n_lc = torch.unique(y * n_c_ids + c, return_counts=True)
+    n_l, n_c = torch.bincount(y), torch.bincount(c)
+
+    def plogn(counts, denom):                                     # sum of (m / n) log(n / denom) over the terms, ascending
+        p = counts.double() / n
+        return float(torch.sort(p * torch.log(n / denom.double())).values.sum())
+
+    i_yc = plogn(n_lc, n_l[cells // n_c_ids] * n_c[cells % n_c_ids] / n_lc.double())
+    h_y, h_c = plogn(n_l, n_l), plogn(n_c, n_c)
+    nmi = 1.0 if h_y + h_c == 0 else 2.0 * i_yc / (h_y + h_c)
+
+    def pairs(m):
+        return int((m * (m - 1) // 2).sum())
+
+    tp, pc, pl = pairs(n_lc), pairs(n_c), pairs(n_l)
+    prec = tp / pc if pc else 0.0
+    rec = tp / pl if pl else 0.0
+    f1 = 2.0 * prec * rec / (prec + rec) if prec + rec > 0 else 0.0
+    return nmi, f1
+
+
 def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
     """(query, query labels, gallery, gallery labels, self_offset) as the evaluator takes them: contiguous 2-D CUDA fp32 rows, fp32
     labels; gallery=None is self-retrieval."""
