@@ -143,7 +143,10 @@ void npair_destroy(npair_ctx* ctx);
 int npair_forward(npair_ctx* ctx, const float* d_feat, const float* d_label, float tops_host[5], void* stream);
 
 /* Backward_gpu.  loss_weight = top[0]->cpu_diff()[0] (.cu:435).  d_feat_diff: Q x D fp32, OVERWRITTEN
- * (bottom[0]->mutable_gpu_diff(); beta = 0 at .cu:448, propagate_down ignored).  Asynchronous on `stream`. */
+ * (bottom[0]->mutable_gpu_diff(); beta = 0 at .cu:448, propagate_down ignored).  Asynchronous on `stream`.
+ * Every gradient output (d_feat_diff here and in npair_forward_backward / npair_backward_gathered, d_local_half and d_total_half of
+ * npair_backward_partial) must be 16-byte aligned, as cudaMalloc, Caffe blobs and torch allocations are: the gradient kernels
+ * store it with vector stores.  Otherwise the call returns NPAIR_E_ARG before it enqueues anything.  Inputs may have any alignment. */
 int npair_backward(npair_ctx* ctx, float loss_weight, float* d_feat_diff, void* stream);
 
 /* npair_forward + npair_backward with a single host synchronisation: the backward is enqueued behind the forward's kernels (the

@@ -337,22 +337,24 @@ __global__ void p2p_wait_kernel(const uint32_t* __restrict__ flags /*[world]*/, 
   }
 }
 
-// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K)
+// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K).  Slice s starts at part + s*n: 16-byte loads and
+// stores only when every slice and `out` start 16-byte aligned (n % 4 == 0), otherwise one float at a time -- the same sums either way.
 __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, long long n, float* __restrict__ out, float beta) {
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
-  for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
-    if (i + 3 < n) {
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x, nth = static_cast<long long>(gridDim.x) * blockDim.x;
+  const bool vec = (n & 3) == 0 && ((reinterpret_cast<uintptr_t>(part) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+  if (vec) {
+    for (long long i = t0 * 4; i < n; i += nth * 4) {
       float4 a = *reinterpret_cast<const float4*>(part + i);
       for (int s = 1; s < splits; ++s) { const float4 b = *reinterpret_cast<const float4*>(part + s * n + i); a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
       if (beta != 0.f) { const float4 o = *reinterpret_cast<const float4*>(out + i); a.x += beta * o.x; a.y += beta * o.y; a.z += beta * o.z; a.w += beta * o.w; }
       *reinterpret_cast<float4*>(out + i) = a;
-    } else {
-      for (long long j = i; j < n; ++j) {
-        float a = part[j];
-        for (int s = 1; s < splits; ++s) a += part[s * n + j];
-        if (beta != 0.f) a += beta * out[j];
-        out[j] = a;
-      }
+    }
+  } else {
+    for (long long i = t0; i < n; i += nth) {
+      float a = part[i];
+      for (int s = 1; s < splits; ++s) a += part[s * n + i];
+      if (beta != 0.f) a += beta * out[i];
+      out[i] = a;
     }
   }
 }
@@ -1208,9 +1210,18 @@ static int backward_impl(npair_ctx* c, float loss_weight, float* d_diff, float* 
 
 int npair_bwd_exchange_mode(const npair_ctx* c) { return c ? c->bwd_mode : NPAIR_E_ARG; }
 
+// The gradient kernels write their outputs with 8- and 16-byte stores, so every output pointer must be 16-byte aligned (cudaMalloc,
+// Caffe blobs and torch allocations are).  NULL passes: the callers test for it themselves.
+static int check_out_aligned(npair_ctx* c, const float* p, const char* name) {
+  if ((reinterpret_cast<uintptr_t>(p) & 15) == 0) return NPAIR_OK;
+  c->err = fmt("%s is not 16-byte aligned", name);
+  return NPAIR_E_ARG;
+}
+
 int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_diff) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
+  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
   if (!c->fwd_done) { c->err = "npair_backward called without a successful npair_forward"; return NPAIR_E_STATE; }
   if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator: use npair_backward_partial / npair_backward_gathered"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1227,6 +1238,7 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
                            void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !d_diff || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
   if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   c->defer_sync = true;
@@ -1250,6 +1262,8 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
 int npair_backward_partial(npair_ctx* c, float loss_weight, float* d_local_half, float* d_total_half, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_local_half || (c->world > 1 && !d_total_half)) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
+  if (check_out_aligned(c, d_local_half, "d_local_half") != NPAIR_OK) return NPAIR_E_ARG;
+  if (c->world > 1 && check_out_aligned(c, d_total_half, "d_total_half") != NPAIR_OK) return NPAIR_E_ARG;
   if (!c->fwd_done) { c->err = "npair_backward_partial called without a successful forward"; return NPAIR_E_STATE; }
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1269,6 +1283,7 @@ int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
 int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_total, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_rs_total || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
   if (!c->fwd_done) { c->err = "npair_backward_gathered called without a successful forward"; return NPAIR_E_STATE; }
   if (c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -109,6 +109,37 @@ __device__ __forceinline__ float fast_exp_m2(float sv, float m2) {
 // --------------------------------------------------------------------------------------------
 // absmax / asum  (caffe_gpu_asum .cu:400; operand pre-scale for PREC_FP16X2)
 // --------------------------------------------------------------------------------------------
+// x[4q .. 4q + 3]: one 16-byte load (VEC: x is 16-byte aligned) or four 4-byte loads
+template <bool VEC>
+__device__ __forceinline__ float4 load4(const float* __restrict__ x, long long q) {
+  if (VEC) return __ldg(reinterpret_cast<const float4*>(x) + q);
+  return make_float4(__ldg(x + 4 * q), __ldg(x + 4 * q + 1), __ldg(x + 4 * q + 2), __ldg(x + 4 * q + 3));
+}
+// This thread's share of sum |x| (and of max |x| when want_max) over x[0, n): groups of 4 a grid stride apart, four groups in flight,
+// then the last n % 4 elements.  VEC: 16-byte loads (x 16-byte aligned); otherwise the same elements in the same order through
+// 4-byte loads, so the asum top does not depend on where the caller's buffer starts.
+template <bool VEC>
+__device__ __forceinline__ void abs_sum_max(const float* __restrict__ x, long long n, long long t0, long long stride, bool want_max,
+                                            float& sum, float& mx) {
+  const long long n4 = n >> 2;
+  long long i = t0;
+  for (; i + 3 * stride < n4; i += 4 * stride) {
+    const float4 a = load4<VEC>(x, i), b = load4<VEC>(x, i + stride), c = load4<VEC>(x, i + 2 * stride), d = load4<VEC>(x, i + 3 * stride);
+    const float a0 = fabsf(a.x), a1 = fabsf(a.y), a2 = fabsf(a.z), a3 = fabsf(a.w), b0 = fabsf(b.x), b1 = fabsf(b.y), b2 = fabsf(b.z), b3 = fabsf(b.w);
+    const float c0 = fabsf(c.x), c1 = fabsf(c.y), c2 = fabsf(c.z), c3 = fabsf(c.w), d0 = fabsf(d.x), d1 = fabsf(d.y), d2 = fabsf(d.z), d3 = fabsf(d.w);
+    sum += (a0 + a1) + (a2 + a3) + (b0 + b1) + (b2 + b3) + (c0 + c1) + (c2 + c3) + (d0 + d1) + (d2 + d3);
+    if (want_max) {
+      mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(a0, a1), fmaxf(a2, a3)), fmaxf(fmaxf(b0, b1), fmaxf(b2, b3))));
+      mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(c0, c1), fmaxf(c2, c3)), fmaxf(fmaxf(d0, d1), fmaxf(d2, d3))));
+    }
+  }
+  for (; i < n4; i += stride) {
+    const float4 a = load4<VEC>(x, i);
+    sum += (fabsf(a.x) + fabsf(a.y)) + (fabsf(a.z) + fabsf(a.w));
+    if (want_max) mx = fmaxf(mx, fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))));
+  }
+  for (long long j = (n4 << 2) + t0; j < n; j += stride) { sum += fabsf(x[j]); if (want_max) mx = fmaxf(mx, fabsf(x[j])); }
+}
 // One kernel: per-block partial |x| sums (local rows) and max|x| (all rows), the reset of the per-row statistics, and --
 // in the last block to finish (ticket) -- the final asum, the power-of-two operand scale and the reset of the step state.
 // Returns true in the block that finished last (it has written the step's scalars to *bs).
@@ -119,31 +150,10 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
   float sum = 0.f, mx = 0.f;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  // 16-byte loads, four in flight per thread (cudaMalloc'd / framework blobs are 16-byte aligned; otherwise the scalar loop)
+  // 16-byte loads, four in flight per thread (cudaMalloc'd / framework blobs are 16-byte aligned; otherwise 4-byte loads)
   const bool same_range = want_scale && xl == xt && nl == ntot;    // world == 1: one sweep gives both the sum and the maximum
-  if ((reinterpret_cast<uintptr_t>(xl) & 15) == 0) {
-    const float4* x4 = reinterpret_cast<const float4*>(xl);
-    const long long n4 = nl >> 2;
-    long long i = t0;
-    for (; i + 3 * stride < n4; i += 4 * stride) {
-      const float4 a = __ldg(x4 + i), b = __ldg(x4 + i + stride), c = __ldg(x4 + i + 2 * stride), d = __ldg(x4 + i + 3 * stride);
-      const float a0 = fabsf(a.x), a1 = fabsf(a.y), a2 = fabsf(a.z), a3 = fabsf(a.w), b0 = fabsf(b.x), b1 = fabsf(b.y), b2 = fabsf(b.z), b3 = fabsf(b.w);
-      const float c0 = fabsf(c.x), c1 = fabsf(c.y), c2 = fabsf(c.z), c3 = fabsf(c.w), d0 = fabsf(d.x), d1 = fabsf(d.y), d2 = fabsf(d.z), d3 = fabsf(d.w);
-      sum += (a0 + a1) + (a2 + a3) + (b0 + b1) + (b2 + b3) + (c0 + c1) + (c2 + c3) + (d0 + d1) + (d2 + d3);
-      if (same_range) {
-        mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(a0, a1), fmaxf(a2, a3)), fmaxf(fmaxf(b0, b1), fmaxf(b2, b3))));
-        mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(c0, c1), fmaxf(c2, c3)), fmaxf(fmaxf(d0, d1), fmaxf(d2, d3))));
-      }
-    }
-    for (; i < n4; i += stride) {
-      const float4 a = __ldg(x4 + i);
-      sum += (fabsf(a.x) + fabsf(a.y)) + (fabsf(a.z) + fabsf(a.w));
-      if (same_range) mx = fmaxf(mx, fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))));
-    }
-    for (long long j = (n4 << 2) + t0; j < nl; j += stride) { sum += fabsf(xl[j]); if (same_range) mx = fmaxf(mx, fabsf(xl[j])); }
-  } else {
-    for (long long i = t0; i < nl; i += stride) { sum += fabsf(xl[i]); if (same_range) mx = fmaxf(mx, fabsf(xl[i])); }
-  }
+  if ((reinterpret_cast<uintptr_t>(xl) & 15) == 0) abs_sum_max<true>(xl, nl, t0, stride, same_range, sum, mx);
+  else abs_sum_max<false>(xl, nl, t0, stride, same_range, sum, mx);
   if (want_scale && !same_range) {
     if ((reinterpret_cast<uintptr_t>(xt) & 15) == 0) {
       const float4* x4 = reinterpret_cast<const float4*>(xt);
@@ -1700,9 +1710,13 @@ __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const float* __restrict
   if (r >= rows) return;
   const float* xr = x + static_cast<long long>(r) * dim;
   float* yr = y + static_cast<long long>(r) * dim;
-  const bool vec = (dim & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+  // dim % 4 == 0: each lane sums groups of 4 features (16-byte loads when both pointers allow, otherwise 4-byte loads in the same
+  // order, so y does not depend on where x starts); else lane-strided features
+  const bool quad = (dim & 3) == 0;
+  const bool vec = quad && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
   float ss = 0.f;
   if (vec) for (int d = lane * 4; d < dim; d += 128) { const float4 v = *reinterpret_cast<const float4*>(xr + d); ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss); }
+  else if (quad) for (int d = lane * 4; d < dim; d += 128) for (int e = 0; e < 4; ++e) ss = fmaf(xr[d + e], xr[d + e], ss);
   else for (int d = lane; d < dim; d += 32) ss = fmaf(xr[d], xr[d], ss);
   ss = warp_sum(ss);
   const float nrm = sqrtf(ss);
@@ -1721,11 +1735,14 @@ __global__ void __launch_bounds__(256) l2norm_bwd_kernel(const float* __restrict
   const float* yr = y + static_cast<long long>(r) * dim;
   const float* gr = dy + static_cast<long long>(r) * dim;
   float* dr = dx + static_cast<long long>(r) * dim;
-  const bool vec = (dim & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
+  const bool quad = (dim & 3) == 0;            // as in l2norm_fwd_kernel: the summation order depends on dim only
+  const bool vec = quad && ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
   float dot = 0.f;
   if (vec) for (int d = lane * 4; d < dim; d += 128) {
     const float4 a = *reinterpret_cast<const float4*>(yr + d), g = *reinterpret_cast<const float4*>(gr + d);
     dot = fmaf(a.x, g.x, dot); dot = fmaf(a.y, g.y, dot); dot = fmaf(a.z, g.z, dot); dot = fmaf(a.w, g.w, dot);
+  } else if (quad) {
+    for (int d = lane * 4; d < dim; d += 128) for (int e = 0; e < 4; ++e) dot = fmaf(yr[d + e], gr[d + e], dot);
   } else for (int d = lane; d < dim; d += 32) dot = fmaf(yr[d], gr[d], dot);
   dot = warp_sum(dot);
   const float inv = inv_norm[r];

@@ -30,6 +30,32 @@ def test_standalone_forward_backward(oracle):
         assert not y.cpu().numpy()[R // 2].any() and not dx.cpu().numpy()[R // 2].any()
 
 
+@pytest.mark.parametrize("R,D", [(64, 128), (1000, 200), (7, 3)])
+def test_standalone_buffers_at_any_offset(R, D):
+    """Every buffer 1, 2 or 3 floats into a larger allocation: the 4-byte-load fallback keeps the summation order of the 16-byte
+    path, so y, 1/||x|| and dx are bit for bit those of aligned buffers."""
+    import torch
+    x, _ = _raw_inputs(R, D, 5 + R)
+    dy = np.random.default_rng(R + 1).standard_normal((R, D)).astype(np.float32)
+    xt, dyt = torch.from_numpy(x).cuda(), torch.from_numpy(dy).cuda()
+    y0, inv0 = capi.l2normalize_forward(xt)
+    dx0 = capi.l2normalize_backward(y0, inv0, dyt)
+    L, st = capi.lib(), torch.cuda.current_stream().cuda_stream
+    for off in (1, 2, 3):
+        def at(t):
+            buf = torch.full((t.numel() + off,), float("nan"), dtype=torch.float32, device="cuda")
+            v = buf[off:].view(t.shape)
+            v.copy_(t)
+            return v
+        xv, dyv, y, dx = at(xt), at(dyt), at(torch.empty_like(xt)), at(torch.empty_like(xt))
+        inv = at(torch.empty_like(inv0))
+        assert L.npair_l2normalize_forward(xv.data_ptr(), R, D, y.data_ptr(), inv.data_ptr(), st) == 0
+        assert L.npair_l2normalize_backward(y.data_ptr(), inv.data_ptr(), dyv.data_ptr(), R, D, dx.data_ptr(), st) == 0
+        torch.cuda.synchronize()
+        for got, want, what in ((y, y0, "y"), (inv, inv0, "1/||x||"), (dx, dx0, "dx")):
+            assert torch.equal(got.view(torch.int32), want.view(torch.int32)), f"R{R} D{D} offset {off}: {what}"
+
+
 @pytest.mark.parametrize("B,D,mining", [(512, 128, "usage"), (1000, 200, "default"), (2048, 512, "usage")])
 def test_fused_normalize_input_world1(oracle, B, D, mining):
     import torch

@@ -108,6 +108,17 @@ def test_blocks_every_accepted_mining(mining):
     _compare(x, lab, Q, 1, 256, f"{mining}", **mining)
 
 
+@pytest.mark.parametrize("Q,D,height,chunk", [(999, 101, 256, 0), (999, 101, 384, 0), (1001, 130, 256, 64)])
+def test_blocks_ragged_shapes(Q, D, height, chunk):
+    """Q*D % 4 != 0 and a short last block (231 or 233 rows): every block's split-K reduce sums slices that are not 16-byte
+    aligned, and D = 101 takes the gradient drain's scalar stores.  grad_chunk_cols = 64 puts the chunk key's m_blk0 term (the
+    block's first 128-row tile) into the first chunk of every tile."""
+    from npairloss_b200 import synth
+    x, lab = _inputs(Q, D=D, seed=Q + D)
+    lab[-1] = lab[-2]                   # an odd batch's last image joins the class before it: every row has a positive
+    _compare(x, lab, Q, 1, height, f"Q{Q} D{D} h{height} chunk{chunk}", grad_chunk_cols=chunk, **synth.USAGE_MINING)
+
+
 def test_blocks_every_accepted_mining_world2():
     from npairloss_b200 import synth
     Q = 600
