@@ -4,14 +4,11 @@ on planted blobs; repeatability; the torch API's NMI / F1 against a numpy oracle
 import numpy as np
 import pytest
 
+from eval_ref import cuda, update_ref
+
 pytestmark = pytest.mark.gpu
 
 PRECS = (0, 1, 2)          # capi.PREC_FP32_BF16X3, PREC_BF16, PREC_FP32_FP16X2
-
-
-def _cuda(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def _unit_rows(n, D, rng):
@@ -40,26 +37,6 @@ def _kmeans(x, k, init, max_iter, prec, ev=None):
             ev.close()
 
 
-def _sigma_exp(x):
-    """e with pre_scale(max|x|) = 2^-e (max|x| = m 2^e, m in [0.5, 1))"""
-    return int(np.frexp(np.float32(np.abs(x).max()))[1])
-
-
-def _update_ref(x, assign, C):
-    """The header's fixed-point update: int64 sums of rint(x * sigma * 2^32), then (float)(ldexp(sum / count, -32) * 2^e); an empty
-    cluster keeps its centroid."""
-    e = _sigma_exp(x)
-    q = np.rint((x * np.float32(2.0 ** -e)).astype(np.float64) * 2.0 ** 32).astype(np.int64)
-    k = C.shape[0]
-    S = np.zeros((k, x.shape[1]), np.int64)
-    np.add.at(S, assign, q)
-    cnt = np.bincount(assign, minlength=k)
-    out = C.copy()
-    ne = cnt > 0
-    out[ne] = (np.ldexp(S[ne].astype(np.float64) / cnt[ne, None], -32) * 2.0 ** e).astype(np.float32)
-    return out
-
-
 def test_first_assignment_exact_with_planted_ties():
     """Entries k/8: every similarity, bias and score is exact in every format, so the assignment is the int64 argmax, lowest index on
     ties.  Centroid pairs with identical vectors (a copied row, a repeated init index) tie for every point: the higher one is empty."""
@@ -77,7 +54,7 @@ def test_first_assignment_exact_with_planted_ties():
     want = np.argmax(score, axis=1)                    # first maximum: lowest index
     planted = [7, 20, 299, 150, 200]
     assert not np.isin(planted, want).any()
-    xt = _cuda(x)
+    xt = cuda(x)
     for prec in PRECS:
         r = _kmeans(xt, k, init.tolist(), 1, prec)
         np.testing.assert_array_equal(r["assign"], want, err_msg=f"prec {prec}")
@@ -96,12 +73,12 @@ def test_update_rule_bit_for_bit(prec):
     x = _lowdim(n, D, rng)
     init = rng.choice(n, size=k, replace=False)
     init[250] = init[5]
-    xt = _cuda(x)
+    xt = cuda(x)
     prev = _kmeans(xt, k, init.tolist(), 1, prec)
     for t in range(1, 5):
         nxt = _kmeans(xt, k, init.tolist(), t + 1, prec)
         assert prev["stats"][0] == t and nxt["stats"][0] == t + 1, (t, prev["stats"], nxt["stats"])
-        want = _update_ref(x, prev["assign"], prev["centroids"])
+        want = update_ref(x, prev["assign"], prev["centroids"])
         np.testing.assert_array_equal(nxt["centroids"].view(np.uint32), want.view(np.uint32), err_msg=f"t={t}")
         empty = np.setdiff1d(np.arange(k), prev["assign"])
         if t == 1:
@@ -167,7 +144,7 @@ def test_assignment_is_argmin_after_updates(prec):
     rng = np.random.default_rng(20260813 + prec)
     x = _lowdim(n, D, rng)
     init = rng.choice(n, size=k, replace=False)
-    xt = _cuda(x)
+    xt = cuda(x)
     r = _kmeans(xt, k, init.tolist(), 5, prec)
     assert r["stats"][0] == 5
     exact = _check_argmin(prec, xt, r["assign"], r["centroids"])
@@ -189,7 +166,7 @@ def test_converges_on_planted_blobs(prec):
     rng = np.random.default_rng(20260814 + prec)
     x, lab = _blobs(n_per, k, D, rng)
     init = [c * n_per + int(rng.integers(n_per)) for c in range(k)]      # one row per blob, in blob order
-    xt = _cuda(x)
+    xt = cuda(x)
     r = _kmeans(xt, k, init, 20, prec)
     it, changed, empty = r["stats"]
     assert changed == 0 and it < 20 and empty == 0, r["stats"]
@@ -208,7 +185,7 @@ def test_repeatable(prec):
     rng = np.random.default_rng(20260815 + prec)
     x = _unit_rows(n, D, rng)
     init = rng.choice(n, size=k, replace=False).tolist()
-    xt = _cuda(x)
+    xt = cuda(x)
     ev = capi.Evaluator(n, k, D, prec)
     try:
         runs = [_kmeans(xt, k, init, 8, prec, ev), _kmeans(xt, k, init, 8, prec, ev)]
@@ -250,7 +227,7 @@ def test_clustering_metrics_api():
     lab = np.repeat(np.arange(n_lab), per).astype(np.float32) * 3.0 - 7.0
     x = centers[np.repeat(np.arange(n_lab), per)] + 0.35 * rng.standard_normal((n_lab * per, D)).astype(np.float32)
     x = (x / np.linalg.norm(x, axis=1, keepdims=True)).astype(np.float32)
-    xt, lt = _cuda(x), _cuda(lab).to(torch.int64)
+    xt, lt = cuda(x), cuda(lab).to(torch.int64)
     out, assign, cent = clustering_metrics(xt, lt, seed=3)
     assert cent.shape == (n_lab, D) and assign.shape == (n_lab * per,)           # k=None: the number of labels
     nmi, f1 = _nmi_f1_ref(lab, assign.cpu().numpy())
@@ -287,7 +264,7 @@ def test_sop_sized_run():
     centers = _unit_rows(k, D, rng)
     x = centers[rng.integers(0, k, size=n)] + 0.6 * rng.standard_normal((n, D)).astype(np.float32) / np.sqrt(D)
     x = (x / np.linalg.norm(x, axis=1, keepdims=True)).astype(np.float32)
-    xt = _cuda(x)
+    xt = cuda(x)
     init = rng.choice(n, size=k, replace=False).tolist()
     ws, km = capi.eval_workspace_bytes(n, k, D, prec), capi.eval_kmeans_bytes(n, k, D)
     _kmeans(xt[:512], 16, list(range(16)), 2, prec)                            # loads the kernels

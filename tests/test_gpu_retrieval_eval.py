@@ -4,42 +4,11 @@ similarities, agreement with the layer's retrieval tops, and a set whose similar
 import numpy as np
 import pytest
 
+from eval_ref import cuda, map_ref, planted
+
 pytestmark = pytest.mark.gpu
 
 PRECS = (0, 1, 2)          # capi.PREC_FP32_BF16X3, PREC_BF16, PREC_FP32_FP16X2
-
-
-def _cuda(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _ranks_exact(Sq, ql, gl, self_offset):
-    """int64 brute force: rank_i = #{j != self : s_ij >= p*_i}, 0 without a positive."""
-    nq, ng = Sq.shape
-    valid = np.ones((nq, ng), bool)
-    if self_offset >= 0:
-        valid[np.arange(nq), self_offset + np.arange(nq)] = False
-    same = (ql[:, None] == gl[None, :]) & valid
-    out = np.zeros(nq, np.int64)
-    for i in range(nq):
-        if same[i].any():
-            p = Sq[i][same[i]].max()
-            out[i] = int(((Sq[i] >= p) & valid[i]).sum())
-    return out
-
-
-def _planted(n, D, n_cls, rng):
-    """Entries k/8 with integer k in [-8, 8] (every similarity exact in every operand format), some rows duplicated under another
-    label so that equal scores tie with the best positive, and a few singleton labels (no positive)."""
-    K = rng.integers(-8, 9, size=(n, D)).astype(np.int64)
-    lab = rng.integers(0, n_cls, size=n).astype(np.float32)
-    for a, b in rng.integers(0, n, size=(n // 6, 2)):
-        if a != b:
-            K[b] = K[a]
-            lab[b] = lab[a] + 1000.0
-    lab[rng.integers(0, n, size=5)] = 5000.0 + np.arange(5)
-    return K, lab
 
 
 @pytest.mark.parametrize("prec", PRECS)
@@ -48,28 +17,28 @@ def test_exact_ranks_with_planted_ties(prec):
     rng = np.random.default_rng(20171225 + prec)
     # self-retrieval, ragged n and D
     n, D = 301, 37
-    K, lab = _planted(n, D, 60, rng)
+    K, lab = planted(n, D, 60, rng)
     x = (K / 8.0).astype(np.float32)
     ev = capi.Evaluator(n, n, D, prec)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     got = ev.rank(xt, lt, xt, lt, 0).cpu().numpy()
-    want = _ranks_exact(K @ K.T, lab, lab, 0)
+    want = map_ref(K @ K.T, lab, lab, 0)[3]
     assert (want > 1).sum() > 10 and (want == 0).sum() >= 5
     np.testing.assert_array_equal(got, want)
     ev.close()
     # query / gallery: disjoint sets, and queries that are a subset of the gallery
     nq, ng, D = 157, 389, 61
-    Kg, lg = _planted(ng, D, 50, rng)
+    Kg, lg = planted(ng, D, 50, rng)
     Kq = rng.integers(-8, 9, size=(nq, D)).astype(np.int64)
     Kq[: nq // 3] = Kg[rng.integers(0, ng, size=nq // 3)]           # exact duplicates of gallery rows
     lq = rng.integers(0, 50, size=nq).astype(np.float32)
     ev = capi.Evaluator(nq, ng, D, prec)
-    qt, qlt, gt, glt = _cuda((Kq / 8.0).astype(np.float32)), _cuda(lq), _cuda((Kg / 8.0).astype(np.float32)), _cuda(lg)
-    np.testing.assert_array_equal(ev.rank(qt, qlt, gt, glt, -1).cpu().numpy(), _ranks_exact(Kq @ Kg.T, lq, lg, -1))
+    qt, qlt, gt, glt = cuda((Kq / 8.0).astype(np.float32)), cuda(lq), cuda((Kg / 8.0).astype(np.float32)), cuda(lg)
+    np.testing.assert_array_equal(ev.rank(qt, qlt, gt, glt, -1).cpu().numpy(), map_ref(Kq @ Kg.T, lq, lg, -1)[3])
     k = 101
     sub, subl = gt[k:k + nq].contiguous(), glt[k:k + nq].contiguous()
     np.testing.assert_array_equal(ev.rank(sub, subl, gt, glt, k).cpu().numpy(),
-                                  _ranks_exact(Kg[k:k + nq] @ Kg.T, lg[k:k + nq], lg, k))
+                                  map_ref(Kg[k:k + nq] @ Kg.T, lg[k:k + nq], lg, k)[3])
     ev.close()
 
 
@@ -79,7 +48,7 @@ def test_ranks_within_fp64_bounds(prec, D):
     from npairloss_b200 import capi, synth
     n = 2000
     x, lab = synth.make_inputs(n, D, 20171226 + D, imgs_per_class=4, noise=1.5)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     rank = ev.rank(xt, lt, xt, lt, 0).cpu().numpy()
     ev.close()
@@ -103,7 +72,7 @@ def test_symmetric_tiles_equal_full_tiles(prec):
         pytest.skip("this device's MMA is not bitwise symmetric in this operand format")
     n, D = 1000, 96
     x, lab = synth.make_inputs(n, D, 20171227, imgs_per_class=3, noise=2.0)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     r_sym = ev.rank(xt, lt, xt, lt, 0)
     r_full = ev.rank(xt, lt, xt.clone(), lt.clone(), 0)      # another buffer: every tile is computed
@@ -118,7 +87,7 @@ def test_sharded_gallery_equals_one_call(prec):
     from npairloss_b200 import capi, synth
     n, D = 1100, 64
     x, lab = synth.make_inputs(n, D, 20171228, imgs_per_class=4, noise=2.0)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     bounds = [0, 170, 777, n]                                  # three uneven shards
     ev = capi.Evaluator(n, n, D, prec)
     # the first 400 rows as queries against the rest (disjoint), and self-retrieval, whose one call computes only the tiles of the
@@ -151,7 +120,7 @@ def test_sees_the_layers_similarities(prec):
     x = rng.standard_normal((n, D)).astype(np.float32)
     x /= np.linalg.norm(x, axis=1, keepdims=True)
     lab = rng.integers(0, n // 3, size=n).astype(np.float32)           # about 3 rows per label, some without a positive
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ctx = capi.Context(capi.make_config(n, D, sim_precision=prec))
     ctx.forward(xt, lt)
     S = ctx.debug_read(0, n * n).reshape(n, n)
@@ -174,7 +143,7 @@ def test_agrees_with_layer_tops():
     from npairloss_b200.torch_api import recall_at_k
     Q, D = 2048, 128
     x, lab = synth.make_inputs(Q, D, 20171229, noise=1.5)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ctx = capi.Context(capi.make_config(Q, D))
     tops = ctx.forward(xt, lt)
     ctx.close()
@@ -189,7 +158,7 @@ def test_recall_api_modes():
     from npairloss_b200 import capi, synth
     from npairloss_b200.torch_api import recall_at_k
     x, lab = synth.make_inputs(600, 64, 20171231, imgs_per_class=3, noise=2.0)
-    xt, lt = _cuda(x), _cuda(lab).long()
+    xt, lt = cuda(x), cuda(lab).long()
     rec, rank = recall_at_k(xt, lt)
     assert list(rec) == [1, 2, 4, 8] and all(0.0 <= v <= 1.0 for v in rec.values())
     assert rec[1] <= rec[2] <= rec[4] <= rec[8]
@@ -208,7 +177,7 @@ def test_batch_beyond_similarity_matrix():
     from npairloss_b200 import capi, synth
     B, D = 196608, 128
     x, lab = synth.make_inputs(B, D, 20171232, imgs_per_class=4, noise=1.5)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     del x
     ws = capi.eval_workspace_bytes(B, B, D)
     capi.Evaluator(256, 256, D).close()                        # loads the module

@@ -4,71 +4,11 @@ agreement with fp64 similarities; and a set whose similarity matrix would not fi
 import numpy as np
 import pytest
 
+from eval_ref import check_map, cuda, map_ref, planted
+
 pytestmark = pytest.mark.gpu
 
 PRECS = (0, 1, 2)          # capi.PREC_FP32_BF16X3, PREC_BF16, PREC_FP32_FP16X2
-
-
-def _cuda(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _map_ref(S, ql, gl, self_offset):
-    """Host loop of the header's definitions: (map_r, r_precision, R, rank) per query.  S is exact (int64) or the library's fp32
-    similarities; MAP@R is summed in fp64 in ascending k and divided by R last, as the library does."""
-    nq, ng = S.shape
-    valid = np.ones((nq, ng), bool)
-    if self_offset >= 0:
-        valid[np.arange(nq), self_offset + np.arange(nq)] = False
-    eq = ql[:, None] == gl[None, :]
-    same, neg = eq & valid, ~eq & valid
-    map_r, r_prec = np.full(nq, np.nan), np.full(nq, np.nan)
-    R, rank = same.sum(1).astype(np.int32), np.zeros(nq, np.int32)
-    for i in range(nq):
-        if R[i] == 0:
-            continue
-        p = np.sort(S[i][same[i]])[::-1]
-        sn = np.sort(S[i][neg[i]])
-        neg_ge = len(sn) - np.searchsorted(sn, p, side="left")       # negatives >= p_k
-        total, hits = 0.0, 0
-        for k in range(1, R[i] + 1):
-            pk = k + int(neg_ge[k - 1])
-            if pk > R[i]:
-                break
-            total += k / pk
-            hits += 1
-        map_r[i], r_prec[i] = total / int(R[i]), hits / int(R[i])
-        rank[i] = int((p == p[0]).sum()) + int(neg_ge[0])
-    return map_r, r_prec, R, rank
-
-
-def _bits_equal(got, want):
-    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
-    np.testing.assert_array_equal(np.isnan(got), np.isnan(want))
-    ok = ~np.isnan(want)
-    np.testing.assert_array_equal(got[ok].view(np.uint64), want[ok].view(np.uint64))
-
-
-def _check(out, ref):
-    m, rp, R, rank = ref
-    _bits_equal(out["map_r"].cpu().numpy(), m)
-    _bits_equal(out["r_precision"].cpu().numpy(), rp)
-    np.testing.assert_array_equal(out["R"].cpu().numpy(), R)
-    np.testing.assert_array_equal(out["rank"].cpu().numpy(), rank)
-
-
-def _planted(n, D, n_cls, rng):
-    """As in test_gpu_retrieval_eval: entries k/8 (every similarity exact in every format), duplicated rows under another label so that
-    negatives tie positives, and a few singleton labels (no positive)."""
-    K = rng.integers(-8, 9, size=(n, D)).astype(np.int64)
-    lab = rng.integers(0, n_cls, size=n).astype(np.float32)
-    for a, b in rng.integers(0, n, size=(n // 6, 2)):
-        if a != b:
-            K[b] = K[a]
-            lab[b] = lab[a] + 1000.0
-    lab[rng.integers(0, n, size=5)] = 5000.0 + np.arange(5)
-    return K, lab
 
 
 @pytest.mark.parametrize("prec", PRECS)
@@ -77,30 +17,30 @@ def test_exact_map_with_planted_ties(prec):
     from npairloss_b200 import capi
     rng = np.random.default_rng(20171301 + prec)
     n, D = 301, 37
-    K, lab = _planted(n, D, 40, rng)
-    xt, lt = _cuda((K / 8.0).astype(np.float32)), _cuda(lab)
+    K, lab = planted(n, D, 40, rng)
+    xt, lt = cuda((K / 8.0).astype(np.float32)), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     out = ev.map_at_r(xt, lt, xt, lt, 0)
-    ref = _map_ref(K @ K.T, lab, lab, 0)
+    ref = map_ref(K @ K.T, lab, lab, 0)
     assert (ref[2] == 0).sum() >= 5 and (ref[2] >= 3).sum() > 50 and (ref[0][ref[2] > 0] < 1).sum() > 20
-    _check(out, ref)
+    check_map(out, ref)
     assert torch.equal(out["rank"], ev.rank(xt, lt, xt, lt, 0))
     ev.close()
     # disjoint sets, and queries that are a subset of the gallery
     nq, ng, D = 157, 389, 61
-    Kg, lg = _planted(ng, D, 30, rng)
+    Kg, lg = planted(ng, D, 30, rng)
     Kq = rng.integers(-8, 9, size=(nq, D)).astype(np.int64)
     Kq[: nq // 3] = Kg[rng.integers(0, ng, size=nq // 3)]
     lq = rng.integers(0, 30, size=nq).astype(np.float32)
     ev = capi.Evaluator(nq, ng, D, prec)
-    qt, qlt, gt, glt = _cuda((Kq / 8.0).astype(np.float32)), _cuda(lq), _cuda((Kg / 8.0).astype(np.float32)), _cuda(lg)
+    qt, qlt, gt, glt = cuda((Kq / 8.0).astype(np.float32)), cuda(lq), cuda((Kg / 8.0).astype(np.float32)), cuda(lg)
     out = ev.map_at_r(qt, qlt, gt, glt, -1)
-    _check(out, _map_ref(Kq @ Kg.T, lq, lg, -1))
+    check_map(out, map_ref(Kq @ Kg.T, lq, lg, -1))
     assert torch.equal(out["rank"], ev.rank(qt, qlt, gt, glt, -1))
     k = 101
     sub, subl = gt[k:k + nq].contiguous(), glt[k:k + nq].contiguous()
     out = ev.map_at_r(sub, subl, gt, glt, k)
-    _check(out, _map_ref(Kg[k:k + nq] @ Kg.T, lg[k:k + nq], lg, k))
+    check_map(out, map_ref(Kg[k:k + nq] @ Kg.T, lg[k:k + nq], lg, k))
     assert torch.equal(out["rank"], ev.rank(sub, subl, gt, glt, k))
     ev.close()
 
@@ -114,7 +54,7 @@ def test_map_on_the_layers_similarities(prec):
     x = rng.standard_normal((n, D)).astype(np.float32)
     x /= np.linalg.norm(x, axis=1, keepdims=True)
     lab = rng.integers(0, n // 6, size=n).astype(np.float32)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ctx = capi.Context(capi.make_config(n, D, sim_precision=prec))
     ctx.forward(xt, lt)
     S = ctx.debug_read(0, n * n).reshape(n, n)
@@ -122,9 +62,9 @@ def test_map_on_the_layers_similarities(prec):
     ev = capi.Evaluator(n, n, D, prec)
     out = ev.map_at_r(xt, lt, xt, lt, 0)
     ev.close()
-    ref = _map_ref(S, lab, lab, 0)
+    ref = map_ref(S, lab, lab, 0)
     assert (ref[2] >= 4).sum() > 100
-    _check(out, ref)
+    check_map(out, ref)
 
 
 @pytest.mark.parametrize("prec", PRECS)
@@ -136,7 +76,7 @@ def test_symmetric_tiles_equal_full_tiles(prec):
     n, D = 1000, 96
     x, lab = synth.make_inputs(n, D, 20171303, imgs_per_class=7, noise=2.0)
     lab[::97] = -1.0 - np.arange(len(lab[::97]))                     # some queries without a positive
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     a = ev.map_at_r(xt, lt, xt, lt, 0)
     b = ev.map_at_r(xt, lt, xt.clone(), lt.clone(), 0)                # another buffer: every tile is computed
@@ -155,23 +95,23 @@ def test_long_lists_repeatable_and_no_positive(prec):
     K = rng.integers(-8, 9, size=(n, D)).astype(np.int64)
     K[:3000] += 3 * rng.integers(-1, 2, size=(10, D)).astype(np.int64)[np.arange(3000) // 300]   # a weak class structure
     lab = np.concatenate([np.arange(3000) // 300, 100 + np.arange(10)]).astype(np.float32)
-    xt, lt = _cuda((K / 8.0).astype(np.float32)), _cuda(lab)
+    xt, lt = cuda((K / 8.0).astype(np.float32)), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     a = ev.map_at_r(xt, lt, xt, lt, 0)
     b = ev.map_at_r(xt, lt, xt, lt, 0)
-    ref = _map_ref(K @ K.T, lab, lab, 0)
+    ref = map_ref(K @ K.T, lab, lab, 0)
     ev.close()
     for k in a:
         assert a[k].cpu().numpy().tobytes() == b[k].cpu().numpy().tobytes(), k
     assert (ref[2][:3000] == 299).all() and (ref[2][3000:] == 0).all()
     assert 0.05 < np.nanmean(ref[0]) < 0.95
-    _check(a, ref)
+    check_map(a, ref)
     assert np.isnan(a["map_r"].cpu().numpy()[3000:]).all() and np.isnan(a["r_precision"].cpu().numpy()[3000:]).all()
 
 
 def _map_fp64(x, lab):
     S = x.astype(np.float64) @ x.astype(np.float64).T
-    return _map_ref(S, lab, lab, 0)[0]
+    return map_ref(S, lab, lab, 0)[0]
 
 
 @pytest.mark.parametrize("prec", (0, 2))
@@ -180,7 +120,7 @@ def test_mean_map_against_fp64(prec, D):
     from npairloss_b200 import capi, synth
     n = 2000
     x, lab = synth.make_inputs(n, D, 20171305 + D, imgs_per_class=8, noise=2.5)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     ev = capi.Evaluator(n, n, D, prec)
     got = ev.map_at_r(xt, lt, xt, lt, 0)["map_r"].cpu().numpy()
     ev.close()
@@ -195,7 +135,7 @@ def test_retrieval_metrics_api():
     from npairloss_b200.torch_api import recall_at_k, retrieval_metrics
     x, lab = synth.make_inputs(600, 64, 20171306, imgs_per_class=3, noise=2.0)
     lab[:4] = [900.0, 901.0, 902.0, 903.0]                             # four queries without a positive
-    xt, lt = _cuda(x), _cuda(lab).long()
+    xt, lt = cuda(x), cuda(lab).long()
     res, per = retrieval_metrics(xt, lt, ks=(1, 5))
     rec, rank = recall_at_k(xt, lt, ks=(1, 5))
     assert torch.equal(per["rank"], rank)
@@ -215,7 +155,7 @@ def test_batch_beyond_similarity_matrix():
     from npairloss_b200 import capi, synth
     B, D, imgs = 196608, 128, 4
     x, lab = synth.make_inputs(B, D, 20171307, imgs_per_class=imgs, noise=1.5)
-    xt, lt = _cuda(x), _cuda(lab)
+    xt, lt = cuda(x), cuda(lab)
     del x
     ws = capi.eval_workspace_bytes(B, B, D)
     capi.Evaluator(256, 256, D).close()                                # loads the module
