@@ -465,13 +465,7 @@ static int select_mask(const npair_config& c, int region) {
          (c.an_region == region && is_rel(c.an_method) && !sn_is_max(c.diffsn) ? 2 : 0);
 }
 
-// device buffers of a context
-enum { B_XTOT, B_LABTOT, B_YNORM, B_DY, B_INV_NORM, B_S, B_XS, B_XST, B_XCAT_A, B_XCAT_B, B_H, B_XLT, B_HT, B_OUT2, B_RS_TOTAL,
-       B_PART, B_ROWS, B_BS, B_PARTIAL, B_GHIST, B_GCAND, B_SYM_TILES, B_XCH_SRC, B_XCH_ALL, B_P2P_REGION, B_P2P_TICKET, B_P2P_PEERS,
-       B_COUNT };
-
-// What a context decides from its configuration and two device facts, and the byte size of every device buffer it allocates
-// (0: not allocated).  The peer-memory exchange buffers are sized as if the context had a communicator and peer access.
+// What a context decides from its configuration and two device facts (ctx_buffers sizes its device buffers from these decisions)
 struct Plan {
   int N, nsplit, bk_grad;
   long long Dp, Np, Qp, ldS;     // padded feature / all-rows / local-rows extents of the operand pieces, row stride of S
@@ -492,7 +486,6 @@ struct Plan {
   int lsel_mask, gsel_mask;      // radix selects (select_mask) of the LOCAL / GLOBAL region
   bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
   XchgLayout xl;
-  size_t bytes[B_COUNT];
 };
 
 static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
@@ -535,39 +528,71 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
   p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
   if (p.want_p2p_feat || p.want_p2p_rec) p.xl = xchg_layout(cfg.Q, cfg.D, W, p.wscope);
-
-  size_t* b = p.bytes;
-  const size_t f = sizeof(float), ns = p.nsplit;
-  if (multi) { b[B_XTOT] = f * N * D; b[B_LABTOT] = f * N; }                    // all-gather targets
-  if (cfg.normalize_input) { b[B_YNORM] = b[B_DY] = f * Q * D; b[B_INV_NORM] = f * Q; }   // y, dy, 1/||x||
-  b[B_S] = f * p.s_rows * p.ldS;
-  if (!p.cat) b[B_XS] = 2 * ns * N * p.Dp;                                      // operand pieces [ns][N][Dp]
-  b[B_XST] = 2 * ns * D * p.Np;                                                 // transposed pieces [ns][D][Np]
-  if (p.cat) b[B_XCAT_A] = b[B_XCAT_B] = 2 * N * p.kcat;                         // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
-  if (!p.fused_grad) b[B_H] = 2 * ns * Q * p.Np;                                // materialised gradient weights
-  if (rs) { b[B_XLT] = 2 * ns * D * p.Qp; b[B_HT] = 2 * ns * N * p.Qp; b[B_OUT2] = f * N * D; }
-  if (p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) b[B_RS_TOTAL] = sizeof(RowRecord) * N;   // gathered row records
-  if (p.grad_split.splits > 1) b[B_PART] = f * split_part(p.grad_split.splits, cfg.Q, D);   // split-K partial products
-  b[B_ROWS] = (4 * 13 + sizeof(RowRecord)) * Q + 64;   // 13 row arrays of Q 4-byte words (RowArrays) + the 32-byte aligned row records
-  b[B_BS] = sizeof(BlockScalars);
-  b[B_PARTIAL] = f * 2048;
-  b[B_GHIST] = sizeof(unsigned long long) * 4096;
-  b[B_GCAND] = sizeof(uint32_t) * 2ull * p.gcand_cap;
-  b[B_SYM_TILES] = sizeof(int2) * p.n_sym_tiles;
-  if (p.wscope) { b[B_XCH_SRC] = f * NPAIR_XCH_FLOATS; b[B_XCH_ALL] = f * NPAIR_XCH_FLOATS * W; }   // the latter for NCCL
-  if (p.want_p2p_feat || p.want_p2p_rec) {
-    b[B_P2P_REGION] = f * p.xl.floats; b[B_P2P_TICKET] = sizeof(unsigned int); b[B_P2P_PEERS] = sizeof(float*) * W;
-  }
   return p;
 }
 
-// cudaMalloc of a planned buffer: nothing for 0 bytes, optionally zero-filled
-template <class T>
-static cudaError_t dev_alloc(T** p, size_t bytes, bool zero) {
-  if (bytes == 0) return cudaSuccess;
-  cudaError_t e = cudaMalloc(p, bytes);
-  if (e == cudaSuccess && zero) e = cudaMemset(*p, 0, bytes);
-  return e;
+// ------------------------------------------------------------------------------------------------ device memory
+// Bump carver of a buffer cut into several arrays: take<T>(count, align) returns the next `count` T at an `align`-byte offset.  Over a
+// null base it only measures, so the one function that cuts a region also gives its size (`bytes` after the last take).
+struct Carve {
+  char* base;
+  size_t bytes = 0;
+  template <class T>
+  T* take(long long count, size_t align = alignof(T)) {
+    bytes = (bytes + align - 1) / align * align;
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += sizeof(T) * count;
+    return p;
+  }
+};
+
+// The device buffers of a context or an evaluator, listed once each (ctx_buffers, eval_buffers) and run through one of two modes.
+// Sizing only adds up their bytes.  Allocating gives every buffer a cudaMalloc of its own, zero-filled when asked, and frees them
+// all in release() or the destructor.  After a failure own() does nothing more: the list runs to its end and `err` holds the first.
+struct DevMem {
+  explicit DevMem(bool allocate = true) : allocate(allocate) {}
+  DevMem(const DevMem&) = delete;
+  ~DevMem() { release(); }
+  // *p = a buffer of `n` bytes (null if its cudaMalloc fails); 0 bytes: none
+  template <class T>
+  void own(T** p, size_t n, bool zero) {
+    if (n == 0 || err != cudaSuccess) return;
+    bytes += n;
+    if (!allocate) return;
+    if ((err = cudaMalloc(p, n)) != cudaSuccess) { *p = nullptr; return; }
+    held.push_back(*p);
+    if (zero) err = cudaMemset(*p, 0, n);
+  }
+  // One buffer for a region that `carve(Carve&)` cuts into arrays: carved over a null base to measure it, then over the buffer
+  template <class F>
+  void own_carved(bool zero, F carve) {
+    Carve size{nullptr}, cut{nullptr};
+    carve(size);
+    own(&cut.base, size.bytes, zero);
+    carve(cut);
+  }
+  void release() {
+    for (void* q : held) cudaFree(q);
+    held.clear(); bytes = 0; err = cudaSuccess;
+  }
+  const bool allocate;
+  size_t bytes = 0;                   // of the buffers listed (and held) so far
+  cudaError_t err = cudaSuccess;
+  std::vector<void*> held;
+};
+
+// The statistics of RowArrays, which the evaluator's queries have too: four ordered-uint statistics and the same-label count per row
+static void carve_stats(Carve& cv, long long rows, RowArrays* ra) {
+  ra->st_minw = cv.take<uint32_t>(rows); ra->st_maxw = cv.take<uint32_t>(rows); ra->st_maxb = cv.take<uint32_t>(rows);
+  ra->st_maxall = cv.take<uint32_t>(rows); ra->cnt_same = cv.take<int>(rows);
+}
+// A context's RowArrays: the statistics, thresholds, row results and [3][Q] hit flags, then the row records 32-byte aligned
+static void carve_rows(Carve& cv, long long Q, RowArrays* ra) {
+  carve_stats(cv, Q, ra);
+  ra->posi_thr = cv.take<float>(Q); ra->nega_thr = cv.take<float>(Q);
+  ra->A = cv.take<float>(Q); ra->T = cv.take<float>(Q); ra->logv = cv.take<float>(Q);
+  ra->hits = cv.take<int>(3 * Q);
+  ra->rowrec = cv.take<RowRecord>(Q, 32);
 }
 
 // ------------------------------------------------------------------------------------------------ context
@@ -575,7 +600,7 @@ static cudaError_t dev_alloc(T** p, size_t bytes, bool zero) {
 struct npair_ctx : Plan {
   npair_config cfg;
   int Q, D, world, rank, prec, sms, device;
-  // device scratch
+  DevMem mem;                    // owns the device scratch below (ctx_buffers, p2p_buffers)
   float* Xtot_buf = nullptr;     // world > 1: all-gather target
   float* labtot_buf = nullptr;
   float* S = nullptr;
@@ -594,15 +619,14 @@ struct npair_ctx : Plan {
   uint32_t xch_epoch = 0;              // small exchanges of the world-scope mode (several per step)
   float* xch_src = nullptr;            // [8192] staging of this rank's contribution
   float* xch_all = nullptr;            // NCCL fallback: gathered [world][8192]
-  float** p2p_peer_base = nullptr;     // device array [world] of the ranks' regions; set only once every peer's region is mapped
+  float** p2p_peer_base = nullptr;     // device array [world] of the ranks' regions; filled once every peer's region is mapped
   unsigned int* p2p_ticket = nullptr;
   std::vector<void*> p2p_opened;
   uint32_t p2p_fwd_epoch = 0, p2p_rec_epoch = 0;
   int2* sym_tiles = nullptr;     // world == 1: (m_blk, n_blk) of the similarity tiles touching the upper triangle
   int s_block_row0 = -1;         // row-block similarity mode: first row of the block S holds (-1: none)
   float* part = nullptr;         // split-K partial products of the gradient GEMM
-  void* row_block = nullptr;     // backing store of RowArrays
-  RowArrays ra;
+  RowArrays ra;                  // one buffer (row_arrays_at)
   BlockScalars* bs = nullptr;
   float* partial = nullptr;
   unsigned long long* ghist = nullptr;   // [2][2048] 64-bit digit counts of the GLOBAL radix select
@@ -627,6 +651,38 @@ struct npair_ctx : Plan {
   bool ev_used[NPAIR_PROF_PHASES] = {};
 };
 
+// The device buffers of a context with its configuration and plan, each with its size and zero-fill; returns the first failure
+static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
+  const long long Q = c->cfg.Q, D = c->cfg.D, N = c->N;
+  const size_t f = sizeof(float), ns = c->nsplit;
+  if (c->cfg.world > 1) { m.own(&c->Xtot_buf, f * N * D, false); m.own(&c->labtot_buf, f * N, false); }   // all-gather targets
+  if (c->cfg.normalize_input) { m.own(&c->Ynorm, f * Q * D, false); m.own(&c->dY, f * Q * D, false); m.own(&c->inv_norm, f * Q, false); }   // y, dy, 1/||x||
+  m.own(&c->S, f * c->s_rows * c->ldS, true);
+  if (!c->cat) m.own(&c->Xs, 2 * ns * N * c->Dp, true);                              // operand pieces [ns][N][Dp]
+  m.own(&c->XsT, 2 * ns * D * c->Np, true);                                           // transposed pieces [ns][D][Np]
+  if (c->cat) { m.own(&c->XcatA, 2 * N * c->kcat, true); m.own(&c->XcatB, 2 * N * c->kcat, true); }   // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  if (!c->fused_grad) m.own(&c->H, 2 * ns * Q * c->Np, true);                        // materialised gradient weights
+  if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) { m.own(&c->XlT, 2 * ns * D * c->Qp, true); m.own(&c->HT, 2 * ns * N * c->Qp, true); m.own(&c->OUT2, f * N * D, false); }
+  if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) m.own(&c->rs_total, sizeof(RowRecord) * N, false);   // gathered row records
+  if (c->grad_split.splits > 1) m.own(&c->part, f * split_part(c->grad_split.splits, c->cfg.Q, D), false);   // split-K partial products
+  m.own_carved(true, [c](Carve& cv) { carve_rows(cv, c->cfg.Q, &c->ra); });
+  m.own(&c->bs, sizeof(BlockScalars), true);
+  m.own(&c->partial, f * 2048, false);
+  m.own(&c->ghist, sizeof(unsigned long long) * 4096, true);
+  m.own(&c->gcand, sizeof(uint32_t) * 2ull * c->gcand_cap, false);
+  m.own(&c->sym_tiles, sizeof(int2) * c->n_sym_tiles, false);
+  if (c->wscope) { m.own(&c->xch_src, f * NPAIR_XCH_FLOATS, false); m.own(&c->xch_all, f * NPAIR_XCH_FLOATS * c->cfg.world, false); }   // the latter for NCCL
+  return m.err;
+}
+// The peer-memory exchange buffers of a context with a communicator and peer access: the region the ranks push into (exported whole
+// by cudaIpcGetMemHandle, hence an allocation of its own), the push kernel's ticket and the device array of the ranks' regions
+static cudaError_t p2p_buffers(npair_ctx* c, DevMem& m) {
+  m.own(&c->p2p_region, sizeof(float) * c->xl.floats, true);
+  m.own(&c->p2p_ticket, sizeof(unsigned int), true);
+  m.own(&c->p2p_peer_base, sizeof(float*) * c->cfg.world, false);
+  return m.err;
+}
+
 struct PhaseTimer {
   npair_ctx* c; int ph; cudaStream_t st;
   PhaseTimer(npair_ctx* c_, int ph_, cudaStream_t st_) : c(c_), ph(ph_), st(st_) {
@@ -645,8 +701,8 @@ struct PhaseTimer {
       return NPAIR_E_CUDA;                                                                               \
     }                                                                                                    \
   } while (0)
-// The same while a context or an evaluator is created, before it exists for npair_last_error: the message goes to g_create_err.  The
-// object under construction is held by a unique_ptr, which releases it on the early return.
+// The same while a context or an evaluator is created, before it exists for npair_last_error, and in calls that have neither: the
+// message goes to g_create_err.  An object under construction is held by a unique_ptr, which releases it on the early return.
 #define CREATE_TRY(call)                                                                                 \
   do {                                                                                                   \
     cudaError_t e__ = (call);                                                                            \
@@ -721,10 +777,13 @@ void npair_config_default(npair_config* c, int32_t Q, int32_t D) {
 size_t npair_workspace_bytes(const npair_config* cfg) {
   std::string e;
   if (validate(cfg, &e) != NPAIR_OK) return 0;
-  const Plan p = plan_of(*cfg, NPAIR_H100_SXM_SMS, true);
-  size_t total = 0;
-  for (size_t b : p.bytes) total += b;
-  return total;
+  npair_ctx c;
+  c.cfg = *cfg;
+  static_cast<Plan&>(c) = plan_of(*cfg, NPAIR_H100_SXM_SMS, true);
+  DevMem sizing(false);
+  ctx_buffers(&c, sizing);
+  if (c.want_p2p_feat || c.want_p2p_rec) p2p_buffers(&c, sizing);   // as if the context had a communicator and peer access
+  return sizing.bytes;
 }
 
 const char* npair_last_error(const npair_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
@@ -744,10 +803,8 @@ void npair_destroy(npair_ctx* c) {
   if (!c) return;
   if (c->device >= 0) cudaSetDevice(c->device);
   for (void* q : c->p2p_opened) cudaIpcCloseMemHandle(q);
-  cudaFree(c->p2p_region); cudaFree(c->p2p_peer_base); cudaFree(c->p2p_ticket);
+  c->mem.release();
   if (c->comm && c->own_comm) release_comm(c->comm);
-  cudaFree(c->Xtot_buf); cudaFree(c->labtot_buf); cudaFree(c->S); cudaFree(c->Xs); cudaFree(c->XsT); cudaFree(c->XlT);
-  cudaFree(c->H); cudaFree(c->HT); cudaFree(c->OUT2); cudaFree(c->part); cudaFree(c->sym_tiles); cudaFree(c->XcatA); cudaFree(c->XcatB); cudaFree(c->rs_total); cudaFree(c->row_block); cudaFree(c->bs); cudaFree(c->partial); cudaFree(c->ghist); cudaFree(c->gcand); cudaFree(c->Ynorm); cudaFree(c->dY); cudaFree(c->inv_norm); cudaFree(c->xch_src); cudaFree(c->xch_all);
   if (c->tops_pinned) cudaFreeHost(c->tops_pinned);
   if (c->ev_made) for (int i = 0; i < NPAIR_PROF_PHASES; ++i) { cudaEventDestroy(c->ev[i][0]); cudaEventDestroy(c->ev[i][1]); }
   delete c;
@@ -823,45 +880,10 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym);
   c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
   const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit;
-  const size_t* b = c->bytes;
-  CREATE_TRY(dev_alloc(&c->Xtot_buf, b[B_XTOT], false));
-  CREATE_TRY(dev_alloc(&c->labtot_buf, b[B_LABTOT], false));
-  CREATE_TRY(dev_alloc(&c->Ynorm, b[B_YNORM], false));
-  CREATE_TRY(dev_alloc(&c->dY, b[B_DY], false));
-  CREATE_TRY(dev_alloc(&c->inv_norm, b[B_INV_NORM], false));
-  CREATE_TRY(dev_alloc(&c->S, b[B_S], true));
-  CREATE_TRY(dev_alloc(&c->Xs, b[B_XS], true));
-  CREATE_TRY(dev_alloc(&c->XsT, b[B_XST], true));
-  CREATE_TRY(dev_alloc(&c->XcatA, b[B_XCAT_A], true));
-  CREATE_TRY(dev_alloc(&c->XcatB, b[B_XCAT_B], true));
-  CREATE_TRY(dev_alloc(&c->H, b[B_H], true));
-  CREATE_TRY(dev_alloc(&c->XlT, b[B_XLT], true));
-  CREATE_TRY(dev_alloc(&c->HT, b[B_HT], true));
-  CREATE_TRY(dev_alloc(&c->OUT2, b[B_OUT2], false));
-  CREATE_TRY(dev_alloc(&c->rs_total, b[B_RS_TOTAL], false));
-  CREATE_TRY(dev_alloc(&c->part, b[B_PART], false));
-  CREATE_TRY(dev_alloc(&c->row_block, b[B_ROWS], true));
-  CREATE_TRY(dev_alloc(&c->bs, b[B_BS], true));
-  CREATE_TRY(dev_alloc(&c->partial, b[B_PARTIAL], false));
-  CREATE_TRY(dev_alloc(&c->ghist, b[B_GHIST], true));
-  CREATE_TRY(dev_alloc(&c->gcand, b[B_GCAND], false));
-  CREATE_TRY(dev_alloc(&c->sym_tiles, b[B_SYM_TILES], false));
-  CREATE_TRY(dev_alloc(&c->xch_src, b[B_XCH_SRC], false));
-  CREATE_TRY(dev_alloc(&c->xch_all, b[B_XCH_ALL], false));
-  {
-    uint32_t* w = static_cast<uint32_t*>(c->row_block);
-    RowArrays& ra = c->ra;
-    ra.st_minw = w; w += Q; ra.st_maxw = w; w += Q; ra.st_maxb = w; w += Q; ra.st_maxall = w; w += Q;
-    ra.cnt_same = reinterpret_cast<int*>(w); w += Q;
-    ra.posi_thr = reinterpret_cast<float*>(w); w += Q; ra.nega_thr = reinterpret_cast<float*>(w); w += Q;
-    ra.A = reinterpret_cast<float*>(w); w += Q; ra.T = reinterpret_cast<float*>(w); w += Q; ra.logv = reinterpret_cast<float*>(w); w += Q;
-    ra.hits = reinterpret_cast<int*>(w); w += 3 * Q;
-    w = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(w) + 31) & ~static_cast<uintptr_t>(31));
-    ra.rowrec = reinterpret_cast<RowRecord*>(w);
-  }
+  CREATE_TRY(ctx_buffers(c, c->mem));
   if (c->sym_tiles) {
     const std::vector<int2> tl = sym_tile_list(Q, N);
-    CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), b[B_SYM_TILES], cudaMemcpyHostToDevice));
+    CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), sizeof(int2) * tl.size(), cudaMemcpyHostToDevice));
   }
   CREATE_TRY(cudaHostAlloc(&c->tops_pinned, 64, cudaHostAllocMapped));
   memset(c->tops_pinned, 0, 64);
@@ -904,12 +926,11 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       c->own_comm = true;
     }
   }
-  if (c->comm && b[B_P2P_REGION] && !getenv("NPAIR_NO_P2P")) {
+  if (c->comm && (c->want_p2p_feat || c->want_p2p_rec) && !getenv("NPAIR_NO_P2P")) {
     // one exported region per rank; handles travel over the NCCL communicator once (a 64-byte all-gather)
     NcclApi* api = nccl_api();
     const int W = c->world;
-    CREATE_TRY(dev_alloc(&c->p2p_region, b[B_P2P_REGION], true));
-    CREATE_TRY(dev_alloc(&c->p2p_ticket, b[B_P2P_TICKET], true));
+    CREATE_TRY(p2p_buffers(c, c->mem));
     cudaIpcMemHandle_t mine;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     CREATE_TRY(cudaIpcGetMemHandle(&mine, c->p2p_region));
@@ -934,8 +955,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
       pb[q] = static_cast<float*>(a);
     }
     if (mapped) {
-      CREATE_TRY(dev_alloc(&c->p2p_peer_base, b[B_P2P_PEERS], false));
-      CREATE_TRY(cudaMemcpy(c->p2p_peer_base, pb.data(), b[B_P2P_PEERS], cudaMemcpyHostToDevice));
+      CREATE_TRY(cudaMemcpy(c->p2p_peer_base, pb.data(), sizeof(float*) * W, cudaMemcpyHostToDevice));
       c->p2p_feat = c->want_p2p_feat; c->p2p_rec = c->want_p2p_rec;
     }
     // (no peer access between some pair of GPUs: the NCCL paths are used; every rank takes the same decision only if the
@@ -975,7 +995,7 @@ static const float* p2p_wait(npair_ctx* c, int kind, uint32_t ep, int part, cuda
 // [world][NPAIR_XCH_FLOATS]; all ranks then reduce them in rank order, so decisions are identical everywhere.
 static int xchg_small(npair_ctx* c, const float* src, int n, const float** all, cudaStream_t st) {
   if (src != c->xch_src) CUDA_TRY(c, cudaMemcpyAsync(c->xch_src, src, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-  if (c->p2p_peer_base) {
+  if (c->p2p_feat || c->p2p_rec) {                   // the peers' regions are mapped
     const uint32_t ep = ++c->xch_epoch;
     p2p_push(c, XCHG_SMALL, ep, grid_for(n / 4, 8), c->xch_src, n, XP_XCH, nullptr, 0, XP_XCH, st);
     *all = p2p_wait(c, XCHG_SMALL, ep, XP_XCH, st);
@@ -1520,57 +1540,52 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int ns = SPLIT_FORMATS[precision].pieces, bk = bk_of(precision, EPI_OUT);
   const long long Kp = round_up(K, 64);
-  uint16_t *As = nullptr, *Bs = nullptr, *dummyT = nullptr;
-  BlockScalars* bs = nullptr; float* partial = nullptr;
-  int rc = NPAIR_OK;
   int dev = 0, sms = NPAIR_H100_SXM_SMS;
   cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-#define DG_TRY(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { g_create_err = fmt("%s: %s", #call, cudaGetErrorString(e__)); rc = NPAIR_E_CUDA; goto done; } } while (0)
-  {
-    const long long Mt = round_up(M, 64), Nt = round_up(Nn, 64);
-    const long long tmax = Mt > Nt ? Mt : Nt;
-    DG_TRY(cudaMalloc(&As, 2ull * ns * M * Kp)); DG_TRY(cudaMalloc(&Bs, 2ull * ns * Nn * Kp));
-    DG_TRY(cudaMalloc(&dummyT, 2ull * ns * K * tmax));
-    DG_TRY(cudaMalloc(&bs, sizeof(BlockScalars))); DG_TRY(cudaMemset(bs, 0, sizeof(BlockScalars)));
-    DG_TRY(cudaMalloc(&partial, sizeof(float) * 2048));
-    // one common power-of-two scale over both operands (the layer multiplies X by X^T, i.e. a single matrix), from max|A| and
-    // max|B| as the step's operand preparation finds them (no rows: nothing else is touched)
-    float sc[2] = {1.f, 1.f};                  // x_scale, x_inv_scale
-    if (precision == PREC_FP16X2) {
-      const float* op[2] = {dA, dB};
-      const long long n[2] = {static_cast<long long>(M) * K, static_cast<long long>(Nn) * K};
-      float mx[2] = {0.f, 0.f};
-      for (int i = 0; i < 2; ++i) {
-        launch_prep_reduce(op[i], n[i], op[i], n[i], partial, 1, RowArrays{}, 0, bs, st);
-        DG_TRY(cudaMemcpyAsync(&mx[i], &bs->x_absmax, 4, cudaMemcpyDeviceToHost, st));
-      }
-      DG_TRY(cudaStreamSynchronize(st));
-      const PreScale ps = pre_scale(mx[0] > mx[1] ? mx[0] : mx[1]);
-      sc[0] = ps.scale; sc[1] = ps.inv;
+  const long long Mt = round_up(M, 64), Nt = round_up(Nn, 64);
+  const long long tmax = Mt > Nt ? Mt : Nt;
+  uint16_t *As = nullptr, *Bs = nullptr, *dummyT = nullptr;
+  BlockScalars* bs = nullptr; float* partial = nullptr;
+  DevMem mem;                                  // freed on every return
+  mem.own(&As, 2ull * ns * M * Kp, false); mem.own(&Bs, 2ull * ns * Nn * Kp, false);
+  mem.own(&dummyT, 2ull * ns * K * tmax, false);
+  mem.own(&bs, sizeof(BlockScalars), true);
+  mem.own(&partial, sizeof(float) * 2048, false);
+  CREATE_TRY(mem.err);
+  // one common power-of-two scale over both operands (the layer multiplies X by X^T, i.e. a single matrix), from max|A| and
+  // max|B| as the step's operand preparation finds them (no rows: nothing else is touched)
+  float sc[2] = {1.f, 1.f};                  // x_scale, x_inv_scale
+  if (precision == PREC_FP16X2) {
+    const float* op[2] = {dA, dB};
+    const long long n[2] = {static_cast<long long>(M) * K, static_cast<long long>(Nn) * K};
+    float mx[2] = {0.f, 0.f};
+    for (int i = 0; i < 2; ++i) {
+      launch_prep_reduce(op[i], n[i], op[i], n[i], partial, 1, RowArrays{}, 0, bs, st);
+      CREATE_TRY(cudaMemcpyAsync(&mx[i], &bs->x_absmax, 4, cudaMemcpyDeviceToHost, st));
     }
-    DG_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
-    launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
-    launch_split(dB, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
-    GemmParams gp; memset(&gp, 0, sizeof(gp));
-    gp.M = M; gp.Nn = Nn; gp.ts = tile_sched(M, Nn, (K + bk - 1) / bk);
-    gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f;
-    // EPI_OUT applies the inverse scale once; both operands were scaled -> fold the second factor into alpha
-    gp.alpha = sc[1]; gp.dev_scale = &bs->x_inv_scale;
-    if (backend == NPAIR_GEMM_TCGEN05) {
-      CUtensorMap ta, tb; std::string te;
-      if (!make_tmap_pieces(&ta, As, K, M, ns, Kp, static_cast<long long>(M) * Kp, bk, 128, &te) ||
-          !make_tmap_pieces(&tb, Bs, K, Nn, ns, Kp, static_cast<long long>(Nn) * Kp, bk, 256, &te)) { g_create_err = te; rc = NPAIR_E_CUDA; goto done; }
-      DG_TRY(allow_smem(gemm_kernel(precision, EPI_OUT)));
-      DG_TRY(launch_gemm(precision, EPI_OUT, ta, tb, ta, gp, sms, st));
-    } else {
-      DG_TRY(launch_simt_gemm(precision, EPI_OUT, As, Kp, static_cast<long long>(M) * Kp, Bs, Kp, static_cast<long long>(Nn) * Kp, K, gp, st));
-    }
-    DG_TRY(cudaStreamSynchronize(st));
+    CREATE_TRY(cudaStreamSynchronize(st));
+    const PreScale ps = pre_scale(mx[0] > mx[1] ? mx[0] : mx[1]);
+    sc[0] = ps.scale; sc[1] = ps.inv;
   }
-done:
-  cudaFree(As); cudaFree(Bs); cudaFree(dummyT); cudaFree(bs); cudaFree(partial);
-#undef DG_TRY
-  return rc;
+  CREATE_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
+  launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
+  launch_split(dB, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
+  GemmParams gp; memset(&gp, 0, sizeof(gp));
+  gp.M = M; gp.Nn = Nn; gp.ts = tile_sched(M, Nn, (K + bk - 1) / bk);
+  gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f;
+  // EPI_OUT applies the inverse scale once; both operands were scaled -> fold the second factor into alpha
+  gp.alpha = sc[1]; gp.dev_scale = &bs->x_inv_scale;
+  if (backend == NPAIR_GEMM_TCGEN05) {
+    CUtensorMap ta, tb; std::string te;
+    if (!make_tmap_pieces(&ta, As, K, M, ns, Kp, static_cast<long long>(M) * Kp, bk, 128, &te) ||
+        !make_tmap_pieces(&tb, Bs, K, Nn, ns, Kp, static_cast<long long>(Nn) * Kp, bk, 256, &te)) { g_create_err = te; return NPAIR_E_CUDA; }
+    CREATE_TRY(allow_smem(gemm_kernel(precision, EPI_OUT)));
+    CREATE_TRY(launch_gemm(precision, EPI_OUT, ta, tb, ta, gp, sms, st));
+  } else {
+    CREATE_TRY(launch_simt_gemm(precision, EPI_OUT, As, Kp, static_cast<long long>(M) * Kp, Bs, Kp, static_cast<long long>(Nn) * Kp, K, gp, st));
+  }
+  CREATE_TRY(cudaStreamSynchronize(st));
+  return NPAIR_OK;
 }
 
 }  // extern "C"
@@ -1578,15 +1593,12 @@ done:
 // ------------------------------------------------------------------------------------------------ retrieval evaluation (DESIGN 8)
 // Not part of the reference layer.  Queries go to the A format and gallery rows to the B format of the K-concatenated operands, so the
 // similarity GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
-enum { E_CAT_A, E_CAT_B, E_ROWS, E_BS, E_SYM_TILES, E_COUNT_BUFS };
-static constexpr int EVAL_ROW_WORDS = 5;        // the statistics of RowArrays: four ordered-uint statistics and the same-label count per query
 static constexpr int EVAL_NO_SELF = -(1 << 30); // a self offset that matches no column (rows and columns stay below 2^30)
 
 struct EvalPlan {
   int max_q, max_g, D, prec;
   long long Dp, kcat;           // padded feature extent, K extent of the concatenated operands (mma_passes * Dp)
   int n_sym_tiles;              // tile-list capacity: self-retrieval over min(max_q, max_g) rows
-  size_t bytes[E_COUNT_BUFS];
 };
 
 static int eval_validate(long long max_q, long long max_g, long long D, int prec, std::string* err) {
@@ -1603,60 +1615,66 @@ static EvalPlan eval_plan_of(int max_q, int max_g, int D, int prec) {
   p.kcat = mma_passes(SPLIT_FORMATS[prec].pieces) * p.Dp;
   const int n = max_q < max_g ? max_q : max_g;
   p.n_sym_tiles = static_cast<int>(sym_tile_count(n, n));
-  size_t* b = p.bytes;
-  b[E_CAT_A] = 2ull * max_q * p.kcat;
-  b[E_CAT_B] = 2ull * max_g * p.kcat;
-  b[E_ROWS] = 4ull * EVAL_ROW_WORDS * max_q + 16;     // + the absmax word
-  b[E_BS] = sizeof(BlockScalars);
-  b[E_SYM_TILES] = sizeof(int2) * p.n_sym_tiles;
   return p;
 }
 
 struct npair_eval : EvalPlan {
   int device = -1, sms = 0;
+  DevMem mem;                     // the workspace (eval_buffers)
   uint16_t *catA = nullptr, *catB = nullptr;
-  void* rows = nullptr;
-  RowArrays ra{};                 // only the statistics (EVAL_ROW_WORDS)
+  RowArrays ra{};                 // only the statistics (carve_stats)
   unsigned int* absmax_bits = nullptr;
   BlockScalars* bs = nullptr;
   int2* sym_tiles = nullptr;
   int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
   std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
-  // MAP@R (npair_eval_map_at_r), grown on demand and kept: per query the segment offsets and gather counters, per positive pair the
-  // positive and its bucket counter (map_at_r_bytes)
-  void* map_rows = nullptr;
-  size_t map_rows_bytes = 0;
-  void* map_pairs = nullptr;
-  size_t map_pairs_bytes = 0;
-  // k-means (npair_eval_kmeans), grown on demand and kept (kmeans_bytes)
-  void* km = nullptr;
-  size_t km_bytes = 0;
+  // MAP@R (MapRows, MapPairs) and k-means (KmeansBufs) buffers, grown on demand and kept
+  DevMem map_rows_mem, map_pairs_mem, km_mem;
+  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr;
   std::string err;
 };
 
-// Device memory of npair_eval_map_at_r beyond the workspace, in the two parts it is allocated in: per query the nq + 1 segment offsets,
-// the gather counter and the {sum R, error bits} word pair; per positive pair the value and the histogram word
-static size_t map_rows_bytes(long long nq) { return 8ull * (nq + 1) + 4ull * nq + 16; }
-static size_t map_pairs_bytes(long long sum_r) { return 8ull * sum_r; }
-// Device memory of npair_eval_kmeans beyond the workspace, in the order it is carved: the int64 sums [k][D], the argmax keys [n], the
-// inertia partials, then the counts [k], the biases [k], the initial rows [k] and the KmeansWords
-static size_t kmeans_bytes(long long n, long long k, long long D) {
-  return 8ull * k * D + 8ull * n + 8ull * KM_INERTIA_BLOCKS + 12ull * k + sizeof(KmeansWords);
+// The evaluator's workspace, each buffer with its size and zero-fill; returns the first failure
+static cudaError_t eval_buffers(npair_eval* ev, DevMem& m) {
+  m.own(&ev->catA, 2ull * ev->max_q * ev->kcat, false);
+  m.own(&ev->catB, 2ull * ev->max_g * ev->kcat, false);
+  m.own_carved(true, [ev](Carve& cv) { carve_stats(cv, ev->max_q, &ev->ra); ev->absmax_bits = cv.take<unsigned int>(1); });
+  m.own(&ev->bs, sizeof(BlockScalars), true);
+  m.own(&ev->sym_tiles, sizeof(int2) * ev->n_sym_tiles, false);
+  return m.err;
 }
 
-// Grows *buf to at least `bytes` (freeing the old one: cudaFree waits for the device); `what` names the buffer in the error text
-static int eval_grow(npair_eval* ev, void** buf, size_t* have, size_t bytes, const char* what) {
-  if (bytes <= *have) return NPAIR_OK;
-  cudaFree(*buf);
-  *buf = nullptr; *have = 0;
-  if (cudaMalloc(buf, bytes) != cudaSuccess) {
-    cudaGetLastError();
-    *buf = nullptr;
-    ev->err = fmt("cannot allocate %zu bytes for %s", bytes, what);
-    return NPAIR_E_CUDA;
+// The device memory of npair_eval_map_at_r and npair_eval_kmeans beyond the workspace.  Each constructor carves one buffer at `base`;
+// over a null base it only measures it.  MAP@R takes two buffers: per query the nq + 1 segment offsets, the {sum R, error bits} word
+// pair and the gather counters; per positive pair the value and the histogram word.
+struct MapRows : Carve {
+  long long* seg; unsigned long long* sum_err; int* fill;
+  MapRows(char* base, long long nq) : Carve{base} { seg = take<long long>(nq + 1); sum_err = take<unsigned long long>(2); fill = take<int>(nq); }
+};
+struct MapPairs : Carve {
+  float* pos; unsigned int* hist;
+  MapPairs(char* base, long long sum_r) : Carve{base} { pos = take<float>(sum_r); hist = take<unsigned int>(sum_r); }
+};
+// k-means takes one: the int64 sums of the members' features, the EPI_ARGMAX keys, the inertia partials, then per cluster its member
+// count, its bias 0.5 ||mu||^2 and its initial row, and the KmeansWords.
+struct KmeansBufs : Carve {
+  long long* sums; unsigned long long* keys; double* partial; int* counts; float* bias; int* rows; KmeansWords* words;
+  KmeansBufs(char* base, long long n, long long k, long long D) : Carve{base} {
+    sums = take<long long>(k * D); keys = take<unsigned long long>(n); partial = take<double>(KM_INERTIA_BLOCKS);
+    counts = take<int>(k); bias = take<float>(k); rows = take<int>(k); words = take<KmeansWords>(1);
   }
-  *have = bytes;
-  return NPAIR_OK;
+};
+
+// Grows the buffer `m` holds at *base to at least `bytes` (cudaFree of the old one waits for the device); `what` names it in errors
+static int eval_grow(npair_eval* ev, DevMem& m, char** base, size_t bytes, const char* what) {
+  if (bytes <= m.bytes) return NPAIR_OK;
+  m.release();
+  m.own(base, bytes, false);
+  if (m.err == cudaSuccess) return NPAIR_OK;
+  cudaGetLastError();
+  m.release();
+  ev->err = fmt("cannot allocate %zu bytes for %s", bytes, what);
+  return NPAIR_E_CUDA;
 }
 
 extern "C" {
@@ -1664,20 +1682,21 @@ extern "C" {
 size_t npair_eval_workspace_bytes(int32_t max_q, int32_t max_g, int32_t D, int32_t prec) {
   std::string e;
   if (eval_validate(max_q, max_g, D, prec, &e) != NPAIR_OK) return 0;
-  const EvalPlan p = eval_plan_of(max_q, max_g, D, prec);
-  size_t total = 0;
-  for (size_t b : p.bytes) total += b;
-  return total;
+  npair_eval ev;
+  static_cast<EvalPlan&>(ev) = eval_plan_of(max_q, max_g, D, prec);
+  DevMem sizing(false);
+  eval_buffers(&ev, sizing);
+  return sizing.bytes;
 }
 
 size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r) {
   if (nq < 1 || sum_r < 0) return 0;
-  return map_rows_bytes(nq) + map_pairs_bytes(sum_r);
+  return MapRows(nullptr, nq).bytes + MapPairs(nullptr, sum_r).bytes;
 }
 
 size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
   if (n < 1 || k < 1 || D < 1 || k > n) return 0;
-  return kmeans_bytes(n, k, D);
+  return KmeansBufs(nullptr, n, k, D).bytes;
 }
 
 const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
@@ -1685,9 +1704,7 @@ const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_
 void npair_eval_destroy(npair_eval* ev) {
   if (!ev) return;
   if (ev->device >= 0) cudaSetDevice(ev->device);
-  cudaFree(ev->catA); cudaFree(ev->catB); cudaFree(ev->rows); cudaFree(ev->bs); cudaFree(ev->sym_tiles);
-  cudaFree(ev->map_rows); cudaFree(ev->map_pairs); cudaFree(ev->km);
-  delete ev;
+  delete ev;                      // its DevMems free its buffers on this device
 }
 
 int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int32_t device, npair_eval** out) {
@@ -1701,16 +1718,7 @@ int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int
   npair_eval* ev = made.get();
   static_cast<EvalPlan&>(*ev) = eval_plan_of(max_q, max_g, D, prec);
   ev->device = dev; ev->sms = sms;
-  const size_t* b = ev->bytes;
-  CREATE_TRY(dev_alloc(&ev->catA, b[E_CAT_A], false));
-  CREATE_TRY(dev_alloc(&ev->catB, b[E_CAT_B], false));
-  CREATE_TRY(dev_alloc(&ev->rows, b[E_ROWS], true));
-  CREATE_TRY(dev_alloc(&ev->bs, b[E_BS], true));
-  CREATE_TRY(dev_alloc(&ev->sym_tiles, b[E_SYM_TILES], false));
-  uint32_t* w = static_cast<uint32_t*>(ev->rows);
-  ev->ra.st_minw = w; w += max_q; ev->ra.st_maxw = w; w += max_q; ev->ra.st_maxb = w; w += max_q; ev->ra.st_maxall = w; w += max_q;
-  ev->ra.cnt_same = reinterpret_cast<int*>(w); w += max_q;
-  ev->absmax_bits = w;
+  CREATE_TRY(eval_buffers(ev, ev->mem));
   const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
                       EPI_BUCKET | EPI_SYM, EPI_ARGMAX};
   for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
@@ -1851,17 +1859,15 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
   CUDA_TRY(ev, cudaSetDevice(ev->device));
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
-  if ((rc = eval_grow(ev, &ev->map_rows, &ev->map_rows_bytes, map_rows_bytes(nq), "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
-  long long* seg = static_cast<long long*>(ev->map_rows);                          // [nq + 1]
-  unsigned long long* sum_err = reinterpret_cast<unsigned long long*>(seg + nq + 1);  // {sum R_i, error bits}
-  int* fill = reinterpret_cast<int*>(sum_err + 2);                                    // [nq]
+  if ((rc = eval_grow(ev, ev->map_rows_mem, &ev->map_rows, MapRows(nullptr, nq).bytes, "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
+  const MapRows rows(ev->map_rows, nq);
   const int* R = ev->ra.cnt_same;
   // sweep 1: R_i, and the one host synchronisation, for sum R_i
   if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
   if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_seg_scan(R, nq, seg, ev->bs, sum_err, st);
+  launch_eval_seg_scan(R, nq, rows.seg, ev->bs, rows.sum_err, st);
   unsigned long long h[2] = {0, 0};
-  CUDA_TRY(ev, cudaMemcpyAsync(h, sum_err, sizeof(h), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ev, cudaMemcpyAsync(h, rows.sum_err, sizeof(h), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ev, cudaStreamSynchronize(st));
   if (h[1] & DERR_GATHER_SLOT) {
     ev->err = "an earlier npair_eval_map_at_r on this evaluator gathered more positives for a query than its statistics sweep counted "
@@ -1869,22 +1875,21 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
     return NPAIR_E_CUDA;
   }
   const long long sum_r = static_cast<long long>(h[0]);
-  if ((rc = eval_grow(ev, &ev->map_pairs, &ev->map_pairs_bytes, map_pairs_bytes(sum_r), "the MAP@R positive pairs")) != NPAIR_OK) return rc;
-  float* pos = static_cast<float*>(ev->map_pairs);
-  unsigned int* hist = reinterpret_cast<unsigned int*>(pos + sum_r);
-  CUDA_TRY(ev, cudaMemsetAsync(fill, 0, sizeof(int) * nq, st));
+  if ((rc = eval_grow(ev, ev->map_pairs_mem, &ev->map_pairs, MapPairs(nullptr, sum_r).bytes, "the MAP@R positive pairs")) != NPAIR_OK) return rc;
+  const MapPairs pairs(ev->map_pairs, sum_r);
+  CUDA_TRY(ev, cudaMemsetAsync(rows.fill, 0, sizeof(int) * nq, st));
   if (sum_r > 0) {
     GemmParams mp{};
     // sweep 2: the positives, unordered, into the histogram words; then sorted into pos
-    mp.seg = seg; mp.fill = fill; mp.pos = reinterpret_cast<float*>(hist);
+    mp.seg = rows.seg; mp.fill = rows.fill; mp.pos = reinterpret_cast<float*>(pairs.hist);
     if ((rc = eval_sweep(ev, EPI_GATHER, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
-    launch_eval_seg_sort(R, seg, nq, reinterpret_cast<const float*>(hist), pos, st);
-    CUDA_TRY(ev, cudaMemsetAsync(hist, 0, sizeof(unsigned int) * sum_r, st));
+    launch_eval_seg_sort(R, rows.seg, nq, reinterpret_cast<const float*>(pairs.hist), pairs.pos, st);
+    CUDA_TRY(ev, cudaMemsetAsync(pairs.hist, 0, sizeof(unsigned int) * sum_r, st));
     // sweep 3: the buckets
-    mp.pos = pos; mp.hist = hist;
+    mp.pos = pairs.pos; mp.hist = pairs.hist;
     if ((rc = eval_sweep(ev, EPI_BUCKET, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
   }
-  launch_eval_map_finish(R, seg, fill, pos, hist, nq, d_map_r, d_r_precision, d_R, d_rank, st);
+  launch_eval_map_finish(R, rows.seg, rows.fill, pairs.pos, pairs.hist, nq, d_map_r, d_r_precision, d_R, d_rank, st);
   CUDA_TRY(ev, cudaGetLastError());
   return NPAIR_OK;
 }
@@ -1908,45 +1913,39 @@ int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, cons
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
   int rc;
-  if ((rc = eval_grow(ev, &ev->km, &ev->km_bytes, kmeans_bytes(n, k, ev->D), "the k-means buffers")) != NPAIR_OK) return rc;
+  if ((rc = eval_grow(ev, ev->km_mem, &ev->km, KmeansBufs(nullptr, n, k, ev->D).bytes, "the k-means buffers")) != NPAIR_OK) return rc;
   const long long D = ev->D;
-  long long* sums = static_cast<long long*>(ev->km);                                  // [k][D]
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(sums + k * D);     // [n]
-  double* partial = reinterpret_cast<double*>(keys + n);                              // [KM_INERTIA_BLOCKS]
-  int* counts = reinterpret_cast<int*>(partial + KM_INERTIA_BLOCKS);                  // [k]
-  float* bias = reinterpret_cast<float*>(counts + k);                                 // [k]
-  int* rows = reinterpret_cast<int*>(bias + k);                                       // [k]
-  KmeansWords* words = reinterpret_cast<KmeansWords*>(rows + k);
+  const KmeansBufs km(ev->km, n, k, D);
   unsigned int* amx = ev->absmax_bits;
-  CUDA_TRY(ev, cudaMemcpyAsync(rows, init_rows, sizeof(int) * k, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ev, cudaMemcpyAsync(km.rows, init_rows, sizeof(int) * k, cudaMemcpyHostToDevice, st));
   // the points, once: max|x| in every format (the update's fixed-point scale), then the A operand
   CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
   launch_eval_prep(x, n * D, nullptr, 0, amx, ev->ra, 0, ev->sms, st);
   launch_eval_split(x, n, ev->D, ev->Dp, ev->prec, 0, -1.f, amx, ev->bs, ev->catA, st);
-  launch_km_gather(x, ev->D, rows, k, d_centroids, st);
+  launch_km_gather(x, ev->D, km.rows, k, d_centroids, st);
   CUDA_TRY(ev, cudaMemsetAsync(d_assign, 0xFF, sizeof(int32_t) * n, st));   // -1: every point of the first sweep changes
-  CUDA_TRY(ev, cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * n, st));
-  CUDA_TRY(ev, cudaMemsetAsync(sums, 0, sizeof(long long) * k * D, st));     // a call that stopped on convergence leaves them set
+  CUDA_TRY(ev, cudaMemsetAsync(km.keys, 0, sizeof(unsigned long long) * n, st));
+  CUDA_TRY(ev, cudaMemsetAsync(km.sums, 0, sizeof(long long) * k * D, st));     // a call that stopped on convergence leaves them set
   GemmParams am{};
-  am.col_bias = bias; am.best = keys;
+  am.col_bias = km.bias; am.best = km.keys;
   KmeansWords h{};
   int t = 0;
   for (;; ++t) {
     const bool last = t + 1 == max_iter;
     launch_eval_split(d_centroids, k, ev->D, ev->Dp, ev->prec, 1, -1.f, amx, ev->bs, ev->catB, st);
-    launch_km_bias(d_centroids, k, ev->D, bias, counts, words, st);
+    launch_km_bias(d_centroids, k, ev->D, km.bias, km.counts, km.words, st);
     if ((rc = eval_sweep(ev, EPI_ARGMAX, n, k, EVAL_NO_SELF, nullptr, nullptr, nullptr, nullptr, false, st, &am)) != NPAIR_OK) return rc;
-    launch_km_assign(keys, x, n, ev->D, amx, k, d_assign, counts, sums, !last, words, st);
-    CUDA_TRY(ev, cudaMemcpyAsync(&h, words, sizeof(h), cudaMemcpyDeviceToHost, st));
+    launch_km_assign(km.keys, x, n, ev->D, amx, k, d_assign, km.counts, km.sums, !last, km.words, st);
+    CUDA_TRY(ev, cudaMemcpyAsync(&h, km.words, sizeof(h), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ev, cudaStreamSynchronize(st));
     if (h.err & DERR_KMEANS_NO_ARGMAX) {
       ev->err = "a point has no centroid with a finite score: x or a centroid holds NaN or infinity";
       return NPAIR_E_CUDA;
     }
     if ((t > 0 && h.changed == 0) || last) break;
-    launch_km_update(sums, counts, amx, k, ev->D, d_centroids, st);
+    launch_km_update(km.sums, km.counts, amx, k, ev->D, d_centroids, st);
   }
-  if (d_inertia) launch_km_inertia(x, d_centroids, d_assign, n, ev->D, partial, d_inertia, st);
+  if (d_inertia) launch_km_inertia(x, d_centroids, d_assign, n, ev->D, km.partial, d_inertia, st);
   CUDA_TRY(ev, cudaGetLastError());
   stats[0] = t + 1;
   stats[1] = static_cast<int32_t>(h.changed);
