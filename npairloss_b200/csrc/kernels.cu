@@ -451,71 +451,64 @@ __device__ __forceinline__ void smem_dec(unsigned int* p) {
   asm volatile("red.shared.add.u32 [%0], -1;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(p))) : "memory");
 }
 
-// Sweep of one row: calls f(key, j, side) for every column j < N with side = 0 (same label as the row) or 1 (different);
-// the self pair is NOT excluded here.  16-byte loads of S (row stride is a multiple of 32 floats) and of the labels.
-template <class F>
-__device__ __forceinline__ void sweep_row(const float* __restrict__ row, int N, const float* __restrict__ lab_cols, float li, bool lab_aligned,
-                                          bool want_same, bool want_diff, F f) {
-  for (int j4 = threadIdx.x * 4; j4 < N; j4 += blockDim.x * 4) {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(row + j4));
-    float ll[4];
-    if (lab_aligned && j4 + 3 < N) {
-      const float4 l = __ldg(reinterpret_cast<const float4*>(lab_cols + j4));
-      ll[0] = l.x; ll[1] = l.y; ll[2] = l.z; ll[3] = l.w;
-    } else {
+// ---- parts shared by the select kernels ----
+#define NPAIR_LSEL_SCAP 128                // same-label entries kept per row (LOCAL)
+
+// Value order -> raw digit of the top `bits` bits of a float (sign first): orders [0, 2^(bits-1)) are the negative floats, whose raw
+// digits descend
+__device__ __forceinline__ uint32_t raw_digit_of_order(uint32_t o, int bits) {
+  const uint32_t half = 1u << (bits - 1);
+  return o < half ? 2u * half - 1u - o : o - half;
+}
+// Below a top digit of the raw bits, the remainders of negative floats sort descending: XOR with this mask (the low rem_bits when the
+// sign bit of `bits` is set) puts a remainder in value order, and back again
+__device__ __forceinline__ uint32_t rem_flip(uint32_t bits, int rem_bits) { return (bits >> 31) ? (1u << rem_bits) - 1u : 0u; }
+
+template <class T>
+__device__ __forceinline__ T warp_incl_sum(T x, int lane) {
 #pragma unroll
-      for (int c = 0; c < 4; ++c) ll[c] = (j4 + c < N) ? __ldg(lab_cols + j4 + c) : li;
-    }
-    const float vv[4] = {v.x, v.y, v.z, v.w};
-    if (j4 + 3 < N && ll[0] != li && ll[1] != li && ll[2] != li && ll[3] != li) {
-      if (want_diff) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) f(f2ord(vv[c]), j4 + c, 1);
-      }
-    } else {
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        if (j4 + c >= N) continue;
-        const int side = (ll[c] == li) ? 0 : 1;
-        if (side == 0 ? want_same : want_diff) f(f2ord(vv[c]), j4 + c, side);
-      }
-    }
-  }
+  for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += t; }
+  return x;
 }
 
-// Block-parallel search of the bin that holds 0-based rank r in hist[0..nbins): returns the bin (or nbins when r is out of range),
-// the rank inside it and its population.  nbins <= 2048, blockDim.x threads (a multiple of 32, <= 1024).  All threads get the result.
-template <class CT>
-__device__ __forceinline__ int find_bin(const CT* hist, int nbins, unsigned long long r, unsigned long long* r_in, unsigned long long* pop,
-                                        unsigned long long* s_scan /*[33]*/, int* s_res /*[1]*/, unsigned long long* s_out /*[2]*/) {
-  const int per = (nbins + blockDim.x - 1) / blockDim.x;
-  const int b0 = threadIdx.x * per;
-  unsigned long long mine = 0;
-  for (int b = b0; b < b0 + per && b < nbins; ++b) mine += hist[b];
-  unsigned long long incl = mine;                                 // inclusive scan over the block
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) s_scan[w] = incl;
-  if (threadIdx.x == 0) *s_res = nbins;
-  __syncthreads();
-  if (w == 0) {
-    unsigned long long x = (lane < static_cast<int>(blockDim.x >> 5)) ? s_scan[lane] : 0ull;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += t; }
-    s_scan[lane] = x;                                             // inclusive warp totals
+// Bin of 0-based rank r among bins 0 .. nb-1 taken in index order, bin b holding cnt(b) entries (cnt folds in any bin-index map); by a
+// warp, nb a multiple of 32 and at most 1024.  Lane l sums bins [l * nb/32, (l+1) * nb/32); the winning lane's bins are then scanned
+// one per lane.  Returns the bin and *r_in, the rank inside it (warp-uniform); nb when r is out of range.
+template <class C>
+__device__ __forceinline__ int warp_find_bin(C cnt, int nb, unsigned int r, unsigned int* r_in, int lane) {
+  const int per = nb >> 5;
+  unsigned int mine = 0;
+  for (int b = 0; b < per; ++b) mine += cnt(lane * per + b);
+  const unsigned int before = warp_incl_sum(mine, lane) - mine;
+  const unsigned int hit = __ballot_sync(0xffffffffu, mine && r >= before && r < before + mine);
+  if (!hit) return nb;
+  const int src = __ffs(hit) - 1;
+  const unsigned int base = __shfl_sync(0xffffffffu, before, src);
+  const int bin = src * per + lane;
+  const unsigned int h = lane < per ? cnt(bin) : 0u;
+  const unsigned int bef = base + warp_incl_sum(h, lane) - h;
+  const int src2 = __ffs(__ballot_sync(0xffffffffu, h && r >= bef && r < bef + h)) - 1;
+  *r_in = r - __shfl_sync(0xffffffffu, bef, src2);
+  return __shfl_sync(0xffffffffu, bin, src2);
+}
+
+// A same-label entry (raw bits) joins its row's list; past NPAIR_LSEL_SCAP entries it is only counted, and the row's sides that need
+// the list take the slow path
+__device__ __forceinline__ void same_append(unsigned int* n, uint32_t* list, uint32_t bits) {
+  const unsigned int k = atomicAdd(n, 1u);
+  if (k < NPAIR_LSEL_SCAP) list[k] = bits;
+}
+
+// Of the n ordered keys key(0 .. n-1), the one of 0-based rank pos (ties by index) is stored to *out as a threshold, by the thread that
+// holds it: threads e0, e0 + step, ... take one key each and count the keys before it
+template <class K>
+__device__ __forceinline__ void store_key_of_rank(K key, unsigned int n, unsigned int pos, unsigned int e0, unsigned int step, float* out) {
+  for (unsigned int e = e0; e < n; e += step) {
+    const uint32_t ke = key(e);
+    unsigned int rk = 0;
+    for (unsigned int t = 0; t < n; ++t) { const uint32_t kt = key(t); rk += (kt < ke || (kt == ke && t < e)) ? 1u : 0u; }
+    if (rk == pos) *out = clamp_thr(ord2f(ke));
   }
-  __syncthreads();
-  const unsigned long long before = (w ? s_scan[w - 1] : 0ull) + incl - mine;
-  if (mine && r >= before && r < before + mine) {                 // exactly one thread
-    unsigned long long cum = before;
-    int b = b0;
-    for (; b < b0 + per && b < nbins; ++b) { const unsigned long long h = hist[b]; if (cum + h > r) break; cum += h; }
-    *s_res = b; s_out[0] = r - cum; s_out[1] = hist[b];
-  }
-  __syncthreads();
-  *r_in = s_out[0]; *pop = s_out[1];
-  return *s_res;
 }
 
 // ---- LOCAL: ONE WARP per row, warp-private histogram -- no block barriers, no block-wide scans ----
@@ -531,7 +524,6 @@ __device__ __forceinline__ int find_bin(const CT* hist, int nbins, unsigned long
 #define NPAIR_LSEL_WARPS 8
 #define NPAIR_LSEL_D1 1024                 // bins of the first digit
 #define NPAIR_LSEL_LCAP 48                 // candidates per lane
-#define NPAIR_LSEL_SCAP 128                // same-label entries kept per row
 #define NPAIR_LSEL_U 4                     // 16-byte loads in flight per lane and array
 struct LselWarp {
   unsigned int hist[NPAIR_LSEL_D1];
@@ -540,32 +532,6 @@ struct LselWarp {
   unsigned int n_same, pad_[3];            // keeps sizeof a multiple of 16 (16-byte stores into hist)
 };
 static_assert(sizeof(LselWarp) % 16 == 0, "LselWarp must keep 16-byte alignment in an array");
-// value order <-> raw 10-bit digit (sign, 8 exponent bits, 1 mantissa bit): order o in [0,512) are the negative floats, descending raw
-__device__ __forceinline__ uint32_t d1_raw_of_order(uint32_t o) { return o < 512u ? 1023u - o : o - 512u; }
-__device__ __forceinline__ uint32_t d1_order_of_raw(uint32_t r) { return r >= 512u ? 1023u - r : r + 512u; }
-
-// rank r (0-based) within bins[0..nb) taken in index order; nb a multiple of 32.  Returns the bin, *r_in, *pop (warp-uniform); nb if out of range.
-__device__ __forceinline__ int warp_find_bin(const unsigned int* bins, int nb, unsigned int r, unsigned int* r_in, unsigned int* pop, int lane) {
-  const int per = nb >> 5;
-  unsigned int mine = 0;
-  for (int b = 0; b < per; ++b) mine += bins[lane * per + b];
-  unsigned int incl = mine;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const unsigned int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  const unsigned int before = incl - mine;
-  const unsigned int hit = __ballot_sync(0xffffffffu, mine && r >= before && r < before + mine);
-  if (!hit) return nb;
-  const int src = __ffs(hit) - 1;
-  int bin = 0; unsigned int ri = 0, pp = 0;
-  if (lane == src) {
-    unsigned int cum = before;
-    int b = 0;
-    for (; b < per; ++b) { const unsigned int h = bins[lane * per + b]; if (cum + h > r) { pp = h; break; } cum += h; }
-    bin = lane * per + b; ri = r - cum;
-  }
-  *r_in = __shfl_sync(0xffffffffu, ri, src); *pop = __shfl_sync(0xffffffffu, pp, src);
-  return __shfl_sync(0xffffffffu, bin, src);
-}
 
 // Generic (slow) select of one side of one row by a warp: 32-bit ordered keys, digits of 10/10/10/2 bits, one sweep of the row per digit.
 __device__ __noinline__ uint32_t slow_select_row(const float* __restrict__ row, int N, const float* __restrict__ lab_cols, float li, int self_col,
@@ -585,8 +551,8 @@ __device__ __noinline__ uint32_t slow_select_row(const float* __restrict__ row, 
       if ((key & mask) == prefix) smem_inc(&hist[(key >> shift) & (nb - 1)]);
     }
     __syncwarp();
-    unsigned int r2, pp;
-    const int d = warp_find_bin(hist, nb < 32 ? 32 : nb, rank, &r2, &pp, lane);
+    unsigned int r2;
+    const int d = warp_find_bin([&](int b) { return hist[b]; }, nb < 32 ? 32 : nb, rank, &r2, lane);
     prefix |= static_cast<uint32_t>(d) << shift; mask |= static_cast<uint32_t>(nb - 1) << shift; rank = r2;
     shift -= 10;
     __syncwarp();
@@ -634,14 +600,14 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
         if (ll[0] == li || ll[1] == li || ll[2] == li || ll[3] == li) {
 #pragma unroll
           for (int c = 0; c < 4; ++c)
-            if (ll[c] == li && jj + c != self_col) { const unsigned int k = atomicAdd(&W.n_same, 1u); if (k < NPAIR_LSEL_SCAP) W.same[k] = vv[c]; }
+            if (ll[c] == li && jj + c != self_col) same_append(&W.n_same, W.same, vv[c]);
         }
       }
     }
     for (int j = n_vec + lane; j < N; j += 32) {                  // ragged tail / unaligned labels
       const uint32_t b = __float_as_uint(row[j]);
       if (want_diff) smem_inc(&W.hist[b >> 22]);
-      if (lab_cols[j] == li && j != self_col) { const unsigned int k = atomicAdd(&W.n_same, 1u); if (k < NPAIR_LSEL_SCAP) W.same[k] = b; }
+      if (lab_cols[j] == li && j != self_col) same_append(&W.n_same, W.same, b);
     }
     __syncwarp();
     const unsigned int ns = W.n_same;                             // == cs
@@ -649,28 +615,24 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
     // ---------------- AP side: the same-label list is short ----------------
     if (want_same) {
       unsigned long long pos = 0;
-      float thr = 0.f;
-      if (cs == 0) { if (lane == 0) atomicOr(&bs->err, DERR_EMPTY_LIST); }
-      else if (!pos_index(sn_ap, static_cast<unsigned long long>(cs), pos)) { if (lane == 0) atomicOr(&bs->err, DERR_POS_RANGE); }
+      if (cs == 0) { if (lane == 0) { atomicOr(&bs->err, DERR_EMPTY_LIST); ra.posi_thr[i] = 0.f; } }
+      else if (!pos_index(sn_ap, static_cast<unsigned long long>(cs), pos)) { if (lane == 0) { atomicOr(&bs->err, DERR_POS_RANGE); ra.posi_thr[i] = 0.f; } }
       else if (ns <= 32) {                                        // rank by counting inside the warp
-        const uint32_t key = lane < static_cast<int>(ns) ? f2ord(__uint_as_float(W.same[lane])) : 0xFFFFFFFFu;
-        unsigned int rk = 0;
-        for (unsigned int t = 0; t < ns; ++t) { const uint32_t kt = __shfl_sync(0xffffffffu, key, t); rk += (kt < key || (kt == key && static_cast<int>(t) < lane)) ? 1u : 0u; }
-        const unsigned int hit = __ballot_sync(0xffffffffu, lane < static_cast<int>(ns) && rk == static_cast<unsigned int>(pos));
-        thr = clamp_thr(ord2f(__shfl_sync(0xffffffffu, key, __ffs(hit) - 1)));
+        store_key_of_rank([&](unsigned int t) { return f2ord(__uint_as_float(W.same[t])); }, ns, static_cast<unsigned int>(pos), lane, 32,
+                          &ra.posi_thr[i]);                                                                // .cu:288
       } else {
-        thr = clamp_thr(ord2f(slow_select_row(row, N, lab_cols, li, self_col, 0, static_cast<unsigned int>(pos), W.hist + 0, lane)));
+        const float thr = clamp_thr(ord2f(slow_select_row(row, N, lab_cols, li, self_col, 0, static_cast<unsigned int>(pos), W.hist + 0, lane)));
+        if (lane == 0) ra.posi_thr[i] = thr;
         // the slow path used the histogram: rebuild digit 1 for the diff side below by falling into its slow path as well
         if (want_diff && lane == 0) W.n_same = NPAIR_LSEL_SCAP + 1;
       }
-      if (lane == 0) ra.posi_thr[i] = thr;                        // .cu:288
       __syncwarp();
     }
     // ---------------- AN side ----------------
     if (want_diff) {
-      const unsigned long long size = static_cast<unsigned long long>(N - 1 - cs);
       unsigned long long pos = 0;
       float thr = 0.f;
+      const unsigned long long size = static_cast<unsigned long long>(N - 1 - cs);
       if (size == 0) { if (lane == 0) atomicOr(&bs->err, DERR_EMPTY_LIST); }
       else if (!pos_index(sn_an, size, pos)) { if (lane == 0) atomicOr(&bs->err, DERR_POS_RANGE); }
       else if (W.n_same > NPAIR_LSEL_SCAP) {
@@ -679,27 +641,10 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
         // excluded keys (same-label entries + the self pair) leave the histogram; then walk the bins in value order
         for (unsigned int e = lane; e <= ns; e += 32) smem_dec(&W.hist[(e < ns ? W.same[e] : self_bits) >> 22]);
         __syncwarp();
-        // permute into value order in place is not needed: lanes own 32 consecutive ORDER positions and read the raw bins they map to
-        unsigned int mine = 0;
-        for (int b = 0; b < 32; ++b) mine += W.hist[d1_raw_of_order(lane * 32 + b)];
-        unsigned int incl = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const unsigned int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        const unsigned int before = incl - mine, r0 = static_cast<unsigned int>(pos);
-        const unsigned int hit = __ballot_sync(0xffffffffu, mine && r0 >= before && r0 < before + mine);
-        const int src = __ffs(hit) - 1;                           // exists: pos < size = sum of the bins
-        // the winning lane's 32 bins, one per lane: a second warp scan instead of a serial walk
-        const unsigned int base = __shfl_sync(0xffffffffu, before, src);
-        const uint32_t my_raw = d1_raw_of_order(src * 32 + lane);
-        const unsigned int h1 = W.hist[my_raw];
-        unsigned int inc2 = h1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const unsigned int t = __shfl_up_sync(0xffffffffu, inc2, o); if (lane >= o) inc2 += t; }
-        const unsigned int bef2 = base + inc2 - h1;
-        const int src2 = __ffs(__ballot_sync(0xffffffffu, h1 && r0 >= bef2 && r0 < bef2 + h1)) - 1;
-        const uint32_t raw = __shfl_sync(0xffffffffu, my_raw, src2);
-        unsigned int rank = r0 - __shfl_sync(0xffffffffu, bef2, src2);
-        const bool negative = raw >= 512u;                        // remainders of negative floats sort descending
+        // the raw bins are read in value order; the bin exists: pos < size = sum of the bins
+        unsigned int rank;
+        const uint32_t raw = raw_digit_of_order(static_cast<uint32_t>(warp_find_bin([&](int o) { return W.hist[raw_digit_of_order(o, 10)]; },
+                                                                                    NPAIR_LSEL_D1, static_cast<unsigned int>(pos), &rank, lane)), 10);
         // ---------------- sweep 2: that bin's elements -> lane-private candidate lists ----------------
         unsigned int cnt = 0;
         for (int j4 = lane * 4; j4 < n_vec; j4 += 128 * NPAIR_LSEL_U) {
@@ -723,8 +668,7 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
           thr = clamp_thr(ord2f(slow_select_row(row, N, lab_cols, li, self_col, 1, static_cast<unsigned int>(pos), W.hist, lane)));
         } else {
           // ---------------- tail: 8 + 7 + 7 bits over the candidates; excluded keys of this bin are subtracted per digit ----------------
-          // in remainder space the order is ascending for positive floats and descending for negative ones: flip the remainders of negatives
-          const uint32_t flip = negative ? 0x3FFFFFu : 0u;
+          const uint32_t flip = rem_flip(raw << 22, 22);
           uint32_t pre = 0, msk = 0;
           const int shifts[3] = {14, 7, 0}, nbits[3] = {8, 7, 7};
 #pragma unroll
@@ -743,8 +687,8 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
               if ((b >> 22) == raw && (k & msk) == pre) smem_dec(&W.hist[(k >> shifts[ps]) & (nb - 1)]);
             }
             __syncwarp();
-            unsigned int r2, p2;
-            const int d = warp_find_bin(W.hist, nb, rank, &r2, &p2, lane);
+            unsigned int r2;
+            const int d = warp_find_bin([&](int b) { return W.hist[b]; }, nb, rank, &r2, lane);
             pre |= static_cast<uint32_t>(d & (nb - 1)) << shifts[ps]; msk |= static_cast<uint32_t>(nb - 1) << shifts[ps]; rank = r2;
             __syncwarp();
           }
@@ -789,17 +733,16 @@ struct LselBlock {
   float red_min[NPAIR_LSB_THREADS / 32], red_max[NPAIR_LSB_THREADS / 32];
   uint32_t red_klo[NPAIR_LSB_THREADS / 32], red_khi[NPAIR_LSB_THREADS / 32];
 };
-// rank r within hist[0 .. PER * 256) in index order; every thread sums PER consecutive bins.  Two barriers; the result is in B.out
-// afterwards (bin == PER * 256: rank out of range).
+
+// Bin of 0-based rank r among hist[0 .. PER * 256) in index order, every thread holding PER consecutive bins in registers.  Two
+// barriers; the result is in B.out afterwards (bin == PER * 256: rank out of range).
 template <int PER>
 __device__ __forceinline__ void block_find_bin_u32(LselBlock& B, unsigned int r) {
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   unsigned int h[PER], mine = 0;
 #pragma unroll
   for (int q = 0; q < PER; ++q) { h[q] = B.hist[tid * PER + q]; mine += h[q]; }
-  unsigned int incl = mine;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const unsigned int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+  const unsigned int incl = warp_incl_sum(mine, lane);
   if (lane == 31) B.warp_tot[w] = incl;
   if (tid == 0) B.out[0] = static_cast<unsigned int>(PER * NPAIR_LSB_THREADS);
   __syncthreads();
@@ -872,7 +815,7 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
 #pragma unroll
           for (int c = 0; c < 4; ++c)
             if (ll[c] == li) {
-              if (jj + c != self_col) { const unsigned int k = atomicAdd(&B.n_same, 1u); if (k < NPAIR_LSEL_SCAP) B.same[k] = v[4 * u + c]; }
+              if (jj + c != self_col) same_append(&B.n_same, B.same, v[4 * u + c]);
               v[4 * u + c] = kNaN;
             }
         }
@@ -883,7 +826,7 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     if (has_tail) {
       const int j = n4 + tid;
       if (lab_cols[j] == li) {
-        if (j != self_col) { const unsigned int k = atomicAdd(&B.n_same, 1u); if (k < NPAIR_LSEL_SCAP) B.same[k] = v[4 * NPAIR_LSB_VPT]; }
+        if (j != self_col) same_append(&B.n_same, B.same, v[4 * NPAIR_LSB_VPT]);
         v[4 * NPAIR_LSB_VPT] = kNaN;
       }
       mn = fminf(mn, __uint_as_float(v[4 * NPAIR_LSB_VPT])); mx = fmaxf(mx, __uint_as_float(v[4 * NPAIR_LSB_VPT]));
@@ -900,17 +843,12 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     unsigned long long pos_ap = 0, pos_an = 0;
     // ---------------- AP side: the same-label list is short; warp 0 ranks it by counting ----------------
     if (want_same) {
-      if (cs == 0) { if (tid == 0) { atomicOr(&bs->err, DERR_EMPTY_LIST); ra.posi_thr[i] = 0.f; } }
-      else if (!pos_index(sn_ap, static_cast<unsigned long long>(cs), pos_ap)) { if (tid == 0) { atomicOr(&bs->err, DERR_POS_RANGE); ra.posi_thr[i] = 0.f; } }
+      int err = 0;
+      if (!side_position(static_cast<unsigned long long>(cs), sn_ap, pos_ap, err)) { if (tid == 0) { atomicOr(&bs->err, err); ra.posi_thr[i] = 0.f; } }
       else if (ns > NPAIR_LSEL_SCAP) slow_ap = true;
-      else if (w == 0) {
-        for (unsigned int e = lane; e < ns; e += 32) {
-          const uint32_t key = f2ord(__uint_as_float(B.same[e]));
-          unsigned int rk = 0;
-          for (unsigned int t = 0; t < ns; ++t) { const uint32_t kt = f2ord(__uint_as_float(B.same[t])); rk += (kt < key || (kt == key && t < e)) ? 1u : 0u; }
-          if (rk == static_cast<unsigned int>(pos_ap)) ra.posi_thr[i] = clamp_thr(ord2f(key));               // .cu:288
-        }
-      }
+      else if (w == 0)
+        store_key_of_rank([&](unsigned int t) { return f2ord(__uint_as_float(B.same[t])); }, ns, static_cast<unsigned int>(pos_ap), lane, 32,
+                          &ra.posi_thr[i]);                                                                // .cu:288
     }
     // ---------------- AN side (every condition below is block-uniform) ----------------
     bool have_an = false, refine = false, by_bin = false;
@@ -918,9 +856,8 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     unsigned int rank = 0;
     uint32_t boff = 0;
     if (want_diff) {
-      const unsigned long long size = static_cast<unsigned long long>(N - 1 - cs);
-      if (size == 0) { if (tid == 0) { atomicOr(&bs->err, DERR_EMPTY_LIST); ra.nega_thr[i] = 0.f; } }
-      else if (!pos_index(sn_an, size, pos_an)) { if (tid == 0) { atomicOr(&bs->err, DERR_POS_RANGE); ra.nega_thr[i] = 0.f; } }
+      int err = 0;
+      if (!side_position(static_cast<unsigned long long>(N - 1 - cs), sn_an, pos_an, err)) { if (tid == 0) { atomicOr(&bs->err, err); ra.nega_thr[i] = 0.f; } }
       else have_an = true;
     }
     if (have_an) {
@@ -982,13 +919,7 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     if (i + static_cast<int>(gridDim.x) < Q) load_row(i + static_cast<int>(gridDim.x));
     if (have_an && !refine) {
       __syncthreads();
-      const unsigned int nc = B.n_cand;                            // <= NPAIR_LSB_CCAP = blockDim
-      if (tid < static_cast<int>(nc)) {
-        const uint32_t key = B.cand[tid];
-        unsigned int rk = 0;
-        for (unsigned int t = 0; t < nc; ++t) { const uint32_t kt = B.cand[t]; rk += (kt < key || (kt == key && static_cast<int>(t) < tid)) ? 1u : 0u; }
-        if (rk == rank) ra.nega_thr[i] = clamp_thr(ord2f(key));                                             // .cu:319
-      }
+      store_key_of_rank([&](unsigned int t) { return B.cand[t]; }, B.n_cand, rank, tid, NPAIR_LSB_THREADS, &ra.nega_thr[i]);   // .cu:319
     }
     if (slow_ap) {                                                 // more than 128 same-label entries: warp 0 redoes the side with plain sweeps
       __syncthreads();
@@ -1032,11 +963,37 @@ struct GlobalSelectBufs {
   int world_scope;            // 1: the digit counts are exchanged between the ranks before the decision
 };
 #define NPAIR_GSEL_STAGE 2048
-__device__ __forceinline__ uint32_t d11_raw_of_order(uint32_t o) { return o < 1024u ? 2047u - o : o - 1024u; }
 
-// Decides one digit of the GLOBAL select from the 64-bit counts in gb.hist (one block; `ordered` = 2048 x 8 bytes of shared memory)
+// Bin of 0-based rank r among bins 0 .. nb-1 taken in index order, bin b holding cnt(b) entries, by the block (any size that is a
+// multiple of 32): every thread sums a run of bins and the one whose run holds r walks it.  Three barriers; afterwards
+// s_out = {bin, rank inside it, its population} (bin == nb: r is out of range).  s_scan: 32 counts of shared memory.
+// Not merged with block_find_bin_u32: holding 64-bit counts in registers the way that finder does raises global_select_kernel, which
+// inlines this decision into its last block, from 55 to 58-60 registers (CUDA 12.9) in every form tried.
+template <class C>
+__device__ __forceinline__ void find_bin(C cnt, int nb, unsigned long long r, unsigned long long* s_scan, unsigned long long* s_out) {
+  const int per = (nb + blockDim.x - 1) / blockDim.x;
+  const int b0 = threadIdx.x * per, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned long long mine = 0;
+  for (int b = b0; b < b0 + per && b < nb; ++b) mine += cnt(b);
+  const unsigned long long incl = warp_incl_sum(mine, lane);
+  if (lane == 31) s_scan[w] = incl;
+  if (threadIdx.x == 0) s_out[0] = static_cast<unsigned long long>(nb);
+  __syncthreads();
+  if (w == 0) s_scan[lane] = warp_incl_sum((lane < static_cast<int>(blockDim.x >> 5)) ? s_scan[lane] : 0ull, lane);   // inclusive warp totals
+  __syncthreads();
+  const unsigned long long before = (w ? s_scan[w - 1] : 0ull) + incl - mine;
+  if (mine && r >= before && r < before + mine) {                 // exactly one thread
+    unsigned long long cum = before;
+    int b = b0;
+    for (; b < b0 + per && b < nb; ++b) { const unsigned long long h = cnt(b); if (cum + h > r) break; cum += h; }
+    s_out[0] = static_cast<unsigned long long>(b); s_out[1] = r - cum; s_out[2] = cnt(b);
+  }
+  __syncthreads();
+}
+
+// Decides one digit of the GLOBAL select from the 64-bit counts in gb.hist (one block; s_scan, s_out: find_bin's shared memory)
 __device__ void global_decide(int pass, bool act0, bool act1, GlobalSelectBufs gb, RowArrays ra, int Q, BlockScalars* bs,
-                              unsigned long long* ordered, unsigned long long* s_scan, int* s_res, unsigned long long* s_out) {
+                              unsigned long long* s_scan, unsigned long long* s_out) {
   const int shift = pass == 1 ? 10 : 0;
   const int nbits = pass == 2 ? 10 : 11;
 #pragma unroll
@@ -1044,23 +1001,19 @@ __device__ void global_decide(int pass, bool act0, bool act1, GlobalSelectBufs g
     if (!(side == 0 ? act0 : act1)) continue;
     const unsigned long long* gh = gb.hist + side * NPAIR_SEL_BINS;
     const int nb = 1 << nbits;
-    __syncthreads();
-    // pass 0 counted RAW digits: walk them in value order (negative floats: descending raw digit)
-    for (int o = threadIdx.x; o < nb; o += blockDim.x) ordered[o] = __ldcg(&gh[pass == 0 ? d11_raw_of_order(o) : static_cast<uint32_t>(o)]);
-    __syncthreads();
-    unsigned long long r2, pp;
-    const int d = find_bin(ordered, nb, bs->sel_rank[side], &r2, &pp, s_scan, s_res, s_out);
-    __syncthreads();
+    // pass 0 counted RAW digits: they are read in value order
+    find_bin([&](int o) { return __ldcg(&gh[pass == 0 ? raw_digit_of_order(o, 11) : static_cast<uint32_t>(o)]); }, nb, bs->sel_rank[side],
+             s_scan, s_out);
     if (threadIdx.x == 0) {
+      const int d = static_cast<int>(s_out[0]);
       if (d >= nb) { bs->err |= DERR_POS_RANGE; bs->sel_active[side] = 0; }
       else {
-        bs->sel_rank[side] = r2;
-        if (pass == 0) { bs->sel_prefix[side] = d11_raw_of_order(static_cast<uint32_t>(d)) << 21; bs->sel_cnt[side] = pp; bs->cand_n[side] = 0; }
+        bs->sel_rank[side] = s_out[1];
+        if (pass == 0) { bs->sel_prefix[side] = raw_digit_of_order(static_cast<uint32_t>(d), 11) << 21; bs->sel_cnt[side] = s_out[2]; bs->cand_n[side] = 0; }
         else bs->sel_prefix[side] |= static_cast<uint32_t>(d) << shift;
         if (pass == 2) {
           const uint32_t p = bs->sel_prefix[side];
-          const uint32_t bits = (p & 0xFFE00000u) | ((p & 0x1FFFFFu) ^ ((p >> 21) >= 1024u ? 0x1FFFFFu : 0u));     // un-flip the remainder
-          const float thr = clamp_thr(__uint_as_float(bits));                    // .cu:303 / :334
+          const float thr = clamp_thr(__uint_as_float(p ^ rem_flip(p, 21)));   // .cu:303 / :334
           if (side == 0) bs->posi_global = thr; else bs->nega_global = thr;
         }
       }
@@ -1086,8 +1039,8 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
   __shared__ unsigned int hist[2][NPAIR_SEL_BINS];
   __shared__ uint32_t stage[2][NPAIR_GSEL_STAGE];
   __shared__ unsigned int s_nst[2], s_base[2];
-  __shared__ unsigned long long s_scan[33], s_out[2];
-  __shared__ int s_res, s_last;
+  __shared__ unsigned long long s_scan[32], s_out[3];
+  __shared__ int s_last;
   const bool act0 = (side_mask & 1) && bs->sel_active[0], act1 = (side_mask & 2) && bs->sel_active[1];
   if (!act0 && !act1) return;
   const bool lab_aligned = (reinterpret_cast<uintptr_t>(lab_cols) & 15) == 0;
@@ -1096,7 +1049,7 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
   const uint32_t dm = (1u << nbits) - 1u;
   // sel_prefix after pass 0: raw digit << 21; after pass 1: | flipped-remainder digit << 10
   const uint32_t raw0 = bs->sel_prefix[0] >> 21, raw1 = bs->sel_prefix[1] >> 21;
-  const uint32_t flip0 = raw0 >= 1024u ? 0x1FFFFFu : 0u, flip1 = raw1 >= 1024u ? 0x1FFFFFu : 0u;
+  const uint32_t flip0 = rem_flip(bs->sel_prefix[0], 21), flip1 = rem_flip(bs->sel_prefix[1], 21);
   const uint32_t mid0 = (bs->sel_prefix[0] >> 10) & 0x7FFu, mid1 = (bs->sel_prefix[1] >> 10) & 0x7FFu;   // pass 2: decided second digit
   const bool comp0 = act0 && pass == 1 && bs->sel_cnt[0] <= gb.cap, comp1 = act1 && pass == 1 && bs->sel_cnt[1] <= gb.cap;   // compaction this pass
   const bool list0 = act0 && pass == 2 && bs->sel_cnt[0] <= gb.cap, list1 = act1 && pass == 2 && bs->sel_cnt[1] <= gb.cap;   // read the list this pass
@@ -1225,14 +1178,12 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
   __threadfence();
   if (threadIdx.x == 0) bs->ticket3 = 0;
   if (gb.world_scope) return;
-  global_decide(pass, act0, act1, gb, ra, Q, bs, reinterpret_cast<unsigned long long*>(&hist[0][0]), s_scan, &s_res, s_out);
+  global_decide(pass, act0, act1, gb, ra, Q, bs, s_scan, s_out);
 }
 // world scope: sum the ranks' digit counts (same order on every rank -> identical decisions), then decide like the last block does
 __global__ void __launch_bounds__(512) global_decide_kernel(const float* __restrict__ xall, int xstride, int world, int side_mask, int pass,
                                                             GlobalSelectBufs gb, RowArrays ra, int Q, BlockScalars* bs) {
-  __shared__ unsigned long long ordered[NPAIR_SEL_BINS];
-  __shared__ unsigned long long s_scan[33], s_out[2];
-  __shared__ int s_res;
+  __shared__ unsigned long long s_scan[32], s_out[3];
   const bool act0 = (side_mask & 1) && bs->sel_active[0], act1 = (side_mask & 2) && bs->sel_active[1];
   if (!act0 && !act1) return;
   for (int b = threadIdx.x; b < 2 * NPAIR_SEL_BINS; b += blockDim.x) {
@@ -1244,7 +1195,7 @@ __global__ void __launch_bounds__(512) global_decide_kernel(const float* __restr
     gb.hist[b] = sum;
   }
   __syncthreads();
-  global_decide(pass, act0, act1, gb, ra, Q, bs, ordered, s_scan, &s_res, s_out);
+  global_decide(pass, act0, act1, gb, ra, Q, bs, s_scan, s_out);
 }
 void launch_global_select_pass(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                                int self_offset, int side_mask, int pass, RowArrays ra, unsigned long long* hist, uint32_t* cand,

@@ -106,7 +106,9 @@ struct BlockScalars {
   // radix-select state, one per side (0 = AP over same pairs, 1 = AN over diff pairs)
   unsigned long long sel_rank[2];          // remaining 0-based rank inside the current prefix bucket
   uint32_t sel_prefix[2];                  // ordered-uint prefix decided so far
-  uint32_t sel_mask[2];                    // which bits of the prefix are decided
+  uint32_t reserved_[2];                   // unused; holds the fields below at their offsets (moved 8 bytes down, x_absmax .. x_inv_scale
+                                           // share the first 128-byte line with the tickets, and the B=8192 D=512 step measured ~1 % slower
+                                           // on an H100 80GB HBM3 at 700 W)
   int sel_active[2];                       // 1 while a GLOBAL relative select is in flight
   unsigned long long sel_cnt[2];           // population of the chosen first-digit bucket (GLOBAL select)
   unsigned int cand_n[2];                  // entries of the compact candidate lists (GLOBAL select)

@@ -22,6 +22,13 @@ __device__ __forceinline__ bool pos_index(float sn, unsigned long long size, uns
   if (ip < 0 || static_cast<unsigned long long>(ip) >= size) return false;
   pos = static_cast<unsigned long long>(ip); return true;
 }
+// The position of a relative select in its list of `size` entries; false with DERR_EMPTY_LIST (empty list) or DERR_POS_RANGE (SN puts
+// the position outside the list) added to err
+__device__ __forceinline__ bool side_position(unsigned long long size, float sn, unsigned long long& pos, int& err) {
+  if (pos_index(sn, size, pos)) return true;
+  err |= size == 0 ? DERR_EMPTY_LIST : DERR_POS_RANGE;
+  return false;
+}
 __device__ __forceinline__ float clamp_thr(float v) { return v >= 0.f ? v : -FLT_MAX; }   // .cu:288,303,319,334
 
 __host__ __device__ __forceinline__ bool is_rel(int m) { return m == M_RELATIVE_HARD || m == M_RELATIVE_EASY; }
@@ -62,12 +69,9 @@ __device__ inline void finish_thresholds(unsigned long long n_same, unsigned lon
   for (int side = 0; side < 2; ++side) {
     const bool arm = side == 0 ? arm_ap : arm_an;
     bs->sel_active[side] = 0;
-    if (arm) {
-      unsigned long long pos = 0;
-      const unsigned long long size = side == 0 ? n_same : n_diff;
-      if (size == 0) err |= DERR_EMPTY_LIST;
-      else if (!pos_index(side == 0 ? mp.identsn : mp.diffsn, size, pos)) err |= DERR_POS_RANGE;
-      else { bs->sel_active[side] = 1; bs->sel_rank[side] = pos; bs->sel_prefix[side] = 0; bs->sel_mask[side] = 0; }
+    unsigned long long pos = 0;
+    if (arm && side_position(side == 0 ? n_same : n_diff, side == 0 ? mp.identsn : mp.diffsn, pos, err)) {
+      bs->sel_active[side] = 1; bs->sel_rank[side] = pos; bs->sel_prefix[side] = 0;
     }
   }
   bs->err |= err;

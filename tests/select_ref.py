@@ -97,7 +97,7 @@ def _order_of_digit(d, bits):
 
 def bucket_of_rank(vals, p, bits):
     """The raw `bits`-bit leading digit (sign, exponent, top mantissa bits) of the bucket that holds 0-based rank p of `vals`, found by
-    walking the bucket counts in value order (the rule of d11_raw_of_order / d1_raw_of_order), and that bucket's population."""
+    walking the bucket counts in value order (the rule of raw_digit_of_order), and that bucket's population."""
     half = 1 << (bits - 1)
     hist = np.bincount(_order_of_digit(_digit(vals, bits), bits), minlength=2 * half)
     o = int(np.searchsorted(np.cumsum(hist), p, side="right"))
