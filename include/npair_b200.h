@@ -17,7 +17,12 @@
  * Conventions: plain pointers and sizes, no C++ or torch types; every function returns 0 on success or a
  * negative NPAIR_E_* code, with a human-readable message from npair_last_error().  No exceptions cross the ABI.
  * Device pointers are on the context's device; `stream` is a cudaStream_t passed as void* (NULL = legacy default).
- * A context is not re-entrant; use one per rank (one process per GPU).
+ * A context is not re-entrant; use one per rank (one process per GPU).  Successive calls may pass different streams: a context records
+ * an event behind every call's work, and a call on another stream than the previous call first makes its stream wait for it, so the
+ * context's own scratch is never rewritten while an earlier call's kernels read it (a call on the same stream adds no wait).  The
+ * caller still orders its own buffers (inputs, gradient outputs) across streams.  A stream is recognised by its handle: a stream destroyed
+ * while the context's work on it may still run, and a new stream that reuses the handle, look like one stream, so synchronise (or pass
+ * the context another stream) before destroying one it used.  An evaluator (npair_eval) orders its calls the same way.
  */
 #ifndef NPAIR_B200_H_
 #define NPAIR_B200_H_
@@ -204,7 +209,7 @@ unsigned long long npair_kernel_launches(void);
 int npair_util_f64_to_f32(const double* d_src, float* d_dst, size_t n, void* stream);
 int npair_util_f32_to_f64(const float* d_src, double* d_dst, size_t n, void* stream);
 
-/* Introspection for parity tests (copies device scratch to host; synchronises the context's last stream).
+/* Introspection for parity tests (copies device scratch to host; waits for the work of the context's last call, on any stream).
  * which: 0 = S (Q x N similarities, row-major, ld = N; NPAIR_E_STATE in row-block similarity mode)      1 = posi_thr[Q]   2 = nega_thr[Q]
  *        3 = min_within[Q]  4 = max_between[Q]  5 = max_all[Q]  6 = A[Q]  7 = T[Q]  8 = same-label count[Q]
  *        9 = max_within[Q]  10 = operand pre-scale (1 float) */

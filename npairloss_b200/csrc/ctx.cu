@@ -581,6 +581,41 @@ struct DevMem {
   std::vector<void*> held;
 };
 
+// The order of a context's (or an evaluator's) calls across the caller's streams.  Every call that enqueues work records `done` on its
+// stream behind that work, and a call on another stream first makes its stream wait for `done`: the scratch buffers are the object's
+// own, so the caller cannot order around them.  Calls on the stream of the previous call enqueue nothing extra beyond the record.
+struct StreamOrder {
+  StreamOrder() = default;
+  StreamOrder(const StreamOrder&) = delete;
+  ~StreamOrder() { if (done) cudaEventDestroy(done); }
+  cudaError_t create() { return cudaEventCreateWithFlags(&done, cudaEventDisableTiming); }
+  // Records `done` behind the current call's work on `st`, once per call: a call that waits on the host for its results (the
+  // forward's tops) marks before it waits, the others when they return
+  void mark(cudaStream_t st) {
+    if (!open) return;
+    open = false;
+    if (cudaEventRecord(done, st) == cudaSuccess) { stream = st; recorded = true; }
+  }
+  cudaEvent_t done = nullptr;
+  cudaStream_t stream = nullptr;      // the stream `done` was last recorded on
+  bool recorded = false;
+  bool open = false;                  // a call has entered and not yet marked
+};
+// One call's work on `st`: enter() waits for the previous call when that ran on another stream; `done` is recorded at the latest when
+// the call returns, also after an error (what it enqueued before failing is still running)
+struct OrderedCall {
+  OrderedCall(StreamOrder& o_, cudaStream_t st_) : o(o_), st(st_) {}
+  OrderedCall(const OrderedCall&) = delete;
+  cudaError_t enter() {
+    const cudaError_t e = o.recorded && o.stream != st ? cudaStreamWaitEvent(st, o.done, 0) : cudaSuccess;
+    o.open = e == cudaSuccess;
+    return e;
+  }
+  ~OrderedCall() { o.mark(st); }
+  StreamOrder& o;
+  cudaStream_t st;
+};
+
 // The statistics of RowArrays, which the evaluator's queries have too: four ordered-uint statistics and the same-label count per row
 static void carve_stats(Carve& cv, long long rows, RowArrays* ra) {
   ra->st_minw = cv.take<uint32_t>(rows); ra->st_maxw = cv.take<uint32_t>(rows); ra->st_maxb = cv.take<uint32_t>(rows);
@@ -642,7 +677,7 @@ struct npair_ctx : Plan {
   const float* y_local = nullptr;   // normalize_input: this rank's normalised rows
   const float *x_total = nullptr, *lab_total = nullptr;
   bool fwd_done = false;
-  cudaStream_t last_stream = nullptr;
+  StreamOrder order;              // the calls' order across streams; debug_read and profile_read wait for its event
   std::string err;
   // optional per-phase CUDA-event timing (npair_profile_enable)
   bool prof = false;
@@ -888,6 +923,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   CREATE_TRY(cudaHostAlloc(&c->tops_pinned, 64, cudaHostAllocMapped));
   memset(c->tops_pinned, 0, 64);
   CREATE_TRY(cudaHostGetDevicePointer(&c->tops_dev, c->tops_pinned, 0));
+  CREATE_TRY(c->order.create());
   // the dynamic shared memory of the kernels this context launches, allowed on its device
   if (c->lsel_mask) CREATE_TRY(allow_local_select_smem());
   if (cfg->gemm_backend == NPAIR_GEMM_TCGEN05) {
@@ -1021,6 +1057,7 @@ static MiningParams mining_of(const npair_config& c) {
 // after ~2 s fall back to the synchronisation, which reports the error.  Then the device error bits become the return code, and the
 // tops are copied out.
 static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
+  c->order.mark(st);                               // everything of the call is enqueued: the event goes in before the host waits
   volatile unsigned int* seqp = reinterpret_cast<volatile unsigned int*>(c->tops_pinned) + 6;
   unsigned long long spins = 0;
   while (*seqp != c->tops_seq) {
@@ -1037,13 +1074,21 @@ static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
 }
 
 static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st);
+static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st);
 
 int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  c->fwd_done = false; c->last_stream = st; c->ext_gathered = false;
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
+  return forward_rank(c, d_feat, d_label, tops_host, st);
+}
+
+// npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward
+static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st) {
+  c->fwd_done = false; c->ext_gathered = false;
   const int Q = c->Q, D = c->D;
   if (c->cfg.normalize_input) {               // fused L2Normalize producer (usage/def.prototxt:115-120): the layer works on x / ||x||
     PhaseTimer pt(c, 1, st);
@@ -1080,7 +1125,9 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
   if (!d_feat_total || !d_label_total || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  c->fwd_done = false; c->last_stream = st; c->ext_gathered = true;
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
+  c->fwd_done = false; c->ext_gathered = true;
   if (c->cfg.normalize_input) {               // the gathered bottoms are raw embeddings: normalise all N rows (1 / ||x|| kept for the local ones)
     PhaseTimer pt(c, 1, st);
     float* dst = c->world > 1 ? c->Xtot_buf : c->Ynorm;
@@ -1246,7 +1293,8 @@ int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream)
   if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator: use npair_backward_partial / npair_backward_gathered"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  c->last_stream = st;
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
   return backward_impl(c, loss_weight, d_diff, nullptr, nullptr, st);
 }
 
@@ -1261,14 +1309,18 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
   if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
   if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
   c->defer_sync = true;
-  int rc = npair_forward(c, d_feat, d_label, tops_host, stream);
+  int rc = forward_rank(c, d_feat, d_label, tops_host, st);
   c->defer_sync = false;
   if (rc != NPAIR_OK) return rc;
   c->fwd_done = true;                                  // enqueued; confirmed (or revoked) after the synchronisation below
   rc = backward_impl(c, loss_weight, d_diff, nullptr, nullptr, st);
   if (rc != NPAIR_OK) { c->fwd_done = false; return rc; }
-  // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step
+  // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step.
+  // finish_forward records `done` behind the backward
   rc = finish_forward(c, tops_host, st);
   if (rc != NPAIR_OK) c->fwd_done = false;
   return rc;
@@ -1288,15 +1340,19 @@ int npair_backward_partial(npair_ctx* c, float loss_weight, float* d_local_half,
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  c->last_stream = st;
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
   return backward_impl(c, loss_weight, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, st);
 }
 
 int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
   if (!c || !d_out) return NPAIR_E_ARG;
   if (!c->fwd_done) { c->err = "npair_row_scalars called without a successful forward"; return NPAIR_E_STATE; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowrec, sizeof(RowRecord) * c->Q, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
+  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowrec, sizeof(RowRecord) * c->Q, cudaMemcpyDeviceToDevice, st));
   return NPAIR_OK;
 }
 
@@ -1308,7 +1364,8 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
   if (c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(c, cudaSetDevice(c->device));
-  c->last_stream = st;
+  OrderedCall oc(c->order, st);
+  CUDA_TRY(c, oc.enter());
   return backward_impl(c, loss_weight, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), st);
 }
 
@@ -1433,7 +1490,7 @@ unsigned long long npair_kernel_launches(void) { return npair::g_kernel_launches
 int npair_profile_read(npair_ctx* c, float* ms_out) {
   if (!c || !ms_out) return NPAIR_E_ARG;
   CUDA_TRY(c, cudaSetDevice(c->device));
-  CUDA_TRY(c, cudaStreamSynchronize(c->last_stream));
+  CUDA_TRY(c, cudaEventSynchronize(c->order.done));
   for (int i = 0; i < NPAIR_PROF_PHASES; ++i) {
     ms_out[i] = 0.f;
     if (c->ev_made && c->ev_used[i]) { float ms = 0.f; CUDA_TRY(c, cudaEventElapsedTime(&ms, c->ev[i][0], c->ev[i][1])); ms_out[i] = ms; }
@@ -1454,7 +1511,7 @@ __global__ void int_to_float_kernel(const int* __restrict__ in, float* __restric
 int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
   if (!c || !dst) return NPAIR_E_ARG;
   CUDA_TRY(c, cudaSetDevice(c->device));
-  CUDA_TRY(c, cudaStreamSynchronize(c->last_stream));
+  CUDA_TRY(c, cudaEventSynchronize(c->order.done));
   const int Q = c->Q, N = c->N;
   if (which == 0) {
     if (c->n_blocks > 1) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
@@ -1631,6 +1688,7 @@ struct npair_eval : EvalPlan {
   // MAP@R (MapRows, MapPairs) and k-means (KmeansBufs) buffers, grown on demand and kept
   DevMem map_rows_mem, map_pairs_mem, km_mem;
   char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr;
+  StreamOrder order;              // the calls' order across streams
   std::string err;
 };
 
@@ -1719,6 +1777,7 @@ int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int
   static_cast<EvalPlan&>(*ev) = eval_plan_of(max_q, max_g, D, prec);
   ev->device = dev; ev->sms = sms;
   CREATE_TRY(eval_buffers(ev, ev->mem));
+  CREATE_TRY(ev->order.create());
   const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
                       EPI_BUCKET | EPI_SYM, EPI_ARGMAX};
   for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
@@ -1799,6 +1858,8 @@ int npair_eval_rank(npair_eval* ev, const float* q, const float* ql, int32_t nq,
   if (!ql || !gl || !d_rank) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
+  OrderedCall oc(ev->order, st);
+  CUDA_TRY(ev, oc.enter());
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   float* cut = reinterpret_cast<float*>(ev->ra.st_minw);   // p* overwrites a statistic sweep 2 does not read
@@ -1819,6 +1880,8 @@ int npair_eval_best_positive(npair_eval* ev, const float* q, const float* ql, in
   if (!ql || !gl || !d_best) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
+  OrderedCall oc(ev->order, st);
+  CUDA_TRY(ev, oc.enter());
   const int self_col = eval_self_col(self_offset, gallery_row0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
@@ -1836,6 +1899,8 @@ int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g,
   if (!d_cut || !d_count) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
+  OrderedCall oc(ev->order, st);
+  CUDA_TRY(ev, oc.enter());
   const int self_col = eval_self_col(self_offset, gallery_row0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
@@ -1857,6 +1922,8 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
   if (!ql || !gl || !d_map_r || !d_r_precision) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
+  OrderedCall oc(ev->order, st);
+  CUDA_TRY(ev, oc.enter());
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_grow(ev, ev->map_rows_mem, &ev->map_rows, MapRows(nullptr, nq).bytes, "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
@@ -1912,6 +1979,8 @@ int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, cons
     if (init_rows[c] < 0 || init_rows[c] >= n) { ev->err = fmt("init_rows[%d] = %d is not a row of x", c, init_rows[c]); return NPAIR_E_ARG; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(ev, cudaSetDevice(ev->device));
+  OrderedCall oc(ev->order, st);
+  CUDA_TRY(ev, oc.enter());
   int rc;
   if ((rc = eval_grow(ev, ev->km_mem, &ev->km, KmeansBufs(nullptr, n, k, ev->D).bytes, "the k-means buffers")) != NPAIR_OK) return rc;
   const long long D = ev->D;

@@ -70,9 +70,12 @@ def gpu_step_world(x, lab, Q, world, mining, prec, backend, loss_weight=1.0, num
     return dict(tops=tops, dx=dx, S=S, posi=posi, nega=nega, mode=mode)
 
 
-def check_parity(oracle, x, lab, Q, world, mining, prec, backend, loss_weight=1.0, num_tops=5, tag="", bwd_exchange=0, **cfg_extra):
+def check_parity(oracle, x, lab, Q, world, mining, prec, backend, loss_weight=1.0, num_tops=5, tag="", bwd_exchange=0, gpu=None,
+                 **cfg_extra):
+    """gpu: a result of gpu_step_world with these arguments, to check instead of running the step again."""
     N, D = x.shape
-    g = gpu_step_world(x, lab, Q, world, mining, prec, backend, loss_weight, num_tops, bwd_exchange=bwd_exchange, **cfg_extra)
+    g = gpu if gpu is not None else gpu_step_world(x, lab, Q, world, mining, prec, backend, loss_weight, num_tops,
+                                                   bwd_exchange=bwd_exchange, **cfg_extra)
     if g["mode"] != 1:
         # single-rank symmetric tiles / row-scalar exchange both rely on a bitwise symmetric similarity matrix
         assert np.array_equal(g["S"], g["S"].T), f"{tag} S is not bitwise symmetric (mode {g['mode']})"

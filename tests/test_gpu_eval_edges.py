@@ -360,10 +360,33 @@ SCRIPT = [("rank", 600, 0, 1), ("map", 300, 0, 1), ("map_full", 300, 0, 1), ("ra
           ("kmeans", 200, 7, 2.0 ** -16), ("rank", 600, 0, 2.0 ** -16), ("rank_full", 600, 0, 1), ("map", 31, 0, 1), ("rank", 600, 0, 1)]
 
 
+NO_WAIT = 12        # before this step, the device holds the 600-row symmetric tile list (steps 10 and 11)
+
+
+def _unordered_calls(torch, ev, x, lab, side, fresh):
+    """A rank call on the main stream queued behind a sleep, then at once a rank call on `side` with no wait_stream before it.  The
+    queued call (600 rows, symmetric tiles) finds its tile list already on the device and does not upload it; the side call (300
+    rows) uploads its own, shorter and different, list into the same buffer.  The evaluator must make the side call wait for the
+    queued one: otherwise the side call runs during the sleep, and the queued call then sweeps the 300-row list's tiles."""
+    assert SCRIPT[NO_WAIT - 2][:2] == ("rank", 600) and SCRIPT[NO_WAIT - 1][:2] == ("rank_full", 600)
+    assert SCRIPT[0] == ("rank", 600, 0, 1) and SCRIPT[3] == ("rank", 300, 0, 1)
+    xq, lq = torch.from_numpy(x[:600]).cuda(), torch.from_numpy(lab[:600]).cuda()
+    xs, ls = torch.from_numpy(x[:300]).cuda(), torch.from_numpy(lab[:300]).cuda()
+    torch.cuda.synchronize()
+    torch.cuda._sleep(100_000_000)                      # about 50 ms
+    queued = ev.rank(xq, lq, xq, lq, 0)
+    with torch.cuda.stream(side):
+        unwaited = ev.rank(xs, ls, xs, ls, 0)
+    torch.cuda.synchronize()
+    assert _bytes(queued) == fresh[0], "the rank call queued on the main stream"
+    assert _bytes(unwaited) == fresh[3], "the side-stream call issued without a wait"
+
+
 @pytest.mark.parametrize("prec", PRECS, ids=PREC_NAME.get)
 def test_long_lived_evaluator(prec):
     """rank -> map_at_r -> kmeans -> best_positive / count -> rank on one evaluator with spare capacity: shrinking and growing sizes,
-    symmetric and full tiles at one n, max|x| changing by 2^16 between calls (the fp16x2 pre-scale), the second half on a side stream.
+    symmetric and full tiles at one n, max|x| changing by 2^16 between calls (the fp16x2 pre-scale), the second half on a side stream,
+    and one side-stream call issued without a wait while a call on the main stream is still queued (_unordered_calls).
     Each result is bit for bit that of a fresh evaluator made for exactly that call: nothing the evaluator keeps between calls (the
     symmetric tile list, the absmax word, the error word, the grown MAP@R and k-means buffers) leaks into the next one."""
     import torch
@@ -381,6 +404,8 @@ def test_long_lived_evaluator(prec):
     side = torch.cuda.Stream()
     try:
         for i, step in enumerate(SCRIPT):
+            if i == NO_WAIT:
+                _unordered_calls(torch, ev, x, lab, side, fresh)
             if i < len(SCRIPT) // 2:
                 got = _call(ev, step, x, lab)
             else:
