@@ -434,7 +434,8 @@ void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars
 // already narrows the k-th element down to a few percent of the row: those CANDIDATES are compacted (21-bit remainders) and the
 // last two digits are decided on the compact list -- S is read once from HBM (LOCAL: one more time from L1/L2; GLOBAL: twice).
 // Both sides (same-label list for AP, diff-label list for AN) are handled in the same sweep when both are relative.
-// The self pair is counted by the vectorised sweep and taken out again by one thread (it is always a same-label entry).
+// The self pair is in neither list, whatever its label (.cu:54): it is recognised by its column, never by its label, since a NaN
+// label is not equal to itself.
 // --------------------------------------------------------------------------------------------
 #define NPAIR_SEL_BINS 2048
 
@@ -705,8 +706,9 @@ __global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(
 // The warp-per-row kernel above is bound by its instruction count and by its few warps in flight (ncu: 56 M warp instructions, 29 %
 // issue slots with 16 warps per SM).  This kernel holds a row in the registers of 256 threads (8 independent 16-byte loads each, S is
 // read ONCE) and bins by VALUE with three instructions per entry:
-//   pass 0   label test: entries with the row's label (the self pair among them) go to the short same-label list and are replaced by
-//            NaN in the registers -- fminf / fmaxf skip NaN, so the value range [lo, hi] of the entries that stay needs no branch
+//   pass 0   label test: entries with the row's label go to the short same-label list, and they and the self pair (by column: a
+//            NaN-labelled row's self pair has no label match) are replaced by NaN in the registers -- fminf / fmaxf skip NaN, so the
+//            value range [lo, hi] of the entries that stay needs no branch
 //   pass 1   bin*4 = mantissa of fmaf(s, 4*2048/(hi-lo), 2^23 + 4 - lo*that): one FFMA, one AND, one shared-memory reduction.  The map
 //            is monotone in s, so the wanted rank lies in the bin where the running count crosses it; bins hold a few dozen entries and
 //            lanes rarely collide.  NaN lands in bin 4095, which nobody reads.
@@ -811,13 +813,12 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
       if (jj < n4) {
         const float4 l = __ldg(reinterpret_cast<const float4*>(lab_cols + jj));
         const float ll[4] = {l.x, l.y, l.z, l.w};
-        if (l.x == li || l.y == li || l.z == li || l.w == li) {
+        if (static_cast<unsigned int>(self_col - jj) < 4u || l.x == li || l.y == li || l.z == li || l.w == li) {
 #pragma unroll
-          for (int c = 0; c < 4; ++c)
-            if (ll[c] == li) {
-              if (jj + c != self_col) same_append(&B.n_same, B.same, v[4 * u + c]);
-              v[4 * u + c] = kNaN;
-            }
+          for (int c = 0; c < 4; ++c) {
+            if (ll[c] == li && jj + c != self_col) same_append(&B.n_same, B.same, v[4 * u + c]);
+            if (ll[c] == li || jj + c == self_col) v[4 * u + c] = kNaN;
+          }
         }
 #pragma unroll
         for (int c = 0; c < 4; ++c) { mn = fminf(mn, __uint_as_float(v[4 * u + c])); mx = fmaxf(mx, __uint_as_float(v[4 * u + c])); }
@@ -825,10 +826,9 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     }
     if (has_tail) {
       const int j = n4 + tid;
-      if (lab_cols[j] == li) {
-        if (j != self_col) same_append(&B.n_same, B.same, v[4 * NPAIR_LSB_VPT]);
-        v[4 * NPAIR_LSB_VPT] = kNaN;
-      }
+      const bool same = lab_cols[j] == li;
+      if (same && j != self_col) same_append(&B.n_same, B.same, v[4 * NPAIR_LSB_VPT]);
+      if (same || j == self_col) v[4 * NPAIR_LSB_VPT] = kNaN;
       mn = fminf(mn, __uint_as_float(v[4 * NPAIR_LSB_VPT])); mx = fmaxf(mx, __uint_as_float(v[4 * NPAIR_LSB_VPT]));
     }
 #pragma unroll
@@ -1098,7 +1098,8 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
         if (j4 >= N) continue;
         const uint32_t vv[4] = {vq[u].x, vq[u].y, vq[u].z, vq[u].w};
         const float* ll = lq[u];
-        if (j4 + 3 < N && ll[0] != li && ll[1] != li && ll[2] != li && ll[3] != li) {     // four diff-label pairs: the common case
+        const bool no_self = self_col < j4 || self_col > j4 + 3;
+        if (j4 + 3 < N && no_self && ll[0] != li && ll[1] != li && ll[2] != li && ll[3] != li) {     // four diff-label pairs: the common case
           if (sweep1) {
             if (pass == 0) {
 #pragma unroll

@@ -24,6 +24,22 @@ import torch
 from . import capi
 
 
+def _fp32_labels(label):
+    """Labels as the library compares them: fp32.  Any numeric dtype is accepted whose values fp32 holds exactly; a value it does not
+    (an int64 id above 2^24 that would round onto its neighbour, a float64 fraction) raises ValueError instead of silently merging two
+    classes.  fp32 labels pass unchanged, NaN included."""
+    lab = label.to(torch.float32)
+    if label.dtype != torch.float32:
+        exact = lab.to(label.dtype) == label
+        if label.is_floating_point():
+            exact |= torch.isnan(label)
+        if not bool(exact.all()):
+            bad = label[~exact].reshape(-1)[0].item()
+            raise ValueError(f"labels of dtype {label.dtype} that fp32 cannot hold exactly (e.g. {bad!r}); the library compares labels in "
+                             "fp32, so such labels would merge classes: renumber them as integers below 2^24")
+    return lab
+
+
 class _NPairFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, label, owner):
@@ -82,7 +98,7 @@ class NPairLoss(torch.nn.Module):
         if feat.dtype != torch.float32:
             raise TypeError("NPairLoss computes in fp32 like the reference (Dtype=float); cast the embeddings")
         feat2 = feat.reshape(feat.shape[0], -1).contiguous()
-        label = label.to(torch.float32).contiguous()          # labels are stored as Dtype in the reference (bottom[1])
+        label = _fp32_labels(label).contiguous()               # labels are stored as Dtype in the reference (bottom[1])
         loss, tops = _NPairFunction.apply(feat2, label, self)
         return loss, tops
 
@@ -93,8 +109,8 @@ def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), preci
 
     gallery=None: self-retrieval, every query against all the others.  Otherwise query/gallery with disjoint sets, or, with
     `self_offset` = k, queries that are gallery rows k, k+1, ...  Takes CUDA fp32 embeddings as given (L2-normalise them first for
-    cosine similarity); labels of any numeric dtype.  Returns ({K: recall}, rank) with rank the int32 CUDA tensor of the best
-    positive's rank per query (0: the query has no positive)."""
+    cosine similarity); labels of any numeric dtype whose values fp32 holds exactly (ValueError otherwise).  Returns ({K: recall},
+    rank) with rank the int32 CUDA tensor of the best positive's rank per query (0: the query has no positive)."""
     q, ql, g, gl, off = _retrieval_sets("recall_at_k", query, qlabel, gallery, glabel, self_offset)
     ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
     try:
@@ -139,8 +155,8 @@ def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi
     """NMI and F1 of a k-means clustering of a whole embedding set, the clustering half of the metric-learning protocol (Sohn 2016;
     Song et al. 2016), with Lloyd's k-means on the tensor cores (Evaluator.kmeans, DESIGN 8.2; not part of the reference layer).
 
-    Takes CUDA fp32 embeddings as given (L2-normalise them first for cosine geometry) and labels of any numeric dtype, compared as
-    floats.  k=None: the number of distinct labels.  Centroid c starts as row init[c] of
+    Takes CUDA fp32 embeddings as given (L2-normalise them first for cosine geometry) and labels of any numeric dtype that fp32 holds
+    exactly (ValueError otherwise), compared as floats.  k=None: the number of distinct labels.  Centroid c starts as row init[c] of
     init = torch.randperm(n, generator=torch.Generator().manual_seed(seed))[:k], so the same seed gives the same result; there is
     one run, no restarts.  Returns ({"nmi", "f1", "inertia", "iterations", "converged", "empty_clusters"}, assign, centroids) with
     the scores of clustering_scores, "converged" whether the last sweep changed no assignment, and assign / centroids CUDA tensors."""
@@ -164,13 +180,13 @@ def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi
 
 
 def clustering_scores(labels, assign):
-    """(NMI, F1) of the clustering `assign` against `labels` (compared as floats), by fp64 / int64 bookkeeping over the non-zero
-    cells of the contingency table, on the tensors' device.
+    """(NMI, F1) of the clustering `assign` against `labels` (compared as fp32 floats; ValueError for labels fp32 cannot hold
+    exactly), by fp64 / int64 bookkeeping over the non-zero cells of the contingency table, on the tensors' device.
       NMI = 2 I(Y;C) / (H(Y) + H(C)), natural log, over the non-empty clusters; 1.0 when both entropies are 0.
       F1  = pairwise: TP = sum over cells of C(n_lc, 2), precision = TP / sum_c C(n_c, 2), recall = TP / sum_l C(n_l, 2); a 0/0 term
             counts as 0, and F1 = 0 when precision + recall = 0.
     Each entropy and the mutual information sum their terms in ascending order, so a perfect clustering gives exactly 1.0."""
-    lab = labels.reshape(-1).to(torch.float32)
+    lab = _fp32_labels(labels.reshape(-1))
     a = assign.reshape(-1).to(device=lab.device, dtype=torch.int64)
     if lab.numel() != a.numel():
         raise ValueError("labels and assign differ in length")
@@ -205,7 +221,7 @@ def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
     if not query.is_cuda or query.dtype != torch.float32:
         raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
     q = query.reshape(query.shape[0], -1).contiguous()
-    ql = qlabel.to(device=q.device, dtype=torch.float32).contiguous()
+    ql = _fp32_labels(qlabel.to(q.device)).contiguous()
     if gallery is None:
         if glabel is not None:
             raise ValueError("glabel without gallery")
@@ -216,7 +232,7 @@ def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
         if not gallery.is_cuda or gallery.dtype != torch.float32:
             raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
         g = gallery.reshape(gallery.shape[0], -1).contiguous()
-        gl = glabel.to(device=q.device, dtype=torch.float32).contiguous()
+        gl = _fp32_labels(glabel.to(q.device)).contiguous()
         off = -1 if self_offset is None else self_offset
     if g.shape[1] != q.shape[1]:
         raise ValueError("query and gallery dimensions differ")

@@ -69,6 +69,34 @@ def test_second_forward_invalidates_the_first_graph():
         raise AssertionError("stale backward must raise")
 
 
+def test_labels_fp32_cannot_hold_are_refused():
+    """The library compares labels in fp32: int64 ids that round onto each other, or float64 fractions, would merge classes."""
+    made = []
+    m = torch_api.NPairLoss(_context_factory=lambda c, n: made.append(FakeContext(c, n)) or made[-1])
+    x = torch.randn(2, 4)
+    for bad in (torch.tensor([2 ** 24, 2 ** 24 + 1], dtype=torch.int64), torch.tensor([0.1, 1.0], dtype=torch.float64)):
+        try:
+            m(x, bad)
+        except ValueError as e:
+            assert "fp32" in str(e)
+        else:
+            raise AssertionError(f"labels {bad.tolist()} ({bad.dtype}) must be refused")
+    assert not made or not made[0].calls, "a refused batch reached the library"
+    ok = torch.tensor([2 ** 24 - 1, -(2 ** 24) + 1], dtype=torch.int64)
+    m(x, ok)
+    m(x, torch.tensor([0.5, float("inf")], dtype=torch.float64))
+    nan = torch.tensor([float("nan"), 3.0], dtype=torch.float32)
+    assert torch_api._fp32_labels(nan) is nan or torch.equal(torch_api._fp32_labels(nan).view(torch.int32), nan.view(torch.int32))
+    assert torch.equal(torch_api._fp32_labels(torch.tensor([float("nan"), 2.0], dtype=torch.float64)).isnan(), torch.tensor([True, False]))
+    assert [c[0] for c in made[0].calls] == ["fwd", "fwd"] and made[0].calls[0][4] == torch.float32
+    for bad in (torch.tensor([2 ** 24, 2 ** 24 + 1]), torch.tensor([0.1], dtype=torch.float64)):
+        try:
+            torch_api.clustering_scores(bad, torch.zeros(bad.numel(), dtype=torch.int64))
+        except ValueError:
+            continue
+        raise AssertionError("clustering_scores must refuse labels fp32 cannot hold")
+
+
 def test_true_gradient_doubles_the_reference_value():
     m = torch_api.NPairLoss(true_gradient=True, _context_factory=lambda c, n: FakeContext(c, n))
     x = torch.randn(4, 3, requires_grad=True)
