@@ -414,6 +414,9 @@ static XchgLayout xchg_layout(int Q, int D, int world, bool world_scope) {
   l.floats = o + round_up(6ll * world, 4);
   return l;
 }
+// XCH is read as 64-bit fields (BlockStats, TopSums, digit counts): every part before it spans an even number of floats (it is two
+// parity buffers), and so does each rank's slot, so every slot is 8-byte aligned
+static_assert(NPAIR_XCH_FLOATS % 2 == 0, "XCH slots hold 64-bit fields");
 // Index of the flag `rank` raises after an exchange of `kind` into the buffers of parity `par`; rank 0's starts the world's flags
 enum { XCHG_FEATURES, XCHG_RECORDS, XCHG_SMALL };
 static inline int xchg_flag(int kind, int par, int world, int rank) { return (2 * kind + par) * world + rank; }
@@ -481,7 +484,6 @@ struct Plan {
   int s_rows;                    // rows of the S buffer: all Q (S materialised), or one block in row-block similarity mode
   int n_blocks;                  // blocks of s_rows rows that the row pass and the fused gradient walk; 1: S materialised
   int sweep_epi;                 // the forward's similarity sweep: statistics, + symmetric tiles, + stores to S if there is one block
-  bool fuse_thr;                 // the threshold pick runs in the sweep's last CTA (not in world scope: it needs the world's statistics)
   bool wscope;                   // world-scope mode: global_scope at world > 1
   int lsel_mask, gsel_mask;      // radix selects (select_mask) of the LOCAL / GLOBAL region
   bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
@@ -501,7 +503,6 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.s_rows = blk_rows ? blk_rows : cfg.Q;
   p.n_blocks = (cfg.Q + p.s_rows - 1) / p.s_rows;
   p.wscope = cfg.global_scope && multi;
-  p.fuse_thr = tc && !p.wscope;
   p.lsel_mask = select_mask(cfg, NPAIR_LOCAL);
   p.gsel_mask = select_mask(cfg, NPAIR_GLOBAL);
   // The row-record exchange needs S[j][m] on rank r to equal S[m][j] on the rank that owns row m BIT FOR BIT, i.e. a tensor-core
@@ -666,9 +667,9 @@ struct npair_ctx : Plan {
   float* partial = nullptr;
   unsigned long long* ghist = nullptr;   // [2][2048] 64-bit digit counts of the GLOBAL radix select
   uint32_t* gcand = nullptr;     // [2][gcand_cap] compacted candidates of the GLOBAL radix select
-  float* tops_pinned = nullptr;  // host-mapped: 5 tops + err(int) + sequence number of the forward that wrote them
+  TopsBlock* tops_pinned = nullptr;   // host-mapped
   unsigned int tops_seq = 0;
-  float* tops_dev = nullptr;
+  TopsBlock* tops_dev = nullptr;
   CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_kcat)
   // nccl
   void* comm = nullptr; bool own_comm = false;
@@ -920,8 +921,8 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     const std::vector<int2> tl = sym_tile_list(Q, N);
     CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), sizeof(int2) * tl.size(), cudaMemcpyHostToDevice));
   }
-  CREATE_TRY(cudaHostAlloc(&c->tops_pinned, 64, cudaHostAllocMapped));
-  memset(c->tops_pinned, 0, 64);
+  CREATE_TRY(cudaHostAlloc(&c->tops_pinned, sizeof(TopsBlock), cudaHostAllocMapped));
+  memset(c->tops_pinned, 0, sizeof(TopsBlock));
   CREATE_TRY(cudaHostGetDevicePointer(&c->tops_dev, c->tops_pinned, 0));
   CREATE_TRY(c->order.create());
   // the dynamic shared memory of the kernels this context launches, allowed on its device
@@ -1058,7 +1059,7 @@ static MiningParams mining_of(const npair_config& c) {
 // tops are copied out.
 static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
   c->order.mark(st);                               // everything of the call is enqueued: the event goes in before the host waits
-  volatile unsigned int* seqp = reinterpret_cast<volatile unsigned int*>(c->tops_pinned) + 6;
+  volatile unsigned int* seqp = &c->tops_pinned->seq;
   unsigned long long spins = 0;
   while (*seqp != c->tops_seq) {
     if (++spins > (1ull << 28)) { CUDA_TRY(c, cudaStreamSynchronize(st)); if (*seqp != c->tops_seq) { c->err = "the forward kernels finished without publishing their results"; return NPAIR_E_CUDA; } break; }
@@ -1066,10 +1067,10 @@ static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
     if ((spins & 0x3FFull) == 0) sched_yield();   // ranks that share a core (fewer cores than ranks, an inherited binding) take turns quickly
   }
   __sync_synchronize();
-  const int derr = reinterpret_cast<int*>(c->tops_pinned)[5];
+  const int derr = c->tops_pinned->err;
   if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
   if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
-  for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned[t] : 0.f;
+  for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned->tops[t] : 0.f;
   return NPAIR_OK;
 }
 
@@ -1157,7 +1158,8 @@ static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_
   gp.a_row0 = r0; gp.S = c->S; gp.ldS = c->ldS;
   if (epi & EPI_STATS) {
     gp.lab_rows = c->cur_label; gp.lab_cols = c->lab_total; gp.self_offset = c->rank * c->Q;
-    gp.fuse_thr = c->fuse_thr ? 1 : 0; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
+    gp.fuse_thr = 1; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
+    gp.thr_out = c->wscope ? reinterpret_cast<BlockStats*>(c->xch_src) : nullptr;   // world scope: the rank's record for the exchange
   }
   return launch_gemm(c->prec, epi, c->tm_simA, c->tm_simB, c->tm_S, gp, c->sms, st);
 }
@@ -1205,10 +1207,11 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
   // ---- thresholds (.cu:275-337) ----
   {
     PhaseTimer pt(c, 3, st);
-    if (!c->fuse_thr) launch_thresholds(c->ra, Q, N, mp, c->bs, c->partial, c->wscope ? c->xch_src : nullptr, st);
+    // the tensor-core similarity sweep picked them in its last CTA, in world scope up to the exchange of its statistics
+    if (c->cfg.gemm_backend != NPAIR_GEMM_TCGEN05) launch_thresholds(c->ra, Q, N, mp, c->bs, st);
     if (c->wscope) {
       const float* all = nullptr;
-      const int rc = xchg_small(c, c->xch_src, 8, &all, st);
+      const int rc = xchg_small(c, c->xch_src, sizeof(BlockStats) / sizeof(float), &all, st);
       if (rc != NPAIR_OK) return rc;
       launch_thresholds_world(all, NPAIR_XCH_FLOATS, c->world, N, mp, c->bs, st);
     }
@@ -1238,12 +1241,12 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
       if (c->lsel_mask && c->n_blocks > 1) local_select(c, r0, rows, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
       launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
-                      c->wscope ? c->xch_src : nullptr, c->tops_seq, r0, rows, c->n_blocks == 1, st);
+                      c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr, c->tops_seq, r0, rows, c->n_blocks == 1, st);
     }
     if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
       const float* all = nullptr;
-      const int rc = xchg_small(c, c->xch_src, 8, &all, st);
+      const int rc = xchg_small(c, c->xch_src, sizeof(TopSums) / sizeof(float), &all, st);
       if (rc != NPAIR_OK) return rc;
       launch_tops_world(all, NPAIR_XCH_FLOATS, c->world, N, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     }

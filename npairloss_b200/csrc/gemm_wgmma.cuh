@@ -85,7 +85,7 @@ struct GemmParams {
   uint32_t* st_maxb;
   uint32_t* st_maxall;
   int* cnt_same;           // per-row number of same-label non-self columns
-  // fused threshold pick (.cu:275-337): the last CTA to finish runs thresholds_one_block (thresholds.cuh); fuse_thr = 0: separate kernel
+  // fused threshold pick (.cu:275-337): the last CTA to finish runs thresholds_one_block (thresholds.cuh) with thr_out below
   int fuse_thr;
   RowArrays ra;
   MiningParams mp;
@@ -107,6 +107,8 @@ struct GemmParams {
   // ---- EPI_ARGMAX ----
   const float* col_bias;          // [Nn] subtracted from column c's similarities
   unsigned long long* best;       // [M] argmax keys, pre-zeroed
+  // ---- fuse_thr ----
+  BlockStats* thr_out;            // NULL: the thresholds are finished here; world scope: receives the rank's statistics for the exchange
 };
 
 // BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
@@ -676,7 +678,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     __syncthreads();
     if (s_last_cta) {
       __threadfence();
-      thresholds_one_block(p.ra, p.M, p.Nn, p.mp, p.bs, smem);     // the operand ring is idle: reuse its first bytes as scratch
+      thresholds_one_block(p.ra, p.M, p.Nn, p.mp, p.bs, smem, p.thr_out);   // the operand ring is idle: reuse its first bytes as scratch
       if (threadIdx.x == 0) p.bs->ticket2 = 0;
     }
   }

@@ -354,76 +354,26 @@ void launch_row_stats_ref(const float* S, long long ldS, int Q, int N, const flo
 }
 
 // --------------------------------------------------------------------------------------------
-// thresholds (.cu:275-337).  One block.  Non-relative modes and the pos==size-1 relative shortcut are
+// thresholds (.cu:275-337): thresholds_one_block (thresholds.cuh).  Non-relative modes and the pos==size-1 relative shortcut are
 // closed forms of the row statistics; general relative modes arm the radix selects below.
 // --------------------------------------------------------------------------------------------
-// Multi-block: every block reduces its slice of the row statistics and writes the LOCAL-region thresholds of its rows
-// (they need no global value); the last block to finish (ticket) combines the per-block partials into the block-wide
-// sizes / extrema, the GLOBAL-region thresholds (read directly by the row pass) and the radix-select arming.
-struct ThrPartial { unsigned long long ns; float mn, mxw, mxb; int err; };
-__global__ void __launch_bounds__(256) thresholds_kernel(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, ThrPartial* part,
-                                                         float* __restrict__ xout /*world scope: 6 floats of block statistics, else NULL*/) {
-  __shared__ unsigned long long s_ns[8];
-  __shared__ float s_mn[8], s_mxw[8], s_mxb[8];
-  __shared__ int s_err, s_last;
-  if (threadIdx.x == 0) s_err = 0;
-  __syncthreads();
-  unsigned long long ns = 0; float mn = FLT_MAX, mxw = -FLT_MAX, mxb = -FLT_MAX;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Q; i += gridDim.x * blockDim.x) {
-    const int cs = ra.cnt_same[i];
-    const float r_mn = ord2f(ra.st_minw[i]), r_mxw = ord2f(ra.st_maxw[i]), r_mxb = ord2f(ra.st_maxb[i]);
-    ns += static_cast<unsigned long long>(cs);
-    mn = fminf(mn, r_mn); mxw = fmaxf(mxw, r_mxw); mxb = fmaxf(mxb, r_mxb);
-    local_thresholds(ra, mp, i, N, cs, r_mn, r_mxw, r_mxb, &s_err);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) ns += __shfl_xor_sync(0xffffffffu, ns, o);
-  mn = warp_min(mn); mxw = warp_max(mxw); mxb = warp_max(mxb);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { s_ns[w] = ns; s_mn[w] = mn; s_mxw[w] = mxw; s_mxb[w] = mxb; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    ThrPartial t; t.ns = 0; t.mn = FLT_MAX; t.mxw = -FLT_MAX; t.mxb = -FLT_MAX; t.err = s_err;
-    for (int k = 0; k < (blockDim.x >> 5); ++k) { t.ns += s_ns[k]; t.mn = fminf(t.mn, s_mn[k]); t.mxw = fmaxf(t.mxw, s_mxw[k]); t.mxb = fmaxf(t.mxb, s_mxb[k]); }
-    part[blockIdx.x] = t;
-    __threadfence();
-    s_last = (atomicAdd(&bs->ticket2, 1u) == gridDim.x - 1) ? 1 : 0;
-  }
-  __syncthreads();
-  if (!s_last || threadIdx.x != 0) return;
-  __threadfence();
-  unsigned long long n_same = 0; float gmin_w = FLT_MAX, gmax_w = -FLT_MAX, gmax_b = -FLT_MAX; int err = 0;
-  for (int g = 0; g < static_cast<int>(gridDim.x); ++g) {
-    const ThrPartial t = part[g];
-    n_same += t.ns; gmin_w = fminf(gmin_w, t.mn); gmax_w = fmaxf(gmax_w, t.mxw); gmax_b = fmaxf(gmax_b, t.mxb); err |= t.err;
-  }
-  bs->ticket2 = 0;
-  if (xout) {          // world scope: this rank's block statistics go to the exchange; thresholds_world_kernel finishes
-    xout[0] = __uint_as_float(static_cast<uint32_t>(n_same)); xout[1] = __uint_as_float(static_cast<uint32_t>(n_same >> 32));
-    xout[2] = gmin_w; xout[3] = gmax_w; xout[4] = gmax_b; xout[5] = __int_as_float(err);
-    return;
-  }
-  finish_thresholds(n_same, static_cast<unsigned long long>(Q) * static_cast<unsigned long long>(N - 1) - n_same, gmin_w, gmax_w, gmax_b, err, mp, bs);
+// SIMT backend (the tensor-core similarity sweep runs the pick in its last CTA)
+__global__ void __launch_bounds__(1024) thresholds_kernel(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs) {
+  __shared__ __align__(8) unsigned char scratch[THRESHOLDS_SCRATCH_BYTES];
+  thresholds_one_block(ra, Q, N, mp, bs, scratch, nullptr);
 }
 // world scope (npair_config.global_scope): every rank reduces the world's block statistics in the same order -> identical thresholds
-__global__ void thresholds_world_kernel(const float* __restrict__ xall /*[world][xstride]*/, int xstride, int world, long long N, MiningParams mp,
+__global__ void thresholds_world_kernel(const BlockStats* __restrict__ xall, int xstride, int world, long long N, MiningParams mp,
                                         BlockScalars* bs) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  unsigned long long n_same = 0; float gmin_w = FLT_MAX, gmax_w = -FLT_MAX, gmax_b = -FLT_MAX; int err = 0;
-  for (int r = 0; r < world; ++r) {
-    const float* x = xall + static_cast<long long>(r) * xstride;
-    n_same += static_cast<unsigned long long>(__float_as_uint(x[0])) | (static_cast<unsigned long long>(__float_as_uint(x[1])) << 32);
-    gmin_w = fminf(gmin_w, x[2]); gmax_w = fmaxf(gmax_w, x[3]); gmax_b = fmaxf(gmax_b, x[4]); err |= __float_as_int(x[5]);
-  }
-  finish_thresholds(n_same, static_cast<unsigned long long>(N) * static_cast<unsigned long long>(N - 1) - n_same, gmin_w, gmax_w, gmax_b, err, mp, bs);
+  finish_thresholds(xall, world, xstride, static_cast<unsigned long long>(N), N, mp, bs);
 }
 void launch_thresholds_world(const float* xall, int xstride, int world, long long N, MiningParams mp, BlockScalars* bs, cudaStream_t st) {
-  thresholds_world_kernel<<<1, 32, 0, st>>>(xall, xstride, world, N, mp, bs);
+  thresholds_world_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const BlockStats*>(xall), xstride, world, N, mp, bs);
   count_launch();
 }
-void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, float* scratch, float* xout, cudaStream_t st) {
-  int grid = (Q + 255) / 256; if (grid > 64) grid = 64; if (grid < 1) grid = 1;
-  thresholds_kernel<<<grid, 256, 0, st>>>(ra, Q, N, mp, bs, reinterpret_cast<ThrPartial*>(scratch), xout);
+void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, cudaStream_t st) {
+  thresholds_kernel<<<1, 1024, 0, st>>>(ra, Q, N, mp, bs);
   count_launch();
 }
 
@@ -1189,10 +1139,7 @@ __global__ void __launch_bounds__(512) global_decide_kernel(const float* __restr
   if (!act0 && !act1) return;
   for (int b = threadIdx.x; b < 2 * NPAIR_SEL_BINS; b += blockDim.x) {
     unsigned long long sum = 0;
-    for (int r = 0; r < world; ++r) {
-      const float* x = xall + static_cast<long long>(r) * xstride + 2 * b;
-      sum += static_cast<unsigned long long>(__float_as_uint(x[0])) | (static_cast<unsigned long long>(__float_as_uint(x[1])) << 32);
-    }
+    for (int r = 0; r < world; ++r) sum += reinterpret_cast<const unsigned long long*>(xall + static_cast<long long>(r) * xstride)[b];
     gb.hist[b] = sum;
   }
   __syncthreads();
@@ -1266,10 +1213,32 @@ __device__ __forceinline__ void lse_elem(float sv, float lab, float li, float sc
   if (same) A += es;
 }
 
-// Loss, retrieval ratios, asum and error word from the Q rows' results, by one block.  The summation order depends on the block
-// size only (threads stride the rows, then warps in order), so a separate launch with the same size gives the same bits.
-__device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockScalars* bs, int num_tops, float* __restrict__ tops,
-                                                   float* __restrict__ xout, unsigned int seq) {
+// The tops of `rows` rows (loss, retrieval ratios, asum) and the error word from the reduction, in order from record 0, of n records
+// `stride` floats apart (world scope: one per rank, rows = N; per rank: n = 1, rows = Q), published to the host with the sequence number
+__device__ __forceinline__ void publish_tops(const TopSums* recs, int n, long long stride, long long rows, int num_tops, TopsBlock* out,
+                                             unsigned int seq) {
+  double ls = recs[0].loss_sum, asum = recs[0].asum;
+  long long h[3] = {recs[0].hits[0], recs[0].hits[1], recs[0].hits[2]};
+  int err = recs[0].err;
+  for (int r = 1; r < n; ++r) {
+    const TopSums& t = rank_record(recs, stride, r);
+    ls += t.loss_sum; h[0] += t.hits[0]; h[1] += t.hits[1]; h[2] += t.hits[2]; asum += t.asum; err |= t.err;
+  }
+  float tops[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+  tops[0] = static_cast<float>(ls) / static_cast<float>(-rows);                               // .cu:384-385
+  for (int t = 1; t <= num_tops - 2 && t <= 3; ++t) tops[t] = static_cast<float>(h[t - 1]) / static_cast<float>(rows);   // .cu:205
+  tops[num_tops - 1] = static_cast<float>(asum) / static_cast<float>(rows);                   // .cu:400-401 (always the LAST top)
+  for (int t = 0; t < 5; ++t) out->tops[t] = tops[t];
+  out->err = err;
+  __threadfence_system();
+  *reinterpret_cast<volatile unsigned int*>(&out->seq) = seq;     // the tops are visible on the host before the sequence number
+}
+
+// The Q rows' TopSums by one block, published (xout == NULL) or written to *xout (world scope: the rank's record for the exchange).
+// The summation order depends on the block size only (threads stride the rows, then warps in order), so a separate launch with the
+// same size gives the same bits.
+__device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* __restrict__ tops,
+                                                   TopSums* __restrict__ xout, unsigned int seq) {
   const int lane = threadIdx.x & 31;
   __shared__ double s_l[8];
   __shared__ int s_h[3][8];
@@ -1298,25 +1267,11 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
   if (lane == 0) { s_l[w] = ls; s_h[0][w] = h[0]; s_h[1][w] = h[1]; s_h[2][w] = h[2]; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    ls = 0.0; h[0] = h[1] = h[2] = 0;
-    for (int k = 0; k < (blockDim.x >> 5); ++k) { ls += s_l[k]; h[0] += s_h[0][k]; h[1] += s_h[1][k]; h[2] += s_h[2][k]; }
-    if (xout) {        // world scope: sums only; tops_world_kernel divides by the world's N after the exchange
-      const unsigned long long lb = static_cast<unsigned long long>(__double_as_longlong(ls));
-      xout[0] = __uint_as_float(static_cast<uint32_t>(lb)); xout[1] = __uint_as_float(static_cast<uint32_t>(lb >> 32));
-      xout[2] = __int_as_float(h[0]); xout[3] = __int_as_float(h[1]); xout[4] = __int_as_float(h[2]);
-      xout[5] = bs->asum; xout[6] = __int_as_float(bs->err);
-      bs->ticket = 0;
-      return;
-    }
-    float out[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    out[0] = static_cast<float>(ls) / static_cast<float>(-Q);                       // .cu:384-385
-    for (int t = 1; t <= num_tops - 2 && t <= 3; ++t) out[t] = static_cast<float>(h[t - 1]) / static_cast<float>(Q);   // .cu:205
-    out[num_tops - 1] = bs->asum / static_cast<float>(Q);                           // .cu:400-401 (always the LAST top)
-    for (int t = 0; t < 5; ++t) tops[t] = out[t];
-    reinterpret_cast<int*>(tops)[5] = bs->err;
+    TopSums s{0.0, {0, 0, 0}, bs->asum, bs->err};
+    for (int k = 0; k < (blockDim.x >> 5); ++k) { s.loss_sum += s_l[k]; s.hits[0] += s_h[0][k]; s.hits[1] += s_h[1][k]; s.hits[2] += s_h[2][k]; }
     bs->ticket = 0;
-    __threadfence_system();
-    reinterpret_cast<volatile unsigned int*>(tops)[6] = seq;     // tops are visible on the host before the sequence number
+    if (xout) *xout = s;
+    else publish_tops(&s, 1, 0, Q, num_tops, tops, seq);
   }
 }
 
@@ -1331,8 +1286,8 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
 __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
                                                        const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
                                                        int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs,
-                                                       int num_tops, float* __restrict__ tops, float log2_world,
-                                                       float* __restrict__ xout /*world scope: this rank's partial tops, else NULL*/,
+                                                       int num_tops, TopsBlock* __restrict__ tops, float log2_world,
+                                                       TopSums* __restrict__ xout /*world scope: this rank's tops sums, else NULL*/,
                                                        int wpr /*warps per row: 1, 2, 4 or 8 (few rows per rank: keep the SMs full)*/,
                                                        unsigned int seq /*written behind the tops: the host polls it*/,
                                                        int row0, int rows /*rows [row0, row0 + rows) of the rank; S holds them from row 0*/,
@@ -1374,7 +1329,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
     const int self_col = i + self_offset;
     const float max_all = ord2f(ra.st_maxall[i]);
     m2 = max_all * LOG2E;
-    // GLOBAL-region thresholds are block-wide scalars (thresholds_kernel / global_pick_kernel); LOCAL ones are per row
+    // GLOBAL-region thresholds are block-wide scalars (finish_thresholds / global_decide); LOCAL ones are per row
     const float posi = mp.ap_region == REGION_GLOBAL ? bs->posi_global : ra.posi_thr[i];
     const float nega = mp.an_region == REGION_GLOBAL ? bs->nega_global : ra.nega_thr[i];
     if (lane == 0 && part == 0) { ra.posi_thr[i] = posi; ra.nega_thr[i] = nega; }   // kept per row for inspection (npair_debug_read)
@@ -1475,7 +1430,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
   __threadfence();
   lse_finalize_block(Q, ra, bs, num_tops, tops, xout, seq);
 }
-__global__ void lse_finalize_kernel(int Q, RowArrays ra, BlockScalars* bs, int num_tops, float* __restrict__ tops, unsigned int seq) {
+__global__ void lse_finalize_kernel(int Q, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* __restrict__ tops, unsigned int seq) {
   lse_finalize_block(Q, ra, bs, num_tops, tops, nullptr, seq);
 }
 // Launch shape of the row pass, from the rank's row count Q (never from a row block's: the warps per row set the summation order
@@ -1500,7 +1455,7 @@ static void lse_shape(int Q, int N, int* wpr_out, int* threads_out) {
   *threads_out = wpb * 32;
 }
 void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, int world, float* xout,
+                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
                      unsigned int seq, int row0, int rows, bool finalize, cudaStream_t st) {
   int wpr = 1, threads = 256;
   lse_shape(Q, N, &wpr, &threads);
@@ -1510,7 +1465,7 @@ void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* l
                                             xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq, row0, rows, finalize ? 1 : 0);
   count_launch();
 }
-void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st) {
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st) {
   int wpr = 1, threads = 256;
   lse_shape(Q, N, &wpr, &threads);
   lse_finalize_kernel<<<1, threads, 0, st>>>(Q, ra, bs, num_tops, tops_dev, seq);
@@ -1703,29 +1658,14 @@ __global__ void __launch_bounds__(256) l2norm_bwd_kernel(const float* __restrict
     *reinterpret_cast<float4*>(dr + d) = make_float4((g.x - a.x * dot) * inv, (g.y - a.y * dot) * inv, (g.z - a.z * dot) * inv, (g.w - a.w * dot) * inv);
   } else for (int d = lane; d < dim; d += 32) dr[d] = (gr[d] - yr[d] * dot) * inv;
 }
-// world scope: tops from the ranks' partial sums, normalised by the world's N (identical on every rank)
-__global__ void tops_world_kernel(const float* __restrict__ xall, int xstride, int world, long long N, int num_tops, float* __restrict__ tops,
+// world scope: tops from the ranks' sums, normalised by the world's N (identical on every rank)
+__global__ void tops_world_kernel(const TopSums* __restrict__ xall, int xstride, int world, long long N, int num_tops, TopsBlock* __restrict__ tops,
                                   unsigned int seq) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  double ls = 0.0; long long h[3] = {0, 0, 0}; double asum = 0.0; int err = 0;
-  for (int r = 0; r < world; ++r) {
-    const float* x = xall + static_cast<long long>(r) * xstride;
-    const unsigned long long lb = static_cast<unsigned long long>(__float_as_uint(x[0])) | (static_cast<unsigned long long>(__float_as_uint(x[1])) << 32);
-    ls += __longlong_as_double(static_cast<long long>(lb));
-    h[0] += __float_as_int(x[2]); h[1] += __float_as_int(x[3]); h[2] += __float_as_int(x[4]);
-    asum += x[5]; err |= __float_as_int(x[6]);
-  }
-  float out[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-  out[0] = static_cast<float>(ls) / static_cast<float>(-N);
-  for (int t = 1; t <= num_tops - 2 && t <= 3; ++t) out[t] = static_cast<float>(h[t - 1]) / static_cast<float>(N);
-  out[num_tops - 1] = static_cast<float>(asum) / static_cast<float>(N);
-  for (int t = 0; t < 5; ++t) tops[t] = out[t];
-  reinterpret_cast<int*>(tops)[5] = err;
-  __threadfence_system();
-  reinterpret_cast<volatile unsigned int*>(tops)[6] = seq;
+  publish_tops(xall, world, xstride, N, num_tops, tops, seq);
 }
-void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st) {
-  tops_world_kernel<<<1, 32, 0, st>>>(xall, xstride, world, N, num_tops, tops_dev, seq);
+void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st) {
+  tops_world_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const TopSums*>(xall), xstride, world, N, num_tops, tops_dev, seq);
   count_launch();
 }
 

@@ -93,6 +93,38 @@ struct RowRecord {
 static_assert(sizeof(RowRecord) == 32, "row records are exchanged as 32 raw bytes");
 constexpr long long ROW_RECORD_FLOATS = sizeof(RowRecord) / sizeof(float);   // exchanges count floats
 
+// One rank's contribution to a world-scope reduction (global_scope), exchanged as raw bytes in its slot of the small exchange; the
+// per-rank finish is the same reduction over the one record of its own rank.
+// The statistics the threshold pick reduces over a block of rows (finish_thresholds, thresholds.cuh): the number of same-label pairs,
+// min / max same-label and max diff-label similarity, DERR_* bits
+struct BlockStats {
+  unsigned long long n_same;
+  float gmin_w, gmax_w, gmax_b;
+  int err;
+};
+static_assert(sizeof(BlockStats) == 24, "block statistics are exchanged as 24 raw bytes");
+// The sums the tops are made of (publish_tops, kernels.cu): sum of the rows' log(A/T), retrieval hits at k = 1, 5, 10, sum |x|, DERR_* bits
+struct TopSums {
+  double loss_sum;
+  int hits[3];
+  float asum;
+  int err;
+};
+static_assert(sizeof(TopSums) == 32, "tops sums are exchanged as 32 raw bytes");
+// Record r of an exchange that holds one record per rank, `stride` floats apart
+template <class T>
+__host__ __device__ __forceinline__ const T& rank_record(const T* recs, long long stride, int r) {
+  return *reinterpret_cast<const T*>(reinterpret_cast<const float*>(recs) + r * stride);
+}
+
+// What a forward publishes to the host, in mapped pinned memory: the tops, the DERR_* bits, then the forward's sequence number, which
+// is stored last (the host polls it)
+struct TopsBlock {
+  float tops[5];
+  int err;
+  unsigned int seq;
+};
+
 // Global (per-rank-block) scalars living in device memory.
 struct BlockScalars {
   unsigned long long n_same, n_diff;       // sizes of ident_global / diff_global (.cu:225-265)
@@ -101,7 +133,7 @@ struct BlockScalars {
   float posi_global, nega_global;          // GLOBAL-region thresholds (valid when the region is GLOBAL)
   int err;                                 // DERR_* bits
   unsigned int ticket;                     // block-completion counter of the row pass (last block finalises)
-  unsigned int ticket2;                    // block-completion counter of the thresholds kernel
+  unsigned int ticket2;                    // block-completion counter of the similarity sweep (its last CTA picks the thresholds)
   unsigned int ticket0;                    // block-completion counter of the prep kernel
   // radix-select state, one per side (0 = AP over same pairs, 1 = AN over diff pairs)
   unsigned long long sel_rank[2];          // remaining 0-based rank inside the current prefix bucket
@@ -179,10 +211,12 @@ void launch_split(const float* x_total, int N, int D, int prec, const BlockScala
                   uint16_t* XcatA /*or NULL*/, uint16_t* XcatB, long long Dp, cudaStream_t st);
 void launch_row_stats_ref(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                           int self_offset, RowArrays ra, cudaStream_t st);
-// xout: NULL, or (world scope) 6 floats receiving this rank's block statistics instead of the final thresholds
-void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, float* scratch /*>= 2 KB*/, float* xout, cudaStream_t st);
+// The threshold pick of the rank's Q rows by one block (SIMT backend; the tensor-core similarity sweep runs it in its last CTA)
+void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, cudaStream_t st);
+// World scope: the thresholds of the world's N rows from the ranks' BlockStats, which lie xstride floats apart in xall
 void launch_thresholds_world(const float* xall, int xstride, int world, long long N, MiningParams mp, BlockScalars* bs, cudaStream_t st);
-void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st);
+// World scope: the tops of the world's N rows from the ranks' TopSums, which lie xstride floats apart in xall
+void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // side_mask: bit 0 = AP threshold over the same-label list, bit 1 = AN threshold over the diff-label list
 void launch_local_select(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                          int self_offset, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
@@ -191,16 +225,16 @@ cudaError_t allow_local_select_smem();
 void launch_global_select_pass(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
                                int self_offset, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
                                uint32_t* cand /*[2][cand_cap]*/, unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st);
-// world scope: xall = the ranks' exchanged [2][2048] 64-bit digit counts
+// world scope: the ranks' [2][2048] 64-bit digit counts lie xstride floats apart in xall
 void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
                           uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
 // Row pass over rows [row0, row0 + rows) of the rank (S points at row row0's similarities; lab_rows, self_offset and ra are the
 // rank's).  finalize: the last block also reduces the Q rows' results into the tops; otherwise launch_lse_finalize does, once.
+// xout: NULL, or (world scope) receives the rank's TopSums instead of the tops
 void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev /*[5]+err*/,
-                     int world, float* xout /*world scope: 7 floats of partial tops, else NULL*/, unsigned int seq, int row0, int rows,
-                     bool finalize, cudaStream_t st);
-void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, float* tops_dev, unsigned int seq, cudaStream_t st);
+                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev,
+                     int world, TopSums* xout, unsigned int seq, int row0, int rows, bool finalize, cudaStream_t st);
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-record
 // exchange: rs_total = the world's N records, all-gathered)
 enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
