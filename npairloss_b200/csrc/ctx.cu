@@ -602,20 +602,6 @@ struct StreamOrder {
   bool recorded = false;
   bool open = false;                  // a call has entered and not yet marked
 };
-// One call's work on `st`: enter() waits for the previous call when that ran on another stream; `done` is recorded at the latest when
-// the call returns, also after an error (what it enqueued before failing is still running)
-struct OrderedCall {
-  OrderedCall(StreamOrder& o_, cudaStream_t st_) : o(o_), st(st_) {}
-  OrderedCall(const OrderedCall&) = delete;
-  cudaError_t enter() {
-    const cudaError_t e = o.recorded && o.stream != st ? cudaStreamWaitEvent(st, o.done, 0) : cudaSuccess;
-    o.open = e == cudaSuccess;
-    return e;
-  }
-  ~OrderedCall() { o.mark(st); }
-  StreamOrder& o;
-  cudaStream_t st;
-};
 
 // The statistics of RowArrays, which the evaluator's queries have too: four ordered-uint statistics and the same-label count per row
 static void carve_stats(Carve& cv, long long rows, RowArrays* ra) {
@@ -646,9 +632,6 @@ struct npair_ctx : Plan {
   RowRecord* rs_total = nullptr;   // row-scalar mode: the world's N row records, all-gathered
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
-  bool rs_gathered = false;
-  bool ext_gathered = false;      // the current forward came through npair_forward_gathered (external collectives)
-  bool defer_sync = false;        // npair_forward_backward: the forward returns after enqueueing, the caller synchronises later
   // peer-memory exchange (world > 1 with a communicator; NPAIR_FLAG_NCCL_FEATURES / _RECORDS fall back to NCCL)
   bool p2p_feat = false, p2p_rec = false;
   float* p2p_region = nullptr;         // laid out by xl (XchgLayout)
@@ -673,11 +656,14 @@ struct npair_ctx : Plan {
   CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_kcat)
   // nccl
   void* comm = nullptr; bool own_comm = false;
-  // per-step state
-  const float* cur_feat = nullptr; const float* cur_label = nullptr;
-  const float* y_local = nullptr;   // normalize_input: this rank's normalised rows
-  const float *x_total = nullptr, *lab_total = nullptr;
-  bool fwd_done = false;
+  // What a forward leaves for the calls after it.  Each forward that enters resets the whole record; a refused one leaves it alone.
+  struct Step {
+    const float* label = nullptr;                            // this rank's labels
+    const float *x_total = nullptr, *lab_total = nullptr;    // the world's rows (normalised under normalize_input) and labels
+    bool ext_gathered = false;     // through npair_forward_gathered: the caller did the collectives
+    bool rec_gathered = false;     // the NCCL all-gather of the row records has been enqueued (at the first backward)
+    bool fwd_done = false;         // the forward succeeded: a backward may follow
+  } step;
   StreamOrder order;              // the calls' order across streams; debug_read and profile_read wait for its event
   std::string err;
   // optional per-phase CUDA-event timing (npair_profile_enable)
@@ -747,6 +733,26 @@ struct PhaseTimer {
       return NPAIR_E_CUDA;                                                                               \
     }                                                                                                    \
   } while (0)
+
+// The frame of every C ABI call that enqueues work for a context or an evaluator (`Obj`), on the caller's stream: enter() makes the
+// object's device current and waits for the previous call when that ran on another stream (StreamOrder), failures going to the object's
+// `err`.  `done` is recorded at the latest when the call returns, also after an error (what it enqueued before failing is still
+// running).  A call refused before enter() enqueues nothing and records nothing.
+template <class Obj>
+struct OrderedCall {
+  OrderedCall(Obj* obj_, void* stream) : obj(obj_), st(static_cast<cudaStream_t>(stream)) {}
+  OrderedCall(const OrderedCall&) = delete;
+  int enter() {
+    StreamOrder& o = obj->order;
+    CUDA_TRY(obj, cudaSetDevice(obj->device));
+    if (o.recorded && o.stream != st) CUDA_TRY(obj, cudaStreamWaitEvent(st, o.done, 0));
+    o.open = true;
+    return NPAIR_OK;
+  }
+  ~OrderedCall() { obj->order.mark(st); }
+  Obj* const obj;
+  const cudaStream_t st;
+};
 
 // Makes `device` (< 0: the current one) current for a new context or evaluator, which needs an sm_90 device; its id and SM count
 static int open_device(int device, int* dev, int* sms) {
@@ -1056,7 +1062,7 @@ static MiningParams mining_of(const npair_config& c) {
 // this forward's sequence number: polling that word returns a few microseconds earlier than a stream synchronisation and does not
 // wait for anything enqueued behind the row pass (the row-record push, a backward).  A fault in a kernel never writes the number:
 // after ~2 s fall back to the synchronisation, which reports the error.  Then the device error bits become the return code, and the
-// tops are copied out.
+// tops are copied out.  Only this return of NPAIR_OK makes the step's forward a successful one.
 static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
   c->order.mark(st);                               // everything of the call is enqueued: the event goes in before the host waits
   volatile unsigned int* seqp = &c->tops_pinned->seq;
@@ -1071,30 +1077,33 @@ static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
   if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
   if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
   for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned->tops[t] : 0.f;
+  c->step.fwd_done = true;
   return NPAIR_OK;
 }
 
-static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st);
-static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st);
-
-int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
-  if (!c) return NPAIR_E_ARG;
-  if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  return forward_rank(c, d_feat, d_label, tops_host, st);
+// The preconditions of the calls after a forward; a call they refuse enqueues nothing
+static int need_forward(npair_ctx* c, const char* call) {
+  if (c->step.fwd_done) return NPAIR_OK;
+  c->err = fmt("%s called without a successful forward", call);
+  return NPAIR_E_STATE;
+}
+// world > 1: the library's own collectives need a communicator; `instead` names the external-collectives calls
+static int need_comm(npair_ctx* c, const char* instead) {
+  if (c->world == 1 || c->comm) return NPAIR_OK;
+  c->err = fmt("context was created without a communicator: use %s", instead);
+  return NPAIR_E_STATE;
 }
 
-// npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward
-static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st) {
-  c->fwd_done = false; c->ext_gathered = false;
+static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st);
+
+// Enqueues npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward
+static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, cudaStream_t st) {
+  c->step = npair_ctx::Step{d_label};
   const int Q = c->Q, D = c->D;
   if (c->cfg.normalize_input) {               // fused L2Normalize producer (usage/def.prototxt:115-120): the layer works on x / ||x||
     PhaseTimer pt(c, 1, st);
     launch_l2norm_fwd(d_feat, Q, D, c->Ynorm, c->inv_norm, st);
-    d_feat = c->Ynorm; c->y_local = c->Ynorm;
+    d_feat = c->Ynorm;
   }
   // ---- GatherFeatureAndLabel (.cu:17-43): one NCCL group, device to device over NVLink ----
   if (c->world > 1 && c->p2p_feat) {
@@ -1102,10 +1111,9 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     const uint32_t ep = ++c->p2p_fwd_epoch;
     const long long QD = static_cast<long long>(Q) * D;
     p2p_push(c, XCHG_FEATURES, ep, grid_for(QD / 4, 2 * c->sms), d_feat, QD, XP_X, d_label, Q, XP_LAB, st);
-    c->x_total = p2p_wait(c, XCHG_FEATURES, ep, XP_X, st);
-    c->lab_total = c->p2p_region + c->xl.off(XP_LAB, ep & 1u, 0);
+    c->step.x_total = p2p_wait(c, XCHG_FEATURES, ep, XP_X, st);
+    c->step.lab_total = c->p2p_region + c->xl.off(XP_LAB, ep & 1u, 0);
   } else if (c->world > 1) {
-    if (!c->comm) { c->err = "context was created without a communicator: use npair_forward_gathered"; return NPAIR_E_STATE; }
     PhaseTimer pt(c, 0, st);
     NcclApi* api = nccl_api();
     int r = api->GroupStart();
@@ -1114,9 +1122,20 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     int r2 = api->GroupEnd();
     if (r == 0) r = r2;
     if (r != 0) { c->err = fmt("ncclAllGather: %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
-    c->x_total = c->Xtot_buf; c->lab_total = c->labtot_buf;
-  } else { c->x_total = d_feat; c->lab_total = d_label; }
-  return forward_impl(c, d_feat, d_label, tops_host, st);
+    c->step.x_total = c->Xtot_buf; c->step.lab_total = c->labtot_buf;
+  } else { c->step.x_total = d_feat; c->step.lab_total = d_label; }
+  return forward_impl(c, d_feat, st);
+}
+
+int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = forward_rank(c, d_feat, d_label, call.st)) != NPAIR_OK) return rc;
+  return finish_forward(c, tops_host, call.st);
 }
 
 /* External-collectives variant: the caller already holds the all-gathered N x D features and N labels (rank r's rows are
@@ -1124,21 +1143,19 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
 int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float* d_label_total, float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat_total || !d_label_total || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  c->fwd_done = false; c->ext_gathered = true;
+  OrderedCall call(c, stream);
+  int rc;
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const long long r0 = static_cast<long long>(c->rank) * c->Q;
+  float* const normed = c->world > 1 ? c->Xtot_buf : c->Ynorm;     // normalize_input: the N normalised rows
+  c->step = npair_ctx::Step{d_label_total + r0, c->cfg.normalize_input ? normed : d_feat_total, d_label_total, true};
   if (c->cfg.normalize_input) {               // the gathered bottoms are raw embeddings: normalise all N rows (1 / ||x|| kept for the local ones)
-    PhaseTimer pt(c, 1, st);
-    float* dst = c->world > 1 ? c->Xtot_buf : c->Ynorm;
-    launch_l2norm_fwd(d_feat_total, c->N, c->D, dst, nullptr, st);
-    launch_l2norm_fwd(d_feat_total + static_cast<long long>(c->rank) * c->Q * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, st);
-    c->y_local = c->Ynorm;
-    d_feat_total = dst;
+    PhaseTimer pt(c, 1, call.st);
+    launch_l2norm_fwd(d_feat_total, c->N, c->D, normed, nullptr, call.st);
+    launch_l2norm_fwd(d_feat_total + r0 * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
   }
-  c->x_total = d_feat_total; c->lab_total = d_label_total;
-  return forward_impl(c, d_feat_total + static_cast<long long>(c->rank) * c->Q * c->D, d_label_total + static_cast<long long>(c->rank) * c->Q, tops_host, st);
+  if ((rc = forward_impl(c, c->step.x_total + r0 * c->D, call.st)) != NPAIR_OK) return rc;
+  return finish_forward(c, tops_host, call.st);
 }
 
 // The per-row arrays from row r0 on, for kernels that see rows [r0, ..) as their rows [0, ..).  `hits` ([3][Q]) cannot be offset this
@@ -1157,7 +1174,7 @@ static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_
   GemmParams gp = sim_sweep(epi, rows, c->N, c->kcat, &c->bs->x_inv_scale, c->sym_tiles, c->n_sym_tiles, c->ra);
   gp.a_row0 = r0; gp.S = c->S; gp.ldS = c->ldS;
   if (epi & EPI_STATS) {
-    gp.lab_rows = c->cur_label; gp.lab_cols = c->lab_total; gp.self_offset = c->rank * c->Q;
+    gp.lab_rows = c->step.label; gp.lab_cols = c->step.lab_total; gp.self_offset = c->rank * c->Q;
     gp.fuse_thr = 1; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
     gp.thr_out = c->wscope ? reinterpret_cast<BlockStats*>(c->xch_src) : nullptr;   // world scope: the rank's record for the exchange
   }
@@ -1175,21 +1192,21 @@ static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
 
 // LOCAL relative selects of rows [r0, r0 + rows), which the S buffer holds
 static void local_select(npair_ctx* c, int r0, int rows, cudaStream_t st) {
-  launch_local_select(c->S, c->ldS, rows, c->N, c->cur_label + r0, c->lab_total, c->rank * c->Q + r0, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn,
+  launch_local_select(c->S, c->ldS, rows, c->N, c->step.label + r0, c->step.lab_total, c->rank * c->Q + r0, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn,
                       rows_from(c->ra, r0), c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
 }
 
-static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], cudaStream_t st) {
+static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
-  c->cur_feat = d_feat; c->cur_label = d_label;
+  const float* d_label = c->step.label;
   const int self_off = c->rank * Q;
   // ---- operand preparation: |x| sum (top asum, .cu:400), power-of-two pre-scale, split to tensor-core pieces ----
   {
     PhaseTimer pt(c, 1, st);
-    launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->x_total, static_cast<long long>(N) * D, c->partial,
+    launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->step.x_total, static_cast<long long>(N) * D, c->partial,
                        c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-    launch_split(c->x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    launch_split(c->step.x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
   }
   // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) over all Q rows; S is stored
   //      only when it is materialised, and is then block 0 of the row pass ----
@@ -1202,7 +1219,7 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
     gp.M = Q; gp.Nn = N; gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
     CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_STORE_S, c->Xs + static_cast<long long>(self_off) * c->Dp, c->Dp, static_cast<long long>(N) * c->Dp,
                                  c->Xs, c->Dp, static_cast<long long>(N) * c->Dp, D, gp, st));
-    launch_row_stats_ref(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, c->ra, st);
+    launch_row_stats_ref(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, c->ra, st);
   }
   // ---- thresholds (.cu:275-337) ----
   {
@@ -1219,7 +1236,7 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
     // validate()); LOCAL selects of row blocks run in the row pass, block by block
     if (c->gsel_mask) {
       for (int pass = 0; pass < 3; ++pass) {
-        launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, c->gsel_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
+        launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, c->gsel_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
                                   c->wscope ? 1 : 0, c->bs, c->sms, st);
         if (c->wscope) {
           const float* all = nullptr;
@@ -1240,7 +1257,7 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
       if (c->lsel_mask && c->n_blocks > 1) local_select(c, r0, rows, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
-      launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
+      launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
                       c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr, c->tops_seq, r0, rows, c->n_blocks == 1, st);
     }
     if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
@@ -1251,19 +1268,16 @@ static int forward_impl(npair_ctx* c, const float* d_feat, const float* d_label,
       launch_tops_world(all, NPAIR_XCH_FLOATS, c->world, N, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     }
   }
-  c->rs_gathered = false;          // the NCCL row-record gather is enqueued at the start of the backward
-  if (c->p2p_rec && c->comm && c->x_total != nullptr && !c->ext_gathered) {
-    // peer-memory exchange: push this rank's 32-byte row records to every rank now; the backward only waits for the flags
+  if (c->p2p_rec && !c->step.ext_gathered) {
+    // peer-memory exchange: push this rank's 32-byte row records to every rank now; the backward only waits for the flags.  (The NCCL
+    // row-record gather is enqueued at the start of the backward.)
     PhaseTimer pt(c, 8, st);
     const uint32_t ep = ++c->p2p_rec_epoch;
     p2p_push(c, XCHG_RECORDS, ep, grid_for(2ll * Q, 64), reinterpret_cast<const float*>(c->ra.rowrec), ROW_RECORD_FLOATS * Q, XP_REC,
              nullptr, 0, XP_REC, st);
   }
   CUDA_TRY(c, cudaGetLastError());
-  if (c->defer_sync) return NPAIR_OK;              // npair_forward_backward enqueues the backward first, then waits once
-  const int rc = finish_forward(c, tops_host, st);
-  c->fwd_done = rc == NPAIR_OK;
-  return rc;
+  return NPAIR_OK;
 }
 
 static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
@@ -1274,7 +1288,7 @@ static int backward_impl(npair_ctx* c, float loss_weight, float* d_diff, float* 
   const int rc = backward_core(c, loss_weight, c->dY, nullptr, d_rs_ext, st);
   if (rc != NPAIR_OK) return rc;
   PhaseTimer pt(c, 5, st);
-  launch_l2norm_bwd(c->y_local, c->inv_norm, c->dY, c->Q, c->D, d_diff, st);
+  launch_l2norm_bwd(c->Ynorm, c->inv_norm, c->dY, c->Q, c->D, d_diff, st);
   return NPAIR_OK;
 }
 
@@ -1291,14 +1305,13 @@ static int check_out_aligned(npair_ctx* c, const float* p, const char* name) {
 int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_diff) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
-  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
-  if (!c->fwd_done) { c->err = "npair_backward called without a successful npair_forward"; return NPAIR_E_STATE; }
-  if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator: use npair_backward_partial / npair_backward_gathered"; return NPAIR_E_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  return backward_impl(c, loss_weight, d_diff, nullptr, nullptr, st);
+  int rc;
+  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
+  if ((rc = need_forward(c, "npair_backward")) != NPAIR_OK) return rc;
+  if ((rc = need_comm(c, "npair_backward_partial / npair_backward_gathered")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  return backward_impl(c, loss_weight, d_diff, nullptr, nullptr, call.st);
 }
 
 /* Forward + backward with ONE host synchronisation: the backward (whose loss weight is a constant of the net, top[0]'s diff)
@@ -1309,24 +1322,16 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
                            void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !d_diff || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
-  if (c->world > 1 && !c->comm) { c->err = "context was created without a communicator"; return NPAIR_E_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  c->defer_sync = true;
-  int rc = forward_rank(c, d_feat, d_label, tops_host, st);
-  c->defer_sync = false;
-  if (rc != NPAIR_OK) return rc;
-  c->fwd_done = true;                                  // enqueued; confirmed (or revoked) after the synchronisation below
-  rc = backward_impl(c, loss_weight, d_diff, nullptr, nullptr, st);
-  if (rc != NPAIR_OK) { c->fwd_done = false; return rc; }
+  int rc;
+  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
+  if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = forward_rank(c, d_feat, d_label, call.st)) != NPAIR_OK) return rc;
+  if ((rc = backward_impl(c, loss_weight, d_diff, nullptr, nullptr, call.st)) != NPAIR_OK) return rc;
   // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step.
   // finish_forward records `done` behind the backward
-  rc = finish_forward(c, tops_host, st);
-  if (rc != NPAIR_OK) c->fwd_done = false;
-  return rc;
+  return finish_forward(c, tops_host, call.st);
 }
 
 /* External-collectives variant of Backward_gpu up to the all-reduce (.cu:420-460):
@@ -1337,39 +1342,36 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
 int npair_backward_partial(npair_ctx* c, float loss_weight, float* d_local_half, float* d_total_half, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_local_half || (c->world > 1 && !d_total_half)) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
-  if (check_out_aligned(c, d_local_half, "d_local_half") != NPAIR_OK) return NPAIR_E_ARG;
-  if (c->world > 1 && check_out_aligned(c, d_total_half, "d_total_half") != NPAIR_OK) return NPAIR_E_ARG;
-  if (!c->fwd_done) { c->err = "npair_backward_partial called without a successful forward"; return NPAIR_E_STATE; }
+  int rc;
+  if ((rc = check_out_aligned(c, d_local_half, "d_local_half")) != NPAIR_OK) return rc;
+  if (c->world > 1 && (rc = check_out_aligned(c, d_total_half, "d_total_half")) != NPAIR_OK) return rc;
+  if ((rc = need_forward(c, "npair_backward_partial")) != NPAIR_OK) return rc;
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  return backward_impl(c, loss_weight, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, st);
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  return backward_impl(c, loss_weight, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, call.st);
 }
 
 int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
   if (!c || !d_out) return NPAIR_E_ARG;
-  if (!c->fwd_done) { c->err = "npair_row_scalars called without a successful forward"; return NPAIR_E_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowrec, sizeof(RowRecord) * c->Q, cudaMemcpyDeviceToDevice, st));
+  int rc;
+  if ((rc = need_forward(c, "npair_row_scalars")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  CUDA_TRY(c, cudaMemcpyAsync(d_out, c->ra.rowrec, sizeof(RowRecord) * c->Q, cudaMemcpyDeviceToDevice, call.st));
   return NPAIR_OK;
 }
 
 int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_total, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_rs_total || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  if (check_out_aligned(c, d_diff, "the gradient pointer") != NPAIR_OK) return NPAIR_E_ARG;
-  if (!c->fwd_done) { c->err = "npair_backward_gathered called without a successful forward"; return NPAIR_E_STATE; }
+  int rc;
+  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
+  if ((rc = need_forward(c, "npair_backward_gathered")) != NPAIR_OK) return rc;
   if (c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  OrderedCall oc(c->order, st);
-  CUDA_TRY(c, oc.enter());
-  return backward_impl(c, loss_weight, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), st);
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  return backward_impl(c, loss_weight, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), call.st);
 }
 
 // d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
@@ -1393,17 +1395,17 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     bw_mode = BW_ROWSCAL;
     if (d_rs_ext) rs_total = d_rs_ext;
     else {
-      if (c->p2p_rec && !c->ext_gathered) {
+      if (c->p2p_rec && !c->step.ext_gathered) {
         PhaseTimer pt(c, 8, st);
         rs_total = reinterpret_cast<const RowRecord*>(p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st));
-      } else if (!c->rs_gathered) {
-        // the only backward exchange: Q row records per rank (replaces the N x D MPI_Allreduce of .cu:462-489)
-        if (!c->comm) { c->err = "no communicator: use npair_backward_gathered with externally gathered row records"; return NPAIR_E_STATE; }
+      } else if (!c->step.rec_gathered) {
+        // the only backward exchange: Q row records per rank (replaces the N x D MPI_Allreduce of .cu:462-489); the callers without
+        // d_rs_ext checked for the communicator (need_comm)
         PhaseTimer pt(c, 8, st);
         NcclApi* api = nccl_api();
         int r = api->AllGather(c->ra.rowrec, c->rs_total, ROW_RECORD_FLOATS * Q, NCCL_FLOAT32, c->comm, st);
         if (r != 0) { c->err = fmt("ncclAllGather(row records): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
-        c->rs_gathered = true;
+        c->step.rec_gathered = true;
         rs_total = c->rs_total;
       } else rs_total = c->rs_total;
     }
@@ -1437,7 +1439,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   }
   {
     PhaseTimer pt(c, 5, st);
-    launch_build_weights(c->S, c->ldS, Q, N, c->cur_label, c->lab_total, self_off, c->world, bw_mode, rs_total, mp, c->ra, c->prec, c->H, c->Np, c->HT, c->Qp, st);
+    launch_build_weights(c->S, c->ldS, Q, N, c->step.label, c->step.lab_total, self_off, c->world, bw_mode, rs_total, mp, c->ra, c->prec, c->H, c->Np, c->HT, c->Qp, st);
   }
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.dev_scale = &c->bs->x_inv_scale;
@@ -1490,10 +1492,17 @@ int npair_profile_enable(npair_ctx* c, int on) {
 /* milliseconds of each phase of the most recent forward+backward; synchronises the stream.  ms_out[9]. */
 unsigned long long npair_kernel_launches(void) { return npair::g_kernel_launches; }
 
-int npair_profile_read(npair_ctx* c, float* ms_out) {
-  if (!c || !ms_out) return NPAIR_E_ARG;
+// The host reads a context's buffers once the work of its last call has finished
+static int await_calls(npair_ctx* c) {
   CUDA_TRY(c, cudaSetDevice(c->device));
   CUDA_TRY(c, cudaEventSynchronize(c->order.done));
+  return NPAIR_OK;
+}
+
+int npair_profile_read(npair_ctx* c, float* ms_out) {
+  if (!c || !ms_out) return NPAIR_E_ARG;
+  const int rc = await_calls(c);
+  if (rc != NPAIR_OK) return rc;
   for (int i = 0; i < NPAIR_PROF_PHASES; ++i) {
     ms_out[i] = 0.f;
     if (c->ev_made && c->ev_used[i]) { float ms = 0.f; CUDA_TRY(c, cudaEventElapsedTime(&ms, c->ev[i][0], c->ev[i][1])); ms_out[i] = ms; }
@@ -1513,8 +1522,8 @@ __global__ void int_to_float_kernel(const int* __restrict__ in, float* __restric
 
 int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
   if (!c || !dst) return NPAIR_E_ARG;
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  CUDA_TRY(c, cudaEventSynchronize(c->order.done));
+  const int rc = await_calls(c);
+  if (rc != NPAIR_OK) return rc;
   const int Q = c->Q, N = c->N;
   if (which == 0) {
     if (c->n_blocks > 1) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
@@ -1859,10 +1868,9 @@ int npair_eval_rank(npair_eval* ev, const float* q, const float* ql, int32_t nq,
   int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
   if (rc != NPAIR_OK) return rc;
   if (!ql || !gl || !d_rank) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(ev, cudaSetDevice(ev->device));
-  OrderedCall oc(ev->order, st);
-  CUDA_TRY(ev, oc.enter());
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   float* cut = reinterpret_cast<float*>(ev->ra.st_minw);   // p* overwrites a statistic sweep 2 does not read
@@ -1881,10 +1889,9 @@ int npair_eval_best_positive(npair_eval* ev, const float* q, const float* ql, in
   int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
   if (rc != NPAIR_OK) return rc;
   if (!ql || !gl || !d_best) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(ev, cudaSetDevice(ev->device));
-  OrderedCall oc(ev->order, st);
-  CUDA_TRY(ev, oc.enter());
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
   const int self_col = eval_self_col(self_offset, gallery_row0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
@@ -1900,10 +1907,9 @@ int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g,
   int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
   if (rc != NPAIR_OK) return rc;
   if (!d_cut || !d_count) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(ev, cudaSetDevice(ev->device));
-  OrderedCall oc(ev->order, st);
-  CUDA_TRY(ev, oc.enter());
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
   const int self_col = eval_self_col(self_offset, gallery_row0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
@@ -1923,10 +1929,9 @@ int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t
   int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
   if (rc != NPAIR_OK) return rc;
   if (!ql || !gl || !d_map_r || !d_r_precision) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(ev, cudaSetDevice(ev->device));
-  OrderedCall oc(ev->order, st);
-  CUDA_TRY(ev, oc.enter());
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
   const int self_col = eval_self_col(self_offset, 0);
   const bool sym = eval_sym(q, nq, g, ng, self_col);
   if ((rc = eval_grow(ev, ev->map_rows_mem, &ev->map_rows, MapRows(nullptr, nq).bytes, "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
@@ -1980,11 +1985,10 @@ int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, cons
   if (max_iter < 1) { ev->err = "max_iter must be >= 1"; return NPAIR_E_ARG; }
   for (int c = 0; c < k; ++c)
     if (init_rows[c] < 0 || init_rows[c] >= n) { ev->err = fmt("init_rows[%d] = %d is not a row of x", c, init_rows[c]); return NPAIR_E_ARG; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(ev, cudaSetDevice(ev->device));
-  OrderedCall oc(ev->order, st);
-  CUDA_TRY(ev, oc.enter());
   int rc;
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
   if ((rc = eval_grow(ev, ev->km_mem, &ev->km, KmeansBufs(nullptr, n, k, ev->D).bytes, "the k-means buffers")) != NPAIR_OK) return rc;
   const long long D = ev->D;
   const KmeansBufs km(ev->km, n, k, D);
