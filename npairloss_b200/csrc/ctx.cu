@@ -1158,23 +1158,18 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
   return finish_forward(c, tops_host, call.st);
 }
 
-// The per-row arrays from row r0 on, for kernels that see rows [r0, ..) as their rows [0, ..).  `hits` ([3][Q]) cannot be offset this
-// way: such kernels must not use it.
-static RowArrays rows_from(const RowArrays& ra, int r0) {
-  RowArrays v = ra;
-  v.st_minw += r0; v.st_maxw += r0; v.st_maxb += r0; v.st_maxall += r0; v.cnt_same += r0;
-  v.posi_thr += r0; v.nega_thr += r0; v.A += r0; v.T += r0; v.logv += r0;
-  v.hits = nullptr;
-  v.rowrec += r0;
-  return v;
+// What a kernel reads of rows [r0, r0 + rows) of the current step's S, which the S buffer holds from its row 0
+static SimRows sim_rows(const npair_ctx* c, int r0, int rows) {
+  return SimRows{c->S, c->ldS, c->Q, c->N, r0, rows, c->step.label, c->step.lab_total, c->rank * c->Q};
 }
 
 // The similarity GEMM over rows [r0, r0 + rows) of the rank's S through the epilogue `epi` (gemm_wgmma.cuh)
 static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_t st) {
+  const SimRows sim = sim_rows(c, r0, rows);
   GemmParams gp = sim_sweep(epi, rows, c->N, c->kcat, &c->bs->x_inv_scale, c->sym_tiles, c->n_sym_tiles, c->ra);
-  gp.a_row0 = r0; gp.S = c->S; gp.ldS = c->ldS;
+  gp.a_row0 = sim.row0; gp.S = c->S; gp.ldS = sim.ldS;
   if (epi & EPI_STATS) {
-    gp.lab_rows = c->step.label; gp.lab_cols = c->step.lab_total; gp.self_offset = c->rank * c->Q;
+    gp.lab_rows = sim.lab_rows; gp.lab_cols = sim.lab_cols; gp.self_offset = sim.col0;
     gp.fuse_thr = 1; gp.ra = c->ra; gp.mp = mining_of(c->cfg); gp.bs = c->bs;
     gp.thr_out = c->wscope ? reinterpret_cast<BlockStats*>(c->xch_src) : nullptr;   // world scope: the rank's record for the exchange
   }
@@ -1190,17 +1185,11 @@ static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
   return e;
 }
 
-// LOCAL relative selects of rows [r0, r0 + rows), which the S buffer holds
-static void local_select(npair_ctx* c, int r0, int rows, cudaStream_t st) {
-  launch_local_select(c->S, c->ldS, rows, c->N, c->step.label + r0, c->step.lab_total, c->rank * c->Q + r0, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn,
-                      rows_from(c->ra, r0), c->bs, c->sms, (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0, st);
-}
-
 static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
-  const float* d_label = c->step.label;
   const int self_off = c->rank * Q;
+  const bool lsel_warp = (c->cfg.flags & NPAIR_FLAG_LSEL_WARP) != 0;
   // ---- operand preparation: |x| sum (top asum, .cu:400), power-of-two pre-scale, split to tensor-core pieces ----
   {
     PhaseTimer pt(c, 1, st);
@@ -1219,7 +1208,7 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
     gp.M = Q; gp.Nn = N; gp.S = c->S; gp.ldS = c->ldS; gp.dev_scale = &c->bs->x_inv_scale;
     CUDA_TRY(c, launch_simt_gemm(c->prec, EPI_STORE_S, c->Xs + static_cast<long long>(self_off) * c->Dp, c->Dp, static_cast<long long>(N) * c->Dp,
                                  c->Xs, c->Dp, static_cast<long long>(N) * c->Dp, D, gp, st));
-    launch_row_stats_ref(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, c->ra, st);
+    launch_row_stats_ref(sim_rows(c, 0, Q), c->ra, st);
   }
   // ---- thresholds (.cu:275-337) ----
   {
@@ -1236,8 +1225,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
     // validate()); LOCAL selects of row blocks run in the row pass, block by block
     if (c->gsel_mask) {
       for (int pass = 0; pass < 3; ++pass) {
-        launch_global_select_pass(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, c->gsel_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap,
-                                  c->wscope ? 1 : 0, c->bs, c->sms, st);
+        launch_global_select_pass(sim_rows(c, 0, Q), c->gsel_mask, pass, c->ra, c->ghist, c->gcand, c->gcand_cap, c->wscope ? 1 : 0, c->bs, c->sms,
+                                  st);
         if (c->wscope) {
           const float* all = nullptr;
           const int rc = xchg_small(c, reinterpret_cast<const float*>(c->ghist), NPAIR_XCH_FLOATS, &all, st);
@@ -1246,7 +1235,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
         }
       }
     }
-    if (c->lsel_mask && c->n_blocks == 1) local_select(c, 0, Q, st);
+    if (c->lsel_mask && c->n_blocks == 1)
+      launch_local_select(sim_rows(c, 0, Q), c->lsel_mask, c->cfg.identsn, c->cfg.diffsn, c->ra, c->bs, c->sms, lsel_warp, st);
   }
   // ---- selection + counts + exp + masked sums + log + retrieval in one pass (.cu:343-398), per block of rows of S ----
   {
@@ -1255,10 +1245,12 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
     for (int r0 = 0; r0 < Q; r0 += c->s_rows) {
       const int rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
-      if (c->lsel_mask && c->n_blocks > 1) local_select(c, r0, rows, st);
+      const SimRows sim = sim_rows(c, r0, rows);
+      if (c->lsel_mask && c->n_blocks > 1)
+        launch_local_select(sim, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn, c->ra, c->bs, c->sms, lsel_warp, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
-      launch_lse_rows(c->S, c->ldS, Q, N, d_label, c->step.lab_total, self_off, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world,
-                      c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr, c->tops_seq, r0, rows, c->n_blocks == 1, st);
+      launch_lse_rows(sim, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world, c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr,
+                      c->tops_seq, c->n_blocks == 1, st);
     }
     if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
@@ -1384,7 +1376,6 @@ static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, flo
 static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
-  const int self_off = c->rank * Q;
   // loss_weight / dot_normalizer (.cu:427,448); world scope: the normaliser is the world's batch and the transposed term is not
   // divided by the world size, i.e. exactly what a single rank holding the whole batch computes
   const float lw_over_q = loss_weight / static_cast<float>(c->wscope ? N : Q);
@@ -1429,8 +1420,10 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     for (int k = 0; k < c->n_blocks; ++k) {
       const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
       CUDA_TRY(c, recompute_sim_block(c, r0, st));
-      fp.Q = rows; fp.ts = tile_sched(rows, D, c->grad_kblocks, c->grad_split); fp.m_blk0 = r0 / TileShape::BM;
-      fp.rowrec = c->ra.rowrec + r0; fp.self_offset = self_off + r0; fp.out = d_diff + static_cast<long long>(r0) * D;
+      // the fused kernel's rows start at the block: its record, self column and output rows are those of rank row sim.row0
+      const SimRows sim = sim_rows(c, r0, rows);
+      fp.Q = sim.rows; fp.ts = tile_sched(sim.rows, D, c->grad_kblocks, c->grad_split); fp.m_blk0 = sim.row0 / TileShape::BM;
+      fp.rowrec = c->ra.rowrec + sim.row0; fp.self_offset = sim.self_col(sim.row0); fp.out = d_diff + static_cast<long long>(sim.row0) * D;
       CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
       if (fp.ts.splits > 1) reduce_splits(c, fp.ts.splits, rows, fp.out, 0.f, st);
     }
@@ -1439,7 +1432,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   }
   {
     PhaseTimer pt(c, 5, st);
-    launch_build_weights(c->S, c->ldS, Q, N, c->step.label, c->step.lab_total, self_off, c->world, bw_mode, rs_total, mp, c->ra, c->prec, c->H, c->Np, c->HT, c->Qp, st);
+    launch_build_weights(sim_rows(c, 0, Q), c->world, bw_mode, rs_total, mp, c->ra, c->prec, c->H, c->Np, c->HT, c->Qp, st);
   }
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.dev_scale = &c->bs->x_inv_scale;

@@ -1,5 +1,6 @@
 // kernels.cu -- HBM-bound kernels of the N-pair hot path (everything except the two tensor-core contractions).
 // Each kernel cites the reference code it replaces (paths relative to /root/reference).
+#include <cassert>
 #include <cstdlib>
 #include "kernels.cuh"
 #include <cuda.h>
@@ -326,19 +327,17 @@ void launch_split(const float* x_total, int N, int D, int prec, const BlockScala
 // statistics init / reference row statistics (caffe_set of the three stat blobs, .cu:230-236)
 // --------------------------------------------------------------------------------------------
 // One block per row; same outputs as the sim-GEMM epilogue.  Used by the SIMT cross-check backend and by tests.
-__global__ void row_stats_ref_kernel(const float* __restrict__ S, long long ldS, int Q, int N, const float* __restrict__ lab_rows,
-                                     const float* __restrict__ lab_cols, int self_offset, RowArrays ra) {
-  const int i = blockIdx.x;
-  const float li = lab_rows[i];
-  const int self_col = i + self_offset;
+__global__ void row_stats_ref_kernel(const __grid_constant__ SimRows sim, RowArrays ra) {
+  const int i = sim.row0 + blockIdx.x;
+  const float li = __ldg(sim.lab_rows + i);
   float minw = FLT_MAX, maxw = -FLT_MAX, maxb = -FLT_MAX, maxall = -FLT_MAX;
   int cnt = 0;
-  const float* row = S + static_cast<long long>(i) * ldS;
-  for (int j = threadIdx.x; j < N; j += blockDim.x) {
-    if (j == self_col) continue;
-    const float v = row[j];
+  const float* row = sim.row(i);
+  for (int j = threadIdx.x; j < sim.N; j += blockDim.x) {
+    if (j == sim.self_col(i)) continue;
+    const float v = __ldg(row + j);
     maxall = fmaxf(maxall, v);
-    if (lab_cols[j] == li) { minw = fminf(minw, v); maxw = fmaxf(maxw, v); ++cnt; } else maxb = fmaxf(maxb, v);
+    if (__ldg(sim.lab_cols + j) == li) { minw = fminf(minw, v); maxw = fmaxf(maxw, v); ++cnt; } else maxb = fmaxf(maxb, v);
   }
   minw = warp_min(minw); maxw = warp_max(maxw); maxb = warp_max(maxb); maxall = warp_max(maxall); cnt = warp_sum_i(cnt);
   if ((threadIdx.x & 31) == 0) {
@@ -347,9 +346,8 @@ __global__ void row_stats_ref_kernel(const float* __restrict__ S, long long ldS,
     if (cnt) atomicAdd(&ra.cnt_same[i], cnt);
   }
 }
-void launch_row_stats_ref(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, RowArrays ra, cudaStream_t st) {
-  row_stats_ref_kernel<<<Q, 256, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, ra);
+void launch_row_stats_ref(SimRows sim, RowArrays ra, cudaStream_t st) {
+  row_stats_ref_kernel<<<sim.rows, 256, 0, st>>>(sim, ra);
   count_launch();
 }
 
@@ -511,20 +509,20 @@ __device__ __noinline__ uint32_t slow_select_row(const float* __restrict__ row, 
   return prefix;
 }
 
-__global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
-                                                                              const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
-                                                                              int self_offset, int side_mask /*1 AP, 2 AN*/, float sn_ap, float sn_an,
-                                                                              RowArrays ra, BlockScalars* bs) {
+__global__ void __launch_bounds__(32 * NPAIR_LSEL_WARPS, 2) local_select_kernel(const __grid_constant__ SimRows sim, int side_mask /*1 AP, 2 AN*/, float sn_ap,
+                                                                              float sn_an, RowArrays ra, BlockScalars* bs) {
   extern __shared__ __align__(16) unsigned char lsel_smem[];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   LselWarp& W = reinterpret_cast<LselWarp*>(lsel_smem)[w];
   const bool want_same = side_mask & 1, want_diff = side_mask & 2;
+  const int N = sim.N;
+  const float* lab_cols = sim.lab_cols;
   const bool lab_aligned = (reinterpret_cast<uintptr_t>(lab_cols) & 15) == 0;
   const int nwarps = gridDim.x * NPAIR_LSEL_WARPS;
-  for (int i = blockIdx.x * NPAIR_LSEL_WARPS + w; i < Q; i += nwarps) {
-    const float li = lab_rows[i];
-    const int self_col = i + self_offset;
-    const float* row = S + static_cast<long long>(i) * ldS;
+  for (int i = sim.row0 + blockIdx.x * NPAIR_LSEL_WARPS + w; i < sim.row0 + sim.rows; i += nwarps) {
+    const float li = __ldg(sim.lab_rows + i);
+    const int self_col = sim.self_col(i);
+    const float* row = sim.row(i);
     const int cs = ra.cnt_same[i];
     // ---------------- sweep 1 ----------------
     for (int b = lane * 4; b < NPAIR_LSEL_D1; b += 128) *reinterpret_cast<uint4*>(&W.hist[b]) = make_uint4(0u, 0u, 0u, 0u);
@@ -722,22 +720,23 @@ __device__ __forceinline__ uint4 ldg_stream_u4(const float* p) {
 // byte offset (bin * 4) of an entry in the histogram: monotone in f; NaN -> 0x3FFC
 __device__ __forceinline__ uint32_t lsb_off(uint32_t bits, float s4, float c0) { return __float_as_uint(__fmaf_rn(__uint_as_float(bits), s4, c0)) & 0x3FFCu; }
 
-__global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_select_block_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
-                                                                                   const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
-                                                                                   int self_offset, int side_mask /*1 AP, 2 AN*/, float sn_ap, float sn_an,
-                                                                                   RowArrays ra, BlockScalars* bs) {
+__global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_select_block_kernel(const __grid_constant__ SimRows sim, int side_mask /*1 AP, 2 AN*/,
+                                                                                   float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs) {
   __shared__ __align__(16) LselBlock B;
   constexpr uint32_t kNaN = 0x7FFFFFFFu;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const bool want_same = side_mask & 1, want_diff = side_mask & 2;
   // whole 4-column groups come through 16-byte loads (rows start 128-byte aligned: ldS is a multiple of 32); the last N % 4 columns
   // sit in one extra register of threads 0..2
+  const int N = sim.N;
+  const float* lab_cols = sim.lab_cols;
   const int n4 = N & ~3;
   const bool has_tail = tid < N - n4;
   uint32_t v[4 * NPAIR_LSB_VPT + 1];       // [32] = the tail column (NaN where there is none)
-  int i = blockIdx.x;
+  const int row_end = sim.row0 + sim.rows;
+  int i = sim.row0 + blockIdx.x;
   auto load_row = [&](int r) {
-    const float* row = S + static_cast<long long>(r) * ldS;
+    const float* row = sim.row(r);
 #pragma unroll
     for (int u = 0; u < NPAIR_LSB_VPT; ++u) {
       const int jj = (u * NPAIR_LSB_THREADS + tid) * 4;
@@ -747,10 +746,10 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
     }
     v[4 * NPAIR_LSB_VPT] = has_tail ? __float_as_uint(row[n4 + tid]) : kNaN;
   };
-  if (i < Q) load_row(i);
-  for (; i < Q; i += gridDim.x) {
-    const float li = lab_rows[i];
-    const int self_col = i + self_offset;
+  if (i < row_end) load_row(i);
+  for (; i < row_end; i += gridDim.x) {
+    const float li = __ldg(sim.lab_rows + i);
+    const int self_col = sim.self_col(i);
     const int cs = ra.cnt_same[i];
     for (int b = tid * 4; b < NPAIR_LSB_HIST; b += NPAIR_LSB_THREADS * 4) *reinterpret_cast<uint4*>(&B.hist[b]) = make_uint4(0u, 0u, 0u, 0u);
     if (tid == 0) { B.n_same = 0; B.n_cand = 0; }
@@ -763,7 +762,7 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
       if (jj < n4) {
         const float4 l = __ldg(reinterpret_cast<const float4*>(lab_cols + jj));
         const float ll[4] = {l.x, l.y, l.z, l.w};
-        if (static_cast<unsigned int>(self_col - jj) < 4u || l.x == li || l.y == li || l.z == li || l.w == li) {
+        if (sim.self_in4(i, jj) || l.x == li || l.y == li || l.z == li || l.w == li) {
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
             if (ll[c] == li && jj + c != self_col) same_append(&B.n_same, B.same, v[4 * u + c]);
@@ -865,8 +864,8 @@ __global__ void __launch_bounds__(NPAIR_LSB_THREADS, NPAIR_LSB_MINB) local_selec
       }
     }
     // ---------------- the registers are free: the next row streams in while this row's pick runs ----------------
-    const float* row = S + static_cast<long long>(i) * ldS;
-    if (i + static_cast<int>(gridDim.x) < Q) load_row(i + static_cast<int>(gridDim.x));
+    const float* row = sim.row(i);
+    if (i + static_cast<int>(gridDim.x) < row_end) load_row(i + static_cast<int>(gridDim.x));
     if (have_an && !refine) {
       __syncthreads();
       store_key_of_rank([&](unsigned int t) { return B.cand[t]; }, B.n_cand, rank, tid, NPAIR_LSB_THREADS, &ra.nega_thr[i]);   // .cu:319
@@ -882,19 +881,18 @@ static constexpr int LSEL_SMEM = static_cast<int>(sizeof(LselWarp)) * NPAIR_LSEL
 cudaError_t allow_local_select_smem() {
   return cudaFuncSetAttribute(local_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LSEL_SMEM);
 }
-void launch_local_select(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                         int self_offset, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st) {
-  if (!force_warp_kernel && N <= NPAIR_LSB_THREADS * NPAIR_LSB_VPT * 4 && (reinterpret_cast<uintptr_t>(lab_cols) & 15) == 0 && (ldS & 3) == 0) {
-    int grid = sms * NPAIR_LSB_MINB; if (grid > Q) grid = Q;
-    local_select_block_kernel<<<grid, NPAIR_LSB_THREADS, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, side_mask, sn_ap, sn_an, ra, bs);
+void launch_local_select(SimRows sim, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st) {
+  if (!force_warp_kernel && sim.N <= NPAIR_LSB_THREADS * NPAIR_LSB_VPT * 4 && (reinterpret_cast<uintptr_t>(sim.lab_cols) & 15) == 0 && (sim.ldS & 3) == 0) {
+    int grid = sms * NPAIR_LSB_MINB; if (grid > sim.rows) grid = sim.rows;
+    local_select_block_kernel<<<grid, NPAIR_LSB_THREADS, 0, st>>>(sim, side_mask, sn_ap, sn_an, ra, bs);
     count_launch();
     return;
   }
   const int per_sm = (227 * 1024) / (LSEL_SMEM + 1024);
   int grid = sms * (per_sm < 1 ? 1 : per_sm);
-  const int need = (Q + NPAIR_LSEL_WARPS - 1) / NPAIR_LSEL_WARPS;
+  const int need = (sim.rows + NPAIR_LSEL_WARPS - 1) / NPAIR_LSEL_WARPS;
   if (grid > need) grid = need;
-  local_select_kernel<<<grid, 32 * NPAIR_LSEL_WARPS, LSEL_SMEM, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, side_mask, sn_ap, sn_an, ra, bs);
+  local_select_kernel<<<grid, 32 * NPAIR_LSEL_WARPS, LSEL_SMEM, st>>>(sim, side_mask, sn_ap, sn_an, ra, bs);
   count_launch();
 }
 
@@ -1025,9 +1023,9 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
 
   if (sweep0 || sweep1) {
     for (int i = blockIdx.x; i < Q; i += gridDim.x) {
+      const SimRows sim{S, ldS, Q, N, 0, Q, lab_rows, lab_cols, self_offset};    // the rank's whole S
       const float li = lab_rows[i];
-      const int self_col = i + self_offset;
-      const float* row = S + static_cast<long long>(i) * ldS;
+      const float* row = sim.row(i);
       // two 16-byte groups per thread in flight (S and labels): the sweeps are latency-bound otherwise
       for (int j0 = threadIdx.x * 4; j0 < N; j0 += blockDim.x * 8) {
         uint4 vq[2]; float lq[2][4];
@@ -1048,7 +1046,7 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
         if (j4 >= N) continue;
         const uint32_t vv[4] = {vq[u].x, vq[u].y, vq[u].z, vq[u].w};
         const float* ll = lq[u];
-        const bool no_self = self_col < j4 || self_col > j4 + 3;
+        const bool no_self = !sim.self_in4(i, j4);
         if (j4 + 3 < N && no_self && ll[0] != li && ll[1] != li && ll[2] != li && ll[3] != li) {     // four diff-label pairs: the common case
           if (sweep1) {
             if (pass == 0) {
@@ -1062,7 +1060,7 @@ __global__ void __launch_bounds__(512) global_select_kernel(const float* __restr
         } else {
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
-            if (j4 + c >= N || j4 + c == self_col) continue;                    // the self pair is in neither list (.cu:54)
+            if (j4 + c >= N || j4 + c == sim.self_col(i)) continue;             // the self pair is in neither list (.cu:54)
             const int side = (ll[c] == li) ? 0 : 1;
             if (!(side == 0 ? sweep0 : sweep1)) continue;
             if (pass == 0) smem_inc(&hist[side][vv[c] >> 21]);
@@ -1145,12 +1143,13 @@ __global__ void __launch_bounds__(512) global_decide_kernel(const float* __restr
   __syncthreads();
   global_decide(pass, act0, act1, gb, ra, Q, bs, s_scan, s_out);
 }
-void launch_global_select_pass(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                               int self_offset, int side_mask, int pass, RowArrays ra, unsigned long long* hist, uint32_t* cand,
-                               unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st) {
-  int grid = sms * 4; if (grid > Q) grid = Q;
+void launch_global_select_pass(SimRows sim, int side_mask, int pass, RowArrays ra, unsigned long long* hist, uint32_t* cand, unsigned int cand_cap,
+                               int world_scope, BlockScalars* bs, int sms, cudaStream_t st) {
+  assert(sim.row0 == 0 && sim.rows == sim.Q && "the GLOBAL select sweeps the rank's whole S");
+  int grid = sms * 4; if (grid > sim.rows) grid = sim.rows;
   GlobalSelectBufs gb; gb.hist = hist; gb.cand = cand; gb.cap = cand_cap; gb.world_scope = world_scope;
-  global_select_kernel<<<grid, 512, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, side_mask, pass, gb, ra, bs);
+  // positional arguments, from which the kernel builds its view of the whole S: as a view parameter it compiles to other, slower code
+  global_select_kernel<<<grid, 512, 0, st>>>(sim.S, sim.ldS, sim.Q, sim.N, sim.lab_rows, sim.lab_cols, sim.col0, side_mask, pass, gb, ra, bs);
   count_launch();
 }
 void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
@@ -1283,15 +1282,11 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
 #ifndef NPAIR_LSE_MINB
 #define NPAIR_LSE_MINB 3
 #endif
-__global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
-                                                       const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
-                                                       int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs,
+__global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __grid_constant__ SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs,
                                                        int num_tops, TopsBlock* __restrict__ tops, float log2_world,
                                                        TopSums* __restrict__ xout /*world scope: this rank's tops sums, else NULL*/,
                                                        int wpr /*warps per row: 1, 2, 4 or 8 (few rows per rank: keep the SMs full)*/,
-                                                       unsigned int seq /*written behind the tops: the host polls it*/,
-                                                       int row0, int rows /*rows [row0, row0 + rows) of the rank; S holds them from row 0*/,
-                                                       int finalize) {
+                                                       unsigned int seq /*written behind the tops: the host polls it*/, int finalize) {
   const int lane = threadIdx.x & 31;
   __shared__ float s_pA[8], s_pT[8];
   __shared__ int s_pc[8];
@@ -1302,16 +1297,18 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
 #endif
   const int blk = NPAIR_LSE_REV ? static_cast<int>(gridDim.x - 1 - blockIdx.x) : static_cast<int>(blockIdx.x);
   const int wib = threadIdx.x >> 5;
-  const int il = blk * ((blockDim.x >> 5) / wpr) + wib / wpr;  // row of S
-  const int i = row0 + il;                                      // row of the rank
+  const int il = blk * ((blockDim.x >> 5) / wpr) + wib / wpr;  // row of the launch
+  const int i = sim.row0 + il;                                  // row of the rank
+  const int Q = sim.Q, N = sim.N;
+  const float* lab_cols = sim.lab_cols;
   const int part = wib % wpr;                                   // this warp's column segment of the row
   float A = 0.f, T = 0.f; int c = 0;
   float m2 = 0.f, thr_p = 0.f, thr_n = 0.f, li = 0.f; int cs = 0;
-  if (il < rows) {
+  if (il < sim.rows) {
     // the first block of this warp's segment is requested before anything else: the per-row set-up below (dependent loads of the row
     // statistics, the retrieval cut's expf search) then runs under the DRAM latency instead of in front of it
     constexpr int U = NPAIR_LSE_U;
-    const float* row = S + static_cast<long long>(il) * ldS;
+    const float* row = sim.row(i);
     // this warp's segment [c_lo, c_hi) of the row: multiples of 512 columns
     const int seg = ((N + wpr - 1) / wpr + 128 * U - 1) / (128 * U) * (128 * U);
     const int c_lo = min(N, part * seg), c_hi = min(N, c_lo + seg);
@@ -1325,8 +1322,8 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
 #pragma unroll
       for (int u = 0; u < U; ++u) v[u] = ldg_stream(srow4 + 32 * u);
     }
-    li = lab_rows[i];
-    const int self_col = i + self_offset;
+    li = __ldg(sim.lab_rows + i);
+    const int self_col = sim.self_col(i);
     const float max_all = ord2f(ra.st_maxall[i]);
     m2 = max_all * LOG2E;
     // GLOBAL-region thresholds are block-wide scalars (finish_thresholds / global_decide); LOCAL ones are per row
@@ -1358,7 +1355,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
           const int j4 = base + u * 128 + lane * 4;
           const float vv[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
           const float ll[4] = {l[u].x, l[u].y, l[u].z, l[u].w};
-          const bool no_self = (self_col < j4 || self_col > j4 + 3);
+          const bool no_self = !sim.self_in4(i, j4);
           if (no_self && ll[0] != li && ll[1] != li && ll[2] != li && ll[3] != li) {
             // four diff-label pairs (all but ~cnt_same/4 groups of a row): no label-dependent selects, 8 instructions per pair
 #pragma unroll
@@ -1405,7 +1402,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const flo
       for (int q = 0; q < wpr; ++q) { A += s_pA[wib + q]; T += s_pT[wib + q]; c += s_pc[wib + q]; }
     }
   }
-  if (il < rows && part == 0) {
+  if (il < sim.rows && part == 0) {
     if (lane == 0) {
       ra.A[i] = A; ra.T[i] = T;                                 // T = A + B (.cu:380)
       ra.logv[i] = (A == 0.f || T == 0.f) ? 0.f : logf(A / T);  // .cu:162-169
@@ -1454,15 +1451,14 @@ static void lse_shape(int Q, int N, int* wpr_out, int* threads_out) {
   while (wpb > 1 && (Q + wpb - 1) / wpb < 296) wpb >>= 1;     // keep >= 2 blocks per SM when the rank has few rows
   *threads_out = wpb * 32;
 }
-void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
-                     unsigned int seq, int row0, int rows, bool finalize, cudaStream_t st) {
+void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
+                     unsigned int seq, bool finalize, cudaStream_t st) {
   int wpr = 1, threads = 256;
-  lse_shape(Q, N, &wpr, &threads);
+  lse_shape(sim.Q, sim.N, &wpr, &threads);
   const int rows_per_blk = threads / 32 / wpr;
-  const int grid = (rows + rows_per_blk - 1) / rows_per_blk;
-  lse_rows_kernel<<<grid, threads, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, mp, ra, bs, num_tops, tops_dev,
-                                            xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq, row0, rows, finalize ? 1 : 0);
+  const int grid = (sim.rows + rows_per_blk - 1) / rows_per_blk;
+  lse_rows_kernel<<<grid, threads, 0, st>>>(sim, mp, ra, bs, num_tops, tops_dev, xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq,
+                                            finalize ? 1 : 0);
   count_launch();
 }
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st) {
@@ -1525,13 +1521,12 @@ __device__ __forceinline__ void store_quad(uint16_t* __restrict__ base, long lon
 //   transposed term G[m][j] of row m on another rank is evaluated here from S[j][m] and row m's all-gathered scalars:
 //     H[j][m] = g'(S[j][m]; row j) + (1/world) g'(S[j][m]; row m)          -- no N x D reduce-scatter (.cu:455-497)
 template <int PREC, int MODE>
-__global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __restrict__ S, long long ldS, int Q, int N,
-                                                            const float* __restrict__ lab_rows, const float* __restrict__ lab_cols,
-                                                            int self_offset, float inv_world, const RowRecord* __restrict__ rs_total,
+__global__ void __launch_bounds__(256, 4) build_weights_kernel(const __grid_constant__ SimRows sim, float inv_world, const RowRecord* __restrict__ rs_total,
                                                             MiningParams mp, RowArrays ra,
                                                             uint16_t* __restrict__ H, long long ldH, uint16_t* __restrict__ HT, long long ldHT) {
   constexpr bool SYM = (MODE != BW_SPLIT);      // both symmetric modes add the row-m term
   constexpr int TS = 64;
+  const int Q = sim.Q, N = sim.N;
   const int ta = blockIdx.y, tb = blockIdx.x;
   __shared__ RowScal sc_a[TS], sc_b[TS];
   const int a0 = ta * TS, b0 = tb * TS;
@@ -1547,7 +1542,7 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
       sc_b[mm] = row_scal(m < N ? rs_total + m : nullptr, inv_world);
     } else {
       RowScal r = row_scal(nullptr, 1.f);
-      if (m < N) r.lab = lab_cols[m];
+      if (m < N) r.lab = sim.lab_cols[m];
       sc_b[mm] = r;
     }
   }
@@ -1557,14 +1552,14 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
 #pragma unroll
   for (int e = 0; e < 4; ++e) rb4[e] = sc_b[4 * tc + e];
   // block-uniform fast path: tile fully inside the matrix and not touching the self-pair diagonal
-  const bool interior = (a0 + TS <= Q) && (b0 + TS <= N) && (a0 + self_offset + TS <= b0 || b0 + TS <= a0 + self_offset);
+  const bool interior = (a0 + TS <= Q) && (b0 + TS <= N) && (sim.self_col(a0) + TS <= b0 || b0 + TS <= sim.self_col(a0));
   const long long psH = static_cast<long long>(Q) * ldH;
   float gT[4][4];                                        // BW_SPLIT: transposed copy for HT
   float4 v4[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {                          // all four 16-byte loads in flight before the arithmetic
     v4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (ja0 + i < Q && mb0 < N) v4[i] = *reinterpret_cast<const float4*>(S + static_cast<long long>(ja0 + i) * ldS + mb0);
+    if (ja0 + i < Q && mb0 < N) v4[i] = *reinterpret_cast<const float4*>(sim.row(ja0 + i) + mb0);
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -1575,7 +1570,7 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
     for (int e = 0; e < 4; ++e) {
       const int j = ja0 + i, m = mb0 + e;
       float x = 0.f;
-      if (interior || (j < Q && m < N && m != j + self_offset)) {
+      if (interior || (j < Q && m < N && m != sim.self_col(j))) {
         const bool same = rsa.lab == rb4[e].lab;
         x = gprime(sv[e], same, rsa, sgn_p, sgn_n);
         if (SYM) x += gprime(sv[e], same, rb4[e], sgn_p, sgn_n);
@@ -1592,15 +1587,15 @@ __global__ void __launch_bounds__(256, 4) build_weights_kernel(const float* __re
       if (mb0 + e < N && ja0 < ldHT) store_quad<PREC>(HT, psT, static_cast<long long>(mb0 + e) * ldHT + ja0, gT[e]);   // rows beyond Q are zero
   }
 }
-void launch_build_weights(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
+void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH, uint16_t* HT, long long ldHT, cudaStream_t st) {
-  dim3 grid((N + 63) / 64, (Q + 63) / 64);
+  assert(sim.row0 == 0 && sim.rows == sim.Q && "the weight builder sweeps the rank's whole S");
+  dim3 grid((sim.N + 63) / 64, (sim.Q + 63) / 64);
   const float inv_world = 1.f / static_cast<float>(world);
   with_prec(prec, [&](auto P) {
     auto kernel = mode == BW_SYM ? build_weights_kernel<P, BW_SYM> : mode == BW_ROWSCAL ? build_weights_kernel<P, BW_ROWSCAL>
                                                                                         : build_weights_kernel<P, BW_SPLIT>;
-    kernel<<<grid, 256, 0, st>>>(S, ldS, Q, N, lab_rows, lab_cols, self_offset, inv_world, rs_total, mp, ra, H, ldH, HT, ldHT);
+    kernel<<<grid, 256, 0, st>>>(sim, inv_world, rs_total, mp, ra, H, ldH, HT, ldHT);
   });
   count_launch();
 }

@@ -179,6 +179,26 @@ struct RowArrays {
   RowRecord* rowrec;         // [Q] what the backward needs of each row
 };
 
+// What one launch reads of the rank's Q x N similarity matrix: rows [row0, row0 + rows) of the rank, which the buffer S holds from
+// its row 0 (a materialised S is the one block row0 = 0, rows = Q).  Kernels index RANK rows i -- labels, RowArrays (hits[k * Q + i]
+// included) -- unshifted and reach row i's similarities through row(i).  Row i's self pair is column self_col(i), excluded by
+// position whatever its label (a NaN label equals nothing, its own included).  Kernels take the view as a const __grid_constant__
+// parameter (a plain one spills more in the selects, CUDA 12.9); its pointers are no __restrict__ parameters, so loads that must
+// stay read-only say so with __ldg.
+struct SimRows {
+  const float* S;
+  long long ldS;
+  int Q, N;                  // the rank's rows, the world's columns
+  int row0, rows;
+  const float* lab_rows;     // [Q] the rank's labels
+  const float* lab_cols;     // [N] the world's labels
+  int col0;                  // world column of rank row 0: rank * Q
+  __host__ __device__ __forceinline__ const float* row(int i) const { return S + static_cast<long long>(i - row0) * ldS; }
+  __host__ __device__ __forceinline__ int self_col(int i) const { return i + col0; }
+  // whether row i's self column is one of the four columns j4 .. j4 + 3
+  __host__ __device__ __forceinline__ bool self_in4(int i, int j4) const { return !(self_col(i) < j4 || self_col(i) > j4 + 3); }
+};
+
 // order-preserving float <-> uint32 map so atomicMin/atomicMax work on floats of either sign
 __host__ __device__ __forceinline__ uint32_t f2ord(float f) {
 #ifdef __CUDA_ARCH__
@@ -209,8 +229,7 @@ void launch_split(const float* x_total, int N, int D, int prec, const BlockScala
                   uint16_t* Xs, long long ldXs /*Dp*/, uint16_t* XsT, long long ldXsT /*Np*/,
                   uint16_t* XlT, long long ldXlT /*Qp, or 0*/, int row0_local, int Q,
                   uint16_t* XcatA /*or NULL*/, uint16_t* XcatB, long long Dp, cudaStream_t st);
-void launch_row_stats_ref(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, RowArrays ra, cudaStream_t st);
+void launch_row_stats_ref(SimRows sim, RowArrays ra, cudaStream_t st);
 // The threshold pick of the rank's Q rows by one block (SIMT backend; the tensor-core similarity sweep runs it in its last CTA)
 void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, cudaStream_t st);
 // World scope: the thresholds of the world's N rows from the ranks' BlockStats, which lie xstride floats apart in xall
@@ -218,28 +237,25 @@ void launch_thresholds_world(const float* xall, int xstride, int world, long lon
 // World scope: the tops of the world's N rows from the ranks' TopSums, which lie xstride floats apart in xall
 void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // side_mask: bit 0 = AP threshold over the same-label list, bit 1 = AN threshold over the diff-label list
-void launch_local_select(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                         int self_offset, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
+void launch_local_select(SimRows sim, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
 // lets the current device launch the one-warp-per-row local select with its dynamic shared memory (above the default limit)
 cudaError_t allow_local_select_smem();
-void launch_global_select_pass(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                               int self_offset, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
+// over the rank's whole S (sim.row0 == 0, sim.rows == Q)
+void launch_global_select_pass(SimRows sim, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
                                uint32_t* cand /*[2][cand_cap]*/, unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st);
 // world scope: the ranks' [2][2048] 64-bit digit counts lie xstride floats apart in xall
 void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
                           uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
-// Row pass over rows [row0, row0 + rows) of the rank (S points at row row0's similarities; lab_rows, self_offset and ra are the
-// rank's).  finalize: the last block also reduces the Q rows' results into the tops; otherwise launch_lse_finalize does, once.
-// xout: NULL, or (world scope) receives the rank's TopSums instead of the tops
-void launch_lse_rows(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                     int self_offset, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev,
-                     int world, TopSums* xout, unsigned int seq, int row0, int rows, bool finalize, cudaStream_t st);
+// Row pass over the rows of sim.  finalize: the last block also reduces the Q rows' results into the tops; otherwise
+// launch_lse_finalize does, once.  xout: NULL, or (world scope) receives the rank's TopSums instead of the tops
+void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
+                     unsigned int seq, bool finalize, cudaStream_t st);
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-record
 // exchange: rs_total = the world's N records, all-gathered)
 enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
-void launch_build_weights(const float* S, long long ldS, int Q, int N, const float* lab_rows, const float* lab_cols,
-                          int self_offset, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
+// over the rank's whole S (sim.row0 == 0, sim.rows == Q)
+void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH /*Np*/, uint16_t* HT, long long ldHT /*Qp*/, cudaStream_t st);
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);

@@ -281,16 +281,20 @@ def test_relabelling_is_bitwise(cuda, family, Q, world, flags):
 
 
 # ------------------------------------------------------------------------------------------------------------------ 5. row blocks
-@pytest.mark.parametrize("family", ["shuffled", "nan"])
-def test_row_blocks(cuda, family):
-    """NPAIR_SIM_BLOCK_ROWS(256) at Q = 999 is bit for bit the materialised path (checked against the oracle in test_medium_shapes).
-    Row-block mode refuses a GLOBAL relative side with a general SN, so the GLOBAL mining here is global_hard."""
+@pytest.mark.parametrize("family,world", [("shuffled", 1), ("nan", 1), ("shuffled", 2), ("nan", 2)],
+                         ids=["shuffled", "nan", "shuffled-w2", "nan-w2"])
+def test_row_blocks(cuda, family, world):
+    """NPAIR_SIM_BLOCK_ROWS(256) at Q = 999 per rank is bit for bit the materialised path (checked against the oracle in
+    test_medium_shapes).  At world 2 a block's self columns are offset by both the rank and the block, and with NaN labels only their
+    position keeps the self pairs out of the LOCAL selects.  Row-block mode refuses a GLOBAL relative side with a general SN, so the
+    GLOBAL mining here is global_hard."""
     from test_gpu_sim_blocks import _compare
     Q = 999
-    x, lab = family_inputs(family, Q, 101, seed=Q + 101 + FAMILIES.index(family), noise=2.5)
+    D = 101 if world == 1 else 128          # each rank's slice of the gradient must start on the 16-byte grid
+    x, lab = family_inputs(family, Q * world, D, seed=Q + D + FAMILIES.index(family), noise=2.5)
     for name in ("usage", "local_rel_an", "global_hard"):
         for flags in ((0, capi.FLAG_LSEL_WARP) if name.startswith("local") else (0,)):
-            _compare(x, lab, Q, 1, 256, f"{family} {name} f{flags} row blocks", flags=flags, **MEDIUM_MININGS[name])
+            _compare(x, lab, Q, world, 256, f"{family} w{world} {name} f{flags} row blocks", flags=flags, **MEDIUM_MININGS[name])
 
 
 # ------------------------------------------------------------------------------------------------------------------ 6. headline size
