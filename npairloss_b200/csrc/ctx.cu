@@ -24,18 +24,13 @@
 #include "../../include/npair_b200.h"
 #include "gemm_wgmma.cuh"
 #include "grad_fused.cuh"
+#include "host.cuh"
 #include "kernels.cuh"
 
 namespace npair {
 
 // ------------------------------------------------------------------------------------------------ errors
-static thread_local std::string g_create_err;
-
-static std::string fmt(const char* f, ...) {
-  char buf[1024];
-  va_list ap; va_start(ap, f); vsnprintf(buf, sizeof(buf), f, ap); va_end(ap);
-  return std::string(buf);
-}
+thread_local std::string g_create_err;
 
 // ------------------------------------------------------------------------------------------------ NCCL (dlopen)
 struct NcclId { char internal[128]; };
@@ -121,8 +116,8 @@ static PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
 }
 
 // 3-D map over NSPLIT stacked 2-byte matrices [piece][rows][ld]; inner extent `cols` (<= ld), box {bk, box_rows, 1}
-static bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int pieces, long long ld_elems,
-                             long long piece_stride_elems, int bk, int box_rows, std::string* err) {
+bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int pieces, long long ld_elems,
+                      long long piece_stride_elems, int bk, int box_rows, std::string* err) {
   auto fn = tmap_encode_fn();
   if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
   cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(pieces)};
@@ -138,14 +133,14 @@ static bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int row
 
 // The similarity GEMM's operand maps over K-concatenated rows of kcat elements (split_kernel): `a` over rows_a rows from A (128-row
 // boxes), `b` over rows_b rows from B (256-row boxes), both in 64-element K blocks
-static bool make_tmap_kcat(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, long long kcat,
-                           std::string* err) {
+bool make_tmap_kcat(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, long long kcat,
+                    std::string* err) {
   return make_tmap_pieces(a, A, static_cast<int>(kcat), rows_a, 1, kcat, rows_a * kcat, 64, 128, err) &&
          make_tmap_pieces(b, B, static_cast<int>(kcat), rows_b, 1, kcat, rows_b * kcat, 64, 256, err);
 }
 
 // 2-D fp32 map over the similarity matrix [rows x ld], inner extent `cols`, box {32, 32}, 128B swizzle (TMA stores)
-static bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int rows, long long ld_elems, std::string* err, int box_rows = 32) {
+bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int rows, long long ld_elems, std::string* err, int box_rows) {
   auto fn = tmap_encode_fn();
   if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
@@ -156,143 +151,6 @@ static bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int 
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { *err = fmt("cuTensorMapEncodeTiled(S) failed (%d): cols=%d rows=%d ld=%lld", (int)r, cols, rows, ld_elems); return false; }
   return true;
-}
-
-// ------------------------------------------------------------------------------------------------ GEMM launchers
-static int gemm_grid(const TileSched& ts, int sms) { return ts.num_tiles() < sms ? ts.num_tiles() : sms; }   // one CTA per tile, at most one per SM
-
-// K-block per (operand format, GEMM role); see GemmCfg
-static constexpr int bk_of(int prec, int epi) {
-  if (epi != EPI_OUT) return 64;                 // similarity GEMM: single pass, 64-element K blocks
-  return prec == PREC_BF16 ? 64 : 32;
-}
-
-// A GEMM kernel instantiation with its launch shape.  Its dynamic shared memory exceeds the default limit, so every device that
-// launches it has to allow that much first (allow_smem).
-struct GemmKernel { void (*fn)(CUtensorMap, CUtensorMap, CUtensorMap, GemmParams); int threads, smem; };
-struct FusedKernel { void (*fn)(CUtensorMap, CUtensorMap, FusedGradParams); int threads, smem; };
-template <class K>
-static cudaError_t allow_smem(const K& k) {
-  return k.fn ? cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem) : cudaErrorInvalidValue;
-}
-
-template <int NSPLIT, bool BF16, int EPI, int BK>
-static GemmKernel gemm_t() {
-  using Cfg = GemmCfg<NSPLIT, BK, EPI>;
-  return GemmKernel{split_gemm_kernel<NSPLIT, BF16, EPI, BK>, Cfg::THREADS, Cfg::SMEM_BYTES};
-}
-// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  Only the
-// epilogues the host composes are instantiated.
-template <bool BF16>
-static GemmKernel sim_gemm_t(int epi) {
-  switch (epi) {
-    case EPI_STORE_S | EPI_STATS: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS, 64>();
-    case EPI_STORE_S | EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS | EPI_SYM, 64>();
-    case EPI_STATS: return gemm_t<1, BF16, EPI_STATS, 64>();
-    case EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STATS | EPI_SYM, 64>();
-    case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
-    case EPI_COUNT: return gemm_t<1, BF16, EPI_COUNT, 64>();                       // retrieval evaluation
-    case EPI_COUNT | EPI_SYM: return gemm_t<1, BF16, EPI_COUNT | EPI_SYM, 64>();
-    case EPI_GATHER: return gemm_t<1, BF16, EPI_GATHER, 64>();                     // MAP@R evaluation
-    case EPI_GATHER | EPI_SYM: return gemm_t<1, BF16, EPI_GATHER | EPI_SYM, 64>();
-    case EPI_BUCKET: return gemm_t<1, BF16, EPI_BUCKET, 64>();
-    case EPI_BUCKET | EPI_SYM: return gemm_t<1, BF16, EPI_BUCKET | EPI_SYM, 64>();
-    case EPI_ARGMAX: return gemm_t<1, BF16, EPI_ARGMAX, 64>();                     // k-means assignment
-    default: return GemmKernel{nullptr, 0, 0};
-  }
-}
-// `epi`: EPI_OUT for the gradient GEMM (A = split gradient weights, B = split transposed features), else a similarity epilogue
-static GemmKernel gemm_kernel(int prec, int epi) {
-  return with_prec(prec, [epi](auto P) {
-    constexpr SplitFormat f = SPLIT_FORMATS[P];
-    return epi != EPI_OUT ? sim_gemm_t<f.bf16>(epi) : gemm_t<f.pieces, f.bf16, EPI_OUT, bk_of(P, EPI_OUT)>();
-  });
-}
-// `sm`: fp32 tensor map of the similarity matrix for EPI_STORE_S's TMA stores (ignored otherwise: pass any valid map)
-static cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
-  const GemmKernel k = gemm_kernel(prec, epi);
-  if (!k.fn) return cudaErrorInvalidValue;
-  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(a, b, sm, p);
-  count_launch();
-  return cudaGetLastError();
-}
-
-static FusedKernel fused_kernel(int prec) {
-  return with_prec(prec, [](auto P) {
-    constexpr SplitFormat f = SPLIT_FORMATS[P];
-    return FusedKernel{fused_grad_kernel<f.pieces, f.bf16>, FusedCfg<f.pieces>::THREADS, FusedCfg<f.pieces>::SMEM_BYTES};
-  });
-}
-static cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
-  const FusedKernel k = fused_kernel(prec);
-  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(b, sm, p);
-  count_launch();
-  return cudaGetLastError();
-}
-
-// SIMT cross-check of the same contraction on the same split operands (tests only; NPAIR_GEMM_SIMT_CHECK).
-template <int PREC>
-__device__ __forceinline__ float piece_sum(const uint16_t* base, long long off, long long ps) {
-  if (PREC == PREC_BF16) return __bfloat162float(__ushort_as_bfloat16(base[off]));
-  if (PREC == PREC_FP16X2) return __half2float(__ushort_as_half(base[off])) + __half2float(__ushort_as_half(base[ps + off]));
-  return __bfloat162float(__ushort_as_bfloat16(base[off])) + __bfloat162float(__ushort_as_bfloat16(base[ps + off])) +
-         __bfloat162float(__ushort_as_bfloat16(base[2 * ps + off]));
-}
-// OUT = 1: the gradient GEMM's EPI_OUT epilogue; OUT = 0: the similarity store
-template <int PREC, int OUT>
-__global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restrict__ A, long long lda, long long psA,
-                                                        const uint16_t* __restrict__ B, long long ldb, long long psB, int K, GemmParams p) {
-  __shared__ float As[16][65], Bs[16][65];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-  float acc[4][4] = {};
-  for (int k0 = 0; k0 < K; k0 += 16) {
-    for (int e = threadIdx.x; e < 64 * 16; e += 256) {
-      const int r = e >> 4, kk = e & 15;
-      const int gm = m0 + r, gn = n0 + r, gk = k0 + kk;
-      As[kk][r] = (gm < p.M && gk < K) ? piece_sum<PREC>(A, static_cast<long long>(gm) * lda + gk, psA) : 0.f;
-      Bs[kk][r] = (gn < p.Nn && gk < K) ? piece_sum<PREC>(B, static_cast<long long>(gn) * ldb + gk, psB) : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < 16; ++kk) {
-      float a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { a[i] = As[kk][ty * 4 + i]; b[i] = Bs[kk][tx * 4 + i]; }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  const float inv = p.dev_scale ? *p.dev_scale : 1.f;
-  for (int i = 0; i < 4; ++i) {
-    const int row = m0 + ty * 4 + i;
-    if (row >= p.M) continue;
-    for (int j = 0; j < 4; ++j) {
-      const int col = n0 + tx * 4 + j;
-      if (col >= p.Nn) continue;
-      if (!OUT) p.S[static_cast<long long>(row) * p.ldS + col] = acc[i][j] * inv * inv;
-      else {
-        float* d = p.out + static_cast<long long>(row) * p.ldo + col;
-        float o = p.alpha * inv * acc[i][j];
-        if (p.beta != 0.f) o += p.beta * *d;
-        *d = o;
-      }
-    }
-  }
-}
-// `epi`: EPI_OUT, or EPI_STORE_S for the similarity matrix
-static cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long long lda, long long psA, const uint16_t* B, long long ldb,
-                                    long long psB, int K, const GemmParams& p, cudaStream_t st) {
-  dim3 grid((p.Nn + 63) / 64, (p.M + 63) / 64);
-  with_prec(prec, [&](auto P) {
-    auto kernel = epi == EPI_OUT ? simt_gemm_kernel<P, 1> : simt_gemm_kernel<P, 0>;
-    kernel<<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);
-  });
-  count_launch();
-  return cudaGetLastError();
 }
 
 // ---- peer-memory exchange (world > 1, one process per GPU, NVLink / NVSwitch) ----
@@ -337,55 +195,6 @@ __global__ void p2p_wait_kernel(const uint32_t* __restrict__ flags /*[world]*/, 
   }
 }
 
-// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K).  Slice s starts at part + s*n: 16-byte loads and
-// stores only when every slice and `out` start 16-byte aligned (n % 4 == 0), otherwise one float at a time -- the same sums either way.
-__global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, long long n, float* __restrict__ out, float beta) {
-  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x, nth = static_cast<long long>(gridDim.x) * blockDim.x;
-  const bool vec = (n & 3) == 0 && ((reinterpret_cast<uintptr_t>(part) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-  if (vec) {
-    for (long long i = t0 * 4; i < n; i += nth * 4) {
-      float4 a = *reinterpret_cast<const float4*>(part + i);
-      for (int s = 1; s < splits; ++s) { const float4 b = *reinterpret_cast<const float4*>(part + s * n + i); a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-      if (beta != 0.f) { const float4 o = *reinterpret_cast<const float4*>(out + i); a.x += beta * o.x; a.y += beta * o.y; a.z += beta * o.z; a.w += beta * o.w; }
-      *reinterpret_cast<float4*>(out + i) = a;
-    }
-  } else {
-    for (long long i = t0; i < n; i += nth) {
-      float a = part[i];
-      for (int s = 1; s < splits; ++s) a += part[s * n + i];
-      if (beta != 0.f) a += beta * out[i];
-      out[i] = a;
-    }
-  }
-}
-// Split-K of a gradient GEMM: when its output has too few tiles to fill the SMs (strong scaling: Q = B/world shrinks), the K range
-// is cut into at most 16 slices of at least min_kb K blocks each; splitk_reduce_kernel sums the slices' partial products.
-struct SplitK { int splits, kb_per_split; };
-static SplitK split_k(int num_kblocks, int tiles, int sms, int min_kb) {
-  int splits = sms / (tiles > 0 ? tiles : 1);
-  if (splits > 16) splits = 16;
-  if (splits > num_kblocks / min_kb) splits = num_kblocks / min_kb;
-  if (splits < 1) splits = 1;
-  const int kpb = (num_kblocks + splits - 1) / splits;
-  return SplitK{(num_kblocks + kpb - 1) / kpb, kpb};                    // no empty split
-}
-
-// The tile schedule of either GEMM kernel over a rows x cols output and num_kblocks K blocks, split-K `sk` (default: none)
-using TileShape = GemmCfg<1, 64, EPI_OUT>;
-static_assert(TileShape::BM == FusedCfg<1>::BM && TileShape::BN == FusedCfg<1>::BN, "both GEMM kernels share one tile shape");
-static TileSched tile_sched(int rows, int cols, int num_kblocks, SplitK sk) {
-  return TileSched{num_kblocks, (rows + TileShape::BM - 1) / TileShape::BM, (cols + TileShape::BN - 1) / TileShape::BN, nullptr, 0, sk.splits, sk.kb_per_split};
-}
-static TileSched tile_sched(int rows, int cols, int num_kblocks) { return tile_sched(rows, cols, num_kblocks, SplitK{1, num_kblocks}); }
-
-// blocks of 256 threads for `work` items: at least one, at most max_blocks
-static inline int grid_for(long long work, int max_blocks) {
-  const long long nb = (work + 255) / 256;
-  return static_cast<int>(nb < 1 ? 1 : (nb > max_blocks ? max_blocks : nb));
-}
-
-static inline long long round_up(long long v, long long m) { return (v + m - 1) / m * m; }
-
 }  // namespace npair
 
 using namespace npair;
@@ -420,39 +229,6 @@ static_assert(NPAIR_XCH_FLOATS % 2 == 0, "XCH slots hold 64-bit fields");
 // Index of the flag `rank` raises after an exchange of `kind` into the buffers of parity `par`; rank 0's starts the world's flags
 enum { XCHG_FEATURES, XCHG_RECORDS, XCHG_SMALL };
 static inline int xchg_flag(int kind, int par, int world, int rank) { return (2 * kind + par) * world + rank; }
-
-// world == 1: S = X X^T is symmetric, so the similarity GEMM computes only the tiles (m_blk, n_blk) whose 256 columns reach the
-// 128-row block's diagonal or beyond
-static std::vector<int2> sym_tile_list(int Q, int N) {
-  std::vector<int2> tl;
-  const TileSched ts = tile_sched(Q, N, 0);
-  for (int mb = 0; mb < ts.tiles_m; ++mb)
-    for (int nb = mb / 2; nb < ts.tiles_n; ++nb) tl.push_back(make_int2(mb, nb));
-  return tl;
-}
-// sym_tile_list(Q, N).size()
-static long long sym_tile_count(int Q, int N) {
-  const TileSched ts = tile_sched(Q, N, 0);
-  long long n = 0;
-  for (int mb = 0; mb < ts.tiles_m; ++mb) n += mb / 2 < ts.tiles_n ? ts.tiles_n - mb / 2 : 0;
-  return n;
-}
-
-// A sweep of the similarity GEMM over rows x cols of the K-concatenated operands of K extent kcat (make_tmap_kcat): 128 x 256 tiles
-// of 64-element K blocks, no split-K, the accumulators scaled by the square of *inv_scale; under EPI_SYM only the tiles of
-// `sym_tiles`, and under EPI_STATS the per-row statistics of `ra`
-static GemmParams sim_sweep(int epi, int rows, int cols, long long kcat, const float* inv_scale, const int2* sym_tiles, int n_sym_tiles,
-                            const RowArrays& ra) {
-  GemmParams gp; memset(&gp, 0, sizeof(gp));
-  gp.M = rows; gp.Nn = cols;
-  gp.ts = tile_sched(rows, cols, static_cast<int>(kcat / 64));
-  gp.dev_scale = inv_scale;
-  if (epi & EPI_SYM) { gp.ts.tile_list = sym_tiles; gp.ts.num_tiles_list = n_sym_tiles; }
-  if (epi & EPI_STATS) {
-    gp.st_minw = ra.st_minw; gp.st_maxw = ra.st_maxw; gp.st_maxb = ra.st_maxb; gp.st_maxall = ra.st_maxall; gp.cnt_same = ra.cnt_same;
-  }
-  return gp;
-}
 
 // Row-block similarity mode (NPAIR_SIM_BLOCK_ROWS): the block height in rows, a multiple of 128; 0 when the mode is off or the
 // height reaches Q (the materialised path)
@@ -533,81 +309,6 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
 }
 
 // ------------------------------------------------------------------------------------------------ device memory
-// Bump carver of a buffer cut into several arrays: take<T>(count, align) returns the next `count` T at an `align`-byte offset.  Over a
-// null base it only measures, so the one function that cuts a region also gives its size (`bytes` after the last take).
-struct Carve {
-  char* base;
-  size_t bytes = 0;
-  template <class T>
-  T* take(long long count, size_t align = alignof(T)) {
-    bytes = (bytes + align - 1) / align * align;
-    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
-    bytes += sizeof(T) * count;
-    return p;
-  }
-};
-
-// The device buffers of a context or an evaluator, listed once each (ctx_buffers, eval_buffers) and run through one of two modes.
-// Sizing only adds up their bytes.  Allocating gives every buffer a cudaMalloc of its own, zero-filled when asked, and frees them
-// all in release() or the destructor.  After a failure own() does nothing more: the list runs to its end and `err` holds the first.
-struct DevMem {
-  explicit DevMem(bool allocate = true) : allocate(allocate) {}
-  DevMem(const DevMem&) = delete;
-  ~DevMem() { release(); }
-  // *p = a buffer of `n` bytes (null if its cudaMalloc fails); 0 bytes: none
-  template <class T>
-  void own(T** p, size_t n, bool zero) {
-    if (n == 0 || err != cudaSuccess) return;
-    bytes += n;
-    if (!allocate) return;
-    if ((err = cudaMalloc(p, n)) != cudaSuccess) { *p = nullptr; return; }
-    held.push_back(*p);
-    if (zero) err = cudaMemset(*p, 0, n);
-  }
-  // One buffer for a region that `carve(Carve&)` cuts into arrays: carved over a null base to measure it, then over the buffer
-  template <class F>
-  void own_carved(bool zero, F carve) {
-    Carve size{nullptr}, cut{nullptr};
-    carve(size);
-    own(&cut.base, size.bytes, zero);
-    carve(cut);
-  }
-  void release() {
-    for (void* q : held) cudaFree(q);
-    held.clear(); bytes = 0; err = cudaSuccess;
-  }
-  const bool allocate;
-  size_t bytes = 0;                   // of the buffers listed (and held) so far
-  cudaError_t err = cudaSuccess;
-  std::vector<void*> held;
-};
-
-// The order of a context's (or an evaluator's) calls across the caller's streams.  Every call that enqueues work records `done` on its
-// stream behind that work, and a call on another stream first makes its stream wait for `done`: the scratch buffers are the object's
-// own, so the caller cannot order around them.  Calls on the stream of the previous call enqueue nothing extra beyond the record.
-struct StreamOrder {
-  StreamOrder() = default;
-  StreamOrder(const StreamOrder&) = delete;
-  ~StreamOrder() { if (done) cudaEventDestroy(done); }
-  cudaError_t create() { return cudaEventCreateWithFlags(&done, cudaEventDisableTiming); }
-  // Records `done` behind the current call's work on `st`, once per call: a call that waits on the host for its results (the
-  // forward's tops) marks before it waits, the others when they return
-  void mark(cudaStream_t st) {
-    if (!open) return;
-    open = false;
-    if (cudaEventRecord(done, st) == cudaSuccess) { stream = st; recorded = true; }
-  }
-  cudaEvent_t done = nullptr;
-  cudaStream_t stream = nullptr;      // the stream `done` was last recorded on
-  bool recorded = false;
-  bool open = false;                  // a call has entered and not yet marked
-};
-
-// The statistics of RowArrays, which the evaluator's queries have too: four ordered-uint statistics and the same-label count per row
-static void carve_stats(Carve& cv, long long rows, RowArrays* ra) {
-  ra->st_minw = cv.take<uint32_t>(rows); ra->st_maxw = cv.take<uint32_t>(rows); ra->st_maxb = cv.take<uint32_t>(rows);
-  ra->st_maxall = cv.take<uint32_t>(rows); ra->cnt_same = cv.take<int>(rows);
-}
 // A context's RowArrays: the statistics, thresholds, row results and [3][Q] hit flags, then the row records 32-byte aligned
 static void carve_rows(Carve& cv, long long Q, RowArrays* ra) {
   carve_stats(cv, Q, ra);
@@ -715,47 +416,7 @@ struct PhaseTimer {
   }
 };
 
-#define CUDA_TRY(ctx, call)                                                                              \
-  do {                                                                                                   \
-    cudaError_t e__ = (call);                                                                            \
-    if (e__ != cudaSuccess) {                                                                            \
-      (ctx)->err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);      \
-      return NPAIR_E_CUDA;                                                                               \
-    }                                                                                                    \
-  } while (0)
-// The same while a context or an evaluator is created, before it exists for npair_last_error, and in calls that have neither: the
-// message goes to g_create_err.  An object under construction is held by a unique_ptr, which releases it on the early return.
-#define CREATE_TRY(call)                                                                                 \
-  do {                                                                                                   \
-    cudaError_t e__ = (call);                                                                            \
-    if (e__ != cudaSuccess) {                                                                            \
-      g_create_err = fmt("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__);    \
-      return NPAIR_E_CUDA;                                                                               \
-    }                                                                                                    \
-  } while (0)
-
-// The frame of every C ABI call that enqueues work for a context or an evaluator (`Obj`), on the caller's stream: enter() makes the
-// object's device current and waits for the previous call when that ran on another stream (StreamOrder), failures going to the object's
-// `err`.  `done` is recorded at the latest when the call returns, also after an error (what it enqueued before failing is still
-// running).  A call refused before enter() enqueues nothing and records nothing.
-template <class Obj>
-struct OrderedCall {
-  OrderedCall(Obj* obj_, void* stream) : obj(obj_), st(static_cast<cudaStream_t>(stream)) {}
-  OrderedCall(const OrderedCall&) = delete;
-  int enter() {
-    StreamOrder& o = obj->order;
-    CUDA_TRY(obj, cudaSetDevice(obj->device));
-    if (o.recorded && o.stream != st) CUDA_TRY(obj, cudaStreamWaitEvent(st, o.done, 0));
-    o.open = true;
-    return NPAIR_OK;
-  }
-  ~OrderedCall() { obj->order.mark(st); }
-  Obj* const obj;
-  const cudaStream_t st;
-};
-
-// Makes `device` (< 0: the current one) current for a new context or evaluator, which needs an sm_90 device; its id and SM count
-static int open_device(int device, int* dev, int* sms) {
+int npair::open_device(int device, int* dev, int* sms) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) {
     g_create_err = "no CUDA device: libnpair_b200 has no CPU fallback (the oracle under oracle/ is test-only)";
@@ -1647,378 +1308,6 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
     CREATE_TRY(launch_simt_gemm(precision, EPI_OUT, As, Kp, static_cast<long long>(M) * Kp, Bs, Kp, static_cast<long long>(Nn) * Kp, K, gp, st));
   }
   CREATE_TRY(cudaStreamSynchronize(st));
-  return NPAIR_OK;
-}
-
-}  // extern "C"
-
-// ------------------------------------------------------------------------------------------------ retrieval evaluation (DESIGN 8)
-// Not part of the reference layer.  Queries go to the A format and gallery rows to the B format of the K-concatenated operands, so the
-// similarity GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
-static constexpr int EVAL_NO_SELF = -(1 << 30); // a self offset that matches no column (rows and columns stay below 2^30)
-
-struct EvalPlan {
-  int max_q, max_g, D, prec;
-  long long Dp, kcat;           // padded feature extent, K extent of the concatenated operands (mma_passes * Dp)
-  int n_sym_tiles;              // tile-list capacity: self-retrieval over min(max_q, max_g) rows
-};
-
-static int eval_validate(long long max_q, long long max_g, long long D, int prec, std::string* err) {
-  if (max_q < 1 || max_g < 1 || D < 1) { *err = "max_queries, max_gallery and D must be >= 1"; return NPAIR_E_ARG; }
-  if (max_q >= (1 << 30) || max_g >= (1 << 30) || D >= (1 << 24)) { *err = "max_queries and max_gallery must be < 2^30, D < 2^24"; return NPAIR_E_ARG; }
-  if (prec < 0 || prec > 2) { *err = "bad precision"; return NPAIR_E_ARG; }
-  return NPAIR_OK;
-}
-
-static EvalPlan eval_plan_of(int max_q, int max_g, int D, int prec) {
-  EvalPlan p{};
-  p.max_q = max_q; p.max_g = max_g; p.D = D; p.prec = prec;
-  p.Dp = round_up(D, 64);
-  p.kcat = mma_passes(SPLIT_FORMATS[prec].pieces) * p.Dp;
-  const int n = max_q < max_g ? max_q : max_g;
-  p.n_sym_tiles = static_cast<int>(sym_tile_count(n, n));
-  return p;
-}
-
-struct npair_eval : EvalPlan {
-  int device = -1, sms = 0;
-  DevMem mem;                     // the workspace (eval_buffers)
-  uint16_t *catA = nullptr, *catB = nullptr;
-  RowArrays ra{};                 // only the statistics (carve_stats)
-  unsigned int* absmax_bits = nullptr;
-  BlockScalars* bs = nullptr;
-  int2* sym_tiles = nullptr;
-  int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
-  std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
-  // MAP@R (MapRows, MapPairs) and k-means (KmeansBufs) buffers, grown on demand and kept
-  DevMem map_rows_mem, map_pairs_mem, km_mem;
-  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr;
-  StreamOrder order;              // the calls' order across streams
-  std::string err;
-};
-
-// The evaluator's workspace, each buffer with its size and zero-fill; returns the first failure
-static cudaError_t eval_buffers(npair_eval* ev, DevMem& m) {
-  m.own(&ev->catA, 2ull * ev->max_q * ev->kcat, false);
-  m.own(&ev->catB, 2ull * ev->max_g * ev->kcat, false);
-  m.own_carved(true, [ev](Carve& cv) { carve_stats(cv, ev->max_q, &ev->ra); ev->absmax_bits = cv.take<unsigned int>(1); });
-  m.own(&ev->bs, sizeof(BlockScalars), true);
-  m.own(&ev->sym_tiles, sizeof(int2) * ev->n_sym_tiles, false);
-  return m.err;
-}
-
-// The device memory of npair_eval_map_at_r and npair_eval_kmeans beyond the workspace.  Each constructor carves one buffer at `base`;
-// over a null base it only measures it.  MAP@R takes two buffers: per query the nq + 1 segment offsets, the {sum R, error bits} word
-// pair and the gather counters; per positive pair the value and the histogram word.
-struct MapRows : Carve {
-  long long* seg; unsigned long long* sum_err; int* fill;
-  MapRows(char* base, long long nq) : Carve{base} { seg = take<long long>(nq + 1); sum_err = take<unsigned long long>(2); fill = take<int>(nq); }
-};
-struct MapPairs : Carve {
-  float* pos; unsigned int* hist;
-  MapPairs(char* base, long long sum_r) : Carve{base} { pos = take<float>(sum_r); hist = take<unsigned int>(sum_r); }
-};
-// k-means takes one: the int64 sums of the members' features, the EPI_ARGMAX keys, the inertia partials, then per cluster its member
-// count, its bias 0.5 ||mu||^2 and its initial row, and the KmeansWords.
-struct KmeansBufs : Carve {
-  long long* sums; unsigned long long* keys; double* partial; int* counts; float* bias; int* rows; KmeansWords* words;
-  KmeansBufs(char* base, long long n, long long k, long long D) : Carve{base} {
-    sums = take<long long>(k * D); keys = take<unsigned long long>(n); partial = take<double>(KM_INERTIA_BLOCKS);
-    counts = take<int>(k); bias = take<float>(k); rows = take<int>(k); words = take<KmeansWords>(1);
-  }
-};
-
-// Grows the buffer `m` holds at *base to at least `bytes` (cudaFree of the old one waits for the device); `what` names it in errors
-static int eval_grow(npair_eval* ev, DevMem& m, char** base, size_t bytes, const char* what) {
-  if (bytes <= m.bytes) return NPAIR_OK;
-  m.release();
-  m.own(base, bytes, false);
-  if (m.err == cudaSuccess) return NPAIR_OK;
-  cudaGetLastError();
-  m.release();
-  ev->err = fmt("cannot allocate %zu bytes for %s", bytes, what);
-  return NPAIR_E_CUDA;
-}
-
-extern "C" {
-
-size_t npair_eval_workspace_bytes(int32_t max_q, int32_t max_g, int32_t D, int32_t prec) {
-  std::string e;
-  if (eval_validate(max_q, max_g, D, prec, &e) != NPAIR_OK) return 0;
-  npair_eval ev;
-  static_cast<EvalPlan&>(ev) = eval_plan_of(max_q, max_g, D, prec);
-  DevMem sizing(false);
-  eval_buffers(&ev, sizing);
-  return sizing.bytes;
-}
-
-size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r) {
-  if (nq < 1 || sum_r < 0) return 0;
-  return MapRows(nullptr, nq).bytes + MapPairs(nullptr, sum_r).bytes;
-}
-
-size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
-  if (n < 1 || k < 1 || D < 1 || k > n) return 0;
-  return KmeansBufs(nullptr, n, k, D).bytes;
-}
-
-const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
-
-void npair_eval_destroy(npair_eval* ev) {
-  if (!ev) return;
-  if (ev->device >= 0) cudaSetDevice(ev->device);
-  delete ev;                      // its DevMems free its buffers on this device
-}
-
-int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int32_t device, npair_eval** out) {
-  if (!out) { g_create_err = "null out"; return NPAIR_E_ARG; }
-  *out = nullptr;
-  int rc = eval_validate(max_q, max_g, D, prec, &g_create_err);
-  if (rc != NPAIR_OK) return rc;
-  int dev = -1, sms = 0;
-  if ((rc = open_device(device, &dev, &sms)) != NPAIR_OK) return rc;
-  std::unique_ptr<npair_eval, void (*)(npair_eval*)> made(new npair_eval(), npair_eval_destroy);   // until it is handed out
-  npair_eval* ev = made.get();
-  static_cast<EvalPlan&>(*ev) = eval_plan_of(max_q, max_g, D, prec);
-  ev->device = dev; ev->sms = sms;
-  CREATE_TRY(eval_buffers(ev, ev->mem));
-  CREATE_TRY(ev->order.create());
-  const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
-                      EPI_BUCKET | EPI_SYM, EPI_ARGMAX};
-  for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
-  *out = made.release();
-  return NPAIR_OK;
-}
-
-}  // extern "C"
-
-// Arguments shared by the three calls.  self_offset is global, the shard holds gallery rows [gallery_row0, gallery_row0 + ng).
-static int eval_check(npair_eval* ev, const float* q, int nq, const float* g, int ng, int self_offset, int gallery_row0, float absmax,
-                      bool whole_gallery) {
-  if (!q || !g) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  if (nq < 1 || ng < 1) { ev->err = "nq and ng must be >= 1"; return NPAIR_E_ARG; }
-  if (nq > ev->max_q || ng > ev->max_g) { ev->err = fmt("nq = %d, ng = %d exceed the evaluator's capacity (%d, %d)", nq, ng, ev->max_q, ev->max_g); return NPAIR_E_ARG; }
-  if (self_offset < -1) { ev->err = "self_offset must be -1 (disjoint sets) or >= 0"; return NPAIR_E_ARG; }
-  if (whole_gallery && self_offset >= 0 && static_cast<long long>(self_offset) + nq > ng) { ev->err = "self_offset + nq exceeds ng"; return NPAIR_E_ARG; }
-  if (gallery_row0 < 0) { ev->err = "gallery_row0 must be >= 0"; return NPAIR_E_ARG; }
-  if (!(absmax >= 0.f) && !whole_gallery) { ev->err = "absmax must be max|x| over the queries and the whole gallery (>= 0)"; return NPAIR_E_ARG; }
-  if (!std::isfinite(absmax) && !whole_gallery) { ev->err = "absmax must be finite"; return NPAIR_E_ARG; }
-  return NPAIR_OK;
-}
-
-// Self column of query 0 inside the shard (EVAL_NO_SELF: none), and whether the sweeps use the symmetric tile list: the query set is
-// the whole gallery shard, as one buffer, with every query its own row
-static int eval_self_col(int self_offset, int gallery_row0) { return self_offset < 0 ? EVAL_NO_SELF : self_offset - gallery_row0; }
-static bool eval_sym(const float* q, int nq, const float* g, int ng, int self_col) { return q == g && nq == ng && self_col == 0; }
-
-// Operand preparation: the statistics reset, the pre-scale (from max|x| over both sets unless the caller gives it) and both operands
-static int eval_prepare(npair_eval* ev, const float* q, int nq, const float* g, int ng, float absmax, bool sym, cudaStream_t st) {
-  const long long D = ev->D;
-  unsigned int* amx = nullptr;
-  if (absmax < 0.f && ev->prec == PREC_FP16X2) {
-    amx = ev->absmax_bits;
-    CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
-  }
-  launch_eval_prep(q, nq * D, sym ? nullptr : g, ng * D, amx, ev->ra, nq, ev->sms, st);
-  launch_eval_split(q, nq, ev->D, ev->Dp, ev->prec, 0, absmax, amx, ev->bs, ev->catA, st);
-  launch_eval_split(g, ng, ev->D, ev->Dp, ev->prec, 1, absmax, amx, ev->bs, ev->catB, st);
-  CUDA_TRY(ev, cudaGetLastError());
-  return NPAIR_OK;
-}
-
-// One sweep of the similarity GEMM over the prepared operands: EPI_STATS, EPI_GATHER or EPI_BUCKET (labels, and `map` for the MAP@R
-// sweeps), EPI_COUNT (cut, count) or EPI_ARGMAX (`map`'s col_bias and best), + EPI_SYM when `sym`
-static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, const float* ql, const float* gl, const float* cut, int32_t* count,
-                      bool sym, cudaStream_t st, const GemmParams* map = nullptr) {
-  if (sym) {
-    if (ev->sym_n != nq) {
-      ev->sym_host = sym_tile_list(nq, nq);
-      CUDA_TRY(ev, cudaMemcpyAsync(ev->sym_tiles, ev->sym_host.data(), sizeof(int2) * ev->sym_host.size(), cudaMemcpyHostToDevice, st));
-      ev->sym_n = nq;
-    }
-    epi |= EPI_SYM;
-  }
-  GemmParams gp = sim_sweep(epi, nq, ng, ev->kcat, &ev->bs->x_inv_scale, ev->sym_tiles, static_cast<int>(ev->sym_host.size()), ev->ra);
-  gp.self_offset = self_col;
-  if (epi & (EPI_STATS | EPI_GATHER | EPI_BUCKET)) { gp.lab_rows = ql; gp.lab_cols = gl; }
-  else { gp.cut = cut; gp.count = count; }
-  if (map) {
-    gp.cnt_same = ev->ra.cnt_same; gp.bs = ev->bs; gp.seg = map->seg; gp.fill = map->fill; gp.pos = map->pos; gp.hist = map->hist;
-    gp.col_bias = map->col_bias; gp.best = map->best;
-  }
-  CUtensorMap ta, tb;
-  std::string te;
-  if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
-  CUDA_TRY(ev, launch_gemm(ev->prec, epi, ta, tb, ta, gp, ev->sms, st));
-  return NPAIR_OK;
-}
-
-extern "C" {
-
-int npair_eval_rank(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng, int32_t self_offset,
-                    int32_t* d_rank, void* stream) {
-  if (!ev) return NPAIR_E_ARG;
-  int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
-  if (rc != NPAIR_OK) return rc;
-  if (!ql || !gl || !d_rank) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  OrderedCall call(ev, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  const cudaStream_t st = call.st;
-  const int self_col = eval_self_col(self_offset, 0);
-  const bool sym = eval_sym(q, nq, g, ng, self_col);
-  float* cut = reinterpret_cast<float*>(ev->ra.st_minw);   // p* overwrites a statistic sweep 2 does not read
-  if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
-  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_best(ev->ra, nq, cut, st);
-  CUDA_TRY(ev, cudaMemsetAsync(d_rank, 0, sizeof(int32_t) * nq, st));
-  if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, cut, d_rank, sym, st)) != NPAIR_OK) return rc;
-  CUDA_TRY(ev, cudaGetLastError());
-  return NPAIR_OK;
-}
-
-int npair_eval_best_positive(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng,
-                             int32_t self_offset, int32_t gallery_row0, float absmax, float* d_best, void* stream) {
-  if (!ev) return NPAIR_E_ARG;
-  int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
-  if (rc != NPAIR_OK) return rc;
-  if (!ql || !gl || !d_best) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  OrderedCall call(ev, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  const cudaStream_t st = call.st;
-  const int self_col = eval_self_col(self_offset, gallery_row0);
-  const bool sym = eval_sym(q, nq, g, ng, self_col);
-  if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
-  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_best(ev->ra, nq, d_best, st);
-  CUDA_TRY(ev, cudaGetLastError());
-  return NPAIR_OK;
-}
-
-int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g, int32_t ng, int32_t self_offset, int32_t gallery_row0,
-                     float absmax, const float* d_cut, int32_t* d_count, void* stream) {
-  if (!ev) return NPAIR_E_ARG;
-  int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax, false);
-  if (rc != NPAIR_OK) return rc;
-  if (!d_cut || !d_count) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  OrderedCall call(ev, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  const cudaStream_t st = call.st;
-  const int self_col = eval_self_col(self_offset, gallery_row0);
-  const bool sym = eval_sym(q, nq, g, ng, self_col);
-  if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
-  CUDA_TRY(ev, cudaMemsetAsync(d_count, 0, sizeof(int32_t) * nq, st));
-  if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, d_cut, d_count, sym, st)) != NPAIR_OK) return rc;
-  CUDA_TRY(ev, cudaGetLastError());
-  return NPAIR_OK;
-}
-
-// MAP@R in three sweeps over the same prepared operands and tile geometry (DESIGN 8): the statistics sweep gives R_i, EPI_GATHER
-// collects every query's positives into its segment, a sort orders each segment, and EPI_BUCKET places every negative that reaches the
-// query's smallest positive among them.  The gather writes its unordered positives into the histogram words, which the sort reads and
-// which are then cleared for the bucket sweep: 8 bytes per positive pair in all.
-int npair_eval_map_at_r(npair_eval* ev, const float* q, const float* ql, int32_t nq, const float* g, const float* gl, int32_t ng,
-                        int32_t self_offset, double* d_map_r, double* d_r_precision, int32_t* d_R, int32_t* d_rank, void* stream) {
-  if (!ev) return NPAIR_E_ARG;
-  int rc = eval_check(ev, q, nq, g, ng, self_offset, 0, -1.f, true);
-  if (rc != NPAIR_OK) return rc;
-  if (!ql || !gl || !d_map_r || !d_r_precision) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  OrderedCall call(ev, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  const cudaStream_t st = call.st;
-  const int self_col = eval_self_col(self_offset, 0);
-  const bool sym = eval_sym(q, nq, g, ng, self_col);
-  if ((rc = eval_grow(ev, ev->map_rows_mem, &ev->map_rows, MapRows(nullptr, nq).bytes, "the MAP@R per-query offsets")) != NPAIR_OK) return rc;
-  const MapRows rows(ev->map_rows, nq);
-  const int* R = ev->ra.cnt_same;
-  // sweep 1: R_i, and the one host synchronisation, for sum R_i
-  if ((rc = eval_prepare(ev, q, nq, g, ng, -1.f, sym, st)) != NPAIR_OK) return rc;
-  if ((rc = eval_sweep(ev, EPI_STATS, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st)) != NPAIR_OK) return rc;
-  launch_eval_seg_scan(R, nq, rows.seg, ev->bs, rows.sum_err, st);
-  unsigned long long h[2] = {0, 0};
-  CUDA_TRY(ev, cudaMemcpyAsync(h, rows.sum_err, sizeof(h), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(ev, cudaStreamSynchronize(st));
-  if (h[1] & DERR_GATHER_SLOT) {
-    ev->err = "an earlier npair_eval_map_at_r on this evaluator gathered more positives for a query than its statistics sweep counted "
-              "(that query's results were NaN)";
-    return NPAIR_E_CUDA;
-  }
-  const long long sum_r = static_cast<long long>(h[0]);
-  if ((rc = eval_grow(ev, ev->map_pairs_mem, &ev->map_pairs, MapPairs(nullptr, sum_r).bytes, "the MAP@R positive pairs")) != NPAIR_OK) return rc;
-  const MapPairs pairs(ev->map_pairs, sum_r);
-  CUDA_TRY(ev, cudaMemsetAsync(rows.fill, 0, sizeof(int) * nq, st));
-  if (sum_r > 0) {
-    GemmParams mp{};
-    // sweep 2: the positives, unordered, into the histogram words; then sorted into pos
-    mp.seg = rows.seg; mp.fill = rows.fill; mp.pos = reinterpret_cast<float*>(pairs.hist);
-    if ((rc = eval_sweep(ev, EPI_GATHER, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
-    launch_eval_seg_sort(R, rows.seg, nq, reinterpret_cast<const float*>(pairs.hist), pairs.pos, st);
-    CUDA_TRY(ev, cudaMemsetAsync(pairs.hist, 0, sizeof(unsigned int) * sum_r, st));
-    // sweep 3: the buckets
-    mp.pos = pairs.pos; mp.hist = pairs.hist;
-    if ((rc = eval_sweep(ev, EPI_BUCKET, nq, ng, self_col, ql, gl, nullptr, nullptr, sym, st, &mp)) != NPAIR_OK) return rc;
-  }
-  launch_eval_map_finish(R, rows.seg, rows.fill, pairs.pos, pairs.hist, nq, d_map_r, d_r_precision, d_R, d_rank, st);
-  CUDA_TRY(ev, cudaGetLastError());
-  return NPAIR_OK;
-}
-
-// Lloyd's k-means on the evaluator's operands (DESIGN 8.2): the points are split once into the A format, with the pre-scale sigma of
-// max|x|, which also bounds every centroid (a mean lies in its members' convex hull); each iteration splits the centroids into the B
-// format with the same sigma, sweeps EPI_ARGMAX against their biases 0.5 ||mu||^2, decodes the keys while adding the members'
-// fixed-point features into int64 sums, reads back {changed, err} and, unless it stops, replaces each non-empty centroid by its mean.
-int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, const int32_t* init_rows, int32_t max_iter, float* d_centroids,
-                      int32_t* d_assign, double* d_inertia, int32_t stats[3], void* stream) {
-  if (!ev) return NPAIR_E_ARG;
-  if (!x || !init_rows || !d_centroids || !d_assign || !stats) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
-  if (n < 1 || k < 1 || k > n) { ev->err = fmt("k-means needs 1 <= k <= n (n = %d, k = %d)", n, k); return NPAIR_E_ARG; }
-  if (n > ev->max_q || k > ev->max_g) {
-    ev->err = fmt("n = %d points, k = %d centroids exceed the evaluator's capacity (%d, %d)", n, k, ev->max_q, ev->max_g);
-    return NPAIR_E_ARG;
-  }
-  if (max_iter < 1) { ev->err = "max_iter must be >= 1"; return NPAIR_E_ARG; }
-  for (int c = 0; c < k; ++c)
-    if (init_rows[c] < 0 || init_rows[c] >= n) { ev->err = fmt("init_rows[%d] = %d is not a row of x", c, init_rows[c]); return NPAIR_E_ARG; }
-  int rc;
-  OrderedCall call(ev, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  const cudaStream_t st = call.st;
-  if ((rc = eval_grow(ev, ev->km_mem, &ev->km, KmeansBufs(nullptr, n, k, ev->D).bytes, "the k-means buffers")) != NPAIR_OK) return rc;
-  const long long D = ev->D;
-  const KmeansBufs km(ev->km, n, k, D);
-  unsigned int* amx = ev->absmax_bits;
-  CUDA_TRY(ev, cudaMemcpyAsync(km.rows, init_rows, sizeof(int) * k, cudaMemcpyHostToDevice, st));
-  // the points, once: max|x| in every format (the update's fixed-point scale), then the A operand
-  CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
-  launch_eval_prep(x, n * D, nullptr, 0, amx, ev->ra, 0, ev->sms, st);
-  launch_eval_split(x, n, ev->D, ev->Dp, ev->prec, 0, -1.f, amx, ev->bs, ev->catA, st);
-  launch_km_gather(x, ev->D, km.rows, k, d_centroids, st);
-  CUDA_TRY(ev, cudaMemsetAsync(d_assign, 0xFF, sizeof(int32_t) * n, st));   // -1: every point of the first sweep changes
-  CUDA_TRY(ev, cudaMemsetAsync(km.keys, 0, sizeof(unsigned long long) * n, st));
-  CUDA_TRY(ev, cudaMemsetAsync(km.sums, 0, sizeof(long long) * k * D, st));     // a call that stopped on convergence leaves them set
-  GemmParams am{};
-  am.col_bias = km.bias; am.best = km.keys;
-  KmeansWords h{};
-  int t = 0;
-  for (;; ++t) {
-    const bool last = t + 1 == max_iter;
-    launch_eval_split(d_centroids, k, ev->D, ev->Dp, ev->prec, 1, -1.f, amx, ev->bs, ev->catB, st);
-    launch_km_bias(d_centroids, k, ev->D, km.bias, km.counts, km.words, st);
-    if ((rc = eval_sweep(ev, EPI_ARGMAX, n, k, EVAL_NO_SELF, nullptr, nullptr, nullptr, nullptr, false, st, &am)) != NPAIR_OK) return rc;
-    launch_km_assign(km.keys, x, n, ev->D, amx, k, d_assign, km.counts, km.sums, !last, km.words, st);
-    CUDA_TRY(ev, cudaMemcpyAsync(&h, km.words, sizeof(h), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ev, cudaStreamSynchronize(st));
-    if (h.err & DERR_KMEANS_NO_ARGMAX) {
-      ev->err = "a point has no centroid with a finite score: x or a centroid holds NaN or infinity";
-      return NPAIR_E_CUDA;
-    }
-    if ((t > 0 && h.changed == 0) || last) break;
-    launch_km_update(km.sums, km.counts, amx, k, ev->D, d_centroids, st);
-  }
-  if (d_inertia) launch_km_inertia(x, d_centroids, d_assign, n, ev->D, km.partial, d_inertia, st);
-  CUDA_TRY(ev, cudaGetLastError());
-  stats[0] = t + 1;
-  stats[1] = static_cast<int32_t>(h.changed);
-  stats[2] = k - static_cast<int32_t>(h.nonempty);
   return NPAIR_OK;
 }
 

@@ -1,0 +1,91 @@
+// device.cuh -- device helpers that more than one kernel unit uses: the warp reductions, the operand split and its K-concatenated row
+// writer, and the reset of a row's statistics.
+#pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cfloat>
+
+#include "kernels.cuh"
+
+namespace npair {
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ int warp_sum_i(int v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ float warp_min(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// split an fp32 value into 2-byte pieces (see gemm_wgmma.cuh header)
+template <int PREC>
+__device__ __forceinline__ void split3(float v, uint16_t& p0, uint16_t& p1, uint16_t& p2) {
+  if (PREC == PREC_BF16) {
+    p0 = __bfloat16_as_ushort(__float2bfloat16_rn(v)); p1 = 0; p2 = 0;
+  } else if (PREC == PREC_FP16X2) {
+    const __half h = __float2half_rn(v);
+    const float r = v - __half2float(h);
+    p0 = __half_as_ushort(h); p1 = __half_as_ushort(__float2half_rn(r)); p2 = 0;
+  } else {
+    const __nv_bfloat16 h = __float2bfloat16_rn(v);
+    const float r1 = v - __bfloat162float(h);
+    const __nv_bfloat16 m = __float2bfloat16_rn(r1);
+    const float r2 = r1 - __bfloat162float(m);
+    p0 = __bfloat16_as_ushort(h); p1 = __bfloat16_as_ushort(m); p2 = __bfloat16_as_ushort(__float2bfloat16_rn(r2));
+  }
+}
+// Eight consecutive features v, times the pre-scale sc, as pieces: p[e][s] is piece s of feature e, pk[s] the eight pieces s packed into
+// one 16-byte group (only the format's pieces are packed)
+template <int PREC>
+__device__ __forceinline__ void split8(const float (&v)[8], float sc, uint16_t (&p)[8][3], uint4 (&pk)[3]) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split3<PREC>(v[e] * sc, p[e][0], p[e][1], p[e][2]);
+#pragma unroll
+  for (int s = 0; s < SPLIT_FORMATS[PREC].pieces; ++s)
+    pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
+                       p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
+}
+// The packed pieces pk of features [d, d + 8) into one row of the K-concatenated operands of the bitwise-symmetric similarity GEMM,
+// in the A (side_b = false) or B format; one Dp-long segment per MMA pass:
+//   bf16   : A row = B row = [ hi ]                                                                                       K_cat = Dp
+//   fp16x2 : A row = [ hi | hi(8) lo(8) ... ]                         B row = [ hi | lo(8) hi(8) ... ]                  K_cat = 3*Dp
+//   bf16x3 : A row = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B row = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]   K_cat = 6*Dp
+// ONE K=16 MMA then sums 8 products p_j*q_m and the 8 mirrored products q_j*p_m: swapping the operand roles only
+// permutes the products inside an instruction, whose sum is order-invariant (measured: tests/diag_mma_symmetry.py),
+// so S[j][m] == S[m][j] bit for bit, on one rank and across ranks.
+template <int PREC>
+__device__ __forceinline__ void store_kcat_row(uint16_t* row, long long Dp, int d, const uint4 (&pk)[3], bool side_b) {
+  *reinterpret_cast<uint4*>(row + d) = pk[0];
+  if (PREC == PREC_FP16X2) {
+    *reinterpret_cast<uint4*>(row + Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(row + Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+  } else if (PREC == PREC_BF16X3) {
+    *reinterpret_cast<uint4*>(row + Dp + d) = pk[1];
+    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d) = side_b ? pk[1] : pk[0];
+    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
+    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d) = side_b ? pk[2] : pk[0];
+    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[2];
+  }
+}
+
+// Row i's statistics before a similarity sweep accumulates into them (caffe_set of the stat blobs, .cu:230-236)
+__device__ __forceinline__ void reset_row_stats(const RowArrays& ra, long long i) {
+  ra.st_minw[i] = f2ord(FLT_MAX); ra.st_maxw[i] = f2ord(-FLT_MAX);
+  ra.st_maxb[i] = f2ord(-FLT_MAX); ra.st_maxall[i] = f2ord(-FLT_MAX);
+  ra.cnt_same[i] = 0;
+}
+
+}  // namespace npair

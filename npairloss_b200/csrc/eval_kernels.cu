@@ -1,0 +1,329 @@
+// eval_kernels.cu -- the retrieval evaluator's and k-means's kernels (DESIGN 8): operand preparation, the MAP@R segments and the
+// k-means steps around the similarity GEMM's sweeps.
+#include <cuda.h>
+#include <cfloat>
+
+#include "device.cuh"
+#include "kernels.cuh"
+
+namespace npair {
+
+// --------------------------------------------------------------------------------------------
+// retrieval evaluation (DESIGN 8; not part of the reference layer): operand preparation of two matrices and the best-positive cut
+// --------------------------------------------------------------------------------------------
+// max|x| over the queries and the gallery (g == NULL: the gallery is the query set) into *absmax_bits, which is pre-zeroed (the bits
+// of non-negative floats order like the floats; NaN is skipped by fmaxf), and the reset of the per-query statistics.
+__global__ void __launch_bounds__(256) eval_prep_kernel(const float* __restrict__ q, long long nq_el, const float* __restrict__ g, long long ng_el,
+                                                        unsigned int* absmax_bits, RowArrays ra, int nq) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (absmax_bits) {
+    float mx = 0.f;
+    for (long long i = t0; i < nq_el; i += stride) mx = fmaxf(mx, fabsf(__ldg(q + i)));
+    if (g) for (long long i = t0; i < ng_el; i += stride) mx = fmaxf(mx, fabsf(__ldg(g + i)));
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(absmax_bits, __float_as_uint(mx));
+  }
+  for (long long i = t0; i < nq; i += stride) reset_row_stats(ra, i);
+}
+void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, RowArrays ra, int nq,
+                      int sms, cudaStream_t st) {
+  const long long work = absmax_bits ? (nq_el > ng_el ? nq_el : ng_el) / 16 : nq;   // threads: ~16 elements each
+  long long nb = (work + 255) / 256;
+  nb = nb < 1 ? 1 : (nb > 8 * sms ? 8 * sms : nb);
+  eval_prep_kernel<<<static_cast<int>(nb), 256, 0, st>>>(q, nq_el, g, ng_el, absmax_bits, ra, nq);
+  count_launch();
+}
+
+// Rows of x to one side of the K-concatenated operands of the similarity GEMM (side_b = 0: the A format of the queries, 1: the B format
+// of the gallery), through the layer's store_kcat_row.  Thread = 8 features of one row.  The pre-scale is the layer's rule applied to
+// max|x| over both sets: `absmax` when the caller gives it (>= 0), else *absmax_bits.
+template <int PREC>
+__global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict__ x, int rows, int D, long long Dp, int side_b, float absmax,
+                                                         const unsigned int* __restrict__ absmax_bits, BlockScalars* bs,
+                                                         uint16_t* __restrict__ out) {
+  constexpr int NS = SPLIT_FORMATS[PREC].pieces;
+  PreScale ps{1.f, 1.f};
+  if (PREC == PREC_FP16X2) ps = pre_scale(absmax >= 0.f ? absmax : __uint_as_float(*absmax_bits));
+  if (blockIdx.x == 0 && threadIdx.x == 0 && !side_b) { bs->x_scale = ps.scale; bs->x_inv_scale = ps.inv; }
+  const long long groups = Dp / 8, i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= rows * groups) return;
+  const long long n = i / groups;
+  const int d = static_cast<int>(i - n * groups) * 8;
+  const float* xr = x + n * D;
+  float v[8];
+  if (d + 7 < D && (D & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const float4 a4 = __ldg(reinterpret_cast<const float4*>(xr + d)), b4 = __ldg(reinterpret_cast<const float4*>(xr + d + 4));
+    v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = d + e < D ? __ldg(xr + d + e) : 0.f;
+  }
+  uint16_t p[8][3];
+  uint4 pk[3];
+  split8<PREC>(v, ps.scale, p, pk);
+  store_kcat_row<PREC>(out + n * (mma_passes(NS) * Dp), Dp, d, pk, side_b);
+}
+void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
+                       BlockScalars* bs, uint16_t* out, cudaStream_t st) {
+  const long long work = static_cast<long long>(rows) * (Dp / 8);
+  with_prec(prec, [&](auto P) {
+    eval_split_kernel<P><<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(x, rows, D, Dp, side_b, absmax, absmax_bits, bs, out);
+  });
+  count_launch();
+}
+
+// Best positive of each query from the statistics sweep: max over same-label non-self gallery rows, -inf when there is none
+__global__ void eval_best_kernel(RowArrays ra, int nq, float* __restrict__ best) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nq) best[i] = ra.cnt_same[i] > 0 ? ord2f(ra.st_maxw[i]) : -INFINITY;
+}
+void launch_eval_best(RowArrays ra, int nq, float* best, cudaStream_t st) {
+  eval_best_kernel<<<(nq + 255) / 256, 256, 0, st>>>(ra, nq, best);
+  count_launch();
+}
+
+// MAP@R: 64-bit segment offsets of the queries' positives, by one block.  Thread t sums a contiguous run of counts, the block scans
+// the runs, and each thread writes its run's offsets.
+__global__ void __launch_bounds__(1024) eval_seg_scan_kernel(const int* __restrict__ cnt, int nq, long long* __restrict__ seg, BlockScalars* bs,
+                                                             unsigned long long* __restrict__ sum_err) {
+  __shared__ long long s_warp[32];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int per = (nq + 1023) / 1024, i0 = min(nq, t * per), i1 = min(nq, i0 + per);
+  long long run = 0;
+  for (int i = i0; i < i1; ++i) run += cnt[i];
+  long long incl = run;                                      // inclusive scan: across the warp, then across the warps
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) s_warp[w] = incl;
+  __syncthreads();
+  if (w == 0) {
+    long long x = s_warp[lane], xi = x;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, xi, o);
+      if (lane >= o) xi += y;
+    }
+    s_warp[lane] = xi - x;                                   // exclusive prefix of each warp
+  }
+  __syncthreads();
+  long long off = s_warp[w] + incl - run;
+  for (int i = i0; i < i1; ++i) { seg[i] = off; off += cnt[i]; }
+  if (t == 1023) {
+    seg[nq] = off;
+    sum_err[0] = static_cast<unsigned long long>(off);
+    sum_err[1] = static_cast<unsigned long long>(bs->err);
+    bs->err = 0;
+  }
+}
+void launch_eval_seg_scan(const int* cnt, int nq, long long* seg, BlockScalars* bs, unsigned long long* sum_err, cudaStream_t st) {
+  eval_seg_scan_kernel<<<1, 1024, 0, st>>>(cnt, nq, seg, bs, sum_err);
+  count_launch();
+}
+
+// One warp per query: the rank of each positive in its segment is the number of larger keys plus the number of equal keys before it,
+// so every key lands on its own slot.  O(R_i^2 / 32) per query; the segments of metric-learning sets are short.
+__global__ void __launch_bounds__(256) eval_seg_sort_kernel(const int* __restrict__ cnt, const long long* __restrict__ seg, int nq,
+                                                            const float* __restrict__ src, float* __restrict__ dst) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= nq) return;
+  const int R = cnt[i];
+  const float* s = src + seg[i];
+  float* d = dst + seg[i];
+  for (int a = 0; a < R; a += 32) {
+    const int k = a + lane;
+    const uint32_t mine = k < R ? f2ord(s[k]) : 0u;
+    int r = 0;
+    for (int b = 0; b < R; b += 32) {
+      const uint32_t other = b + lane < R ? f2ord(s[b + lane]) : 0u;
+      const int n = min(32, R - b);
+      for (int j = 0; j < n; ++j) {
+        const uint32_t o = __shfl_sync(0xffffffffu, other, j);
+        r += (o > mine || (o == mine && b + j < k)) ? 1 : 0;
+      }
+    }
+    if (k < R) d[r] = ord2f(mine);
+  }
+}
+void launch_eval_seg_sort(const int* cnt, const long long* seg, int nq, const float* src, float* dst, cudaStream_t st) {
+  eval_seg_sort_kernel<<<(nq + 7) / 8, 256, 0, st>>>(cnt, seg, nq, src, dst);
+  count_launch();
+}
+
+// One thread per query, k = 1..R ascending: neg_ge(k) = sum of hist[b < k], pos_k = k + neg_ge(k).  fp64, summed in ascending k and
+// divided by R last, so a host loop in the same order gives the same bits.  rank = c_1 + neg_ge(1), c_1 = #{k : p_k = p_1}: the rank
+// of npair_eval_rank.
+__global__ void __launch_bounds__(256) eval_map_finish_kernel(const int* __restrict__ cnt, const long long* __restrict__ seg,
+                                                              const int* __restrict__ fill, const float* __restrict__ pos,
+                                                              const unsigned int* __restrict__ hist, int nq, double* __restrict__ map_r,
+                                                              double* __restrict__ r_precision, int* __restrict__ R_out, int* __restrict__ rank) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nq) return;
+  const int R = cnt[i];
+  double m = __longlong_as_double(0x7ff8000000000000ll), rp = m;
+  int rk = 0;
+  if (R > 0 && fill[i] == R) {
+    const float* p = pos + seg[i];
+    const unsigned int* h = hist + seg[i];
+    int c1 = 1;
+    while (c1 < R && p[c1] == p[0]) ++c1;
+    rk = c1 + static_cast<int>(h[0]);
+    double sum = 0.0;
+    long long neg_ge = 0;
+    int hits = 0;
+    for (int k = 1; k <= R; ++k) {
+      neg_ge += h[k - 1];
+      const long long pk = k + neg_ge;
+      if (pk > R) break;                                     // pos_k only grows with k
+      sum += static_cast<double>(k) / static_cast<double>(pk);
+      ++hits;
+    }
+    m = sum / R;
+    rp = static_cast<double>(hits) / R;
+  }
+  map_r[i] = m;
+  r_precision[i] = rp;
+  if (R_out) R_out[i] = R;
+  if (rank) rank[i] = rk;
+}
+void launch_eval_map_finish(const int* cnt, const long long* seg, const int* fill, const float* pos, const unsigned int* hist, int nq,
+                            double* map_r, double* r_precision, int* R_out, int* rank, cudaStream_t st) {
+  eval_map_finish_kernel<<<(nq + 255) / 256, 256, 0, st>>>(cnt, seg, fill, pos, hist, nq, map_r, r_precision, R_out, rank);
+  count_launch();
+}
+
+// --------------------------------------------------------------------------------------------
+// k-means (npair_eval_kmeans, DESIGN 8.2): everything around the EPI_ARGMAX sweep
+// --------------------------------------------------------------------------------------------
+// Centroid c = row rows[c] of x.  Thread = one feature of one centroid.
+__global__ void __launch_bounds__(256) km_gather_kernel(const float* __restrict__ x, int D, const int* __restrict__ rows, int k,
+                                                        float* __restrict__ C) {
+  const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<long long>(k) * D) return;
+  const long long c = e / D;
+  C[e] = x[static_cast<long long>(rows[c]) * D + (e - c * D)];
+}
+void launch_km_gather(const float* x, int D, const int* rows, int k, float* C, cudaStream_t st) {
+  const long long work = static_cast<long long>(k) * D;
+  km_gather_kernel<<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(x, D, rows, k, C);
+  count_launch();
+}
+
+// One warp per centroid: bias[c] = 0.5f * ||C_c||^2 in fp32 (per-lane fmaf chains over d = lane mod 32, then the warp tree), and the
+// iteration's reset of counts[c]; thread 0 also clears the {changed, err, nonempty} words.
+__global__ void __launch_bounds__(256) km_bias_kernel(const float* __restrict__ C, int k, int D, float* __restrict__ bias,
+                                                      int* __restrict__ counts, KmeansWords* words) {
+  const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *words = KmeansWords{0u, 0u, 0u, 0u};
+  if (c >= k) return;
+  const float* r = C + static_cast<long long>(c) * D;
+  float s = 0.f;
+  for (int d = lane; d < D; d += 32) s = fmaf(r[d], r[d], s);
+  s = warp_sum(s);
+  if (lane == 0) { bias[c] = 0.5f * s; counts[c] = 0; }
+}
+void launch_km_bias(const float* C, int k, int D, float* bias, int* counts, KmeansWords* words, cudaStream_t st) {
+  km_bias_kernel<<<(k + 7) / 8, 256, 0, st>>>(C, k, D, bias, counts, words);
+  count_launch();
+}
+
+// One warp per point: decode and clear its argmax key, count a changed assignment and a cluster's first member, and (accumulate)
+// add the point's fixed-point features q = rint(x * sigma * 2^32) to its cluster's int64 sums.  Integer atomics: the sums do not
+// depend on the order the points arrive in.
+__global__ void __launch_bounds__(256) km_assign_kernel(unsigned long long* __restrict__ best, const float* __restrict__ x, int n, int D,
+                                                        const unsigned int* __restrict__ absmax_bits, int k, int* __restrict__ assign,
+                                                        int* __restrict__ counts, long long* __restrict__ sums, int accumulate,
+                                                        KmeansWords* words) {
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  bool changed = false, first = false;
+  if (i < n) {
+    unsigned int a = 0;
+    if (lane == 0) {
+      const unsigned long long key = best[i];
+      best[i] = 0;
+      a = 0xFFFFFFFFu - static_cast<unsigned int>(key);
+      if (key == 0 || a >= static_cast<unsigned int>(k)) { a = 0; atomicOr(&words->err, static_cast<unsigned int>(DERR_KMEANS_NO_ARGMAX)); }
+      changed = assign[i] != static_cast<int>(a);
+      assign[i] = static_cast<int>(a);
+      first = atomicAdd(&counts[a], 1) == 0;
+    }
+    a = __shfl_sync(0xffffffffu, a, 0);
+    if (accumulate) {
+      const float sigma = pre_scale(__uint_as_float(*absmax_bits)).scale;
+      const float* xr = x + static_cast<long long>(i) * D;
+      unsigned long long* sr = reinterpret_cast<unsigned long long*>(sums + static_cast<long long>(a) * D);
+      for (int d = lane; d < D; d += 32)    // x * sigma in (-1, 1) and the scaling by 2^32 are exact; one rounding, to nearest even
+        atomicAdd(&sr[d], static_cast<unsigned long long>(__float2ll_rn((__ldg(xr + d) * sigma) * 4294967296.f)));
+    }
+  }
+  const int n_changed = __syncthreads_count(changed), n_first = __syncthreads_count(first);
+  if (threadIdx.x == 0) {
+    if (n_changed) atomicAdd(&words->changed, static_cast<unsigned int>(n_changed));
+    if (n_first) atomicAdd(&words->nonempty, static_cast<unsigned int>(n_first));
+  }
+}
+void launch_km_assign(unsigned long long* best, const float* x, int n, int D, const unsigned int* absmax_bits, int k, int* assign,
+                      int* counts, long long* sums, bool accumulate, KmeansWords* words, cudaStream_t st) {
+  km_assign_kernel<<<(n + 7) / 8, 256, 0, st>>>(best, x, n, D, absmax_bits, k, assign, counts, sums, accumulate ? 1 : 0, words);
+  count_launch();
+}
+
+// Thread = one feature of one centroid: the mean of a non-empty cluster, (float)(ldexp((double)sum / count, -32) * (1 / sigma)), every
+// step exactly rounded so a host loop in fp64 gives the same bits; an empty cluster keeps its centroid.  Clears the sums.
+__global__ void __launch_bounds__(256) km_update_kernel(long long* __restrict__ sums, const int* __restrict__ counts,
+                                                        const unsigned int* __restrict__ absmax_bits, int k, int D, float* __restrict__ C) {
+  const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<long long>(k) * D) return;
+  const int cnt = counts[e / D];
+  if (cnt > 0) {
+    const double inv = pre_scale(__uint_as_float(*absmax_bits)).inv;
+    C[e] = static_cast<float>(ldexp(static_cast<double>(sums[e]) / static_cast<double>(cnt), -32) * inv);
+    sums[e] = 0;
+  }
+}
+void launch_km_update(long long* sums, const int* counts, const unsigned int* absmax_bits, int k, int D, float* C, cudaStream_t st) {
+  const long long work = static_cast<long long>(k) * D;
+  km_update_kernel<<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(sums, counts, absmax_bits, k, D, C);
+  count_launch();
+}
+
+// Inertia in fp64 in a fixed order: warp w of the fixed grid takes points w, w + KM_INERTIA_BLOCKS * 8, ..., each lane its features
+// d = lane mod 32; the warp tree, the block's warps in order, then one thread over the blocks in order.
+__global__ void __launch_bounds__(256) km_inertia_kernel(const float* __restrict__ x, const float* __restrict__ C,
+                                                         const int* __restrict__ assign, int n, int D, double* __restrict__ partial) {
+  __shared__ double s_w[8];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double s = 0.0;
+  for (int i = blockIdx.x * 8 + w; i < n; i += KM_INERTIA_BLOCKS * 8) {
+    const float* xr = x + static_cast<long long>(i) * D;
+    const float* cr = C + static_cast<long long>(assign[i]) * D;
+    for (int d = lane; d < D; d += 32) {
+      const double e = static_cast<double>(xr[d]) - static_cast<double>(cr[d]);
+      s = fma(e, e, s);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) s_w[w] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int j = 0; j < 8; ++j) b += s_w[j];
+    partial[blockIdx.x] = b;
+  }
+}
+__global__ void km_inertia_finish_kernel(const double* __restrict__ partial, double* __restrict__ out) {
+  double s = 0.0;
+  for (int b = 0; b < KM_INERTIA_BLOCKS; ++b) s += partial[b];
+  *out = s;
+}
+void launch_km_inertia(const float* x, const float* C, const int* assign, int n, int D, double* partial, double* out, cudaStream_t st) {
+  km_inertia_kernel<<<KM_INERTIA_BLOCKS, 256, 0, st>>>(x, C, assign, n, D, partial);
+  km_inertia_finish_kernel<<<1, 1, 0, st>>>(partial, out);
+  count_launch(2);
+}
+
+}  // namespace npair

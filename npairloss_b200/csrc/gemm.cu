@@ -1,0 +1,158 @@
+// gemm.cu -- the one unit that instantiates the GEMM kernels: the wgmma similarity and gradient GEMMs (gemm_wgmma.cuh), the fused
+// gradient GEMM (grad_fused.cuh), the SIMT cross-check GEMM and the split-K reduce, with their launchers (declared in host.cuh).
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+
+#include "gemm_wgmma.cuh"
+#include "grad_fused.cuh"
+#include "host.cuh"
+#include "kernels.cuh"
+
+namespace npair {
+
+// ------------------------------------------------------------------------------------------------ GEMM launchers
+static int gemm_grid(const TileSched& ts, int sms) { return ts.num_tiles() < sms ? ts.num_tiles() : sms; }   // one CTA per tile, at most one per SM
+
+template <int NSPLIT, bool BF16, int EPI, int BK>
+static GemmKernel gemm_t() {
+  using Cfg = GemmCfg<NSPLIT, BK, EPI>;
+  return GemmKernel{split_gemm_kernel<NSPLIT, BF16, EPI, BK>, Cfg::THREADS, Cfg::SMEM_BYTES};
+}
+// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  Only the
+// epilogues the host composes are instantiated.
+template <bool BF16>
+static GemmKernel sim_gemm_t(int epi) {
+  switch (epi) {
+    case EPI_STORE_S | EPI_STATS: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS, 64>();
+    case EPI_STORE_S | EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS | EPI_SYM, 64>();
+    case EPI_STATS: return gemm_t<1, BF16, EPI_STATS, 64>();
+    case EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STATS | EPI_SYM, 64>();
+    case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
+    case EPI_COUNT: return gemm_t<1, BF16, EPI_COUNT, 64>();                       // retrieval evaluation
+    case EPI_COUNT | EPI_SYM: return gemm_t<1, BF16, EPI_COUNT | EPI_SYM, 64>();
+    case EPI_GATHER: return gemm_t<1, BF16, EPI_GATHER, 64>();                     // MAP@R evaluation
+    case EPI_GATHER | EPI_SYM: return gemm_t<1, BF16, EPI_GATHER | EPI_SYM, 64>();
+    case EPI_BUCKET: return gemm_t<1, BF16, EPI_BUCKET, 64>();
+    case EPI_BUCKET | EPI_SYM: return gemm_t<1, BF16, EPI_BUCKET | EPI_SYM, 64>();
+    case EPI_ARGMAX: return gemm_t<1, BF16, EPI_ARGMAX, 64>();                     // k-means assignment
+    default: return GemmKernel{nullptr, 0, 0};
+  }
+}
+// `epi`: EPI_OUT for the gradient GEMM (A = split gradient weights, B = split transposed features), else a similarity epilogue
+GemmKernel gemm_kernel(int prec, int epi) {
+  return with_prec(prec, [epi](auto P) {
+    constexpr SplitFormat f = SPLIT_FORMATS[P];
+    return epi != EPI_OUT ? sim_gemm_t<f.bf16>(epi) : gemm_t<f.pieces, f.bf16, EPI_OUT, bk_of(P, EPI_OUT)>();
+  });
+}
+// `sm`: fp32 tensor map of the similarity matrix for EPI_STORE_S's TMA stores (ignored otherwise: pass any valid map)
+cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st) {
+  const GemmKernel k = gemm_kernel(prec, epi);
+  if (!k.fn) return cudaErrorInvalidValue;
+  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(a, b, sm, p);
+  count_launch();
+  return cudaGetLastError();
+}
+
+FusedKernel fused_kernel(int prec) {
+  return with_prec(prec, [](auto P) {
+    constexpr SplitFormat f = SPLIT_FORMATS[P];
+    return FusedKernel{fused_grad_kernel<f.pieces, f.bf16>, FusedCfg<f.pieces>::THREADS, FusedCfg<f.pieces>::SMEM_BYTES};
+  });
+}
+cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
+  const FusedKernel k = fused_kernel(prec);
+  k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(b, sm, p);
+  count_launch();
+  return cudaGetLastError();
+}
+
+// SIMT cross-check of the same contraction on the same split operands (tests only; NPAIR_GEMM_SIMT_CHECK).
+template <int PREC>
+__device__ __forceinline__ float piece_sum(const uint16_t* base, long long off, long long ps) {
+  if (PREC == PREC_BF16) return __bfloat162float(__ushort_as_bfloat16(base[off]));
+  if (PREC == PREC_FP16X2) return __half2float(__ushort_as_half(base[off])) + __half2float(__ushort_as_half(base[ps + off]));
+  return __bfloat162float(__ushort_as_bfloat16(base[off])) + __bfloat162float(__ushort_as_bfloat16(base[ps + off])) +
+         __bfloat162float(__ushort_as_bfloat16(base[2 * ps + off]));
+}
+// OUT = 1: the gradient GEMM's EPI_OUT epilogue; OUT = 0: the similarity store
+template <int PREC, int OUT>
+__global__ void __launch_bounds__(256) simt_gemm_kernel(const uint16_t* __restrict__ A, long long lda, long long psA,
+                                                        const uint16_t* __restrict__ B, long long ldb, long long psB, int K, GemmParams p) {
+  __shared__ float As[16][65], Bs[16][65];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
+  float acc[4][4] = {};
+  for (int k0 = 0; k0 < K; k0 += 16) {
+    for (int e = threadIdx.x; e < 64 * 16; e += 256) {
+      const int r = e >> 4, kk = e & 15;
+      const int gm = m0 + r, gn = n0 + r, gk = k0 + kk;
+      As[kk][r] = (gm < p.M && gk < K) ? piece_sum<PREC>(A, static_cast<long long>(gm) * lda + gk, psA) : 0.f;
+      Bs[kk][r] = (gn < p.Nn && gk < K) ? piece_sum<PREC>(B, static_cast<long long>(gn) * ldb + gk, psB) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < 16; ++kk) {
+      float a[4], b[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { a[i] = As[kk][ty * 4 + i]; b[i] = Bs[kk][tx * 4 + i]; }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+  const float inv = p.dev_scale ? *p.dev_scale : 1.f;
+  for (int i = 0; i < 4; ++i) {
+    const int row = m0 + ty * 4 + i;
+    if (row >= p.M) continue;
+    for (int j = 0; j < 4; ++j) {
+      const int col = n0 + tx * 4 + j;
+      if (col >= p.Nn) continue;
+      if (!OUT) p.S[static_cast<long long>(row) * p.ldS + col] = acc[i][j] * inv * inv;
+      else {
+        float* d = p.out + static_cast<long long>(row) * p.ldo + col;
+        float o = p.alpha * inv * acc[i][j];
+        if (p.beta != 0.f) o += p.beta * *d;
+        *d = o;
+      }
+    }
+  }
+}
+// `epi`: EPI_OUT, or EPI_STORE_S for the similarity matrix
+cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long long lda, long long psA, const uint16_t* B, long long ldb,
+                             long long psB, int K, const GemmParams& p, cudaStream_t st) {
+  dim3 grid((p.Nn + 63) / 64, (p.M + 63) / 64);
+  with_prec(prec, [&](auto P) {
+    auto kernel = epi == EPI_OUT ? simt_gemm_kernel<P, 1> : simt_gemm_kernel<P, 0>;
+    kernel<<<grid, 256, 0, st>>>(A, lda, psA, B, ldb, psB, K, p);
+  });
+  count_launch();
+  return cudaGetLastError();
+}
+
+// out = sum_s part[s] + beta*out, fixed summation order (deterministic split-K).  Slice s starts at part + s*n: 16-byte loads and
+// stores only when every slice and `out` start 16-byte aligned (n % 4 == 0), otherwise one float at a time -- the same sums either way.
+__global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, long long n, float* __restrict__ out, float beta) {
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x, nth = static_cast<long long>(gridDim.x) * blockDim.x;
+  const bool vec = (n & 3) == 0 && ((reinterpret_cast<uintptr_t>(part) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+  if (vec) {
+    for (long long i = t0 * 4; i < n; i += nth * 4) {
+      float4 a = *reinterpret_cast<const float4*>(part + i);
+      for (int s = 1; s < splits; ++s) { const float4 b = *reinterpret_cast<const float4*>(part + s * n + i); a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
+      if (beta != 0.f) { const float4 o = *reinterpret_cast<const float4*>(out + i); a.x += beta * o.x; a.y += beta * o.y; a.z += beta * o.z; a.w += beta * o.w; }
+      *reinterpret_cast<float4*>(out + i) = a;
+    }
+  } else {
+    for (long long i = t0; i < n; i += nth) {
+      float a = part[i];
+      for (int s = 1; s < splits; ++s) a += part[s * n + i];
+      if (beta != 0.f) a += beta * out[i];
+      out[i] = a;
+    }
+  }
+}
+
+}  // namespace npair

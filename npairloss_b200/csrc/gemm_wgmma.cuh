@@ -47,7 +47,7 @@ namespace npair {
 //               which is independent of the tile order.  No self exclusion, no labels.  Used alone, with full tiles (no EPI_SYM).
 enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64, EPI_GATHER = 128, EPI_BUCKET = 256, EPI_ARGMAX = 512 };
 
-// Persistent tile schedule of both wgmma GEMMs (host: tile_sched, ctx.cu).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
+// Persistent tile schedule of both wgmma GEMMs (host: tile_sched, host.cuh).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
 // output tile (m_blk, n_blk) or tile_list[t], K blocks [kb0, kb1) of split-K slice `split`.  split moves fastest, then n_blk, m_blk.
 struct Tile { int m_blk, n_blk, split, kb0, kb1; };
 struct TileSched {

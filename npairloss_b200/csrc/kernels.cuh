@@ -236,16 +236,6 @@ void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars
 void launch_thresholds_world(const float* xall, int xstride, int world, long long N, MiningParams mp, BlockScalars* bs, cudaStream_t st);
 // World scope: the tops of the world's N rows from the ranks' TopSums, which lie xstride floats apart in xall
 void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
-// side_mask: bit 0 = AP threshold over the same-label list, bit 1 = AN threshold over the diff-label list
-void launch_local_select(SimRows sim, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
-// lets the current device launch the one-warp-per-row local select with its dynamic shared memory (above the default limit)
-cudaError_t allow_local_select_smem();
-// over the rank's whole S (sim.row0 == 0, sim.rows == Q)
-void launch_global_select_pass(SimRows sim, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
-                               uint32_t* cand /*[2][cand_cap]*/, unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st);
-// world scope: the ranks' [2][2048] 64-bit digit counts lie xstride floats apart in xall
-void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
-                          uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
 // Row pass over the rows of sim.  finalize: the last block also reduces the Q rows' results into the tops; otherwise
 // launch_lse_finalize does, once.  xout: NULL, or (world scope) receives the rank's TopSums instead of the tops
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
@@ -260,7 +250,20 @@ void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);
 
-// Retrieval evaluation (DESIGN 8).  `ra` holds only the per-query statistics of the similarity GEMM's EPI_STATS epilogue (st_*, cnt_same).
+// launchers of the radix selects (select.cu)
+// side_mask: bit 0 = AP threshold over the same-label list, bit 1 = AN threshold over the diff-label list
+void launch_local_select(SimRows sim, int side_mask, float sn_ap, float sn_an, RowArrays ra, BlockScalars* bs, int sms, bool force_warp_kernel, cudaStream_t st);
+// lets the current device launch the one-warp-per-row local select with its dynamic shared memory (above the default limit)
+cudaError_t allow_local_select_smem();
+// over the rank's whole S (sim.row0 == 0, sim.rows == Q)
+void launch_global_select_pass(SimRows sim, int side_mask, int pass /*0,1,2*/, RowArrays ra, unsigned long long* hist /*[2][2048], zero*/,
+                               uint32_t* cand /*[2][cand_cap]*/, unsigned int cand_cap, int world_scope, BlockScalars* bs, int sms, cudaStream_t st);
+// world scope: the ranks' [2][2048] 64-bit digit counts lie xstride floats apart in xall
+void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
+                          uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
+
+// Retrieval evaluation (DESIGN 8; launchers in eval_kernels.cu).  `ra` holds only the per-query statistics of the similarity GEMM's
+// EPI_STATS epilogue (st_*, cnt_same).
 // max|x| over queries and gallery (g == NULL: the query set is the gallery) into the pre-zeroed *absmax_bits (NULL: no reduction),
 // and the reset of the nq queries' statistics
 void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, RowArrays ra, int nq,

@@ -11,8 +11,10 @@ def funcs(path):
         if m:
             if cur: d[cur] = hashlib.md5("\n".join(buf).encode()).hexdigest()
             cur, buf = m.group(1), []
-        elif cur:
-            buf.append(l)
+        elif cur and l.lstrip().startswith("/*"):
+            # instruction and encoding lines only, blanks collapsed: cuobjdump pads the instruction column to the widest instruction
+            # of the object, and the headers between objects follow the last kernel of each, so neither may depend on the object
+            buf.append(" ".join(l.split()))
     if cur: d[cur] = hashlib.md5("\n".join(buf).encode()).hexdigest()
     return d
 

@@ -4,7 +4,7 @@ The thresholds restate DESIGN §4.1 independently of the C++ oracle: the same-la
 row (LOCAL) or of the whole Q x N block (GLOBAL), the self pair excluded; the order statistic at the reference's fp32 `pos()`; negative
 picks clamped to -FLT_MAX.  The unclamped pick is returned too, so a test can assert that its pick is visible through the clamp.
 
-The path predicates restate the size rules of `plan_of` (ctx.cu) and the digit rules of the select kernels (kernels.cu), so a test can
+The path predicates restate the size rules of `plan_of` (ctx.cu) and the digit rules of the select kernels (select.cu), so a test can
 assert that its data reaches the path it is named after.
 """
 import numpy as np

@@ -58,6 +58,14 @@ def test_no_cpu_fallback():
     assert e.value.code == -2 and "no CPU fallback" in str(e.value)
 
 
+@pytest.mark.skipif(_have_gpu(), reason="checks the no-GPU failure mode")
+def test_no_cpu_fallback_for_the_evaluator():
+    """npair_eval_create fails like npair_create, and npair_eval_last_error(NULL) reads the message the shared device check wrote."""
+    with pytest.raises(capi.NpairError) as e:
+        capi.Evaluator(8, 8, 4)
+    assert e.value.code == -2 and "no CPU fallback" in str(e.value)
+
+
 def test_config_defaults_cover_the_abi2_extensions():
     """npair_config_default: proto defaults (caffe.proto:4-7,19-22) and every ABI-2 extension switched off."""
     import ctypes as C

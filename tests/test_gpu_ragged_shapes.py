@@ -43,7 +43,7 @@ def _cdiv(a, b):
 
 
 def grad_splits(Q, D, world, prec, fused, sms):
-    """split_k (ctx.cu) restated: split-K slices of the rank's Q x D gradient GEMM, whose K is the N = Q*world sample index in blocks
+    """split_k (host.cuh) restated: split-K slices of the rank's Q x D gradient GEMM, whose K is the N = Q*world sample index in blocks
     of 32 (fused kernel, >= 8 blocks per slice) or of the split GEMM's K block (>= 4 per slice), on 128 x 256 output tiles."""
     kb = _cdiv(Q * world, 32 if fused or prec != BF16 else 64)
     tiles = _cdiv(Q, 128) * _cdiv(D, 256)

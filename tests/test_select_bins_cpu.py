@@ -1,4 +1,4 @@
-"""CPU model of the value-bin map of local_select_block_kernel (npairloss_b200/csrc/kernels.cu, lsb_off): bin*4 is read from the mantissa of
+"""CPU model of the value-bin map of local_select_block_kernel (npairloss_b200/csrc/select.cu, lsb_off): bin*4 is read from the mantissa of
 fmaf(s, s4, c0) with s4 = 4*2048/(hi-lo), c0 = fmaf(-lo, s4, 2^23 + 4).  The kernel relies on three properties of that map, checked
 here in float32 arithmetic for many value ranges: it is monotone in s, every s in [lo, hi] lands inside the 2304 bins the find walks
 , and NaN (an excluded entry) lands in bin 4095.  Ranges for which the kernel's own guard (`map_ok`) rejects the
