@@ -304,6 +304,25 @@ int npair_eval_kmeans(npair_eval* ev, const float* d_x, int32_t n, int32_t k, co
 /* Device memory npair_eval_kmeans adds on top of the workspace (grown on demand, kept until npair_eval_destroy): 8 * k * D + 8 * n +
  * 12 * k + 2064 bytes.  0 for bad arguments (n, k or D < 1, k > n). */
 size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D);
+/* Exact k nearest neighbours (DESIGN 8.3).  For query i the candidates are the gallery rows j of this call other than query i's own
+ * (self_offset, global, -1: none; as in npair_eval_best_positive), with s_ij the library's similarity in `precision`: the same bits as
+ * the layer's S and as npair_eval_rank's sweeps.  Row i of d_sim / d_index (nq x k, row-major) holds the k candidates that come first
+ * in the total order "s descending, then global gallery index ascending", where NaN ranks below every number (-inf included); d_index
+ * is global: gallery_row0 + the column in the shard.  The output bits do not depend on block_rows, the stream, repeated calls or a
+ * fresh evaluator.  Sharding: with a shared absmax (>= 0: max|x| over the queries and the WHOLE gallery, as for npair_eval_count),
+ * merging the shards' lists of a query by the same order and keeping the first k gives the one-call result bit for bit.  absmax < 0:
+ * the pre-scale is reduced over this call's queries and gallery.
+ * 1 <= k <= NPAIR_EVAL_KNN_MAX_K, and k <= ng - 1 when some query's own row lies in this shard, else k <= ng.  block_rows: queries per
+ * block of S, a multiple of 128, or 0 for 1024; the call holds min(block_rows, nq rounded up to 128) rows.  Anything else is
+ * NPAIR_E_ARG, checked on the host before anything is enqueued.  Asynchronous on `stream`.
+ * Device memory: on top of the workspace, npair_eval_knn_bytes(ng, k, block_rows) (an upper bound: the call caps the rows at nq),
+ * grown on demand and kept until npair_eval_destroy; nothing of size nq x ng is held. */
+#define NPAIR_EVAL_KNN_MAX_K 1024
+int npair_eval_knn(npair_eval* ev, const float* d_query, int32_t nq, const float* d_gallery, int32_t ng, int32_t self_offset,
+                   int32_t gallery_row0, float absmax, int32_t k, int32_t block_rows, float* d_sim, int32_t* d_index, void* stream);
+/* Device memory npair_eval_knn adds on top of the workspace: one block of S, 4 * block_rows * round_up(ng, 32) bytes (block_rows 0:
+ * 1024).  0 for bad arguments (ng < 1, k outside [1, min(ng, NPAIR_EVAL_KNN_MAX_K)], block_rows not 0 or a multiple of 128). */
+size_t npair_eval_knn_bytes(int32_t ng, int32_t k, int32_t block_rows);
 
 #ifdef __cplusplus
 }

@@ -45,7 +45,7 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
-           "npair_eval_kmeans", "npair_eval_kmeans_bytes"]
+           "npair_eval_kmeans", "npair_eval_kmeans_bytes", "npair_eval_knn", "npair_eval_knn_bytes"]
 
 _LIB = None
 
@@ -113,6 +113,9 @@ def lib():
         L.npair_eval_kmeans.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, vp]
         L.npair_eval_kmeans_bytes.argtypes = [i32, i32, i32]
         L.npair_eval_kmeans_bytes.restype = C.c_size_t
+        L.npair_eval_knn.argtypes = [vp, vp, i32, vp, i32, i32, i32, C.c_float, i32, i32, vp, vp, vp]
+        L.npair_eval_knn_bytes.argtypes = [i32, i32, i32]
+        L.npair_eval_knn_bytes.restype = C.c_size_t
         _LIB = L
     return _LIB
 
@@ -253,6 +256,11 @@ def eval_kmeans_bytes(n: int, k: int, D: int) -> int:
     return int(lib().npair_eval_kmeans_bytes(n, k, D))
 
 
+def eval_knn_bytes(ng: int, k: int, block_rows: int = 0) -> int:
+    """Device bytes Evaluator.knn adds on top of the workspace for a gallery of ng rows (block_rows 0: the default; 0 if invalid)."""
+    return int(lib().npair_eval_knn_bytes(ng, k, block_rows))
+
+
 class Evaluator:
     """Retrieval evaluation (include/npair_b200.h, DESIGN 8): the rank of every query's best positive among the gallery, computed on
     the tensor cores without storing the similarity matrix.  Takes contiguous CUDA fp32 tensors; results are int32 / fp32 CUDA
@@ -315,6 +323,18 @@ class Evaluator:
                                            self_offset, gallery_row0, C.c_float(absmax), self._arg(cut, 1), count.data_ptr(),
                                            torch.cuda.current_stream().cuda_stream))
         return count
+
+    def knn(self, query, gallery, k, self_offset=-1, gallery_row0=0, absmax=-1.0, block_rows=0):
+        """npair_eval_knn: each query's k nearest gallery rows, s descending, then global gallery index ascending (NaN last).  Returns
+        (fp32 sim[nq, k], int32 index[nq, k]) with index = gallery_row0 + the row in `gallery`; absmax >= 0 for a gallery shard."""
+        import torch
+        nq, dev = query.shape[0], query.device
+        sim = torch.empty(nq, int(k), dtype=torch.float32, device=dev)
+        index = torch.empty(nq, int(k), dtype=torch.int32, device=dev)
+        self._check(lib().npair_eval_knn(self._h, self._arg(query, 2), nq, self._arg(gallery, 2), gallery.shape[0], self_offset,
+                                         gallery_row0, C.c_float(absmax), int(k), block_rows, sim.data_ptr(), index.data_ptr(),
+                                         torch.cuda.current_stream().cuda_stream))
+        return sim, index
 
     def map_at_r(self, query, qlabel, gallery, glabel, self_offset=-1):
         """npair_eval_map_at_r: fp64 map_r[nq] and r_precision[nq] (NaN where a query has no positive), int32 R[nq] and rank[nq]

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
+#include <cstdint>
 #include <memory>
 #include <string>
 #include <vector>
@@ -52,9 +53,9 @@ struct npair_eval : EvalPlan {
   int2* sym_tiles = nullptr;
   int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
   std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
-  // MAP@R (MapRows, MapPairs) and k-means (KmeansBufs) buffers, grown on demand and kept
-  DevMem map_rows_mem, map_pairs_mem, km_mem;
-  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr;
+  // MAP@R (MapRows, MapPairs), k-means (KmeansBufs) and k-NN (KnnBlock) buffers, grown on demand and kept
+  DevMem map_rows_mem, map_pairs_mem, km_mem, knn_mem;
+  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr, *knn = nullptr;
   StreamOrder order;              // the calls' order across streams
   std::string err;
 };
@@ -89,6 +90,18 @@ struct KmeansBufs : Carve {
     counts = take<int>(k); bias = take<float>(k); rows = take<int>(k); words = take<KmeansWords>(1);
   }
 };
+// k-NN takes one: a block of `rows` rows of S, each round_up(ng, 32) floats long (the stride the similarity GEMM's stores need)
+struct KnnBlock : Carve {
+  float* S; long long ldS;
+  KnnBlock(char* base, long long rows, long long ng) : Carve{base}, ldS(round_up(ng, 32)) { S = take<float>(rows * ldS); }
+};
+static_assert(KNN_MAX_K == NPAIR_EVAL_KNN_MAX_K, "the select's capacity is the call's limit on k");
+static constexpr int KNN_DEFAULT_BLOCK_ROWS = 1024;
+// Rows of S a k-NN call holds: block_rows (0: the default), capped at nq rounded up to the 128-row tile
+static int knn_block_rows(int block_rows, int nq) {
+  const long long rows = block_rows ? block_rows : KNN_DEFAULT_BLOCK_ROWS, cap = round_up(nq, 128);
+  return static_cast<int>(rows < cap ? rows : cap);
+}
 
 // Grows the buffer `m` holds at *base to at least `bytes` (cudaFree of the old one waits for the device); `what` names it in errors
 static int eval_grow(npair_eval* ev, DevMem& m, char** base, size_t bytes, const char* what) {
@@ -124,6 +137,11 @@ size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
   return KmeansBufs(nullptr, n, k, D).bytes;
 }
 
+size_t npair_eval_knn_bytes(int32_t ng, int32_t k, int32_t block_rows) {
+  if (ng < 1 || k < 1 || k > NPAIR_EVAL_KNN_MAX_K || k > ng || block_rows < 0 || block_rows % 128) return 0;
+  return KnnBlock(nullptr, block_rows ? block_rows : KNN_DEFAULT_BLOCK_ROWS, ng).bytes;
+}
+
 const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
 
 void npair_eval_destroy(npair_eval* ev) {
@@ -146,8 +164,9 @@ int npair_eval_create(int32_t max_q, int32_t max_g, int32_t D, int32_t prec, int
   CREATE_TRY(eval_buffers(ev, ev->mem));
   CREATE_TRY(ev->order.create());
   const int epis[] = {EPI_STATS, EPI_STATS | EPI_SYM, EPI_COUNT, EPI_COUNT | EPI_SYM, EPI_GATHER, EPI_GATHER | EPI_SYM, EPI_BUCKET,
-                      EPI_BUCKET | EPI_SYM, EPI_ARGMAX};
+                      EPI_BUCKET | EPI_SYM, EPI_ARGMAX, EPI_STORE_S};
   for (int epi : epis) CREATE_TRY(allow_smem(gemm_kernel(prec, epi)));
+  CREATE_TRY(allow_knn_select_smem());
   *out = made.release();
   return NPAIR_OK;
 }
@@ -270,6 +289,45 @@ int npair_eval_count(npair_eval* ev, const float* q, int32_t nq, const float* g,
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, sym, st)) != NPAIR_OK) return rc;
   CUDA_TRY(ev, cudaMemsetAsync(d_count, 0, sizeof(int32_t) * nq, st));
   if ((rc = eval_sweep(ev, EPI_COUNT, nq, ng, self_col, nullptr, nullptr, d_cut, d_count, sym, st)) != NPAIR_OK) return rc;
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+// k nearest neighbours (DESIGN 8.3): the operands once, then per block of block_rows queries the layer's store-only recompute of that
+// row block of S (full tiles) and one select block per query row.  Every entry of S has the same bits whatever block holds it.
+int npair_eval_knn(npair_eval* ev, const float* q, int32_t nq, const float* g, int32_t ng, int32_t self_offset, int32_t gallery_row0,
+                   float absmax, int32_t k, int32_t block_rows, float* d_sim, int32_t* d_index, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  int rc = eval_check(ev, q, nq, g, ng, self_offset, gallery_row0, absmax < 0.f ? 0.f : absmax, false);
+  if (rc != NPAIR_OK) return rc;
+  if (!d_sim || !d_index) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (static_cast<long long>(gallery_row0) + ng > INT32_MAX) { ev->err = "gallery_row0 + ng exceeds the int32 index range"; return NPAIR_E_ARG; }
+  if (block_rows < 0 || block_rows % 128) { ev->err = fmt("block_rows = %d must be 0 or a positive multiple of 128", block_rows); return NPAIR_E_ARG; }
+  // the self columns of the queries, [self_col, self_col + nq), where they meet the shard's columns
+  long long self_col = self_offset < 0 ? EVAL_NO_SELF : static_cast<long long>(self_offset) - gallery_row0;
+  if (self_col >= ng || self_col + nq <= 0) self_col = EVAL_NO_SELF;
+  const int valid = self_col == EVAL_NO_SELF ? ng : ng - 1;
+  if (k < 1 || k > NPAIR_EVAL_KNN_MAX_K || k > valid) {
+    ev->err = fmt("k = %d must lie in [1, %d] and not exceed the %d candidate columns of a query", k, NPAIR_EVAL_KNN_MAX_K, valid);
+    return NPAIR_E_ARG;
+  }
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
+  const int rows = knn_block_rows(block_rows, nq);
+  if ((rc = eval_grow(ev, ev->knn_mem, &ev->knn, KnnBlock(nullptr, rows, ng).bytes, "the k-NN block of S")) != NPAIR_OK) return rc;
+  const KnnBlock blk(ev->knn, rows, ng);
+  if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, false, st)) != NPAIR_OK) return rc;
+  CUtensorMap ta, tb;
+  std::string te;
+  if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
+  for (int r0 = 0; r0 < nq; r0 += rows) {
+    const int m = nq - r0 < rows ? nq - r0 : rows;
+    GemmParams gp = sim_sweep(EPI_STORE_S, m, ng, ev->kcat, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
+    gp.a_row0 = r0; gp.S = blk.S; gp.ldS = blk.ldS;
+    CUDA_TRY(ev, launch_gemm(ev->prec, EPI_STORE_S, ta, tb, ta, gp, ev->sms, st));
+    launch_knn_select(blk.S, blk.ldS, m, ng, k, r0, static_cast<int>(self_col), gallery_row0, d_sim, d_index, st);
+  }
   CUDA_TRY(ev, cudaGetLastError());
   return NPAIR_OK;
 }

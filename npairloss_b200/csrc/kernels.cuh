@@ -261,6 +261,14 @@ void launch_global_select_pass(SimRows sim, int side_mask, int pass /*0,1,2*/, R
 // world scope: the ranks' [2][2048] 64-bit digit counts lie xstride floats apart in xall
 void launch_global_decide(const float* xall, int xstride, int world, int side_mask, int pass, RowArrays ra, int Q, unsigned long long* hist,
                           uint32_t* cand, unsigned int cand_cap, BlockScalars* bs, cudaStream_t st);
+// k nearest neighbours (npair_eval_knn): for each of the `rows` rows of the stored block S (stride ldS, a multiple of 32), query
+// q0 + r, its k <= KNN_MAX_K largest columns j < ng other than column q0 + r + self_col0, by s descending (NaN last), then j ascending,
+// into rows q0 + r of out_sim / out_idx [.. x k] (out_idx = col_base + j)
+constexpr int KNN_MAX_K = 1024;
+void launch_knn_select(const float* S, long long ldS, int rows, int ng, int k, int q0, int self_col0, int col_base, float* out_sim,
+                       int* out_idx, cudaStream_t st);
+// lets the current device launch the k-NN select with its dynamic shared memory (above the default limit)
+cudaError_t allow_knn_select_smem();
 
 // Retrieval evaluation (DESIGN 8; launchers in eval_kernels.cu).  `ra` holds only the per-query statistics of the similarity GEMM's
 // EPI_STATS epilogue (st_*, cnt_same).

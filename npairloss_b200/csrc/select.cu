@@ -793,4 +793,135 @@ void launch_global_decide(const float* xall, int xstride, int world, int side_ma
   count_launch();
 }
 
+// ---- k nearest neighbours (npair_eval_knn, DESIGN 8.3): ONE BLOCK per row of a stored block of S ----
+// Every valid column j of a row gets the 64-bit key (ord(s) << 32) | ~j, ord(NaN) = 0: keys are distinct, and descending key order is
+// the call's total order (s descending, NaN last, then j ascending).  The row's k largest keys are those >= T, T the k-th largest key,
+// which an MSB-first radix select builds digit by digit (11 / 11 / 10 bits of ord(s), then 11 / 11 / 10 of ~j).  It stops at the first
+// digit whose chosen bin is taken whole (the k-th key is the bin's smallest); T is then the decided prefix, its lower bits zero.  Ties
+// in s are decided by the column bits like any other digit, so nothing depends on the order of atomics.  Rows of at most KNN_CAP
+// columns are compacted into shared memory with one read of S; longer rows (SOP-sized) take the first digit from S and compact that
+// bin and everything above it, or, when those exceed KNN_CAP entries (a mass of ties), run every digit and the final pass over S.
+// The <= KNN_MAX_K survivors are sorted by a bitonic network in shared memory.
+#define NPAIR_KNN_THREADS 512
+#define NPAIR_KNN_CAP 8192                  // keys a row's candidates may take in shared memory
+#define NPAIR_KNN_U 4                       // 16-byte loads in flight per thread
+struct KnnSmem {
+  unsigned long long cand[NPAIR_KNN_CAP];
+  unsigned long long top[KNN_MAX_K];
+  unsigned int hist[2048];
+  unsigned long long s_scan[32], s_out[3];
+  unsigned int n_cand, n_top;
+};
+static constexpr int KNN_SMEM = static_cast<int>(sizeof(KnnSmem));
+
+__device__ __forceinline__ unsigned long long knn_key(uint32_t bits, int j) {
+  const float s = __uint_as_float(bits);
+  return (static_cast<unsigned long long>(s != s ? 0u : f2ord(s)) << 32) | static_cast<uint32_t>(~j);
+}
+// f(key) for every valid column of `row` (j < ng, j != sc): 16-byte loads, which stay inside the row (its stride is a multiple of 32)
+template <class F>
+__device__ __forceinline__ void knn_row_keys(const float* __restrict__ row, int ng, int sc, F f) {
+  for (int j0 = threadIdx.x * 4; j0 < ng; j0 += NPAIR_KNN_THREADS * 4 * NPAIR_KNN_U) {
+    uint4 v[NPAIR_KNN_U];
+#pragma unroll
+    for (int u = 0; u < NPAIR_KNN_U; ++u) {
+      const int jj = j0 + u * NPAIR_KNN_THREADS * 4;
+      if (jj < ng) v[u] = ldg_stream_u4(row + jj);
+    }
+#pragma unroll
+    for (int u = 0; u < NPAIR_KNN_U; ++u) {
+      const int jj = j0 + u * NPAIR_KNN_THREADS * 4;
+      if (jj >= ng) continue;
+      const uint32_t vv[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (jj + c < ng && jj + c != sc) f(knn_key(vv[c], jj + c));
+    }
+  }
+}
+
+__global__ void __launch_bounds__(NPAIR_KNN_THREADS, 2) knn_select_kernel(const float* __restrict__ S, long long ldS, int ng, int k, int q0,
+                                                                          int self_col0, int col_base, float* __restrict__ out_sim,
+                                                                          int* __restrict__ out_idx) {
+  extern __shared__ __align__(16) unsigned char knn_smem[];
+  KnnSmem& K = *reinterpret_cast<KnnSmem*>(knn_smem);
+  const int tid = threadIdx.x, qi = q0 + static_cast<int>(blockIdx.x);
+  const float* row = S + static_cast<long long>(blockIdx.x) * ldS;
+  const int sc = qi + self_col0;
+  const auto from_row = [&](auto f) { knn_row_keys(row, ng, sc, f); };
+  const auto from_cand = [&](auto f) { const unsigned int n = K.n_cand; for (unsigned int e = tid; e < n; e += NPAIR_KNN_THREADS) f(K.cand[e]); };
+  unsigned long long pre = 0, msk = 0;      // decided digits of T, and their bits
+  unsigned int rank = static_cast<unsigned int>(k - 1);   // of the k-th key among the keys that share the prefix, from the top
+  unsigned int pop = 0;                     // keys in the chosen bin of the last digit
+  int shift = 64;
+  bool done = false;
+  // one digit: histogram of the keys that share the prefix, then the bin of `rank` walking down from the top bin.  Every thread takes
+  // the bin's rank and population from s_out before the closing barrier: the next digit clears the histogram without waiting
+  const auto digit = [&](auto keys) {
+    const int bits = (shift == 42 || shift == 10) ? 10 : 11, nb = 1 << bits;
+    shift -= bits;
+    for (int b = tid; b < nb; b += NPAIR_KNN_THREADS) K.hist[b] = 0;
+    __syncthreads();
+    keys([&](unsigned long long key) { if ((key & msk) == pre) smem_inc(&K.hist[(key >> shift) & (nb - 1)]); });
+    __syncthreads();
+    find_bin([&](int o) { return static_cast<unsigned long long>(K.hist[nb - 1 - o]); }, nb, rank, K.s_scan, K.s_out);
+    const unsigned long long d = static_cast<unsigned long long>(nb - 1) - K.s_out[0];
+    const unsigned int r_in = static_cast<unsigned int>(K.s_out[1]);
+    pop = static_cast<unsigned int>(K.s_out[2]);
+    pre |= d << shift; msk |= static_cast<unsigned long long>(nb - 1) << shift;
+    rank = r_in;
+    done = r_in + 1 == pop || shift == 0;
+    __syncthreads();                        // s_out is read by every thread before it changes
+  };
+  // the keys >= pre of `keys` into `list` (n: its count)
+  const auto collect = [&](auto keys, unsigned long long* list, unsigned int* n) {
+    if (tid == 0) *n = 0;
+    __syncthreads();
+    keys([&](unsigned long long key) { if (key >= pre) list[atomicAdd(n, 1u)] = key; });
+    __syncthreads();
+  };
+  bool in_smem = true;
+  if (ng > NPAIR_KNN_CAP) {
+    digit(from_row);
+    in_smem = (k - 1 - rank) + pop <= NPAIR_KNN_CAP;     // what the compaction keeps; block-uniform
+  }
+  if (in_smem) {
+    collect(from_row, K.cand, &K.n_cand);
+    while (!done) digit(from_cand);
+    collect(from_cand, K.top, &K.n_top);
+  } else {
+    while (!done) digit(from_row);
+    collect(from_row, K.top, &K.n_top);
+  }
+  // bitonic sort, descending, of the k keys padded with zeros (no valid key is 0: ~j has its top bits set)
+  int n2 = 1;
+  while (n2 < k) n2 <<= 1;
+  for (int e = k + tid; e < n2; e += NPAIR_KNN_THREADS) K.top[e] = 0ull;
+  for (int size = 2; size <= n2; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      __syncthreads();
+      for (int t = tid; t < (n2 >> 1); t += NPAIR_KNN_THREADS) {
+        const int i = 2 * t - (t & (stride - 1)), j = i + stride;
+        const unsigned long long a = K.top[i], b = K.top[j];
+        if ((a < b) == ((i & size) == 0)) { K.top[i] = b; K.top[j] = a; }
+      }
+    }
+  }
+  __syncthreads();
+  for (int t = tid; t < k; t += NPAIR_KNN_THREADS) {
+    const unsigned long long key = K.top[t];
+    const uint32_t o = static_cast<uint32_t>(key >> 32);
+    out_sim[static_cast<long long>(qi) * k + t] = o ? ord2f(o) : __uint_as_float(0x7FC00000u);
+    out_idx[static_cast<long long>(qi) * k + t] = col_base + static_cast<int>(~static_cast<uint32_t>(key));
+  }
+}
+cudaError_t allow_knn_select_smem() {
+  return cudaFuncSetAttribute(knn_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KNN_SMEM);
+}
+void launch_knn_select(const float* S, long long ldS, int rows, int ng, int k, int q0, int self_col0, int col_base, float* out_sim,
+                       int* out_idx, cudaStream_t st) {
+  knn_select_kernel<<<rows, NPAIR_KNN_THREADS, KNN_SMEM, st>>>(S, ldS, ng, k, q0, self_col0, col_base, out_sim, out_idx);
+  count_launch();
+}
+
 }  // namespace npair

@@ -218,9 +218,7 @@ def clustering_scores(labels, assign):
 def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
     """(query, query labels, gallery, gallery labels, self_offset) as the evaluator takes them: contiguous 2-D CUDA fp32 rows, fp32
     labels; gallery=None is self-retrieval."""
-    if not query.is_cuda or query.dtype != torch.float32:
-        raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
-    q = query.reshape(query.shape[0], -1).contiguous()
+    q = _embeddings(who, query)
     ql = _fp32_labels(qlabel.to(q.device)).contiguous()
     if gallery is None:
         if glabel is not None:
@@ -229,11 +227,57 @@ def _retrieval_sets(who, query, qlabel, gallery, glabel, self_offset):
     else:
         if glabel is None:
             raise ValueError("gallery without glabel")
-        if not gallery.is_cuda or gallery.dtype != torch.float32:
-            raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
-        g = gallery.reshape(gallery.shape[0], -1).contiguous()
+        g = _embeddings(who, gallery)
         gl = _fp32_labels(glabel.to(q.device)).contiguous()
         off = -1 if self_offset is None else self_offset
     if g.shape[1] != q.shape[1]:
         raise ValueError("query and gallery dimensions differ")
     return q, ql, g, gl, off
+
+
+def _embeddings(who, x):
+    """x as the evaluator takes embeddings: contiguous 2-D CUDA fp32 rows."""
+    if not x.is_cuda or x.dtype != torch.float32:
+        raise TypeError(f"{who} takes CUDA float32 embeddings (there is no CPU path)")
+    return x.reshape(x.shape[0], -1).contiguous()
+
+
+def knn(query, gallery=None, *, k, precision=capi.PREC_FP32_FP16X2, self_offset=None, block_rows=None):
+    """Exact k nearest neighbours of every query among the gallery rows (Evaluator.knn, DESIGN 8.3; not part of the reference layer),
+    by the library's similarity: the same values recall_at_k ranks by.
+
+    Sets as in recall_at_k, without labels: gallery=None is self-retrieval, every row against all the others; otherwise disjoint
+    query / gallery sets, or, with `self_offset` = o, queries that are gallery rows o, o+1, ...  Row i lists the k gallery rows that
+    come first by similarity descending, then gallery index ascending; a NaN similarity ranks below every number.  block_rows: queries
+    per block of the similarity matrix the call holds (a multiple of 128; None: 1024), which changes memory, never the result.
+    Returns (sim [nq, k] fp32, index [nq, k] int64) CUDA tensors."""
+    q = _embeddings("knn", query)
+    if gallery is None:
+        g, off = q, 0 if self_offset is None else self_offset
+    else:
+        g, off = _embeddings("knn", gallery), -1 if self_offset is None else self_offset
+    if g.shape[1] != q.shape[1]:
+        raise ValueError("query and gallery dimensions differ")
+    ev = capi.Evaluator(q.shape[0], g.shape[0], q.shape[1], precision, q.device.index or 0)
+    try:
+        sim, index = ev.knn(q, g, int(k), off, block_rows=int(block_rows or 0))
+    finally:
+        ev.close()
+    return sim, index.long()
+
+
+def knn_merge(sims, indices, k):
+    """Merges the k-NN lists of the same queries over several gallery shards (each from Evaluator.knn with the shard's gallery_row0 and
+    a shared absmax) into the first k by knn's order: similarity descending with NaN last, then index ascending.  Takes sequences of
+    [nq, k_s] tensors on one device; stable sorts, so ties are decided by the index alone.  Returns (sim [nq, k], index [nq, k] int64)."""
+    s = torch.cat([t.to(torch.float32) for t in sims], dim=1)
+    ix = torch.cat([t.to(torch.int64) for t in indices], dim=1)
+    if not 1 <= int(k) <= s.shape[1]:
+        raise ValueError(f"knn_merge: k = {k} outside [1, {s.shape[1]}]")
+    order = torch.argsort(ix, dim=1, stable=True)
+    nan = torch.isnan(s)
+    key = torch.where(nan, torch.full_like(s, float("-inf")), s)
+    order = order.gather(1, torch.argsort(key.gather(1, order), dim=1, descending=True, stable=True))
+    order = order.gather(1, torch.argsort(nan.gather(1, order).to(torch.uint8), dim=1, stable=True))
+    order = order[:, :int(k)]
+    return s.gather(1, order), ix.gather(1, order)
