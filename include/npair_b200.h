@@ -323,6 +323,29 @@ int npair_eval_knn(npair_eval* ev, const float* d_query, int32_t nq, const float
 /* Device memory npair_eval_knn adds on top of the workspace: one block of S, 4 * block_rows * round_up(ng, 32) bytes (block_rows 0:
  * 1024).  0 for bad arguments (ng < 1, k outside [1, min(ng, NPAIR_EVAL_KNN_MAX_K)], block_rows not 0 or a multiple of 128). */
 size_t npair_eval_knn_bytes(int32_t ng, int32_t k, int32_t block_rows);
+/* Hard negative class mining (Sohn, "Improved Deep Metric Learning with Multi-class N-pair Loss Objective", NIPS 2016; DESIGN 8.4):
+ * each N-pair batch's classes chosen greedily from a pool.  d_class_emb: n_classes x D fp32, one row per class (n_classes <= both
+ * max_queries and max_gallery: the class set takes the A and the B format).  s(a, b) is the library's similarity of class rows a and b
+ * in `precision`, the pre-scale from max|x| over d_class_emb: the same bits as the layer's S and as npair_eval_knn self-retrieval.
+ * pools_host: n_batches HOST pools of pool_size distinct class ids in [0, n_classes), row-major.  Batch t, pool p = pools_host[t]:
+ *   position 0 is the seed, sel = {p[0]};
+ *   at steps 1 .. classes_per_batch - 1 every unselected position j scores v_j = max over c in sel of s(c, p[j]) (NaN ranks below
+ *   every number: v_j is NaN only when every term is), and the pick is the unselected j with the largest v_j, ties to the LOWEST j
+ *   (the maximum of the distinct keys (ord(v) << 32) | ~j, ord(NaN) = 0).  Pools drawn at random make that the paper's random tie-break.
+ * d_batches[t][0 .. classes_per_batch) = the class ids in the order picked; d_scores (may be NULL) the v each was picked at, NaN for the
+ * seed.  Batch t depends only on its pool, classes_per_batch and the bits of S: not on n_batches, the other pools, the stream, repeated
+ * calls or a fresh evaluator.  2 <= classes_per_batch <= pool_size <= NPAIR_EVAL_CLASS_POOL_MAX, n_batches >= 1; anything else, an id
+ * out of range, an id twice in one pool or a null pointer is NPAIR_E_ARG, checked on the host before anything is enqueued.
+ * The call prepares the operands, stores the whole n_classes x round_up(n_classes, 32) S in one sweep, uploads the pools and runs one
+ * greedy kernel, one block per batch.  Asynchronous on `stream`.  Device memory: on top of the workspace,
+ * npair_eval_class_batches_bytes(n_classes, pool_size, n_batches), grown on demand and kept until npair_eval_destroy. */
+#define NPAIR_EVAL_CLASS_POOL_MAX 16384
+int npair_eval_class_batches(npair_eval* ev, const float* d_class_emb, int32_t n_classes, const int32_t* pools_host /* [n_batches][pool_size] */,
+                             int32_t pool_size, int32_t n_batches, int32_t classes_per_batch,
+                             int32_t* d_batches /* [n_batches][classes_per_batch] */, float* d_scores /* may be NULL */, void* stream);
+/* Device memory npair_eval_class_batches adds on top of the workspace: 4 * n_classes * round_up(n_classes, 32) + 4 * n_batches *
+ * pool_size bytes.  0 for bad arguments (n_classes or n_batches < 1, pool_size outside [2, min(n_classes, NPAIR_EVAL_CLASS_POOL_MAX)]). */
+size_t npair_eval_class_batches_bytes(int32_t n_classes, int32_t pool_size, int32_t n_batches);
 
 #ifdef __cplusplus
 }

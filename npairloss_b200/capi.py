@@ -45,7 +45,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
-           "npair_eval_kmeans", "npair_eval_kmeans_bytes", "npair_eval_knn", "npair_eval_knn_bytes"]
+           "npair_eval_kmeans", "npair_eval_kmeans_bytes", "npair_eval_knn", "npair_eval_knn_bytes",
+           "npair_eval_class_batches", "npair_eval_class_batches_bytes"]
 
 _LIB = None
 
@@ -116,6 +117,9 @@ def lib():
         L.npair_eval_knn.argtypes = [vp, vp, i32, vp, i32, i32, i32, C.c_float, i32, i32, vp, vp, vp]
         L.npair_eval_knn_bytes.argtypes = [i32, i32, i32]
         L.npair_eval_knn_bytes.restype = C.c_size_t
+        L.npair_eval_class_batches.argtypes = [vp, vp, i32, vp, i32, i32, i32, vp, vp, vp]
+        L.npair_eval_class_batches_bytes.argtypes = [i32, i32, i32]
+        L.npair_eval_class_batches_bytes.restype = C.c_size_t
         _LIB = L
     return _LIB
 
@@ -261,6 +265,14 @@ def eval_knn_bytes(ng: int, k: int, block_rows: int = 0) -> int:
     return int(lib().npair_eval_knn_bytes(ng, k, block_rows))
 
 
+def eval_class_batches_bytes(n_classes: int, pool_size: int, n_batches: int) -> int:
+    """Device bytes Evaluator.class_batches adds on top of the workspace: the class set's whole S and the pools (0 if invalid)."""
+    return int(lib().npair_eval_class_batches_bytes(n_classes, pool_size, n_batches))
+
+
+CLASS_POOL_MAX = 16384   # NPAIR_EVAL_CLASS_POOL_MAX
+
+
 class Evaluator:
     """Retrieval evaluation (include/npair_b200.h, DESIGN 8): the rank of every query's best positive among the gallery, computed on
     the tensor cores without storing the similarity matrix.  Takes contiguous CUDA fp32 tensors; results are int32 / fp32 CUDA
@@ -335,6 +347,29 @@ class Evaluator:
                                          gallery_row0, C.c_float(absmax), int(k), block_rows, sim.data_ptr(), index.data_ptr(),
                                          torch.cuda.current_stream().cuda_stream))
         return sim, index
+
+    def class_batches(self, class_emb, pools, n, scores=True):
+        """npair_eval_class_batches (DESIGN 8.4): hard negative class mining over the rows of class_emb [C, D], one row per class.
+        pools: host int array [b, P] of distinct class ids per row (numpy, a CPU tensor or nested lists); batch t seeds with pools[t][0]
+        and adds, n - 1 times, the pool class whose largest similarity to the classes already picked is the largest (NaN last, ties to
+        the lower pool position).  Returns (int32 batches[b, n], fp32 scores[b, n] with NaN for the seed, or None when scores=False)."""
+        import numpy as np
+        import torch
+        p = np.asarray(pools.cpu() if isinstance(pools, torch.Tensor) else pools)
+        if p.ndim != 2 or p.dtype.kind not in "iu":
+            raise ValueError("pools must be a 2-D integer array [n_batches, pool_size]")
+        if p.dtype != np.int32:
+            if p.size and (p.min() < 0 or p.max() >= 2 ** 31):
+                raise ValueError("pool entries must be class ids")   # the library checks them against n_classes
+            p = p.astype(np.int32)
+        p = np.ascontiguousarray(p)
+        nb, dev = p.shape[0], class_emb.device
+        batches = torch.empty(nb, int(n), dtype=torch.int32, device=dev)
+        sc = torch.empty(nb, int(n), dtype=torch.float32, device=dev) if scores else None
+        self._check(lib().npair_eval_class_batches(self._h, self._arg(class_emb, 2), class_emb.shape[0], p.ctypes.data, p.shape[1], nb,
+                                                   int(n), batches.data_ptr(), sc.data_ptr() if scores else None,
+                                                   torch.cuda.current_stream().cuda_stream))
+        return batches, sc
 
     def map_at_r(self, query, qlabel, gallery, glabel, self_offset=-1):
         """npair_eval_map_at_r: fp64 map_r[nq] and r_precision[nq] (NaN where a query has no positive), int32 R[nq] and rank[nq]

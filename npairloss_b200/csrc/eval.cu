@@ -53,9 +53,9 @@ struct npair_eval : EvalPlan {
   int2* sym_tiles = nullptr;
   int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
   std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
-  // MAP@R (MapRows, MapPairs), k-means (KmeansBufs) and k-NN (KnnBlock) buffers, grown on demand and kept
-  DevMem map_rows_mem, map_pairs_mem, km_mem, knn_mem;
-  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr, *knn = nullptr;
+  // MAP@R (MapRows, MapPairs), k-means (KmeansBufs), k-NN (KnnBlock) and class-mining (ClassBatchBufs) buffers, grown on demand and kept
+  DevMem map_rows_mem, map_pairs_mem, km_mem, knn_mem, cb_mem;
+  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr, *knn = nullptr, *cb = nullptr;
   StreamOrder order;              // the calls' order across streams
   std::string err;
 };
@@ -102,6 +102,14 @@ static int knn_block_rows(int block_rows, int nq) {
   const long long rows = block_rows ? block_rows : KNN_DEFAULT_BLOCK_ROWS, cap = round_up(nq, 128);
   return static_cast<int>(rows < cap ? rows : cap);
 }
+// Class mining takes one: the whole S of the class set, C rows of round_up(C, 32) floats, then the pools [n_batches][pool_size]
+struct ClassBatchBufs : Carve {
+  float* S; long long ldS; int* pools;
+  ClassBatchBufs(char* base, long long C, long long pool_size, long long n_batches) : Carve{base}, ldS(round_up(C, 32)) {
+    S = take<float>(C * ldS); pools = take<int>(n_batches * pool_size);
+  }
+};
+static_assert(CLASS_POOL_MAX == NPAIR_EVAL_CLASS_POOL_MAX, "the greedy kernel's capacity is the call's limit on the pool size");
 
 // Grows the buffer `m` holds at *base to at least `bytes` (cudaFree of the old one waits for the device); `what` names it in errors
 static int eval_grow(npair_eval* ev, DevMem& m, char** base, size_t bytes, const char* what) {
@@ -140,6 +148,11 @@ size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
 size_t npair_eval_knn_bytes(int32_t ng, int32_t k, int32_t block_rows) {
   if (ng < 1 || k < 1 || k > NPAIR_EVAL_KNN_MAX_K || k > ng || block_rows < 0 || block_rows % 128) return 0;
   return KnnBlock(nullptr, block_rows ? block_rows : KNN_DEFAULT_BLOCK_ROWS, ng).bytes;
+}
+
+size_t npair_eval_class_batches_bytes(int32_t n_classes, int32_t pool_size, int32_t n_batches) {
+  if (n_classes < 1 || n_batches < 1 || pool_size < 2 || pool_size > n_classes || pool_size > NPAIR_EVAL_CLASS_POOL_MAX) return 0;
+  return ClassBatchBufs(nullptr, n_classes, pool_size, n_batches).bytes;
 }
 
 const char* npair_eval_last_error(const npair_eval* ev) { return ev ? ev->err.c_str() : g_create_err.c_str(); }
@@ -328,6 +341,52 @@ int npair_eval_knn(npair_eval* ev, const float* q, int32_t nq, const float* g, i
     CUDA_TRY(ev, launch_gemm(ev->prec, EPI_STORE_S, ta, tb, ta, gp, ev->sms, st));
     launch_knn_select(blk.S, blk.ldS, m, ng, k, r0, static_cast<int>(self_col), gallery_row0, d_sim, d_index, st);
   }
+  CUDA_TRY(ev, cudaGetLastError());
+  return NPAIR_OK;
+}
+
+// Hard negative class mining (DESIGN 8.4): the class set's operands, the whole S of the class set by the store-only sweep (the k-NN
+// block code with one block, full tiles), the pools, and one greedy block per batch over S.
+int npair_eval_class_batches(npair_eval* ev, const float* x, int32_t C, const int32_t* pools, int32_t P, int32_t nb, int32_t n,
+                             int32_t* d_batches, float* d_scores, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  if (!x || !pools || !d_batches) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (C < 1 || C > ev->max_q || C > ev->max_g) {
+    ev->err = fmt("n_classes = %d must lie in [1, %d]: the evaluator's capacity (%d, %d)", C, ev->max_q < ev->max_g ? ev->max_q : ev->max_g,
+                  ev->max_q, ev->max_g);
+    return NPAIR_E_ARG;
+  }
+  if (P < 2 || P > C || P > NPAIR_EVAL_CLASS_POOL_MAX) {
+    ev->err = fmt("pool_size = %d must lie in [2, %d] (n_classes = %d, NPAIR_EVAL_CLASS_POOL_MAX = %d)", P,
+                  C < NPAIR_EVAL_CLASS_POOL_MAX ? C : NPAIR_EVAL_CLASS_POOL_MAX, C, NPAIR_EVAL_CLASS_POOL_MAX);
+    return NPAIR_E_ARG;
+  }
+  if (n < 2 || n > P) { ev->err = fmt("classes_per_batch = %d must lie in [2, pool_size = %d]", n, P); return NPAIR_E_ARG; }
+  if (nb < 1) { ev->err = "n_batches must be >= 1"; return NPAIR_E_ARG; }
+  std::vector<int> seen(C, -1);   // the last pool each class appeared in
+  for (int t = 0; t < nb; ++t)
+    for (int j = 0; j < P; ++j) {
+      const int id = pools[static_cast<long long>(t) * P + j];
+      if (id < 0 || id >= C) { ev->err = fmt("pool %d position %d: class %d is not in [0, %d)", t, j, id, C); return NPAIR_E_ARG; }
+      if (seen[id] == t) { ev->err = fmt("pool %d holds class %d twice", t, id); return NPAIR_E_ARG; }
+      seen[id] = t;
+    }
+  int rc;
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
+  if ((rc = eval_grow(ev, ev->cb_mem, &ev->cb, ClassBatchBufs(nullptr, C, P, nb).bytes, "the class set's S and the pools")) != NPAIR_OK)
+    return rc;
+  const ClassBatchBufs cb(ev->cb, C, P, nb);
+  if ((rc = eval_prepare(ev, x, C, x, C, -1.f, false, st)) != NPAIR_OK) return rc;
+  CUtensorMap ta, tb;
+  std::string te;
+  if (!make_tmap_kcat(&ta, &tb, ev->catA, C, ev->catB, C, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
+  GemmParams gp = sim_sweep(EPI_STORE_S, C, C, ev->kcat, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
+  gp.a_row0 = 0; gp.S = cb.S; gp.ldS = cb.ldS;
+  CUDA_TRY(ev, launch_gemm(ev->prec, EPI_STORE_S, ta, tb, ta, gp, ev->sms, st));
+  CUDA_TRY(ev, cudaMemcpyAsync(cb.pools, pools, sizeof(int32_t) * nb * P, cudaMemcpyHostToDevice, st));
+  launch_class_batches(cb.S, cb.ldS, cb.pools, P, nb, n, d_batches, d_scores, ev->sms, st);
   CUDA_TRY(ev, cudaGetLastError());
   return NPAIR_OK;
 }

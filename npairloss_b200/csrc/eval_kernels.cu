@@ -326,4 +326,89 @@ void launch_km_inertia(const float* x, const float* C, const int* assign, int n,
   count_launch(2);
 }
 
+// --------------------------------------------------------------------------------------------
+// hard negative class mining (npair_eval_class_batches, DESIGN 8.4): the greedy pick of each batch's classes from the stored S
+// --------------------------------------------------------------------------------------------
+// The maximum of a 64-bit key over the warp: of the high words, then of the low words among the lanes that hold the maximal high word
+__device__ __forceinline__ unsigned long long warp_max_key(unsigned long long key) {
+  const uint32_t hi = static_cast<uint32_t>(key >> 32), mh = __reduce_max_sync(0xffffffffu, hi);
+  const uint32_t ml = __reduce_max_sync(0xffffffffu, hi == mh ? static_cast<uint32_t>(key) : 0u);
+  return (static_cast<unsigned long long>(mh) << 32) | ml;
+}
+
+// One block of round_up(ceil(P / CB_ENTRIES), 32) threads per batch, as many as the SMs hold at once; the grid strides over the batches.
+// Pool position j = tid + e * blockDim.x (e < CB_ENTRIES) lives in thread tid's registers: its
+// class id[e] (-1 once picked, and past the pool) and v[e], the fmaxf of S over the picked classes' rows (NaN before the first term).
+// A step gathers the last pick's row of S at every live id, all loads in flight together, folds them into v, and takes the block
+// maximum of the distinct keys (ord(v) << 32) | ~j, ord(NaN) = 0, with 0 for a picked entry: a live key is never 0, since ~j has its
+// top bits set.  Warp maxima, one shared-memory stage across the warps, and the winner's owner hands its class to every thread through
+// shared memory: two barriers per step.  Keys are distinct, so the pick does not depend on the reduction order.
+__global__ void __launch_bounds__(CB_THREADS) class_batch_kernel(const float* __restrict__ S, long long ldS, const int* __restrict__ pools,
+                                                                 int P, int nb, int n, int* __restrict__ batches,
+                                                                 float* __restrict__ scores) {
+  __shared__ unsigned long long s_key[CB_THREADS / 32];
+  __shared__ int s_pick;
+  const int tid = threadIdx.x, lane = tid & 31, T = blockDim.x;
+  const float qnan = __uint_as_float(0x7FC00000u);
+  for (int t = blockIdx.x; t < nb; t += gridDim.x) {
+    const int* pool = pools + static_cast<long long>(t) * P;
+    int* out = batches + static_cast<long long>(t) * n;
+    float* out_v = scores ? scores + static_cast<long long>(t) * n : nullptr;
+    int id[CB_ENTRIES];
+    float v[CB_ENTRIES];
+#pragma unroll
+    for (int e = 0; e < CB_ENTRIES; ++e) {
+      const int j = tid + e * T;
+      id[e] = j > 0 && j < P ? __ldg(pool + j) : -1;       // position 0, the seed, is picked
+      v[e] = qnan;
+    }
+    int c = __ldg(pool);
+    if (tid == 0) {
+      out[0] = c;
+      if (out_v) out_v[0] = qnan;
+    }
+    for (int s = 1; s < n; ++s) {
+      const float* row = S + static_cast<long long>(c) * ldS;
+      float x[CB_ENTRIES];
+#pragma unroll
+      for (int e = 0; e < CB_ENTRIES; ++e) x[e] = id[e] >= 0 ? __ldg(row + id[e]) : qnan;
+      unsigned long long best = 0;
+#pragma unroll
+      for (int e = 0; e < CB_ENTRIES; ++e) {
+        v[e] = fmaxf(v[e], x[e]);
+        const unsigned long long key = (static_cast<unsigned long long>(v[e] != v[e] ? 0u : f2ord(v[e])) << 32) |
+                                       static_cast<uint32_t>(~(tid + e * T));
+        if (id[e] >= 0 && key > best) best = key;
+      }
+      best = warp_max_key(best);
+      if (lane == 0) s_key[tid >> 5] = best;
+      __syncthreads();
+      best = warp_max_key(lane < (T >> 5) ? s_key[lane] : 0ull);
+      const int win = static_cast<int>(~static_cast<uint32_t>(best));
+      int picked = -1;
+#pragma unroll
+      for (int e = 0; e < CB_ENTRIES; ++e)
+        if (tid + e * T == win) { picked = id[e]; id[e] = -1; }
+      if (picked >= 0) {
+        s_pick = picked;
+        out[s] = picked;
+        const uint32_t o = static_cast<uint32_t>(best >> 32);
+        if (out_v) out_v[s] = o ? ord2f(o) : qnan;
+      }
+      __syncthreads();
+      c = s_pick;
+    }
+  }
+}
+void launch_class_batches(const float* S, long long ldS, const int* pools, int P, int nb, int n, int* batches, float* scores, int sms,
+                          cudaStream_t st) {
+  static_assert(CB_THREADS * CB_ENTRIES >= CLASS_POOL_MAX, "one block holds the largest pool");
+  const int threads = ((P + CB_ENTRIES - 1) / CB_ENTRIES + 31) / 32 * 32;
+  int per_sm = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, class_batch_kernel, threads, 0);
+  const long long cap = static_cast<long long>(sms) * (per_sm > 0 ? per_sm : 1);
+  class_batch_kernel<<<static_cast<int>(nb < cap ? nb : cap), threads, 0, st>>>(S, ldS, pools, P, nb, n, batches, scores);
+  count_launch();
+}
+
 }  // namespace npair

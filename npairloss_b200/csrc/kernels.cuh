@@ -307,5 +307,13 @@ void launch_km_assign(unsigned long long* best, const float* x, int n, int D, co
 void launch_km_update(long long* sums, const int* counts, const unsigned int* absmax_bits, int k, int D, float* C, cudaStream_t st);
 // *out = sum_i ||x_i - C[assign[i]]||^2 in fp64, in a fixed order (partial: KM_INERTIA_BLOCKS doubles of scratch)
 void launch_km_inertia(const float* x, const float* C, const int* assign, int n, int D, double* partial, double* out, cudaStream_t st);
+// Hard negative class mining (npair_eval_class_batches, DESIGN 8.4): for each of the nb pools (pools [nb][P], P <= CLASS_POOL_MAX,
+// distinct ids < the rows of S), the greedy batch of n >= 2 classes over the stored S (row c = class c, stride ldS) into batches
+// [nb][n] and, unless NULL, the scores they were picked at into scores [nb][n] (NaN for the seed).  One block per batch, CB_ENTRIES
+// pool positions per thread in registers, at most sms times the blocks an SM holds.
+constexpr int CB_THREADS = 1024, CB_ENTRIES = 16;
+constexpr int CLASS_POOL_MAX = 16384;
+void launch_class_batches(const float* S, long long ldS, const int* pools, int P, int nb, int n, int* batches, float* scores, int sms,
+                          cudaStream_t st);
 
 }  // namespace npair

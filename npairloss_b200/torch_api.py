@@ -19,6 +19,8 @@ the backward refuses to run against a newer forward.
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import capi
@@ -281,3 +283,60 @@ def knn_merge(sims, indices, k):
     order = order.gather(1, torch.argsort(nan.gather(1, order).to(torch.uint8), dim=1, stable=True))
     order = order[:, :int(k)]
     return s.gather(1, order), ix.gather(1, order)
+
+
+def hard_class_batches(class_emb, classes_per_batch, num_batches, pool_size=None, seed=0, precision=capi.PREC_FP32_FP16X2):
+    """Hard negative class mining (Sohn 2016; Evaluator.class_batches, DESIGN 8.4; not part of the reference layer): the classes of
+    num_batches N-pair batches, each chosen greedily from a random pool by the library's similarity of the class embeddings.
+
+    class_emb: CUDA fp32 [C, D], one row per class (class_embeddings makes them from example embeddings).  Pool t is
+    torch.randperm(C, generator=g)[:pool_size] for t = 0, 1, ... in order, g = torch.Generator().manual_seed(seed); pool_size=None is
+    min(C, capi.CLASS_POOL_MAX).  Batch t seeds with pool t's first class, then adds, classes_per_batch - 1 times, the pool class whose
+    largest similarity to the classes already in the batch is the largest (a NaN similarity ranks last; ties go to the earlier pool
+    position, a random tie-break since pools are random).  Returns (batches [num_batches, classes_per_batch] int64 class indices in the
+    order picked, scores [num_batches, classes_per_batch] fp32: the similarity each class was picked at, NaN for the seed), CUDA tensors."""
+    x = _embeddings("hard_class_batches", class_emb)
+    C, D = x.shape
+    P = min(C, capi.CLASS_POOL_MAX) if pool_size is None else int(pool_size)
+    g = torch.Generator().manual_seed(int(seed))
+    pools = torch.stack([torch.randperm(C, generator=g)[:P] for _ in range(int(num_batches))]) if int(num_batches) > 0 \
+        else torch.empty(0, P, dtype=torch.int64)
+    ev = capi.Evaluator(C, C, D, precision, x.device.index or 0)
+    try:
+        batches, scores = ev.class_batches(x, pools, int(classes_per_batch))
+    finally:
+        ev.close()
+    return batches.long(), scores
+
+
+def class_embeddings(emb, labels, normalize=True):
+    """One embedding per class: the mean of its examples' rows, for hard_class_batches.  Returns (class_labels fp32 [C] ascending,
+    class_emb fp32 [C, D]), row c the class class_labels[c].
+
+    The mean is the fixed-point rule of the k-means update (DESIGN 8.2): with sigma the pre-scale of max|x| over emb (a power of two
+    with max|x * sigma| in [0.5, 1)), int64 sums of rint(x * sigma * 2^32), exact and independent of order, then
+    (float)(ldexp(sum / count, -32) / sigma); so the result has the same bits on every run and device.  Labels of any numeric dtype
+    that fp32 holds exactly; NaN labels raise ValueError.  normalize=True then L2-normalises each row (npair_l2normalize_forward, CUDA
+    only); normalize=False also takes CPU tensors."""
+    if emb.dtype != torch.float32:
+        raise TypeError("class_embeddings takes float32 embeddings")
+    x = emb.reshape(emb.shape[0], -1).contiguous()
+    if normalize and not x.is_cuda:
+        raise TypeError("class_embeddings(normalize=True) takes CUDA embeddings (the normalisation has no CPU path)")
+    lab = _fp32_labels(labels.reshape(-1).to(x.device))
+    if lab.numel() != x.shape[0]:
+        raise ValueError("emb and labels differ in length")
+    if bool(torch.isnan(lab).any()):
+        raise ValueError("class_embeddings: a NaN label belongs to no class")
+    amax = float(x.abs().max()) if x.numel() else 0.0
+    if not math.isfinite(amax):
+        raise ValueError("class_embeddings takes finite embeddings")
+    e = math.frexp(amax)[1] if amax > 0 else 0
+    class_labels, cls = torch.unique(lab, sorted=True, return_inverse=True)
+    q = torch.round((x * (2.0 ** -e)).double() * 2.0 ** 32).long()          # x * sigma and the scaling by 2^32 are exact
+    sums = torch.zeros(class_labels.numel(), x.shape[1], dtype=torch.int64, device=x.device).index_add_(0, cls, q)
+    count = torch.bincount(cls, minlength=class_labels.numel()).double()
+    mean = ((sums.double() / count[:, None]) * 2.0 ** -32 * 2.0 ** e).float()
+    if normalize:
+        mean = capi.l2normalize_forward(mean)[0]
+    return class_labels, mean
