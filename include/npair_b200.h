@@ -182,6 +182,34 @@ int npair_backward_partial(npair_ctx* ctx, float loss_weight, float* d_local_hal
 int npair_row_scalars(npair_ctx* ctx, float* d_out_8Q, void* stream);
 int npair_backward_gathered(npair_ctx* ctx, float loss_weight, const float* d_rs_total, float* d_feat_diff, void* stream);
 
+/* ---- cross-batch memory, not part of the reference layer (Wang et al., "Cross-Batch Memory for Embedding Learning", CVPR 2020;
+ * DESIGN 4.3) ----
+ * A world-1 context whose forward may take, besides the current batch x (Q x D) and its labels, m <= max_memory_rows memory rows
+ * x_mem (m x D fp32) with labels (m fp32): embeddings of earlier batches that the caller keeps.  The database is X_total = [x; x_mem],
+ * N = Q + m; the anchors are rows 0 .. Q-1 only (anchor i's self column is i).  S = x . X_total^T (Q x N) in the context's operand
+ * format, with the fp16x2 pre-scale from max|x| over both sets; every mining rule, region, threshold, the row pass, the tops and the
+ * loss normaliser Q are those of the reference's rank-0 block over N columns (the GLOBAL region is the Q x N block, the retrieval
+ * counters rank over N - 1 columns); feature_asum covers the current rows only.  The backward (npair_backward, npair_backward_partial
+ * with d_total_half NULL) returns for the current rows (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x), the reference's world-1 blend with
+ * the transposed term not divided by anything; the memory rows get no gradient.  A call's results depend only on the configuration,
+ * Q, m and the inputs: not on max_memory_rows, earlier calls or the rows a call with a larger m left behind.  The forward reads
+ * d_mem_feat / d_mem_label and nothing later does: the caller may overwrite them in stream order once npair_forward_memory returns
+ * (the current batch stays under the rule of npair_forward).  normalize_input normalises the current rows; memory rows are used as
+ * given (keep the normalised rows the layer saw, npair_l2normalize_forward).  After a forward with m > 0, npair_debug_read(0) returns
+ * the Q x (Q + m) S with ld = Q + m.
+ * Accepted: the tensor-core backend (fused gradient kernel or NPAIR_FLAG_NO_FUSED_GRAD), every operand format, every mining
+ * combination, normalize_input.  NPAIR_E_ARG, at creation (max_memory_rows > 0) or at the call, checked on the host before anything
+ * is enqueued: world > 1, row-block similarity mode, the SIMT backend, global_scope, m < 0, m > max_memory_rows, or a null memory
+ * pointer with m > 0.
+ *   npair_create_memory           : a context for up to max_memory_rows memory rows; max_memory_rows = 0 is npair_create(cfg, NULL, out)
+ *   npair_memory_workspace_bytes  : its device memory (as npair_workspace_bytes; equal to it for max_memory_rows = 0, 0 when refused)
+ *   npair_forward_memory          : npair_forward over [x; x_mem].  m = 0 is npair_forward, bit for bit.  Then npair_backward,
+ *                                   npair_backward_partial (world 1) and npair_row_scalars work as after npair_forward. */
+int npair_create_memory(const npair_config* cfg, int32_t max_memory_rows, npair_ctx** out);
+size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows);
+int npair_forward_memory(npair_ctx* ctx, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label,
+                         int32_t m, float tops_host[5], void* stream);
+
 /* The L2Normalize producer layer of the reference net (usage/def.prototxt:115-120; its source is not part of the reference tree):
  * y[r][:] = x[r][:] / ||x[r][:]||_2 (a zero row stays zero), and its backward dx = (dy - y (y . dy)) / ||x||.  Stand-alone entry
  * points for a host framework's own L2Normalize layer; npair_config.normalize_input = 1 runs the same kernels inside

@@ -42,6 +42,8 @@ def sim_block_flags(rows: int) -> int:
 EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_id", "npair_create", "npair_create_with_comm",
            "npair_destroy", "npair_forward", "npair_backward", "npair_forward_backward", "npair_forward_gathered", "npair_backward_partial", "npair_bwd_exchange_mode", "npair_row_scalars", "npair_backward_gathered", "npair_profile_enable", "npair_profile_read", "npair_kernel_launches", "npair_util_f64_to_f32", "npair_util_f32_to_f64", "npair_last_error", "npair_version", "npair_debug_read",
            "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
+           # cross-batch memory (not part of the reference layer)
+           "npair_create_memory", "npair_memory_workspace_bytes", "npair_forward_memory",
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
@@ -82,6 +84,10 @@ def lib():
         L.npair_destroy.argtypes = [vp]
         L.npair_destroy.restype = None
         L.npair_forward.argtypes = [vp, vp, vp, fp, vp]
+        L.npair_create_memory.argtypes = [C.POINTER(NpairConfig), C.c_int32, C.POINTER(vp)]
+        L.npair_memory_workspace_bytes.argtypes = [C.POINTER(NpairConfig), C.c_int32]
+        L.npair_memory_workspace_bytes.restype = C.c_size_t
+        L.npair_forward_memory.argtypes = [vp, vp, vp, vp, vp, C.c_int32, fp, vp]
         L.npair_backward.argtypes = [vp, C.c_float, vp, vp]
         L.npair_forward_gathered.argtypes = [vp, vp, vp, fp, vp]
         L.npair_backward_partial.argtypes = [vp, C.c_float, vp, vp, vp]
@@ -143,15 +149,27 @@ def nccl_unique_id() -> bytes:
     return buf.raw
 
 
-class Context:
-    """One per rank.  forward()/backward() take torch CUDA tensors (device pointers) and return host scalars."""
+def memory_workspace_bytes(cfg: NpairConfig, memory_rows: int) -> int:
+    """Device bytes a Context(cfg, memory_rows=memory_rows) allocates (npair_memory_workspace_bytes; 0 for a refused configuration)."""
+    return int(lib().npair_memory_workspace_bytes(C.byref(cfg), int(memory_rows)))
 
-    def __init__(self, cfg: NpairConfig, nccl_id: bytes | None = None):
+
+class Context:
+    """One per rank.  forward()/backward() take torch CUDA tensors (device pointers) and return host scalars.
+    memory_rows > 0: a cross-batch memory context (npair_create_memory, DESIGN 4.3) whose forward_memory takes up to that many rows."""
+
+    def __init__(self, cfg: NpairConfig, nccl_id: bytes | None = None, memory_rows: int = 0):
         L = lib()
         self.cfg = cfg
+        self.memory_rows = int(memory_rows)
         self._h = C.c_void_p()
         idbuf = C.create_string_buffer(nccl_id, 128) if nccl_id is not None else None
-        rc = L.npair_create(C.byref(cfg), idbuf, C.byref(self._h))
+        if self.memory_rows > 0:
+            if nccl_id is not None:
+                raise ValueError("a cross-batch memory context is a world-1 context: it takes no NCCL id")
+            rc = L.npair_create_memory(C.byref(cfg), self.memory_rows, C.byref(self._h))
+        else:
+            rc = L.npair_create(C.byref(cfg), idbuf, C.byref(self._h))
         if rc:
             raise NpairError(rc, L.npair_last_error(None).decode())
 
@@ -197,6 +215,27 @@ class Context:
         assert feat.is_cuda and label.is_cuda and feat.dtype == torch.float32 and label.dtype == torch.float32
         assert feat.is_contiguous() and label.is_contiguous()
         return self.forward_ptr(feat.data_ptr(), label.data_ptr(), torch.cuda.current_stream().cuda_stream)
+
+    def forward_memory_ptr(self, feat_ptr: int, label_ptr: int, mem_feat_ptr, mem_label_ptr, m: int, stream: int = 0):
+        tops = (C.c_float * 5)()
+        self._check(lib().npair_forward_memory(self._h, feat_ptr, label_ptr, mem_feat_ptr, mem_label_ptr, int(m), tops, stream))
+        return [tops[i] for i in range(5)]
+
+    def forward_memory(self, feat, label, mem_feat, mem_label, m=None):
+        """npair_forward_memory: the forward over [feat; mem_feat[:m]] with anchors feat only (m = None: all rows of mem_feat).
+        mem_feat / mem_label may be None for m = 0; the library reads them during this call only."""
+        import torch
+        assert feat.is_cuda and label.is_cuda and feat.dtype == torch.float32 and label.dtype == torch.float32
+        assert feat.is_contiguous() and label.is_contiguous()
+        if m is None:
+            m = 0 if mem_feat is None else mem_feat.shape[0]
+        mp = lp = None
+        if mem_feat is not None:
+            assert mem_feat.is_cuda and mem_feat.dtype == torch.float32 and mem_feat.is_contiguous() and mem_feat.shape[0] >= m
+            assert mem_label is not None and mem_label.is_cuda and mem_label.dtype == torch.float32 and mem_label.is_contiguous()
+            assert mem_label.shape[0] >= m
+            mp, lp = mem_feat.data_ptr(), mem_label.data_ptr()
+        return self.forward_memory_ptr(feat.data_ptr(), label.data_ptr(), mp, lp, m, torch.cuda.current_stream().cuda_stream)
 
     def backward(self, loss_weight, diff):
         import torch

@@ -256,6 +256,7 @@ struct Plan {
   int grad_chunk_kb;             // accumulation chunk of the gradient GEMM in 32-column K blocks (grad_fused.cuh); 0 = unchunked
   int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
   SplitK grad_split;             // and its split-K
+  int split_cap;                 // split_k_cap of that K: a memory context's partial buffer holds this many slices, enough for any m <= M
   int n_sym_tiles;
   int s_rows;                    // rows of the S buffer: all Q (S materialised), or one block in row-block similarity mode
   int n_blocks;                  // blocks of s_rows rows that the row pass and the fused gradient walk; 1: S materialised
@@ -266,10 +267,12 @@ struct Plan {
   XchgLayout xl;
 };
 
-static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
+// mem_rows: the cross-batch memory rows m of a world-1 step (DESIGN 4.3), database columns Q + m; a memory context's buffers are
+// those of its capacity M, and each call re-plans what depends on the call's own N (set_call_rows)
+static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric, int mem_rows = 0) {
   Plan p{};
   const int prec = cfg.sim_precision, W = cfg.world;
-  const long long Q = cfg.Q, D = cfg.D, N = Q * W;
+  const long long Q = cfg.Q, D = cfg.D, N = Q * W + mem_rows;
   const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
   p.N = static_cast<int>(N);
   p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_grad = bk_of(prec, EPI_OUT);
@@ -300,7 +303,9 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
   p.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
   const int tiles = tile_sched(cfg.Q, cfg.D, p.grad_kblocks).num_tiles();
   p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
-  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES)) p.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, p.N));
+  p.split_cap = tc ? split_k_cap(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : 1;
+  // memory rows are no anchors: S is not symmetric, every tile is computed
+  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES) && mem_rows == 0) p.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, p.N));
   p.sweep_epi = EPI_STATS | (p.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
   p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
   p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
@@ -310,12 +315,13 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric) {
 
 // ------------------------------------------------------------------------------------------------ device memory
 // A context's RowArrays: the statistics, thresholds, row results and [3][Q] hit flags, then the row records 32-byte aligned
-static void carve_rows(Carve& cv, long long Q, RowArrays* ra) {
+// (a memory context's record table: the Q row records followed by the records of up to M memory rows)
+static void carve_rows(Carve& cv, long long Q, long long mem_cap, RowArrays* ra) {
   carve_stats(cv, Q, ra);
   ra->posi_thr = cv.take<float>(Q); ra->nega_thr = cv.take<float>(Q);
   ra->A = cv.take<float>(Q); ra->T = cv.take<float>(Q); ra->logv = cv.take<float>(Q);
   ra->hits = cv.take<int>(3 * Q);
-  ra->rowrec = cv.take<RowRecord>(Q, 32);
+  ra->rowrec = cv.take<RowRecord>(Q + mem_cap, 32);
 }
 
 // ------------------------------------------------------------------------------------------------ context
@@ -323,6 +329,9 @@ static void carve_rows(Carve& cv, long long Q, RowArrays* ra) {
 struct npair_ctx : Plan {
   npair_config cfg;
   int Q, D, world, rank, prec, sms, device;
+  int mem_cap = 0;               // cross-batch memory: the most memory rows a call may pass (npair_create_memory), 0 without
+  int mem_rows = 0;              // the memory rows the N-dependent part of the plan and the tensor maps are set for (set_call_rows)
+  float* labcat = nullptr;       // memory context: the labels of the current rows and the memory rows, [Q + M]
   DevMem mem;                    // owns the device scratch below (ctx_buffers, p2p_buffers)
   float* Xtot_buf = nullptr;     // world > 1: all-gather target
   float* labtot_buf = nullptr;
@@ -364,6 +373,9 @@ struct npair_ctx : Plan {
     bool ext_gathered = false;     // through npair_forward_gathered: the caller did the collectives
     bool rec_gathered = false;     // the NCCL all-gather of the row records has been enqueued (at the first backward)
     bool fwd_done = false;         // the forward succeeded: a backward may follow
+    // cross-batch memory (npair_forward_memory with m > 0): the caller's memory rows and labels.  Only the forward reads them; the
+    // backward only tests x_mem for whether the step had memory rows
+    const float *x_mem = nullptr, *lab_mem = nullptr;
   } step;
   StreamOrder order;              // the calls' order across streams; debug_read and profile_read wait for its event
   std::string err;
@@ -378,22 +390,27 @@ struct npair_ctx : Plan {
 static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   const long long Q = c->cfg.Q, D = c->cfg.D, N = c->N;
   const size_t f = sizeof(float), ns = c->nsplit;
+  if (c->mem_cap) m.own(&c->labcat, f * N, false);                                      // [x; x_mem]'s labels
   if (c->cfg.world > 1) { m.own(&c->Xtot_buf, f * N * D, false); m.own(&c->labtot_buf, f * N, false); }   // all-gather targets
   if (c->cfg.normalize_input) { m.own(&c->Ynorm, f * Q * D, false); m.own(&c->dY, f * Q * D, false); m.own(&c->inv_norm, f * Q, false); }   // y, dy, 1/||x||
   m.own(&c->S, f * c->s_rows * c->ldS, true);
   if (!c->cat) m.own(&c->Xs, 2 * ns * N * c->Dp, true);                              // operand pieces [ns][N][Dp]
   m.own(&c->XsT, 2 * ns * D * c->Np, true);                                           // transposed pieces [ns][D][Np]
-  if (c->cat) { m.own(&c->XcatA, 2 * N * c->kcat, true); m.own(&c->XcatB, 2 * N * c->kcat, true); }   // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  if (c->cat) { m.own(&c->XcatA, 2 * Q * c->cfg.world * c->kcat, true); m.own(&c->XcatB, 2 * N * c->kcat, true); }   // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3); A: anchors only
   if (!c->fused_grad) m.own(&c->H, 2 * ns * Q * c->Np, true);                        // materialised gradient weights
   if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) { m.own(&c->XlT, 2 * ns * D * c->Qp, true); m.own(&c->HT, 2 * ns * N * c->Qp, true); m.own(&c->OUT2, f * N * D, false); }
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) m.own(&c->rs_total, sizeof(RowRecord) * N, false);   // gathered row records
-  if (c->grad_split.splits > 1) m.own(&c->part, f * split_part(c->grad_split.splits, c->cfg.Q, D), false);   // split-K partial products
-  m.own_carved(true, [c](Carve& cv) { carve_rows(cv, c->cfg.Q, &c->ra); });
+  // split-K partial products.  A memory context's calls take the split-K of their own N = Q + m (set_call_rows), which is not monotone
+  // in m: the buffer holds split_cap slices of the capacity's N, a bound of every smaller N's count
+  const int slices = c->mem_cap ? c->split_cap : c->grad_split.splits;
+  if (slices > 1) m.own(&c->part, f * split_part(slices, c->cfg.Q, D), false);
+  m.own_carved(true, [c](Carve& cv) { carve_rows(cv, c->cfg.Q, c->mem_cap, &c->ra); });
   m.own(&c->bs, sizeof(BlockScalars), true);
   m.own(&c->partial, f * 2048, false);
   m.own(&c->ghist, sizeof(unsigned long long) * 4096, true);
   m.own(&c->gcand, sizeof(uint32_t) * 2ull * c->gcand_cap, false);
-  m.own(&c->sym_tiles, sizeof(int2) * c->n_sym_tiles, false);
+  // a memory context mirrors tiles in its calls with m = 0 only
+  m.own(&c->sym_tiles, sizeof(int2) * (c->mem_cap ? sym_tile_count(c->cfg.Q, c->cfg.Q) : c->n_sym_tiles), false);
   if (c->wscope) { m.own(&c->xch_src, f * NPAIR_XCH_FLOATS, false); m.own(&c->xch_all, f * NPAIR_XCH_FLOATS * c->cfg.world, false); }   // the latter for NCCL
   return m.err;
 }
@@ -463,6 +480,18 @@ static int validate(const npair_config* c, std::string* err) {
   return NPAIR_OK;
 }
 
+// Cross-batch memory (DESIGN 4.3) of up to M rows: a world-1 step on the tensor cores over one materialised S, per-rank mining
+static int validate_memory(const npair_config* c, long long M, std::string* err) {
+  if (M < 0) { *err = "max_memory_rows must be >= 0"; return NPAIR_E_ARG; }
+  if (M == 0) return NPAIR_OK;
+  if (c->world != 1) { *err = "a cross-batch memory needs world = 1"; return NPAIR_E_ARG; }
+  if (c->gemm_backend != NPAIR_GEMM_TCGEN05) { *err = "a cross-batch memory needs the tensor-core backend"; return NPAIR_E_ARG; }
+  if (sim_block_rows(*c)) { *err = "a cross-batch memory does not support row-block similarity mode"; return NPAIR_E_ARG; }
+  if (c->global_scope) { *err = "a cross-batch memory does not support global_scope"; return NPAIR_E_ARG; }
+  if (c->Q + M > 0x7fffffffLL) { *err = "Q + max_memory_rows exceeds int32"; return NPAIR_E_ARG; }
+  return NPAIR_OK;
+}
+
 extern "C" {
 
 const char* npair_version(void) { return "npairloss_b200 0.1 (abi 1; sm_90a wgmma/TMA)"; }
@@ -477,17 +506,19 @@ void npair_config_default(npair_config* c, int32_t Q, int32_t D) {
   c->global_scope = 0; c->normalize_input = 0; c->grad_chunk_cols = 0; c->flags = 0;
 }
 
-size_t npair_workspace_bytes(const npair_config* cfg) {
+size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows) {
   std::string e;
-  if (validate(cfg, &e) != NPAIR_OK) return 0;
+  if (validate(cfg, &e) != NPAIR_OK || validate_memory(cfg, max_memory_rows, &e) != NPAIR_OK) return 0;
   npair_ctx c;
   c.cfg = *cfg;
-  static_cast<Plan&>(c) = plan_of(*cfg, NPAIR_H100_SXM_SMS, true);
+  c.mem_cap = max_memory_rows;
+  static_cast<Plan&>(c) = plan_of(*cfg, NPAIR_H100_SXM_SMS, true, max_memory_rows);
   DevMem sizing(false);
   ctx_buffers(&c, sizing);
   if (c.want_p2p_feat || c.want_p2p_rec) p2p_buffers(&c, sizing);   // as if the context had a communicator and peer access
   return sizing.bytes;
 }
+size_t npair_workspace_bytes(const npair_config* cfg) { return npair_memory_workspace_bytes(cfg, 0); }
 
 const char* npair_last_error(const npair_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
 
@@ -513,7 +544,7 @@ void npair_destroy(npair_ctx* c) {
   delete c;
 }
 
-static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, npair_ctx** out);
+static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out);
 // One-off device check (per process, device and operand format): a 192 x 192 similarity matrix computed with EVERY tile (no mirroring)
 // must come out bitwise symmetric.
 static bool mma_is_symmetric(int prec, int device) {
@@ -529,7 +560,7 @@ static bool mma_is_symmetric(int prec, int device) {
   npair_config_default(&cfg, Q, D);
   cfg.sim_precision = prec; cfg.device = device; cfg.flags = NPAIR_INTERNAL_FULL_TILES; cfg.num_tops = 2;
   npair_ctx* t = nullptr;
-  if (create_impl(&cfg, nullptr, nullptr, &t) == NPAIR_OK) {
+  if (create_impl(&cfg, nullptr, nullptr, 0, &t) == NPAIR_OK) {
     std::vector<float> x(static_cast<size_t>(Q) * D), lab(Q), S(static_cast<size_t>(Q) * t->ldS);
     uint32_t rng = 12345u;
     for (int r = 0; r < Q; ++r) {
@@ -559,17 +590,61 @@ static bool mma_is_symmetric(int prec, int device) {
   return ok;
 }
 
-static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, npair_ctx** out) {
+// The tensor maps over the operands, S and the gradient weights, whose column (or row) extents are the context's current N
+static bool make_maps(npair_ctx* c, std::string* te) {
+  const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit, bkg = c->bk_grad;
+  // similarity: A = the rank's rows, B = all rows of the K-concatenated operands (PREC_BF16: Xs, whose one piece is that format)
+  const uint16_t* catA = c->cat ? c->XcatA : c->Xs;
+  const uint16_t* catB = c->cat ? c->XcatB : c->Xs;
+  bool ok = make_tmap_kcat(&c->tm_simA, &c->tm_simB, catA +static_cast<long long>(c->rank) * Q * c->kcat, Q, catB, N, c->kcat, te);
+  ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, c->s_rows, c->ldS, te);
+  // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
+  if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, te);
+  ok = ok && make_tmap_pieces(&c->tm_b1B, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, bkg, 256, te);
+  if (c->fused_grad) {
+    ok = ok && make_tmap_pieces(&c->tm_fB, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, te);
+    ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, te, 128);
+  }
+  if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) {   // gradient 2: A = HT [N x Q], B = XlT [D x Q]; K = Q
+    ok = ok && make_tmap_pieces(&c->tm_b2A, c->HT, Q, N, ns, c->Qp, static_cast<long long>(N) * c->Qp, bkg, 128, te);
+    ok = ok && make_tmap_pieces(&c->tm_b2B, c->XlT, Q, D, ns, c->Qp, static_cast<long long>(D) * c->Qp, bkg, 256, te);
+  }
+  return ok;
+}
+
+// A memory context's calls with m memory rows: everything that depends on the database size N = Q + m -- the tile schedules, the
+// gradient's K blocks and split-K, the GLOBAL candidate capacity, the symmetric tiles (m = 0 only) and the tensor-map extents -- is
+// that of a context planned for exactly m rows, so no result depends on the capacity or on the rows an earlier call left past Q + m.
+// The buffers keep the capacity's layout (ldS, Np), which changes no value.
+static int set_call_rows(npair_ctx* c, int m) {
+  if (!c->mem_cap || m == c->mem_rows) return NPAIR_OK;
+  c->step.fwd_done = false;                        // the previous step's S and records no longer match the plan
+  const Plan p = plan_of(c->cfg, c->sms, true, m);
+  if (p.grad_split.splits > c->split_cap) {        // ruled out by split_k_cap; never write past the partial buffer
+    c->err = fmt("internal: m = %d needs %d split-K slices, the buffer holds %d", m, p.grad_split.splits, c->split_cap);
+    return NPAIR_E_STATE;
+  }
+  c->N = p.N; c->gcand_cap = p.gcand_cap; c->grad_kblocks = p.grad_kblocks; c->grad_split = p.grad_split;
+  c->n_sym_tiles = p.n_sym_tiles; c->sweep_epi = p.sweep_epi;
+  c->mem_rows = -1;                                // until the maps match
+  std::string te;
+  if (!make_maps(c, &te)) { c->err = te; return NPAIR_E_CUDA; }
+  c->mem_rows = m;
+  return NPAIR_OK;
+}
+
+static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out) {
   if (!out) { g_create_err = "null out"; return NPAIR_E_ARG; }
   *out = nullptr;
   std::string e;
   int rc = validate(cfg, &e);
+  if (rc == NPAIR_OK) rc = validate_memory(cfg, mem_cap, &e);
   if (rc != NPAIR_OK) { g_create_err = e; return rc; }
   int device = -1, sms = 0;
   if ((rc = open_device(cfg->device, &device, &sms)) != NPAIR_OK) return rc;
   std::unique_ptr<npair_ctx, void (*)(npair_ctx*)> made(new npair_ctx(), npair_destroy);   // until it is handed out
   npair_ctx* c = made.get();
-  c->cfg = *cfg; c->device = device; c->sms = sms;
+  c->cfg = *cfg; c->device = device; c->sms = sms; c->mem_cap = mem_cap; c->mem_rows = mem_cap;
   // only the multi-rank row-record backward on the tensor cores and the row-block similarity mode depend on the check, which itself
   // creates a single-rank context
   const bool blocks = sim_block_rows(*cfg) > 0;
@@ -580,12 +655,12 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
                    "would not match the rows the statistics were taken from";
     return NPAIR_E_ARG;
   }
-  static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym);
+  static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym, mem_cap);
   c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
-  const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit;
+  const int Q = c->Q;
   CREATE_TRY(ctx_buffers(c, c->mem));
-  if (c->sym_tiles) {
-    const std::vector<int2> tl = sym_tile_list(Q, N);
+  if (c->sym_tiles) {                              // world 1 (a memory context: its calls with m = 0), where N = Q
+    const std::vector<int2> tl = sym_tile_list(Q, Q);
     CREATE_TRY(cudaMemcpy(c->sym_tiles, tl.data(), sizeof(int2) * tl.size(), cudaMemcpyHostToDevice));
   }
   CREATE_TRY(cudaHostAlloc(&c->tops_pinned, sizeof(TopsBlock), cudaHostAllocMapped));
@@ -596,28 +671,12 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   if (c->lsel_mask) CREATE_TRY(allow_local_select_smem());
   if (cfg->gemm_backend == NPAIR_GEMM_TCGEN05) {
     CREATE_TRY(allow_smem(gemm_kernel(c->prec, c->sweep_epi)));
+    if (mem_cap) CREATE_TRY(allow_smem(gemm_kernel(c->prec, plan_of(*cfg, c->sms, sym).sweep_epi)));   // its calls with m = 0
     if (c->n_blocks > 1) CREATE_TRY(allow_smem(gemm_kernel(c->prec, EPI_STORE_S)));
     CREATE_TRY(c->fused_grad ? allow_smem(fused_kernel(c->prec)) : allow_smem(gemm_kernel(c->prec, EPI_OUT)));
     // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
     std::string te;
-    const int bkg = c->bk_grad;
-    // similarity: A = the rank's rows, B = all rows of the K-concatenated operands (PREC_BF16: Xs, whose one piece is that format)
-    const uint16_t* catA = c->cat ? c->XcatA : c->Xs;
-    const uint16_t* catB = c->cat ? c->XcatB : c->Xs;
-    bool ok = make_tmap_kcat(&c->tm_simA, &c->tm_simB, catA +static_cast<long long>(c->rank) * Q * c->kcat, Q, catB, N, c->kcat, &te);
-    ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, c->s_rows, c->ldS, &te);
-    // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
-    if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, &te);
-    ok = ok && make_tmap_pieces(&c->tm_b1B, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, bkg, 256, &te);
-    if (c->fused_grad) {
-      ok = ok && make_tmap_pieces(&c->tm_fB, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, &te);
-      ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, &te, 128);
-    }
-    if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) {   // gradient 2: A = HT [N x Q], B = XlT [D x Q]; K = Q
-      ok = ok && make_tmap_pieces(&c->tm_b2A, c->HT, Q, N, ns, c->Qp, static_cast<long long>(N) * c->Qp, bkg, 128, &te);
-      ok = ok && make_tmap_pieces(&c->tm_b2B, c->XlT, Q, D, ns, c->Qp, static_cast<long long>(D) * c->Qp, bkg, 256, &te);
-    }
-    if (!ok) { g_create_err = te; return NPAIR_E_CUDA; }
+    if (!make_maps(c, &te)) { g_create_err = te; return NPAIR_E_CUDA; }
   }
   // ---- NCCL ----
   if (c->world > 1 && (id128 || ext_comm)) {
@@ -672,10 +731,13 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   return NPAIR_OK;
 }
 
-int npair_create(const npair_config* cfg, const void* id128, npair_ctx** out) { return create_impl(cfg, id128, nullptr, out); }
+int npair_create(const npair_config* cfg, const void* id128, npair_ctx** out) { return create_impl(cfg, id128, nullptr, 0, out); }
 int npair_create_with_comm(const npair_config* cfg, void* comm, npair_ctx** out) {
   if (cfg && cfg->world > 1 && !comm) { g_create_err = "null communicator"; return NPAIR_E_ARG; }
-  return create_impl(cfg, nullptr, comm, out);
+  return create_impl(cfg, nullptr, comm, 0, out);
+}
+int npair_create_memory(const npair_config* cfg, int32_t max_memory_rows, npair_ctx** out) {
+  return create_impl(cfg, nullptr, nullptr, max_memory_rows, out);
 }
 
 // Peer-memory exchange of `kind`: pushes this rank's nA floats of srcA (and nB of srcB) into part partA (partB) of every rank's
@@ -759,6 +821,8 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st);
 
 // Enqueues npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward
 static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, cudaStream_t st) {
+  const int rc = set_call_rows(c, 0);
+  if (rc != NPAIR_OK) return rc;
   c->step = npair_ctx::Step{d_label};
   const int Q = c->Q, D = c->D;
   if (c->cfg.normalize_input) {               // fused L2Normalize producer (usage/def.prototxt:115-120): the layer works on x / ||x||
@@ -807,6 +871,7 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
   OrderedCall call(c, stream);
   int rc;
   if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = set_call_rows(c, 0)) != NPAIR_OK) return rc;
   const long long r0 = static_cast<long long>(c->rank) * c->Q;
   float* const normed = c->world > 1 ? c->Xtot_buf : c->Ynorm;     // normalize_input: the N normalised rows
   c->step = npair_ctx::Step{d_label_total + r0, c->cfg.normalize_input ? normed : d_feat_total, d_label_total, true};
@@ -816,6 +881,32 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
     launch_l2norm_fwd(d_feat_total + r0 * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
   }
   if ((rc = forward_impl(c, c->step.x_total + r0 * c->D, call.st)) != NPAIR_OK) return rc;
+  return finish_forward(c, tops_host, call.st);
+}
+
+/* Cross-batch memory (DESIGN 4.3): the database is [x; x_mem], Q + m rows, whose first Q are the anchors.  The memory rows are read
+ * where they lie (two-source operand preparation), and their records in the table after the Q row records switch their transposed
+ * gradient term off.  m = 0 is npair_forward. */
+int npair_forward_memory(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label, int32_t m,
+                         float tops_host[5], void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !tops_host || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = validate_memory(&c->cfg, 1, &c->err)) != NPAIR_OK) return rc;
+  if (m < 0 || m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", m, c->mem_cap); return NPAIR_E_ARG; }
+  if (m == 0) return npair_forward(c, d_feat, d_label, tops_host, stream);
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = set_call_rows(c, m)) != NPAIR_OK) return rc;
+  c->step = npair_ctx::Step{d_label, nullptr, c->labcat};
+  c->step.x_mem = d_mem_feat; c->step.lab_mem = d_mem_label;
+  if (c->cfg.normalize_input) {               // the current rows only: the memory holds rows the layer has already seen
+    PhaseTimer pt(c, 1, call.st);
+    launch_l2norm_fwd(d_feat, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
+    d_feat = c->Ynorm;
+  }
+  c->step.x_total = d_feat;
+  if ((rc = forward_impl(c, d_feat, call.st)) != NPAIR_OK) return rc;
   return finish_forward(c, tops_host, call.st);
 }
 
@@ -854,9 +945,17 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
   // ---- operand preparation: |x| sum (top asum, .cu:400), power-of-two pre-scale, split to tensor-core pieces ----
   {
     PhaseTimer pt(c, 1, st);
-    launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->step.x_total, static_cast<long long>(N) * D, c->partial,
-                       c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-    launch_split(c->step.x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    if (c->step.x_mem) {                       // cross-batch memory: rows [Q, N) are the caller's memory rows, read where they lie
+      const int m = N - Q;
+      launch_memory_rows(c->step.label, Q, c->step.lab_mem, m, c->labcat, c->ra.rowrec, st);
+      launch_prep_reduce_memory(d_feat, static_cast<long long>(Q) * D, c->step.x_mem, static_cast<long long>(m) * D, c->partial,
+                                c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
+      launch_split_memory(d_feat, Q, c->step.x_mem, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XcatA, c->XcatB, c->Dp, st);
+    } else {
+      launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->step.x_total, static_cast<long long>(N) * D, c->partial,
+                         c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
+      launch_split(c->step.x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    }
   }
   // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) over all Q rows; S is stored
   //      only when it is materialised, and is then block 0 of the row pass ----
@@ -1062,6 +1161,12 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
       } else rs_total = c->rs_total;
     }
   } else if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) bw_mode = BW_SPLIT;
+  if (c->step.x_mem) {
+    // cross-batch memory: the table of the Q row records and the memory rows' records (RowRecord::memory), whose transposed terms
+    // are 0, so that the gradient is (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x) with nothing divided
+    bw_mode = BW_ROWSCAL;
+    rs_total = c->ra.rowrec;
+  }
   if (tc && c->fused_grad) {
     // weights are produced inside the gradient GEMM: no H in HBM
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));

@@ -60,11 +60,17 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
 // Split-K of a gradient GEMM: when its output has too few tiles to fill the SMs (strong scaling: Q = B/world shrinks), the K range
 // is cut into at most 16 slices of at least min_kb K blocks each; splitk_reduce_kernel sums the slices' partial products.
 struct SplitK { int splits, kb_per_split; };
-inline SplitK split_k(int num_kblocks, int tiles, int sms, int min_kb) {
+// The split count split_k starts from, before it drops empty splits: an upper bound of split_k(...).splits that never decreases with
+// num_kblocks.  split_k's own count can decrease (sms 132, 8 tiles, min_kb 8: 80 K blocks give 10 splits, 81 give 9), so a buffer that
+// must hold the slices of any K up to some maximum is sized from this bound at that maximum.
+inline int split_k_cap(int num_kblocks, int tiles, int sms, int min_kb) {
   int splits = sms / (tiles > 0 ? tiles : 1);
   if (splits > 16) splits = 16;
   if (splits > num_kblocks / min_kb) splits = num_kblocks / min_kb;
-  if (splits < 1) splits = 1;
+  return splits < 1 ? 1 : splits;
+}
+inline SplitK split_k(int num_kblocks, int tiles, int sms, int min_kb) {
+  const int splits = split_k_cap(num_kblocks, tiles, sms, min_kb);
   const int kpb = (num_kblocks + splits - 1) / splits;
   return SplitK{(num_kblocks + kpb - 1) / kpb, kpb};                    // no empty split
 }

@@ -67,6 +67,8 @@ __device__ __forceinline__ void abs_sum_max(const float* __restrict__ x, long lo
 // One kernel: per-block partial |x| sums (local rows) and max|x| (all rows), the reset of the per-row statistics, and --
 // in the last block to finish (ticket) -- the final asum, the power-of-two operand scale and the reset of the step state.
 // Returns true in the block that finished last (it has written the step's scalars to *bs).
+// DISJOINT (cross-batch memory): xt holds rows other than xl's, so max |x| is taken over both and the sum over xl alone.
+template <bool DISJOINT = false>
 __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, long long nl, const float* __restrict__ xt, long long ntot,
                                                  float* __restrict__ partial, int want_scale, RowArrays ra, int Q, BlockScalars* bs) {
   __shared__ float s_sum[8], s_max[8];
@@ -75,9 +77,10 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   // 16-byte loads, four in flight per thread (cudaMalloc'd / framework blobs are 16-byte aligned; otherwise 4-byte loads)
-  const bool same_range = want_scale && xl == xt && nl == ntot;    // world == 1: one sweep gives both the sum and the maximum
-  if ((reinterpret_cast<uintptr_t>(xl) & 15) == 0) abs_sum_max<true>(xl, nl, t0, stride, same_range, sum, mx);
-  else abs_sum_max<false>(xl, nl, t0, stride, same_range, sum, mx);
+  const bool same_range = !DISJOINT && want_scale && xl == xt && nl == ntot;    // world == 1: one sweep gives both the sum and the maximum
+  const bool local_max = DISJOINT ? want_scale != 0 : same_range;
+  if ((reinterpret_cast<uintptr_t>(xl) & 15) == 0) abs_sum_max<true>(xl, nl, t0, stride, local_max, sum, mx);
+  else abs_sum_max<false>(xl, nl, t0, stride, local_max, sum, mx);
   if (want_scale && !same_range) {
     if ((reinterpret_cast<uintptr_t>(xt) & 15) == 0) {
       const float4* x4 = reinterpret_cast<const float4*>(xt);
@@ -140,6 +143,20 @@ void launch_prep_reduce(const float* x_local, long long n_local, const float* x_
   int nb = static_cast<int>((nmax + 256 * 16 - 1) / (256 * 16));
   if (nb < 1) nb = 1; if (nb > 592) nb = 592;
   prep_reduce_kernel<<<nb, 256, 0, st>>>(x_local, n_local, x_total, n_total, partial, want_scale, ra, Q, bs);
+  count_launch();
+}
+// Cross-batch memory (DESIGN 4.3): the current rows xl and the memory rows xm are two buffers.  The grid is sized from both, as
+// launch_prep_reduce sizes it for one buffer of Q + m rows, so the asum of the current rows is summed in the same order.
+__global__ void __launch_bounds__(256) prep_reduce_memory_kernel(const float* __restrict__ xl, long long nl, const float* __restrict__ xm,
+                                                                 long long nm, float* __restrict__ partial, int want_scale, RowArrays ra, int Q,
+                                                                 BlockScalars* bs) {
+  prep_reduce_body<true>(xl, nl, xm, nm, partial, want_scale, ra, Q, bs);
+}
+void launch_prep_reduce_memory(const float* x_local, long long n_local, const float* x_mem, long long n_mem, float* partial, int want_scale,
+                               RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st) {
+  int nb = static_cast<int>((n_local + n_mem + 256 * 16 - 1) / (256 * 16));
+  if (nb < 1) nb = 1; if (nb > 592) nb = 592;
+  prep_reduce_memory_kernel<<<nb, 256, 0, st>>>(x_local, n_local, x_mem, n_mem, partial, want_scale, ra, Q, bs);
   count_launch();
 }
 
@@ -237,6 +254,55 @@ __global__ void __launch_bounds__(256) split_kernel(SplitArgs a, const BlockScal
   split_load(a, blockIdx.x, blockIdx.y, v);
   split_tile<PREC>(a, (PREC == PREC_FP16X2) ? bs->x_scale : 1.f, blockIdx.x, blockIdx.y, v, 0);
 }
+// Cross-batch memory: rows [0, a.Q) from a.x, rows [a.Q, a.N) from xm.  A 32-row tile may straddle the two buffers, so each row is
+// loaded from its own one; the transposed pieces are then written as by split_kernel, in 16-byte segments across the boundary.
+__device__ __forceinline__ void split_load_memory(const SplitArgs& a, const float* __restrict__ xm, int tile_d, int tile_n, float (&v)[8]) {
+  const int N = a.N, D = a.D;
+  const int t = threadIdx.x, nl = t >> 3, dg = t & 7;
+  const int n = tile_n * 32 + nl, d = tile_d * 64 + 8 * dg;
+  const bool rowok = n < N;
+  const float* x = n < a.Q ? a.x + static_cast<long long>(n) * D : xm + static_cast<long long>(n - a.Q) * D;
+  if (rowok && d + 7 < D && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {   // the row starts 16-byte aligned: so does x + d
+    const float4 a4 = *reinterpret_cast<const float4*>(x + d);
+    const float4 b4 = *reinterpret_cast<const float4*>(x + d + 4);
+    v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = (rowok && d + e < D) ? x[d + e] : 0.f;
+  }
+}
+template <int PREC>
+__global__ void __launch_bounds__(256) split_memory_kernel(SplitArgs a, const float* __restrict__ xm, const BlockScalars* __restrict__ bs) {
+  float v[8];
+  split_load_memory(a, xm, blockIdx.x, blockIdx.y, v);
+  split_tile<PREC>(a, (PREC == PREC_FP16X2) ? bs->x_scale : 1.f, blockIdx.x, blockIdx.y, v, 0);
+}
+void launch_split_memory(const float* x, int Q, const float* x_mem, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs,
+                         long long ldXs, uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st) {
+  dim3 grid((D + 63) / 64, (N + 31) / 32);
+  const SplitArgs a{x, N, D, Xs, ldXs, XsT, ldXsT, nullptr, 0, 0, Q, XcatA, XcatB, Dp};
+  with_prec(prec, [&](auto P) { split_memory_kernel<P><<<grid, 256, 0, st>>>(a, x_mem, bs); });
+  count_launch();
+}
+// The labels of the Q current rows and the m memory rows into lab_total [Q + m], and the memory rows' records into rec[Q, Q + m): a
+// memory row is never an anchor, so its record switches its transposed gradient term off exactly (RowRecord::memory) and keeps its label,
+// which decides whether the anchor's own term treats the pair as same-label or different-label.
+__global__ void memory_rows_kernel(const float* __restrict__ label, int Q, const float* __restrict__ mem_label, int m,
+                                   float* __restrict__ lab_total, RowRecord* __restrict__ rec) {
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Q + m; i += stride) {
+    if (i < Q) { lab_total[i] = label[i]; continue; }
+    const float l = mem_label[i - Q];
+    lab_total[i] = l;
+    rec[i] = RowRecord::memory(l);
+  }
+}
+void launch_memory_rows(const float* label, int Q, const float* mem_label, int m, float* lab_total, RowRecord* rec, cudaStream_t st) {
+  const int blocks = (Q + m + 255) / 256;
+  memory_rows_kernel<<<blocks < 1024 ? blocks : 1024, 256, 0, st>>>(label, Q, mem_label, m, lab_total, rec);
+  count_launch();
+}
+
 void launch_split(const float* x_total, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs, long long ldXs,
                   uint16_t* XsT, long long ldXsT, uint16_t* XlT, long long ldXlT, int row0_local, int Q,
                   uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st) {

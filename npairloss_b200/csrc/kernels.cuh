@@ -82,6 +82,10 @@ struct RowRecord {
     const float4* h = reinterpret_cast<const float4*>(records);
     return RowRecord{h[2 * k], h[2 * k + 1]};
   }
+  // The record of a cross-batch memory row (DESIGN 4.3), which is never an anchor: +inf exponent offsets, -inf thresholds and zero
+  // weight factors make its transposed gradient term exactly 0 in both weight builders; its label is the row's real one, since the
+  // anchor's own term tells same-label from different-label pairs by the column record's label
+  __host__ __device__ static RowRecord memory(float label) { return make(INFINITY, -INFINITY, INFINITY, label, -INFINITY, 0.f, 0.f); }
   __host__ __device__ float m2c() const { return lo.x; }
   __host__ __device__ float thr_n() const { return lo.y; }
   __host__ __device__ float m2() const { return lo.z; }
@@ -229,6 +233,15 @@ void launch_split(const float* x_total, int N, int D, int prec, const BlockScala
                   uint16_t* Xs, long long ldXs /*Dp*/, uint16_t* XsT, long long ldXsT /*Np*/,
                   uint16_t* XlT, long long ldXlT /*Qp, or 0*/, int row0_local, int Q,
                   uint16_t* XcatA /*or NULL*/, uint16_t* XcatB, long long Dp, cudaStream_t st);
+// Cross-batch memory (DESIGN 4.3): the operand preparation of the current rows x_local and the memory rows x_mem, two buffers.  max |x|
+// (the pre-scale) over both, the asum over x_local alone
+void launch_prep_reduce_memory(const float* x_local, long long n_local, const float* x_mem, long long n_mem, float* partial /*[2*1024]*/,
+                               int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st);
+// launch_split of the N = Q + m rows [x (Q rows); x_mem] at world 1: the memory rows land at row Q of every B-side operand
+void launch_split_memory(const float* x, int Q, const float* x_mem, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs,
+                         long long ldXs, uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st);
+// lab_total[0, Q + m) = [label; mem_label], rec[Q + i] = RowRecord::memory(mem_label[i])
+void launch_memory_rows(const float* label, int Q, const float* mem_label, int m, float* lab_total, RowRecord* rec, cudaStream_t st);
 void launch_row_stats_ref(SimRows sim, RowArrays ra, cudaStream_t st);
 // The threshold pick of the rank's Q rows by one block (SIMT backend; the tensor-core similarity sweep runs it in its last CTA)
 void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, cudaStream_t st);
@@ -241,8 +254,9 @@ void launch_tops_world(const float* xall, int xstride, int world, long long N, i
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
                      unsigned int seq, bool finalize, cudaStream_t st);
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
-// mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (world > 1, row-record
-// exchange: rs_total = the world's N records, all-gathered)
+// mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (rs_total = one record per column: at
+// world > 1 the world's N row records, all-gathered; in a cross-batch memory step at world 1, the Q row records followed by the m
+// memory rows' RowRecord::memory records, whose transposed terms are 0)
 enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
 // over the rank's whole S (sim.row0 == 0, sim.rows == Q)
 void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,

@@ -16,6 +16,11 @@ trained with the reference layer sees.
 The library context is stateful (S and the row records of the last forward): a second forward through the same module before the
 backward of the first would silently change what that backward computes.  Every forward therefore stamps a generation number and
 the backward refuses to run against a newer forward.
+
+CROSS-BATCH MEMORY.  NPairLoss(memory_rows=M) (world = 1) keeps the last M embeddings and labels it has seen in a device FIFO ring and
+passes them to every forward as extra database rows (npair_forward_memory, DESIGN 4.3; Wang et al., CVPR 2020): they take part in the
+mining and in the softmax of the current anchors but receive no gradient.  reset_memory() empties the ring, so when the memory starts
+(XBM warms up for some iterations first) is the caller's choice.
 """
 from __future__ import annotations
 
@@ -46,7 +51,10 @@ class _NPairFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, label, owner):
         layer = owner._context(feat)
-        tops = layer.forward(feat, label)                     # blocks until the five scalars are on the host (as the reference)
+        if owner._mem_cap:
+            tops = owner._forward_memory(layer, feat, label)
+        else:
+            tops = layer.forward(feat, label)                 # blocks until the five scalars are on the host (as the reference)
         owner._generation += 1
         ctx.owner, ctx.layer, ctx.generation = owner, layer, owner._generation
         ctx.save_for_backward(feat, label)                    # the C ABI wants both unchanged until the backward is enqueued
@@ -71,17 +79,72 @@ class _NPairFunction(torch.autograd.Function):
 class NPairLoss(torch.nn.Module):
     """Module form; the library context is created on first use for the (rows, dims, device) it sees and re-created when
     they change.  Keyword arguments are the fields of capi.make_config (mining regions/methods, margins, SN, precision,
-    normalize_input, ...)."""
+    normalize_input, ...).
 
-    def __init__(self, world: int = 1, rank: int = 0, nccl_id: bytes | None = None, true_gradient: bool = False, _context_factory=None, **config):
+    memory_rows=M > 0 (world = 1 only): a cross-batch memory of the last M rows this module has seen.  Each forward passes the ring's
+    m = min(rows enqueued, M) valid rows, slots 0 .. m-1 in slot order, and then enqueues the batch's own rows, detached (under
+    normalize_input the normalised rows the layer used), so a batch is never in the memory during its own step.  The ring survives the
+    context being re-created for a new batch size; it is emptied when the dimension or device changes and by reset_memory()."""
+
+    def __init__(self, world: int = 1, rank: int = 0, nccl_id: bytes | None = None, true_gradient: bool = False, _context_factory=None,
+                 memory_rows: int = 0, **config):
         super().__init__()
         if true_gradient and world != 1:
             raise ValueError("true_gradient is defined for world = 1 (the reference's multi-rank blend is not a gradient of one loss)")
+        if int(memory_rows) < 0:
+            raise ValueError("memory_rows must be >= 0")
+        if int(memory_rows) and world != 1:
+            raise ValueError("a cross-batch memory (memory_rows > 0) is defined for world = 1")
         self._config, self._world, self._rank, self._nccl_id = dict(config), world, rank, nccl_id
-        self._factory = _context_factory or (lambda cfg, nid: capi.Context(cfg, nid))
+        self._mem_cap = int(memory_rows)
+        if _context_factory is not None:
+            self._factory = _context_factory
+        elif self._mem_cap:
+            self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._mem_cap)
+        else:
+            self._factory = lambda cfg, nid: capi.Context(cfg, nid)
         self._ctx, self._key = None, None
         self._generation = 0
         self._true_gradient = bool(true_gradient)
+        self._mem_x = self._mem_l = None      # the ring: [M, D] rows and [M] fp32 labels, allocated at the first forward
+        self._mem_count = 0                   # rows enqueued since the last reset (the valid slots are 0 .. min(count, M) - 1)
+
+    def reset_memory(self):
+        """Empties the cross-batch memory: the next forward sees no memory rows."""
+        self._mem_count = 0
+
+    def memory(self):
+        """(rows [m, D], labels [m]) the next forward passes as its memory: views of the ring's valid slots, in slot order."""
+        m = min(self._mem_count, self._mem_cap)
+        if self._mem_x is None:
+            return None, None
+        return self._mem_x[:m], self._mem_l[:m]
+
+    def _forward_memory(self, layer, feat, label):
+        d = feat.shape[1]
+        if self._mem_x is None or self._mem_x.shape[1] != d or self._mem_x.device != feat.device:
+            self._mem_x = torch.empty(self._mem_cap, d, dtype=torch.float32, device=feat.device)
+            self._mem_l = torch.empty(self._mem_cap, dtype=torch.float32, device=feat.device)
+            self._mem_count = 0
+        m = min(self._mem_count, self._mem_cap)
+        tops = layer.forward_memory(feat, label, self._mem_x, self._mem_l, m)
+        # the forward has read the memory: this batch's rows go in behind it, in stream order
+        rows = feat.detach()
+        if self._config.get("normalize_input"):
+            rows = capi.l2normalize_forward(rows)[0]
+        q = rows.shape[0]
+        if q > self._mem_cap:                 # a batch larger than the memory leaves its last M rows
+            rows, label, self._mem_count = rows[q - self._mem_cap:], label[q - self._mem_cap:], self._mem_count + q - self._mem_cap
+            q = self._mem_cap
+        head = self._mem_count % self._mem_cap
+        first = min(q, self._mem_cap - head)
+        self._mem_x[head:head + first].copy_(rows[:first])
+        self._mem_l[head:head + first].copy_(label[:first])
+        if first < q:
+            self._mem_x[:q - first].copy_(rows[first:])
+            self._mem_l[:q - first].copy_(label[first:])
+        self._mem_count += q
+        return tops
 
     def _context(self, feat):
         q, d = feat.shape[0], feat[0].numel()
