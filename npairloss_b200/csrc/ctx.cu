@@ -1010,7 +1010,7 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
         launch_local_select(sim, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn, c->ra, c->bs, c->sms, lsel_warp, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
       launch_lse_rows(sim, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world, c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr,
-                      c->tops_seq, c->n_blocks == 1, st);
+                      weight_scale_log2(c->prec), c->tops_seq, c->n_blocks == 1, st);
     }
     if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
     if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
@@ -1137,8 +1137,9 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   // loss_weight / dot_normalizer (.cu:427,448); world scope: the normaliser is the world's batch and the transposed term is not
-  // divided by the world size, i.e. exactly what a single rank holding the whole batch computes
-  const float lw_over_q = loss_weight / static_cast<float>(c->wscope ? N : Q);
+  // divided by the world size, i.e. exactly what a single rank holding the whole batch computes.  Times 2^-k: the row records build
+  // every gradient weight at 2^k times its value (weight_scale_log2), an exact power of two that the GEMMs' alpha undoes
+  const float lw_over_q = ldexpf(loss_weight / static_cast<float>(c->wscope ? N : Q), -weight_scale_log2(c->prec));
   const bool tc = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
   const RowRecord* rs_total = nullptr;
   int bw_mode = BW_SYM;

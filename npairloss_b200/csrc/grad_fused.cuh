@@ -104,8 +104,8 @@ __device__ __forceinline__ int chunk_end(int c0, int kb0, int kb1, int ch, int k
 // One row's view for the weight builder (neutral when the row does not exist: thresholds -inf -> nothing selected)
 struct RowRec { float m2r, tn, m2, lab, tp, cA; int self_col; };
 
-// Weight of the pair (row, column m): two exponentials whose arguments already carry the factors 1/T (and 1/world for the
-// transposed term) -- see lse_rows_kernel -- switched off by a -inf argument when the pair is not selected.  Same-label pairs use
+// Weight of the pair (row, column m): two exponentials whose arguments already carry the factors 2^k / T (and 1/world for the
+// transposed term; k = weight_scale_log2) -- see lse_rows_kernel -- switched off by a -inf argument when the pair is not selected.  Same-label pairs use
 // the positive rule and weights; the self pair and columns beyond N weigh nothing.
 // Branch-free: the label test selects the two exponentials' arguments and then the result, so the eight weights of a K step form
 // independent straight-line chains that the scheduler interleaves (a branch per weight serialised their shared-memory and MUFU

@@ -488,7 +488,8 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
 #define NPAIR_LSE_MINB 3
 #endif
 __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __grid_constant__ SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs,
-                                                       int num_tops, TopsBlock* __restrict__ tops, float log2_world,
+                                                       int num_tops, TopsBlock* __restrict__ tops,
+                                                       float m2c_off /*log2(world) - k*/, float wscale /*2^k: weight_scale_log2*/,
                                                        TopSums* __restrict__ xout /*world scope: this rank's tops sums, else NULL*/,
                                                        int wpr /*warps per row: 1, 2, 4 or 8 (few rows per rank: keep the SMs full)*/,
                                                        unsigned int seq /*written behind the tops: the host polls it*/, int finalize) {
@@ -618,7 +619,7 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
       const float invA = A == 0.f ? 0.f : 1.f / A;              // Get_Query_Diff_Part zero rules (.cu:410-415)
       const float invT = T == 0.f ? 0.f : 1.f / T;
       const float cA = invT - invA;
-      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + log2_world, thr_n, m2, li, thr_p, cA, invT);
+      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + m2c_off, thr_n, m2, li, thr_p, cA * wscale, invT * wscale);
     }
   }
   if (!finalize) return;
@@ -657,13 +658,14 @@ static void lse_shape(int Q, int N, int* wpr_out, int* threads_out) {
   *threads_out = wpb * 32;
 }
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
-                     unsigned int seq, bool finalize, cudaStream_t st) {
+                     int wlog2, unsigned int seq, bool finalize, cudaStream_t st) {
   int wpr = 1, threads = 256;
   lse_shape(sim.Q, sim.N, &wpr, &threads);
   const int rows_per_blk = threads / 32 / wpr;
   const int grid = (sim.rows + rows_per_blk - 1) / rows_per_blk;
-  lse_rows_kernel<<<grid, threads, 0, st>>>(sim, mp, ra, bs, num_tops, tops_dev, xout ? 0.f : log2f(static_cast<float>(world)), xout, wpr, seq,
-                                            finalize ? 1 : 0);
+  const float log2_world = xout ? 0.f : log2f(static_cast<float>(world));
+  lse_rows_kernel<<<grid, threads, 0, st>>>(sim, mp, ra, bs, num_tops, tops_dev, log2_world - static_cast<float>(wlog2), ldexpf(1.f, wlog2), xout,
+                                            wpr, seq, finalize ? 1 : 0);
   count_launch();
 }
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st) {

@@ -69,9 +69,12 @@ __device__ __forceinline__ float an_thr(float t, int m) {     // diff-label rule
 // pushes, the NCCL all-gather, npair_row_scalars / npair_backward_gathered), so this is the one description of its layout.  The two
 // 16-byte halves are loaded and stored as vectors; the first holds all that a diff-label pair needs.
 //   m2     max_all * log2(e), the row's exponent offset
-//   m2c    m2 + log2(T) + log2(world) (+inf when T == 0): a diff-label weight exp(s - max) / T / world is ONE exponential 2^(s*log2(e) - m2c)
+//   m2c    m2 + log2(T) + log2(world) - k (+inf when T == 0): a diff-label weight 2^k exp(s - max) / T / world is ONE exponential
+//          2^(s*log2(e) - m2c)
 //   thr_n  the an_thr-transformed diff-label threshold;  thr_p  the ap_thr-transformed same-label threshold
-//   cA     same-label weight factor 1/T - 1/A;  cT  diff-label weight factor 1/T
+//   cA     same-label weight factor 2^k (1/T - 1/A);  cT  diff-label weight factor 2^k / T
+// so every gradient weight built from records comes out scaled by 2^k, k = weight_scale_log2(format), and the gradient GEMM's alpha
+// carries 2^-k.
 struct RowRecord {
   float4 lo, hi;   // {m2c, thr_n, m2, label}, {thr_p, cA, cT, 0}
   __host__ __device__ static RowRecord make(float m2c, float thr_n, float m2, float label, float thr_p, float cA, float cT) {
@@ -95,6 +98,13 @@ struct RowRecord {
   __host__ __device__ float cT() const { return hi.z; }
 };
 static_assert(sizeof(RowRecord) == 32, "row records are exchanged as 32 raw bytes");
+// log2 of the scale the gradient weights of format `prec` are built at.  An fp16x2 weight is split into fp16 hi + lo pieces; unscaled,
+// the lo piece of a weight below about 2^-3 falls into fp16's subnormal range (spacing 2^-24), an absolute error of up to 2^-25 per
+// weight, which does not average out when the rows are clustered and their weights nearly equal.  Every weight lies in [-1, 1]
+// (exp(s - max) / T and exp(s - max) (1/T - 1/A) with exp(s - max) <= A <= T), and the world-1 operand H = g'(j, m) + g'(m, j) in
+// [-2, 2]; 2^14 * 2 = 32768 stays below fp16's largest finite 65504 (2^15 * 2 would not), so k = 14 is the largest safe scale and
+// keeps the lo piece normal down to weights of about 2^-17.  bf16 pieces have fp32's exponent range: no scale.
+__host__ __device__ constexpr int weight_scale_log2(int prec) { return prec == PREC_FP16X2 ? 14 : 0; }
 constexpr long long ROW_RECORD_FLOATS = sizeof(RowRecord) / sizeof(float);   // exchanges count floats
 
 // One rank's contribution to a world-scope reduction (global_scope), exchanged as raw bytes in its slot of the small exchange; the
@@ -250,9 +260,10 @@ void launch_thresholds_world(const float* xall, int xstride, int world, long lon
 // World scope: the tops of the world's N rows from the ranks' TopSums, which lie xstride floats apart in xall
 void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // Row pass over the rows of sim.  finalize: the last block also reduces the Q rows' results into the tops; otherwise
-// launch_lse_finalize does, once.  xout: NULL, or (world scope) receives the rank's TopSums instead of the tops
+// launch_lse_finalize does, once.  xout: NULL, or (world scope) receives the rank's TopSums instead of the tops.  wlog2: the records'
+// weight scale, weight_scale_log2 of the operand format
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
-                     unsigned int seq, bool finalize, cudaStream_t st);
+                     int wlog2, unsigned int seq, bool finalize, cudaStream_t st);
 void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (rs_total = one record per column: at
 // world > 1 the world's N row records, all-gathered; in a cross-batch memory step at world 1, the Q row records followed by the m
