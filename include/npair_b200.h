@@ -210,6 +210,41 @@ size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_
 int npair_forward_memory(npair_ctx* ctx, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label,
                          int32_t m, float tops_host[5], void* stream);
 
+/* ---- asynchronous training step and CUDA-graph capture, world 1 only (DESIGN 4.4) ----
+ * The calls above that return tops on the host wait for them.  These do not: they return once the step's work is enqueued, making
+ * no host wait and no host read of device data, so the host can queue the next step and a whole step can be captured into a CUDA
+ * graph.  Results are those of the synchronous calls, bit for bit.  At world > 1 all four return NPAIR_E_ARG before enqueuing anything.
+ *   npair_forward_async        : npair_forward with the tops written in stream order to d_tops, 5 fp32 in device memory: the bits
+ *                                tops_host would receive (0 past num_tops).  Counts as a successful forward, so a backward may follow
+ *                                at once.  When a device error bit is set (the cases npair_forward reports as NPAIR_E_EMPTY_LIST or
+ *                                NPAIR_E_POS_RANGE), all five tops are NaN, the gradient of the step is unspecified and the bit is
+ *                                kept for npair_async_status.
+ *   npair_forward_memory_async : npair_forward_memory (same arguments and refusals) with the tops written as above.
+ *   npair_backward_device_weight: npair_backward with the loss weight read in stream order from one fp32 in device memory (for
+ *                                example the autograd gradient of the loss, or a loss scaler's scale): the gradient bits of
+ *                                npair_backward(*d_loss_weight), after either kind of forward.
+ *   npair_async_status         : waits for the work of the context's last call, then returns NPAIR_E_EMPTY_LIST or NPAIR_E_POS_RANGE
+ *                                (in that order) if an asynchronous forward since the previous status call set that error bit, and
+ *                                clears the bits; NPAIR_OK otherwise.  Work replayed from a graph is not a call of the context: make
+ *                                the host wait for the replay's stream first.
+ * Graph capture.  The three enqueuing calls may be captured on a stream in any capture mode (cudaStreamCaptureModeGlobal is the one
+ * torch.cuda.graph uses); inside a capture they make no synchronising call, allocation or event wait.  Rules:
+ *   - A graph holds whole steps: a forward, then its backward.  A replay depends only on the captured buffers' contents (the inputs,
+ *     d_tops, the loss weight, the memory rows) and on the context; a memory context's graph holds the m it was captured with.
+ *   - A captured call skips the wait for the previous call's stream: order earlier work of the context before the capture begins
+ *     (torch.cuda.graph synchronises the device first).  It records no event, so no later call waits on the graph; order each
+ *     replay against the context's eager calls on other streams yourself.  Calls on the replay's stream are ordered by the stream.
+ *   - After a replay, the next eager call on the context is a forward.
+ *   - On a capturing stream, and while a call of the context is being captured for the stream-less ones, these return NPAIR_E_STATE
+ *     before any CUDA call that would invalidate the capture: npair_forward, npair_forward_memory, npair_forward_backward,
+ *     npair_forward_gathered, npair_debug_read, npair_profile_read and npair_async_status.  With profiling on
+ *     (npair_profile_enable), the three capturable calls also return NPAIR_E_STATE on a capturing stream. */
+int npair_forward_async(npair_ctx* ctx, const float* d_feat, const float* d_label, float* d_tops, void* stream);
+int npair_forward_memory_async(npair_ctx* ctx, const float* d_feat, const float* d_label, const float* d_mem_feat,
+                               const float* d_mem_label, int32_t m, float* d_tops, void* stream);
+int npair_backward_device_weight(npair_ctx* ctx, const float* d_loss_weight, float* d_feat_diff, void* stream);
+int npair_async_status(npair_ctx* ctx);
+
 /* The L2Normalize producer layer of the reference net (usage/def.prototxt:115-120; its source is not part of the reference tree):
  * y[r][:] = x[r][:] / ||x[r][:]||_2 (a zero row stays zero), and its backward dx = (dy - y (y . dy)) / ||x||.  Stand-alone entry
  * points for a host framework's own L2Normalize layer; npair_config.normalize_input = 1 runs the same kernels inside

@@ -44,6 +44,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
            # cross-batch memory (not part of the reference layer)
            "npair_create_memory", "npair_memory_workspace_bytes", "npair_forward_memory",
+           # asynchronous step and graph capture (not part of the reference layer)
+           "npair_forward_async", "npair_forward_memory_async", "npair_backward_device_weight", "npair_async_status",
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
@@ -89,6 +91,10 @@ def lib():
         L.npair_memory_workspace_bytes.restype = C.c_size_t
         L.npair_forward_memory.argtypes = [vp, vp, vp, vp, vp, C.c_int32, fp, vp]
         L.npair_backward.argtypes = [vp, C.c_float, vp, vp]
+        L.npair_forward_async.argtypes = [vp, vp, vp, vp, vp]
+        L.npair_forward_memory_async.argtypes = [vp, vp, vp, vp, vp, C.c_int32, vp, vp]
+        L.npair_backward_device_weight.argtypes = [vp, vp, vp, vp]
+        L.npair_async_status.argtypes = [vp]
         L.npair_forward_gathered.argtypes = [vp, vp, vp, fp, vp]
         L.npair_backward_partial.argtypes = [vp, C.c_float, vp, vp, vp]
         L.npair_bwd_exchange_mode.argtypes = [vp]
@@ -241,6 +247,52 @@ class Context:
         import torch
         assert diff.is_cuda and diff.dtype == torch.float32 and diff.is_contiguous()
         self.backward_ptr(loss_weight, diff.data_ptr(), torch.cuda.current_stream().cuda_stream)
+
+    # ---- asynchronous step (DESIGN 4.4): world 1, nothing read back on the host, capturable into a CUDA graph ----
+    @staticmethod
+    def _f32(t, what):
+        import torch
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise TypeError(f"{what} must be a contiguous CUDA float32 tensor")
+        return t.data_ptr()
+
+    def forward_async(self, feat, label, tops_out):
+        """npair_forward_async: enqueues the forward and returns at once; tops_out (5 fp32 on the device) receives the tops in stream
+        order, all NaN on a device error (see async_status)."""
+        import torch
+        if tops_out.numel() < 5:
+            raise ValueError("tops_out holds 5 floats")
+        self._check(lib().npair_forward_async(self._h, self._f32(feat, "feat"), self._f32(label, "label"), self._f32(tops_out, "tops_out"),
+                                              torch.cuda.current_stream().cuda_stream))
+        return tops_out
+
+    def forward_memory_async(self, feat, label, mem_feat, mem_label, m, tops_out):
+        """npair_forward_memory_async: forward_memory with the tops written to tops_out as in forward_async."""
+        import torch
+        if tops_out.numel() < 5:
+            raise ValueError("tops_out holds 5 floats")
+        mp = lp = None
+        if mem_feat is not None:
+            if mem_feat.shape[0] < m or mem_label is None or mem_label.shape[0] < m:
+                raise ValueError("the memory holds fewer than m rows")
+            mp, lp = self._f32(mem_feat, "mem_feat"), self._f32(mem_label, "mem_label")
+        self._check(lib().npair_forward_memory_async(self._h, self._f32(feat, "feat"), self._f32(label, "label"), mp, lp, int(m),
+                                                     self._f32(tops_out, "tops_out"), torch.cuda.current_stream().cuda_stream))
+        return tops_out
+
+    def backward_device_weight(self, loss_weight, diff):
+        """npair_backward_device_weight: backward with the loss weight read on the device from loss_weight (a one-element CUDA fp32
+        tensor), with the gradient bits of backward(float(loss_weight))."""
+        import torch
+        if loss_weight.numel() != 1:
+            raise ValueError("loss_weight is one element")
+        self._check(lib().npair_backward_device_weight(self._h, self._f32(loss_weight, "loss_weight"), self._f32(diff, "diff"),
+                                                       torch.cuda.current_stream().cuda_stream))
+
+    def async_status(self):
+        """npair_async_status: waits for the context's last call and raises NpairError (E_EMPTY_LIST or E_POS_RANGE) if an asynchronous
+        forward since the previous status call met a device error; clears it."""
+        self._check(lib().npair_async_status(self._h))
 
     def forward_gathered(self, feat_total, label_total):
         import torch

@@ -363,6 +363,10 @@ struct npair_ctx : Plan {
   TopsBlock* tops_pinned = nullptr;   // host-mapped
   unsigned int tops_seq = 0;
   TopsBlock* tops_dev = nullptr;
+  AsyncWords* aw = nullptr;      // the asynchronous calls' tops, error bits and gradient scale (npair_forward_async, DESIGN 4.4)
+  // the capture a call of this context was last enqueued into (npair_b200.h, graph capture): the stream-less calls that wait for the
+  // context's work are refused while it lasts
+  struct Capture { cudaStream_t st = nullptr; unsigned long long id = 0; } capture;
   CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_kcat)
   // nccl
   void* comm = nullptr; bool own_comm = false;
@@ -406,6 +410,7 @@ static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   if (slices > 1) m.own(&c->part, f * split_part(slices, c->cfg.Q, D), false);
   m.own_carved(true, [c](Carve& cv) { carve_rows(cv, c->cfg.Q, c->mem_cap, &c->ra); });
   m.own(&c->bs, sizeof(BlockScalars), true);
+  m.own(&c->aw, sizeof(AsyncWords), true);
   m.own(&c->partial, f * 2048, false);
   m.own(&c->ghist, sizeof(unsigned long long) * 4096, true);
   m.own(&c->gcand, sizeof(uint32_t) * 2ull * c->gcand_cap, false);
@@ -817,10 +822,38 @@ static int need_comm(npair_ctx* c, const char* instead) {
   return NPAIR_E_STATE;
 }
 
-static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st);
+// The calls that wait on the host (for tops, or for the context's work) would invalidate a CUDA graph capture on their stream: they are
+// refused on a capturing stream before any CUDA call
+static int refuse_capture(npair_ctx* c, void* stream, const char* call) {
+  if (!capture_id(static_cast<cudaStream_t>(stream))) return NPAIR_OK;
+  c->err = fmt("%s waits on the host and cannot be captured into a CUDA graph (use npair_forward_async / npair_backward_device_weight)", call);
+  return NPAIR_E_STATE;
+}
+// ... and the stream-less ones while the capture a call of this context was enqueued into lasts
+static int refuse_in_capture(npair_ctx* c, const char* call) {
+  if (!c->capture.id) return NPAIR_OK;
+  if (capture_id(c->capture.st) != c->capture.id) { c->capture = npair_ctx::Capture{}; return NPAIR_OK; }
+  c->err = fmt("%s waits for the context's work, which a CUDA graph capture holds", call);
+  return NPAIR_E_STATE;
+}
+// The preconditions of the asynchronous calls, checked before anything is enqueued: world 1 (the peer-exchange epochs and the NCCL
+// calls are host state a graph would freeze), and on a capturing stream no profiling (its events could not be read).  *captured: the
+// stream is capturing, which the context notes for refuse_in_capture.
+static int async_entry(npair_ctx* c, void* stream, const char* call, bool* captured) {
+  if (c->world != 1) { c->err = fmt("%s is world-1 only", call); return NPAIR_E_ARG; }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const unsigned long long id = capture_id(st);
+  if (id && c->prof) { c->err = fmt("%s: profiling (npair_profile_enable) cannot be captured into a CUDA graph", call); return NPAIR_E_STATE; }
+  *captured = id != 0;
+  c->capture = id ? npair_ctx::Capture{st, id} : npair_ctx::Capture{};
+  return NPAIR_OK;
+}
 
-// Enqueues npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward
-static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, cudaStream_t st) {
+static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cudaStream_t st);
+
+// Enqueues npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward, whose
+// tops go to `tops` (mapped pinned memory for the synchronous calls, device memory for the asynchronous ones)
+static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, TopsBlock* tops, cudaStream_t st) {
   const int rc = set_call_rows(c, 0);
   if (rc != NPAIR_OK) return rc;
   c->step = npair_ctx::Step{d_label};
@@ -849,7 +882,15 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     if (r != 0) { c->err = fmt("ncclAllGather: %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
     c->step.x_total = c->Xtot_buf; c->step.lab_total = c->labtot_buf;
   } else { c->step.x_total = d_feat; c->step.lab_total = d_label; }
-  return forward_impl(c, d_feat, st);
+  return forward_impl(c, d_feat, tops, st);
+}
+
+// The asynchronous forward's finish: the tops and error bits go from the device TopsBlock to d_tops and the error word in stream order
+static int finish_forward_async(npair_ctx* c, float* d_tops, cudaStream_t st) {
+  launch_async_tops(c->aw, c->cfg.num_tops, d_tops, st);
+  CUDA_TRY(c, cudaGetLastError());
+  c->step.fwd_done = true;
+  return NPAIR_OK;
 }
 
 int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
@@ -857,10 +898,23 @@ int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float
   if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   int rc;
   if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
+  if ((rc = refuse_capture(c, stream, "npair_forward")) != NPAIR_OK) return rc;
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_rank(c, d_feat, d_label, call.st)) != NPAIR_OK) return rc;
+  if ((rc = forward_rank(c, d_feat, d_label, c->tops_dev, call.st)) != NPAIR_OK) return rc;
   return finish_forward(c, tops_host, call.st);
+}
+
+int npair_forward_async(npair_ctx* c, const float* d_feat, const float* d_label, float* d_tops, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !d_tops) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  bool captured = false;
+  if ((rc = async_entry(c, stream, "npair_forward_async", &captured)) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream, captured);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = forward_rank(c, d_feat, d_label, &c->aw->tops, call.st)) != NPAIR_OK) return rc;
+  return finish_forward_async(c, d_tops, call.st);
 }
 
 /* External-collectives variant: the caller already holds the all-gathered N x D features and N labels (rank r's rows are
@@ -868,8 +922,9 @@ int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float
 int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float* d_label_total, float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat_total || !d_label_total || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  OrderedCall call(c, stream);
   int rc;
+  if ((rc = refuse_capture(c, stream, "npair_forward_gathered")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
   if ((rc = set_call_rows(c, 0)) != NPAIR_OK) return rc;
   const long long r0 = static_cast<long long>(c->rank) * c->Q;
@@ -880,34 +935,64 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
     launch_l2norm_fwd(d_feat_total, c->N, c->D, normed, nullptr, call.st);
     launch_l2norm_fwd(d_feat_total + r0 * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
   }
-  if ((rc = forward_impl(c, c->step.x_total + r0 * c->D, call.st)) != NPAIR_OK) return rc;
+  if ((rc = forward_impl(c, c->step.x_total + r0 * c->D, c->tops_dev, call.st)) != NPAIR_OK) return rc;
   return finish_forward(c, tops_host, call.st);
 }
 
 /* Cross-batch memory (DESIGN 4.3): the database is [x; x_mem], Q + m rows, whose first Q are the anchors.  The memory rows are read
  * where they lie (two-source operand preparation), and their records in the table after the Q row records switch their transposed
  * gradient term off.  m = 0 is npair_forward. */
+static int memory_call_args(npair_ctx* c, int m) {
+  const int rc = validate_memory(&c->cfg, 1, &c->err);
+  if (rc != NPAIR_OK) return rc;
+  if (m < 0 || m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", m, c->mem_cap); return NPAIR_E_ARG; }
+  return NPAIR_OK;
+}
+// Enqueues npair_forward_memory with m > 0 memory rows, its tops going to `tops`
+static int forward_memory_rows(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label, int m,
+                               TopsBlock* tops, cudaStream_t st) {
+  const int rc = set_call_rows(c, m);
+  if (rc != NPAIR_OK) return rc;
+  c->step = npair_ctx::Step{d_label, nullptr, c->labcat};
+  c->step.x_mem = d_mem_feat; c->step.lab_mem = d_mem_label;
+  if (c->cfg.normalize_input) {               // the current rows only: the memory holds rows the layer has already seen
+    PhaseTimer pt(c, 1, st);
+    launch_l2norm_fwd(d_feat, c->Q, c->D, c->Ynorm, c->inv_norm, st);
+    d_feat = c->Ynorm;
+  }
+  c->step.x_total = d_feat;
+  return forward_impl(c, d_feat, tops, st);
+}
+
 int npair_forward_memory(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label, int32_t m,
                          float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !tops_host || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   int rc;
-  if ((rc = validate_memory(&c->cfg, 1, &c->err)) != NPAIR_OK) return rc;
-  if (m < 0 || m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", m, c->mem_cap); return NPAIR_E_ARG; }
+  if ((rc = memory_call_args(c, m)) != NPAIR_OK) return rc;
   if (m == 0) return npair_forward(c, d_feat, d_label, tops_host, stream);
+  if ((rc = refuse_capture(c, stream, "npair_forward_memory")) != NPAIR_OK) return rc;
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = set_call_rows(c, m)) != NPAIR_OK) return rc;
-  c->step = npair_ctx::Step{d_label, nullptr, c->labcat};
-  c->step.x_mem = d_mem_feat; c->step.lab_mem = d_mem_label;
-  if (c->cfg.normalize_input) {               // the current rows only: the memory holds rows the layer has already seen
-    PhaseTimer pt(c, 1, call.st);
-    launch_l2norm_fwd(d_feat, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
-    d_feat = c->Ynorm;
-  }
-  c->step.x_total = d_feat;
-  if ((rc = forward_impl(c, d_feat, call.st)) != NPAIR_OK) return rc;
+  if ((rc = forward_memory_rows(c, d_feat, d_label, d_mem_feat, d_mem_label, m, c->tops_dev, call.st)) != NPAIR_OK) return rc;
   return finish_forward(c, tops_host, call.st);
+}
+
+// A memory context captured into a graph holds the m of the capture: the tensor maps and the N-dependent plan of set_call_rows are
+// launch parameters, and the replay reads only the buffers they point at
+int npair_forward_memory_async(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label,
+                               int32_t m, float* d_tops, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !d_tops || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = memory_call_args(c, m)) != NPAIR_OK) return rc;
+  if (m == 0) return npair_forward_async(c, d_feat, d_label, d_tops, stream);
+  bool captured = false;
+  if ((rc = async_entry(c, stream, "npair_forward_memory_async", &captured)) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream, captured);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  if ((rc = forward_memory_rows(c, d_feat, d_label, d_mem_feat, d_mem_label, m, &c->aw->tops, call.st)) != NPAIR_OK) return rc;
+  return finish_forward_async(c, d_tops, call.st);
 }
 
 // What a kernel reads of rows [r0, r0 + rows) of the current step's S, which the S buffer holds from its row 0
@@ -937,7 +1022,7 @@ static cudaError_t recompute_sim_block(npair_ctx* c, int r0, cudaStream_t st) {
   return e;
 }
 
-static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
+static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   const int self_off = c->rank * Q;
@@ -1009,15 +1094,15 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
       if (c->lsel_mask && c->n_blocks > 1)
         launch_local_select(sim, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn, c->ra, c->bs, c->sms, lsel_warp, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
-      launch_lse_rows(sim, mp, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->world, c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr,
+      launch_lse_rows(sim, mp, c->ra, c->bs, c->cfg.num_tops, tops, c->world, c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr,
                       weight_scale_log2(c->prec), c->tops_seq, c->n_blocks == 1, st);
     }
-    if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
+    if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, tops, c->tops_seq, st);
     if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
       const float* all = nullptr;
       const int rc = xchg_small(c, c->xch_src, sizeof(TopSums) / sizeof(float), &all, st);
       if (rc != NPAIR_OK) return rc;
-      launch_tops_world(all, NPAIR_XCH_FLOATS, c->world, N, c->cfg.num_tops, c->tops_dev, c->tops_seq, st);
+      launch_tops_world(all, NPAIR_XCH_FLOATS, c->world, N, c->cfg.num_tops, tops, c->tops_seq, st);
     }
   }
   if (c->p2p_rec && !c->step.ext_gathered) {
@@ -1032,12 +1117,14 @@ static int forward_impl(npair_ctx* c, const float* d_feat, cudaStream_t st) {
   return NPAIR_OK;
 }
 
-static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
+// The loss weight of a backward: a host value, or (d_lw, world 1) one fp32 in device memory read in stream order
+struct LossWeight { float host; const float* dev; };
+static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
 // Backward_gpu (+ the projection of the fused L2Normalize producer: the kernels produce d loss / d y, the caller gets d loss / d x)
-static int backward_impl(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
-  if (!c->cfg.normalize_input) return backward_core(c, loss_weight, d_diff, d_total_ext, d_rs_ext, st);
+static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
+  if (!c->cfg.normalize_input) return backward_core(c, lw, d_diff, d_total_ext, d_rs_ext, st);
   if (d_total_ext) { c->err = "normalize_input: the partial (pre-all-reduce) backward is not available, its sum over ranks would have to be projected"; return NPAIR_E_STATE; }
-  const int rc = backward_core(c, loss_weight, c->dY, nullptr, d_rs_ext, st);
+  const int rc = backward_core(c, lw, c->dY, nullptr, d_rs_ext, st);
   if (rc != NPAIR_OK) return rc;
   PhaseTimer pt(c, 5, st);
   launch_l2norm_bwd(c->Ynorm, c->inv_norm, c->dY, c->Q, c->D, d_diff, st);
@@ -1063,7 +1150,20 @@ int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream)
   if ((rc = need_comm(c, "npair_backward_partial / npair_backward_gathered")) != NPAIR_OK) return rc;
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, loss_weight, d_diff, nullptr, nullptr, call.st);
+  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, call.st);
+}
+
+int npair_backward_device_weight(npair_ctx* c, const float* d_loss_weight, float* d_diff, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_loss_weight || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  bool captured = false;
+  if ((rc = async_entry(c, stream, "npair_backward_device_weight", &captured)) != NPAIR_OK) return rc;
+  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
+  if ((rc = need_forward(c, "npair_backward_device_weight")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream, captured);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  return backward_impl(c, LossWeight{0.f, d_loss_weight}, d_diff, nullptr, nullptr, call.st);
 }
 
 /* Forward + backward with ONE host synchronisation: the backward (whose loss weight is a constant of the net, top[0]'s diff)
@@ -1077,10 +1177,11 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
   int rc;
   if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
   if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
+  if ((rc = refuse_capture(c, stream, "npair_forward_backward")) != NPAIR_OK) return rc;
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_rank(c, d_feat, d_label, call.st)) != NPAIR_OK) return rc;
-  if ((rc = backward_impl(c, loss_weight, d_diff, nullptr, nullptr, call.st)) != NPAIR_OK) return rc;
+  if ((rc = forward_rank(c, d_feat, d_label, c->tops_dev, call.st)) != NPAIR_OK) return rc;
+  if ((rc = backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, call.st)) != NPAIR_OK) return rc;
   // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step.
   // finish_forward records `done` behind the backward
   return finish_forward(c, tops_host, call.st);
@@ -1101,7 +1202,7 @@ int npair_backward_partial(npair_ctx* c, float loss_weight, float* d_local_half,
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE; }
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, loss_weight, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, call.st);
+  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, call.st);
 }
 
 int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
@@ -1123,7 +1224,7 @@ int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_t
   if (c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE; }
   OrderedCall call(c, stream);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, loss_weight, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), call.st);
+  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), call.st);
 }
 
 // d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
@@ -1133,13 +1234,22 @@ static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, flo
   count_launch();
 }
 
-static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
+static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   // loss_weight / dot_normalizer (.cu:427,448); world scope: the normaliser is the world's batch and the transposed term is not
   // divided by the world size, i.e. exactly what a single rank holding the whole batch computes.  Times 2^-k: the row records build
   // every gradient weight at 2^k times its value (weight_scale_log2), an exact power of two that the GEMMs' alpha undoes
-  const float lw_over_q = ldexpf(loss_weight / static_cast<float>(c->wscope ? N : Q), -weight_scale_log2(c->prec));
+  const float lw_over_q = ldexpf(lw.host / static_cast<float>(c->wscope ? N : Q), -weight_scale_log2(c->prec));
+  // The gradient GEMMs scale their accumulators by alpha * *dev_scale.  A device loss weight (world 1: no transposed-term GEMM) enters
+  // through dev_scale instead: grad_scale_kernel writes the host's 0.5f * lw_over_q times the inverse pre-scale, in the same fp32
+  // operations, and alpha = 1 leaves it unchanged, so the gradient has the bits of the host weight of the same value
+  float alpha = 0.5f * lw_over_q;
+  const float* dev_scale = &c->bs->x_inv_scale;
+  if (lw.dev) {
+    launch_grad_scale(lw.dev, c->wscope ? N : Q, weight_scale_log2(c->prec), c->bs, c->aw, st);
+    alpha = 1.f; dev_scale = &c->aw->grad_scale;
+  }
   const bool tc = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
   const RowRecord* rs_total = nullptr;
   int bw_mode = BW_SYM;
@@ -1176,7 +1286,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     fp.inv_world = c->wscope ? 1.f : 1.f / static_cast<float>(c->world);
     fp.log2_world = c->wscope ? 0.f : log2f(static_cast<float>(c->world));
     fp.sgn_p = ap_sign(mp.ap_method); fp.sgn_n = an_sign(mp.an_method);
-    fp.ldo = D; fp.alpha = 0.5f * lw_over_q; fp.beta = 0.f; fp.dev_scale = &c->bs->x_inv_scale;
+    fp.ldo = D; fp.alpha = alpha; fp.beta = 0.f; fp.dev_scale = dev_scale;
     fp.part = c->part;
     fp.chunk_kb = c->grad_chunk_kb;
     // per block of rows of S, starting with the one the forward left in the buffer (a materialised S is the one block): recompute it,
@@ -1202,7 +1312,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
     launch_build_weights(sim_rows(c, 0, Q), c->world, bw_mode, rs_total, mp, c->ra, c->prec, c->H, c->Np, c->HT, c->Qp, st);
   }
   GemmParams gp; memset(&gp, 0, sizeof(gp));
-  gp.dev_scale = &c->bs->x_inv_scale;
+  gp.dev_scale = dev_scale;
   const bool rs_path = c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER;
   if (rs_path) {
     // total = (1/2)(1/k)(lw/Q) * G^T . X_local  (N x D)  -> reduce-scatter (== all-reduce + own slice, .cu:462-497)
@@ -1222,7 +1332,7 @@ static int backward_core(npair_ctx* c, float loss_weight, float* d_diff, float* 
   }
   // d_diff = (1/2)(lw/Q) * H . X_total  (H = G + G^T/world in the symmetric modes; accumulated onto the scattered term otherwise)
   gp.M = Q; gp.Nn = D; gp.ts = tile_sched(Q, D, c->grad_kblocks, c->grad_split);
-  gp.out = d_diff; gp.ldo = D; gp.alpha = 0.5f * lw_over_q; gp.beta = (rs_path && !d_total_ext) ? 1.f : 0.f;
+  gp.out = d_diff; gp.ldo = D; gp.alpha = alpha; gp.beta = (rs_path && !d_total_ext) ? 1.f : 0.f;
   gp.part = c->part;
   {
     PhaseTimer pt(c, 6, st);
@@ -1261,14 +1371,30 @@ static int await_calls(npair_ctx* c) {
 
 int npair_profile_read(npair_ctx* c, float* ms_out) {
   if (!c || !ms_out) return NPAIR_E_ARG;
-  const int rc = await_calls(c);
-  if (rc != NPAIR_OK) return rc;
+  int rc;
+  if ((rc = refuse_in_capture(c, "npair_profile_read")) != NPAIR_OK) return rc;
+  if ((rc = await_calls(c)) != NPAIR_OK) return rc;
   for (int i = 0; i < NPAIR_PROF_PHASES; ++i) {
     ms_out[i] = 0.f;
     if (c->ev_made && c->ev_used[i]) { float ms = 0.f; CUDA_TRY(c, cudaEventElapsedTime(&ms, c->ev[i][0], c->ev[i][1])); ms_out[i] = ms; }
     c->ev_used[i] = false;
   }
   return NPAIR_OK;
+}
+
+int npair_async_status(npair_ctx* c) {
+  if (!c) return NPAIR_E_ARG;
+  if (c->world != 1) { c->err = "npair_async_status is world-1 only"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = refuse_in_capture(c, "npair_async_status")) != NPAIR_OK) return rc;
+  if ((rc = await_calls(c)) != NPAIR_OK) return rc;
+  unsigned int err = 0;
+  CUDA_TRY(c, cudaMemcpy(&err, &c->aw->err, sizeof(err), cudaMemcpyDeviceToHost));
+  if (!err) return NPAIR_OK;
+  CUDA_TRY(c, cudaMemset(&c->aw->err, 0, sizeof(err)));
+  if (err & DERR_EMPTY_LIST) { c->err = "an asynchronous forward indexed an empty same/diff list (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
+  c->err = "an asynchronous forward's identsn/diffsn selected a position outside the list (undefined behaviour in the reference, .cu:285-288)";
+  return NPAIR_E_POS_RANGE;
 }
 
 __global__ void decode_ord_kernel(const uint32_t* __restrict__ in, float* __restrict__ out, int n) {
@@ -1282,8 +1408,9 @@ __global__ void int_to_float_kernel(const int* __restrict__ in, float* __restric
 
 int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
   if (!c || !dst) return NPAIR_E_ARG;
-  const int rc = await_calls(c);
-  if (rc != NPAIR_OK) return rc;
+  int rc;
+  if ((rc = refuse_in_capture(c, "npair_debug_read")) != NPAIR_OK) return rc;
+  if ((rc = await_calls(c)) != NPAIR_OK) return rc;
   const int Q = c->Q, N = c->N;
   if (which == 0) {
     if (c->n_blocks > 1) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }

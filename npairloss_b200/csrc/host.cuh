@@ -224,21 +224,34 @@ inline void carve_stats(Carve& cv, long long rows, RowArrays* ra) {
 // object's device current and waits for the previous call when that ran on another stream (StreamOrder), failures going to the object's
 // `err`.  `done` is recorded at the latest when the call returns, also after an error (what it enqueued before failing is still
 // running).  A call refused before enter() enqueues nothing and records nothing.
+// A call captured into a CUDA graph (`captured`) neither waits nor records: the event lies outside the capture, and one recorded inside
+// it would be a node of the graph that no eager call may wait on.  The caller orders the context's earlier work before the capture and
+// the replays against its eager calls (npair_b200.h, graph capture).
 template <class Obj>
 struct OrderedCall {
-  OrderedCall(Obj* obj_, void* stream) : obj(obj_), st(static_cast<cudaStream_t>(stream)) {}
+  OrderedCall(Obj* obj_, void* stream, bool captured_ = false) : obj(obj_), st(static_cast<cudaStream_t>(stream)), captured(captured_) {}
   OrderedCall(const OrderedCall&) = delete;
   int enter() {
     StreamOrder& o = obj->order;
     CUDA_TRY(obj, cudaSetDevice(obj->device));
-    if (o.recorded && o.stream != st) CUDA_TRY(obj, cudaStreamWaitEvent(st, o.done, 0));
-    o.open = true;
+    if (!captured && o.recorded && o.stream != st) CUDA_TRY(obj, cudaStreamWaitEvent(st, o.done, 0));
+    o.open = !captured;
     return NPAIR_OK;
   }
   ~OrderedCall() { obj->order.mark(st); }
   Obj* const obj;
   const cudaStream_t st;
+  const bool captured;
 };
+
+// The capture `st` takes part in: its id, 0 when the stream is not capturing.  A query that fails (the legacy stream while another
+// stream captures in global mode) counts as a capture, with id ~0.
+inline unsigned long long capture_id(cudaStream_t st) {
+  cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+  unsigned long long id = 0;
+  if (cudaStreamGetCaptureInfo(st, &s, &id) != cudaSuccess) { cudaGetLastError(); return ~0ull; }
+  return s == cudaStreamCaptureStatusNone ? 0 : (id ? id : ~0ull);
+}
 
 // Makes `device` (< 0: the current one) current for a new context or evaluator, which needs an sm_90 device; its id and SM count
 // (ctx.cu).  Its failures go to g_create_err.

@@ -871,6 +871,29 @@ void launch_tops_world(const float* xall, int xstride, int world, long long N, i
   count_launch();
 }
 
+__global__ void async_tops_kernel(AsyncWords* __restrict__ aw, int num_tops, float* __restrict__ d_tops) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const int err = aw->tops.err & (DERR_EMPTY_LIST | DERR_POS_RANGE);
+  for (int t = 0; t < 5; ++t) d_tops[t] = err ? __int_as_float(0x7fc00000) : (t < num_tops ? aw->tops.tops[t] : 0.f);
+  aw->err |= static_cast<unsigned int>(err);
+}
+void launch_async_tops(AsyncWords* aw, int num_tops, float* d_tops, cudaStream_t st) {
+  async_tops_kernel<<<1, 32, 0, st>>>(aw, num_tops, d_tops);
+  count_launch();
+}
+// The fp32 operations of backward_core's host alpha (lw_over_q, then 0.5f times it) and of the GEMMs' alpha * *dev_scale, in order:
+// IEEE division and multiplications (no fast math), and an exact ldexpf
+__global__ void grad_scale_kernel(const float* __restrict__ d_lw, int Q, int wlog2, const BlockScalars* __restrict__ bs,
+                                  AsyncWords* __restrict__ aw) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const float lw_over_q = ldexpf(__fdiv_rn(*d_lw, static_cast<float>(Q)), -wlog2);
+  aw->grad_scale = __fmul_rn(__fmul_rn(0.5f, lw_over_q), bs->x_inv_scale);
+}
+void launch_grad_scale(const float* d_lw, int Q, int wlog2, const BlockScalars* bs, AsyncWords* aw, cudaStream_t st) {
+  grad_scale_kernel<<<1, 32, 0, st>>>(d_lw, Q, wlog2, bs, aw);
+  count_launch();
+}
+
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st) {
   l2norm_fwd_kernel<<<(rows + 7) / 8, 256, 0, st>>>(x, rows, dim, y, inv_norm);
   count_launch();

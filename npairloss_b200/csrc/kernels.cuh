@@ -139,6 +139,15 @@ struct TopsBlock {
   unsigned int seq;
 };
 
+// The asynchronous step's words in device memory (npair_forward_async, npair_backward_device_weight; DESIGN 4.4): the forward publishes
+// its tops here instead of to the host, the error bits of its forwards gather until npair_async_status, and a backward's gradient
+// scale is computed here from the device loss weight
+struct AsyncWords {
+  TopsBlock tops;
+  unsigned int err;        // DERR_* bits of the asynchronous forwards since the last status call
+  float grad_scale;        // (1/2)(lw/Q) 2^-k times the operand's inverse pre-scale: the gradient GEMMs' alpha * *dev_scale
+};
+
 // Global (per-rank-block) scalars living in device memory.
 struct BlockScalars {
   unsigned long long n_same, n_diff;       // sizes of ident_global / diff_global (.cu:225-265)
@@ -272,6 +281,12 @@ enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
 // over the rank's whole S (sim.row0 == 0, sim.rows == Q)
 void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH /*Np*/, uint16_t* HT, long long ldHT /*Qp*/, cudaStream_t st);
+// The asynchronous forward's finish: d_tops[0, 5) = what the host would read of aw->tops (0 past num_tops), or NaN with the error bits
+// added to aw->err when a DERR_EMPTY_LIST / DERR_POS_RANGE bit is set
+void launch_async_tops(AsyncWords* aw, int num_tops, float* d_tops, cudaStream_t st);
+// aw->grad_scale = (0.5f * ldexpf(*d_lw / Q, -wlog2)) * bs->x_inv_scale: the host's alpha of the gradient GEMMs times their device scale,
+// in the same fp32 operations
+void launch_grad_scale(const float* d_lw, int Q, int wlog2, const BlockScalars* bs, AsyncWords* aw, cudaStream_t st);
 void launch_l2norm_fwd(const float* x, int rows, int dim, float* y, float* inv_norm, cudaStream_t st);
 void launch_l2norm_bwd(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx, cudaStream_t st);
 

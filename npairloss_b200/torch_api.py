@@ -21,6 +21,12 @@ CROSS-BATCH MEMORY.  NPairLoss(memory_rows=M) (world = 1) keeps the last M embed
 passes them to every forward as extra database rows (npair_forward_memory, DESIGN 4.3; Wang et al., CVPR 2020): they take part in the
 mining and in the softmax of the current anchors but receive no gradient.  reset_memory() empties the ring, so when the memory starts
 (XBM warms up for some iterations first) is the caller's choice.
+
+ASYNCHRONOUS STEP.  NPairLoss(blocking=False) (world = 1) makes no host synchronisation: the forward writes the tops into a 5-float CUDA
+tensor (npair_forward_async) and the loss is its element 0 on the device; the backward reads grad_loss on the device
+(npair_backward_device_weight) instead of calling .item().  Same values, bit for bit, as blocking=True.  A whole training step through it
+can be captured with torch.cuda.graph (DESIGN 4.4); a device error (the cases the blocking forward raises for) gives NaN tops and is
+reported by async_status().  With memory_rows > 0 it runs eagerly only: the ring's head is Python state that a graph would freeze.
 """
 from __future__ import annotations
 
@@ -51,14 +57,21 @@ class _NPairFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, label, owner):
         layer = owner._context(feat)
-        if owner._mem_cap:
-            tops = owner._forward_memory(layer, feat, label)
+        if owner._blocking:
+            if owner._mem_cap:
+                tops = owner._forward_memory(layer, feat, label)
+            else:
+                tops = layer.forward(feat, label)             # blocks until the five scalars are on the host (as the reference)
+            t = torch.tensor(tops, dtype=torch.float32, device=feat.device)
         else:
-            tops = layer.forward(feat, label)                 # blocks until the five scalars are on the host (as the reference)
+            t = torch.empty(5, dtype=torch.float32, device=feat.device)   # under capture: from the graph's pool
+            if owner._mem_cap:
+                owner._forward_memory(layer, feat, label, t)
+            else:
+                layer.forward_async(feat, label, t)
         owner._generation += 1
         ctx.owner, ctx.layer, ctx.generation = owner, layer, owner._generation
         ctx.save_for_backward(feat, label)                    # the C ABI wants both unchanged until the backward is enqueued
-        t = torch.tensor(tops, dtype=torch.float32, device=feat.device)
         ctx.mark_non_differentiable(t)
         return t[0].clone(), t
 
@@ -69,8 +82,11 @@ class _NPairFunction(torch.autograd.Function):
                                "context holds the newer batch.  Use one NPairLoss module per outstanding graph.")
         feat, _label = ctx.saved_tensors
         diff = torch.empty_like(feat)
-        # the reference scales by top[0]->cpu_diff()[0] (.cu:435): a host scalar, hence the .item()
-        ctx.layer.backward(float(grad_loss.item()), diff)
+        if ctx.owner._blocking:
+            # the reference scales by top[0]->cpu_diff()[0] (.cu:435): a host scalar, hence the .item()
+            ctx.layer.backward(float(grad_loss.item()), diff)
+        else:
+            ctx.layer.backward_device_weight(grad_loss.detach().to(torch.float32).contiguous().reshape(1), diff)
         if ctx.owner._true_gradient:
             diff.mul_(2.0)
         return diff, None, None
@@ -84,11 +100,16 @@ class NPairLoss(torch.nn.Module):
     memory_rows=M > 0 (world = 1 only): a cross-batch memory of the last M rows this module has seen.  Each forward passes the ring's
     m = min(rows enqueued, M) valid rows, slots 0 .. m-1 in slot order, and then enqueues the batch's own rows, detached (under
     normalize_input the normalised rows the layer used), so a batch is never in the memory during its own step.  The ring survives the
-    context being re-created for a new batch size; it is emptied when the dimension or device changes and by reset_memory()."""
+    context being re-created for a new batch size; it is emptied when the dimension or device changes and by reset_memory().
+
+    blocking=False (world = 1 only): the asynchronous step of the module docstring.  The loss and the tops are computed on the device and
+    nothing waits for them; async_status() reports a device error of the forwards since the last call."""
 
     def __init__(self, world: int = 1, rank: int = 0, nccl_id: bytes | None = None, true_gradient: bool = False, _context_factory=None,
-                 memory_rows: int = 0, **config):
+                 memory_rows: int = 0, blocking: bool = True, **config):
         super().__init__()
+        if not blocking and world != 1:
+            raise ValueError("blocking=False is defined for world = 1 (the multi-rank exchanges keep host state per step)")
         if true_gradient and world != 1:
             raise ValueError("true_gradient is defined for world = 1 (the reference's multi-rank blend is not a gradient of one loss)")
         if int(memory_rows) < 0:
@@ -106,6 +127,7 @@ class NPairLoss(torch.nn.Module):
         self._ctx, self._key = None, None
         self._generation = 0
         self._true_gradient = bool(true_gradient)
+        self._blocking = bool(blocking)
         self._mem_x = self._mem_l = None      # the ring: [M, D] rows and [M] fp32 labels, allocated at the first forward
         self._mem_count = 0                   # rows enqueued since the last reset (the valid slots are 0 .. min(count, M) - 1)
 
@@ -120,14 +142,23 @@ class NPairLoss(torch.nn.Module):
             return None, None
         return self._mem_x[:m], self._mem_l[:m]
 
-    def _forward_memory(self, layer, feat, label):
+    def async_status(self):
+        """blocking=False: waits for the module's last library call and raises capi.NpairError if a forward since the previous call met a
+        device error (its tops are NaN); nothing to report before the first forward."""
+        if self._ctx is not None:
+            self._ctx.async_status()
+
+    def _forward_memory(self, layer, feat, label, tops_out=None):
         d = feat.shape[1]
         if self._mem_x is None or self._mem_x.shape[1] != d or self._mem_x.device != feat.device:
             self._mem_x = torch.empty(self._mem_cap, d, dtype=torch.float32, device=feat.device)
             self._mem_l = torch.empty(self._mem_cap, dtype=torch.float32, device=feat.device)
             self._mem_count = 0
         m = min(self._mem_count, self._mem_cap)
-        tops = layer.forward_memory(feat, label, self._mem_x, self._mem_l, m)
+        if tops_out is None:
+            tops = layer.forward_memory(feat, label, self._mem_x, self._mem_l, m)
+        else:
+            tops = layer.forward_memory_async(feat, label, self._mem_x, self._mem_l, m, tops_out)
         # the forward has read the memory: this batch's rows go in behind it, in stream order
         rows = feat.detach()
         if self._config.get("normalize_input"):
@@ -162,6 +193,9 @@ class NPairLoss(torch.nn.Module):
     def forward(self, feat, label):
         if feat.dtype != torch.float32:
             raise TypeError("NPairLoss computes in fp32 like the reference (Dtype=float); cast the embeddings")
+        if not self._blocking and self._mem_cap and feat.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("NPairLoss(memory_rows > 0, blocking=False) cannot be captured into a CUDA graph: the memory ring's head "
+                               "and count are Python state that the graph would freeze")
         feat2 = feat.reshape(feat.shape[0], -1).contiguous()
         label = _fp32_labels(label).contiguous()               # labels are stored as Dtype in the reference (bottom[1])
         loss, tops = _NPairFunction.apply(feat2, label, self)
