@@ -275,7 +275,11 @@ int npair_util_f32_to_f64(const float* d_src, double* d_dst, size_t n, void* str
 /* Introspection for parity tests (copies device scratch to host; waits for the work of the context's last call, on any stream).
  * which: 0 = S (Q x N similarities, row-major, ld = N; NPAIR_E_STATE in row-block similarity mode)      1 = posi_thr[Q]   2 = nega_thr[Q]
  *        3 = min_within[Q]  4 = max_between[Q]  5 = max_all[Q]  6 = A[Q]  7 = T[Q]  8 = same-label count[Q]
- *        9 = max_within[Q]  10 = operand pre-scale (1 float) */
+ *        9 = max_within[Q]  10 = operand pre-scale (1 float)  11 = log(A/T)[Q] (0 where A or T is 0)
+ *        12 = retrieval hit flags [3][Q] for k = 1, 5, 10, as 0 / 1
+ * Statistics of a row with no same-label column keep their reset values: min_within FLT_MAX, max_within -FLT_MAX, count 0 (and
+ * max_between -FLT_MAX with no diff-label column).  A and T are fp32 sums of ex2.approx.ftz(s log2(e) - max_all log2(e)) over the
+ * selected pairs: a term below 2^-126 is 0 (DESIGN 5). */
 int npair_debug_read(npair_ctx* ctx, int which, float* host_dst, size_t n_floats);
 
 /* 1 if a similarity matrix computed on this device with every tile (no mirroring) in operand format `precision` comes out bitwise

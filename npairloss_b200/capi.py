@@ -330,6 +330,7 @@ class Context:
         return [ms[i] for i in range(9)]
 
     def debug_read(self, which: int, n: int):
+        """npair_debug_read: n floats of introspection array `which` (0 = S, Q x N; 12 = the hit flags, 3 x Q; 10 = one float; else Q)."""
         import numpy as np
         out = np.zeros(n, dtype=np.float32)
         self._check(lib().npair_debug_read(self._h, which, out.ctypes.data_as(C.POINTER(C.c_float)), n))

@@ -1423,7 +1423,8 @@ int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
     CUDA_TRY(c, cudaMemcpy(dst, &c->bs->x_scale, sizeof(float), cudaMemcpyDeviceToHost));
     return NPAIR_OK;
   }
-  if (n < static_cast<size_t>(Q)) { c->err = "buffer too small"; return NPAIR_E_ARG; }
+  const int cnt = which == 12 ? 3 * Q : Q;       // 12: the three hit flags, k = 1, 5, 10
+  if (n < static_cast<size_t>(cnt)) { c->err = "buffer too small"; return NPAIR_E_ARG; }
   const float* src = nullptr; const uint32_t* osrc = nullptr; const int* isrc = nullptr;
   switch (which) {
     case 1: src = c->ra.posi_thr; break;
@@ -1435,14 +1436,16 @@ int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
     case 7: src = c->ra.T; break;
     case 8: isrc = c->ra.cnt_same; break;
     case 9: osrc = c->ra.st_maxw; break;
+    case 11: src = c->ra.logv; break;
+    case 12: isrc = c->ra.hits; break;
     default: c->err = "unknown debug selector"; return NPAIR_E_ARG;
   }
-  if (src) { CUDA_TRY(c, cudaMemcpy(dst, src, sizeof(float) * Q, cudaMemcpyDeviceToHost)); return NPAIR_OK; }
+  if (src) { CUDA_TRY(c, cudaMemcpy(dst, src, sizeof(float) * cnt, cudaMemcpyDeviceToHost)); return NPAIR_OK; }
   float* tmp = nullptr;
-  CUDA_TRY(c, cudaMalloc(&tmp, sizeof(float) * Q));
-  if (osrc) decode_ord_kernel<<<(Q + 255) / 256, 256>>>(osrc, tmp, Q);
-  else int_to_float_kernel<<<(Q + 255) / 256, 256>>>(isrc, tmp, Q);
-  cudaError_t e = cudaMemcpy(dst, tmp, sizeof(float) * Q, cudaMemcpyDeviceToHost);
+  CUDA_TRY(c, cudaMalloc(&tmp, sizeof(float) * cnt));
+  if (osrc) decode_ord_kernel<<<(cnt + 255) / 256, 256>>>(osrc, tmp, cnt);
+  else int_to_float_kernel<<<(cnt + 255) / 256, 256>>>(isrc, tmp, cnt);
+  cudaError_t e = cudaMemcpy(dst, tmp, sizeof(float) * cnt, cudaMemcpyDeviceToHost);
   cudaFree(tmp);
   CUDA_TRY(c, e);
   return NPAIR_OK;

@@ -619,7 +619,16 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
       const float invA = A == 0.f ? 0.f : 1.f / A;              // Get_Query_Diff_Part zero rules (.cu:410-415)
       const float invT = T == 0.f ? 0.f : 1.f / T;
       const float cA = invT - invA;
-      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + m2c_off, thr_n, m2, li, thr_p, cA * wscale, invT * wscale);
+      // The factors 2^k / A and 2^k / T overflow for sums below about 2^(k - 128) (selected positives ~79 nats below the row maximum
+      // at k = 14).  Such a row moves 2^j of its factors into its exponent offset: the builders' exponential 2^(s log2(e) - (m2 - j))
+      // is e 2^j <= 2^j, the factors are 2^(k - j) / A, and every weight e 2^j * 2^(k - j) (1/T - 1/A) keeps its value in
+      // [-2^k, 2^k].  j = max(0, k - 127 - floor(log2 A)) <= k - 1 (a nonzero A is a sum of normal terms, >= 2^-126) leaves every
+      // factor below 2^127; rows with j = 0 keep every bit.  m2c carries no j: it is only an exponent offset of 2^k e / T / world.
+      const float amin = A > 0.f ? A : T;
+      const int j = amin > 0.f ? max(0, ilogbf(wscale) - 127 - ilogbf(amin)) : 0;
+      const float fsc = ldexpf(wscale, -j);
+      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + m2c_off, thr_n, m2 - static_cast<float>(j), li, thr_p,
+                                     cA * fsc, invT * fsc);
     }
   }
   if (!finalize) return;

@@ -68,13 +68,13 @@ __device__ __forceinline__ float an_thr(float t, int m) {     // diff-label rule
 // What the backward needs of one row, written by the forward row pass (lse_rows_kernel).  It crosses GPUs as raw bytes (peer-memory
 // pushes, the NCCL all-gather, npair_row_scalars / npair_backward_gathered), so this is the one description of its layout.  The two
 // 16-byte halves are loaded and stored as vectors; the first holds all that a diff-label pair needs.
-//   m2     max_all * log2(e), the row's exponent offset
-//   m2c    m2 + log2(T) + log2(world) - k (+inf when T == 0): a diff-label weight 2^k exp(s - max) / T / world is ONE exponential
-//          2^(s*log2(e) - m2c)
+//   m2     max_all * log2(e) - j, the row's exponent offset
+//   m2c    max_all * log2(e) + log2(T) + log2(world) - k (+inf when T == 0): a diff-label weight 2^k exp(s - max) / T / world is ONE
+//          exponential 2^(s*log2(e) - m2c)
 //   thr_n  the an_thr-transformed diff-label threshold;  thr_p  the ap_thr-transformed same-label threshold
-//   cA     same-label weight factor 2^k (1/T - 1/A);  cT  diff-label weight factor 2^k / T
-// so every gradient weight built from records comes out scaled by 2^k, k = weight_scale_log2(format), and the gradient GEMM's alpha
-// carries 2^-k.
+//   cA     same-label weight factor 2^(k-j) (1/T - 1/A);  cT  diff-label weight factor 2^(k-j) / T
+// so every gradient weight built from records, 2^(s*log2(e) - m2) times a factor, comes out scaled by 2^k, k = weight_scale_log2(format),
+// and the gradient GEMM's alpha carries 2^-k.  j is 0 except on rows whose 2^k / A or 2^k / T could pass 2^127 (lse_rows_kernel).
 struct RowRecord {
   float4 lo, hi;   // {m2c, thr_n, m2, label}, {thr_p, cA, cT, 0}
   __host__ __device__ static RowRecord make(float m2c, float thr_n, float m2, float label, float thr_p, float cA, float cT) {
@@ -101,7 +101,8 @@ static_assert(sizeof(RowRecord) == 32, "row records are exchanged as 32 raw byte
 // log2 of the scale the gradient weights of format `prec` are built at.  An fp16x2 weight is split into fp16 hi + lo pieces; unscaled,
 // the lo piece of a weight below about 2^-3 falls into fp16's subnormal range (spacing 2^-24), an absolute error of up to 2^-25 per
 // weight, which does not average out when the rows are clustered and their weights nearly equal.  Every weight lies in [-1, 1]
-// (exp(s - max) / T and exp(s - max) (1/T - 1/A) with exp(s - max) <= A <= T), and the world-1 operand H = g'(j, m) + g'(m, j) in
+// (exp(s - max) / T and exp(s - max) (1/T - 1/A) with exp(s - max) <= A <= T; the factors 1/A and 1/T alone do not, and the row
+// record's exponent offset absorbs what of 2^k / A would overflow, RowRecord), and the world-1 operand H = g'(j, m) + g'(m, j) in
 // [-2, 2]; 2^14 * 2 = 32768 stays below fp16's largest finite 65504 (2^15 * 2 would not), so k = 14 is the largest safe scale and
 // keeps the lo piece normal down to weights of about 2^-17.  bf16 pieces have fp32's exponent range: no scale.
 __host__ __device__ constexpr int weight_scale_log2(int prec) { return prec == PREC_FP16X2 ? 14 : 0; }

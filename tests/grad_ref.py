@@ -150,9 +150,10 @@ def step_memory(x, lab, x_mem, lab_mem, S, loss_weight=1.0, **mining):
     return res
 
 
-def violations(dx, ref, tau, rel=1e-5, k_sgemm=2.0):
+def violations(dx, ref, tau, rel=1e-5, k_sgemm=2.0, floor=TINY, row_extra=0.0):
     """The rules of the module docstring that dx breaks (empty: it passes), and the measured quantities: normwise error, the worst row's
-    error over its allowance (rel and k_sgemm times the SGEMM's error), and the largest |dx - R| / B in units of 2^-24."""
+    error over its allowance (rel and k_sgemm times the SGEMM's error), and the largest |dx - R| / B in units of 2^-24.  floor: the
+    componentwise rule's absolute floor (TINY, or an array broadcast against dx); row_extra: an allowance added to every row's."""
     dx = np.asarray(dx, dtype=np.float64)
     R, B, R32 = ref["R"], ref["B"], ref["R32"]
     e = dx - R
@@ -163,7 +164,7 @@ def violations(dx, ref, tau, rel=1e-5, k_sgemm=2.0):
     if not nE <= max(rel * nR, k_sgemm * n32):
         bad.append(f"normwise {nE / max(nR, TINY):.3e} of |R| (allowed {max(rel * nR, k_sgemm * n32) / max(nR, TINY):.3e})")
     rR, rE, r32 = (np.linalg.norm(a, axis=1) for a in (R, e, R32 - R))
-    allow = np.maximum(rel * rR, k_sgemm * r32) + TINY
+    allow = np.maximum(rel * rR, k_sgemm * r32) + row_extra + TINY
     row_ratio = rE / allow
     if not (row_ratio <= 1).all():
         i = int(np.nanargmax(row_ratio))
@@ -171,7 +172,7 @@ def violations(dx, ref, tau, rel=1e-5, k_sgemm=2.0):
     with np.errstate(divide="ignore", invalid="ignore"):
         ratio = np.where(np.abs(e) <= TINY, 0.0, np.abs(e) / B)
     comp = float(np.nanmax(ratio)) / U24 if ratio.size else 0.0
-    over = ~(np.abs(e) <= tau * B + TINY)
+    over = ~(np.abs(e) <= tau * B + floor)
     if over.any():
         i, j = np.unravel_index(int(np.argmax(np.where(over, ratio, -1.0))), e.shape)
         bad.append(f"componentwise: {int(over.sum())} elements, worst ({i}, {j}) at {comp:.1f} x 2^-24 of B (tau {tau / U24:.1f})")
