@@ -131,12 +131,30 @@ bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int 
   return true;
 }
 
-// The similarity GEMM's operand maps over K-concatenated rows of kcat elements (split_kernel): `a` over rows_a rows from A (128-row
-// boxes), `b` over rows_b rows from B (256-row boxes), both in 64-element K blocks
-bool make_tmap_kcat(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, long long kcat,
-                    std::string* err) {
-  return make_tmap_pieces(a, A, static_cast<int>(kcat), rows_a, 1, kcat, rows_a * kcat, 64, 128, err) &&
-         make_tmap_pieces(b, B, static_cast<int>(kcat), rows_b, 1, kcat, rows_b * kcat, 64, 256, err);
+// 4-D map over one side of the similarity GEMM's pieced operands (SimLayout, pieces >= 2): {8 * bk elements, pieces, K blocks, row
+// groups}, box {8 * bk, pieces, 1, box_rows / 8}, no swizzle -- a stage receives [row group][slot][bk / 8 core matrices]
+static bool make_tmap_sim_side(CUtensorMap* m, const void* base, int rows, SimLayout L, int box_rows, std::string* err) {
+  auto fn = tmap_encode_fn();
+  if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
+  const cuuint64_t blk = 8ull * L.bk(), kbs = static_cast<cuuint64_t>(L.Dp / L.bk());
+  cuuint64_t dims[4] = {blk, static_cast<cuuint64_t>(L.pieces), kbs, static_cast<cuuint64_t>(L.padded_rows(rows) / 8)};
+  cuuint64_t strides[3] = {blk * 2ull, blk * 2ull * L.pieces, blk * 2ull * L.pieces * kbs};
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(blk), static_cast<cuuint32_t>(L.pieces), 1u, static_cast<cuuint32_t>(box_rows / 8)};
+  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *err = fmt("cuTensorMapEncodeTiled(sim) failed (%d): rows=%d pieces=%d Dp=%lld", (int)r, rows, L.pieces, L.Dp); return false; }
+  return true;
+}
+
+// The similarity GEMM's operand maps (SimLayout L, written by split_kernel / eval_split_kernel): `a` over rows_a rows from A (128-row
+// boxes), `b` over rows_b rows from B (256-row boxes), both in the layout's K blocks
+bool make_tmap_sim(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, SimLayout L,
+                   std::string* err) {
+  if (L.pieces == 1)
+    return make_tmap_pieces(a, A, static_cast<int>(L.Dp), rows_a, 1, L.Dp, rows_a * L.Dp, L.bk(), 128, err) &&
+           make_tmap_pieces(b, B, static_cast<int>(L.Dp), rows_b, 1, L.Dp, rows_b * L.Dp, L.bk(), 256, err);
+  return make_tmap_sim_side(a, A, rows_a, L, 128, err) && make_tmap_sim_side(b, B, rows_b, L, 256, err);
 }
 
 // 2-D fp32 map over the similarity matrix [rows x ld], inner extent `cols`, box {32, 32}, 128B swizzle (TMA stores)
@@ -248,10 +266,10 @@ static int select_mask(const npair_config& c, int region) {
 struct Plan {
   int N, nsplit, bk_grad;
   long long Dp, Np, Qp, ldS;     // padded feature / all-rows / local-rows extents of the operand pieces, row stride of S
-  long long kcat;                // K extent of the similarity GEMM's operands: mma_passes(nsplit) * Dp (PREC_BF16: Xs, one piece)
+  SimLayout sim;                 // layout of the similarity GEMM's operands (PREC_BF16: Xs, whose one piece is that layout)
   int bwd_mode;                  // NPAIR_BWDMODE_*
   bool fused_grad;               // the gradient weights are produced inside the gradient GEMM: no H in HBM
-  bool cat;                      // the similarity GEMM reads the K-concatenated operands XcatA / XcatB, not Xs
+  bool cat;                      // the similarity GEMM reads its own operands XcatA / XcatB (SimLayout), not Xs
   unsigned int gcand_cap;        // entries per side of the GLOBAL radix select's candidate lists
   int grad_chunk_kb;             // accumulation chunk of the gradient GEMM in 32-column K blocks (grad_fused.cuh); 0 = unchunked
   int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
@@ -277,7 +295,7 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric, int me
   p.N = static_cast<int>(N);
   p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
-  p.kcat = mma_passes(p.nsplit) * p.Dp;
+  p.sim = SimLayout{p.nsplit, p.Dp};
   const int blk_rows = sim_block_rows(cfg);
   p.s_rows = blk_rows ? blk_rows : cfg.Q;
   p.n_blocks = (cfg.Q + p.s_rows - 1) / p.s_rows;
@@ -338,7 +356,7 @@ struct npair_ctx : Plan {
   float* S = nullptr;
   uint16_t *Xs = nullptr, *XsT = nullptr, *XlT = nullptr, *H = nullptr, *HT = nullptr;
   float* OUT2 = nullptr;         // world > 1: N x D transposed-term product before the reduce-scatter
-  uint16_t *XcatA = nullptr, *XcatB = nullptr;   // K-concatenated operands [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3)
+  uint16_t *XcatA = nullptr, *XcatB = nullptr;   // the similarity GEMM's operands (SimLayout): the rank's Q anchors, all N rows
   RowRecord* rs_total = nullptr;   // row-scalar mode: the world's N row records, all-gathered
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
@@ -367,7 +385,7 @@ struct npair_ctx : Plan {
   // the capture a call of this context was last enqueued into (npair_b200.h, graph capture): the stream-less calls that wait for the
   // context's work are refused while it lasts
   struct Capture { cudaStream_t st = nullptr; unsigned long long id = 0; } capture;
-  CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_kcat)
+  CUtensorMap tm_simA, tm_simB, tm_S, tm_b1A, tm_b1B, tm_b2A, tm_b2B;   // tm_sim*: the similarity GEMM's operands (make_tmap_sim)
   // nccl
   void* comm = nullptr; bool own_comm = false;
   // What a forward leaves for the calls after it.  Each forward that enters resets the whole record; a refused one leaves it alone.
@@ -400,7 +418,7 @@ static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   m.own(&c->S, f * c->s_rows * c->ldS, true);
   if (!c->cat) m.own(&c->Xs, 2 * ns * N * c->Dp, true);                              // operand pieces [ns][N][Dp]
   m.own(&c->XsT, 2 * ns * D * c->Np, true);                                           // transposed pieces [ns][D][Np]
-  if (c->cat) { m.own(&c->XcatA, 2 * Q * c->cfg.world * c->kcat, true); m.own(&c->XcatB, 2 * N * c->kcat, true); }   // [N][3*Dp] (fp16x2) / [N][6*Dp] (bf16x3); A: anchors only
+  if (c->cat) { m.own(&c->XcatA, 2 * c->sim.elems(Q), true); m.own(&c->XcatB, 2 * c->sim.elems(N), true); }   // SimLayout; A: the rank's anchors only
   if (!c->fused_grad) m.own(&c->H, 2 * ns * Q * c->Np, true);                        // materialised gradient weights
   if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) { m.own(&c->XlT, 2 * ns * D * c->Qp, true); m.own(&c->HT, 2 * ns * N * c->Qp, true); m.own(&c->OUT2, f * N * D, false); }
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) m.own(&c->rs_total, sizeof(RowRecord) * N, false);   // gathered row records
@@ -598,10 +616,10 @@ static bool mma_is_symmetric(int prec, int device) {
 // The tensor maps over the operands, S and the gradient weights, whose column (or row) extents are the context's current N
 static bool make_maps(npair_ctx* c, std::string* te) {
   const int Q = c->Q, D = c->D, N = c->N, ns = c->nsplit, bkg = c->bk_grad;
-  // similarity: A = the rank's rows, B = all rows of the K-concatenated operands (PREC_BF16: Xs, whose one piece is that format)
-  const uint16_t* catA = c->cat ? c->XcatA : c->Xs;
-  const uint16_t* catB = c->cat ? c->XcatB : c->Xs;
-  bool ok = make_tmap_kcat(&c->tm_simA, &c->tm_simB, catA +static_cast<long long>(c->rank) * Q * c->kcat, Q, catB, N, c->kcat, te);
+  // similarity: A = the rank's rows, B = all rows (PREC_BF16: Xs, whose one piece is the layout, the rank's rows at row rank * Q)
+  const uint16_t* simA = c->cat ? c->XcatA : c->Xs + static_cast<long long>(c->rank) * Q * c->Dp;
+  const uint16_t* simB = c->cat ? c->XcatB : c->Xs;
+  bool ok = make_tmap_sim(&c->tm_simA, &c->tm_simB, simA, Q, simB, N, c->sim, te);
   ok = ok && make_tmap_f32_store(&c->tm_S, c->S, N, c->s_rows, c->ldS, te);
   // gradient 1: A = H [Q x N], B = XsT [D x N]; K = N
   if (c->H) ok = ok && make_tmap_pieces(&c->tm_b1A, c->H, N, Q, ns, c->Np, static_cast<long long>(Q) * c->Np, bkg, 128, te);
@@ -1003,7 +1021,7 @@ static SimRows sim_rows(const npair_ctx* c, int r0, int rows) {
 // The similarity GEMM over rows [r0, r0 + rows) of the rank's S through the epilogue `epi` (gemm_wgmma.cuh)
 static cudaError_t sim_gemm(npair_ctx* c, int epi, int r0, int rows, cudaStream_t st) {
   const SimRows sim = sim_rows(c, r0, rows);
-  GemmParams gp = sim_sweep(epi, rows, c->N, c->kcat, &c->bs->x_inv_scale, c->sym_tiles, c->n_sym_tiles, c->ra);
+  GemmParams gp = sim_sweep(epi, rows, c->N, c->sim, &c->bs->x_inv_scale, c->sym_tiles, c->n_sym_tiles, c->ra);
   gp.a_row0 = sim.row0; gp.S = c->S; gp.ldS = sim.ldS;
   if (epi & EPI_STATS) {
     gp.lab_rows = sim.lab_rows; gp.lab_cols = sim.lab_cols; gp.self_offset = sim.col0;

@@ -1,5 +1,5 @@
-// device.cuh -- device helpers that more than one kernel unit uses: the warp reductions, the operand split and its K-concatenated row
-// writer, and the reset of a row's statistics.
+// device.cuh -- device helpers that more than one kernel unit uses: the warp reductions, the operand split and the writer of the
+// similarity GEMM's operands, and the reset of a row's statistics.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -58,27 +58,14 @@ __device__ __forceinline__ void split8(const float (&v)[8], float sc, uint16_t (
     pk[s] = make_uint4(p[0][s] | (static_cast<uint32_t>(p[1][s]) << 16), p[2][s] | (static_cast<uint32_t>(p[3][s]) << 16),
                        p[4][s] | (static_cast<uint32_t>(p[5][s]) << 16), p[6][s] | (static_cast<uint32_t>(p[7][s]) << 16));
 }
-// The packed pieces pk of features [d, d + 8) into one row of the K-concatenated operands of the bitwise-symmetric similarity GEMM,
-// in the A (side_b = false) or B format; one Dp-long segment per MMA pass:
-//   bf16   : A row = B row = [ hi ]                                                                                       K_cat = Dp
-//   fp16x2 : A row = [ hi | hi(8) lo(8) ... ]                         B row = [ hi | lo(8) hi(8) ... ]                  K_cat = 3*Dp
-//   bf16x3 : A row = [ hi | mid | hi(8) mid(8) ... | hi(8) lo(8) ... ]   B row = [ hi | mid | mid(8) hi(8) ... | lo(8) hi(8) ... ]   K_cat = 6*Dp
-// ONE K=16 MMA then sums 8 products p_j*q_m and the 8 mirrored products q_j*p_m: swapping the operand roles only
-// permutes the products inside an instruction, whose sum is order-invariant (measured: tests/diag_mma_symmetry.py),
-// so S[j][m] == S[m][j] bit for bit, on one rank and across ranks.
+// The packed pieces pk of features [d, d + 8) of row n into one side (side_b = false: A, true: B) of the similarity GEMM's operands,
+// laid out by SimLayout.  Each piece is stored once; the GEMM forms the cross terms from the pieces in place (split_gemm_kernel).
 template <int PREC>
-__device__ __forceinline__ void store_kcat_row(uint16_t* row, long long Dp, int d, const uint4 (&pk)[3], bool side_b) {
-  *reinterpret_cast<uint4*>(row + d) = pk[0];
-  if (PREC == PREC_FP16X2) {
-    *reinterpret_cast<uint4*>(row + Dp + 2 * d) = side_b ? pk[1] : pk[0];
-    *reinterpret_cast<uint4*>(row + Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
-  } else if (PREC == PREC_BF16X3) {
-    *reinterpret_cast<uint4*>(row + Dp + d) = pk[1];
-    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d) = side_b ? pk[1] : pk[0];
-    *reinterpret_cast<uint4*>(row + 2 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[1];
-    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d) = side_b ? pk[2] : pk[0];
-    *reinterpret_cast<uint4*>(row + 4 * Dp + 2 * d + 8) = side_b ? pk[0] : pk[2];
-  }
+__device__ __forceinline__ void store_sim_row(uint16_t* base, long long Dp, long long n, int d, const uint4 (&pk)[3], bool side_b) {
+  constexpr int NS = SPLIT_FORMATS[PREC].pieces;
+  const SimLayout L{NS, Dp};
+#pragma unroll
+  for (int s = 0; s < NS; ++s) *reinterpret_cast<uint4*>(base + L.offset(n, d, SimLayout::piece_slot(NS, s, side_b))) = pk[s];
 }
 
 // Row i's statistics before a similarity sweep accumulates into them (caffe_set of the stat blobs, .cu:230-236)

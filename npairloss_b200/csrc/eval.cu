@@ -16,13 +16,14 @@
 using namespace npair;
 
 // ------------------------------------------------------------------------------------------------ retrieval evaluation (DESIGN 8)
-// Not part of the reference layer.  Queries go to the A format and gallery rows to the B format of the K-concatenated operands, so the
-// similarity GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
+// Not part of the reference layer.  Queries go to the A side and gallery rows to the B side of the similarity GEMM's operands
+// (SimLayout), so the GEMM sees the layer's operands; sweep 1 is the layer's statistics epilogue (p* = max_within), sweep 2 EPI_COUNT.
 static constexpr int EVAL_NO_SELF = -(1 << 30); // a self offset that matches no column (rows and columns stay below 2^30)
 
 struct EvalPlan {
   int max_q, max_g, D, prec;
-  long long Dp, kcat;           // padded feature extent, K extent of the concatenated operands (mma_passes * Dp)
+  long long Dp;                 // padded feature extent
+  SimLayout sim;                // layout of the similarity GEMM's operands
   int n_sym_tiles;              // tile-list capacity: self-retrieval over min(max_q, max_g) rows
 };
 
@@ -37,7 +38,7 @@ static EvalPlan eval_plan_of(int max_q, int max_g, int D, int prec) {
   EvalPlan p{};
   p.max_q = max_q; p.max_g = max_g; p.D = D; p.prec = prec;
   p.Dp = round_up(D, 64);
-  p.kcat = mma_passes(SPLIT_FORMATS[prec].pieces) * p.Dp;
+  p.sim = SimLayout{SPLIT_FORMATS[prec].pieces, p.Dp};
   const int n = max_q < max_g ? max_q : max_g;
   p.n_sym_tiles = static_cast<int>(sym_tile_count(n, n));
   return p;
@@ -60,10 +61,19 @@ struct npair_eval : EvalPlan {
   std::string err;
 };
 
+// 2-byte elements of an operand buffer of `rows` rows.  npair_eval_workspace_bytes is documented as linear in the set sizes, an
+// operand row costing mma_passes(pieces) * Dp elements, and callers size against it: the buffers keep that size.  SimLayout needs
+// less (pieces * Dp per row, rows padded to 8-row groups) and fits in it from 14 rows (fp16x2) or 7 rows (bf16x3) on; a smaller set
+// takes the layout's own size.
+static long long eval_operand_elems(const EvalPlan& p, long long rows) {
+  const long long kept = mma_passes(p.sim.pieces) * p.Dp * rows, need = p.sim.elems(rows);
+  return kept > need ? kept : need;
+}
+
 // The evaluator's workspace, each buffer with its size and zero-fill; returns the first failure
 static cudaError_t eval_buffers(npair_eval* ev, DevMem& m) {
-  m.own(&ev->catA, 2ull * ev->max_q * ev->kcat, false);
-  m.own(&ev->catB, 2ull * ev->max_g * ev->kcat, false);
+  m.own(&ev->catA, 2ull * eval_operand_elems(*ev, ev->max_q), false);
+  m.own(&ev->catB, 2ull * eval_operand_elems(*ev, ev->max_g), false);
   m.own_carved(true, [ev](Carve& cv) { carve_stats(cv, ev->max_q, &ev->ra); ev->absmax_bits = cv.take<unsigned int>(1); });
   m.own(&ev->bs, sizeof(BlockScalars), true);
   m.own(&ev->sym_tiles, sizeof(int2) * ev->n_sym_tiles, false);
@@ -232,7 +242,7 @@ static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, con
     }
     epi |= EPI_SYM;
   }
-  GemmParams gp = sim_sweep(epi, nq, ng, ev->kcat, &ev->bs->x_inv_scale, ev->sym_tiles, static_cast<int>(ev->sym_host.size()), ev->ra);
+  GemmParams gp = sim_sweep(epi, nq, ng, ev->sim, &ev->bs->x_inv_scale, ev->sym_tiles, static_cast<int>(ev->sym_host.size()), ev->ra);
   gp.self_offset = self_col;
   if (epi & (EPI_STATS | EPI_GATHER | EPI_BUCKET)) { gp.lab_rows = ql; gp.lab_cols = gl; }
   else { gp.cut = cut; gp.count = count; }
@@ -242,7 +252,7 @@ static int eval_sweep(npair_eval* ev, int epi, int nq, int ng, int self_col, con
   }
   CUtensorMap ta, tb;
   std::string te;
-  if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
+  if (!make_tmap_sim(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->sim, &te)) { ev->err = te; return NPAIR_E_CUDA; }
   CUDA_TRY(ev, launch_gemm(ev->prec, epi, ta, tb, ta, gp, ev->sms, st));
   return NPAIR_OK;
 }
@@ -333,10 +343,10 @@ int npair_eval_knn(npair_eval* ev, const float* q, int32_t nq, const float* g, i
   if ((rc = eval_prepare(ev, q, nq, g, ng, absmax, false, st)) != NPAIR_OK) return rc;
   CUtensorMap ta, tb;
   std::string te;
-  if (!make_tmap_kcat(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
+  if (!make_tmap_sim(&ta, &tb, ev->catA, nq, ev->catB, ng, ev->sim, &te)) { ev->err = te; return NPAIR_E_CUDA; }
   for (int r0 = 0; r0 < nq; r0 += rows) {
     const int m = nq - r0 < rows ? nq - r0 : rows;
-    GemmParams gp = sim_sweep(EPI_STORE_S, m, ng, ev->kcat, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
+    GemmParams gp = sim_sweep(EPI_STORE_S, m, ng, ev->sim, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
     gp.a_row0 = r0; gp.S = blk.S; gp.ldS = blk.ldS;
     CUDA_TRY(ev, launch_gemm(ev->prec, EPI_STORE_S, ta, tb, ta, gp, ev->sms, st));
     launch_knn_select(blk.S, blk.ldS, m, ng, k, r0, static_cast<int>(self_col), gallery_row0, d_sim, d_index, st);
@@ -381,8 +391,8 @@ int npair_eval_class_batches(npair_eval* ev, const float* x, int32_t C, const in
   if ((rc = eval_prepare(ev, x, C, x, C, -1.f, false, st)) != NPAIR_OK) return rc;
   CUtensorMap ta, tb;
   std::string te;
-  if (!make_tmap_kcat(&ta, &tb, ev->catA, C, ev->catB, C, ev->kcat, &te)) { ev->err = te; return NPAIR_E_CUDA; }
-  GemmParams gp = sim_sweep(EPI_STORE_S, C, C, ev->kcat, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
+  if (!make_tmap_sim(&ta, &tb, ev->catA, C, ev->catB, C, ev->sim, &te)) { ev->err = te; return NPAIR_E_CUDA; }
+  GemmParams gp = sim_sweep(EPI_STORE_S, C, C, ev->sim, &ev->bs->x_inv_scale, nullptr, 0, ev->ra);
   gp.a_row0 = 0; gp.S = cb.S; gp.ldS = cb.ldS;
   CUDA_TRY(ev, launch_gemm(ev->prec, EPI_STORE_S, ta, tb, ta, gp, ev->sms, st));
   CUDA_TRY(ev, cudaMemcpyAsync(cb.pools, pools, sizeof(int32_t) * nb * P, cudaMemcpyHostToDevice, st));

@@ -35,9 +35,11 @@ void launch_eval_prep(const float* q, long long nq_el, const float* g, long long
   count_launch();
 }
 
-// Rows of x to one side of the K-concatenated operands of the similarity GEMM (side_b = 0: the A format of the queries, 1: the B format
-// of the gallery), through the layer's store_kcat_row.  Thread = 8 features of one row.  The pre-scale is the layer's rule applied to
-// max|x| over both sets: `absmax` when the caller gives it (>= 0), else *absmax_bits.
+// Rows of x to one side of the similarity GEMM's operands (side_b = 0: the A side of the queries, 1: the B side of the gallery),
+// through the layer's store_sim_row; rows [rows, round8(rows)) are zeros.  Thread = 8 features of one row.  With one piece consecutive
+// threads walk a row; with two or three, eight consecutive threads take the 8 rows of a row group at the same features, so that their
+// stores fill whole 128-byte core matrices.  The pre-scale is the layer's rule applied to max|x| over both sets: `absmax` when the
+// caller gives it (>= 0), else *absmax_bits.
 template <int PREC>
 __global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict__ x, int rows, int D, long long Dp, int side_b, float absmax,
                                                          const unsigned int* __restrict__ absmax_bits, BlockScalars* bs,
@@ -47,12 +49,21 @@ __global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict
   if (PREC == PREC_FP16X2) ps = pre_scale(absmax >= 0.f ? absmax : __uint_as_float(*absmax_bits));
   if (blockIdx.x == 0 && threadIdx.x == 0 && !side_b) { bs->x_scale = ps.scale; bs->x_inv_scale = ps.inv; }
   const long long groups = Dp / 8, i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= rows * groups) return;
-  const long long n = i / groups;
-  const int d = static_cast<int>(i - n * groups) * 8;
+  if (i >= SimLayout{NS, Dp}.padded_rows(rows) * groups) return;
+  long long n;
+  int d;
+  if (NS == 1) {
+    n = i / groups; d = static_cast<int>(i - n * groups) * 8;
+  } else {
+    const long long gd = i >> 3, g = gd / groups;     // (row group, 8-feature chunk), row g * 8 + i % 8
+    n = g * 8 + (i & 7); d = static_cast<int>(gd - g * groups) * 8;
+  }
   const float* xr = x + n * D;
   float v[8];
-  if (d + 7 < D && (D & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+  if (n >= rows) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = 0.f;
+  } else if (d + 7 < D && (D & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const float4 a4 = __ldg(reinterpret_cast<const float4*>(xr + d)), b4 = __ldg(reinterpret_cast<const float4*>(xr + d + 4));
     v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
   } else {
@@ -62,11 +73,11 @@ __global__ void __launch_bounds__(256) eval_split_kernel(const float* __restrict
   uint16_t p[8][3];
   uint4 pk[3];
   split8<PREC>(v, ps.scale, p, pk);
-  store_kcat_row<PREC>(out + n * (mma_passes(NS) * Dp), Dp, d, pk, side_b);
+  store_sim_row<PREC>(out, Dp, n, d, pk, side_b);
 }
 void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
                        BlockScalars* bs, uint16_t* out, cudaStream_t st) {
-  const long long work = static_cast<long long>(rows) * (Dp / 8);
+  const long long work = SimLayout{SPLIT_FORMATS[prec].pieces, Dp}.padded_rows(rows) * (Dp / 8);
   with_prec(prec, [&](auto P) {
     eval_split_kernel<P><<<static_cast<unsigned int>((work + 255) / 256), 256, 0, st>>>(x, rows, D, Dp, side_b, absmax, absmax_bits, bs, out);
   });

@@ -19,23 +19,24 @@ static GemmKernel gemm_t() {
   using Cfg = GemmCfg<NSPLIT, BK, EPI>;
   return GemmKernel{split_gemm_kernel<NSPLIT, BF16, EPI, BK>, Cfg::THREADS, Cfg::SMEM_BYTES};
 }
-// Similarity GEMM: always ONE MMA pass over K-concatenated operands (see split_kernel), fp16 or bf16 elements.  Only the
+// Similarity GEMM over the operands of SimLayout (split_kernel, eval_split_kernel), NS pieces of fp16 or bf16 elements.  Only the
 // epilogues the host composes are instantiated.
-template <bool BF16>
+template <int NS, bool BF16>
 static GemmKernel sim_gemm_t(int epi) {
+  constexpr int BK = SimLayout::bk_of(NS);
   switch (epi) {
-    case EPI_STORE_S | EPI_STATS: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS, 64>();
-    case EPI_STORE_S | EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STORE_S | EPI_STATS | EPI_SYM, 64>();
-    case EPI_STATS: return gemm_t<1, BF16, EPI_STATS, 64>();
-    case EPI_STATS | EPI_SYM: return gemm_t<1, BF16, EPI_STATS | EPI_SYM, 64>();
-    case EPI_STORE_S: return gemm_t<1, BF16, EPI_STORE_S, 64>();
-    case EPI_COUNT: return gemm_t<1, BF16, EPI_COUNT, 64>();                       // retrieval evaluation
-    case EPI_COUNT | EPI_SYM: return gemm_t<1, BF16, EPI_COUNT | EPI_SYM, 64>();
-    case EPI_GATHER: return gemm_t<1, BF16, EPI_GATHER, 64>();                     // MAP@R evaluation
-    case EPI_GATHER | EPI_SYM: return gemm_t<1, BF16, EPI_GATHER | EPI_SYM, 64>();
-    case EPI_BUCKET: return gemm_t<1, BF16, EPI_BUCKET, 64>();
-    case EPI_BUCKET | EPI_SYM: return gemm_t<1, BF16, EPI_BUCKET | EPI_SYM, 64>();
-    case EPI_ARGMAX: return gemm_t<1, BF16, EPI_ARGMAX, 64>();                     // k-means assignment
+    case EPI_STORE_S | EPI_STATS: return gemm_t<NS, BF16, EPI_STORE_S | EPI_STATS, BK>();
+    case EPI_STORE_S | EPI_STATS | EPI_SYM: return gemm_t<NS, BF16, EPI_STORE_S | EPI_STATS | EPI_SYM, BK>();
+    case EPI_STATS: return gemm_t<NS, BF16, EPI_STATS, BK>();
+    case EPI_STATS | EPI_SYM: return gemm_t<NS, BF16, EPI_STATS | EPI_SYM, BK>();
+    case EPI_STORE_S: return gemm_t<NS, BF16, EPI_STORE_S, BK>();
+    case EPI_COUNT: return gemm_t<NS, BF16, EPI_COUNT, BK>();                       // retrieval evaluation
+    case EPI_COUNT | EPI_SYM: return gemm_t<NS, BF16, EPI_COUNT | EPI_SYM, BK>();
+    case EPI_GATHER: return gemm_t<NS, BF16, EPI_GATHER, BK>();                     // MAP@R evaluation
+    case EPI_GATHER | EPI_SYM: return gemm_t<NS, BF16, EPI_GATHER | EPI_SYM, BK>();
+    case EPI_BUCKET: return gemm_t<NS, BF16, EPI_BUCKET, BK>();
+    case EPI_BUCKET | EPI_SYM: return gemm_t<NS, BF16, EPI_BUCKET | EPI_SYM, BK>();
+    case EPI_ARGMAX: return gemm_t<NS, BF16, EPI_ARGMAX, BK>();                     // k-means assignment
     default: return GemmKernel{nullptr, 0, 0};
   }
 }
@@ -43,7 +44,7 @@ static GemmKernel sim_gemm_t(int epi) {
 GemmKernel gemm_kernel(int prec, int epi) {
   return with_prec(prec, [epi](auto P) {
     constexpr SplitFormat f = SPLIT_FORMATS[P];
-    return epi != EPI_OUT ? sim_gemm_t<f.bf16>(epi) : gemm_t<f.pieces, f.bf16, EPI_OUT, bk_of(P, EPI_OUT)>();
+    return epi != EPI_OUT ? sim_gemm_t<f.pieces, f.bf16>(epi) : gemm_t<f.pieces, f.bf16, EPI_OUT, bk_of(P, EPI_OUT)>();
   });
 }
 // `sm`: fp32 tensor map of the similarity matrix for EPI_STORE_S's TMA stores (ignored otherwise: pass any valid map)

@@ -6,10 +6,12 @@
 //   NSPLIT=1 bf16            1 pass  (hi.hi)                                  -- throughput mode
 //   NSPLIT=2 fp16 hi+lo      3 passes (hh, hl, lh)      ~2^-22 relative       -- fp32-faithful, pre-scaled inputs
 //   NSPLIT=3 bf16 hi+mid+lo  6 passes (hh,hm,mh,mm,hl,lh) ~2^-24 relative     -- fp32-faithful, any dynamic range
-// All passes accumulate into the same fp32 register accumulator, so the tensor pipe sees one long K loop.
+// All passes accumulate into the same fp32 register accumulator, so the tensor pipe sees one long K loop.  The similarity GEMM at 2 or
+// 3 pieces makes the same products without separate passes: per K block it reads every piece once (SimLayout) and pairs them inside
+// role-symmetric instructions (sim_kblock_mmas).
 //
 // Structure (persistent, one CTA per SM, 384 threads, 128 x 256 tiles): warp 0 TMA producer (3-D boxes {BK, rows, 1 piece} ->
-// swizzled smem ring); warps 4-11 two consumer warpgroups, each issuing wgmma.m64n256k16 for 64 rows of the tile and running the
+// swizzled smem ring; the pieced similarity GEMM: one unswizzled 4-D box per side); warps 4-11 two consumer warpgroups, each issuing wgmma.m64n256k16 for 64 rows of the tile and running the
 // fused epilogue (similarity store + row statistics, or a scaled store of a gradient tile) on its register accumulator.
 // Replaces the reference's cublasSgemm calls: sim GEMM npair_multi_class_loss.cu:218 and the six backward
 // GEMMs .cu:448-460; the EPI_STATS epilogue also replaces GetLabelDiffMtx (.cu:44-66) and the host statistics loop
@@ -45,6 +47,12 @@ namespace npair {
 // EPI_ARGMAX  : k-means assignment (DESIGN 8.2).  Per row, the column c < Nn with the largest s - col_bias[c], the lowest such c on
 //               ties, as one 64-bit atomicMax per row and thread into best[row] of the key (f2ord(score) << 32) | (0xFFFFFFFF - c),
 //               which is independent of the tile order.  No self exclusion, no labels.  Used alone, with full tiles (no EPI_SYM).
+// Timing probes of the similarity sweep (tools/bench_sim_sweep.py builds one library per probe; 0 everywhere else): 1 the MMAs are
+// left out (loads and epilogue kept), 2 the epilogue only stores S, 3 every load reads K block 0 of tile (0, 0), 4 nothing is loaded
+#ifndef NPAIR_SIM_PROBE
+#define NPAIR_SIM_PROBE 0
+#endif
+
 enum { EPI_OUT = 1, EPI_STORE_S = 8, EPI_STATS = 16, EPI_SYM = 32, EPI_COUNT = 64, EPI_GATHER = 128, EPI_BUCKET = 256, EPI_ARGMAX = 512 };
 
 // Persistent tile schedule of both wgmma GEMMs (host: tile_sched, host.cuh).  CTA b computes tiles b, b + gridDim.x, ...; tile t is
@@ -111,17 +119,22 @@ struct GemmParams {
   BlockStats* thr_out;            // NULL: the thresholds are finished here; world scope: receives the rank's statistics for the exchange
 };
 
-// BK_ = K-block in elements = one swizzle span per smem row (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B): the short-K similarity
-// GEMM (K = D) uses 64, the long-K gradient GEMM (K = N) with several pieces 32 (more, smaller stages in flight).
+// BK_ = K-block in elements.  Swizzled operands (the gradient GEMM, and the similarity GEMM at one piece): one swizzle span per smem row
+// (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B); the long-K gradient GEMM (K = N) with several pieces uses 32 (more, smaller stages in
+// flight).  PIECED (the similarity GEMM at 2 or 3 pieces): the operands of SimLayout, unswizzled; a stage holds per side
+// [row group][piece slot][BK / 8 core matrices of 128 bytes], BK = SimLayout::bk_of(NSPLIT).
 // The similarity epilogues need two smem areas besides the operand ring: a 64 x 64 fp32 accumulator staging tile per consumer
 // warpgroup (register fragments -> thread = row) and a 32 x 32 fp32 TMA-store staging tile per consumer warp (mirrored blocks).
 template <int NSPLIT, int BK_, int EPI>
 struct GemmCfg {
   static constexpr int BM = 128, BN = 256;
   static constexpr int BK = BK_;
-  static constexpr int ROW_BYTES = BK * 2;                    // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
-  static constexpr uint32_t LAYOUT = (ROW_BYTES == 128) ? 1u : 2u;   // wgmma descriptor layout type
-  static constexpr uint32_t SBO = 8 * ROW_BYTES;              // byte distance between 8-row groups
+  static constexpr bool PIECED = EPI != EPI_OUT && NSPLIT > 1;
+  static constexpr int ROW_BYTES = BK * 2;                    // one piece of one row in a stage: 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
+  static constexpr uint32_t LAYOUT = PIECED ? 0u : (ROW_BYTES == 128) ? 1u : 2u;   // wgmma descriptor layout type (0: no swizzle)
+  static constexpr uint32_t SBO = PIECED ? 8 * NSPLIT * ROW_BYTES : 8 * ROW_BYTES;  // byte distance between 8-row groups
+  static constexpr uint32_t CORE = 128;                       // PIECED: one 8 x 8 core matrix
+  static constexpr uint32_t SLOT = 8 * ROW_BYTES;             // PIECED: byte distance between piece slots of a row group
   static constexpr int A_PIECE = BM * ROW_BYTES;
   static constexpr int B_PIECE = BN * ROW_BYTES;
   static constexpr int STAGE_BYTES = NSPLIT * (A_PIECE + B_PIECE);
@@ -135,6 +148,7 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_STAGE_BYTES + STORE_STAGE_BYTES + SMEM_AUX + 1024 /*alignment slack*/;
   static constexpr int THREADS = 384;                         // producer warpgroup + 2 consumer warpgroups
   static_assert(STAGES >= 2 && 16 * STAGES <= 192, "operand ring");
+  static_assert(!PIECED || BK == SimLayout::bk_of(NSPLIT), "the similarity GEMM's K block is its operands'");
 };
 
 // The operand ring of both GEMM kernels: per stage a `full` barrier (the producer's arrival + the TMA bytes) and an `empty` barrier
@@ -167,6 +181,33 @@ __device__ __forceinline__ void pass_pieces(int nsplit, int p, int& sa, int& sb)
   const int A[6] = {0, 0, 1, 1, 0, 2};
   const int B[6] = {0, 1, 0, 1, 2, 0};
   sa = A[p]; sb = B[p];
+}
+
+// One K block of the PIECED similarity GEMM (SimLayout), a and b the stage addresses of this warpgroup's rows: per 16 features one hh
+// instruction (core matrices hi[k..k+8), hi[k+8..k+16) on both sides; bf16x3 also mm), then per 8 features c one cross instruction per
+// piece pair (hi, x): core matrix 0 = A's hi and B's x, core matrix 1 = A's x and B's hi, all at features c, so it sums the 16 products
+// hi_a x_b + x_a hi_b.  Each instruction holds the same products when the operand roles swap, and both roles run the same sequence:
+// S comes out bitwise symmetric.  A's slots are (hi, mid, lo), B's (mid, lo, hi) (SimLayout::piece_slot): every leading byte offset,
+// the distance from core matrix 0 to core matrix 1, is positive.
+template <int NSPLIT, bool BF16, class Cfg>
+__device__ __forceinline__ void sim_kblock_mmas(float (&acc)[128], uint32_t a, uint32_t b) {
+  constexpr int BK = Cfg::BK;
+  const auto slot_a = [](int s) { return SimLayout::piece_slot(NSPLIT, s, false) * Cfg::SLOT; };
+  const auto slot_b = [](int s) { return SimLayout::piece_slot(NSPLIT, s, true) * Cfg::SLOT; };
+  // the diagonal terms hh (and mm): two consecutive core matrices of one piece
+#pragma unroll
+  for (int s = 0; s < (NSPLIT == 3 ? 2 : 1); ++s)
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      ptx::wgmma_m64n256k16_ss<BF16>(acc, ptx::make_nosw_desc(a + slot_a(s) + 2 * k * Cfg::CORE, Cfg::CORE, Cfg::SBO),
+                                     ptx::make_nosw_desc(b + slot_b(s) + 2 * k * Cfg::CORE, Cfg::CORE, Cfg::SBO), 1u);
+  // the cross terms (hi, x), x = mid, lo
+#pragma unroll
+  for (int x = 1; x < NSPLIT; ++x)
+#pragma unroll
+    for (int c = 0; c < BK / 8; ++c)
+      ptx::wgmma_m64n256k16_ss<BF16>(acc, ptx::make_nosw_desc(a + slot_a(0) + c * Cfg::CORE, slot_a(x) - slot_a(0), Cfg::SBO),
+                                     ptx::make_nosw_desc(b + slot_b(x) + c * Cfg::CORE, slot_b(0) - slot_b(x), Cfg::SBO), 1u);
 }
 
 // The pair predicate of every similarity epilogue that looks at labels: column idx of a row is a pair iff it lies inside the gallery
@@ -311,7 +352,8 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   using Cfg = GemmCfg<NSPLIT, BK_, EPI>;
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
-  constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = EPI & EPI_STATS, COUNT = EPI & EPI_COUNT;
+  constexpr int PROBE = (EPI != EPI_OUT) ? NPAIR_SIM_PROBE : 0;
+  constexpr bool SYM = EPI & EPI_SYM, STORE = EPI & EPI_STORE_S, STATS = (EPI & EPI_STATS) && PROBE != 2, COUNT = EPI & EPI_COUNT;
   constexpr bool GATHER = EPI & EPI_GATHER, BUCKET = EPI & EPI_BUCKET, ARGMAX = EPI & EPI_ARGMAX;
   constexpr bool LABELS = STATS || GATHER || BUCKET;              // the epilogue needs the tile's labels
   static_assert(!ARGMAX || EPI == EPI_ARGMAX, "EPI_ARGMAX is used alone, with full tiles");
@@ -352,12 +394,22 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       for (int tile = worker; tile < num_tiles; tile += num_workers) {
         const Tile t = p.ts.at(tile);
         for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          uint64_t* full = ring.produce(Cfg::STAGE_BYTES);
+          uint64_t* full = ring.produce(PROBE == 4 ? 0u : Cfg::STAGE_BYTES);
           uint8_t* st = smem + ring.stage * Cfg::STAGE_BYTES;
+          const bool one = PROBE == 3;
+          const int a_row = t.m_blk * BM + (STORE && !STATS ? p.a_row0 : 0);
+          if constexpr (Cfg::PIECED) {     // one box per side: every piece of the K block's row groups (SimLayout)
+            if (PROBE != 4) {
+              ptx::tma_load_4d(st, &tmapA, full, 0, 0, one ? 0 : kb, one ? 0 : a_row / 8);
+              ptx::tma_load_4d(st + NSPLIT * Cfg::A_PIECE, &tmapB, full, 0, 0, one ? 0 : kb, one ? 0 : t.n_blk * BN / 8);
+            }
+            ring.advance();
+            continue;
+          }
 #pragma unroll
-          for (int s = 0; s < NSPLIT; ++s) {
-            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, full, kb * BK, t.m_blk * BM + (STORE && !STATS ? p.a_row0 : 0), s);
-            ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, full, kb * BK, t.n_blk * BN, s);
+          for (int s = 0; s < NSPLIT && PROBE != 4; ++s) {
+            ptx::tma_load_3d(st + s * Cfg::A_PIECE, &tmapA, full, one ? 0 : kb * BK, one ? 0 : a_row, s);
+            ptx::tma_load_3d(st + NSPLIT * Cfg::A_PIECE + s * Cfg::B_PIECE, &tmapB, full, one ? 0 : kb * BK, one ? 0 : t.n_blk * BN, s);
           }
           ring.advance();
         }
@@ -422,9 +474,12 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       int prev = ring.stage;
       for (int kb = t.kb0; kb < t.kb1; ++kb) {
         ring.wait_full();
-        const uint32_t a0 = ptx::smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + g * 64 * Cfg::ROW_BYTES;
+        const uint32_t a0 = ptx::smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + g * 8 * Cfg::SBO;   // this warpgroup's 64 rows
         const uint32_t b0 = ptx::smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + NSPLIT * Cfg::A_PIECE;
         ptx::wgmma_fence();
+        if constexpr (Cfg::PIECED) {
+          if (PROBE != 1) sim_kblock_mmas<NSPLIT, BF16, Cfg>(acc, a0, b0);
+        } else
 #pragma unroll
         for (int ps = 0; ps < Cfg::NPASS; ++ps) {
           int sa, sb;
@@ -433,7 +488,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           for (int k4 = 0; k4 < BK / 16; ++k4) {
             const uint64_t ad = ptx::make_kmajor_desc(a0 + sa * Cfg::A_PIECE + k4 * 32, Cfg::SBO, Cfg::LAYOUT);
             const uint64_t bd = ptx::make_kmajor_desc(b0 + sb * Cfg::B_PIECE + k4 * 32, Cfg::SBO, Cfg::LAYOUT);
-            ptx::wgmma_m64n256k16_ss<BF16>(acc, ad, bd, 1u);
+            if (PROBE != 1) ptx::wgmma_m64n256k16_ss<BF16>(acc, ad, bd, 1u);
           }
         }
         ptx::wgmma_commit();

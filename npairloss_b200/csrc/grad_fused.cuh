@@ -6,7 +6,7 @@
 // H is never written to HBM: per 32-column K block the producer warp (warp 8) brings a 128 x 32 fp32 tile of S, the 32 column
 // records and the B pieces of X^T into shared memory; each thread of the two consumer warpgroups (warps 0-7, 64 rows each)
 // evaluates the weights of its own wgmma A fragment, splits them into 2-byte pieces and passes them as a register operand.
-// Requires a bitwise symmetric S (EPI_SYM tiles at world == 1, K-concatenated operands across ranks).
+// Requires a bitwise symmetric S (EPI_SYM tiles at world == 1, role-symmetric similarity instructions across ranks).
 // Chunked accumulation: the fp32 accumulator drifts over long K (K = database size), so the K range is cut into chunks of
 // `chunk_kb` K blocks, each accumulated from zero and added to the output in fp32 round-to-nearest by the same thread.
 #pragma once

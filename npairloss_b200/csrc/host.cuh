@@ -30,14 +30,14 @@ inline std::string fmt(const char* f, ...) {
 // ------------------------------------------------------------------------------------------------ TMA maps (ctx.cu)
 bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int pieces, long long ld_elems, long long piece_stride_elems,
                       int bk, int box_rows, std::string* err);
-bool make_tmap_kcat(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, long long kcat,
-                    std::string* err);
+bool make_tmap_sim(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, SimLayout L,
+                   std::string* err);
 bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int rows, long long ld_elems, std::string* err, int box_rows = 32);
 
 // ------------------------------------------------------------------------------------------------ GEMM launchers (gemm.cu)
 // K-block per (operand format, GEMM role); see GemmCfg
 constexpr int bk_of(int prec, int epi) {
-  if (epi != EPI_OUT) return 64;                 // similarity GEMM: single pass, 64-element K blocks
+  if (epi != EPI_OUT) return SimLayout::bk_of(SPLIT_FORMATS[prec].pieces);   // similarity GEMM: the K block of its operands
   return prec == PREC_BF16 ? 64 : 32;
 }
 
@@ -108,14 +108,14 @@ inline long long sym_tile_count(int Q, int N) {
   return n;
 }
 
-// A sweep of the similarity GEMM over rows x cols of the K-concatenated operands of K extent kcat (make_tmap_kcat): 128 x 256 tiles
-// of 64-element K blocks, no split-K, the accumulators scaled by the square of *inv_scale; under EPI_SYM only the tiles of
-// `sym_tiles`, and under EPI_STATS the per-row statistics of `ra`
-inline GemmParams sim_sweep(int epi, int rows, int cols, long long kcat, const float* inv_scale, const int2* sym_tiles, int n_sym_tiles,
+// A sweep of the similarity GEMM over rows x cols of operands laid out by L (make_tmap_sim): 128 x 256 tiles over the layout's K
+// blocks, no split-K, the accumulators scaled by the square of *inv_scale; under EPI_SYM only the tiles of `sym_tiles`, and under
+// EPI_STATS the per-row statistics of `ra`
+inline GemmParams sim_sweep(int epi, int rows, int cols, SimLayout L, const float* inv_scale, const int2* sym_tiles, int n_sym_tiles,
                             const RowArrays& ra) {
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.M = rows; gp.Nn = cols;
-  gp.ts = tile_sched(rows, cols, static_cast<int>(kcat / 64));
+  gp.ts = tile_sched(rows, cols, static_cast<int>(L.Dp / L.bk()));
   gp.dev_scale = inv_scale;
   if (epi & EPI_SYM) { gp.ts.tile_list = sym_tiles; gp.ts.num_tiles_list = n_sym_tiles; }
   if (epi & EPI_STATS) {

@@ -212,17 +212,21 @@ __device__ __forceinline__ void split_tile(const SplitArgs& a, float sc, int til
   // every destination row is padded to a multiple of 64 elements (Dp), so whole 16-byte groups can be stored even when
   // D is ragged: the excess elements are zeros (v = 0 above), which is what the similarity GEMM reads past D (its K extent is Dp
   // per segment) and which lies beyond the TMA extent of every other map
-  if (rowok && d < Dp) {
+  if (rowok && d < Dp && Xs) {     // Xs is NULL when the similarity GEMM reads the operands XcatA / XcatB below
     const long long ps = static_cast<long long>(N) * ldXs;
-    if (Xs)      // NULL when the similarity GEMM reads the K-concatenated operands below
 #pragma unroll
-      for (int s = 0; s < NS; ++s) *reinterpret_cast<uint4*>(Xs + s * ps + static_cast<long long>(n) * ldXs + d) = pk[s];
-    // K-concatenated operands of the bitwise-symmetric similarity GEMM: every row in the B format, and the rank's own rows, the only
-    // ones that are ever an A operand, also in the A format
-    if (PREC != PREC_BF16 && XcatA) {
-      const long long kcat = mma_passes(NS) * Dp;
-      store_kcat_row<PREC>(XcatB + static_cast<long long>(n) * kcat, Dp, d, pk, true);
-      if (n >= row0 && n < row0 + Q) store_kcat_row<PREC>(XcatA + static_cast<long long>(n) * kcat, Dp, d, pk, false);
+    for (int s = 0; s < NS; ++s) *reinterpret_cast<uint4*>(Xs + s * ps + static_cast<long long>(n) * ldXs + d) = pk[s];
+  }
+  // the similarity GEMM's operands (SimLayout): every row in the B format, and the rank's own rows, the only ones that are ever an A
+  // operand, also in the A format at their local index; the rows that pad either side to a whole row group are zeros (v = 0 past N)
+  if (PREC != PREC_BF16 && XcatA && d < Dp) {
+    const SimLayout L{NS, Dp};
+    if (n < L.padded_rows(N)) store_sim_row<PREC>(XcatB, Dp, n, d, pk, true);
+    if (n >= row0 && n < row0 + L.padded_rows(Q)) {
+      uint4 pa[3];
+#pragma unroll
+      for (int s = 0; s < 3; ++s) pa[s] = n < row0 + Q ? pk[s] : make_uint4(0u, 0u, 0u, 0u);
+      store_sim_row<PREC>(XcatA, Dp, n - row0, d, pa, false);
     }
   }
   __syncthreads();
@@ -733,7 +737,7 @@ __device__ __forceinline__ void store_quad(uint16_t* __restrict__ base, long lon
 //     H[j][m] = g'(S[j][m]; row j) + g'(S[j][m]; row m)                       (= G + G^T, .cu:448-497 folded)
 //   needs only the row scalars of BOTH indices, which are local when world == 1.
 // !SYM (world > 1): H[j][m] = g'(j,m) and the transposed copy HT[m][j] (micro-tile transposed in registers).
-// MODE BW_ROWSCAL (world > 1): the similarity GEMM is bitwise symmetric ACROSS ranks (K-concatenated operands), so the
+// MODE BW_ROWSCAL (world > 1): the similarity GEMM is bitwise symmetric ACROSS ranks (role-symmetric instructions), so the
 //   transposed term G[m][j] of row m on another rank is evaluated here from S[j][m] and row m's all-gathered scalars:
 //     H[j][m] = g'(S[j][m]; row j) + (1/world) g'(S[j][m]; row m)          -- no N x D reduce-scatter (.cu:455-497)
 template <int PREC, int MODE>

@@ -29,9 +29,35 @@ struct SplitFormat {
 };
 constexpr SplitFormat SPLIT_FORMATS[3] = {{3, true} /*PREC_BF16X3*/, {1, true} /*PREC_BF16*/, {2, false} /*PREC_FP16X2*/};
 // MMA passes of a product of two operands of `pieces` pieces: one per piece pair (a, b) with a + b < pieces, in the order of
-// pass_pieces.  The K-concatenated operands of the bitwise-symmetric similarity GEMM hold one Dp-long segment per pass (split_tile),
-// so their K extent is mma_passes(pieces) * Dp.
+// pass_pieces.
 __host__ __device__ constexpr int mma_passes(int pieces) { return pieces * (pieces + 1) / 2; }
+
+// The operands of the bitwise-symmetric similarity GEMM (DESIGN 5), one A-side and one B-side buffer of `rows` rows of Dp features.
+//   pieces == 1 (bf16): plain rows [rows][Dp], read in 64-element K blocks through a 128B-swizzled map.
+//   pieces >= 2: every piece once, in wgmma's no-swizzle core-matrix order.  A row group g = n / 8 holds, per K block kb of BK
+//     features, one 16*BK-byte block per piece slot: BK / 8 core matrices of 8 rows x 8 features (128 contiguous bytes each):
+//       element (n, k) of slot s at  ((g * Dp / BK + kb) * pieces + s) * 8 * BK + (k % BK) / 8 * 64 + (n % 8) * 8 + k % 8
+//     so one TMA box {8 * BK, pieces, 1 K block, row groups} is a run of 16 * BK * pieces contiguous bytes per row group.  The slot of
+//     a piece differs between the sides (piece_slot): a cross-term instruction takes core matrix 0 from one piece and core matrix 1
+//     from another piece at the same features, through the descriptor's leading byte offset, which has to be positive.
+//     Rows [rows, round8(rows)) are zeros.
+struct SimLayout {
+  int pieces;
+  long long Dp;     // a multiple of 64
+  __host__ __device__ constexpr static int bk_of(int pieces) { return pieces == 1 ? 64 : (pieces == 2 ? 32 : 16); }
+  __host__ __device__ int bk() const { return bk_of(pieces); }
+  __host__ __device__ long long padded_rows(long long rows) const { return pieces == 1 ? rows : (rows + 7) / 8 * 8; }
+  __host__ __device__ long long elems(long long rows) const { return padded_rows(rows) * pieces * Dp; }
+  // slot of piece s (0 = largest) in side A: the pieces in order; in side B: the largest piece last (fp16x2 [lo][hi], bf16x3
+  // [mid][lo][hi]), so that every cross term (hi, x) has core matrix 1 behind core matrix 0 on both sides
+  __host__ __device__ static int piece_slot(int pieces, int s, bool side_b) { return side_b ? (s == 0 ? pieces - 1 : s - 1) : s; }
+  // element offset of feature k (a multiple of 8) of row n, piece slot `slot`
+  __host__ __device__ long long offset(long long n, long long k, int slot) const {
+    if (pieces == 1) return n * Dp + k;
+    const int bk = bk_of(pieces);
+    return (((n >> 3) * (Dp / bk) + k / bk) * pieces + slot) * 8 * bk + (k % bk) / 8 * 64 + (n & 7) * 8;
+  }
+};
 // Calls f(std::integral_constant<int, PREC>()) for the runtime format `prec`: where a kernel instantiation is chosen by format.
 template <class F>
 inline decltype(auto) with_prec(int prec, F&& f) {
@@ -317,7 +343,7 @@ cudaError_t allow_knn_select_smem();
 // and the reset of the nq queries' statistics
 void launch_eval_prep(const float* q, long long nq_el, const float* g, long long ng_el, unsigned int* absmax_bits, RowArrays ra, int nq,
                       int sms, cudaStream_t st);
-// rows x D fp32 -> the A (side_b = 0) or B (side_b = 1) format of the K-concatenated operands [rows][mma_passes * Dp], pre-scaled by
+// rows x D fp32 -> the A (side_b = 0) or B (side_b = 1) side of the similarity GEMM's operands (SimLayout), pre-scaled by
 // pre_scale of `absmax` (>= 0) or of *absmax_bits; the side-A launch also stores the scale in bs
 void launch_eval_split(const float* x, int rows, int D, long long Dp, int prec, int side_b, float absmax, const unsigned int* absmax_bits,
                        BlockScalars* bs, uint16_t* out, cudaStream_t st);
