@@ -371,6 +371,29 @@ int npair_eval_kmeans(npair_eval* ev, const float* d_x, int32_t n, int32_t k, co
 /* Device memory npair_eval_kmeans adds on top of the workspace (grown on demand, kept until npair_eval_destroy): 8 * k * D + 8 * n +
  * 12 * k + 2064 bytes.  0 for bad arguments (n, k or D < 1, k > n). */
 size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D);
+/* k-means++ seeding (Arthur & Vassilvitskii 2007, with sklearn's greedy local trials; DESIGN 8.2): the k initial rows of
+ * npair_eval_kmeans, rows_host[k] (HOST int32, exactly what npair_eval_kmeans takes as init_rows_host), by exact integer arithmetic:
+ *   sigma = the pre-scale of max|x| over the n points (as npair_eval_kmeans); q_id = rint(x_id * sigma * 2^13) as int16 (|q| <= 2^13);
+ *   d(i, j) = sum_d (q_id - q_jd)^2 in uint64;  D_i = min over the centres chosen so far of d(i, c);  phi = sum_i D_i (exact: n D < 2^36);
+ *   u(seed, t, j) = output number t * 256 + j + 1 of SplitMix64 seeded with `seed`, i.e. mix(seed + (t * 256 + j + 1) * 0x9E3779B97F4A7C15)
+ *     with mix the SplitMix64 finaliser (seed 0: outputs 1, 2, 3 are 0xe220a8397b1dcdaf, 0x6e789e6aa1b965f4, 0x06c45d188009454f);
+ *   step 0: centre 0 = row floor(u(seed, 0, 0) * n / 2^64);
+ *   step t = 1 .. k-1: L trials j < L, target_j = floor(u(seed, t, j) * phi / 2^64), candidate_j = the smallest i with
+ *     D_0 + ... + D_i > target_j (a point at distance 0 from a centre is never drawn; when phi = 0, candidate_j = floor(u * n / 2^64),
+ *     so a centre may repeat); phi_j = sum_i min(D_i, d(i, candidate_j)); centre t = the candidate of least phi_j, ties to the LOWEST j.
+ * L = local_trials in [1, 255], or 0 for sklearn's default 2 + floor(ln k); L = 1 is the classic k-means++.  Centre t depends only on
+ * (x, seed, L, t): with the same explicit L, a run's first t rows are those of a run with k = t.  The rows do not depend on the
+ * evaluator's precision, the stream, earlier calls or a fresh evaluator.  *potential_host (may be NULL) = phi after the last centre.
+ * Two kernels per step and no host wait inside the loop; the call synchronises with the host once, at the end.  NPAIR_E_ARG, checked
+ * on the host before anything is enqueued, for a null pointer, n outside [1, max_queries], k outside [1, n], local_trials outside
+ * [0, 255] or n * D >= 2^36; NPAIR_E_CUDA for NaN or infinite x.  Device memory: on top of the workspace,
+ * npair_eval_kmeans_seed_bytes(n, D, L), grown on demand and kept until npair_eval_destroy. */
+int npair_eval_kmeans_seed(npair_eval* ev, const float* d_x, int32_t n, int32_t k, uint64_t seed, int32_t local_trials,
+                           int32_t* rows_host /* [k] */, uint64_t* potential_host /* final phi, may be NULL */, void* stream);
+/* Device memory npair_eval_kmeans_seed adds on top of the workspace: 2 * n * round_up(D, 16) + (8 * L + 20) * n + 16 * ceil(n / 256)
+ * + 12 * L + 24 bytes, up to alignment, with L = local_trials, or for local_trials = 0 the default L of k = n (an upper bound).  0 for bad
+ * arguments (n or D < 1, local_trials outside [0, 255]). */
+size_t npair_eval_kmeans_seed_bytes(int32_t n, int32_t D, int32_t local_trials);
 /* Exact k nearest neighbours (DESIGN 8.3).  For query i the candidates are the gallery rows j of this call other than query i's own
  * (self_offset, global, -1: none; as in npair_eval_best_positive), with s_ij the library's similarity in `precision`: the same bits as
  * the layer's S and as npair_eval_rank's sweeps.  Row i of d_sim / d_index (nq x k, row-major) holds the k candidates that come first

@@ -49,7 +49,7 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
-           "npair_eval_kmeans", "npair_eval_kmeans_bytes", "npair_eval_knn", "npair_eval_knn_bytes",
+           "npair_eval_kmeans", "npair_eval_kmeans_bytes", "npair_eval_kmeans_seed", "npair_eval_kmeans_seed_bytes", "npair_eval_knn", "npair_eval_knn_bytes",
            "npair_eval_class_batches", "npair_eval_class_batches_bytes"]
 
 _LIB = None
@@ -126,6 +126,9 @@ def lib():
         L.npair_eval_kmeans.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, vp]
         L.npair_eval_kmeans_bytes.argtypes = [i32, i32, i32]
         L.npair_eval_kmeans_bytes.restype = C.c_size_t
+        L.npair_eval_kmeans_seed.argtypes = [vp, vp, i32, i32, C.c_uint64, i32, vp, C.POINTER(C.c_uint64), vp]
+        L.npair_eval_kmeans_seed_bytes.argtypes = [i32, i32, i32]
+        L.npair_eval_kmeans_seed_bytes.restype = C.c_size_t
         L.npair_eval_knn.argtypes = [vp, vp, i32, vp, i32, i32, i32, C.c_float, i32, i32, vp, vp, vp]
         L.npair_eval_knn_bytes.argtypes = [i32, i32, i32]
         L.npair_eval_knn_bytes.restype = C.c_size_t
@@ -352,6 +355,12 @@ def eval_kmeans_bytes(n: int, k: int, D: int) -> int:
     return int(lib().npair_eval_kmeans_bytes(n, k, D))
 
 
+def eval_kmeans_seed_bytes(n: int, D: int, local_trials: int = 0) -> int:
+    """Device bytes Evaluator.kmeans_seed adds on top of the workspace for n points of dimension D (local_trials 0: the default
+    trials of k = n, an upper bound; 0 if invalid)."""
+    return int(lib().npair_eval_kmeans_seed_bytes(n, D, local_trials))
+
+
 def eval_knn_bytes(ng: int, k: int, block_rows: int = 0) -> int:
     """Device bytes Evaluator.knn adds on top of the workspace for a gallery of ng rows (block_rows 0: the default; 0 if invalid)."""
     return int(lib().npair_eval_knn_bytes(ng, k, block_rows))
@@ -496,6 +505,18 @@ class Evaluator:
                                             assign.data_ptr(), inertia.data_ptr(), stats, torch.cuda.current_stream().cuda_stream))
         return {"assign": assign, "centroids": centroids, "inertia": inertia, "iterations": stats[0], "changed": stats[1],
                 "empty": stats[2]}
+
+    def kmeans_seed(self, x, k, seed, local_trials=0):
+        """npair_eval_kmeans_seed (DESIGN 8.2): k-means++ seeding of the rows of x, local_trials trials per step (0: 2 + floor(ln k)),
+        random numbers from SplitMix64 seeded with seed modulo 2^64.  Returns (rows, potential): the k row indices, a list that
+        Evaluator.kmeans takes as init_rows, and the final potential phi (a Python int, in the fixed-point units of the header).
+        Synchronises with the host once, at the end."""
+        import torch
+        rows = (C.c_int32 * max(int(k), 1))()
+        phi = C.c_uint64(0)
+        self._check(lib().npair_eval_kmeans_seed(self._h, self._arg(x, 2), x.shape[0], int(k), C.c_uint64(int(seed) % 2 ** 64),
+                                                 int(local_trials), rows, C.byref(phi), torch.cuda.current_stream().cuda_stream))
+        return [rows[i] for i in range(int(k))], int(phi.value)
 
 
 def debug_gemm(precision, backend, A, B):

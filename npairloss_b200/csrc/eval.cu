@@ -54,9 +54,10 @@ struct npair_eval : EvalPlan {
   int2* sym_tiles = nullptr;
   int sym_n = 0;                  // rows of the tile list on the device (0: none yet)
   std::vector<int2> sym_host;     // its host copy (the source of the asynchronous upload)
-  // MAP@R (MapRows, MapPairs), k-means (KmeansBufs), k-NN (KnnBlock) and class-mining (ClassBatchBufs) buffers, grown on demand and kept
-  DevMem map_rows_mem, map_pairs_mem, km_mem, knn_mem, cb_mem;
-  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr, *knn = nullptr, *cb = nullptr;
+  // MAP@R (MapRows, MapPairs), k-means (KmeansBufs), k-NN (KnnBlock), class-mining (ClassBatchBufs) and k-means++ seeding
+  // (KmSeedBufs) buffers, grown on demand and kept
+  DevMem map_rows_mem, map_pairs_mem, km_mem, knn_mem, cb_mem, kms_mem;
+  char *map_rows = nullptr, *map_pairs = nullptr, *km = nullptr, *knn = nullptr, *cb = nullptr, *kms = nullptr;
   StreamOrder order;              // the calls' order across streams
   std::string err;
 };
@@ -100,6 +101,19 @@ struct KmeansBufs : Carve {
     counts = take<int>(k); bias = take<float>(k); rows = take<int>(k); words = take<KmeansWords>(1);
   }
 };
+// k-means++ seeding takes one: the int16 points (rows of kms_dq(D), 32-byte aligned), their squared norms, D_i, the L trials' distance
+// rows, the per-block totals and inclusive prefixes of D_i, the trials' rows and their phi_j sums, the rows picked (k <= n) and the words
+struct KmSeedBufs : Carve {
+  int16_t* q; unsigned long long *norm, *dmin, *dist, *totals, *prefix, *phi_acc; int *cand, *rows; KmSeedWords* words;
+  KmSeedBufs(char* base, long long n, long long D, long long L) : Carve{base} {
+    const long long nb = (n + KMS_THREADS - 1) / KMS_THREADS;
+    q = take<int16_t>(n * kms_dq(D), 256); norm = take<unsigned long long>(n); dmin = take<unsigned long long>(n);
+    dist = take<unsigned long long>(L * n); totals = take<unsigned long long>(nb); prefix = take<unsigned long long>(nb);
+    phi_acc = take<unsigned long long>(L); cand = take<int>(L); rows = take<int>(n); words = take<KmSeedWords>(1);
+  }
+};
+// Trials per step: local_trials, or 0 for sklearn's 2 + floor(ln k)
+static int kms_trials(int local_trials, int k) { return local_trials ? local_trials : 2 + static_cast<int>(std::floor(std::log(static_cast<double>(k)))); }
 // k-NN takes one: a block of `rows` rows of S, each round_up(ng, 32) floats long (the stride the similarity GEMM's stores need)
 struct KnnBlock : Carve {
   float* S; long long ldS;
@@ -153,6 +167,11 @@ size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r) {
 size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D) {
   if (n < 1 || k < 1 || D < 1 || k > n) return 0;
   return KmeansBufs(nullptr, n, k, D).bytes;
+}
+
+size_t npair_eval_kmeans_seed_bytes(int32_t n, int32_t D, int32_t local_trials) {
+  if (n < 1 || D < 1 || local_trials < 0 || local_trials > KMS_MAX_TRIALS) return 0;
+  return KmSeedBufs(nullptr, n, D, kms_trials(local_trials, n)).bytes;
 }
 
 size_t npair_eval_knn_bytes(int32_t ng, int32_t k, int32_t block_rows) {
@@ -508,6 +527,50 @@ int npair_eval_kmeans(npair_eval* ev, const float* x, int32_t n, int32_t k, cons
   stats[0] = t + 1;
   stats[1] = static_cast<int32_t>(h.changed);
   stats[2] = k - static_cast<int32_t>(h.nonempty);
+  return NPAIR_OK;
+}
+
+// k-means++ seeding (DESIGN 8.2): max|x| and the int16 points once, then per step t the distance kernel over the step's trials (its
+// last block picks centre t) and the update kernel (its last block draws step t + 1's trials); the rows, phi and the error bits are read
+// back once, at the end.
+int npair_eval_kmeans_seed(npair_eval* ev, const float* x, int32_t n, int32_t k, uint64_t seed, int32_t local_trials, int32_t* rows_host,
+                           uint64_t* potential_host, void* stream) {
+  if (!ev) return NPAIR_E_ARG;
+  if (!x || !rows_host) { ev->err = "null pointer argument"; return NPAIR_E_ARG; }
+  if (n < 1 || n > ev->max_q) { ev->err = fmt("n = %d points must lie in [1, %d], the evaluator's query capacity", n, ev->max_q); return NPAIR_E_ARG; }
+  if (k < 1 || k > n) { ev->err = fmt("k-means++ needs 1 <= k <= n (n = %d, k = %d)", n, k); return NPAIR_E_ARG; }
+  if (local_trials < 0 || local_trials > KMS_MAX_TRIALS) {
+    ev->err = fmt("local_trials = %d must lie in [0, %d]", local_trials, KMS_MAX_TRIALS);
+    return NPAIR_E_ARG;
+  }
+  if (static_cast<long long>(n) * ev->D >= (1ll << 36)) {
+    ev->err = fmt("n * D = %lld reaches 2^36: the potential would not fit in 64 bits", static_cast<long long>(n) * ev->D);
+    return NPAIR_E_ARG;
+  }
+  const int L = kms_trials(local_trials, k);
+  int rc;
+  OrderedCall call(ev, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
+  if ((rc = eval_grow(ev, ev->kms_mem, &ev->kms, KmSeedBufs(nullptr, n, ev->D, L).bytes, "the k-means++ buffers")) != NPAIR_OK) return rc;
+  const KmSeedBufs b(ev->kms, n, ev->D, L);
+  unsigned int* amx = ev->absmax_bits;
+  CUDA_TRY(ev, cudaMemsetAsync(amx, 0, sizeof(unsigned int), st));
+  CUDA_TRY(ev, cudaMemsetAsync(b.words, 0, sizeof(KmSeedWords), st));
+  CUDA_TRY(ev, cudaMemsetAsync(b.phi_acc, 0, sizeof(unsigned long long) * L, st));
+  launch_eval_prep(x, static_cast<long long>(n) * ev->D, nullptr, 0, amx, ev->ra, 0, ev->sms, st);
+  launch_kms_quantise(x, n, ev->D, amx, seed, b.q, b.norm, b.dmin, b.cand, b.words, st);
+  for (int t = 0; t < k; ++t) {
+    launch_kms_distance(b.q, b.norm, b.dmin, n, ev->D, b.cand, t ? L : 1, t, b.dist, b.phi_acc, b.rows, b.words, st);
+    launch_kms_update(b.dmin, b.dist, n, seed, t, t + 1 < k ? L : 0, b.totals, b.prefix, b.cand, b.words, st);
+  }
+  CUDA_TRY(ev, cudaGetLastError());
+  KmSeedWords h{};
+  CUDA_TRY(ev, cudaMemcpyAsync(rows_host, b.rows, sizeof(int32_t) * k, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ev, cudaMemcpyAsync(&h, b.words, sizeof(h), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ev, cudaStreamSynchronize(st));
+  if (h.err & DERR_KMEANS_NO_ARGMAX) { ev->err = "x holds NaN or infinity"; return NPAIR_E_CUDA; }
+  if (potential_host) *potential_host = h.phi;
   return NPAIR_OK;
 }
 

@@ -338,6 +338,235 @@ void launch_km_inertia(const float* x, const float* C, const int* assign, int n,
 }
 
 // --------------------------------------------------------------------------------------------
+// k-means++ seeding (npair_eval_kmeans_seed, DESIGN 8.2): exact integer distances, so every sum is order-free and any grid gives the
+// same bits.  Step t = the distance kernel (its last block picks the centre) + the update kernel (its last block draws step t + 1).
+// --------------------------------------------------------------------------------------------
+// u(seed, t, j): output number t * 256 + j + 1 of SplitMix64 seeded with `seed`
+__device__ __forceinline__ unsigned long long kms_u(unsigned long long seed, int t, int j) {
+  unsigned long long z = seed + (static_cast<unsigned long long>(t) * 256 + j + 1) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Inclusive scan of one uint64 per thread over a block of KMS_THREADS threads; *total = the block's sum.  s_w: KMS_THREADS / 32 words.
+__device__ unsigned long long kms_block_scan(unsigned long long v, unsigned long long* s_w, unsigned long long* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned long long incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  __syncthreads();                                           // the previous scan has read s_w
+  if (lane == 31) s_w[w] = incl;
+  __syncthreads();
+  unsigned long long before = 0, all = 0;
+  for (int k = 0; k < KMS_THREADS / 32; ++k) {
+    if (k < w) before += s_w[k];
+    all += s_w[k];
+  }
+  *total = all;
+  return before + incl;
+}
+
+// One warp per point: q = rint((x * sigma) * 2^13) (both products exact, one rounding to nearest even), rows padded with zeros to
+// kms_dq(D); norm = sum q^2; dmin = UINT64_MAX (no centre yet).  Block 0 draws step 0's row.
+__global__ void __launch_bounds__(256) kms_quantise_kernel(const float* __restrict__ x, int n, int D, const unsigned int* __restrict__ absmax_bits,
+                                                           unsigned long long seed, int16_t* __restrict__ q, unsigned long long* __restrict__ norm,
+                                                           unsigned long long* __restrict__ dmin, int* __restrict__ cand, KmSeedWords* words) {
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (blockIdx.x == 0 && threadIdx.x == 0) cand[0] = static_cast<int>(__umul64hi(kms_u(seed, 0, 0), static_cast<unsigned long long>(n)));
+  if (i >= n) return;
+  const float sigma = pre_scale(__uint_as_float(*absmax_bits)).scale;
+  const long long Dq = kms_dq(D);
+  const float* xr = x + static_cast<long long>(i) * D;
+  int16_t* qr = q + i * Dq;
+  unsigned long long s = 0;
+  bool bad = false;
+  for (int d = lane; d < Dq; d += 32) {
+    const float v = d < D ? __ldg(xr + d) : 0.f;
+    int qi = 0;
+    if (isfinite(v)) qi = __float2int_rn((v * sigma) * 8192.f);
+    else bad = true;
+    qr[d] = static_cast<int16_t>(qi);
+    s += static_cast<unsigned long long>(qi * qi);
+  }
+  s = warp_sum_u64(s);
+  if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(&words->err, static_cast<unsigned int>(DERR_KMEANS_NO_ARGMAX));
+  if (lane == 0) { norm[i] = s; dmin[i] = ~0ull; }
+}
+void launch_kms_quantise(const float* x, int n, int D, const unsigned int* absmax_bits, unsigned long long seed, int16_t* q,
+                         unsigned long long* norm, unsigned long long* dmin, int* cand, KmSeedWords* words, cudaStream_t st) {
+  kms_quantise_kernel<<<(n + 7) / 8, 256, 0, st>>>(x, n, D, absmax_bits, seed, q, norm, dmin, cand, words);
+  count_launch();
+}
+
+// One thread per point.  The trials' rows are staged in shared memory as int32, KMS_LC trials by KMS_DC features at a time, and each
+// thread reads its row 16 features (32 bytes) at a time: dot_j = sum q_i q_c in int32 per 16 features (|sum| <= 2^30), added in int64,
+// and d(i, c) = ||q_i||^2 + ||q_c||^2 - 2 dot, exact.  Per-block sums of min(dmin, d) go to phi_acc by 64-bit integer atomics.
+constexpr int KMS_LC = 16, KMS_DC = 512;
+__global__ void __launch_bounds__(KMS_THREADS) kms_distance_kernel(const int16_t* __restrict__ q, const unsigned long long* __restrict__ norm,
+                                                                   const unsigned long long* __restrict__ dmin, int n, int D,
+                                                                   const int* __restrict__ cand, int L, int t,
+                                                                   unsigned long long* __restrict__ dist, unsigned long long* phi_acc,
+                                                                   int* __restrict__ rows, KmSeedWords* words) {
+  __shared__ __align__(16) int s_c[KMS_LC][KMS_DC];
+  __shared__ unsigned long long s_red[KMS_THREADS / 32][KMS_LC];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int i = blockIdx.x * KMS_THREADS + tid;
+  const bool live = i < n;
+  const long long Dq = kms_dq(D);
+  const int16_t* qr = q + static_cast<long long>(live ? i : 0) * Dq;
+  const unsigned long long dm = live ? dmin[i] : 0, ni = live ? norm[i] : 0;
+  for (int jc = 0; jc < L; jc += KMS_LC) {
+    const int lc = min(KMS_LC, L - jc);
+    long long acc[KMS_LC];
+#pragma unroll
+    for (int j = 0; j < KMS_LC; ++j) acc[j] = 0;
+    for (long long d0 = 0; d0 < Dq; d0 += KMS_DC) {
+      const int dc = static_cast<int>(min(static_cast<long long>(KMS_DC), Dq - d0));
+      __syncthreads();                                       // every thread is done with the previous stage
+      for (int e = tid; e < lc * dc; e += KMS_THREADS) {
+        const int j = e / dc, d = e - j * dc;
+        s_c[j][d] = q[static_cast<long long>(cand[jc + j]) * Dq + d0 + d];
+      }
+      __syncthreads();
+      if (live) {
+        for (int d = 0; d < dc; d += 16) {
+          const int4 w0 = __ldg(reinterpret_cast<const int4*>(qr + d0 + d)), w1 = __ldg(reinterpret_cast<const int4*>(qr + d0 + d + 8));
+          const int wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+          int a[16];
+#pragma unroll
+          for (int m = 0; m < 8; ++m) { a[2 * m] = static_cast<int16_t>(wv[m]); a[2 * m + 1] = wv[m] >> 16; }
+#pragma unroll
+          for (int j = 0; j < KMS_LC; ++j) {
+            if (j < lc) {
+              const int4* c4 = reinterpret_cast<const int4*>(&s_c[j][d]);
+              int s = 0;
+#pragma unroll
+              for (int m = 0; m < 4; ++m) {
+                const int4 c = c4[m];
+                s += a[4 * m] * c.x + a[4 * m + 1] * c.y + a[4 * m + 2] * c.z + a[4 * m + 3] * c.w;
+              }
+              acc[j] += s;
+            }
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < KMS_LC; ++j) {
+      if (j < lc) {
+        unsigned long long m = 0;
+        if (live) {
+          const unsigned long long dij = static_cast<unsigned long long>(static_cast<long long>(ni + norm[cand[jc + j]]) - 2 * acc[j]);
+          dist[static_cast<long long>(jc + j) * n + i] = dij;
+          m = dm < dij ? dm : dij;
+        }
+        m = warp_sum_u64(m);
+        if (lane == 0) s_red[w][j] = m;
+      }
+    }
+    __syncthreads();
+    if (tid < lc) {
+      unsigned long long s = 0;
+      for (int k = 0; k < KMS_THREADS / 32; ++k) s += s_red[k][tid];
+      atomicAdd(&phi_acc[jc + tid], s);
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&words->ticket_dist, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last || tid != 0) return;
+  __threadfence();
+  unsigned long long best = 0;
+  int jb = 0;
+  for (int j = 0; j < L; ++j) {
+    const unsigned long long v = atomicExch(&phi_acc[j], 0ull);   // read and clear for the next step
+    if (j == 0 || v < best) { best = v; jb = j; }
+  }
+  words->jstar = static_cast<unsigned int>(jb);
+  rows[t] = cand[jb];
+  words->ticket_dist = 0;
+}
+void launch_kms_distance(const int16_t* q, const unsigned long long* norm, const unsigned long long* dmin, int n, int D, const int* cand,
+                         int L, int t, unsigned long long* dist, unsigned long long* phi_acc, int* rows, KmSeedWords* words, cudaStream_t st) {
+  kms_distance_kernel<<<(n + KMS_THREADS - 1) / KMS_THREADS, KMS_THREADS, 0, st>>>(q, norm, dmin, n, D, cand, L, t, dist, phi_acc, rows,
+                                                                                   words);
+  count_launch();
+}
+
+// One thread per point: dmin = min(dmin, d(i, centre t)), and the block's total.  The last block scans the totals into prefix (phi is
+// the last), then per trial j of step t + 1: target = floor(u phi / 2^64), the block b whose inclusive prefix first exceeds it, and in b
+// the first point whose inclusive prefix exceeds it (a point at distance 0 is never drawn); phi = 0 draws floor(u n / 2^64).
+__global__ void __launch_bounds__(KMS_THREADS) kms_update_kernel(unsigned long long* __restrict__ dmin, const unsigned long long* __restrict__ dist,
+                                                                 int n, unsigned long long seed, int t, int L_next,
+                                                                 unsigned long long* __restrict__ totals, unsigned long long* __restrict__ prefix,
+                                                                 int* __restrict__ cand, KmSeedWords* words) {
+  __shared__ unsigned long long s_w[KMS_THREADS / 32];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, i = blockIdx.x * KMS_THREADS + tid;
+  unsigned long long v = 0;
+  if (i < n) {
+    const unsigned long long dc = dist[static_cast<long long>(words->jstar) * n + i], d0 = dmin[i];
+    v = dc < d0 ? dc : d0;
+    dmin[i] = v;
+  }
+  unsigned long long tot;
+  kms_block_scan(v, s_w, &tot);
+  if (tid == 0) totals[blockIdx.x] = tot;
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&words->ticket_upd, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  const int nb = gridDim.x;
+  unsigned long long carry = 0;
+  for (int b0 = 0; b0 < nb; b0 += KMS_THREADS) {
+    const int b = b0 + tid;
+    const unsigned long long incl = kms_block_scan(b < nb ? __ldcg(totals + b) : 0ull, s_w, &tot);
+    if (b < nb) prefix[b] = carry + incl;
+    carry += tot;
+  }
+  const unsigned long long phi = carry;
+  if (tid == 0) { words->phi = phi; words->ticket_upd = 0; }
+  __syncthreads();                                           // prefix is visible to the whole block
+  for (int j = 0; j < L_next; ++j) {
+    const unsigned long long u = kms_u(seed, t + 1, j);
+    if (phi == 0) {
+      if (tid == 0) cand[j] = static_cast<int>(__umul64hi(u, static_cast<unsigned long long>(n)));
+      continue;
+    }
+    const unsigned long long target = __umul64hi(u, phi);    // < phi
+    int lo = 0, hi = nb - 1;                                 // the first block with prefix > target
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (prefix[mid] > target) hi = mid; else lo = mid + 1;
+    }
+    const unsigned long long r = target - (lo ? prefix[lo - 1] : 0ull);
+    const int idx = lo * KMS_THREADS + tid;
+    const unsigned long long x = idx < n ? __ldcg(dmin + idx) : 0ull;
+    const unsigned long long incl = kms_block_scan(x, s_w, &tot);
+    if (incl > r && incl - x <= r) cand[j] = idx;
+  }
+}
+void launch_kms_update(unsigned long long* dmin, const unsigned long long* dist, int n, unsigned long long seed, int t, int L_next,
+                       unsigned long long* totals, unsigned long long* prefix, int* cand, KmSeedWords* words, cudaStream_t st) {
+  kms_update_kernel<<<(n + KMS_THREADS - 1) / KMS_THREADS, KMS_THREADS, 0, st>>>(dmin, dist, n, seed, t, L_next, totals, prefix, cand, words);
+  count_launch();
+}
+
+// --------------------------------------------------------------------------------------------
 // hard negative class mining (npair_eval_class_batches, DESIGN 8.4): the greedy pick of each batch's classes from the stored S
 // --------------------------------------------------------------------------------------------
 // The maximum of a 64-bit key over the warp: of the high words, then of the low words among the lanes that hold the maximal high word

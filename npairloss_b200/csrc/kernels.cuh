@@ -374,6 +374,25 @@ void launch_km_assign(unsigned long long* best, const float* x, int n, int D, co
 void launch_km_update(long long* sums, const int* counts, const unsigned int* absmax_bits, int k, int D, float* C, cudaStream_t st);
 // *out = sum_i ||x_i - C[assign[i]]||^2 in fp64, in a fixed order (partial: KM_INERTIA_BLOCKS doubles of scratch)
 void launch_km_inertia(const float* x, const float* C, const int* assign, int n, int D, double* partial, double* out, cudaStream_t st);
+// k-means++ seeding (npair_eval_kmeans_seed, DESIGN 8.2): the points as int16 q = rint(x * sigma * 2^13), rows of KMS_DQ(D) elements,
+// exact uint64 distances, one distance kernel and one update-and-sample kernel per step, blocks of KMS_THREADS points
+constexpr int KMS_THREADS = 256;
+constexpr int KMS_MAX_TRIALS = 255;             // u(seed, t, j) numbers j < 256 per step
+__host__ __device__ inline long long kms_dq(long long D) { return (D + 15) / 16 * 16; }
+// What the steps pass each other and the host: the potential phi, the error bits, the step's winning trial and the last-block tickets
+struct KmSeedWords { unsigned long long phi; unsigned int err, jstar, ticket_dist, ticket_upd; };
+// q = the points' int16 rows, norm[i] = sum q_i^2, dmin[i] = UINT64_MAX, cand[0] = step 0's row; DERR_KMEANS_NO_ARGMAX in
+// words->err (pre-zeroed) for a non-finite x
+void launch_kms_quantise(const float* x, int n, int D, const unsigned int* absmax_bits, unsigned long long seed, int16_t* q,
+                         unsigned long long* norm, unsigned long long* dmin, int* cand, KmSeedWords* words, cudaStream_t st);
+// Step t, its L trials cand[0, L): dist[j][i] = d(i, cand[j]), phi_j = sum_i min(dmin[i], dist[j][i]); the last block stores the
+// trial of least phi_j (lowest j on ties) in words->jstar and its row in rows[t]
+void launch_kms_distance(const int16_t* q, const unsigned long long* norm, const unsigned long long* dmin, int n, int D, const int* cand,
+                         int L, int t, unsigned long long* dist, unsigned long long* phi_acc, int* rows, KmSeedWords* words, cudaStream_t st);
+// dmin[i] = min(dmin[i], dist[jstar][i]); the last block scans the block totals into words->phi and, for L_next > 0, draws step t + 1's
+// trials into cand[0, L_next)
+void launch_kms_update(unsigned long long* dmin, const unsigned long long* dist, int n, unsigned long long seed, int t, int L_next,
+                       unsigned long long* totals, unsigned long long* prefix, int* cand, KmSeedWords* words, cudaStream_t st);
 // Hard negative class mining (npair_eval_class_batches, DESIGN 8.4): for each of the nb pools (pools [nb][P], P <= CLASS_POOL_MAX,
 // distinct ids < the rows of S), the greedy batch of n >= 2 classes over the stored S (row c = class c, stride ldS) into batches
 // [nb][n] and, unless NULL, the scores they were picked at into scores [nb][n] (NaN for the seed).  One block per batch, CB_ENTRIES

@@ -250,15 +250,24 @@ def retrieval_metrics(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8),
     return out, per_query
 
 
-def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi.PREC_FP32_FP16X2):
+def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi.PREC_FP32_FP16X2, init="random", n_init=1,
+                       local_trials=0):
     """NMI and F1 of a k-means clustering of a whole embedding set, the clustering half of the metric-learning protocol (Sohn 2016;
     Song et al. 2016), with Lloyd's k-means on the tensor cores (Evaluator.kmeans, DESIGN 8.2; not part of the reference layer).
 
     Takes CUDA fp32 embeddings as given (L2-normalise them first for cosine geometry) and labels of any numeric dtype that fp32 holds
-    exactly (ValueError otherwise), compared as floats.  k=None: the number of distinct labels.  Centroid c starts as row init[c] of
-    init = torch.randperm(n, generator=torch.Generator().manual_seed(seed))[:k], so the same seed gives the same result; there is
-    one run, no restarts.  Returns ({"nmi", "f1", "inertia", "iterations", "converged", "empty_clusters"}, assign, centroids) with
-    the scores of clustering_scores, "converged" whether the last sweep changed no assignment, and assign / centroids CUDA tensors."""
+    exactly (ValueError otherwise), compared as floats.  k=None: the number of distinct labels.  n_init runs, r = 0 .. n_init - 1, each
+    seeded with seed + r and started from k rows of the points:
+      init="random":     centroid c starts as row init[c] of init = torch.randperm(n, generator=torch.Generator().manual_seed(seed + r))[:k]
+      init="k-means++":  the rows of Evaluator.kmeans_seed(x, k, seed + r, local_trials) (exact, GPU; local_trials 0: 2 + floor(ln k))
+    The run with the least inertia (fp64, fixed order) is kept, ties to the lowest r, so the same arguments give the same result; the
+    defaults are one run from a random permutation.  Returns ({"nmi", "f1", "inertia", "iterations", "converged", "empty_clusters",
+    "restart", "inertias"}, assign, centroids) with the scores of clustering_scores, "converged" whether the last sweep changed no
+    assignment, "restart" the r kept, "inertias" every run's inertia, and assign / centroids CUDA tensors of the run kept."""
+    if init not in ("random", "k-means++"):
+        raise ValueError(f'clustering_metrics: init = {init!r} is not "random" or "k-means++"')
+    if int(n_init) < 1:
+        raise ValueError(f"clustering_metrics needs n_init >= 1 (got {n_init})")
     x, lab, _, _, _ = _retrieval_sets("clustering_metrics", emb, labels, None, None, None)
     n, D = x.shape
     if k is None:
@@ -266,16 +275,25 @@ def clustering_metrics(emb, labels, k=None, seed=0, max_iter=100, precision=capi
     k = int(k)
     if not 1 <= k <= n:
         raise ValueError(f"clustering_metrics needs 1 <= k <= n (n = {n}, k = {k})")
-    init = torch.randperm(n, generator=torch.Generator().manual_seed(int(seed)))[:k].tolist()
     ev = capi.Evaluator(n, k, D, precision, x.device.index or 0)
+    best, best_r, inertias = None, 0, []
     try:
-        res = ev.kmeans(x, k, init, max_iter)
+        for r in range(int(n_init)):
+            s = int(seed) + r
+            if init == "random":
+                rows = torch.randperm(n, generator=torch.Generator().manual_seed(s))[:k].tolist()
+            else:
+                rows = ev.kmeans_seed(x, k, s, local_trials)[0]
+            res = ev.kmeans(x, k, rows, max_iter)
+            inertias.append(float(res["inertia"]))
+            if best is None or inertias[-1] < inertias[best_r]:
+                best, best_r = res, r
     finally:
         ev.close()
-    nmi, f1 = clustering_scores(lab, res["assign"])
-    out = {"nmi": nmi, "f1": f1, "inertia": float(res["inertia"]), "iterations": res["iterations"],
-           "converged": res["changed"] == 0, "empty_clusters": res["empty"]}
-    return out, res["assign"], res["centroids"]
+    nmi, f1 = clustering_scores(lab, best["assign"])
+    out = {"nmi": nmi, "f1": f1, "inertia": inertias[best_r], "iterations": best["iterations"], "converged": best["changed"] == 0,
+           "empty_clusters": best["empty"], "restart": best_r, "inertias": inertias}
+    return out, best["assign"], best["centroids"]
 
 
 def clustering_scores(labels, assign):
