@@ -360,7 +360,8 @@ size_t npair_eval_map_at_r_bytes(int32_t nq, int64_t sum_r);
  *      computed in fp32 from the fp32 centroid;
  *   3. stop if t > 0 and no assignment changed, or if t + 1 = max_iter;
  *   4. else C_{t+1} = the members' means by the fixed-point rule below; an EMPTY cluster keeps its centroid.
- * sigma = the pre-scale of max|x| over the points (a power of two with max|x * sigma| in [0.5, 1)), in every format.  Each member adds
+ * sigma = the pre-scale of max|x| over the points, in every format: 2^-e with max|x| = m 2^e, m in [0.5, 1), e clamped to [-126, 127]
+ * (so max|x * sigma| is in [0.5, 1) for max|x| in [2^-127, 2^127), and in [1, 2) above).  Each member adds
  * q_id = rint(x_id * sigma * 2^32) to the int64 sum S_c[d] (64-bit integer atomics: exact, and independent of their order), and
  * mu_c[d] = (float)( ldexp((double)S_c[d] / count_c, -32) * (1 / sigma) ).  Inertia = sum_i ||x_i - mu_{a_i}||^2 in fp64 from the fp32
  * values, in a fixed order.  Every output has the same bits on every call and on a fresh evaluator.
@@ -373,7 +374,8 @@ int npair_eval_kmeans(npair_eval* ev, const float* d_x, int32_t n, int32_t k, co
 size_t npair_eval_kmeans_bytes(int32_t n, int32_t k, int32_t D);
 /* k-means++ seeding (Arthur & Vassilvitskii 2007, with sklearn's greedy local trials; DESIGN 8.2): the k initial rows of
  * npair_eval_kmeans, rows_host[k] (HOST int32, exactly what npair_eval_kmeans takes as init_rows_host), by exact integer arithmetic:
- *   sigma = the pre-scale of max|x| over the n points (as npair_eval_kmeans); q_id = rint(x_id * sigma * 2^13) as int16 (|q| <= 2^13);
+ *   sigma = the pre-scale of max|x| over the n points (as npair_eval_kmeans), halved for max|x| >= 2^127 (2^-max(e, -126) with
+ *     max|x| = m 2^e, m in [0.5, 1)); q_id = rint(x_id * sigma * 2^13) as int16 (|x * sigma| < 1, so |q| <= 2^13);
  *   d(i, j) = sum_d (q_id - q_jd)^2 in uint64;  D_i = min over the centres chosen so far of d(i, c);  phi = sum_i D_i (exact: n D < 2^36);
  *   u(seed, t, j) = output number t * 256 + j + 1 of SplitMix64 seeded with `seed`, i.e. mix(seed + (t * 256 + j + 1) * 0x9E3779B97F4A7C15)
  *     with mix the SplitMix64 finaliser (seed 0: outputs 1, 2, 3 are 0xe220a8397b1dcdaf, 0x6e789e6aa1b965f4, 0x06c45d188009454f);

@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(256) km_assign_kernel(unsigned long long* __re
       const float sigma = pre_scale(__uint_as_float(*absmax_bits)).scale;
       const float* xr = x + static_cast<long long>(i) * D;
       unsigned long long* sr = reinterpret_cast<unsigned long long*>(sums + static_cast<long long>(a) * D);
-      for (int d = lane; d < D; d += 32)    // x * sigma in (-1, 1) and the scaling by 2^32 are exact; one rounding, to nearest even
+      for (int d = lane; d < D; d += 32)    // x * sigma in (-2, 2) and the scaling by 2^32 are exact; one rounding, to nearest even
         atomicAdd(&sr[d], static_cast<unsigned long long>(__float2ll_rn((__ldg(xr + d) * sigma) * 4294967296.f)));
     }
   }
@@ -384,7 +384,9 @@ __global__ void __launch_bounds__(256) kms_quantise_kernel(const float* __restri
   const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (blockIdx.x == 0 && threadIdx.x == 0) cand[0] = static_cast<int>(__umul64hi(kms_u(seed, 0, 0), static_cast<unsigned long long>(n)));
   if (i >= n) return;
-  const float sigma = pre_scale(__uint_as_float(*absmax_bits)).scale;
+  // the points' pre-scale, halved where its clamped exponent leaves max|x * sigma| in [1, 2) (max|x| >= 2^127), so that |q| <= 2^13
+  const float amax = __uint_as_float(*absmax_bits);
+  const float sigma = pre_scale(amax).scale * (amax >= 0x1p127f ? 0.5f : 1.f);
   const long long Dq = kms_dq(D);
   const float* xr = x + static_cast<long long>(i) * D;
   int16_t* qr = q + i * Dq;

@@ -84,7 +84,7 @@ struct GemmParams {
   float* S;            // [M x ldS] fp32 similarities
   long long ldS;       // multiple of 32
   const float* dev_scale;  // device scalar: inverse operand pre-scale (power of two) or NULL.  A similarity epilogue multiplies the
-                           // accumulators by its square (both operands were pre-scaled), EPI_OUT multiplies alpha by it
+                           // accumulators by it twice (both operands were pre-scaled), EPI_OUT multiplies alpha by it
   const float* lab_rows;   // [M]  labels of this rank's rows
   const float* lab_cols;   // [Nn] labels of all columns
   int self_offset;         // rank * Q : column index of row 0's self pair
@@ -370,8 +370,9 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.ts.num_tiles();
+  // a similarity is acc * inv_scale * inv_scale, left to right as the SIMT check computes it: the square alone overflows (underflows)
+  // for a pre-scale exponent above 63 (below -63), and a zero accumulator times an infinite square would be NaN
   const float inv_scale = p.dev_scale ? *p.dev_scale : 1.f;
-  const float out_scale = (EPI != EPI_OUT) ? inv_scale * inv_scale : 1.f;
   const float alpha = p.alpha * inv_scale;
 
   if (warp == 0 && lane == 0) {
@@ -577,7 +578,8 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             const float4 t4 = *reinterpret_cast<const float4*>(accs + srow * 256 + (((half * 8 + q) ^ (srow & 7)) << 4));
-            v[4 * q] = t4.x * out_scale; v[4 * q + 1] = t4.y * out_scale; v[4 * q + 2] = t4.z * out_scale; v[4 * q + 3] = t4.w * out_scale;
+            v[4 * q] = t4.x * inv_scale * inv_scale; v[4 * q + 1] = t4.y * inv_scale * inv_scale;
+            v[4 * q + 2] = t4.z * inv_scale * inv_scale; v[4 * q + 3] = t4.w * inv_scale * inv_scale;
           }
         }
         // direct store, 4 rows x 128 bytes per instruction (whole lines); ldS is a multiple of 32, so a partial last chunk stores
@@ -590,7 +592,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             const int grow = t.m_blk * BM + ew * 32 + rr;
             const int sr = (wi & 1) * 32 + rr;
             float4 o = *reinterpret_cast<const float4*>(accs + sr * 256 + (((half * 8 + cq) ^ (sr & 7)) << 4));
-            o.x *= out_scale; o.y *= out_scale; o.z *= out_scale; o.w *= out_scale;
+            o.x = o.x * inv_scale * inv_scale; o.y = o.y * inv_scale * inv_scale; o.z = o.z * inv_scale * inv_scale; o.w = o.w * inv_scale * inv_scale;
             if (grow < p.M) *reinterpret_cast<float4*>(p.S + static_cast<long long>(grow) * p.ldS + col0 + 4 * cq) = o;
           }
         }
@@ -613,7 +615,7 @@ split_gemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           const bool fast = col0 + 32 <= p.Nn && (self_col < col0 || self_col >= col0 + 32);
           // entry c of this thread's chunk, bit for bit the v[c] above, read back from the staging tile by a runtime index
           const auto staged = [&](int c) {
-            return *reinterpret_cast<const float*>(accs + srow * 256 + (((half * 8 + (c >> 2)) ^ (srow & 7)) << 4) + (c & 3) * 4) * out_scale;
+            return *reinterpret_cast<const float*>(accs + srow * 256 + (((half * 8 + (c >> 2)) ^ (srow & 7)) << 4) + (c & 3) * 4) * inv_scale * inv_scale;
           };
           if constexpr (GATHER) {
             // the warp-uniform label-range skip of EPI_STATS: a chunk without a same-label column for any row of the warp

@@ -200,13 +200,16 @@ struct BlockScalars {
   float x_scale, x_inv_scale;              // pre_scale(x_absmax) for PREC_FP16X2; 1 for other precisions
 };
 
-// The operand pre-scale of a set whose largest |x| is `absmax`: a power of two with max|x * scale| in [0.5, 1), so the split is exact
-// and the inverse undoes it exactly; 1 when absmax is 0 or not finite
+// The operand pre-scale of a set whose largest |x| is `absmax`: scale = 2^-e and inv = 2^e, with absmax = m 2^e, m in [0.5, 1), and e
+// clamped to [-126, 127] so that both are finite (at e = 127 the scale is the subnormal 2^-127, exact since nothing here is built with
+// -ftz).  max|x * scale| is in [0.5, 1) for absmax in [2^-127, 2^127), below 0.5 under it and in [1, 2) above it; the scaling is exact
+// either way, and the inverse undoes it exactly.  1 when absmax is 0 or not finite.
 struct PreScale { float scale, inv; };
 __host__ __device__ inline PreScale pre_scale(float absmax) {
   float sc = 1.f, inv = 1.f;
   if (absmax > 0.f && isfinite(absmax)) {
     int e; frexpf(absmax, &e);                 // absmax = m * 2^e, m in [0.5,1)
+    e = e < -126 ? -126 : (e > 127 ? 127 : e);
     sc = ldexpf(1.f, -e); inv = ldexpf(1.f, e);
   }
   return PreScale{sc, inv};

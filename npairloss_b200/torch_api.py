@@ -429,7 +429,7 @@ def class_embeddings(emb, labels, normalize=True):
     class_emb fp32 [C, D]), row c the class class_labels[c].
 
     The mean is the fixed-point rule of the k-means update (DESIGN 8.2): with sigma the pre-scale of max|x| over emb (a power of two
-    with max|x * sigma| in [0.5, 1)), int64 sums of rint(x * sigma * 2^32), exact and independent of order, then
+    with max|x * sigma| in [0.5, 1), up to its exponent clamp at the ends of the fp32 range), int64 sums of rint(x * sigma * 2^32), exact and independent of order, then
     (float)(ldexp(sum / count, -32) / sigma); so the result has the same bits on every run and device.  Labels of any numeric dtype
     that fp32 holds exactly; NaN labels raise ValueError.  normalize=True then L2-normalises each row (npair_l2normalize_forward, CUDA
     only); normalize=False also takes CPU tensors."""
@@ -446,7 +446,7 @@ def class_embeddings(emb, labels, normalize=True):
     amax = float(x.abs().max()) if x.numel() else 0.0
     if not math.isfinite(amax):
         raise ValueError("class_embeddings takes finite embeddings")
-    e = math.frexp(amax)[1] if amax > 0 else 0
+    e = min(max(math.frexp(amax)[1], -126), 127) if amax > 0 else 0      # pre_scale's exponent: 2^-e and 2^e finite in fp32
     class_labels, cls = torch.unique(lab, sorted=True, return_inverse=True)
     q = torch.round((x * (2.0 ** -e)).double() * 2.0 ** 32).long()          # x * sigma and the scaling by 2^32 are exact
     sums = torch.zeros(class_labels.numel(), x.shape[1], dtype=torch.int64, device=x.device).index_add_(0, cls, q)

@@ -69,8 +69,9 @@ def check_map(out, ref):
 
 
 def sigma_exp(x):
-    """e with pre_scale(max|x|) = 2^-e (max|x| = m 2^e, m in [0.5, 1)); 0 for an all-zero x (sigma = 1)"""
-    return int(np.frexp(np.float32(np.abs(x).max()))[1])
+    """e with pre_scale(max|x|) = 2^-e: max|x| = m 2^e, m in [0.5, 1), clamped to [-126, 127] so that 2^-e and 2^e are finite fp32
+    values; 0 for an all-zero x (sigma = 1)"""
+    return min(max(int(np.frexp(np.float32(np.abs(x).max()))[1]), -126), 127) if np.any(x) else 0
 
 
 def update_ref(x, assign, C):

@@ -28,10 +28,11 @@ def default_trials(k):
 
 
 def quantise(x):
-    """q = rint((x * sigma) * 2^13) in fp32 arithmetic, sigma = pre_scale(max|x|): 2^-e with max|x| = m 2^e, m in [0.5, 1); 1 for 0"""
+    """q = rint((x * sigma) * 2^13) in fp32 arithmetic, sigma = 2^-max(e, -126) with max|x| = m 2^e, m in [0.5, 1) (pre_scale(max|x|),
+    halved where its exponent clamp at 127 would leave |x * sigma| >= 1); 1 for 0"""
     x = np.asarray(x, np.float32)
     amax = np.float32(np.abs(x).max()) if x.size else np.float32(0)
-    sigma = np.float32(2.0 ** -int(np.frexp(amax)[1])) if amax > 0 else np.float32(1)
+    sigma = np.float32(2.0 ** -max(int(np.frexp(amax)[1]), -126)) if amax > 0 else np.float32(1)
     return np.rint((x * sigma) * np.float32(8192)).astype(np.int64)
 
 

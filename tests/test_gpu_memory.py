@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 
 from npairloss_b200 import capi, synth
-from gpu_harness import G_TOL, S_ABS, S_REL
+from gpu_harness import G_TOL
+import sim_ref
 from memory_ref import step_memory
 
 pytestmark = pytest.mark.gpu
@@ -74,10 +75,8 @@ def _same_bits(a, b, tag, S=True):
 def _check_parity(g, x, l, xm, lm, mining, prec, lw, num_tops=5, tag=""):
     """Level 1: S against fp64.  Level 2: the test reference's memory step on the GPU's own S."""
     Q = x.shape[0]
-    xt = np.concatenate([x, xm]).astype(np.float64)
-    S_ref = (x.astype(np.float64) @ xt.T).astype(np.float32)
-    viol = np.abs(g["S"] - S_ref) - (S_ABS[prec] + S_REL[prec] * np.abs(S_ref))
-    assert viol.max() <= 0, f"{tag} L1 S excess {viol.max():.3e}"
+    bad, m = sim_ref.check(g["S"], x, np.concatenate([x, xm]), prec)
+    assert not bad, f"{tag} L1 S: {bad} ({m})"
     tops_o, dx_o, st = step_memory(x, l, xm, lm, lw, S_inject=g["S"], num_tops=num_tops, **mining)
     np.testing.assert_array_equal(g["dbg"][1], st["posi_thr"], err_msg=f"{tag} posi_thr")
     np.testing.assert_array_equal(g["dbg"][2], st["nega_thr"], err_msg=f"{tag} nega_thr")

@@ -8,6 +8,7 @@ import pytest
 from npairloss_b200 import synth
 import grad_ref
 import memory_ref
+import sim_ref
 from grad_ref import U24
 from oracle import npair_oracle_np as onp
 
@@ -95,10 +96,10 @@ def test_every_weight_is_at_most_one(world, kind):
 
 # ----------------------------------------------------------------------------------------- the fp16x2 weight split, emulated
 def _split(w, k):
-    """fp16 hi + lo pieces of 2^k w (round to nearest, subnormals kept, as __floats2half2_rn), undone in fp64."""
+    """fp16 hi + lo pieces of 2^k w (round to nearest, subnormals kept, as __floats2half2_rn), undone in fp64: sim_ref's emulation of
+    the fp16x2 split at pre-scale 1."""
     v = (np.asarray(w, np.float32) * np.float32(2.0 ** k)).astype(np.float32)
-    hi = v.astype(np.float16)
-    lo = (v - hi.astype(np.float32)).astype(np.float16)
+    (hi, lo), _ = sim_ref.pieces(v, sim_ref.FP16X2, absmax=0.5)
     return (hi.astype(np.float64) + lo.astype(np.float64)) / 2.0 ** k
 
 
