@@ -245,6 +245,22 @@ int npair_forward_memory_async(npair_ctx* ctx, const float* d_feat, const float*
 int npair_backward_device_weight(npair_ctx* ctx, const float* d_loss_weight, float* d_feat_diff, void* stream);
 int npair_async_status(npair_ctx* ctx);
 
+/* ---- per-anchor loss weights and per-anchor losses (DESIGN 4.5; not part of the reference layer) ----
+ * The next forwards of this context read Q anchor weights in [0, 1] from d_anchor_weight and write the Q per-anchor losses
+ * (-log(A_i/T_i), unweighted) to d_row_loss, in stream order.  Either may be NULL (unweighted / not written); the pointers
+ * stay until set again.  A forward captured into a CUDA graph keeps the pointers it was captured with.
+ *   loss     tops[0] = -(1/Z) sum_i w_i log(A_i/T_i), Z = Q (N under global_scope); the weights are not renormalised.  Mining, A, T,
+ *            the per-row log values and tops 1-4 do not depend on the weights.
+ *   gradient every backward after the forward returns the gradient of that loss (its 1/2 and 1/world conventions unchanged):
+ *            sum_i w_i times anchor i's terms, through the row records, which carry the weights to the other ranks as well.
+ *   no weights, and w = 1 everywhere, give every result of the unweighted forward bit for bit.
+ *   Memory rows (npair_forward_memory) are no anchors and take no weight.
+ *   A weight outside [0, 1] or NaN is found on the device: the forward's tops are NaN, npair_forward (and the other blocking
+ *   forwards) return NPAIR_E_ARG, and the asynchronous ones keep the error for npair_async_status, which returns NPAIR_E_ARG after
+ *   NPAIR_E_EMPTY_LIST and NPAIR_E_POS_RANGE.  At world > 1 only the rank that read the bad weight reports it: the other ranks'
+ *   gradients of that step are unspecified.  The call itself makes no CUDA call (legal during a capture) and checks nothing but ctx. */
+int npair_set_anchor_io(npair_ctx* ctx, const float* d_anchor_weight, float* d_row_loss);
+
 /* The L2Normalize producer layer of the reference net (usage/def.prototxt:115-120; its source is not part of the reference tree):
  * y[r][:] = x[r][:] / ||x[r][:]||_2 (a zero row stays zero), and its backward dx = (dy - y (y . dy)) / ||x||.  Stand-alone entry
  * points for a host framework's own L2Normalize layer; npair_config.normalize_input = 1 runs the same kernels inside

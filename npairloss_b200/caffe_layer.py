@@ -49,17 +49,19 @@ def lib():
         L.npc_set_cpu_diff.argtypes = [vp, C.c_int]
         L.npc_set_cpu_diff.restype = fp
         L.npc_parse_only.argtypes = [C.c_char_p, fp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_char_p, C.c_int]
+        L.npc_parse_num_bottoms.argtypes = [C.c_char_p]
         L.npc_solver_run.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint, C.c_float, fp, C.c_int]
         L.npc_solver_last_error.restype = C.c_char_p
         _LIB = L
     return _LIB
 
 
-def layer_prototxt(mining: dict, num_tops: int = 5, loss_weights=True) -> str:
-    """A layer block in the format of usage/def.prototxt:121-151."""
+def layer_prototxt(mining: dict, num_tops: int = 5, loss_weights=True, anchor_weights=False) -> str:
+    """A layer block in the format of usage/def.prototxt:121-151; anchor_weights=True adds the third bottom of anchor weights."""
     tops = ["loss3/type_npair_mc", "loss3/type_npair_mc_retrieve_top1", "loss3/type_npair_mc_retrieve_top5",
             "loss3/type_npair_mc_retrieve_top10", "loss3/feature_asum"][:num_tops]
-    lines = ["layer {", '  bottom: "feat_norm"', '  bottom: "label"', '  name: "loss3/type_mb"', '  type: "NPairMultiClassLoss"']
+    lines = ["layer {", '  bottom: "feat_norm"', '  bottom: "label"'] + (['  bottom: "anchor_weight"'] if anchor_weights else [])
+    lines += ['  name: "loss3/type_mb"', '  type: "NPairMultiClassLoss"']
     lines += [f'  top: "{t}"' for t in tops]
     if loss_weights:
         lines += ["  loss_weight: 1"] * num_tops
@@ -81,7 +83,7 @@ def parse_only(prototxt: str):
         raise ValueError(err.value.decode())
     keys = ["margin_ident", "margin_diff", "identsn", "diffsn", "ap_region", "ap_method", "an_region", "an_method"]
     d = {k: (float(out[i]) if i < 4 else int(out[i])) for i, k in enumerate(keys)}
-    return dict(n_layers=n, num_tops=nt.value, n_loss_weights=nl.value, **d)
+    return dict(n_layers=n, num_tops=nt.value, n_loss_weights=nl.value, num_bottoms=int(lib().npc_parse_num_bottoms(prototxt.encode())), **d)
 
 
 class LayerError(RuntimeError):
@@ -89,7 +91,8 @@ class LayerError(RuntimeError):
 
 
 class Layer:
-    """NPairMultiClassLossLayer<float> set up from a prototxt with bottoms (num, channels, height, width) and (num)."""
+    """NPairMultiClassLossLayer<float> set up from a prototxt with bottoms (num, channels, height, width) and (num); a layer block
+    with a third bottom gets a (num) blob of anchor weights, bottom_data(2), initially all 1."""
 
     def __init__(self, prototxt: str, num: int, channels: int, height: int = 1, width: int = 1, world: int = 1, rank: int = 0,
                  nccl_id: bytes | None = None, sim_precision: int = -1):

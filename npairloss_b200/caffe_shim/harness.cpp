@@ -14,7 +14,7 @@ using namespace caffe;
 namespace {
 struct Net {
   shared_ptr<Layer<float> > layer;
-  Blob<float> feat, label;
+  Blob<float> feat, label, weight;      // weight: the optional third bottom (anchor weights), when the layer block names one
   std::vector<Blob<float>*> bottom, top;
   std::vector<Blob<float> > top_store;
   LayerParameter param;
@@ -37,7 +37,8 @@ void set_err(char* buf, int len, const std::string& m) {
 extern "C" {
 
 // Parses `prototxt` (a whole net or a single layer block), instantiates the first layer of type NPairMultiClassLoss
-// through the registry with bottoms shaped (num, channels, height, width) and (num), and runs Layer::SetUp.
+// through the registry with bottoms shaped (num, channels, height, width) and (num) -- plus a third (num) bottom of anchor weights,
+// all 1, when the layer block lists three bottoms -- and runs Layer::SetUp.
 // world/rank set the fork statics Caffe::NUM_GPU / Caffe::RANK; nccl_id (128 B) is required when world > 1.
 void* npc_net_create(const char* prototxt, int num, int channels, int height, int width, int world, int rank,
                      const void* nccl_id, int sim_precision, char* errbuf, int errlen) {
@@ -58,6 +59,12 @@ void* npc_net_create(const char* prototxt, int num, int channels, int height, in
     std::vector<int> ls(1, num);
     n->label.Reshape(ls);
     n->bottom.push_back(&n->feat); n->bottom.push_back(&n->label);
+    if (lp->bottom_size() > 2) {
+      n->weight.Reshape(ls);
+      float* w = n->weight.mutable_cpu_data();
+      for (int i = 0; i < num; ++i) w[i] = 1.f;
+      n->bottom.push_back(&n->weight);
+    }
     n->top_store.resize(lp->top_size());
     for (int t = 0; t < lp->top_size(); ++t) n->top.push_back(&n->top_store[t]);
     n->layer = LayerRegistry<float>::CreateLayer(n->param);
@@ -189,6 +196,15 @@ int npc_parse_only(const char* prototxt, float* out8, int* ntops, int* nloss_wei
       return static_cast<int>(layers.size());
     }
   set_err(errbuf, errlen, "no NPairMultiClassLoss layer");
+  return -1;
+}
+// prototxt reader only: the number of bottoms of the first NPairMultiClassLoss layer, or -1
+int npc_parse_num_bottoms(const char* prototxt) {
+  std::vector<LayerParameter> layers;
+  std::string perr;
+  if (!ReadLayersFromText(prototxt ? prototxt : "", &layers, &perr)) return -1;
+  for (size_t i = 0; i < layers.size(); ++i)
+    if (layers[i].type() == "NPairMultiClassLoss") return layers[i].bottom_size();
   return -1;
 }
 

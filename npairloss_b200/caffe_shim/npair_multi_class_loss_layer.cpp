@@ -17,6 +17,7 @@ NPairMultiClassLossLayer<Dtype>::~NPairMultiClassLossLayer() {
   if (f32_feat_) cudaFree(f32_feat_);
   if (f32_label_) cudaFree(f32_label_);
   if (f32_diff_) cudaFree(f32_diff_);
+  if (f32_weight_) cudaFree(f32_weight_);
 }
 
 template <typename Dtype>
@@ -25,6 +26,7 @@ void NPairMultiClassLossLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bot
   num_ = bottom[0]->num();
   dim_ = bottom[0]->channels() * bottom[0]->height() * bottom[0]->width();      // reference .cu:215
   CHECK_GE(bottom[1]->count(), num_) << "label blob holds fewer than num labels";
+  if (bottom.size() > 2) CHECK_EQ(bottom[2]->count(), num_) << "the anchor weight blob holds one weight per sample";
 
   npair_config cfg;
   npair_config_default(&cfg, num_, dim_);
@@ -54,6 +56,7 @@ void NPairMultiClassLossLayer<Dtype>::LayerSetUp(const vector<Blob<Dtype>*>& bot
     CUDA_CHECK(cudaMalloc(&f32_feat_, sizeof(float) * static_cast<size_t>(num_) * dim_));
     CUDA_CHECK(cudaMalloc(&f32_label_, sizeof(float) * num_));
     CUDA_CHECK(cudaMalloc(&f32_diff_, sizeof(float) * static_cast<size_t>(num_) * dim_));
+    if (bottom.size() > 2) CUDA_CHECK(cudaMalloc(&f32_weight_, sizeof(float) * num_));
   }
 }
 
@@ -61,6 +64,7 @@ template <typename Dtype>
 void NPairMultiClassLossLayer<Dtype>::Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   // batch size is frozen at setup upstream as well (reference .cpp:24-30, SURVEY Q13)
   CHECK_EQ(bottom[0]->num(), num_) << "NPairMultiClassLoss: batch size changed after LayerSetUp";
+  if (bottom.size() > 2) CHECK_EQ(bottom[2]->count(), num_) << "the anchor weight blob holds one weight per sample";
   vector<int> shape(0);                                                         // 0-axis scalars (reference .cpp:160-163)
   for (size_t i = 0; i < top.size(); ++i) top[i]->Reshape(shape);
 }
@@ -80,14 +84,20 @@ void NPairMultiClassLossLayer<Dtype>::Backward_cpu(const vector<Blob<Dtype>*>&, 
 template <typename Dtype>
 void NPairMultiClassLossLayer<Dtype>::Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
   float tops[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+  const bool weighted = bottom.size() > 2;
   int rc;
   if (sizeof(Dtype) == 4) {
+    if (weighted) npair_set_anchor_io(ctx_, reinterpret_cast<const float*>(bottom[2]->gpu_data()), nullptr);
     rc = npair_forward(ctx_, reinterpret_cast<const float*>(bottom[0]->gpu_data()), reinterpret_cast<const float*>(bottom[1]->gpu_data()), tops, nullptr);
   } else {
     rc = npair_util_f64_to_f32(reinterpret_cast<const double*>(bottom[0]->gpu_data()), f32_feat_, static_cast<size_t>(num_) * dim_, nullptr);
     if (rc == NPAIR_OK) rc = npair_util_f64_to_f32(reinterpret_cast<const double*>(bottom[1]->gpu_data()), f32_label_, num_, nullptr);
+    if (rc == NPAIR_OK && weighted) rc = npair_util_f64_to_f32(reinterpret_cast<const double*>(bottom[2]->gpu_data()), f32_weight_, num_, nullptr);
+    if (rc == NPAIR_OK && weighted) npair_set_anchor_io(ctx_, f32_weight_, nullptr);
     if (rc == NPAIR_OK) rc = npair_forward(ctx_, f32_feat_, f32_label_, tops, nullptr);
   }
+  // the weights are in the row records now (the backward reads those): the context's next forward is unweighted unless set again
+  if (weighted) npair_set_anchor_io(ctx_, nullptr, nullptr);
   CHECK_EQ(rc, NPAIR_OK) << "npair_forward: " << npair_last_error(ctx_);
   // [loss, retrieve top-1, top-5, top-10, feature asum]; the last top is always the asum (reference .cu:388-401)
   for (size_t i = 0; i < top.size(); ++i) top[i]->mutable_cpu_data()[0] = static_cast<Dtype>(tops[i]);

@@ -27,7 +27,11 @@ class NPairMultiClassLossLayer : public LossLayer<Dtype> {
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top);
 
   virtual inline const char* type() const { return "NPairMultiClassLoss"; }   // reference .hpp:30
-  virtual inline int ExactNumBottomBlobs() const { return 2; }                // features, labels (.hpp:31)
+  // features, labels (.hpp:31), and, as an extension, an optional third bottom of num anchor weights in [0, 1] (npair_set_anchor_io,
+  // DESIGN 4.5): the loss becomes -(1/num) sum_i w_i log(A_i / T_i) and the gradient that of it.  The weights get no gradient.
+  virtual inline int ExactNumBottomBlobs() const { return -1; }
+  virtual inline int MinBottomBlobs() const { return 2; }
+  virtual inline int MaxBottomBlobs() const { return 3; }
   virtual inline int ExactNumTopBlobs() const { return -1; }                  // .hpp:32
   virtual inline int MinTopBlobs() const { return 1; }                        // .hpp:33
   virtual inline int MaxTopBlobs() const { return 5; }                        // .hpp:34
@@ -48,7 +52,7 @@ class NPairMultiClassLossLayer : public LossLayer<Dtype> {
   int sim_precision_ = -1;
   // Dtype == double: the device path is fp32 (as is the reference's expf/logf/FLT_MAX arithmetic, SURVEY Q14);
   // features/labels/gradients are converted on the device through these staging buffers.
-  float *f32_feat_ = nullptr, *f32_label_ = nullptr, *f32_diff_ = nullptr;
+  float *f32_feat_ = nullptr, *f32_label_ = nullptr, *f32_diff_ = nullptr, *f32_weight_ = nullptr;
 };
 
 }  // namespace caffe

@@ -46,6 +46,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_create_memory", "npair_memory_workspace_bytes", "npair_forward_memory",
            # asynchronous step and graph capture (not part of the reference layer)
            "npair_forward_async", "npair_forward_memory_async", "npair_backward_device_weight", "npair_async_status",
+           # per-anchor loss weights and losses (not part of the reference layer)
+           "npair_set_anchor_io",
            # retrieval evaluation (not part of the reference layer)
            "npair_eval_workspace_bytes", "npair_eval_create", "npair_eval_destroy", "npair_eval_last_error", "npair_eval_rank",
            "npair_eval_best_positive", "npair_eval_count", "npair_eval_map_at_r", "npair_eval_map_at_r_bytes",
@@ -293,9 +295,25 @@ class Context:
                                                        torch.cuda.current_stream().cuda_stream))
 
     def async_status(self):
-        """npair_async_status: waits for the context's last call and raises NpairError (E_EMPTY_LIST or E_POS_RANGE) if an asynchronous
-        forward since the previous status call met a device error; clears it."""
+        """npair_async_status: waits for the context's last call and raises NpairError (E_EMPTY_LIST, E_POS_RANGE, or E_ARG for an
+        anchor weight outside [0, 1]) if an asynchronous forward since the previous status call met a device error; clears it."""
         self._check(lib().npair_async_status(self._h))
+
+    def set_anchor_io(self, weight=None, row_loss=None):
+        """npair_set_anchor_io (DESIGN 4.5): the next forwards read the Q anchor weights in [0, 1] from `weight` and write the Q
+        unweighted per-anchor losses -log(A_i / T_i) to `row_loss`, in stream order; each a contiguous CUDA float32 tensor of Q elements,
+        or None (unweighted / not written).  The library keeps the pointers until the next call: keep the tensors alive until then."""
+        ptrs = []
+        for t, what in ((weight, "weight"), (row_loss, "row_loss")):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if t.numel() != self.cfg.Q:
+                raise ValueError(f"{what} holds Q = {self.cfg.Q} floats, got {t.numel()}")
+            ptrs.append(self._f32(t, what))
+        f = lib().npair_set_anchor_io
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        self._check(f(self._h, ptrs[0], ptrs[1]))
 
     def forward_gathered(self, feat_total, label_total):
         import torch

@@ -374,6 +374,7 @@ struct npair_ctx : Plan {
   int s_block_row0 = -1;         // row-block similarity mode: first row of the block S holds (-1: none)
   float* part = nullptr;         // split-K partial products of the gradient GEMM
   RowArrays ra;                  // one buffer (row_arrays_at)
+  AnchorIO anchor_io{nullptr, nullptr};   // the caller's anchor weights and per-anchor loss output (npair_set_anchor_io, DESIGN 4.5)
   BlockScalars* bs = nullptr;
   float* partial = nullptr;
   unsigned long long* ghist = nullptr;   // [2][2048] 64-bit digit counts of the GLOBAL radix select
@@ -822,6 +823,11 @@ static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
   const int derr = c->tops_pinned->err;
   if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
   if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
+  if (derr & DERR_ANCHOR_WEIGHT) {
+    for (int t = 0; t < 5; ++t) tops_host[t] = __builtin_nanf("");
+    c->err = "an anchor weight (npair_set_anchor_io) is outside [0, 1] or NaN";
+    return NPAIR_E_ARG;
+  }
   for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned->tops[t] : 0.f;
   c->step.fwd_done = true;
   return NPAIR_OK;
@@ -1113,9 +1119,9 @@ static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cuda
         launch_local_select(sim, c->lsel_mask, c->cfg.identsn, c->cfg.diffsn, c->ra, c->bs, c->sms, lsel_warp, st);
       // one block: the row pass's last CTA computes the tops; several: one finaliser over all Q rows after the last block
       launch_lse_rows(sim, mp, c->ra, c->bs, c->cfg.num_tops, tops, c->world, c->wscope ? reinterpret_cast<TopSums*>(c->xch_src) : nullptr,
-                      weight_scale_log2(c->prec), c->tops_seq, c->n_blocks == 1, st);
+                      weight_scale_log2(c->prec), c->tops_seq, c->n_blocks == 1, c->anchor_io, st);
     }
-    if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, tops, c->tops_seq, st);
+    if (c->n_blocks > 1) launch_lse_finalize(Q, N, c->ra, c->bs, c->cfg.num_tops, tops, c->tops_seq, c->anchor_io.weight, st);
     if (c->wscope) {    // loss / retrieval / asum over the world's N rows, identical on every rank (the reference's are per rank, .cu:385)
       const float* all = nullptr;
       const int rc = xchg_small(c, c->xch_src, sizeof(TopSums) / sizeof(float), &all, st);
@@ -1400,6 +1406,13 @@ int npair_profile_read(npair_ctx* c, float* ms_out) {
   return NPAIR_OK;
 }
 
+// Host state only: no CUDA call, so it may be made during a capture; the forwards enqueued after it pass the pointers to the row pass
+int npair_set_anchor_io(npair_ctx* c, const float* d_anchor_weight, float* d_row_loss) {
+  if (!c) return NPAIR_E_ARG;
+  c->anchor_io = AnchorIO{d_anchor_weight, d_row_loss};
+  return NPAIR_OK;
+}
+
 int npair_async_status(npair_ctx* c) {
   if (!c) return NPAIR_E_ARG;
   if (c->world != 1) { c->err = "npair_async_status is world-1 only"; return NPAIR_E_ARG; }
@@ -1411,8 +1424,12 @@ int npair_async_status(npair_ctx* c) {
   if (!err) return NPAIR_OK;
   CUDA_TRY(c, cudaMemset(&c->aw->err, 0, sizeof(err)));
   if (err & DERR_EMPTY_LIST) { c->err = "an asynchronous forward indexed an empty same/diff list (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
-  c->err = "an asynchronous forward's identsn/diffsn selected a position outside the list (undefined behaviour in the reference, .cu:285-288)";
-  return NPAIR_E_POS_RANGE;
+  if (err & DERR_POS_RANGE) {
+    c->err = "an asynchronous forward's identsn/diffsn selected a position outside the list (undefined behaviour in the reference, .cu:285-288)";
+    return NPAIR_E_POS_RANGE;
+  }
+  c->err = "an asynchronous forward read an anchor weight (npair_set_anchor_io) outside [0, 1] or NaN";
+  return NPAIR_E_ARG;
 }
 
 __global__ void decode_ord_kernel(const uint32_t* __restrict__ in, float* __restrict__ out, int n) {

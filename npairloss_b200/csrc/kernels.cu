@@ -444,9 +444,10 @@ __device__ __forceinline__ void publish_tops(const TopSums* recs, int n, long lo
 
 // The Q rows' TopSums by one block, published (xout == NULL) or written to *xout (world scope: the rank's record for the exchange).
 // The summation order depends on the block size only (threads stride the rows, then warps in order), so a separate launch with the
-// same size gives the same bits.
+// same size gives the same bits.  anchor_w (or NULL): the loss sums the fp32 products w_i log(A_i / T_i) (0 at w_i = 0) in the same
+// order; at w = 1 they are the unweighted terms, bit for bit.
 __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* __restrict__ tops,
-                                                   TopSums* __restrict__ xout, unsigned int seq) {
+                                                   TopSums* __restrict__ xout, unsigned int seq, const float* __restrict__ anchor_w) {
   const int lane = threadIdx.x & 31;
   __shared__ double s_l[8];
   __shared__ int s_h[3][8];
@@ -461,6 +462,10 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
       const int r = r0 + u * blockDim.x;
       const bool ok = r < Q;
       lv[u] = ok ? __ldcg(&ra.logv[r]) : 0.f;
+      if (anchor_w) {                                           // a masked row adds 0, even where its log is -inf (A / T underflowed)
+        const float wv = ok ? __ldg(&anchor_w[r]) : 0.f;
+        lv[u] = wv == 0.f ? 0.f : lv[u] * wv;
+      }
       h0[u] = ok ? __ldcg(&ra.hits[r]) : 0; h1[u] = ok ? __ldcg(&ra.hits[Q + r]) : 0; h2[u] = ok ? __ldcg(&ra.hits[2 * Q + r]) : 0;
     }
 #pragma unroll
@@ -475,7 +480,8 @@ __device__ __forceinline__ void lse_finalize_block(int Q, RowArrays ra, BlockSca
   if (lane == 0) { s_l[w] = ls; s_h[0][w] = h[0]; s_h[1][w] = h[1]; s_h[2][w] = h[2]; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    TopSums s{0.0, {0, 0, 0}, bs->asum, bs->err};
+    // err through L2: the row pass's blocks set DERR_ANCHOR_WEIGHT during this launch, and this block's L1 may hold the line
+    TopSums s{0.0, {0, 0, 0}, bs->asum, __ldcg(&bs->err)};
     for (int k = 0; k < (blockDim.x >> 5); ++k) { s.loss_sum += s_l[k]; s.hits[0] += s_h[0][k]; s.hits[1] += s_h[1][k]; s.hits[2] += s_h[2][k]; }
     bs->ticket = 0;
     if (xout) *xout = s;
@@ -496,7 +502,8 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
                                                        float m2c_off /*log2(world) - k*/, float wscale /*2^k: weight_scale_log2*/,
                                                        TopSums* __restrict__ xout /*world scope: this rank's tops sums, else NULL*/,
                                                        int wpr /*warps per row: 1, 2, 4 or 8 (few rows per rank: keep the SMs full)*/,
-                                                       unsigned int seq /*written behind the tops: the host polls it*/, int finalize) {
+                                                       unsigned int seq /*written behind the tops: the host polls it*/, int finalize,
+                                                       const float* __restrict__ anchor_w /*[Q] or NULL*/, float* __restrict__ row_loss /*[Q] or NULL*/) {
   const int lane = threadIdx.x & 31;
   __shared__ float s_pA[8], s_pT[8];
   __shared__ int s_pc[8];
@@ -615,7 +622,9 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
   if (il < sim.rows && part == 0) {
     if (lane == 0) {
       ra.A[i] = A; ra.T[i] = T;                                 // T = A + B (.cu:380)
-      ra.logv[i] = (A == 0.f || T == 0.f) ? 0.f : logf(A / T);  // .cu:162-169
+      const float lv = (A == 0.f || T == 0.f) ? 0.f : logf(A / T);  // .cu:162-169
+      ra.logv[i] = lv;
+      if (row_loss) row_loss[i] = -lv;                          // the unweighted per-anchor loss (DESIGN 4.5)
       const int lim = N - 2;
       ra.hits[i] = (cs > 0 && c <= min(1, lim)) ? 1 : 0;
       ra.hits[Q + i] = (cs > 0 && c <= min(5, lim)) ? 1 : 0;
@@ -631,8 +640,16 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
       const float amin = A > 0.f ? A : T;
       const int j = amin > 0.f ? max(0, ilogbf(wscale) - 127 - ilogbf(amin)) : 0;
       const float fsc = ldexpf(wscale, -j);
-      ra.rowrec[i] = RowRecord::make(T == 0.f ? INFINITY : m2 + log2f(T) + m2c_off, thr_n, m2 - static_cast<float>(j), li, thr_p,
-                                     cA * fsc, invT * fsc);
+      // The anchor weight w (DESIGN 4.5) scales every term of the row: the factors by w, and the diff-label weight, which lives in the
+      // exponent offset m2c, by 2^-log2(w) (+inf at w = 0).  Exact at w = 1 and at w = 2^-i; without weights w = 1.
+      float m2c = T == 0.f ? INFINITY : m2 + log2f(T) + m2c_off;
+      float w = 1.f;
+      if (anchor_w) {
+        w = __ldg(&anchor_w[i]);
+        if (!(w >= 0.f && w <= 1.f)) atomicOr(&bs->err, DERR_ANCHOR_WEIGHT);
+        m2c = w > 0.f ? m2c - log2f(w) : INFINITY;
+      }
+      ra.rowrec[i] = RowRecord::make(m2c, thr_n, m2 - static_cast<float>(j), li, thr_p, cA * fsc * w, invT * fsc * w);
     }
   }
   if (!finalize) return;
@@ -644,10 +661,11 @@ __global__ void __launch_bounds__(256, NPAIR_LSE_MINB) lse_rows_kernel(const __g
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  lse_finalize_block(Q, ra, bs, num_tops, tops, xout, seq);
+  lse_finalize_block(Q, ra, bs, num_tops, tops, xout, seq, anchor_w);
 }
-__global__ void lse_finalize_kernel(int Q, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* __restrict__ tops, unsigned int seq) {
-  lse_finalize_block(Q, ra, bs, num_tops, tops, nullptr, seq);
+__global__ void lse_finalize_kernel(int Q, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* __restrict__ tops, unsigned int seq,
+                                    const float* __restrict__ anchor_w) {
+  lse_finalize_block(Q, ra, bs, num_tops, tops, nullptr, seq, anchor_w);
 }
 // Launch shape of the row pass, from the rank's row count Q (never from a row block's: the warps per row set the summation order
 // of A and T, the block size that of the finaliser).
@@ -671,20 +689,21 @@ static void lse_shape(int Q, int N, int* wpr_out, int* threads_out) {
   *threads_out = wpb * 32;
 }
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
-                     int wlog2, unsigned int seq, bool finalize, cudaStream_t st) {
+                     int wlog2, unsigned int seq, bool finalize, AnchorIO aio, cudaStream_t st) {
   int wpr = 1, threads = 256;
   lse_shape(sim.Q, sim.N, &wpr, &threads);
   const int rows_per_blk = threads / 32 / wpr;
   const int grid = (sim.rows + rows_per_blk - 1) / rows_per_blk;
   const float log2_world = xout ? 0.f : log2f(static_cast<float>(world));
   lse_rows_kernel<<<grid, threads, 0, st>>>(sim, mp, ra, bs, num_tops, tops_dev, log2_world - static_cast<float>(wlog2), ldexpf(1.f, wlog2), xout,
-                                            wpr, seq, finalize ? 1 : 0);
+                                            wpr, seq, finalize ? 1 : 0, aio.weight, aio.row_loss);
   count_launch();
 }
-void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st) {
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, const float* anchor_w,
+                         cudaStream_t st) {
   int wpr = 1, threads = 256;
   lse_shape(Q, N, &wpr, &threads);
-  lse_finalize_kernel<<<1, threads, 0, st>>>(Q, ra, bs, num_tops, tops_dev, seq);
+  lse_finalize_kernel<<<1, threads, 0, st>>>(Q, ra, bs, num_tops, tops_dev, seq, anchor_w);
   count_launch();
 }
 
@@ -886,7 +905,7 @@ void launch_tops_world(const float* xall, int xstride, int world, long long N, i
 
 __global__ void async_tops_kernel(AsyncWords* __restrict__ aw, int num_tops, float* __restrict__ d_tops) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const int err = aw->tops.err & (DERR_EMPTY_LIST | DERR_POS_RANGE);
+  const int err = aw->tops.err & (DERR_EMPTY_LIST | DERR_POS_RANGE | DERR_ANCHOR_WEIGHT);
   for (int t = 0; t < 5; ++t) d_tops[t] = err ? __int_as_float(0x7fc00000) : (t < num_tops ? aw->tops.tops[t] : 0.f);
   aw->err |= static_cast<unsigned int>(err);
 }

@@ -18,6 +18,8 @@ enum { DERR_EMPTY_LIST = 1, DERR_POS_RANGE = 2 };
 enum { DERR_GATHER_SLOT = 4 };
 // k-means: a point's assignment sweep found no column with a score above -inf (a NaN or infinite input)
 enum { DERR_KMEANS_NO_ARGMAX = 8 };
+// the layer: an anchor weight (npair_set_anchor_io) outside [0, 1] or NaN
+enum { DERR_ANCHOR_WEIGHT = 16 };
 
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -101,6 +103,8 @@ __device__ __forceinline__ float an_thr(float t, int m) {     // diff-label rule
 //   cA     same-label weight factor 2^(k-j) (1/T - 1/A);  cT  diff-label weight factor 2^(k-j) / T
 // so every gradient weight built from records, 2^(s*log2(e) - m2) times a factor, comes out scaled by 2^k, k = weight_scale_log2(format),
 // and the gradient GEMM's alpha carries 2^-k.  j is 0 except on rows whose 2^k / A or 2^k / T could pass 2^127 (lse_rows_kernel).
+// A weighted anchor (npair_set_anchor_io, DESIGN 4.5) carries its weight w in [0, 1] in the record: cA w, cT w, and m2c - log2(w)
+// (+inf at w = 0), so every term of the row, its own and its transposed ones, comes out scaled by w.  At w = 1 these are the bits above.
 struct RowRecord {
   float4 lo, hi;   // {m2c, thr_n, m2, label}, {thr_p, cA, cT, 0}
   __host__ __device__ static RowRecord make(float m2c, float thr_n, float m2, float label, float thr_p, float cA, float cT) {
@@ -300,10 +304,13 @@ void launch_thresholds_world(const float* xall, int xstride, int world, long lon
 void launch_tops_world(const float* xall, int xstride, int world, long long N, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
 // Row pass over the rows of sim.  finalize: the last block also reduces the Q rows' results into the tops; otherwise
 // launch_lse_finalize does, once.  xout: NULL, or (world scope) receives the rank's TopSums instead of the tops.  wlog2: the records'
-// weight scale, weight_scale_log2 of the operand format
+// weight scale, weight_scale_log2 of the operand format.  AnchorIO: the rank's Q anchor weights and per-anchor loss output (DESIGN 4.5),
+// each NULL when unused
+struct AnchorIO { const float* weight; float* row_loss; };
 void launch_lse_rows(SimRows sim, MiningParams mp, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, int world, TopSums* xout,
-                     int wlog2, unsigned int seq, bool finalize, cudaStream_t st);
-void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, cudaStream_t st);
+                     int wlog2, unsigned int seq, bool finalize, AnchorIO aio, cudaStream_t st);
+void launch_lse_finalize(int Q, int N, RowArrays ra, BlockScalars* bs, int num_tops, TopsBlock* tops_dev, unsigned int seq, const float* anchor_w,
+                         cudaStream_t st);
 // mode: BW_SPLIT (world > 1, reduce-scatter form: H and HT), BW_SYM (world == 1), BW_ROWSCAL (rs_total = one record per column: at
 // world > 1 the world's N row records, all-gathered; in a cross-batch memory step at world 1, the Q row records followed by the m
 // memory rows' RowRecord::memory records, whose transposed terms are 0)
@@ -312,7 +319,7 @@ enum { BW_SPLIT = 0, BW_SYM = 1, BW_ROWSCAL = 2 };
 void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_total, MiningParams mp, RowArrays ra, int prec,
                           uint16_t* H, long long ldH /*Np*/, uint16_t* HT, long long ldHT /*Qp*/, cudaStream_t st);
 // The asynchronous forward's finish: d_tops[0, 5) = what the host would read of aw->tops (0 past num_tops), or NaN with the error bits
-// added to aw->err when a DERR_EMPTY_LIST / DERR_POS_RANGE bit is set
+// added to aw->err when a DERR_EMPTY_LIST / DERR_POS_RANGE / DERR_ANCHOR_WEIGHT bit is set
 void launch_async_tops(AsyncWords* aw, int num_tops, float* d_tops, cudaStream_t st);
 // aw->grad_scale = (0.5f * ldexpf(*d_lw / Q, -wlog2)) * bs->x_inv_scale: the host's alpha of the gradient GEMMs times their device scale,
 // in the same fp32 operations

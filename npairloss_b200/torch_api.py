@@ -27,6 +27,14 @@ tensor (npair_forward_async) and the loss is its element 0 on the device; the ba
 (npair_backward_device_weight) instead of calling .item().  Same values, bit for bit, as blocking=True.  A whole training step through it
 can be captured with torch.cuda.graph (DESIGN 4.4); a device error (the cases the blocking forward raises for) gives NaN tops and is
 reported by async_status().  With memory_rows > 0 it runs eagerly only: the ring's head is Python state that a graph would freeze.
+
+ANCHOR WEIGHTS.  loss_fn(x, labels, anchor_weight=w) weights anchor i's term by w_i in [0, 1] (npair_set_anchor_io, DESIGN 4.5): the loss
+is -(1/Z) sum_i w_i log(A_i / T_i), Z = Q (Q * world under global_scope), not renormalised, and the backward is its gradient.  A row with
+w_i = 0 still serves the other anchors as a positive or negative, and still gets gradient through their terms.  row_losses=True adds a
+third output, the unweighted per-anchor losses -log(A_i / T_i) (not differentiable).  When w requires grad, its gradient is
+grad_loss * row_loss_i / Z (the analytic one, whatever true_gradient says).  Works with blocking=False and graph capture (w is then a
+static input like the embeddings), memory_rows, normalize_input and world > 1.  A weight outside [0, 1] or NaN makes the blocking
+forward raise capi.NpairError (E_ARG) and the asynchronous one give NaN tops, reported by async_status().
 """
 from __future__ import annotations
 
@@ -55,28 +63,43 @@ def _fp32_labels(label):
 
 class _NPairFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, feat, label, owner):
+    def forward(ctx, feat, label, weight, owner, want_rows):
         layer = owner._context(feat)
-        if owner._blocking:
-            if owner._mem_cap:
-                tops = owner._forward_memory(layer, feat, label)
+        rl = None
+        if want_rows or ctx.needs_input_grad[2]:              # the weights' gradient is made of the per-anchor losses
+            rl = torch.empty(feat.shape[0], dtype=torch.float32, device=feat.device)
+        io = weight is not None or rl is not None
+        if io:
+            layer.set_anchor_io(weight, rl)
+        try:
+            if owner._blocking:
+                if owner._mem_cap:
+                    tops = owner._forward_memory(layer, feat, label)
+                else:
+                    tops = layer.forward(feat, label)         # blocks until the five scalars are on the host (as the reference)
+                t = torch.tensor(tops, dtype=torch.float32, device=feat.device)
             else:
-                tops = layer.forward(feat, label)             # blocks until the five scalars are on the host (as the reference)
-            t = torch.tensor(tops, dtype=torch.float32, device=feat.device)
-        else:
-            t = torch.empty(5, dtype=torch.float32, device=feat.device)   # under capture: from the graph's pool
-            if owner._mem_cap:
-                owner._forward_memory(layer, feat, label, t)
-            else:
-                layer.forward_async(feat, label, t)
+                t = torch.empty(5, dtype=torch.float32, device=feat.device)   # under capture: from the graph's pool
+                if owner._mem_cap:
+                    owner._forward_memory(layer, feat, label, t)
+                else:
+                    layer.forward_async(feat, label, t)
+        finally:
+            if io:                                            # the forward is enqueued: the next one through this context is unweighted
+                layer.set_anchor_io(None, None)
         owner._generation += 1
         ctx.owner, ctx.layer, ctx.generation = owner, layer, owner._generation
         ctx.save_for_backward(feat, label)                    # the C ABI wants both unchanged until the backward is enqueued
+        ctx.row_loss = rl
+        ctx.norm = feat.shape[0] * (owner._world if owner._config.get("global_scope") else 1)   # Z: Q, or N in world scope
+        if want_rows:
+            ctx.mark_non_differentiable(t, rl)
+            return t[0].clone(), t, rl
         ctx.mark_non_differentiable(t)
         return t[0].clone(), t
 
     @staticmethod
-    def backward(ctx, grad_loss, _grad_tops):
+    def backward(ctx, grad_loss, _grad_tops, *_grad_rows):
         if ctx.generation != ctx.owner._generation or ctx.layer is not ctx.owner._ctx:
             raise RuntimeError("NPairLoss: another forward ran through this module after the one being differentiated; the library "
                                "context holds the newer batch.  Use one NPairLoss module per outstanding graph.")
@@ -89,7 +112,10 @@ class _NPairFunction(torch.autograd.Function):
             ctx.layer.backward_device_weight(grad_loss.detach().to(torch.float32).contiguous().reshape(1), diff)
         if ctx.owner._true_gradient:
             diff.mul_(2.0)
-        return diff, None, None
+        grad_w = None
+        if ctx.needs_input_grad[2]:                           # d loss / d w_i = row_loss_i / Z
+            grad_w = grad_loss.to(torch.float32) * ctx.row_loss / ctx.norm
+        return diff, None, grad_w, None, None
 
 
 class NPairLoss(torch.nn.Module):
@@ -190,16 +216,25 @@ class NPairLoss(torch.nn.Module):
                 old.close()
         return self._ctx
 
-    def forward(self, feat, label):
+    def forward(self, feat, label, anchor_weight=None, row_losses=False):
+        """(loss, tops), or (loss, tops, row_loss) with row_losses=True; anchor_weight: None or Q fp32 weights in [0, 1] on feat's
+        device (ANCHOR WEIGHTS in the module docstring)."""
         if feat.dtype != torch.float32:
             raise TypeError("NPairLoss computes in fp32 like the reference (Dtype=float); cast the embeddings")
+        if anchor_weight is not None:
+            if not isinstance(anchor_weight, torch.Tensor) or anchor_weight.dtype != torch.float32:
+                raise TypeError("anchor_weight must be a float32 tensor (weights in [0, 1], one per row of the batch)")
+            if anchor_weight.dim() != 1 or anchor_weight.shape[0] != feat.shape[0]:
+                raise ValueError(f"anchor_weight must have shape [{feat.shape[0]}] (one weight per row), got {list(anchor_weight.shape)}")
+            if anchor_weight.device != feat.device:
+                raise ValueError("anchor_weight must be on the embeddings' device")
+            anchor_weight = anchor_weight.contiguous()
         if not self._blocking and self._mem_cap and feat.is_cuda and torch.cuda.is_current_stream_capturing():
             raise RuntimeError("NPairLoss(memory_rows > 0, blocking=False) cannot be captured into a CUDA graph: the memory ring's head "
                                "and count are Python state that the graph would freeze")
         feat2 = feat.reshape(feat.shape[0], -1).contiguous()
         label = _fp32_labels(label).contiguous()               # labels are stored as Dtype in the reference (bottom[1])
-        loss, tops = _NPairFunction.apply(feat2, label, self)
-        return loss, tops
+        return _NPairFunction.apply(feat2, label, anchor_weight, self, bool(row_losses))
 
 
 def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), precision=capi.PREC_FP32_FP16X2, self_offset=None):
