@@ -264,7 +264,12 @@ int npair_set_anchor_io(npair_ctx* ctx, const float* d_anchor_weight, float* d_r
 /* The L2Normalize producer layer of the reference net (usage/def.prototxt:115-120; its source is not part of the reference tree):
  * y[r][:] = x[r][:] / ||x[r][:]||_2 (a zero row stays zero), and its backward dx = (dy - y (y . dy)) / ||x||.  Stand-alone entry
  * points for a host framework's own L2Normalize layer; npair_config.normalize_input = 1 runs the same kernels inside
- * npair_forward / npair_backward.  d_inv_norm: rows floats (1 / ||x||, 0 for a zero row). */
+ * npair_forward / npair_backward.  d_inv_norm: rows floats (1 / ||x||, 0 for a zero row, +inf where 1 / ||x|| > FLT_MAX).
+ * Every finite row is normalised, at both ends of the fp32 range: a row whose sum of squares overflows or falls below 2^-64 is
+ * redone on x 2^-e (e the exponent of max |x|), which is exact, so y is the y of the scaled row.  A row with a NaN or +-inf element
+ * gives a NaN row and a NaN 1 / ||x||, and a NaN gradient; the other rows do not change.  Where 1 / ||x|| is +inf the gradient is
+ * +-inf, or exactly 0 where dy - y (y . dy) is 0.  The backward of a row whose d_inv_norm is NaN is NaN, whatever its y.
+ * tests/l2norm_ref.py states the componentwise error bounds. */
 int npair_l2normalize_forward(const float* d_x, int rows, int dim, float* d_y, float* d_inv_norm, void* stream);
 int npair_l2normalize_backward(const float* d_y, const float* d_inv_norm, const float* d_dy, int rows, int dim, float* d_dx, void* stream);
 

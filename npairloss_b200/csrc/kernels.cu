@@ -843,7 +843,35 @@ void launch_build_weights(SimRows sim, int world, int mode, const RowRecord* rs_
 // L2Normalize producer (usage/def.prototxt:115-120; the layer's source is not in the reference tree, so the semantics are
 // stated here): y = x / ||x||_2 per sample, a zero row stays zero; backward dx = (dy - y (y . dy)) / ||x||.
 // One warp per row, 16-byte loads, fixed summation order (lane-strided partial sums, then the shuffle tree).
+// Range: the fast path is one pass over the row with no scaling.  When its sum of squares ss is not in [L2_SS_MIN, FLT_MAX] (the
+// squares overflowed, or so many of them were subnormal that their rounding could show), the row is redone on x 2^-e, e the
+// exponent of max|x| clamped as in pre_scale: the scaling is exact, so y is the fast path's y of the scaled row, and 1/||x|| is that
+// row's 1/||x|| times 2^-e (+inf above FLT_MAX).  A row the fast path accepts gives the bits it gave before the rescue existed.
+// A row with a NaN or +-inf element gives a NaN row and a NaN 1/||x||; an all-zero row gives zeros.
 // --------------------------------------------------------------------------------------------
+// ss >= 2^-64: the fast path rounds at most D partial sums in the subnormal range, 2^-150 each, i.e. at most D 2^-86 of ss
+constexpr float L2_SS_MIN = 0x1p-64f;
+// the sum of the squares of x * sc in the order every pass uses; sc = 1 (SCALED false) on the fast path
+template <bool SCALED>
+__device__ __forceinline__ float l2norm_row_ss(const float* xr, int dim, int lane, bool vec, bool quad, float sc) {
+  auto f = [sc](float v) { return SCALED ? v * sc : v; };
+  float ss = 0.f;
+  if (vec) for (int d = lane * 4; d < dim; d += 128) {
+    const float4 v = *reinterpret_cast<const float4*>(xr + d);
+    const float a = f(v.x), b = f(v.y), c = f(v.z), e = f(v.w);
+    ss = fmaf(a, a, ss); ss = fmaf(b, b, ss); ss = fmaf(c, c, ss); ss = fmaf(e, e, ss);
+  } else if (quad) for (int d = lane * 4; d < dim; d += 128) for (int e = 0; e < 4; ++e) { const float a = f(xr[d + e]); ss = fmaf(a, a, ss); }
+  else for (int d = lane; d < dim; d += 32) { const float a = f(xr[d]); ss = fmaf(a, a, ss); }
+  return warp_sum(ss);
+}
+template <bool SCALED>
+__device__ __forceinline__ void l2norm_row_store(const float* xr, float* yr, int dim, int lane, bool vec, float sc, float nrm) {
+  auto f = [sc](float v) { return SCALED ? v * sc : v; };
+  if (vec) for (int d = lane * 4; d < dim; d += 128) {
+    const float4 v = *reinterpret_cast<const float4*>(xr + d);
+    *reinterpret_cast<float4*>(yr + d) = make_float4(f(v.x) / nrm, f(v.y) / nrm, f(v.z) / nrm, f(v.w) / nrm);
+  } else for (int d = lane; d < dim; d += 32) yr[d] = f(xr[d]) / nrm;
+}
 __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const float* __restrict__ x, int rows, int dim, float* __restrict__ y,
                                                          float* __restrict__ inv_norm) {
   const int lane = threadIdx.x & 31;
@@ -855,19 +883,33 @@ __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const float* __restrict
   // order, so y does not depend on where x starts); else lane-strided features
   const bool quad = (dim & 3) == 0;
   const bool vec = quad && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
-  float ss = 0.f;
-  if (vec) for (int d = lane * 4; d < dim; d += 128) { const float4 v = *reinterpret_cast<const float4*>(xr + d); ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss); }
-  else if (quad) for (int d = lane * 4; d < dim; d += 128) for (int e = 0; e < 4; ++e) ss = fmaf(xr[d + e], xr[d + e], ss);
-  else for (int d = lane; d < dim; d += 32) ss = fmaf(xr[d], xr[d], ss);
-  ss = warp_sum(ss);
-  const float nrm = sqrtf(ss);
-  const float inv = nrm > 0.f ? 1.f / nrm : 0.f;
+  const float ss = l2norm_row_ss<false>(xr, dim, lane, vec, quad, 1.f);   // the same value in every lane: the branch is warp-uniform
+  float inv;
+  if (ss >= L2_SS_MIN && ss <= FLT_MAX) {
+    const float nrm = sqrtf(ss);
+    inv = 1.f / nrm;
+    l2norm_row_store<false>(xr, yr, dim, lane, vec, 1.f, nrm);
+  } else {
+    float mx = 0.f;                                                     // fmaxf skips a NaN; ss has caught it
+    for (int d = lane; d < dim; d += 32) mx = fmaxf(mx, fabsf(xr[d]));
+    mx = warp_max(mx);
+    const bool nonfinite = ss != ss || !(mx <= FLT_MAX);               // a NaN or +-inf element
+    if (nonfinite || mx == 0.f) {                                       // ... or a zero row
+      const float fill = nonfinite ? __int_as_float(0x7fc00000) : 0.f;
+      inv = fill;
+      for (int d = lane; d < dim; d += 32) yr[d] = fill;
+    } else {
+      const PreScale ps = pre_scale(mx);
+      const float nrm = sqrtf(l2norm_row_ss<true>(xr, dim, lane, vec, quad, ps.scale));
+      inv = (1.f / nrm) * ps.scale;
+      l2norm_row_store<true>(xr, yr, dim, lane, vec, ps.scale, nrm);
+    }
+  }
   if (lane == 0 && inv_norm) inv_norm[r] = inv;
-  if (vec) for (int d = lane * 4; d < dim; d += 128) {
-    const float4 v = *reinterpret_cast<const float4*>(xr + d);
-    *reinterpret_cast<float4*>(yr + d) = nrm > 0.f ? make_float4(v.x / nrm, v.y / nrm, v.z / nrm, v.w / nrm) : make_float4(0.f, 0.f, 0.f, 0.f);
-  } else for (int d = lane; d < dim; d += 32) yr[d] = nrm > 0.f ? xr[d] / nrm : 0.f;
 }
+// t * inv, except that t = 0 stays 0 where inv = +inf (a row with 1/||x|| above FLT_MAX): such a row's gradient is +-inf or 0.  A
+// finite inv gives the bits of t * inv either way, and a NaN inv a NaN.
+__device__ __forceinline__ float l2norm_dx(float t, float inv) { return t == 0.f && inv == INFINITY ? t : t * inv; }
 __global__ void __launch_bounds__(256) l2norm_bwd_kernel(const float* __restrict__ y, const float* __restrict__ inv_norm, const float* __restrict__ dy,
                                                          int rows, int dim, float* __restrict__ dx) {
   const int lane = threadIdx.x & 31;
@@ -889,8 +931,9 @@ __global__ void __launch_bounds__(256) l2norm_bwd_kernel(const float* __restrict
   const float inv = inv_norm[r];
   if (vec) for (int d = lane * 4; d < dim; d += 128) {
     const float4 a = *reinterpret_cast<const float4*>(yr + d), g = *reinterpret_cast<const float4*>(gr + d);
-    *reinterpret_cast<float4*>(dr + d) = make_float4((g.x - a.x * dot) * inv, (g.y - a.y * dot) * inv, (g.z - a.z * dot) * inv, (g.w - a.w * dot) * inv);
-  } else for (int d = lane; d < dim; d += 32) dr[d] = (gr[d] - yr[d] * dot) * inv;
+    *reinterpret_cast<float4*>(dr + d) = make_float4(l2norm_dx(g.x - a.x * dot, inv), l2norm_dx(g.y - a.y * dot, inv),
+                                                     l2norm_dx(g.z - a.z * dot, inv), l2norm_dx(g.w - a.w * dot, inv));
+  } else for (int d = lane; d < dim; d += 32) dr[d] = l2norm_dx(gr[d] - yr[d] * dot, inv);
 }
 // world scope: tops from the ranks' sums, normalised by the world's N (identical on every rank)
 __global__ void tops_world_kernel(const TopSums* __restrict__ xall, int xstride, int world, long long N, int num_tops, TopsBlock* __restrict__ tops,

@@ -507,9 +507,21 @@ void npo_l2normalize_forward(const float* x, int rows, int dim, float* y, float*
     const float* xr = x + (size_t)r * dim;
     double ss = 0.0;
     for (int d = 0; d < dim; ++d) ss += (double)xr[d] * (double)xr[d];
-    const float nrm = sqrtf((float)ss);
-    if (inv_norm) inv_norm[r] = nrm > 0.f ? 1.f / nrm : 0.f;
-    for (int d = 0; d < dim; ++d) y[(size_t)r * dim + d] = nrm > 0.f ? xr[d] / nrm : 0.f;
+    float* yr = y + (size_t)r * dim;
+    const float ssf = (float)ss;
+    if (ssf >= FLT_MIN && ssf <= FLT_MAX) {          // ordinary rows: fp32 norm of the double sum
+      const float nrm = sqrtf(ssf);
+      if (inv_norm) inv_norm[r] = 1.f / nrm;
+      for (int d = 0; d < dim; ++d) yr[d] = xr[d] / nrm;
+    } else if (ss > 0.0 && ss <= DBL_MAX) {          // the sum left fp32's normal range but not double's: the norm in double
+      const double nrm = sqrt(ss);
+      if (inv_norm) inv_norm[r] = (float)(1.0 / nrm);
+      for (int d = 0; d < dim; ++d) yr[d] = (float)((double)xr[d] / nrm);
+    } else {                                          // a zero row stays zero; a NaN or +-inf element makes the row NaN
+      const float fill = ss == 0.0 ? 0.f : NAN;
+      if (inv_norm) inv_norm[r] = fill;
+      for (int d = 0; d < dim; ++d) yr[d] = fill;
+    }
   }
 }
 
@@ -521,7 +533,10 @@ void npo_l2normalize_backward(const float* y, const float* inv_norm, const float
     double dot = 0.0;
     for (int d = 0; d < dim; ++d) dot += (double)yr[d] * (double)gr[d];
     const float dotf = (float)dot, inv = inv_norm[r];
-    for (int d = 0; d < dim; ++d) dx[(size_t)r * dim + d] = (gr[d] - yr[d] * dotf) * inv;
+    for (int d = 0; d < dim; ++d) {                   // t = 0 stays 0 where inv = +inf (1/||x|| above FLT_MAX)
+      const float t = gr[d] - yr[d] * dotf;
+      dx[(size_t)r * dim + d] = t == 0.f && inv == INFINITY ? t : t * inv;
+    }
   }
 }
 

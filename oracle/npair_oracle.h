@@ -103,7 +103,9 @@ long long npo_pos(float sn, size_t size);
  * (a layer of the private Caffe fork), so this is the textbook definition, stated rather than restated:
  *   forward : y[r][:] = x[r][:] / sqrt(sum_d x[r][d]^2)      (a zero row stays zero)
  *   backward: dx[r][:] = (dy[r][:] - y[r][:] * (y[r][:] . dy[r][:])) / ||x[r]||
- * inv_norm: rows floats, 1/||x|| (0 for a zero row).  Sums in double, rounded to fp32 on store. */
+ * inv_norm: rows floats, 1/||x|| (0 for a zero row, +inf above FLT_MAX).  Sums in double; the norm is sqrtf of the sum rounded
+ * to fp32 when that is a normal float, else taken in double.  A row with a NaN or +-inf element gives a NaN row and a NaN inv_norm.
+ * The backward keeps a component 0 where dy - y (y . dy) is 0 and inv_norm is +inf; a NaN inv_norm gives a NaN row. */
 void npo_l2normalize_forward(const float* x, int rows, int dim, float* y, float* inv_norm);
 void npo_l2normalize_backward(const float* y, const float* inv_norm, const float* dy, int rows, int dim, float* dx);
 
