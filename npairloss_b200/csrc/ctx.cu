@@ -262,37 +262,61 @@ static int select_mask(const npair_config& c, int region) {
          (c.an_region == region && is_rel(c.an_method) && !sn_is_max(c.diffsn) ? 2 : 0);
 }
 
-// What a context decides from its configuration and two device facts (ctx_buffers sizes its device buffers from these decisions)
+// What a context decides from its configuration and two device facts, fixed at its capacity: its modes and buffers (ctx_buffers)
 struct Plan {
-  int N, nsplit, bk_grad;
+  int nsplit, bk_grad;
   long long Dp, Np, Qp, ldS;     // padded feature / all-rows / local-rows extents of the operand pieces, row stride of S
   SimLayout sim;                 // layout of the similarity GEMM's operands (PREC_BF16: Xs, whose one piece is that layout)
   int bwd_mode;                  // NPAIR_BWDMODE_*
   bool fused_grad;               // the gradient weights are produced inside the gradient GEMM: no H in HBM
   bool cat;                      // the similarity GEMM reads its own operands XcatA / XcatB (SimLayout), not Xs
-  unsigned int gcand_cap;        // entries per side of the GLOBAL radix select's candidate lists
   int grad_chunk_kb;             // accumulation chunk of the gradient GEMM in 32-column K blocks (grad_fused.cuh); 0 = unchunked
-  int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
-  SplitK grad_split;             // and its split-K
-  int split_cap;                 // split_k_cap of that K: a memory context's partial buffer holds this many slices, enough for any m <= M
-  int n_sym_tiles;
+  int split_cap;                 // split_k_cap of the gradient GEMM at the capacity: a memory context's partial buffer, enough for any m <= M
   int s_rows;                    // rows of the S buffer: all Q (S materialised), or one block in row-block similarity mode
   int n_blocks;                  // blocks of s_rows rows that the row pass and the fused gradient walk; 1: S materialised
-  int sweep_epi;                 // the forward's similarity sweep: statistics, + symmetric tiles, + stores to S if there is one block
   bool wscope;                   // world-scope mode: global_scope at world > 1
   int lsel_mask, gsel_mask;      // radix selects (select_mask) of the LOCAL / GLOBAL region
   bool want_p2p_feat, want_p2p_rec;   // world > 1: features / row records travel by peer-memory stores rather than NCCL
   XchgLayout xl;
 };
+// What depends on a call's database size N: N = Q * world, or a memory call's Q + m (set_call_rows)
+struct CallPlan {
+  int N;
+  unsigned int gcand_cap;        // entries per side of the GLOBAL radix select's candidate lists
+  int grad_kblocks;              // K blocks of the Q x D gradient GEMM (G . X_total)
+  SplitK grad_split;             // and its split-K
+  int n_sym_tiles;
+  int sweep_epi;                 // the forward's similarity sweep: statistics, + symmetric tiles, + stores to S if there is one block
+};
 
-// mem_rows: the cross-batch memory rows m of a world-1 step (DESIGN 4.3), database columns Q + m; a memory context's buffers are
-// those of its capacity M, and each call re-plans what depends on the call's own N (set_call_rows)
-static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric, int mem_rows = 0) {
+// The plan of a call over m cross-batch memory rows (DESIGN 4.3), database columns Q * world + m
+static CallPlan call_plan(const npair_config& cfg, const Plan& p, int sms, int m) {
+  CallPlan cp{};
+  const long long Q = cfg.Q, N = Q * cfg.world + m;
+  const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
+  cp.N = static_cast<int>(N);
+  // GLOBAL radix select: candidate lists of the chosen first-digit bucket (1/8 of the block, at most 32 M entries per side; a
+  // bigger bucket -- heavily tied data -- takes the three-sweep path)
+  if (p.gsel_mask) {
+    const long long cap = Q * N / 8 + 4096;
+    cp.gcand_cap = static_cast<unsigned int>(cap < (32ll << 20) ? cap : (32ll << 20));
+  }
+  // the fused kernel walks K in 32-column blocks and keeps >= 8 of them (256 columns) per split; the split GEMM keeps >= 4
+  cp.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
+  const int tiles = tile_sched(cfg.Q, cfg.D, cp.grad_kblocks).num_tiles();
+  cp.grad_split = tc ? split_k(cp.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, cp.grad_kblocks};
+  // memory rows are no anchors: S is not symmetric, every tile is computed
+  if (cfg.world == 1 && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES) && m == 0) cp.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, cp.N));
+  cp.sweep_epi = EPI_STATS | (cp.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
+  return cp;
+}
+
+// mem_cap: the most cross-batch memory rows M of a world-1 context's calls (DESIGN 4.3); its buffers are those of N = Q + M
+static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric, int mem_cap = 0) {
   Plan p{};
   const int prec = cfg.sim_precision, W = cfg.world;
-  const long long Q = cfg.Q, D = cfg.D, N = Q * W + mem_rows;
+  const long long Q = cfg.Q, D = cfg.D, N = Q * W + mem_cap;
   const bool tc = cfg.gemm_backend == NPAIR_GEMM_TCGEN05, multi = W > 1;
-  p.N = static_cast<int>(N);
   p.nsplit = SPLIT_FORMATS[prec].pieces; p.bk_grad = bk_of(prec, EPI_OUT);
   p.Dp = round_up(D, 64); p.Np = round_up(N, 64); p.Qp = round_up(Q, 64); p.ldS = round_up(N, 32);
   p.sim = SimLayout{p.nsplit, p.Dp};
@@ -309,22 +333,11 @@ static Plan plan_of(const npair_config& cfg, int sms, bool mma_symmetric, int me
   const bool rs = p.bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER;
   p.fused_grad = tc && !rs && !(cfg.flags & NPAIR_FLAG_NO_FUSED_GRAD);
   p.cat = tc && prec != PREC_BF16;
-  // GLOBAL radix select: candidate lists of the chosen first-digit bucket (1/8 of the block, at most 32 M entries per side; a
-  // bigger bucket -- heavily tied data -- takes the three-sweep path)
-  if (p.gsel_mask) {
-    const long long cap = Q * N / 8 + 4096;
-    p.gcand_cap = static_cast<unsigned int>(cap < (32ll << 20) ? cap : (32ll << 20));
-  }
   // default: 2048 database columns; negative: one accumulator for the whole K range (diagnostic)
   p.grad_chunk_kb = cfg.grad_chunk_cols > 0 ? (cfg.grad_chunk_cols + 31) / 32 : (cfg.grad_chunk_cols < 0 ? 0 : 64);
-  // the fused kernel walks K in 32-column blocks and keeps >= 8 of them (256 columns) per split; the split GEMM keeps >= 4
-  p.grad_kblocks = static_cast<int>(p.fused_grad ? (N + 31) / 32 : (N + p.bk_grad - 1) / p.bk_grad);
-  const int tiles = tile_sched(cfg.Q, cfg.D, p.grad_kblocks).num_tiles();
-  p.grad_split = tc ? split_k(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : SplitK{1, p.grad_kblocks};
-  p.split_cap = tc ? split_k_cap(p.grad_kblocks, tiles, sms, p.fused_grad ? 8 : 4) : 1;
-  // memory rows are no anchors: S is not symmetric, every tile is computed
-  if (!multi && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES) && mem_rows == 0) p.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, p.N));
-  p.sweep_epi = EPI_STATS | (p.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
+  // the split-K bound of the capacity's gradient GEMM, from the fields above (call_plan)
+  const int kb = call_plan(cfg, p, sms, mem_cap).grad_kblocks;
+  p.split_cap = tc ? split_k_cap(kb, tile_sched(cfg.Q, cfg.D, kb).num_tiles(), sms, p.fused_grad ? 8 : 4) : 1;
   p.want_p2p_feat = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_FEATURES);
   p.want_p2p_rec = multi && W <= 32 && !(cfg.flags & NPAIR_FLAG_NCCL_RECORDS) && p.bwd_mode == NPAIR_BWDMODE_ROW_SCALARS;
   if (p.want_p2p_feat || p.want_p2p_rec) p.xl = xchg_layout(cfg.Q, cfg.D, W, p.wscope);
@@ -343,12 +356,12 @@ static void carve_rows(Carve& cv, long long Q, long long mem_cap, RowArrays* ra)
 }
 
 // ------------------------------------------------------------------------------------------------ context
-// A context is its plan plus the buffers and per-step state.
-struct npair_ctx : Plan {
+// A context is its plan, the plan of its current call, the buffers and per-step state.
+struct npair_ctx : Plan, CallPlan {
   npair_config cfg;
   int Q, D, world, rank, prec, sms, device;
   int mem_cap = 0;               // cross-batch memory: the most memory rows a call may pass (npair_create_memory), 0 without
-  int mem_rows = 0;              // the memory rows the N-dependent part of the plan and the tensor maps are set for (set_call_rows)
+  int mem_rows = 0;              // the memory rows the CallPlan and the tensor maps are set for (set_call_rows)
   float* labcat = nullptr;       // memory context: the labels of the current rows and the memory rows, [Q + M]
   DevMem mem;                    // owns the device scratch below (ctx_buffers, p2p_buffers)
   float* Xtot_buf = nullptr;     // world > 1: all-gather target
@@ -392,13 +405,12 @@ struct npair_ctx : Plan {
   // What a forward leaves for the calls after it.  Each forward that enters resets the whole record; a refused one leaves it alone.
   struct Step {
     const float* label = nullptr;                            // this rank's labels
-    const float *x_total = nullptr, *lab_total = nullptr;    // the world's rows (normalised under normalize_input) and labels
+    RowSource x_total{};           // the database's rows (normalised under normalize_input): the world's, or [x; x_mem] (DESIGN 4.3)
+    const float* lab_total = nullptr;                         // and their labels
     bool ext_gathered = false;     // through npair_forward_gathered: the caller did the collectives
     bool rec_gathered = false;     // the NCCL all-gather of the row records has been enqueued (at the first backward)
     bool fwd_done = false;         // the forward succeeded: a backward may follow
-    // cross-batch memory (npair_forward_memory with m > 0): the caller's memory rows and labels.  Only the forward reads them; the
-    // backward only tests x_mem for whether the step had memory rows
-    const float *x_mem = nullptr, *lab_mem = nullptr;
+    const float* lab_mem = nullptr;   // cross-batch memory: the labels of the caller's memory rows x_total.x1 (only the forward reads them)
   } step;
   StreamOrder order;              // the calls' order across streams; debug_read and profile_read wait for its event
   std::string err;
@@ -434,7 +446,7 @@ static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   m.own(&c->ghist, sizeof(unsigned long long) * 4096, true);
   m.own(&c->gcand, sizeof(uint32_t) * 2ull * c->gcand_cap, false);
   // a memory context mirrors tiles in its calls with m = 0 only
-  m.own(&c->sym_tiles, sizeof(int2) * (c->mem_cap ? sym_tile_count(c->cfg.Q, c->cfg.Q) : c->n_sym_tiles), false);
+  m.own(&c->sym_tiles, sizeof(int2) * call_plan(c->cfg, *c, c->sms, 0).n_sym_tiles, false);
   if (c->wscope) { m.own(&c->xch_src, f * NPAIR_XCH_FLOATS, false); m.own(&c->xch_all, f * NPAIR_XCH_FLOATS * c->cfg.world, false); }   // the latter for NCCL
   return m.err;
 }
@@ -534,9 +546,10 @@ size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_
   std::string e;
   if (validate(cfg, &e) != NPAIR_OK || validate_memory(cfg, max_memory_rows, &e) != NPAIR_OK) return 0;
   npair_ctx c;
-  c.cfg = *cfg;
+  c.cfg = *cfg; c.sms = NPAIR_H100_SXM_SMS;
   c.mem_cap = max_memory_rows;
-  static_cast<Plan&>(c) = plan_of(*cfg, NPAIR_H100_SXM_SMS, true, max_memory_rows);
+  static_cast<Plan&>(c) = plan_of(*cfg, c.sms, true, max_memory_rows);
+  static_cast<CallPlan&>(c) = call_plan(*cfg, c, c.sms, max_memory_rows);
   DevMem sizing(false);
   ctx_buffers(&c, sizing);
   if (c.want_p2p_feat || c.want_p2p_rec) p2p_buffers(&c, sizing);   // as if the context had a communicator and peer access
@@ -636,20 +649,19 @@ static bool make_maps(npair_ctx* c, std::string* te) {
   return ok;
 }
 
-// A memory context's calls with m memory rows: everything that depends on the database size N = Q + m -- the tile schedules, the
-// gradient's K blocks and split-K, the GLOBAL candidate capacity, the symmetric tiles (m = 0 only) and the tensor-map extents -- is
-// that of a context planned for exactly m rows, so no result depends on the capacity or on the rows an earlier call left past Q + m.
-// The buffers keep the capacity's layout (ldS, Np), which changes no value.
+// A memory context's calls with m memory rows: the CallPlan -- the tile schedules, the gradient's K blocks and split-K, the GLOBAL
+// candidate capacity, the symmetric tiles (m = 0 only) -- and the tensor-map extents are those of a context planned for exactly m rows,
+// so no result depends on the capacity or on the rows an earlier call left past Q + m.  The buffers keep the capacity's layout (the
+// Plan: ldS, Np), which changes no value.
 static int set_call_rows(npair_ctx* c, int m) {
   if (!c->mem_cap || m == c->mem_rows) return NPAIR_OK;
   c->step.fwd_done = false;                        // the previous step's S and records no longer match the plan
-  const Plan p = plan_of(c->cfg, c->sms, true, m);
+  const CallPlan p = call_plan(c->cfg, *c, c->sms, m);
   if (p.grad_split.splits > c->split_cap) {        // ruled out by split_k_cap; never write past the partial buffer
     c->err = fmt("internal: m = %d needs %d split-K slices, the buffer holds %d", m, p.grad_split.splits, c->split_cap);
     return NPAIR_E_STATE;
   }
-  c->N = p.N; c->gcand_cap = p.gcand_cap; c->grad_kblocks = p.grad_kblocks; c->grad_split = p.grad_split;
-  c->n_sym_tiles = p.n_sym_tiles; c->sweep_epi = p.sweep_epi;
+  static_cast<CallPlan&>(*c) = p;
   c->mem_rows = -1;                                // until the maps match
   std::string te;
   if (!make_maps(c, &te)) { c->err = te; return NPAIR_E_CUDA; }
@@ -680,6 +692,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     return NPAIR_E_ARG;
   }
   static_cast<Plan&>(*c) = plan_of(*cfg, c->sms, sym, mem_cap);
+  static_cast<CallPlan&>(*c) = call_plan(*cfg, *c, c->sms, mem_cap);
   c->Q = cfg->Q; c->D = cfg->D; c->world = cfg->world; c->rank = cfg->rank; c->prec = cfg->sim_precision;
   const int Q = c->Q;
   CREATE_TRY(ctx_buffers(c, c->mem));
@@ -695,7 +708,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   if (c->lsel_mask) CREATE_TRY(allow_local_select_smem());
   if (cfg->gemm_backend == NPAIR_GEMM_TCGEN05) {
     CREATE_TRY(allow_smem(gemm_kernel(c->prec, c->sweep_epi)));
-    if (mem_cap) CREATE_TRY(allow_smem(gemm_kernel(c->prec, plan_of(*cfg, c->sms, sym).sweep_epi)));   // its calls with m = 0
+    if (mem_cap) CREATE_TRY(allow_smem(gemm_kernel(c->prec, call_plan(*cfg, *c, c->sms, 0).sweep_epi)));   // its calls with m = 0
     if (c->n_blocks > 1) CREATE_TRY(allow_smem(gemm_kernel(c->prec, EPI_STORE_S)));
     CREATE_TRY(c->fused_grad ? allow_smem(fused_kernel(c->prec)) : allow_smem(gemm_kernel(c->prec, EPI_OUT)));
     // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
@@ -893,7 +906,7 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     const uint32_t ep = ++c->p2p_fwd_epoch;
     const long long QD = static_cast<long long>(Q) * D;
     p2p_push(c, XCHG_FEATURES, ep, grid_for(QD / 4, 2 * c->sms), d_feat, QD, XP_X, d_label, Q, XP_LAB, st);
-    c->step.x_total = p2p_wait(c, XCHG_FEATURES, ep, XP_X, st);
+    c->step.x_total = {p2p_wait(c, XCHG_FEATURES, ep, XP_X, st), c->N};
     c->step.lab_total = c->p2p_region + c->xl.off(XP_LAB, ep & 1u, 0);
   } else if (c->world > 1) {
     PhaseTimer pt(c, 0, st);
@@ -904,8 +917,8 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     int r2 = api->GroupEnd();
     if (r == 0) r = r2;
     if (r != 0) { c->err = fmt("ncclAllGather: %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
-    c->step.x_total = c->Xtot_buf; c->step.lab_total = c->labtot_buf;
-  } else { c->step.x_total = d_feat; c->step.lab_total = d_label; }
+    c->step.x_total = {c->Xtot_buf, c->N}; c->step.lab_total = c->labtot_buf;
+  } else { c->step.x_total = {d_feat, c->N}; c->step.lab_total = d_label; }
   return forward_impl(c, d_feat, tops, st);
 }
 
@@ -953,13 +966,13 @@ int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float*
   if ((rc = set_call_rows(c, 0)) != NPAIR_OK) return rc;
   const long long r0 = static_cast<long long>(c->rank) * c->Q;
   float* const normed = c->world > 1 ? c->Xtot_buf : c->Ynorm;     // normalize_input: the N normalised rows
-  c->step = npair_ctx::Step{d_label_total + r0, c->cfg.normalize_input ? normed : d_feat_total, d_label_total, true};
+  c->step = npair_ctx::Step{d_label_total + r0, {c->cfg.normalize_input ? normed : d_feat_total, c->N}, d_label_total, true};
   if (c->cfg.normalize_input) {               // the gathered bottoms are raw embeddings: normalise all N rows (1 / ||x|| kept for the local ones)
     PhaseTimer pt(c, 1, call.st);
     launch_l2norm_fwd(d_feat_total, c->N, c->D, normed, nullptr, call.st);
     launch_l2norm_fwd(d_feat_total + r0 * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
   }
-  if ((rc = forward_impl(c, c->step.x_total + r0 * c->D, c->tops_dev, call.st)) != NPAIR_OK) return rc;
+  if ((rc = forward_impl(c, c->step.x_total.x0 + r0 * c->D, c->tops_dev, call.st)) != NPAIR_OK) return rc;
   return finish_forward(c, tops_host, call.st);
 }
 
@@ -977,14 +990,14 @@ static int forward_memory_rows(npair_ctx* c, const float* d_feat, const float* d
                                TopsBlock* tops, cudaStream_t st) {
   const int rc = set_call_rows(c, m);
   if (rc != NPAIR_OK) return rc;
-  c->step = npair_ctx::Step{d_label, nullptr, c->labcat};
-  c->step.x_mem = d_mem_feat; c->step.lab_mem = d_mem_label;
+  c->step = npair_ctx::Step{d_label, {}, c->labcat};
+  c->step.lab_mem = d_mem_label;
   if (c->cfg.normalize_input) {               // the current rows only: the memory holds rows the layer has already seen
     PhaseTimer pt(c, 1, st);
     launch_l2norm_fwd(d_feat, c->Q, c->D, c->Ynorm, c->inv_norm, st);
     d_feat = c->Ynorm;
   }
-  c->step.x_total = d_feat;
+  c->step.x_total = {d_feat, c->Q, d_mem_feat};
   return forward_impl(c, d_feat, tops, st);
 }
 
@@ -1054,17 +1067,10 @@ static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cuda
   // ---- operand preparation: |x| sum (top asum, .cu:400), power-of-two pre-scale, split to tensor-core pieces ----
   {
     PhaseTimer pt(c, 1, st);
-    if (c->step.x_mem) {                       // cross-batch memory: rows [Q, N) are the caller's memory rows, read where they lie
-      const int m = N - Q;
-      launch_memory_rows(c->step.label, Q, c->step.lab_mem, m, c->labcat, c->ra.rowrec, st);
-      launch_prep_reduce_memory(d_feat, static_cast<long long>(Q) * D, c->step.x_mem, static_cast<long long>(m) * D, c->partial,
-                                c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-      launch_split_memory(d_feat, Q, c->step.x_mem, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XcatA, c->XcatB, c->Dp, st);
-    } else {
-      launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, c->step.x_total, static_cast<long long>(N) * D, c->partial,
-                         c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-      launch_split(c->step.x_total, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
-    }
+    const RowSource& xt = c->step.x_total;     // cross-batch memory: rows [Q, N) are the caller's memory rows, read where they lie
+    if (xt.x1) launch_memory_rows(c->step.label, Q, c->step.lab_mem, N - Q, c->labcat, c->ra.rowrec, st);
+    launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, xt, N, D, c->partial, c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
+    launch_split(xt, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
   }
   // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) over all Q rows; S is stored
   //      only when it is materialised, and is then block 0 of the row pass ----
@@ -1296,7 +1302,7 @@ static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
       } else rs_total = c->rs_total;
     }
   } else if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) bw_mode = BW_SPLIT;
-  if (c->step.x_mem) {
+  if (c->step.x_total.x1) {
     // cross-batch memory: the table of the Q row records and the memory rows' records (RowRecord::memory), whose transposed terms
     // are 0, so that the gradient is (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x) with nothing divided
     bw_mode = BW_ROWSCAL;
@@ -1551,10 +1557,10 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
   float sc[2] = {1.f, 1.f};                  // x_scale, x_inv_scale
   if (precision == PREC_FP16X2) {
     const float* op[2] = {dA, dB};
-    const long long n[2] = {static_cast<long long>(M) * K, static_cast<long long>(Nn) * K};
+    const int rows[2] = {M, Nn};
     float mx[2] = {0.f, 0.f};
     for (int i = 0; i < 2; ++i) {
-      launch_prep_reduce(op[i], n[i], op[i], n[i], partial, 1, RowArrays{}, 0, bs, st);
+      launch_prep_reduce(op[i], static_cast<long long>(rows[i]) * K, {op[i], rows[i]}, rows[i], K, partial, 1, RowArrays{}, 0, bs, st);
       CREATE_TRY(cudaMemcpyAsync(&mx[i], &bs->x_absmax, 4, cudaMemcpyDeviceToHost, st));
     }
     CREATE_TRY(cudaStreamSynchronize(st));
@@ -1562,8 +1568,8 @@ int npair_debug_gemm(int precision, int backend, int M, int Nn, int K, const flo
     sc[0] = ps.scale; sc[1] = ps.inv;
   }
   CREATE_TRY(cudaMemcpy(&bs->x_scale, sc, 8, cudaMemcpyHostToDevice));
-  launch_split(dA, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
-  launch_split(dB, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
+  launch_split({dA, M}, M, K, precision, bs, As, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
+  launch_split({dB, Nn}, Nn, K, precision, bs, Bs, Kp, dummyT, tmax, nullptr, 0, 0, 0, nullptr, nullptr, Kp, st);
   GemmParams gp; memset(&gp, 0, sizeof(gp));
   gp.M = M; gp.Nn = Nn; gp.ts = tile_sched(M, Nn, (K + bk - 1) / bk);
   gp.out = dC; gp.ldo = Nn; gp.alpha = 1.f; gp.beta = 0.f;

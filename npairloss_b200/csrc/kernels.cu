@@ -64,37 +64,33 @@ __device__ __forceinline__ void abs_sum_max(const float* __restrict__ x, long lo
   }
   for (long long j = (n4 << 2) + t0; j < n; j += stride) { sum += fabsf(x[j]); if (want_max) mx = fmaxf(mx, fabsf(x[j])); }
 }
-// One kernel: per-block partial |x| sums (local rows) and max|x| (all rows), the reset of the per-row statistics, and --
+// abs_sum_max through 16-byte loads when x is 16-byte aligned (cudaMalloc'd / framework blobs are), 4-byte loads otherwise
+__device__ __forceinline__ void abs_sum_max_at(const float* __restrict__ x, long long n, long long t0, long long stride, bool want_max,
+                                               float& sum, float& mx) {
+  if ((reinterpret_cast<uintptr_t>(x) & 15) == 0) abs_sum_max<true>(x, n, t0, stride, want_max, sum, mx);
+  else abs_sum_max<false>(x, n, t0, stride, want_max, sum, mx);
+}
+// One kernel: per-block partial |x| sums (x_local) and max|x| (x_local and the database), the reset of the per-row statistics, and --
 // in the last block to finish (ticket) -- the final asum, the power-of-two operand scale and the reset of the step state.
-// Returns true in the block that finished last (it has written the step's scalars to *bs).
-// DISJOINT (cross-batch memory): xt holds rows other than xl's, so max |x| is taken over both and the sum over xl alone.
-template <bool DISJOINT = false>
-__device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, long long nl, const float* __restrict__ xt, long long ntot,
-                                                 float* __restrict__ partial, int want_scale, RowArrays ra, int Q, BlockScalars* bs) {
+// The grid fixes the order of the asum: launch_prep_reduce sizes it from the larger of x_local and the database, so the asum of a
+// memory step's current rows is summed in the order of one buffer of Q + m rows.  Eight blocks per SM cap it at 32 registers, which
+// hold each sweep's four 16-byte loads in flight without spilling (uncapped, CUDA 12.9 allocates 40).
+__global__ void __launch_bounds__(256, 8) prep_reduce_kernel(const float* __restrict__ xl, long long nl, RowSource db, int N, int D,
+                                                             float* __restrict__ partial, int want_scale, RowArrays ra, int Q, BlockScalars* bs) {
   __shared__ float s_sum[8], s_max[8];
   __shared__ int s_last;
   float sum = 0.f, mx = 0.f;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  // 16-byte loads, four in flight per thread (cudaMalloc'd / framework blobs are 16-byte aligned; otherwise 4-byte loads)
-  const bool same_range = !DISJOINT && want_scale && xl == xt && nl == ntot;    // world == 1: one sweep gives both the sum and the maximum
-  const bool local_max = DISJOINT ? want_scale != 0 : same_range;
-  if ((reinterpret_cast<uintptr_t>(xl) & 15) == 0) abs_sum_max<true>(xl, nl, t0, stride, local_max, sum, mx);
-  else abs_sum_max<false>(xl, nl, t0, stride, local_max, sum, mx);
-  if (want_scale && !same_range) {
-    if ((reinterpret_cast<uintptr_t>(xt) & 15) == 0) {
-      const float4* x4 = reinterpret_cast<const float4*>(xt);
-      const long long n4 = ntot >> 2;
-      long long i = t0;
-      for (; i + 3 * stride < n4; i += 4 * stride) {
-        const float4 a = __ldg(x4 + i), b = __ldg(x4 + i + stride), c = __ldg(x4 + i + 2 * stride), d = __ldg(x4 + i + 3 * stride);
-        mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))), fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w)))));
-        mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(fabsf(c.x), fabsf(c.y)), fmaxf(fabsf(c.z), fabsf(c.w))), fmaxf(fmaxf(fabsf(d.x), fabsf(d.y)), fmaxf(fabsf(d.z), fabsf(d.w)))));
-      }
-      for (; i < n4; i += stride) { const float4 a = __ldg(x4 + i); mx = fmaxf(mx, fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w)))); }
-      for (long long j = (n4 << 2) + t0; j < ntot; j += stride) mx = fmaxf(mx, fabsf(xt[j]));
-    } else {
-      for (long long i = t0; i < ntot; i += stride) mx = fmaxf(mx, fabsf(xt[i]));
+  abs_sum_max_at(xl, nl, t0, stride, want_scale != 0, sum, mx);
+  if (want_scale) {   // max |x| over the parts of the database that are not x_local itself (world 1: nothing more)
+    const long long n0 = static_cast<long long>(db.n0) * D, n1 = static_cast<long long>(N) * D - n0;
+    float unused = 0.f;
+#pragma unroll 1
+    for (int p = 0; p < 2; ++p) {
+      const float* x = p ? db.x1 : db.x0;
+      const long long n = p ? n1 : n0;
+      if (n > 0 && (x != xl || n != nl)) abs_sum_max_at(x, n, t0, stride, true, unused, mx);
     }
   }
   for (long long i = t0; i < Q; i += stride) reset_row_stats(ra, i);
@@ -110,7 +106,7 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
     s_last = (atomicAdd(&bs->ticket0, 1u) == gridDim.x - 1) ? 1 : 0;
   }
   __syncthreads();
-  if (!s_last) return false;
+  if (!s_last) return;
   __threadfence();
   __shared__ double s_dsum[8];
   double dsum = 0.0; mx = 0.f;
@@ -131,60 +127,43 @@ __device__ __forceinline__ bool prep_reduce_body(const float* __restrict__ xl, l
     bs->cand_n[0] = 0; bs->cand_n[1] = 0;
     bs->n_same = 0; bs->n_diff = 0;
   }
-  return true;
 }
-__global__ void __launch_bounds__(256) prep_reduce_kernel(const float* __restrict__ xl, long long nl, const float* __restrict__ xt, long long ntot,
-                                                          float* __restrict__ partial, int want_scale, RowArrays ra, int Q, BlockScalars* bs) {
-  prep_reduce_body(xl, nl, xt, ntot, partial, want_scale, ra, Q, bs);
-}
-void launch_prep_reduce(const float* x_local, long long n_local, const float* x_total, long long n_total, float* partial,
+void launch_prep_reduce(const float* x_local, long long n_local, RowSource db, int N, int D, float* partial,
                         int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st) {
-  long long nmax = n_local > n_total ? n_local : n_total;
+  const long long n_total = static_cast<long long>(N) * D, nmax = n_local > n_total ? n_local : n_total;
   int nb = static_cast<int>((nmax + 256 * 16 - 1) / (256 * 16));
   if (nb < 1) nb = 1; if (nb > 592) nb = 592;
-  prep_reduce_kernel<<<nb, 256, 0, st>>>(x_local, n_local, x_total, n_total, partial, want_scale, ra, Q, bs);
-  count_launch();
-}
-// Cross-batch memory (DESIGN 4.3): the current rows xl and the memory rows xm are two buffers.  The grid is sized from both, as
-// launch_prep_reduce sizes it for one buffer of Q + m rows, so the asum of the current rows is summed in the same order.
-__global__ void __launch_bounds__(256) prep_reduce_memory_kernel(const float* __restrict__ xl, long long nl, const float* __restrict__ xm,
-                                                                 long long nm, float* __restrict__ partial, int want_scale, RowArrays ra, int Q,
-                                                                 BlockScalars* bs) {
-  prep_reduce_body<true>(xl, nl, xm, nm, partial, want_scale, ra, Q, bs);
-}
-void launch_prep_reduce_memory(const float* x_local, long long n_local, const float* x_mem, long long n_mem, float* partial, int want_scale,
-                               RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st) {
-  int nb = static_cast<int>((n_local + n_mem + 256 * 16 - 1) / (256 * 16));
-  if (nb < 1) nb = 1; if (nb > 592) nb = 592;
-  prep_reduce_memory_kernel<<<nb, 256, 0, st>>>(x_local, n_local, x_mem, n_mem, partial, want_scale, ra, Q, bs);
+  prep_reduce_kernel<<<nb, 256, 0, st>>>(x_local, n_local, db, N, D, partial, want_scale, ra, Q, bs);
   count_launch();
 }
 
 // --------------------------------------------------------------------------------------------
-// operand split: x_total fp32 [N x D] -> Xs[s][N][ldXs] (K-major for the similarity GEMM) and the transposed
+// operand split: the database's rows fp32 [N x D] -> Xs[s][N][ldXs] (K-major for the similarity GEMM) and the transposed
 // XsT[s][D][ldXsT] (K-major for the gradient GEMM whose K is the sample index); XlT = local columns only.
 // --------------------------------------------------------------------------------------------
 // Block = 256 threads, tile = 32 rows (n) x 64 features (d).  Thread (nl = t/8, dg = t%8) converts 8 consecutive features of
 // one row: two 16-byte loads, one 16-byte store per piece / section; the transposed pieces go through a shared tile so
 // that they, too, are written as 16-byte row segments.
 struct SplitArgs {
-  const float* x; int N, D;
+  RowSource x; int N, D;
   uint16_t* Xs; long long ldXs; uint16_t* XsT; long long ldXsT; uint16_t* XlT; long long ldXlT; int row0, Q;
   uint16_t *XcatA, *XcatB; long long Dp;
 };
-// The 8 features thread t of a block converts in tile (tile_d, tile_n): two 16-byte loads (issued early by the fused kernel).
+// The 8 features thread t of a block converts in tile (tile_d, tile_n).  Each row is loaded from its own buffer: a 32-row tile may
+// straddle the two parts of a RowSource, and XsT is written in 16-byte segments of 8 rows, so a shifted pointer would not do.
 __device__ __forceinline__ void split_load(const SplitArgs& a, int tile_d, int tile_n, float (&v)[8]) {
-  const float* __restrict__ x = a.x; const int N = a.N, D = a.D;
+  const int N = a.N, D = a.D;
   const int t = threadIdx.x, nl = t >> 3, dg = t & 7;
   const int n = tile_n * 32 + nl, d = tile_d * 64 + 8 * dg;
   const bool rowok = n < N;
-  if (rowok && d + 7 < D && (D & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {   // 16-byte loads need an aligned base
-    const float4 a4 = *reinterpret_cast<const float4*>(x + static_cast<long long>(n) * D + d);
-    const float4 b4 = *reinterpret_cast<const float4*>(x + static_cast<long long>(n) * D + d + 4);
+  const float* x = a.x.row(n, D);
+  if (rowok && d + 7 < D && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {   // the row starts 16-byte aligned: so does x + d
+    const float4 a4 = *reinterpret_cast<const float4*>(x + d);
+    const float4 b4 = *reinterpret_cast<const float4*>(x + d + 4);
     v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
   } else {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) v[e] = (rowok && d + e < D) ? x[static_cast<long long>(n) * D + d + e] : 0.f;
+    for (int e = 0; e < 8; ++e) v[e] = (rowok && d + e < D) ? x[d + e] : 0.f;
   }
 }
 // One 32-row x 64-feature tile (tile_n, tile_d) by one block of 256 threads from the values split_load fetched.  `buf` alternates
@@ -258,36 +237,6 @@ __global__ void __launch_bounds__(256) split_kernel(SplitArgs a, const BlockScal
   split_load(a, blockIdx.x, blockIdx.y, v);
   split_tile<PREC>(a, (PREC == PREC_FP16X2) ? bs->x_scale : 1.f, blockIdx.x, blockIdx.y, v, 0);
 }
-// Cross-batch memory: rows [0, a.Q) from a.x, rows [a.Q, a.N) from xm.  A 32-row tile may straddle the two buffers, so each row is
-// loaded from its own one; the transposed pieces are then written as by split_kernel, in 16-byte segments across the boundary.
-__device__ __forceinline__ void split_load_memory(const SplitArgs& a, const float* __restrict__ xm, int tile_d, int tile_n, float (&v)[8]) {
-  const int N = a.N, D = a.D;
-  const int t = threadIdx.x, nl = t >> 3, dg = t & 7;
-  const int n = tile_n * 32 + nl, d = tile_d * 64 + 8 * dg;
-  const bool rowok = n < N;
-  const float* x = n < a.Q ? a.x + static_cast<long long>(n) * D : xm + static_cast<long long>(n - a.Q) * D;
-  if (rowok && d + 7 < D && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {   // the row starts 16-byte aligned: so does x + d
-    const float4 a4 = *reinterpret_cast<const float4*>(x + d);
-    const float4 b4 = *reinterpret_cast<const float4*>(x + d + 4);
-    v[0] = a4.x; v[1] = a4.y; v[2] = a4.z; v[3] = a4.w; v[4] = b4.x; v[5] = b4.y; v[6] = b4.z; v[7] = b4.w;
-  } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) v[e] = (rowok && d + e < D) ? x[d + e] : 0.f;
-  }
-}
-template <int PREC>
-__global__ void __launch_bounds__(256) split_memory_kernel(SplitArgs a, const float* __restrict__ xm, const BlockScalars* __restrict__ bs) {
-  float v[8];
-  split_load_memory(a, xm, blockIdx.x, blockIdx.y, v);
-  split_tile<PREC>(a, (PREC == PREC_FP16X2) ? bs->x_scale : 1.f, blockIdx.x, blockIdx.y, v, 0);
-}
-void launch_split_memory(const float* x, int Q, const float* x_mem, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs,
-                         long long ldXs, uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st) {
-  dim3 grid((D + 63) / 64, (N + 31) / 32);
-  const SplitArgs a{x, N, D, Xs, ldXs, XsT, ldXsT, nullptr, 0, 0, Q, XcatA, XcatB, Dp};
-  with_prec(prec, [&](auto P) { split_memory_kernel<P><<<grid, 256, 0, st>>>(a, x_mem, bs); });
-  count_launch();
-}
 // The labels of the Q current rows and the m memory rows into lab_total [Q + m], and the memory rows' records into rec[Q, Q + m): a
 // memory row is never an anchor, so its record switches its transposed gradient term off exactly (RowRecord::memory) and keeps its label,
 // which decides whether the anchor's own term treats the pair as same-label or different-label.
@@ -307,11 +256,11 @@ void launch_memory_rows(const float* label, int Q, const float* mem_label, int m
   count_launch();
 }
 
-void launch_split(const float* x_total, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs, long long ldXs,
+void launch_split(RowSource db, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs, long long ldXs,
                   uint16_t* XsT, long long ldXsT, uint16_t* XlT, long long ldXlT, int row0_local, int Q,
                   uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st) {
   dim3 grid((D + 63) / 64, (N + 31) / 32);
-  const SplitArgs a{x_total, N, D, Xs, ldXs, XsT, ldXsT, XlT, ldXlT, row0_local, Q, XcatA, XcatB, Dp};
+  const SplitArgs a{db, N, D, Xs, ldXs, XsT, ldXsT, XlT, ldXlT, row0_local, Q, XcatA, XcatB, Dp};
   with_prec(prec, [&](auto P) { split_kernel<P><<<grid, 256, 0, st>>>(a, bs); });
   count_launch();
 }

@@ -279,20 +279,24 @@ __host__ __device__ __forceinline__ float ord2f(uint32_t u) {
 extern unsigned long long g_kernel_launches;
 inline void count_launch(int n = 1) { g_kernel_launches += static_cast<unsigned long long>(n); }
 
+// The database's N rows of D features, in at most two buffers: rows [0, n0) from x0, rows [n0, N) from x1 at row n - n0.  One buffer:
+// n0 = N, x1 = NULL.  A cross-batch memory step (DESIGN 4.3) reads [x; x_mem] as {x, Q, x_mem}, where the rows lie.
+struct RowSource {
+  const float* x0; int n0; const float* x1 = nullptr;
+  __host__ __device__ __forceinline__ const float* row(int n, int D) const {
+    return n < n0 ? x0 + static_cast<long long>(n) * D : x1 + static_cast<long long>(n - n0) * D;
+  }
+};
+
 // launchers (kernels.cu)
-void launch_prep_reduce(const float* x_local, long long n_local, const float* x_total, long long n_total, float* partial /*[2*1024]*/,
+// The step's operand preparation: sum |x| over the n_local elements of x_local (the top asum), and when want_scale, max |x| over
+// x_local and the N x D database `db` (the pre-scale); also resets the Q rows' statistics and the step state in bs
+void launch_prep_reduce(const float* x_local, long long n_local, RowSource db, int N, int D, float* partial /*[2*1024]*/,
                         int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st);
-void launch_split(const float* x_total, int N, int D, int prec, const BlockScalars* bs,
+void launch_split(RowSource db, int N, int D, int prec, const BlockScalars* bs,
                   uint16_t* Xs, long long ldXs /*Dp*/, uint16_t* XsT, long long ldXsT /*Np*/,
                   uint16_t* XlT, long long ldXlT /*Qp, or 0*/, int row0_local, int Q,
                   uint16_t* XcatA /*or NULL*/, uint16_t* XcatB, long long Dp, cudaStream_t st);
-// Cross-batch memory (DESIGN 4.3): the operand preparation of the current rows x_local and the memory rows x_mem, two buffers.  max |x|
-// (the pre-scale) over both, the asum over x_local alone
-void launch_prep_reduce_memory(const float* x_local, long long n_local, const float* x_mem, long long n_mem, float* partial /*[2*1024]*/,
-                               int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st);
-// launch_split of the N = Q + m rows [x (Q rows); x_mem] at world 1: the memory rows land at row Q of every B-side operand
-void launch_split_memory(const float* x, int Q, const float* x_mem, int N, int D, int prec, const BlockScalars* bs, uint16_t* Xs,
-                         long long ldXs, uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, cudaStream_t st);
 // lab_total[0, Q + m) = [label; mem_label], rec[Q + i] = RowRecord::memory(mem_label[i])
 void launch_memory_rows(const float* label, int Q, const float* mem_label, int m, float* lab_total, RowRecord* rec, cudaStream_t st);
 void launch_row_stats_ref(SimRows sim, RowArrays ra, cudaStream_t st);
