@@ -59,9 +59,7 @@ _LIB = None
 
 def kernel_launches() -> int:
     """Cumulative number of CUDA kernels libnpair_b200 has launched in this process (include/npair_b200.h)."""
-    f = lib().npair_kernel_launches
-    f.restype = C.c_ulonglong
-    return int(f())
+    return int(lib().npair_kernel_launches())
 
 
 class NpairError(RuntimeError):
@@ -93,6 +91,9 @@ def lib():
         L.npair_memory_workspace_bytes.restype = C.c_size_t
         L.npair_forward_memory.argtypes = [vp, vp, vp, vp, vp, C.c_int32, fp, vp]
         L.npair_backward.argtypes = [vp, C.c_float, vp, vp]
+        L.npair_forward_backward.argtypes = [vp, vp, vp, C.c_float, vp, fp, vp]
+        L.npair_set_anchor_io.argtypes = [vp, vp, vp]
+        L.npair_kernel_launches.restype = C.c_ulonglong
         L.npair_forward_async.argtypes = [vp, vp, vp, vp, vp]
         L.npair_forward_memory_async.argtypes = [vp, vp, vp, vp, vp, C.c_int32, vp, vp]
         L.npair_backward_device_weight.argtypes = [vp, vp, vp, vp]
@@ -139,6 +140,29 @@ def lib():
         L.npair_eval_class_batches_bytes.restype = C.c_size_t
         _LIB = L
     return _LIB
+
+
+def _ptr(t, what, numel=0, dim=None, row=None):
+    """data_ptr() of a tensor the library reads or writes, which must be a contiguous CUDA float32 tensor of `dim` dimensions (when
+    given) and at least `numel` elements; row: a 2-D tensor whose rows hold at least `row` floats.  Raises TypeError for any other kind
+    of tensor and ValueError for one too small, before anything reaches the library: it would take a host pointer for a device one, or
+    read a view as if it were contiguous."""
+    import torch
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+        raise TypeError(f"{what} must be a contiguous CUDA float32 tensor")
+    dim = 2 if row is not None else dim
+    if dim is not None and t.dim() != dim:
+        raise TypeError(f"{what} must have {dim} dimension(s), got {t.dim()}")
+    if row is not None:
+        numel = t.shape[0] * row
+    if t.numel() < numel:
+        raise ValueError(f"{what} holds {t.numel()} floats, the call needs {numel}")
+    return t.data_ptr()
+
+
+def _stream():
+    import torch
+    return torch.cuda.current_stream().cuda_stream
 
 
 def make_config(Q, D, world=1, rank=0, num_tops=5, margin_ident=0.0, margin_diff=0.0, identsn=-1.0, diffsn=-1.0,
@@ -204,95 +228,65 @@ class Context:
         self._check(lib().npair_forward(self._h, feat_ptr, label_ptr, tops, stream))
         return [tops[i] for i in range(5)]
 
-    def backward_ptr(self, loss_weight: float, diff_ptr: int, stream: int = 0):
-        self._check(lib().npair_backward(self._h, C.c_float(loss_weight), diff_ptr, stream))
+    def _rows(self, feat, label, rows=None):
+        """Pointers of `rows` (default Q) rows of features and their labels."""
+        rows = self.cfg.Q if rows is None else rows
+        return _ptr(feat, "feat", rows * self.cfg.D), _ptr(label, "label", rows)
 
-    def forward_backward_ptr(self, feat_ptr: int, label_ptr: int, loss_weight: float, diff_ptr: int, stream: int = 0):
-        tops = (C.c_float * 5)()
-        f = lib().npair_forward_backward
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(C.c_float), C.c_void_p]
-        self._check(f(self._h, feat_ptr, label_ptr, C.c_float(loss_weight), diff_ptr, tops, stream))
-        return [tops[i] for i in range(5)]
+    def _grad(self, diff, what="diff"):
+        return _ptr(diff, what, self.cfg.Q * self.cfg.D)
 
     def forward_backward(self, feat, label, loss_weight, diff):
         """npair_forward_backward: both passes, one host synchronisation."""
-        import torch
-        assert feat.is_cuda and label.is_cuda and diff.is_cuda and feat.is_contiguous() and label.is_contiguous() and diff.is_contiguous()
-        assert feat.dtype == torch.float32 and label.dtype == torch.float32 and diff.dtype == torch.float32
-        return self.forward_backward_ptr(feat.data_ptr(), label.data_ptr(), loss_weight, diff.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        tops = (C.c_float * 5)()
+        self._check(lib().npair_forward_backward(self._h, *self._rows(feat, label), C.c_float(loss_weight), self._grad(diff), tops,
+                                                 _stream()))
+        return [tops[i] for i in range(5)]
 
     def forward(self, feat, label):
-        import torch
-        assert feat.is_cuda and label.is_cuda and feat.dtype == torch.float32 and label.dtype == torch.float32
-        assert feat.is_contiguous() and label.is_contiguous()
-        return self.forward_ptr(feat.data_ptr(), label.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        return self.forward_ptr(*self._rows(feat, label), _stream())
 
     def forward_memory_ptr(self, feat_ptr: int, label_ptr: int, mem_feat_ptr, mem_label_ptr, m: int, stream: int = 0):
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward_memory(self._h, feat_ptr, label_ptr, mem_feat_ptr, mem_label_ptr, int(m), tops, stream))
         return [tops[i] for i in range(5)]
 
+    def _memory(self, mem_feat, mem_label, m):
+        """Pointers of m memory rows and their labels; None for mem_feat None (the library refuses that for m > 0)."""
+        if mem_feat is None:
+            return None, None
+        return _ptr(mem_feat, "mem_feat", int(m) * self.cfg.D), _ptr(mem_label, "mem_label", int(m))
+
     def forward_memory(self, feat, label, mem_feat, mem_label, m=None):
         """npair_forward_memory: the forward over [feat; mem_feat[:m]] with anchors feat only (m = None: all rows of mem_feat).
         mem_feat / mem_label may be None for m = 0; the library reads them during this call only."""
-        import torch
-        assert feat.is_cuda and label.is_cuda and feat.dtype == torch.float32 and label.dtype == torch.float32
-        assert feat.is_contiguous() and label.is_contiguous()
         if m is None:
             m = 0 if mem_feat is None else mem_feat.shape[0]
-        mp = lp = None
-        if mem_feat is not None:
-            assert mem_feat.is_cuda and mem_feat.dtype == torch.float32 and mem_feat.is_contiguous() and mem_feat.shape[0] >= m
-            assert mem_label is not None and mem_label.is_cuda and mem_label.dtype == torch.float32 and mem_label.is_contiguous()
-            assert mem_label.shape[0] >= m
-            mp, lp = mem_feat.data_ptr(), mem_label.data_ptr()
-        return self.forward_memory_ptr(feat.data_ptr(), label.data_ptr(), mp, lp, m, torch.cuda.current_stream().cuda_stream)
+        return self.forward_memory_ptr(*self._rows(feat, label), *self._memory(mem_feat, mem_label, m), m, _stream())
 
     def backward(self, loss_weight, diff):
-        import torch
-        assert diff.is_cuda and diff.dtype == torch.float32 and diff.is_contiguous()
-        self.backward_ptr(loss_weight, diff.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        self._check(lib().npair_backward(self._h, C.c_float(loss_weight), self._grad(diff), _stream()))
 
     # ---- asynchronous step (DESIGN 4.4): world 1, nothing read back on the host, capturable into a CUDA graph ----
-    @staticmethod
-    def _f32(t, what):
-        import torch
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-            raise TypeError(f"{what} must be a contiguous CUDA float32 tensor")
-        return t.data_ptr()
-
     def forward_async(self, feat, label, tops_out):
         """npair_forward_async: enqueues the forward and returns at once; tops_out (5 fp32 on the device) receives the tops in stream
         order, all NaN on a device error (see async_status)."""
-        import torch
-        if tops_out.numel() < 5:
-            raise ValueError("tops_out holds 5 floats")
-        self._check(lib().npair_forward_async(self._h, self._f32(feat, "feat"), self._f32(label, "label"), self._f32(tops_out, "tops_out"),
-                                              torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_forward_async(self._h, *self._rows(feat, label), _ptr(tops_out, "tops_out", 5), _stream()))
         return tops_out
 
     def forward_memory_async(self, feat, label, mem_feat, mem_label, m, tops_out):
         """npair_forward_memory_async: forward_memory with the tops written to tops_out as in forward_async."""
-        import torch
-        if tops_out.numel() < 5:
-            raise ValueError("tops_out holds 5 floats")
-        mp = lp = None
-        if mem_feat is not None:
-            if mem_feat.shape[0] < m or mem_label is None or mem_label.shape[0] < m:
-                raise ValueError("the memory holds fewer than m rows")
-            mp, lp = self._f32(mem_feat, "mem_feat"), self._f32(mem_label, "mem_label")
-        self._check(lib().npair_forward_memory_async(self._h, self._f32(feat, "feat"), self._f32(label, "label"), mp, lp, int(m),
-                                                     self._f32(tops_out, "tops_out"), torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_forward_memory_async(self._h, *self._rows(feat, label), *self._memory(mem_feat, mem_label, m), int(m),
+                                                     _ptr(tops_out, "tops_out", 5), _stream()))
         return tops_out
 
     def backward_device_weight(self, loss_weight, diff):
         """npair_backward_device_weight: backward with the loss weight read on the device from loss_weight (a one-element CUDA fp32
         tensor), with the gradient bits of backward(float(loss_weight))."""
-        import torch
+        lw = _ptr(loss_weight, "loss_weight", 1)
         if loss_weight.numel() != 1:
             raise ValueError("loss_weight is one element")
-        self._check(lib().npair_backward_device_weight(self._h, self._f32(loss_weight, "loss_weight"), self._f32(diff, "diff"),
-                                                       torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_backward_device_weight(self._h, lw, self._grad(diff), _stream()))
 
     def async_status(self):
         """npair_async_status: waits for the context's last call and raises NpairError (E_EMPTY_LIST, E_POS_RANGE, or E_ARG for an
@@ -305,42 +299,34 @@ class Context:
         or None (unweighted / not written).  The library keeps the pointers until the next call: keep the tensors alive until then."""
         ptrs = []
         for t, what in ((weight, "weight"), (row_loss, "row_loss")):
-            if t is None:
-                ptrs.append(None)
-                continue
-            if t.numel() != self.cfg.Q:
+            ptrs.append(None if t is None else _ptr(t, what, self.cfg.Q))
+            if t is not None and t.numel() != self.cfg.Q:
                 raise ValueError(f"{what} holds Q = {self.cfg.Q} floats, got {t.numel()}")
-            ptrs.append(self._f32(t, what))
-        f = lib().npair_set_anchor_io
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        self._check(f(self._h, ptrs[0], ptrs[1]))
+        self._check(lib().npair_set_anchor_io(self._h, *ptrs))
 
     def forward_gathered(self, feat_total, label_total):
-        import torch
-        assert feat_total.is_cuda and feat_total.dtype == torch.float32 and feat_total.is_contiguous()
-        assert label_total.is_cuda and label_total.dtype == torch.float32 and label_total.is_contiguous()
+        """npair_forward_gathered: the world's N = Q * world rows and labels, gathered by the caller."""
         tops = (C.c_float * 5)()
-        self._check(lib().npair_forward_gathered(self._h, feat_total.data_ptr(), label_total.data_ptr(), tops,
-                                                 torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_forward_gathered(self._h, *self._rows(feat_total, label_total, self.cfg.Q * self.cfg.world), tops,
+                                                 _stream()))
         return [tops[i] for i in range(5)]
 
     def backward_partial(self, loss_weight, local_half, total_half=None):
-        import torch
-        self._check(lib().npair_backward_partial(self._h, C.c_float(loss_weight), local_half.data_ptr(),
-                                                 total_half.data_ptr() if total_half is not None else None,
-                                                 torch.cuda.current_stream().cuda_stream))
+        """npair_backward_partial: local_half [Q, D], and at world > 1 total_half [N, D], this rank's addend of the all-reduce."""
+        total = None if total_half is None else _ptr(total_half, "total_half", self.cfg.Q * self.cfg.world * self.cfg.D)
+        self._check(lib().npair_backward_partial(self._h, C.c_float(loss_weight), self._grad(local_half, "local_half"), total, _stream()))
 
     def bwd_exchange_mode(self):
         return lib().npair_bwd_exchange_mode(self._h)
 
     def row_scalars(self, out):
-        import torch
-        self._check(lib().npair_row_scalars(self._h, out.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        """npair_row_scalars: the rank's Q row records, 8 floats each, into out."""
+        self._check(lib().npair_row_scalars(self._h, _ptr(out, "out", 8 * self.cfg.Q), _stream()))
 
     def backward_gathered(self, loss_weight, rs_total, diff):
-        import torch
-        self._check(lib().npair_backward_gathered(self._h, C.c_float(loss_weight), rs_total.data_ptr(), diff.data_ptr(),
-                                                  torch.cuda.current_stream().cuda_stream))
+        """npair_backward_gathered: the backward from the world's row records rs_total (8 floats for each of the N rows)."""
+        rs = _ptr(rs_total, "rs_total", 8 * self.cfg.Q * self.cfg.world)
+        self._check(lib().npair_backward_gathered(self._h, C.c_float(loss_weight), rs, self._grad(diff), _stream()))
 
     def profile_enable(self, on=True):
         self._check(lib().npair_profile_enable(self._h, 1 if on else 0))
@@ -420,51 +406,52 @@ class Evaluator:
         if rc:
             raise NpairError(rc, lib().npair_eval_last_error(self._h).decode())
 
-    @staticmethod
-    def _arg(t, dim):
-        import torch
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == dim):
-            raise TypeError("expected a contiguous CUDA float32 tensor of %d dimension(s)" % dim)
-        return t.data_ptr()
+    def _rows(self, x, what):
+        """The pointer of x, a 2-D tensor of rows of D floats."""
+        return _ptr(x, what, row=self.D)
 
     def rank(self, query, qlabel, gallery, glabel, self_offset=-1):
         """int32 rank[nq] (npair_eval_rank)."""
         import torch
-        rank = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
-        self._check(lib().npair_eval_rank(self._h, self._arg(query, 2), self._arg(qlabel, 1), query.shape[0], self._arg(gallery, 2),
-                                          self._arg(glabel, 1), gallery.shape[0], self_offset, rank.data_ptr(),
-                                          torch.cuda.current_stream().cuda_stream))
+        q, g = self._rows(query, "query"), self._rows(gallery, "gallery")
+        nq, ng = query.shape[0], gallery.shape[0]
+        ql, gl = _ptr(qlabel, "qlabel", nq, 1), _ptr(glabel, "glabel", ng, 1)
+        rank = torch.empty(nq, dtype=torch.int32, device=query.device)
+        self._check(lib().npair_eval_rank(self._h, q, ql, nq, g, gl, ng, self_offset, rank.data_ptr(), _stream()))
         return rank
 
     def best_positive(self, query, qlabel, gallery, glabel, absmax, self_offset=-1, gallery_row0=0):
         """Phase 1 on one gallery shard: fp32 best[nq], -inf where the shard holds no positive."""
         import torch
-        best = torch.empty(query.shape[0], dtype=torch.float32, device=query.device)
-        self._check(lib().npair_eval_best_positive(self._h, self._arg(query, 2), self._arg(qlabel, 1), query.shape[0],
-                                                   self._arg(gallery, 2), self._arg(glabel, 1), gallery.shape[0], self_offset,
-                                                   gallery_row0, C.c_float(absmax), best.data_ptr(),
-                                                   torch.cuda.current_stream().cuda_stream))
+        q, g = self._rows(query, "query"), self._rows(gallery, "gallery")
+        nq, ng = query.shape[0], gallery.shape[0]
+        ql, gl = _ptr(qlabel, "qlabel", nq, 1), _ptr(glabel, "glabel", ng, 1)
+        best = torch.empty(nq, dtype=torch.float32, device=query.device)
+        self._check(lib().npair_eval_best_positive(self._h, q, ql, nq, g, gl, ng, self_offset, gallery_row0, C.c_float(absmax),
+                                                   best.data_ptr(), _stream()))
         return best
 
     def count(self, query, gallery, cut, absmax, self_offset=-1, gallery_row0=0):
         """Phase 2 on one gallery shard: int32 count[nq] of the shard's columns >= cut (0 where cut is -inf)."""
         import torch
-        count = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
-        self._check(lib().npair_eval_count(self._h, self._arg(query, 2), query.shape[0], self._arg(gallery, 2), gallery.shape[0],
-                                           self_offset, gallery_row0, C.c_float(absmax), self._arg(cut, 1), count.data_ptr(),
-                                           torch.cuda.current_stream().cuda_stream))
+        q, g = self._rows(query, "query"), self._rows(gallery, "gallery")
+        nq = query.shape[0]
+        ct = _ptr(cut, "cut", nq, 1)
+        count = torch.empty(nq, dtype=torch.int32, device=query.device)
+        self._check(lib().npair_eval_count(self._h, q, nq, g, gallery.shape[0], self_offset, gallery_row0, C.c_float(absmax), ct,
+                                           count.data_ptr(), _stream()))
         return count
 
     def knn(self, query, gallery, k, self_offset=-1, gallery_row0=0, absmax=-1.0, block_rows=0):
         """npair_eval_knn: each query's k nearest gallery rows, s descending, then global gallery index ascending (NaN last).  Returns
         (fp32 sim[nq, k], int32 index[nq, k]) with index = gallery_row0 + the row in `gallery`; absmax >= 0 for a gallery shard."""
         import torch
+        q, g = self._rows(query, "query"), self._rows(gallery, "gallery")
         nq, dev = query.shape[0], query.device
         sim = torch.empty(nq, int(k), dtype=torch.float32, device=dev)
         index = torch.empty(nq, int(k), dtype=torch.int32, device=dev)
-        self._check(lib().npair_eval_knn(self._h, self._arg(query, 2), nq, self._arg(gallery, 2), gallery.shape[0], self_offset,
-                                         gallery_row0, C.c_float(absmax), int(k), block_rows, sim.data_ptr(), index.data_ptr(),
-                                         torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_eval_knn(self._h, q, nq, g, gallery.shape[0], self_offset, gallery_row0, C.c_float(absmax), int(k),
+                                         block_rows, sim.data_ptr(), index.data_ptr(), _stream()))
         return sim, index
 
     def class_batches(self, class_emb, pools, n, scores=True):
@@ -482,26 +469,27 @@ class Evaluator:
                 raise ValueError("pool entries must be class ids")   # the library checks them against n_classes
             p = p.astype(np.int32)
         p = np.ascontiguousarray(p)
+        emb = self._rows(class_emb, "class_emb")
         nb, dev = p.shape[0], class_emb.device
         batches = torch.empty(nb, int(n), dtype=torch.int32, device=dev)
         sc = torch.empty(nb, int(n), dtype=torch.float32, device=dev) if scores else None
-        self._check(lib().npair_eval_class_batches(self._h, self._arg(class_emb, 2), class_emb.shape[0], p.ctypes.data, p.shape[1], nb,
-                                                   int(n), batches.data_ptr(), sc.data_ptr() if scores else None,
-                                                   torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_eval_class_batches(self._h, emb, class_emb.shape[0], p.ctypes.data, p.shape[1], nb, int(n),
+                                                   batches.data_ptr(), sc.data_ptr() if scores else None, _stream()))
         return batches, sc
 
     def map_at_r(self, query, qlabel, gallery, glabel, self_offset=-1):
         """npair_eval_map_at_r: fp64 map_r[nq] and r_precision[nq] (NaN where a query has no positive), int32 R[nq] and rank[nq]
         (rank as Evaluator.rank).  Synchronises with the host once, to size its positive-pair buffer."""
         import torch
-        nq, dev = query.shape[0], query.device
+        q, g = self._rows(query, "query"), self._rows(gallery, "gallery")
+        nq, ng, dev = query.shape[0], gallery.shape[0], query.device
+        ql, gl = _ptr(qlabel, "qlabel", nq, 1), _ptr(glabel, "glabel", ng, 1)
         map_r = torch.empty(nq, dtype=torch.float64, device=dev)
         r_prec = torch.empty(nq, dtype=torch.float64, device=dev)
         R = torch.empty(nq, dtype=torch.int32, device=dev)
         rank = torch.empty(nq, dtype=torch.int32, device=dev)
-        self._check(lib().npair_eval_map_at_r(self._h, self._arg(query, 2), self._arg(qlabel, 1), nq, self._arg(gallery, 2),
-                                              self._arg(glabel, 1), gallery.shape[0], self_offset, map_r.data_ptr(), r_prec.data_ptr(),
-                                              R.data_ptr(), rank.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_eval_map_at_r(self._h, q, ql, nq, g, gl, ng, self_offset, map_r.data_ptr(), r_prec.data_ptr(),
+                                              R.data_ptr(), rank.data_ptr(), _stream()))
         return {"map_r": map_r, "r_precision": r_prec, "R": R, "rank": rank}
 
     def kmeans(self, x, k, init_rows, max_iter):
@@ -510,6 +498,7 @@ class Evaluator:
         "iterations": sweeps run, "changed": assignments the last sweep changed, "empty": empty clusters}.  Synchronises with the host
         once per iteration."""
         import torch
+        xp = self._rows(x, "x")
         n, dev = x.shape[0], x.device
         init_rows = [int(r) for r in init_rows]
         if len(init_rows) != int(k):
@@ -519,8 +508,8 @@ class Evaluator:
         assign = torch.empty(n, dtype=torch.int32, device=dev)
         inertia = torch.empty((), dtype=torch.float64, device=dev)
         stats = (C.c_int32 * 3)()
-        self._check(lib().npair_eval_kmeans(self._h, self._arg(x, 2), n, int(k), rows, int(max_iter), centroids.data_ptr(),
-                                            assign.data_ptr(), inertia.data_ptr(), stats, torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_eval_kmeans(self._h, xp, n, int(k), rows, int(max_iter), centroids.data_ptr(), assign.data_ptr(),
+                                            inertia.data_ptr(), stats, _stream()))
         return {"assign": assign, "centroids": centroids, "inertia": inertia, "iterations": stats[0], "changed": stats[1],
                 "empty": stats[2]}
 
@@ -529,22 +518,23 @@ class Evaluator:
         random numbers from SplitMix64 seeded with seed modulo 2^64.  Returns (rows, potential): the k row indices, a list that
         Evaluator.kmeans takes as init_rows, and the final potential phi (a Python int, in the fixed-point units of the header).
         Synchronises with the host once, at the end."""
-        import torch
+        xp = self._rows(x, "x")
         rows = (C.c_int32 * max(int(k), 1))()
         phi = C.c_uint64(0)
-        self._check(lib().npair_eval_kmeans_seed(self._h, self._arg(x, 2), x.shape[0], int(k), C.c_uint64(int(seed) % 2 ** 64),
-                                                 int(local_trials), rows, C.byref(phi), torch.cuda.current_stream().cuda_stream))
+        self._check(lib().npair_eval_kmeans_seed(self._h, xp, x.shape[0], int(k), C.c_uint64(int(seed) % 2 ** 64), int(local_trials),
+                                                 rows, C.byref(phi), _stream()))
         return [rows[i] for i in range(int(k))], int(phi.value)
 
 
 def debug_gemm(precision, backend, A, B):
     """C = A @ B.T through the split-operand GEMM (unit test hook)."""
     import torch
+    a = _ptr(A, "A", dim=2)
     M, K = A.shape
+    b = _ptr(B, "B", row=K)
     Nn = B.shape[0]
     Cout = torch.empty((M, Nn), dtype=torch.float32, device=A.device)
-    rc = lib().npair_debug_gemm(precision, backend, M, Nn, K, A.data_ptr(), B.data_ptr(), Cout.data_ptr(),
-                                torch.cuda.current_stream().cuda_stream)
+    rc = lib().npair_debug_gemm(precision, backend, M, Nn, K, a, b, Cout.data_ptr(), _stream())
     if rc:
         raise NpairError(rc, lib().npair_last_error(None).decode())
     return Cout
@@ -553,20 +543,23 @@ def debug_gemm(precision, backend, A, B):
 def l2normalize_forward(x):
     """y = x / ||x||_2 per row (npair_l2normalize_forward); returns (y, inv_norm) as CUDA tensors."""
     import torch
-    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
+    xp = _ptr(x, "x", dim=2)
     y = torch.empty_like(x)
     inv = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
-    rc = lib().npair_l2normalize_forward(x.data_ptr(), x.shape[0], x.shape[1], y.data_ptr(), inv.data_ptr(), torch.cuda.current_stream().cuda_stream)
+    rc = lib().npair_l2normalize_forward(xp, x.shape[0], x.shape[1], y.data_ptr(), inv.data_ptr(), _stream())
     if rc:
         raise NpairError(rc, lib().npair_last_error(None).decode())
     return y, inv
 
 
 def l2normalize_backward(y, inv, dy):
+    """dx of the rows of y (2-D) from their inv_norm and dy (npair_l2normalize_backward); dx has the shape of dy."""
     import torch
+    yp = _ptr(y, "y", dim=2)
+    rows, dim = y.shape
+    ip, dyp = _ptr(inv, "inv", rows), _ptr(dy, "dy", rows * dim)
     dx = torch.empty_like(dy)
-    rc = lib().npair_l2normalize_backward(y.data_ptr(), inv.data_ptr(), dy.data_ptr(), y.shape[0], y.shape[1], dx.data_ptr(),
-                                          torch.cuda.current_stream().cuda_stream)
+    rc = lib().npair_l2normalize_backward(yp, ip, dyp, rows, dim, dx.data_ptr(), _stream())
     if rc:
         raise NpairError(rc, lib().npair_last_error(None).decode())
     return dx

@@ -818,6 +818,23 @@ static MiningParams mining_of(const npair_config& c) {
   return mp;
 }
 
+// The device error bits a forward reports (TopsBlock::err, and AsyncWords::err of the asynchronous forwards), first match first: the
+// return code, and the message of a synchronous forward and of npair_async_status
+struct DeviceError { int bit, code; const char *sync_msg, *async_msg; };
+static const DeviceError DEVICE_ERRORS[] = {
+  {DERR_EMPTY_LIST, NPAIR_E_EMPTY_LIST, "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)",
+   "an asynchronous forward indexed an empty same/diff list (undefined behaviour in the reference, .cu:296/:327/:288)"},
+  {DERR_POS_RANGE, NPAIR_E_POS_RANGE, "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)",
+   "an asynchronous forward's identsn/diffsn selected a position outside the list (undefined behaviour in the reference, .cu:285-288)"},
+  {DERR_ANCHOR_WEIGHT, NPAIR_E_ARG, "an anchor weight (npair_set_anchor_io) is outside [0, 1] or NaN",
+   "an asynchronous forward read an anchor weight (npair_set_anchor_io) outside [0, 1] or NaN"},
+};
+static const DeviceError* device_error(unsigned int bits) {
+  for (const DeviceError& e : DEVICE_ERRORS)
+    if (bits & e.bit) return &e;
+  return nullptr;
+}
+
 // The reference blocks after its forward (host reads of loss / asum, .cu:384,400).  The five tops land in mapped pinned memory followed by
 // this forward's sequence number: polling that word returns a few microseconds earlier than a stream synchronisation and does not
 // wait for anything enqueued behind the row pass (the row-record push, a backward).  A fault in a kernel never writes the number:
@@ -833,13 +850,10 @@ static int finish_forward(npair_ctx* c, float tops_host[5], cudaStream_t st) {
     if ((spins & 0x3FFull) == 0) sched_yield();   // ranks that share a core (fewer cores than ranks, an inherited binding) take turns quickly
   }
   __sync_synchronize();
-  const int derr = c->tops_pinned->err;
-  if (derr & DERR_EMPTY_LIST) { c->err = "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
-  if (derr & DERR_POS_RANGE) { c->err = "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)"; return NPAIR_E_POS_RANGE; }
-  if (derr & DERR_ANCHOR_WEIGHT) {
-    for (int t = 0; t < 5; ++t) tops_host[t] = __builtin_nanf("");
-    c->err = "an anchor weight (npair_set_anchor_io) is outside [0, 1] or NaN";
-    return NPAIR_E_ARG;
+  if (const DeviceError* e = device_error(c->tops_pinned->err)) {
+    if (e->bit == DERR_ANCHOR_WEIGHT) for (int t = 0; t < 5; ++t) tops_host[t] = __builtin_nanf("");
+    c->err = e->sync_msg;
+    return e->code;
   }
   for (int t = 0; t < 5; ++t) tops_host[t] = t < c->cfg.num_tops ? c->tops_pinned->tops[t] : 0.f;
   c->step.fwd_done = true;
@@ -886,30 +900,31 @@ static int async_entry(npair_ctx* c, void* stream, const char* call, bool* captu
   return NPAIR_OK;
 }
 
-static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cudaStream_t st);
+// The gradient kernels write their outputs with 8- and 16-byte stores, so every output pointer must be 16-byte aligned (cudaMalloc,
+// Caffe blobs and torch allocations are).  NULL passes: the callers test for it themselves.
+static int check_out_aligned(npair_ctx* c, const float* p, const char* name) {
+  if ((reinterpret_cast<uintptr_t>(p) & 15) == 0) return NPAIR_OK;
+  c->err = fmt("%s is not 16-byte aligned", name);
+  return NPAIR_E_ARG;
+}
 
-// Enqueues npair_forward on the rank's own bottoms: the fused L2Normalize, the feature all-gather, then the layer's forward, whose
-// tops go to `tops` (mapped pinned memory for the synchronous calls, device memory for the asynchronous ones)
-static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label, TopsBlock* tops, cudaStream_t st) {
-  const int rc = set_call_rows(c, 0);
-  if (rc != NPAIR_OK) return rc;
-  c->step = npair_ctx::Step{d_label};
+static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cudaStream_t st);
+// The loss weight of a backward: a host value, or (d_lw, world 1) one fp32 in device memory read in stream order
+struct LossWeight { float host; const float* dev; };
+static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
+
+// ---- GatherFeatureAndLabel (.cu:17-43) at world > 1: the world's rows and labels into the step, by peer-memory stores or one NCCL
+//      group, device to device over NVLink ----
+static int gather_rows(npair_ctx* c, const float* d_feat, const float* d_label, cudaStream_t st) {
   const int Q = c->Q, D = c->D;
-  if (c->cfg.normalize_input) {               // fused L2Normalize producer (usage/def.prototxt:115-120): the layer works on x / ||x||
-    PhaseTimer pt(c, 1, st);
-    launch_l2norm_fwd(d_feat, Q, D, c->Ynorm, c->inv_norm, st);
-    d_feat = c->Ynorm;
-  }
-  // ---- GatherFeatureAndLabel (.cu:17-43): one NCCL group, device to device over NVLink ----
-  if (c->world > 1 && c->p2p_feat) {
-    PhaseTimer pt(c, 0, st);
+  PhaseTimer pt(c, 0, st);
+  if (c->p2p_feat) {
     const uint32_t ep = ++c->p2p_fwd_epoch;
     const long long QD = static_cast<long long>(Q) * D;
     p2p_push(c, XCHG_FEATURES, ep, grid_for(QD / 4, 2 * c->sms), d_feat, QD, XP_X, d_label, Q, XP_LAB, st);
     c->step.x_total = {p2p_wait(c, XCHG_FEATURES, ep, XP_X, st), c->N};
     c->step.lab_total = c->p2p_region + c->xl.off(XP_LAB, ep & 1u, 0);
-  } else if (c->world > 1) {
-    PhaseTimer pt(c, 0, st);
+  } else {
     NcclApi* api = nccl_api();
     int r = api->GroupStart();
     if (r == 0) r = api->AllGather(d_feat, c->Xtot_buf, static_cast<size_t>(Q) * D, NCCL_FLOAT32, c->comm, st);
@@ -918,12 +933,87 @@ static int forward_rank(npair_ctx* c, const float* d_feat, const float* d_label,
     if (r == 0) r = r2;
     if (r != 0) { c->err = fmt("ncclAllGather: %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
     c->step.x_total = {c->Xtot_buf, c->N}; c->step.lab_total = c->labtot_buf;
-  } else { c->step.x_total = {d_feat, c->N}; c->step.lab_total = d_label; }
-  return forward_impl(c, d_feat, tops, st);
+  }
+  return NPAIR_OK;
 }
 
-// The asynchronous forward's finish: the tops and error bits go from the device TopsBlock to d_tops and the error word in stream order
-static int finish_forward_async(npair_ctx* c, float* d_tops, cudaStream_t st) {
+// The rows a forward's database is made of: the caller's own Q rows (the library gathers the world's at world > 1), the world's N rows
+// the caller gathered itself (rank r's rows are [r*Q, (r+1)*Q), npair_forward_gathered), or a cross-batch memory call's [x; x_mem]
+// (DESIGN 4.3), whose m = 0 is the caller's own rows
+enum Database { DB_OWN, DB_GATHERED, DB_MEMORY };
+struct StepRows {
+  Database db;
+  const float *x, *label;
+  const float *x_mem = nullptr, *label_mem = nullptr;
+  int m = 0;
+};
+
+// Starts a forward's step: the plan of its database size, a fresh Step, the fused L2Normalize producer (usage/def.prototxt:115-120)
+// and the database's rows and labels.  *anchors: the rank's Q rows as the layer reads them.
+static int begin_step(npair_ctx* c, const StepRows& in, const float** anchors, cudaStream_t st) {
+  const int rc = set_call_rows(c, in.m);
+  if (rc != NPAIR_OK) return rc;
+  const bool gathered = in.db == DB_GATHERED;
+  const long long r0 = gathered ? static_cast<long long>(c->rank) * c->Q : 0;   // the rank's rows among the gathered ones
+  c->step = npair_ctx::Step{};
+  c->step.label = in.label + r0;
+  const float* x = in.x + r0 * c->D;
+  if (c->cfg.normalize_input) {               // the layer works on x / ||x|| (1 / ||x|| kept for the rank's rows)
+    PhaseTimer pt(c, 1, st);
+    // gathered rows are raw embeddings: at world > 1 the database's N rows are normalised too.  Memory rows are rows the layer has
+    // already seen.
+    if (gathered && c->world > 1) launch_l2norm_fwd(in.x, c->N, c->D, c->Xtot_buf, nullptr, st);
+    launch_l2norm_fwd(x, c->Q, c->D, c->Ynorm, c->inv_norm, st);
+    x = c->Ynorm;
+  }
+  *anchors = x;
+  if (gathered) {
+    const float* all = !c->cfg.normalize_input ? in.x : c->world > 1 ? c->Xtot_buf : c->Ynorm;
+    c->step.x_total = {all, c->N};
+    c->step.lab_total = in.label;
+    c->step.ext_gathered = true;
+    *anchors = all + r0 * c->D;
+  } else if (in.m > 0) {                      // the memory rows are read where they lie (two-source operand preparation)
+    c->step.x_total = {x, c->Q, in.x_mem};
+    c->step.lab_total = c->labcat;
+    c->step.lab_mem = in.label_mem;
+  } else if (c->world > 1) {
+    return gather_rows(c, x, in.label, st);
+  } else {
+    c->step.x_total = {x, c->N};
+    c->step.lab_total = in.label;
+  }
+  return NPAIR_OK;
+}
+
+// Every forward entry after its null-pointer check: the preconditions, the step and the layer's forward, npair_forward_backward's
+// backward (d_diff), then the finish.  The tops go to tops_host (mapped pinned memory that the call waits on) or, asynchronous, to d_tops
+// in stream order.  `name` names the entry in the refusals.
+static int forward_call(npair_ctx* c, const char* name, const StepRows& rows, float* tops_host, float* d_tops, float* d_diff,
+                        float loss_weight, void* stream) {
+  int rc;
+  if (rows.db == DB_MEMORY) {                 // a memory context's configuration, and at most its M memory rows
+    if ((rc = validate_memory(&c->cfg, 1, &c->err)) != NPAIR_OK) return rc;
+    if (rows.m < 0 || rows.m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", rows.m, c->mem_cap); return NPAIR_E_ARG; }
+  }
+  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
+  bool captured = false;
+  if (d_tops) {
+    if ((rc = async_entry(c, stream, name, &captured)) != NPAIR_OK) return rc;
+  } else {
+    if (rows.db != DB_GATHERED && (rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
+    if ((rc = refuse_capture(c, stream, name)) != NPAIR_OK) return rc;
+  }
+  OrderedCall call(c, stream, captured);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const cudaStream_t st = call.st;
+  const float* anchors = nullptr;
+  if ((rc = begin_step(c, rows, &anchors, st)) != NPAIR_OK) return rc;
+  if ((rc = forward_impl(c, anchors, d_tops ? &c->aw->tops : c->tops_dev, st)) != NPAIR_OK) return rc;
+  // the backward goes in right behind the forward's kernels: finish_forward waits for the tops only, and records `done` behind it
+  if (d_diff && (rc = backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, st)) != NPAIR_OK) return rc;
+  if (tops_host) return finish_forward(c, tops_host, st);
+  // asynchronous: the tops and error bits go from the device TopsBlock to d_tops and the error word in stream order
   launch_async_tops(c->aw, c->cfg.num_tops, d_tops, st);
   CUDA_TRY(c, cudaGetLastError());
   c->step.fwd_done = true;
@@ -933,25 +1023,13 @@ static int finish_forward_async(npair_ctx* c, float* d_tops, cudaStream_t st) {
 int npair_forward(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
-  if ((rc = refuse_capture(c, stream, "npair_forward")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_rank(c, d_feat, d_label, c->tops_dev, call.st)) != NPAIR_OK) return rc;
-  return finish_forward(c, tops_host, call.st);
+  return forward_call(c, "npair_forward", StepRows{DB_OWN, d_feat, d_label}, tops_host, nullptr, nullptr, 0.f, stream);
 }
 
 int npair_forward_async(npair_ctx* c, const float* d_feat, const float* d_label, float* d_tops, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !d_tops) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  bool captured = false;
-  if ((rc = async_entry(c, stream, "npair_forward_async", &captured)) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream, captured);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_rank(c, d_feat, d_label, &c->aw->tops, call.st)) != NPAIR_OK) return rc;
-  return finish_forward_async(c, d_tops, call.st);
+  return forward_call(c, "npair_forward_async", StepRows{DB_OWN, d_feat, d_label}, nullptr, d_tops, nullptr, 0.f, stream);
 }
 
 /* External-collectives variant: the caller already holds the all-gathered N x D features and N labels (rank r's rows are
@@ -959,60 +1037,19 @@ int npair_forward_async(npair_ctx* c, const float* d_feat, const float* d_label,
 int npair_forward_gathered(npair_ctx* c, const float* d_feat_total, const float* d_label_total, float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat_total || !d_label_total || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = refuse_capture(c, stream, "npair_forward_gathered")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = set_call_rows(c, 0)) != NPAIR_OK) return rc;
-  const long long r0 = static_cast<long long>(c->rank) * c->Q;
-  float* const normed = c->world > 1 ? c->Xtot_buf : c->Ynorm;     // normalize_input: the N normalised rows
-  c->step = npair_ctx::Step{d_label_total + r0, {c->cfg.normalize_input ? normed : d_feat_total, c->N}, d_label_total, true};
-  if (c->cfg.normalize_input) {               // the gathered bottoms are raw embeddings: normalise all N rows (1 / ||x|| kept for the local ones)
-    PhaseTimer pt(c, 1, call.st);
-    launch_l2norm_fwd(d_feat_total, c->N, c->D, normed, nullptr, call.st);
-    launch_l2norm_fwd(d_feat_total + r0 * c->D, c->Q, c->D, c->Ynorm, c->inv_norm, call.st);
-  }
-  if ((rc = forward_impl(c, c->step.x_total.x0 + r0 * c->D, c->tops_dev, call.st)) != NPAIR_OK) return rc;
-  return finish_forward(c, tops_host, call.st);
+  return forward_call(c, "npair_forward_gathered", StepRows{DB_GATHERED, d_feat_total, d_label_total}, tops_host, nullptr, nullptr, 0.f,
+                      stream);
 }
 
 /* Cross-batch memory (DESIGN 4.3): the database is [x; x_mem], Q + m rows, whose first Q are the anchors.  The memory rows are read
  * where they lie (two-source operand preparation), and their records in the table after the Q row records switch their transposed
- * gradient term off.  m = 0 is npair_forward. */
-static int memory_call_args(npair_ctx* c, int m) {
-  const int rc = validate_memory(&c->cfg, 1, &c->err);
-  if (rc != NPAIR_OK) return rc;
-  if (m < 0 || m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", m, c->mem_cap); return NPAIR_E_ARG; }
-  return NPAIR_OK;
-}
-// Enqueues npair_forward_memory with m > 0 memory rows, its tops going to `tops`
-static int forward_memory_rows(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label, int m,
-                               TopsBlock* tops, cudaStream_t st) {
-  const int rc = set_call_rows(c, m);
-  if (rc != NPAIR_OK) return rc;
-  c->step = npair_ctx::Step{d_label, {}, c->labcat};
-  c->step.lab_mem = d_mem_label;
-  if (c->cfg.normalize_input) {               // the current rows only: the memory holds rows the layer has already seen
-    PhaseTimer pt(c, 1, st);
-    launch_l2norm_fwd(d_feat, c->Q, c->D, c->Ynorm, c->inv_norm, st);
-    d_feat = c->Ynorm;
-  }
-  c->step.x_total = {d_feat, c->Q, d_mem_feat};
-  return forward_impl(c, d_feat, tops, st);
-}
-
+ * gradient term off.  m = 0 is npair_forward, by whose name its refusals go. */
 int npair_forward_memory(npair_ctx* c, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label, int32_t m,
                          float tops_host[5], void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !tops_host || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = memory_call_args(c, m)) != NPAIR_OK) return rc;
-  if (m == 0) return npair_forward(c, d_feat, d_label, tops_host, stream);
-  if ((rc = refuse_capture(c, stream, "npair_forward_memory")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_memory_rows(c, d_feat, d_label, d_mem_feat, d_mem_label, m, c->tops_dev, call.st)) != NPAIR_OK) return rc;
-  return finish_forward(c, tops_host, call.st);
+  return forward_call(c, m ? "npair_forward_memory" : "npair_forward", StepRows{DB_MEMORY, d_feat, d_label, d_mem_feat, d_mem_label, m},
+                      tops_host, nullptr, nullptr, 0.f, stream);
 }
 
 // A memory context captured into a graph holds the m of the capture: the tensor maps and the N-dependent plan of set_call_rows are
@@ -1021,15 +1058,19 @@ int npair_forward_memory_async(npair_ctx* c, const float* d_feat, const float* d
                                int32_t m, float* d_tops, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_feat || !d_label || !d_tops || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = memory_call_args(c, m)) != NPAIR_OK) return rc;
-  if (m == 0) return npair_forward_async(c, d_feat, d_label, d_tops, stream);
-  bool captured = false;
-  if ((rc = async_entry(c, stream, "npair_forward_memory_async", &captured)) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream, captured);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_memory_rows(c, d_feat, d_label, d_mem_feat, d_mem_label, m, &c->aw->tops, call.st)) != NPAIR_OK) return rc;
-  return finish_forward_async(c, d_tops, call.st);
+  return forward_call(c, m ? "npair_forward_memory_async" : "npair_forward_async",
+                      StepRows{DB_MEMORY, d_feat, d_label, d_mem_feat, d_mem_label, m}, nullptr, d_tops, nullptr, 0.f, stream);
+}
+
+/* Forward + backward with ONE host synchronisation: the backward (whose loss weight is a constant of the net, top[0]'s diff)
+ * is enqueued right behind the forward's kernels, then the call waits for the five tops.  Saves the host round trip between
+ * the two calls (the GPU idles for it: ~20 us of a 0.4 ms step at B = 8192).  Same results as npair_forward + npair_backward;
+ * when the forward reports an error the gradient buffer holds garbage and the context needs a new forward. */
+int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_label, float loss_weight, float* d_diff, float tops_host[5],
+                           void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !d_diff || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  return forward_call(c, "npair_forward_backward", StepRows{DB_OWN, d_feat, d_label}, tops_host, nullptr, d_diff, loss_weight, stream);
 }
 
 // What a kernel reads of rows [r0, r0 + rows) of the current step's S, which the S buffer holds from its row 0
@@ -1147,8 +1188,6 @@ static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cuda
   return NPAIR_OK;
 }
 
-// The loss weight of a backward: a host value, or (d_lw, world 1) one fp32 in device memory read in stream order
-struct LossWeight { float host; const float* dev; };
 static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
 // Backward_gpu (+ the projection of the fused L2Normalize producer: the kernels produce d loss / d y, the caller gets d loss / d x)
 static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
@@ -1163,58 +1202,42 @@ static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
 
 int npair_bwd_exchange_mode(const npair_ctx* c) { return c ? c->bwd_mode : NPAIR_E_ARG; }
 
-// The gradient kernels write their outputs with 8- and 16-byte stores, so every output pointer must be 16-byte aligned (cudaMalloc,
-// Caffe blobs and torch allocations are).  NULL passes: the callers test for it themselves.
-static int check_out_aligned(npair_ctx* c, const float* p, const char* name) {
-  if ((reinterpret_cast<uintptr_t>(p) & 15) == 0) return NPAIR_OK;
-  c->err = fmt("%s is not 16-byte aligned", name);
-  return NPAIR_E_ARG;
+// What a backward continues: the rank's step with the library's own exchange at world > 1, the external collectives' partial sums
+// (npair_backward_partial), or the world's row records the caller gathered (npair_backward_gathered)
+enum BackwardKind { BWD_OWN, BWD_PARTIAL, BWD_GATHERED };
+
+// Every backward entry after its null-pointer check: the preconditions, then the backward.  lw.dev: the asynchronous call.  d_total:
+// npair_backward_partial's addend of the all-reduce (world > 1); d_rs: npair_backward_gathered's N row records.
+static int backward_call(npair_ctx* c, const char* name, BackwardKind kind, LossWeight lw, float* d_diff, float* d_total,
+                         const RowRecord* d_rs, void* stream) {
+  int rc;
+  bool captured = false;
+  if (lw.dev && (rc = async_entry(c, stream, name, &captured)) != NPAIR_OK) return rc;
+  if ((rc = check_out_aligned(c, d_diff, kind == BWD_PARTIAL ? "d_local_half" : "the gradient pointer")) != NPAIR_OK) return rc;
+  if ((rc = check_out_aligned(c, d_total, "d_total_half")) != NPAIR_OK) return rc;
+  if ((rc = need_forward(c, name)) != NPAIR_OK) return rc;
+  if (kind == BWD_OWN && (rc = need_comm(c, "npair_backward_partial / npair_backward_gathered")) != NPAIR_OK) return rc;
+  if (kind == BWD_PARTIAL && c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) {
+    c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE;
+  }
+  if (kind == BWD_GATHERED && c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) {
+    c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE;
+  }
+  OrderedCall call(c, stream, captured);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  return backward_impl(c, lw, d_diff, d_total, d_rs, call.st);
 }
 
 int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_diff) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
-  if ((rc = need_forward(c, "npair_backward")) != NPAIR_OK) return rc;
-  if ((rc = need_comm(c, "npair_backward_partial / npair_backward_gathered")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, call.st);
+  return backward_call(c, "npair_backward", BWD_OWN, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, stream);
 }
 
 int npair_backward_device_weight(npair_ctx* c, const float* d_loss_weight, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_loss_weight || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  bool captured = false;
-  if ((rc = async_entry(c, stream, "npair_backward_device_weight", &captured)) != NPAIR_OK) return rc;
-  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
-  if ((rc = need_forward(c, "npair_backward_device_weight")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream, captured);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, LossWeight{0.f, d_loss_weight}, d_diff, nullptr, nullptr, call.st);
-}
-
-/* Forward + backward with ONE host synchronisation: the backward (whose loss weight is a constant of the net, top[0]'s diff)
- * is enqueued right behind the forward's kernels, then the call waits for the five tops.  Saves the host round trip between
- * the two calls (the GPU idles for it: ~20 us of a 0.4 ms step at B = 8192).  Same results as npair_forward + npair_backward;
- * when the forward reports an error the gradient buffer holds garbage and the context needs a new forward. */
-int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_label, float loss_weight, float* d_diff, float tops_host[5],
-                           void* stream) {
-  if (!c) return NPAIR_E_ARG;
-  if (!d_feat || !d_label || !d_diff || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
-  if ((rc = need_comm(c, "npair_forward_gathered")) != NPAIR_OK) return rc;
-  if ((rc = refuse_capture(c, stream, "npair_forward_backward")) != NPAIR_OK) return rc;
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  if ((rc = forward_rank(c, d_feat, d_label, c->tops_dev, call.st)) != NPAIR_OK) return rc;
-  if ((rc = backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, call.st)) != NPAIR_OK) return rc;
-  // wait for the forward's tops only: the gradient kernels keep running while the caller prepares (and enqueues) its next step.
-  // finish_forward records `done` behind the backward
-  return finish_forward(c, tops_host, call.st);
+  return backward_call(c, "npair_backward_device_weight", BWD_OWN, LossWeight{0.f, d_loss_weight}, d_diff, nullptr, nullptr, stream);
 }
 
 /* External-collectives variant of Backward_gpu up to the all-reduce (.cu:420-460):
@@ -1225,14 +1248,8 @@ int npair_forward_backward(npair_ctx* c, const float* d_feat, const float* d_lab
 int npair_backward_partial(npair_ctx* c, float loss_weight, float* d_local_half, float* d_total_half, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_local_half || (c->world > 1 && !d_total_half)) { c->err = "null gradient pointer"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = check_out_aligned(c, d_local_half, "d_local_half")) != NPAIR_OK) return rc;
-  if (c->world > 1 && (rc = check_out_aligned(c, d_total_half, "d_total_half")) != NPAIR_OK) return rc;
-  if ((rc = need_forward(c, "npair_backward_partial")) != NPAIR_OK) return rc;
-  if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE; }
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_local_half, c->world > 1 ? d_total_half : nullptr, nullptr, call.st);
+  return backward_call(c, "npair_backward_partial", BWD_PARTIAL, LossWeight{loss_weight, nullptr}, d_local_half,
+                       c->world > 1 ? d_total_half : nullptr, nullptr, stream);
 }
 
 int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
@@ -1248,13 +1265,8 @@ int npair_row_scalars(npair_ctx* c, float* d_out, void* stream) {
 int npair_backward_gathered(npair_ctx* c, float loss_weight, const float* d_rs_total, float* d_diff, void* stream) {
   if (!c) return NPAIR_E_ARG;
   if (!d_rs_total || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
-  int rc;
-  if ((rc = check_out_aligned(c, d_diff, "the gradient pointer")) != NPAIR_OK) return rc;
-  if ((rc = need_forward(c, "npair_backward_gathered")) != NPAIR_OK) return rc;
-  if (c->bwd_mode != NPAIR_BWDMODE_ROW_SCALARS) { c->err = "this context does not exchange row scalars (see npair_bwd_exchange_mode)"; return NPAIR_E_STATE; }
-  OrderedCall call(c, stream);
-  if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, LossWeight{loss_weight, nullptr}, d_diff, nullptr, reinterpret_cast<const RowRecord*>(d_rs_total), call.st);
+  return backward_call(c, "npair_backward_gathered", BWD_GATHERED, LossWeight{loss_weight, nullptr}, d_diff, nullptr,
+                       reinterpret_cast<const RowRecord*>(d_rs_total), stream);
 }
 
 // d_diff[rows x D] = sum of the gradient GEMM's split-K partial products (+ beta * d_diff)
@@ -1264,6 +1276,40 @@ static void reduce_splits(npair_ctx* c, int splits, int rows, float* d_diff, flo
   count_launch();
 }
 
+// The column records the gradient weights read and the weight builder's mode (BW_*).  The row-record exchange reads the world's N row
+// records: the caller's (d_rs_ext), the peers' pushed ones, or the NCCL all-gather's, enqueued at the step's first backward.  A memory
+// step reads its table of the Q row records and the memory rows' records.  Otherwise *rs_total is NULL: the rank's own records.
+static int column_records(npair_ctx* c, const RowRecord* d_rs_ext, const RowRecord** rs_total, int* bw_mode, cudaStream_t st) {
+  const int Q = c->Q;
+  *rs_total = nullptr;
+  *bw_mode = BW_SYM;
+  if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) {
+    *bw_mode = BW_ROWSCAL;
+    if (d_rs_ext) *rs_total = d_rs_ext;
+    else {
+      if (c->p2p_rec && !c->step.ext_gathered) {
+        PhaseTimer pt(c, 8, st);
+        *rs_total = reinterpret_cast<const RowRecord*>(p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st));
+      } else if (!c->step.rec_gathered) {
+        // the only backward exchange: Q row records per rank (replaces the N x D MPI_Allreduce of .cu:462-489); the callers without
+        // d_rs_ext checked for the communicator (need_comm)
+        PhaseTimer pt(c, 8, st);
+        NcclApi* api = nccl_api();
+        int r = api->AllGather(c->ra.rowrec, c->rs_total, ROW_RECORD_FLOATS * Q, NCCL_FLOAT32, c->comm, st);
+        if (r != 0) { c->err = fmt("ncclAllGather(row records): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
+        c->step.rec_gathered = true;
+        *rs_total = c->rs_total;
+      } else *rs_total = c->rs_total;
+    }
+  } else if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) *bw_mode = BW_SPLIT;
+  if (c->step.x_total.x1) {
+    // cross-batch memory: the table of the Q row records and the memory rows' records (RowRecord::memory), whose transposed terms
+    // are 0, so that the gradient is (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x) with nothing divided
+    *bw_mode = BW_ROWSCAL;
+    *rs_total = c->ra.rowrec;
+  }
+  return NPAIR_OK;
+}
 static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
@@ -1283,31 +1329,8 @@ static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
   const bool tc = c->cfg.gemm_backend == NPAIR_GEMM_TCGEN05;
   const RowRecord* rs_total = nullptr;
   int bw_mode = BW_SYM;
-  if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) {
-    bw_mode = BW_ROWSCAL;
-    if (d_rs_ext) rs_total = d_rs_ext;
-    else {
-      if (c->p2p_rec && !c->step.ext_gathered) {
-        PhaseTimer pt(c, 8, st);
-        rs_total = reinterpret_cast<const RowRecord*>(p2p_wait(c, XCHG_RECORDS, c->p2p_rec_epoch, XP_REC, st));
-      } else if (!c->step.rec_gathered) {
-        // the only backward exchange: Q row records per rank (replaces the N x D MPI_Allreduce of .cu:462-489); the callers without
-        // d_rs_ext checked for the communicator (need_comm)
-        PhaseTimer pt(c, 8, st);
-        NcclApi* api = nccl_api();
-        int r = api->AllGather(c->ra.rowrec, c->rs_total, ROW_RECORD_FLOATS * Q, NCCL_FLOAT32, c->comm, st);
-        if (r != 0) { c->err = fmt("ncclAllGather(row records): %s", api->GetErrorString(r)); return NPAIR_E_NCCL; }
-        c->step.rec_gathered = true;
-        rs_total = c->rs_total;
-      } else rs_total = c->rs_total;
-    }
-  } else if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) bw_mode = BW_SPLIT;
-  if (c->step.x_total.x1) {
-    // cross-batch memory: the table of the Q row records and the memory rows' records (RowRecord::memory), whose transposed terms
-    // are 0, so that the gradient is (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x) with nothing divided
-    bw_mode = BW_ROWSCAL;
-    rs_total = c->ra.rowrec;
-  }
+  const int rc = column_records(c, d_rs_ext, &rs_total, &bw_mode, st);
+  if (rc != NPAIR_OK) return rc;
   if (tc && c->fused_grad) {
     // weights are produced inside the gradient GEMM: no H in HBM
     FusedGradParams fp; memset(&fp, 0, sizeof(fp));
@@ -1429,13 +1452,10 @@ int npair_async_status(npair_ctx* c) {
   CUDA_TRY(c, cudaMemcpy(&err, &c->aw->err, sizeof(err), cudaMemcpyDeviceToHost));
   if (!err) return NPAIR_OK;
   CUDA_TRY(c, cudaMemset(&c->aw->err, 0, sizeof(err)));
-  if (err & DERR_EMPTY_LIST) { c->err = "an asynchronous forward indexed an empty same/diff list (undefined behaviour in the reference, .cu:296/:327/:288)"; return NPAIR_E_EMPTY_LIST; }
-  if (err & DERR_POS_RANGE) {
-    c->err = "an asynchronous forward's identsn/diffsn selected a position outside the list (undefined behaviour in the reference, .cu:285-288)";
-    return NPAIR_E_POS_RANGE;
-  }
-  c->err = "an asynchronous forward read an anchor weight (npair_set_anchor_io) outside [0, 1] or NaN";
-  return NPAIR_E_ARG;
+  const DeviceError* e = device_error(err);        // launch_async_tops adds the bits of DEVICE_ERRORS only
+  if (!e) { c->err = fmt("unknown asynchronous error bits 0x%x", err); return NPAIR_E_CUDA; }
+  c->err = e->async_msg;
+  return e->code;
 }
 
 __global__ void decode_ord_kernel(const uint32_t* __restrict__ in, float* __restrict__ out, int n) {
