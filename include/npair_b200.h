@@ -245,6 +245,35 @@ int npair_forward_memory_async(npair_ctx* ctx, const float* d_feat, const float*
 int npair_backward_device_weight(npair_ctx* ctx, const float* d_loss_weight, float* d_feat_diff, void* stream);
 int npair_async_status(npair_ctx* ctx);
 
+/* ---- cross-batch memory kept by the context (DESIGN 4.3.1) ----
+ * A memory context that owns the ring of its memory rows: M slots of fp32 rows and labels in device memory, and a 64-bit count of the
+ * rows pushed since the last load.  A ring forward takes m = min(count, M) memory rows, slots 0 .. m-1 in slot order, and gives every
+ * result of npair_forward_memory(_async) over those rows bit for bit (tops, S, the debug arrays, the row records, anchor weights and
+ * per-anchor losses, the backward after it).  Then it pushes the batch, in stream order on the device: the rows the layer used (x / ||x||
+ * under normalize_input) and the labels go to slots (count + i) mod M, a batch larger than M leaving its last M rows, and count += Q.
+ * The split operand pieces of the ring's rows stay in the context from step to step: a step re-splits only the rows pushed since their
+ * pieces were written, the tile at row Q + m when m changed, and all of them when the fp16x2 pre-scale changed.
+ *   npair_create_memory_ring / npair_memory_ring_workspace_bytes : refuse what npair_create_memory refuses; the ring starts empty
+ *   npair_forward_ring(_async) : the forward and the push.  On a ring context every other forward returns NPAIR_E_STATE, and a ring
+ *                                forward on another context does.  The backward entries follow as after npair_forward_memory.
+ *   npair_memory_ring_read     : the m valid slots' rows (m x D) and labels into d_rows / d_labels (M rows always suffice), and the
+ *                                count (one int64) into d_count, all in stream order
+ *   npair_memory_ring_load     : restores what a read wrote: min(count, M) rows and labels in slot order and the count; count = 0 is
+ *                                the reset (the pointers may then be NULL).  count < 0 is NPAIR_E_ARG.
+ * Capture.  A ring forward can be captured (npair_forward_ring_async) only when the ring is full, count >= M, so that every replay has
+ * m = M; before that it returns NPAIR_E_STATE before any CUDA call, with the rows still missing in the message.  Replays advance the
+ * ring on the device, and an eager ring forward after them continues from the device count.  A replay that finds count < M (a load
+ * with a smaller count since the capture) reads and writes no slot, gives NaN tops and keeps an error for npair_async_status
+ * (NPAIR_E_STATE).  Read and load return NPAIR_E_STATE on a capturing stream.
+ * npair_debug_read(13): the 32-row database tiles (rows 32 t .. 32 t + 31 of [x; ring]) the last ring forward re-split from the ring,
+ * past the batch's own tiles: their number k, then the k tile indices ascending (n >= k + 1). */
+int npair_create_memory_ring(const npair_config* cfg, int32_t max_memory_rows, npair_ctx** out);
+size_t npair_memory_ring_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows);
+int npair_forward_ring(npair_ctx* ctx, const float* d_feat, const float* d_label, float tops_host[5], void* stream);
+int npair_forward_ring_async(npair_ctx* ctx, const float* d_feat, const float* d_label, float* d_tops, void* stream);
+int npair_memory_ring_read(npair_ctx* ctx, float* d_rows, float* d_labels, int64_t* d_count, void* stream);
+int npair_memory_ring_load(npair_ctx* ctx, const float* d_rows, const float* d_labels, int64_t count, void* stream);
+
 /* ---- per-anchor loss weights and per-anchor losses (DESIGN 4.5; not part of the reference layer) ----
  * The next forwards of this context read Q anchor weights in [0, 1] from d_anchor_weight and write the Q per-anchor losses
  * (-log(A_i/T_i), unweighted) to d_row_loss, in stream order.  Either may be NULL (unweighted / not written); the pointers
@@ -298,6 +327,7 @@ int npair_util_f32_to_f64(const float* d_src, double* d_dst, size_t n, void* str
  *        3 = min_within[Q]  4 = max_between[Q]  5 = max_all[Q]  6 = A[Q]  7 = T[Q]  8 = same-label count[Q]
  *        9 = max_within[Q]  10 = operand pre-scale (1 float)  11 = log(A/T)[Q] (0 where A or T is 0)
  *        12 = retrieval hit flags [3][Q] for k = 1, 5, 10, as 0 / 1
+ *        13 = the ring tiles the last ring forward re-split (count, then the tiles; npair_forward_ring, NPAIR_E_STATE on other contexts)
  * Statistics of a row with no same-label column keep their reset values: min_within FLT_MAX, max_within -FLT_MAX, count 0 (and
  * max_between -FLT_MAX with no diff-label column).  A and T are fp32 sums of ex2.approx.ftz(s log2(e) - max_all log2(e)) over the
  * selected pairs: a term below 2^-126 is 0 (DESIGN 5). */

@@ -44,6 +44,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_debug_gemm", "npair_debug_mma_symmetric", "npair_l2normalize_forward", "npair_l2normalize_backward",
            # cross-batch memory (not part of the reference layer)
            "npair_create_memory", "npair_memory_workspace_bytes", "npair_forward_memory",
+           "npair_create_memory_ring", "npair_memory_ring_workspace_bytes", "npair_forward_ring", "npair_forward_ring_async",
+           "npair_memory_ring_read", "npair_memory_ring_load",
            # asynchronous step and graph capture (not part of the reference layer)
            "npair_forward_async", "npair_forward_memory_async", "npair_backward_device_weight", "npair_async_status",
            # per-anchor loss weights and losses (not part of the reference layer)
@@ -90,6 +92,13 @@ def lib():
         L.npair_memory_workspace_bytes.argtypes = [C.POINTER(NpairConfig), C.c_int32]
         L.npair_memory_workspace_bytes.restype = C.c_size_t
         L.npair_forward_memory.argtypes = [vp, vp, vp, vp, vp, C.c_int32, fp, vp]
+        L.npair_create_memory_ring.argtypes = [C.POINTER(NpairConfig), C.c_int32, C.POINTER(vp)]
+        L.npair_memory_ring_workspace_bytes.argtypes = [C.POINTER(NpairConfig), C.c_int32]
+        L.npair_memory_ring_workspace_bytes.restype = C.c_size_t
+        L.npair_forward_ring.argtypes = [vp, vp, vp, fp, vp]
+        L.npair_forward_ring_async.argtypes = [vp, vp, vp, vp, vp]
+        L.npair_memory_ring_read.argtypes = [vp, vp, vp, vp, vp]
+        L.npair_memory_ring_load.argtypes = [vp, vp, vp, C.c_int64, vp]
         L.npair_backward.argtypes = [vp, C.c_float, vp, vp]
         L.npair_forward_backward.argtypes = [vp, vp, vp, C.c_float, vp, fp, vp]
         L.npair_set_anchor_io.argtypes = [vp, vp, vp]
@@ -184,22 +193,31 @@ def nccl_unique_id() -> bytes:
     return buf.raw
 
 
-def memory_workspace_bytes(cfg: NpairConfig, memory_rows: int) -> int:
-    """Device bytes a Context(cfg, memory_rows=memory_rows) allocates (npair_memory_workspace_bytes; 0 for a refused configuration)."""
-    return int(lib().npair_memory_workspace_bytes(C.byref(cfg), int(memory_rows)))
+def memory_workspace_bytes(cfg: NpairConfig, memory_rows: int, ring: bool = False) -> int:
+    """Device bytes a Context(cfg, memory_rows=memory_rows, ring=ring) allocates (npair_memory_workspace_bytes /
+    npair_memory_ring_workspace_bytes; 0 for a refused configuration)."""
+    f = lib().npair_memory_ring_workspace_bytes if ring else lib().npair_memory_workspace_bytes
+    return int(f(C.byref(cfg), int(memory_rows)))
 
 
 class Context:
     """One per rank.  forward()/backward() take torch CUDA tensors (device pointers) and return host scalars.
-    memory_rows > 0: a cross-batch memory context (npair_create_memory, DESIGN 4.3) whose forward_memory takes up to that many rows."""
+    memory_rows > 0: a cross-batch memory context (npair_create_memory, DESIGN 4.3) whose forward_memory takes up to that many rows.
+    ring=True: a context that keeps its memory ring of memory_rows slots itself (npair_create_memory_ring, DESIGN 4.3.1): forward_ring,
+    forward_ring_async, ring_read and ring_load."""
 
-    def __init__(self, cfg: NpairConfig, nccl_id: bytes | None = None, memory_rows: int = 0):
+    def __init__(self, cfg: NpairConfig, nccl_id: bytes | None = None, memory_rows: int = 0, ring: bool = False):
         L = lib()
         self.cfg = cfg
         self.memory_rows = int(memory_rows)
+        self.ring = bool(ring)
         self._h = C.c_void_p()
         idbuf = C.create_string_buffer(nccl_id, 128) if nccl_id is not None else None
-        if self.memory_rows > 0:
+        if self.ring:
+            if nccl_id is not None:
+                raise ValueError("a cross-batch memory context is a world-1 context: it takes no NCCL id")
+            rc = L.npair_create_memory_ring(C.byref(cfg), self.memory_rows, C.byref(self._h))
+        elif self.memory_rows > 0:
             if nccl_id is not None:
                 raise ValueError("a cross-batch memory context is a world-1 context: it takes no NCCL id")
             rc = L.npair_create_memory(C.byref(cfg), self.memory_rows, C.byref(self._h))
@@ -280,6 +298,37 @@ class Context:
                                                      _ptr(tops_out, "tops_out", 5), _stream()))
         return tops_out
 
+    # ---- the context's own memory ring (ring=True, DESIGN 4.3.1) ----
+    def forward_ring(self, feat, label):
+        """npair_forward_ring: forward_memory over the ring's min(count, M) slots, then the batch's rows go into the ring."""
+        tops = (C.c_float * 5)()
+        self._check(lib().npair_forward_ring(self._h, *self._rows(feat, label), tops, _stream()))
+        return [tops[i] for i in range(5)]
+
+    def forward_ring_async(self, feat, label, tops_out):
+        """npair_forward_ring_async: forward_ring with the tops written to tops_out as in forward_async; capturable once the ring is
+        full."""
+        self._check(lib().npair_forward_ring_async(self._h, *self._rows(feat, label), _ptr(tops_out, "tops_out", 5), _stream()))
+        return tops_out
+
+    def ring_read(self, rows, labels, count):
+        """npair_memory_ring_read: the valid slots into rows [M, D] and labels [M] (the first min(count, M) of each), and the push count
+        into count, a one-element CUDA int64 tensor; all in stream order."""
+        import torch
+        if not (isinstance(count, torch.Tensor) and count.is_cuda and count.dtype == torch.int64 and count.numel() >= 1):
+            raise TypeError("count must be a CUDA int64 tensor of one element")
+        M, D = self.memory_rows, self.cfg.D
+        self._check(lib().npair_memory_ring_read(self._h, _ptr(rows, "rows", M * D), _ptr(labels, "labels", M), count.data_ptr(),
+                                                 _stream()))
+
+    def ring_load(self, rows, labels, count):
+        """npair_memory_ring_load: restores min(count, M) rows and labels in slot order and the push count (a host int); count = 0
+        (rows and labels may be None) empties the ring."""
+        count = int(count)
+        m = min(max(count, 0), self.memory_rows)
+        ptrs = (None, None) if rows is None else (_ptr(rows, "rows", m * self.cfg.D), _ptr(labels, "labels", m))
+        self._check(lib().npair_memory_ring_load(self._h, *ptrs, count, _stream()))
+
     def backward_device_weight(self, loss_weight, diff):
         """npair_backward_device_weight: backward with the loss weight read on the device from loss_weight (a one-element CUDA fp32
         tensor), with the gradient bits of backward(float(loss_weight))."""
@@ -337,7 +386,8 @@ class Context:
         return [ms[i] for i in range(9)]
 
     def debug_read(self, which: int, n: int):
-        """npair_debug_read: n floats of introspection array `which` (0 = S, Q x N; 12 = the hit flags, 3 x Q; 10 = one float; else Q)."""
+        """npair_debug_read: n floats of introspection array `which` (0 = S, Q x N; 12 = the hit flags, 3 x Q; 10 = one float; 13 = the
+        count k of ring tiles the last ring forward re-split, then the k tiles; else Q)."""
         import numpy as np
         out = np.zeros(n, dtype=np.float32)
         self._check(lib().npair_debug_read(self._h, which, out.ctypes.data_as(C.POINTER(C.c_float)), n))

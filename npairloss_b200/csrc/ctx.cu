@@ -363,6 +363,9 @@ struct npair_ctx : Plan, CallPlan {
   int mem_cap = 0;               // cross-batch memory: the most memory rows a call may pass (npair_create_memory), 0 without
   int mem_rows = 0;              // the memory rows the CallPlan and the tensor maps are set for (set_call_rows)
   float* labcat = nullptr;       // memory context: the labels of the current rows and the memory rows, [Q + M]
+  bool ring = false;             // the memory rows are the context's own ring (npair_create_memory_ring, DESIGN 4.3.1)
+  Ring rg{};                     // its buffers, rg.M = mem_cap
+  long long ring_count = 0;      // rows pushed since the last load as the host enqueued them; exact below M (a capture needs >= M)
   DevMem mem;                    // owns the device scratch below (ctx_buffers, p2p_buffers)
   float* Xtot_buf = nullptr;     // world > 1: all-gather target
   float* labtot_buf = nullptr;
@@ -421,11 +424,21 @@ struct npair_ctx : Plan, CallPlan {
   bool ev_used[NPAIR_PROF_PHASES] = {};
 };
 
+// 32-row tiles of the database rows [0, Q + M) of a ring context (RING_TILE)
+static long long ring_tiles(long long Q, long long M) { return (Q + M + RING_TILE - 1) / RING_TILE; }
+
 // The device buffers of a context with its configuration and plan, each with its size and zero-fill; returns the first failure
 static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   const long long Q = c->cfg.Q, D = c->cfg.D, N = c->N;
   const size_t f = sizeof(float), ns = c->nsplit;
   if (c->mem_cap) m.own(&c->labcat, f * N, false);                                      // [x; x_mem]'s labels
+  if (c->ring) {                                                                         // the memory ring, slot s = database row Q + s
+    const long long M = c->mem_cap, tiles = ring_tiles(Q, M);
+    m.own(&c->rg.x, f * M * D, false); m.own(&c->rg.label, f * M, true); m.own(&c->rg.rowmax, f * M, false);
+    m.own(&c->rg.dirty, sizeof(int) * tiles, true); m.own(&c->rg.list, sizeof(int) * tiles, false);
+    m.own(&c->rg.st, sizeof(RingState), true);
+    c->rg.M = c->mem_cap;
+  }
   if (c->cfg.world > 1) { m.own(&c->Xtot_buf, f * N * D, false); m.own(&c->labtot_buf, f * N, false); }   // all-gather targets
   if (c->cfg.normalize_input) { m.own(&c->Ynorm, f * Q * D, false); m.own(&c->dY, f * Q * D, false); m.own(&c->inv_norm, f * Q, false); }   // y, dy, 1/||x||
   m.own(&c->S, f * c->s_rows * c->ldS, true);
@@ -542,12 +555,12 @@ void npair_config_default(npair_config* c, int32_t Q, int32_t D) {
   c->global_scope = 0; c->normalize_input = 0; c->grad_chunk_cols = 0; c->flags = 0;
 }
 
-size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows) {
+static size_t workspace_bytes(const npair_config* cfg, int32_t max_memory_rows, bool ring) {
   std::string e;
   if (validate(cfg, &e) != NPAIR_OK || validate_memory(cfg, max_memory_rows, &e) != NPAIR_OK) return 0;
   npair_ctx c;
   c.cfg = *cfg; c.sms = NPAIR_H100_SXM_SMS;
-  c.mem_cap = max_memory_rows;
+  c.mem_cap = max_memory_rows; c.ring = ring;
   static_cast<Plan&>(c) = plan_of(*cfg, c.sms, true, max_memory_rows);
   static_cast<CallPlan&>(c) = call_plan(*cfg, c, c.sms, max_memory_rows);
   DevMem sizing(false);
@@ -555,6 +568,8 @@ size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_
   if (c.want_p2p_feat || c.want_p2p_rec) p2p_buffers(&c, sizing);   // as if the context had a communicator and peer access
   return sizing.bytes;
 }
+size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows) { return workspace_bytes(cfg, max_memory_rows, false); }
+size_t npair_memory_ring_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows) { return workspace_bytes(cfg, max_memory_rows, true); }
 size_t npair_workspace_bytes(const npair_config* cfg) { return npair_memory_workspace_bytes(cfg, 0); }
 
 const char* npair_last_error(const npair_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
@@ -581,7 +596,7 @@ void npair_destroy(npair_ctx* c) {
   delete c;
 }
 
-static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out);
+static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out, bool ring = false);
 // One-off device check (per process, device and operand format): a 192 x 192 similarity matrix computed with EVERY tile (no mirroring)
 // must come out bitwise symmetric.
 static bool mma_is_symmetric(int prec, int device) {
@@ -669,7 +684,7 @@ static int set_call_rows(npair_ctx* c, int m) {
   return NPAIR_OK;
 }
 
-static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out) {
+static int create_impl(const npair_config* cfg, const void* id128, void* ext_comm, int mem_cap, npair_ctx** out, bool ring) {
   if (!out) { g_create_err = "null out"; return NPAIR_E_ARG; }
   *out = nullptr;
   std::string e;
@@ -680,7 +695,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
   if ((rc = open_device(cfg->device, &device, &sms)) != NPAIR_OK) return rc;
   std::unique_ptr<npair_ctx, void (*)(npair_ctx*)> made(new npair_ctx(), npair_destroy);   // until it is handed out
   npair_ctx* c = made.get();
-  c->cfg = *cfg; c->device = device; c->sms = sms; c->mem_cap = mem_cap; c->mem_rows = mem_cap;
+  c->cfg = *cfg; c->device = device; c->sms = sms; c->mem_cap = mem_cap; c->mem_rows = mem_cap; c->ring = ring;
   // only the multi-rank row-record backward on the tensor cores and the row-block similarity mode depend on the check, which itself
   // creates a single-rank context
   const bool blocks = sim_block_rows(*cfg) > 0;
@@ -776,6 +791,9 @@ int npair_create_with_comm(const npair_config* cfg, void* comm, npair_ctx** out)
 int npair_create_memory(const npair_config* cfg, int32_t max_memory_rows, npair_ctx** out) {
   return create_impl(cfg, nullptr, nullptr, max_memory_rows, out);
 }
+int npair_create_memory_ring(const npair_config* cfg, int32_t max_memory_rows, npair_ctx** out) {
+  return create_impl(cfg, nullptr, nullptr, max_memory_rows, out, true);
+}
 
 // Peer-memory exchange of `kind`: pushes this rank's nA floats of srcA (and nB of srcB) into part partA (partB) of every rank's
 // region, in the buffers of the epoch's parity, then raises this rank's flag of (kind, parity) in every region.
@@ -822,6 +840,9 @@ static MiningParams mining_of(const npair_config& c) {
 // return code, and the message of a synchronous forward and of npair_async_status
 struct DeviceError { int bit, code; const char *sync_msg, *async_msg; };
 static const DeviceError DEVICE_ERRORS[] = {
+  // first: the step ran over slots it did not fill, so whatever else its kernels found is a consequence
+  {DERR_RING_NOT_FULL, NPAIR_E_STATE, "the memory ring held fewer rows than the forward was enqueued for",
+   "a replayed ring forward found the memory ring not full (npair_memory_ring_load with count < max_memory_rows after the capture)"},
   {DERR_EMPTY_LIST, NPAIR_E_EMPTY_LIST, "an empty same/diff list was indexed (undefined behaviour in the reference, .cu:296/:327/:288)",
    "an asynchronous forward indexed an empty same/diff list (undefined behaviour in the reference, .cu:296/:327/:288)"},
   {DERR_POS_RANGE, NPAIR_E_POS_RANGE, "identsn/diffsn select a position outside the list (undefined behaviour in the reference, .cu:285-288)",
@@ -946,6 +967,7 @@ struct StepRows {
   const float *x, *label;
   const float *x_mem = nullptr, *label_mem = nullptr;
   int m = 0;
+  bool ring = false;             // a DB_MEMORY step over the context's ring (npair_forward_ring)
 };
 
 // Starts a forward's step: the plan of its database size, a fresh Step, the fused L2Normalize producer (usage/def.prototxt:115-120)
@@ -992,6 +1014,16 @@ static int begin_step(npair_ctx* c, const StepRows& in, const float** anchors, c
 static int forward_call(npair_ctx* c, const char* name, const StepRows& rows, float* tops_host, float* d_tops, float* d_diff,
                         float loss_weight, void* stream) {
   int rc;
+  if (rows.ring != c->ring) {                 // a ring forward would find no ring; any other would overwrite the ring's cached pieces
+    c->err = rows.ring ? fmt("%s needs a context from npair_create_memory_ring", name)
+                       : fmt("%s: this context keeps its memory ring (npair_create_memory_ring): use npair_forward_ring(_async)", name);
+    return NPAIR_E_STATE;
+  }
+  if (rows.ring && c->ring_count < c->mem_cap && capture_id(static_cast<cudaStream_t>(stream))) {   // every replay must find m = M
+    c->err = fmt("%s: a ring forward can be captured once the ring is full: it holds %lld of %d rows, %lld more to push eagerly", name,
+                 c->ring_count, c->mem_cap, c->mem_cap - c->ring_count);
+    return NPAIR_E_STATE;
+  }
   if (rows.db == DB_MEMORY) {                 // a memory context's configuration, and at most its M memory rows
     if ((rc = validate_memory(&c->cfg, 1, &c->err)) != NPAIR_OK) return rc;
     if (rows.m < 0 || rows.m > c->mem_cap) { c->err = fmt("m = %d memory rows outside [0, %d] (npair_create_memory)", rows.m, c->mem_cap); return NPAIR_E_ARG; }
@@ -1015,6 +1047,7 @@ static int forward_call(npair_ctx* c, const char* name, const StepRows& rows, fl
   if (tops_host) return finish_forward(c, tops_host, st);
   // asynchronous: the tops and error bits go from the device TopsBlock to d_tops and the error word in stream order
   launch_async_tops(c->aw, c->cfg.num_tops, d_tops, st);
+  if (c->ring) launch_ring_tops(c->aw, d_tops, st);
   CUDA_TRY(c, cudaGetLastError());
   c->step.fwd_done = true;
   return NPAIR_OK;
@@ -1060,6 +1093,64 @@ int npair_forward_memory_async(npair_ctx* c, const float* d_feat, const float* d
   if (!d_feat || !d_label || !d_tops || (m > 0 && (!d_mem_feat || !d_mem_label))) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   return forward_call(c, m ? "npair_forward_memory_async" : "npair_forward_async",
                       StepRows{DB_MEMORY, d_feat, d_label, d_mem_feat, d_mem_label, m}, nullptr, d_tops, nullptr, 0.f, stream);
+}
+
+/* Cross-batch memory kept by the context (DESIGN 4.3.1): npair_forward_memory over the ring's m = min(count, M) slots in slot order,
+ * then the batch's rows the layer used and its labels go into the ring. */
+static StepRows ring_step_rows(npair_ctx* c, const float* d_feat, const float* d_label) {
+  const int m = static_cast<int>(c->ring_count < c->mem_cap ? c->ring_count : c->mem_cap);
+  return StepRows{DB_MEMORY, d_feat, d_label, c->rg.x, c->rg.label, m, true};
+}
+int npair_forward_ring(npair_ctx* c, const float* d_feat, const float* d_label, float tops_host[5], void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !tops_host) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  return forward_call(c, "npair_forward_ring", ring_step_rows(c, d_feat, d_label), tops_host, nullptr, nullptr, 0.f, stream);
+}
+int npair_forward_ring_async(npair_ctx* c, const float* d_feat, const float* d_label, float* d_tops, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_feat || !d_label || !d_tops) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  return forward_call(c, "npair_forward_ring_async", ring_step_rows(c, d_feat, d_label), nullptr, d_tops, nullptr, 0.f, stream);
+}
+
+// The preconditions of npair_memory_ring_read / _load: a ring context, and no capture (the host count would not follow a replay)
+static int ring_entry(npair_ctx* c, void* stream, const char* call) {
+  if (!c->ring) { c->err = fmt("%s needs a context from npair_create_memory_ring", call); return NPAIR_E_STATE; }
+  if (capture_id(static_cast<cudaStream_t>(stream))) { c->err = fmt("%s cannot be captured into a CUDA graph", call); return NPAIR_E_STATE; }
+  return NPAIR_OK;
+}
+int npair_memory_ring_read(npair_ctx* c, float* d_rows, float* d_labels, int64_t* d_count, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_rows || !d_labels || !d_count) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = ring_entry(c, stream, "npair_memory_ring_read")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const long long m = c->ring_count < c->mem_cap ? c->ring_count : c->mem_cap;
+  if (m) {
+    CUDA_TRY(c, cudaMemcpyAsync(d_rows, c->rg.x, sizeof(float) * m * c->D, cudaMemcpyDeviceToDevice, call.st));
+    CUDA_TRY(c, cudaMemcpyAsync(d_labels, c->rg.label, sizeof(float) * m, cudaMemcpyDeviceToDevice, call.st));
+  }
+  CUDA_TRY(c, cudaMemcpyAsync(d_count, &c->rg.st->count, sizeof(int64_t), cudaMemcpyDeviceToDevice, call.st));
+  return NPAIR_OK;
+}
+int npair_memory_ring_load(npair_ctx* c, const float* d_rows, const float* d_labels, int64_t count, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (count < 0) { c->err = "count must be >= 0"; return NPAIR_E_ARG; }
+  if (count > 0 && (!d_rows || !d_labels)) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  int rc;
+  if ((rc = ring_entry(c, stream, "npair_memory_ring_load")) != NPAIR_OK) return rc;
+  OrderedCall call(c, stream);
+  if ((rc = call.enter()) != NPAIR_OK) return rc;
+  const long long m = count < c->mem_cap ? count : c->mem_cap;
+  if (m) {
+    CUDA_TRY(c, cudaMemcpyAsync(c->rg.x, d_rows, sizeof(float) * m * c->D, cudaMemcpyDeviceToDevice, call.st));
+    CUDA_TRY(c, cudaMemcpyAsync(c->rg.label, d_labels, sizeof(float) * m, cudaMemcpyDeviceToDevice, call.st));
+  }
+  launch_ring_loaded(c->rg, static_cast<int>(m), c->D, static_cast<int>(ring_tiles(c->Q, c->mem_cap)), static_cast<unsigned long long>(count),
+                     call.st);
+  CUDA_TRY(c, cudaGetLastError());
+  c->ring_count = count;
+  return NPAIR_OK;
 }
 
 /* Forward + backward with ONE host synchronisation: the backward (whose loss weight is a constant of the net, top[0]'s diff)
@@ -1110,8 +1201,17 @@ static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cuda
     PhaseTimer pt(c, 1, st);
     const RowSource& xt = c->step.x_total;     // cross-batch memory: rows [Q, N) are the caller's memory rows, read where they lie
     if (xt.x1) launch_memory_rows(c->step.label, Q, c->step.lab_mem, N - Q, c->labcat, c->ra.rowrec, st);
-    launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, xt, N, D, c->partial, c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
-    launch_split(xt, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    if (c->ring) {
+      // the ring's rows: their max |x| from the slots' row maxima, and only their stale tiles re-split; then, with nothing left to read
+      // the fp32 slots, this batch's rows go in (their pieces are written by the next step's split: the backward reads the old ones)
+      launch_ring_prep(d_feat, Q, D, c->rg, N - Q, c->partial, c->prec == PREC_FP16X2 ? 1 : 0, c->ra, c->bs, st);
+      launch_ring_split(d_feat, Q, D, c->rg, N - Q, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XcatA, c->XcatB, c->Dp, c->sms, st);
+      launch_ring_push(d_feat, c->step.label, Q, D, c->rg, st);
+      c->ring_count += Q;
+    } else {
+      launch_prep_reduce(d_feat, static_cast<long long>(Q) * D, xt, N, D, c->partial, c->prec == PREC_FP16X2 ? 1 : 0, c->ra, Q, c->bs, st);
+      launch_split(xt, N, D, c->prec, c->bs, c->Xs, c->Dp, c->XsT, c->Np, c->XlT, c->Qp, self_off, Q, c->XcatA, c->XcatB, c->Dp, st);
+    }
   }
   // ---- S = X_local . X_total^T (.cu:218) with fused masks + row statistics (.cu:44-66, :225-265) over all Q rows; S is stored
   //      only when it is materialised, and is then block 0 of the row pass ----
@@ -1477,6 +1577,17 @@ int npair_debug_read(npair_ctx* c, int which, float* dst, size_t n) {
     if (c->n_blocks > 1) { c->err = "row-block similarity mode: S is never held whole"; return NPAIR_E_STATE; }
     if (n < static_cast<size_t>(Q) * N) { c->err = "buffer too small"; return NPAIR_E_ARG; }
     CUDA_TRY(c, cudaMemcpy2D(dst, sizeof(float) * N, c->S, sizeof(float) * c->ldS, sizeof(float) * N, Q, cudaMemcpyDeviceToHost));
+    return NPAIR_OK;
+  }
+  if (which == 13) {                               // the ring tiles the last ring forward re-split: their count, then the tiles
+    if (!c->ring) { c->err = "debug_read(13) needs a context from npair_create_memory_ring"; return NPAIR_E_STATE; }
+    int k = 0;
+    CUDA_TRY(c, cudaMemcpy(&k, &c->rg.st->n_list, sizeof(int), cudaMemcpyDeviceToHost));
+    if (n < static_cast<size_t>(k) + 1) { c->err = "buffer too small"; return NPAIR_E_ARG; }
+    std::vector<int> t(k);
+    if (k) CUDA_TRY(c, cudaMemcpy(t.data(), c->rg.list, sizeof(int) * k, cudaMemcpyDeviceToHost));
+    dst[0] = static_cast<float>(k);
+    for (int i = 0; i < k; ++i) dst[1 + i] = static_cast<float>(t[i]);
     return NPAIR_OK;
   }
   if (which == 10) {

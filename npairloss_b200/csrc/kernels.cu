@@ -128,6 +128,50 @@ __global__ void __launch_bounds__(256, 8) prep_reduce_kernel(const float* __rest
     bs->n_same = 0; bs->n_diff = 0;
   }
 }
+// prep_reduce_kernel's two reductions for ring_prep_kernel, the same operations in the same order (prep_reduce_kernel keeps its own
+// copy: calling these from it changes its register allocation).  The block totals: partial[block] = the block's sum and
+// partial[1024 + block] its max; true in the last block to finish (ticket), which then finishes the step's prep in prep_finish
+__device__ __forceinline__ bool prep_block_done(float sum, float mx, float* __restrict__ partial, BlockScalars* bs, float (&s_sum)[8],
+                                                float (&s_max)[8]) {
+  __shared__ int s_last;
+  sum = warp_sum(sum); mx = warp_max(mx);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { s_sum[w] = sum; s_max[w] = mx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    sum = 0.f; mx = 0.f;
+    for (int k = 0; k < (blockDim.x >> 5); ++k) { sum += s_sum[k]; mx = fmaxf(mx, s_max[k]); }
+    partial[blockIdx.x] = sum; partial[1024 + blockIdx.x] = mx;
+    __threadfence();
+    s_last = (atomicAdd(&bs->ticket0, 1u) == gridDim.x - 1) ? 1 : 0;
+  }
+  __syncthreads();
+  return s_last != 0;
+}
+// The last block: the asum and max |x| over the blocks' partials, the power-of-two operand scale and the reset of the step state
+__device__ __forceinline__ void prep_finish(const float* __restrict__ partial, int want_scale, BlockScalars* bs, float (&s_max)[8]) {
+  __threadfence();
+  __shared__ double s_dsum[8];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  double dsum = 0.0; float mx = 0.f;
+  for (int b = threadIdx.x; b < static_cast<int>(gridDim.x); b += blockDim.x) { dsum += __ldcg(&partial[b]); mx = fmaxf(mx, __ldcg(&partial[1024 + b])); }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { dsum += __shfl_xor_sync(0xffffffffu, dsum, o); mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o)); }
+  if (l == 0) { s_dsum[w] = dsum; s_max[w] = mx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    dsum = 0.0; mx = 0.f;
+    for (int k = 0; k < (blockDim.x >> 5); ++k) { dsum += s_dsum[k]; mx = fmaxf(mx, s_max[k]); }
+    bs->asum = static_cast<float>(dsum);
+    bs->x_absmax = mx;
+    float sc = 1.f, inv = 1.f;
+    if (want_scale) { const PreScale ps = pre_scale(mx); sc = ps.scale; inv = ps.inv; }
+    bs->x_scale = sc; bs->x_inv_scale = inv;
+    bs->err = 0; bs->ticket = 0; bs->ticket2 = 0; bs->ticket0 = 0; bs->ticket3 = 0; bs->sel_active[0] = 0; bs->sel_active[1] = 0;
+    bs->cand_n[0] = 0; bs->cand_n[1] = 0;
+    bs->n_same = 0; bs->n_diff = 0;
+  }
+}
 void launch_prep_reduce(const float* x_local, long long n_local, RowSource db, int N, int D, float* partial,
                         int want_scale, RowArrays ra, int Q, BlockScalars* bs, cudaStream_t st) {
   const long long n_total = static_cast<long long>(N) * D, nmax = n_local > n_total ? n_local : n_total;
@@ -262,6 +306,162 @@ void launch_split(RowSource db, int N, int D, int prec, const BlockScalars* bs, 
   dim3 grid((D + 63) / 64, (N + 31) / 32);
   const SplitArgs a{db, N, D, Xs, ldXs, XsT, ldXsT, XlT, ldXlT, row0_local, Q, XcatA, XcatB, Dp};
   with_prec(prec, [&](auto P) { split_kernel<P><<<grid, 256, 0, st>>>(a, bs); });
+  count_launch();
+}
+
+// --------------------------------------------------------------------------------------------
+// cross-batch memory ring (npair_create_memory_ring, DESIGN 4.3.1)
+// --------------------------------------------------------------------------------------------
+// m = min(count, M), the memory rows a ring step over the device count would take
+__device__ __forceinline__ int ring_rows(const Ring& r) {
+  const unsigned long long c = r.st->count;
+  return c < static_cast<unsigned long long>(r.M) ? static_cast<int>(c) : r.M;
+}
+// prep_reduce_kernel over [x; ring[0, m)] with the memory rows' max |x| taken from the slots' row maxima (a maximum has the same bits in
+// any order, and each row maximum is the fmaxf of the same |x| values), on the grid launch_prep_reduce gives Q + m rows.  The last block
+// then plans the step's refresh of the ring's operand pieces: the ring tiles [bt, nt) that split_tile must rewrite so that every
+// piece equals what launch_split writes for this step's N = Q + m at this step's pre-scale.
+__global__ void __launch_bounds__(256) ring_prep_kernel(const float* __restrict__ xl, int Q, int D, Ring r, int m, float* __restrict__ partial,
+                                                        int want_scale, RowArrays ra, BlockScalars* bs) {
+  __shared__ float s_sum[8], s_max[8];
+  const bool bad = ring_rows(r) != m;
+  float sum = 0.f, mx = 0.f;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  abs_sum_max_at(xl, static_cast<long long>(Q) * D, t0, stride, want_scale != 0, sum, mx);
+  if (want_scale && !bad)
+    for (long long i = t0; i < m; i += stride) mx = fmaxf(mx, __ldg(r.rowmax + i));
+  for (long long i = t0; i < Q; i += stride) reset_row_stats(ra, i);
+  if (!prep_block_done(sum, mx, partial, bs, s_sum, s_max)) return;
+  prep_finish(partial, want_scale, bs, s_max);
+  __syncthreads();
+  RingState* rs = r.st;
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  if (bad) {                                   // no slot is read, split or written this step
+    if (t == 0) { rs->bad = 1; rs->n_list = 0; bs->err = DERR_RING_NOT_FULL; }
+    return;
+  }
+  const float scale = *reinterpret_cast<volatile float*>(&bs->x_scale);
+  const int bt = (Q + RING_TILE - 1) / RING_TILE, nt = (Q + m + RING_TILE - 1) / RING_TILE;
+  const bool full = !rs->valid || rs->cached_scale != scale;
+  const int boundary = m != rs->cached_m ? (Q + m - 1) / RING_TILE : -1;   // its rows past Q + m are zeros in the pieces
+  __shared__ int s_cnt[8], s_base;
+  if (t == 0) s_base = 0;
+  for (int k0 = 0; k0 < nt; k0 += blockDim.x) {
+    const int k = k0 + t;
+    bool take = false;
+    if (k < nt) {                              // every tile below nt is current after this step's split
+      const int d = r.dirty[k];
+      take = k >= bt && (full || d || k == boundary);
+      if (d) r.dirty[k] = 0;
+    }
+    const unsigned int b = __ballot_sync(0xffffffffu, take);
+    if (lane == 0) s_cnt[w] = __popc(b);
+    __syncthreads();
+    int off = s_base;
+    for (int j = 0; j < w; ++j) off += s_cnt[j];
+    if (take) r.list[off + __popc(b & ((1u << lane) - 1u))] = k;
+    __syncthreads();
+    if (t == 0) for (int j = 0; j < (blockDim.x >> 5); ++j) s_base += s_cnt[j];
+    __syncthreads();
+  }
+  if (t == 0) { rs->n_list = s_base; rs->bad = 0; rs->valid = 1; rs->cached_m = m; rs->cached_scale = scale; }
+}
+void launch_ring_prep(const float* x, int Q, int D, Ring r, int m, float* partial, int want_scale, RowArrays ra, BlockScalars* bs,
+                      cudaStream_t st) {
+  const long long n_total = static_cast<long long>(Q + m) * D;    // launch_prep_reduce's grid for Q + m rows
+  int nb = static_cast<int>((n_total + 256 * 16 - 1) / (256 * 16));
+  if (nb < 1) nb = 1; if (nb > 592) nb = 592;
+  ring_prep_kernel<<<nb, 256, 0, st>>>(x, Q, D, r, m, partial, want_scale, ra, bs);
+  count_launch();
+}
+
+// The batch's tiles [0, bt), then the listed ring tiles, each split by split_load / split_tile as split_kernel splits it: a persistent
+// grid, each block alternating its transposition buffers from tile to tile
+template <int PREC>
+__global__ void __launch_bounds__(256) ring_split_kernel(SplitArgs a, const BlockScalars* __restrict__ bs, const RingState* __restrict__ rs,
+                                                         const int* __restrict__ list, int bt) {
+  const int dt = (a.D + 63) / 64;
+  const int total = (bt + rs->n_list) * dt;
+  const float sc = (PREC == PREC_FP16X2) ? bs->x_scale : 1.f;
+  int buf = 0;
+  for (int i = blockIdx.x; i < total; i += gridDim.x, buf ^= 1) {
+    const int k = i / dt, tile_d = i - k * dt;
+    const int tile_n = k < bt ? k : __ldg(list + (k - bt));
+    float v[8];
+    split_load(a, tile_d, tile_n, v);
+    split_tile<PREC>(a, sc, tile_d, tile_n, v, buf);
+  }
+}
+void launch_ring_split(const float* x, int Q, int D, Ring r, int m, int prec, const BlockScalars* bs, uint16_t* Xs, long long ldXs,
+                       uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, int sms, cudaStream_t st) {
+  const int N = Q + m, bt = (Q + RING_TILE - 1) / RING_TILE;
+  const long long most = static_cast<long long>((N + RING_TILE - 1) / RING_TILE) * ((D + 63) / 64);
+  const int grid = static_cast<int>(most < 8ll * sms ? most : 8ll * sms);
+  const SplitArgs a{RowSource{x, Q, r.x}, N, D, Xs, ldXs, XsT, ldXsT, nullptr, 0, 0, Q, XcatA, XcatB, Dp};
+  with_prec(prec, [&](auto P) { ring_split_kernel<P><<<grid, 256, 0, st>>>(a, bs, r.st, r.list, bt); });
+  count_launch();
+}
+
+// One warp per pushed row: its D floats into the slot, max |x| of the row (fmaxf from 0, as abs_sum_max), the label and the tile's
+// dirty flag; the last block advances the count
+__global__ void __launch_bounds__(256) ring_push_kernel(const float* __restrict__ x, const float* __restrict__ label, int Q, int D, Ring r) {
+  RingState* rs = r.st;
+  if (rs->bad) return;
+  const unsigned long long c = rs->count;
+  const int M = r.M, lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5), gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  for (int row = (Q > M ? Q - M : 0) + gw; row < Q; row += warps) {   // a batch larger than the ring leaves its last M rows
+    const int slot = static_cast<int>((c + static_cast<unsigned long long>(row)) % static_cast<unsigned long long>(M));
+    const float* src = x + static_cast<long long>(row) * D;
+    float* dst = r.x + static_cast<long long>(slot) * D;
+    float mx = 0.f;
+    for (int d = lane; d < D; d += 32) { const float v = src[d]; dst[d] = v; mx = fmaxf(mx, fabsf(v)); }
+    mx = warp_max(mx);
+    if (lane == 0) { r.rowmax[slot] = mx; r.label[slot] = label[row]; r.dirty[(Q + slot) / RING_TILE] = 1; }
+  }
+  __shared__ int s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) { __threadfence(); s_last = atomicAdd(&rs->ticket, 1u) == gridDim.x - 1; }
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) { rs->count = c + static_cast<unsigned long long>(Q); rs->ticket = 0; }
+}
+void launch_ring_push(const float* x, const float* label, int Q, int D, Ring r, cudaStream_t st) {
+  const int rows = Q < r.M ? Q : r.M;
+  const int blocks = (rows + 7) / 8;
+  ring_push_kernel<<<blocks < 1 ? 1 : (blocks > 1024 ? 1024 : blocks), 256, 0, st>>>(x, label, Q, D, r);
+  count_launch();
+}
+
+__global__ void ring_tops_kernel(AsyncWords* __restrict__ aw, float* __restrict__ d_tops) {
+  if (threadIdx.x != 0 || blockIdx.x != 0 || !(aw->tops.err & DERR_RING_NOT_FULL)) return;
+  for (int t = 0; t < 5; ++t) d_tops[t] = __int_as_float(0x7fc00000);
+  aw->err |= DERR_RING_NOT_FULL;
+}
+void launch_ring_tops(AsyncWords* aw, float* d_tops, cudaStream_t st) {
+  ring_tops_kernel<<<1, 32, 0, st>>>(aw, d_tops);
+  count_launch();
+}
+
+__global__ void __launch_bounds__(256) ring_loaded_kernel(Ring r, int m, int D, int tiles, unsigned long long count) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5), gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  for (int slot = gw; slot < m; slot += warps) {
+    const float* src = r.x + static_cast<long long>(slot) * D;
+    float mx = 0.f;
+    for (int d = lane; d < D; d += 32) mx = fmaxf(mx, fabsf(src[d]));
+    mx = warp_max(mx);
+    if (lane == 0) r.rowmax[slot] = mx;
+  }
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < tiles; k += gridDim.x * blockDim.x) r.dirty[k] = 0;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    RingState* rs = r.st;
+    rs->count = count; rs->valid = 0; rs->cached_m = 0; rs->cached_scale = 0.f; rs->bad = 0; rs->n_list = 0; rs->ticket = 0;
+  }
+}
+void launch_ring_loaded(Ring r, int m, int D, int tiles, unsigned long long count, cudaStream_t st) {
+  const int blocks = (m + 7) / 8;
+  ring_loaded_kernel<<<blocks < 1 ? 1 : (blocks > 1024 ? 1024 : blocks), 256, 0, st>>>(r, m, D, tiles, count);
   count_launch();
 }
 

@@ -20,6 +20,9 @@ enum { DERR_GATHER_SLOT = 4 };
 enum { DERR_KMEANS_NO_ARGMAX = 8 };
 // the layer: an anchor weight (npair_set_anchor_io) outside [0, 1] or NaN
 enum { DERR_ANCHOR_WEIGHT = 16 };
+// a ring forward (npair_forward_ring) found fewer rows in the context's memory ring than the m it was enqueued for: a replayed graph
+// after npair_memory_ring_load with count < M
+enum { DERR_RING_NOT_FULL = 32 };
 
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -299,6 +302,42 @@ void launch_split(RowSource db, int N, int D, int prec, const BlockScalars* bs,
                   uint16_t* XcatA /*or NULL*/, uint16_t* XcatB, long long Dp, cudaStream_t st);
 // lab_total[0, Q + m) = [label; mem_label], rec[Q + i] = RowRecord::memory(mem_label[i])
 void launch_memory_rows(const float* label, int Q, const float* mem_label, int m, float* lab_total, RowRecord* rec, cudaStream_t st);
+
+// The cross-batch memory ring a context keeps (npair_create_memory_ring, DESIGN 4.3.1).  Slot s holds a row the layer used and its
+// label; it is database row Q + s of a step with m = min(count, M) memory rows.  The split operand pieces of the ring's rows stay in
+// the context's operand buffers from step to step: a step re-splits only the 32-row database tiles (RING_TILE) whose pieces are stale.
+constexpr int RING_TILE = 32;                   // the rows of one split_tile
+struct RingState {
+  unsigned long long count;    // rows pushed since the last load
+  int valid;                   // the pieces of rows [Q, Q + cached_m) were split at the pre-scale cached_scale
+  int cached_m;
+  float cached_scale;
+  int bad;                     // this step's m is not min(count, M): nothing reads or writes the slots (DERR_RING_NOT_FULL)
+  int n_list;                  // ring tiles this step re-splits: list[0, n_list)
+  unsigned int ticket;         // last-block counter of the push
+};
+struct Ring {
+  float *x, *label, *rowmax;   // [M][D] rows, [M] labels, [M] max |x| of each slot's row
+  int* dirty;                  // [database tiles] 1: a slot of the tile was pushed since its pieces were split
+  int* list;                   // [database tiles] the ring tiles the step re-splits, ascending
+  RingState* st;
+  int M;
+};
+// A ring step's launches, in order.  prep: launch_prep_reduce over [x; ring[0, m)] (same grid, asum bits and x_absmax), with max |x|
+// of the memory rows from the slots' row maxima; its last block also flags a step whose m is not min(count, M) and lists the ring
+// tiles to re-split: all of them when the pre-scale differs from the cached one, else those with a pushed slot and, when m changed,
+// the tile of row Q + m - 1.
+void launch_ring_prep(const float* x, int Q, int D, Ring r, int m, float* partial, int want_scale, RowArrays ra, BlockScalars* bs,
+                      cudaStream_t st);
+// split: writes what launch_split writes for [x; ring[0, m)], for the Q batch rows' tiles and the listed ring tiles only
+void launch_ring_split(const float* x, int Q, int D, Ring r, int m, int prec, const BlockScalars* bs, uint16_t* Xs, long long ldXs,
+                       uint16_t* XsT, long long ldXsT, uint16_t* XcatA, uint16_t* XcatB, long long Dp, int sms, cudaStream_t st);
+// push: the last min(Q, M) rows of x and their labels into slots (count + r) mod M, their row maxima, the tiles' dirty flags, count += Q
+void launch_ring_push(const float* x, const float* label, int Q, int D, Ring r, cudaStream_t st);
+// the asynchronous forward's finish after launch_async_tops: NaN tops and the error bit kept in aw->err for a DERR_RING_NOT_FULL step
+void launch_ring_tops(AsyncWords* aw, float* d_tops, cudaStream_t st);
+// after a load of m = min(count, M) slots: their row maxima, the count, no valid pieces, no dirty tile
+void launch_ring_loaded(Ring r, int m, int D, int tiles, unsigned long long count, cudaStream_t st);
 void launch_row_stats_ref(SimRows sim, RowArrays ra, cudaStream_t st);
 // The threshold pick of the rank's Q rows by one block (SIMT backend; the tensor-core similarity sweep runs it in its last CTA)
 void launch_thresholds(RowArrays ra, int Q, int N, MiningParams mp, BlockScalars* bs, cudaStream_t st);

@@ -28,6 +28,10 @@ tensor (npair_forward_async) and the loss is its element 0 on the device; the ba
 can be captured with torch.cuda.graph (DESIGN 4.4); a device error (the cases the blocking forward raises for) gives NaN tops and is
 reported by async_status().  With memory_rows > 0 it runs eagerly only: the ring's head is Python state that a graph would freeze.
 
+LIBRARY MEMORY.  NPairLoss(memory_rows=M, library_memory=True) keeps the ring in the library context instead (npair_forward_ring,
+DESIGN 4.3.1): the same results bit for bit, the ring advanced on the device, and only the ring rows pushed since the last step
+re-split.  With blocking=False a whole step can then be captured with torch.cuda.graph once the ring is full (M rows pushed).
+
 ANCHOR WEIGHTS.  loss_fn(x, labels, anchor_weight=w) weights anchor i's term by w_i in [0, 1] (npair_set_anchor_io, DESIGN 4.5): the loss
 is -(1/Z) sum_i w_i log(A_i / T_i), Z = Q (Q * world under global_scope), not renormalised, and the backward is its gradient.  A row with
 w_i = 0 still serves the other anchors as a positive or negative, and still gets gradient through their terms.  row_losses=True adds a
@@ -72,7 +76,13 @@ class _NPairFunction(torch.autograd.Function):
         if io:
             layer.set_anchor_io(weight, rl)
         try:
-            if owner._blocking:
+            if owner._library_memory:
+                if owner._blocking:
+                    t = torch.tensor(layer.forward_ring(feat, label), dtype=torch.float32, device=feat.device)
+                else:
+                    t = layer.forward_ring_async(feat, label, torch.empty(5, dtype=torch.float32, device=feat.device))
+                owner._mem_count += feat.shape[0]
+            elif owner._blocking:
                 if owner._mem_cap:
                     tops = owner._forward_memory(layer, feat, label)
                 else:
@@ -128,11 +138,14 @@ class NPairLoss(torch.nn.Module):
     normalize_input the normalised rows the layer used), so a batch is never in the memory during its own step.  The ring survives the
     context being re-created for a new batch size; it is emptied when the dimension or device changes and by reset_memory().
 
+    library_memory=True (with memory_rows > 0): the ring lives in the library context (LIBRARY MEMORY in the module docstring), with the
+    same slots, results and rules; memory() returns copies, and the ring is carried into a context re-created for a new batch size.
+
     blocking=False (world = 1 only): the asynchronous step of the module docstring.  The loss and the tops are computed on the device and
     nothing waits for them; async_status() reports a device error of the forwards since the last call."""
 
     def __init__(self, world: int = 1, rank: int = 0, nccl_id: bytes | None = None, true_gradient: bool = False, _context_factory=None,
-                 memory_rows: int = 0, blocking: bool = True, **config):
+                 memory_rows: int = 0, blocking: bool = True, library_memory: bool = False, **config):
         super().__init__()
         if not blocking and world != 1:
             raise ValueError("blocking=False is defined for world = 1 (the multi-rank exchanges keep host state per step)")
@@ -144,8 +157,13 @@ class NPairLoss(torch.nn.Module):
             raise ValueError("a cross-batch memory (memory_rows > 0) is defined for world = 1")
         self._config, self._world, self._rank, self._nccl_id = dict(config), world, rank, nccl_id
         self._mem_cap = int(memory_rows)
+        self._library_memory = bool(library_memory)
+        if self._library_memory and not self._mem_cap:
+            raise ValueError("library_memory=True needs memory_rows > 0")
         if _context_factory is not None:
             self._factory = _context_factory
+        elif self._library_memory:
+            self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._mem_cap, ring=True)
         elif self._mem_cap:
             self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._mem_cap)
         else:
@@ -155,18 +173,39 @@ class NPairLoss(torch.nn.Module):
         self._true_gradient = bool(true_gradient)
         self._blocking = bool(blocking)
         self._mem_x = self._mem_l = None      # the ring: [M, D] rows and [M] fp32 labels, allocated at the first forward
-        self._mem_count = 0                   # rows enqueued since the last reset (the valid slots are 0 .. min(count, M) - 1)
+        self._ring_device = None              # library_memory: the device of the context's ring
+        # rows enqueued since the last reset (the valid slots are 0 .. min(count, M) - 1); library_memory: as this module enqueued them,
+        # which a replayed graph does not add to (only whether the ring is full matters then)
+        self._mem_count = 0
 
     def reset_memory(self):
         """Empties the cross-batch memory: the next forward sees no memory rows."""
         self._mem_count = 0
+        if self._library_memory and self._ctx is not None:
+            self._ctx.ring_load(None, None, 0)
 
     def memory(self):
-        """(rows [m, D], labels [m]) the next forward passes as its memory: views of the ring's valid slots, in slot order."""
+        """(rows [m, D], labels [m]) the next forward passes as its memory, in slot order: views of the ring's valid slots, or with
+        library_memory copies read from the context."""
+        if self._library_memory:
+            if self._ctx is None:
+                return None, None
+            x, lab, count = self._read_ring(self._ctx)
+            m = min(count, self._mem_cap)
+            return x[:m], lab[:m]
         m = min(self._mem_count, self._mem_cap)
         if self._mem_x is None:
             return None, None
         return self._mem_x[:m], self._mem_l[:m]
+
+    def _read_ring(self, layer):
+        """(rows [M, D], labels [M], push count) of a library_memory context's ring."""
+        dev = self._ring_device
+        x = torch.empty(self._mem_cap, layer.cfg.D, dtype=torch.float32, device=dev)
+        lab = torch.empty(self._mem_cap, dtype=torch.float32, device=dev)
+        count = torch.zeros(1, dtype=torch.int64, device=dev)
+        layer.ring_read(x, lab, count)
+        return x, lab, int(count.item())
 
     def async_status(self):
         """blocking=False: waits for the module's last library call and raises capi.NpairError if a forward since the previous call met a
@@ -203,15 +242,38 @@ class NPairLoss(torch.nn.Module):
         self._mem_count += q
         return tops
 
+    def _capture_refusal(self, feat):
+        """Why a library_memory step on feat cannot be captured now, or None: every replay must find the ring full."""
+        if self._blocking:
+            return "NPairLoss(blocking=True) waits for its tops on the host and cannot be captured: use blocking=False"
+        q = feat.shape[0]
+        if (q, feat[0].numel(), feat.device.index) != self._key:
+            return ("NPairLoss(library_memory=True): run an eager step with this batch shape before capturing one (it creates the "
+                    "library context and carries the memory ring into it)")
+        if self._mem_count < self._mem_cap:
+            left = self._mem_cap - self._mem_count
+            return (f"NPairLoss(library_memory=True) can be captured once its memory ring is full: {left} of its {self._mem_cap} rows "
+                    f"are missing; run {-(-left // q)} more eager step(s) of {q} rows first")
+        return None
+
     def _context(self, feat):
         q, d = feat.shape[0], feat[0].numel()
         key = (q, d, feat.device.index)
         if key != self._key:
-            old = self._ctx
+            old, old_key = self._ctx, self._key
             cfg = capi.make_config(q, d, world=self._world, rank=self._rank, device=feat.device.index or 0, **self._config)
             # the new context is created BEFORE the old one is closed: contexts made with the same NCCL id share one
             # communicator inside the library, which must stay referenced (a unique id can be consumed only once)
             self._ctx, self._key = self._factory(cfg, self._nccl_id), key
+            if self._library_memory:
+                # the ring survives a new batch size as the module's own ring does (slots do not depend on Q); a new dimension or
+                # device starts it empty
+                self._ring_device = feat.device
+                if old is not None and old_key[1:] == key[1:]:
+                    x, lab, self._mem_count = self._read_ring(old)
+                    self._ctx.ring_load(x, lab, self._mem_count)
+                else:
+                    self._mem_count = 0
             if old is not None and hasattr(old, "close"):
                 old.close()
         return self._ctx
@@ -229,7 +291,11 @@ class NPairLoss(torch.nn.Module):
             if anchor_weight.device != feat.device:
                 raise ValueError("anchor_weight must be on the embeddings' device")
             anchor_weight = anchor_weight.contiguous()
-        if not self._blocking and self._mem_cap and feat.is_cuda and torch.cuda.is_current_stream_capturing():
+        if self._library_memory and feat.is_cuda and torch.cuda.is_current_stream_capturing():
+            refusal = self._capture_refusal(feat)
+            if refusal:
+                raise RuntimeError(refusal)
+        elif not self._blocking and self._mem_cap and feat.is_cuda and torch.cuda.is_current_stream_capturing():
             raise RuntimeError("NPairLoss(memory_rows > 0, blocking=False) cannot be captured into a CUDA graph: the memory ring's head "
                                "and count are Python state that the graph would freeze")
         feat2 = feat.reshape(feat.shape[0], -1).contiguous()
