@@ -101,7 +101,9 @@ enum {
   NPAIR_FLAG_GRAD_1CTA = 4,       /* no effect on sm_90 (every GEMM runs one CTA per tile); kept for ABI compatibility       */
   NPAIR_FLAG_NCCL_RECORDS = 8,    /* world > 1: exchange the row records with ncclAllGather instead of NVLink peer stores    */
   NPAIR_FLAG_NCCL_FEATURES = 16,  /* world > 1: gather the features with ncclAllGather instead of NVLink peer loads          */
-  NPAIR_FLAG_LSEL_WARP = 32       /* LOCAL RELATIVE_* select: warp-per-row kernel also for rows that fit the block-per-row one */
+  NPAIR_FLAG_LSEL_WARP = 32,      /* LOCAL RELATIVE_* select: warp-per-row kernel also for rows that fit the block-per-row one */
+  NPAIR_FLAG_GRAD_GENERAL = 64    /* fused gradient: build every weight with the general builder, also where the different-label
+                                     one applies (DESIGN 4); the gradient is bit for bit the same, so this exists for tests only   */
 };
 
 /* Row-block similarity mode: flags bits 16-27 hold a block height in units of 128 rows (0 = off: the whole Q x N similarity matrix S

@@ -26,7 +26,7 @@ class NpairConfig(C.Structure):
                 ("global_scope", C.c_int32), ("normalize_input", C.c_int32), ("grad_chunk_cols", C.c_int32), ("flags", C.c_int32)]
 
 
-FLAG_NO_FUSED_GRAD, FLAG_SIM_1CTA, FLAG_GRAD_1CTA, FLAG_NCCL_RECORDS, FLAG_NCCL_FEATURES, FLAG_LSEL_WARP = 1, 2, 4, 8, 16, 32
+FLAG_NO_FUSED_GRAD, FLAG_SIM_1CTA, FLAG_GRAD_1CTA, FLAG_NCCL_RECORDS, FLAG_NCCL_FEATURES, FLAG_LSEL_WARP, FLAG_GRAD_GENERAL = 1, 2, 4, 8, 16, 32, 64
 # row-block similarity mode: flags bits 16-27 = block height in units of 128 rows (NPAIR_SIM_BLOCK_ROWS)
 SIM_BLOCK_SHIFT, SIM_BLOCK_MAX_UNITS = 16, 0xFFF
 

@@ -1442,6 +1442,7 @@ static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
     fp.ldo = D; fp.alpha = alpha; fp.beta = 0.f; fp.dev_scale = dev_scale;
     fp.part = c->part;
     fp.chunk_kb = c->grad_chunk_kb;
+    fp.general_only = (c->cfg.flags & NPAIR_FLAG_GRAD_GENERAL) != 0;
     // per block of rows of S, starting with the one the forward left in the buffer (a materialised S is the one block): recompute it,
     // then its gradient rows.  The split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output
     // bit is the materialised path's

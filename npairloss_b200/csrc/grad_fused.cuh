@@ -16,8 +16,16 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "gemm_wgmma.cuh"
 #include "ptx.cuh"
+
+// Probe builds for tools/bench_grad_sweep.py, which time the gradient phase with one part of the kernel left out: 1 constant weight
+// fragments (no weight build), 2 no MMAs.  The probes compute garbage.
+#ifndef NPAIR_GRAD_PROBE
+#define NPAIR_GRAD_PROBE 0
+#endif
 
 namespace npair {
 
@@ -35,6 +43,7 @@ struct FusedGradParams {
   float* out; long long ldo;
   float alpha, beta;
   const float* dev_scale;       // inverse operand pre-scale (power of two) or NULL
+  int general_only;             // NPAIR_FLAG_GRAD_GENERAL: every weight through pair_weight (tests compare the two builders)
   int m_blk0;                   // row-block mode: the rank's 128-row tile that local tile 0 stands for (0 otherwise).  Only the
                                 // accumulation-chunk key uses it; rowrec / out / self_offset are passed already offset
 };
@@ -110,26 +119,43 @@ struct RowRec { float m2r, tn, m2, lab, tp, cA; int self_col; };
 // Branch-free: the label test selects the two exponentials' arguments and then the result, so the eight weights of a K step form
 // independent straight-line chains that the scheduler interleaves (a branch per weight serialised their shared-memory and MUFU
 // latencies, and with two consumer warps per scheduler nothing else hid them).  Each case performs exactly the operations it would
-// on its own.  The selects are PTX selp: written as C conditionals, the compiler turned them back into branches.
-__device__ __forceinline__ float select_f32(bool c, float a, float b) {
+// on its own.  The selects are PTX setp + selp on the compare itself: written as C conditionals, the compiler turned them back into
+// branches, and a bool passed into the asm cost a conversion and a second compare per select.
+__device__ __forceinline__ float select_le(float x, float y, float a, float b) {   // x <= y ? a : b (false when either is NaN)
   float r;
-  asm("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"(static_cast<int>(c)));
+  asm("{\n\t.reg .pred q;\n\tsetp.le.f32 q, %1, %2;\n\tselp.f32 %0, %3, %4, q;\n\t}" : "=f"(r) : "f"(x), "f"(y), "f"(a), "f"(b));
   return r;
+}
+__device__ __forceinline__ float select_eq(float x, float y, float a, float b) {   // !(x != y) ? a : b (false when either is NaN)
+  float r;
+  asm("{\n\t.reg .pred q;\n\tsetp.eq.f32 q, %1, %2;\n\tselp.f32 %0, %3, %4, q;\n\t}" : "=f"(r) : "f"(x), "f"(y), "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float ex2_approx(float a) {
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(a));
+  return e;
 }
 __device__ __forceinline__ float pair_weight(float s, const RowRecord& c, const RowRec& r, int m, const FusedGradParams& p) {
   // c: the record of the column's row
-  const bool same = !(c.label() != r.lab);
   const float kn = s * p.sgn_n;                  // HARD / RELATIVE_HARD negatives compare -s
-  const float a1 = select_f32(same, fmaf(s, LOG2E, -r.m2), select_f32(kn <= r.tn, fmaf(s, LOG2E, -r.m2r), -INFINITY));
-  const float a2 = select_f32(same, fmaf(s, LOG2E, -c.m2()), select_f32(kn <= c.thr_n(), fmaf(s, LOG2E, -c.m2c()), -INFINITY));
-  float e1, e2;                                  // same-label: the forward row pass's exponential (fast_exp_m2)
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(a2));
+  const float a1 = select_eq(c.label(), r.lab, fmaf(s, LOG2E, -r.m2), select_le(kn, r.tn, fmaf(s, LOG2E, -r.m2r), -INFINITY));
+  const float a2 = select_eq(c.label(), r.lab, fmaf(s, LOG2E, -c.m2()), select_le(kn, c.thr_n(), fmaf(s, LOG2E, -c.m2c()), -INFINITY));
+  const float e1 = ex2_approx(a1), e2 = ex2_approx(a2);   // same-label: the forward row pass's exponential (fast_exp_m2)
   const float kp = s * p.sgn_p;
-  const float w1 = select_f32(kp <= r.tp, e1 * r.cA, 0.f);
-  const float w2 = select_f32(kp <= c.thr_p(), e2 * c.cA(), 0.f);
-  const float g = select_f32(same, fmaf(w2, p.inv_world, w1), e1 + e2);
+  const float w1 = select_le(kp, r.tp, e1 * r.cA, 0.f);
+  const float w2 = select_le(kp, c.thr_p(), e2 * c.cA(), 0.f);
+  const float g = select_eq(c.label(), r.lab, fmaf(w2, p.inv_world, w1), e1 + e2);
   return (m == r.self_col || m >= p.N) ? 0.f : g;
+}
+// pair_weight of a different-label pair that is not the self pair and lies below N: the same operations on the different-label
+// side, with the sign of the compare folded in (-s is s * -1 exactly).  cm2c, cthr: the column record's m2c and thr_n.
+template <bool NEG>
+__device__ __forceinline__ float diff_weight(float s, float cm2c, float cthr, const RowRec& r) {
+  const float kn = NEG ? -s : s;
+  const float e1 = ex2_approx(select_le(kn, r.tn, fmaf(s, LOG2E, -r.m2r), -INFINITY));
+  const float e2 = ex2_approx(select_le(kn, cthr, fmaf(s, LOG2E, -cm2c), -INFINITY));
+  return e1 + e2;
 }
 
 __device__ __forceinline__ RowRec load_rowrec(const FusedGradParams& p, int row) {
@@ -198,10 +224,59 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
     const int c4 = lane & 3;
     const int rl0 = g * 64 + wi * 16 + (lane >> 2);  // tile rows of this thread's fragment: rl0, rl0 + 8
     // A fragment of K step k2 of K block kb (in ring stage `st_idx`): columns 16*k2 + 2*c4 + {0, 1} (t = 0) and + 8 (t = 1),
-    // rows rl0 (h = 0) and rl0 + 8 (h = 1)
-    auto build = [&](uint32_t (&af)[NSPLIT][4], const RowRec (&rr)[2], int st_idx, int kb, int k2) {
+    // rows rl0 (h = 0) and rl0 + 8 (h = 1).  The different-label builder fills the fragment first; when a pair of the warp's 16 x 16
+    // block is same-label, a self pair (self columns [self0, self0 + 16)) or a column past N (one warp-uniform vote per K step), the
+    // general builder rebuilds it.  At one same-label column per row that is almost no step, whatever the order of the labels, and the
+    // vote's label loads and compares stay off the build's dependency chain.
+    auto build = [&](uint32_t (&af)[NSPLIT][4], const RowRec (&rr)[2], int self0, int st_idx, int kb, int k2) {
       const uint8_t* s_tile = smem + st_idx * Cfg::STAGE_BYTES + NSPLIT * Cfg::B_PIECE;
       const RowRecord* crec = reinterpret_cast<const RowRecord*>(s_tile + Cfg::S_TILE);
+      if (NPAIR_GRAD_PROBE == 1) {
+#pragma unroll
+        for (int s = 0; s < NSPLIT; ++s)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) af[s][i] = 0x3c003c00u;
+        return;
+      }
+      const int m0 = kb * BK + 16 * k2;
+      // the step's similarities, read by both builders
+      float2 s2[2][2];
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        const int k = 16 * k2 + 8 * t + 2 * c4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rl = rl0 + 8 * h;
+          s2[t][h] = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
+        }
+      }
+      float4 lo[2][2];                            // first record halves {m2c, thr_n, m2, label} of columns m, m + 1 of t = 0, 1
+      bool general = p.general_only || m0 > p.N - 16 || static_cast<unsigned>(m0 - self0 + 15) < 31u;
+#pragma unroll
+      for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          lo[t][e] = RowRecord::load(crec, 16 * k2 + 8 * t + 2 * c4 + e).lo;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) general |= !(lo[t][e].w != rr[h].lab);
+        }
+      {
+        auto diff = [&](auto neg) {
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint32_t o[3];
+              split_pair<NSPLIT, BF16>(diff_weight<decltype(neg)::value>(s2[t][h].x, lo[t][0].x, lo[t][0].y, rr[h]),
+                                       diff_weight<decltype(neg)::value>(s2[t][h].y, lo[t][1].x, lo[t][1].y, rr[h]), o);
+#pragma unroll
+              for (int s = 0; s < NSPLIT; ++s) af[s][2 * t + h] = o[s];
+            }
+          }
+        };
+        if (p.sgn_n < 0.f) diff(std::true_type()); else diff(std::false_type());
+      }
+      if (!__any_sync(0xffffffffu, general)) return;
 #pragma unroll
       for (int t = 0; t < 2; ++t) {
         const int k = 16 * k2 + 8 * t + 2 * c4;
@@ -210,10 +285,8 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
         const RowRecord c0 = RowRecord::load(crec, k), c1 = RowRecord::load(crec, k + 1);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int rl = rl0 + 8 * h;
-          const float2 s2 = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
-          const float w0 = pair_weight(s2.x, c0, rr[h], m, p);
-          const float w1 = pair_weight(s2.y, c1, rr[h], m + 1, p);
+          const float w0 = pair_weight(s2[t][h].x, c0, rr[h], m, p);
+          const float w1 = pair_weight(s2[t][h].y, c1, rr[h], m + 1, p);
           uint32_t o[3];
           split_pair<NSPLIT, BF16>(w0, w1, o);
 #pragma unroll
@@ -229,12 +302,14 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
       RowRec rr[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) rr[h] = load_rowrec(p, t.m_blk * BM + rl0 + 8 * h);
+      const int self0 = t.m_blk * BM + g * 64 + wi * 16 + p.self_offset;   // self column of the warp's first row
       float acc[128];
       uint32_t af[2][NSPLIT][4];
+      uint32_t sink = 0;                          // NPAIR_GRAD_PROBE 2: what the MMAs would have read
       for (int c0 = t.kb0, c1; c0 < t.kb1; c0 = c1) {
         c1 = chunk_end(c0, t.kb0, t.kb1, p.chunk_kb, ckey);
         ring.wait_full();
-        build(af[0], rr, ring.stage, c0, 0);
+        build(af[0], rr, self0, ring.stage, c0, 0);
         int prev = ring.stage;
         for (int kb = c0; kb < c1; ++kb) {
           const int cur = ring.stage;
@@ -248,21 +323,24 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
               int sa, sb;
               pass_pieces(NSPLIT, ps, sa, sb);
               const uint64_t bd = ptx::make_kmajor_desc(b0 + sb * Cfg::B_PIECE + k2 * 32, 512u, 2u);   // SWIZZLE_64B, 8 rows = 512 B
-              ptx::wgmma_m64n256k16_rs<BF16>(acc, af[k2 & 1][sa], bd, ((kb - c0) | ps | k2) != 0 ? 1u : 0u);
+              if (NPAIR_GRAD_PROBE != 2) ptx::wgmma_m64n256k16_rs<BF16>(acc, af[k2 & 1][sa], bd, ((kb - c0) | ps | k2) != 0 ? 1u : 0u);
+              else for (int i = 0; i < 4; ++i) sink ^= af[k2 & 1][sa][i];
             }
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>();                  // the previous step retired: its A buffer is free, and so is its stage
             if (k2 == 0 && kb != c0) ring.release(prev, lane);
             if (k2 + 1 < KSTEPS) {
-              build(af[(k2 + 1) & 1], rr, cur, kb, k2 + 1);
+              build(af[(k2 + 1) & 1], rr, self0, cur, kb, k2 + 1);
             } else if (kb + 1 < c1) {
               ring.wait_full();
-              build(af[0], rr, ring.stage, kb + 1, 0);
+              build(af[0], rr, self0, ring.stage, kb + 1, 0);
             }
           }
           prev = cur;
         }
         ptx::wgmma_wait<0>();
+        if (NPAIR_GRAD_PROBE == 2)
+          for (int j = 0; j < 128; ++j) acc[j] = __uint_as_float(sink);
         ptx::fence_regs(acc);
         ring.release(prev, lane);
         // drain the chunk: first chunk of the tile stores (+ beta * out), later chunks add (fp32 RN)
