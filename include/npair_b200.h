@@ -193,7 +193,7 @@ int npair_backward_gathered(npair_ctx* ctx, float loss_weight, const float* d_rs
  * loss normaliser Q are those of the reference's rank-0 block over N columns (the GLOBAL region is the Q x N block, the retrieval
  * counters rank over N - 1 columns); feature_asum covers the current rows only.  The backward (npair_backward, npair_backward_partial
  * with d_total_half NULL) returns for the current rows (1/2)(lw/Q)(G . X_total + G[:, 0:Q]^T . x), the reference's world-1 blend with
- * the transposed term not divided by anything; the memory rows get no gradient.  A call's results depend only on the configuration,
+ * the transposed term not divided by anything; the memory rows get no gradient from it (npair_backward_memory returns theirs).  A call's results depend only on the configuration,
  * Q, m and the inputs: not on max_memory_rows, earlier calls or the rows a call with a larger m left behind.  The forward reads
  * d_mem_feat / d_mem_label and nothing later does: the caller may overwrite them in stream order once npair_forward_memory returns
  * (the current batch stays under the rule of npair_forward).  normalize_input normalises the current rows; memory rows are used as
@@ -211,6 +211,21 @@ int npair_create_memory(const npair_config* cfg, int32_t max_memory_rows, npair_
 size_t npair_memory_workspace_bytes(const npair_config* cfg, int32_t max_memory_rows);
 int npair_forward_memory(npair_ctx* ctx, const float* d_feat, const float* d_label, const float* d_mem_feat, const float* d_mem_label,
                          int32_t m, float tops_host[5], void* stream);
+
+/* ---- the memory rows' gradient (DESIGN 4.6): memory rows as learnable database rows (class proxies, a second encoder's rows) ----
+ * After npair_forward_memory(_async) with m memory rows y (as the caller passed them: normalize_input normalises the current rows only):
+ *   d_feat_diff : Q x D, the bits npair_backward (npair_backward_device_weight) writes after the same forward, on every format;
+ *   d_mem_diff  : m x D, d_mem_diff[p] = (1/2)(lw/Q) sum_i G[i][Q + p] x_i, with G the anchors' weights of that gradient (the same
+ *                 mining, anchor weights, 1/2 convention and scales) and x_i the anchors as the layer read them.  Twice it is the
+ *                 analytic gradient of the loss with respect to y.  m = 0 leaves d_mem_diff untouched.
+ * As every result of a memory step, both depend only on the configuration, Q, m and the inputs.  The device-weight call reads the loss
+ * weight as npair_backward_device_weight does and is capturable under the same rules (a graph holds a forward_memory_async and its
+ * backward).  Refused on the host before anything is enqueued: NPAIR_E_ARG for a null pointer, one not 16-byte aligned, or a
+ * context with NPAIR_FLAG_NO_FUSED_GRAD (the fused gradient kernel is the only path); NPAIR_E_STATE without a successful forward,
+ * when the last forward was not a memory forward, and on a ring context (npair_create_memory_ring: its rows are the ring's detached
+ * slots).  Profile phase 7 times the memory-row part. */
+int npair_backward_memory(npair_ctx* ctx, float loss_weight, float* d_feat_diff, float* d_mem_diff, void* stream);
+int npair_backward_memory_device_weight(npair_ctx* ctx, const float* d_loss_weight, float* d_feat_diff, float* d_mem_diff, void* stream);
 
 /* ---- asynchronous training step and CUDA-graph capture, world 1 only (DESIGN 4.4) ----
  * The calls above that return tops on the host wait for them.  These do not: they return once the step's work is enqueued, making
@@ -309,7 +324,8 @@ const char* npair_version(void);
 
 /* Per-phase CUDA-event timing on the caller's stream (used by bench.py for the roofline of the dominant kernel).
  * ms_out[9]: 0 forward all-gather  1 operand prep  2 similarity GEMM (+fused statistics)  3 thresholds / radix selects
- *            4 forward row pass + finalize  5 backward weight builder  6 gradient GEMM  7 transposed gradient GEMM
+ *            4 forward row pass + finalize  5 backward weight builder  6 gradient GEMM  7 transposed gradient GEMM (world > 1;
+ *            at world 1 the memory-row gradient of npair_backward_memory)
  *            8 backward exchange (row-scalar all-gather or reduce-scatter)
  * Row-block similarity mode: 2 = the statistics sweep (+ fused threshold pick), 3 = 0, 4 = the forward's block recomputes, LOCAL
  * relative selects and row passes + finalize, 6 = the backward's block recomputes and gradient kernels. */

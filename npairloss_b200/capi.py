@@ -48,6 +48,8 @@ EXPORTS = ["npair_config_default", "npair_workspace_bytes", "npair_nccl_unique_i
            "npair_memory_ring_read", "npair_memory_ring_load",
            # asynchronous step and graph capture (not part of the reference layer)
            "npair_forward_async", "npair_forward_memory_async", "npair_backward_device_weight", "npair_async_status",
+           # the memory rows' gradient (not part of the reference layer)
+           "npair_backward_memory", "npair_backward_memory_device_weight",
            # per-anchor loss weights and losses (not part of the reference layer)
            "npair_set_anchor_io",
            # retrieval evaluation (not part of the reference layer)
@@ -106,6 +108,8 @@ def lib():
         L.npair_forward_async.argtypes = [vp, vp, vp, vp, vp]
         L.npair_forward_memory_async.argtypes = [vp, vp, vp, vp, vp, C.c_int32, vp, vp]
         L.npair_backward_device_weight.argtypes = [vp, vp, vp, vp]
+        L.npair_backward_memory.argtypes = [vp, C.c_float, vp, vp, vp]
+        L.npair_backward_memory_device_weight.argtypes = [vp, vp, vp, vp, vp]
         L.npair_async_status.argtypes = [vp]
         L.npair_forward_gathered.argtypes = [vp, vp, vp, fp, vp]
         L.npair_backward_partial.argtypes = [vp, C.c_float, vp, vp, vp]
@@ -211,6 +215,7 @@ class Context:
         self.cfg = cfg
         self.memory_rows = int(memory_rows)
         self.ring = bool(ring)
+        self.last_m = 0                       # memory rows of the last forward (backward_memory's m x D output)
         self._h = C.c_void_p()
         idbuf = C.create_string_buffer(nccl_id, 128) if nccl_id is not None else None
         if self.ring:
@@ -244,6 +249,7 @@ class Context:
     def forward_ptr(self, feat_ptr: int, label_ptr: int, stream: int = 0):
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward(self._h, feat_ptr, label_ptr, tops, stream))
+        self.last_m = 0
         return [tops[i] for i in range(5)]
 
     def _rows(self, feat, label, rows=None):
@@ -259,6 +265,7 @@ class Context:
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward_backward(self._h, *self._rows(feat, label), C.c_float(loss_weight), self._grad(diff), tops,
                                                  _stream()))
+        self.last_m = 0
         return [tops[i] for i in range(5)]
 
     def forward(self, feat, label):
@@ -267,6 +274,7 @@ class Context:
     def forward_memory_ptr(self, feat_ptr: int, label_ptr: int, mem_feat_ptr, mem_label_ptr, m: int, stream: int = 0):
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward_memory(self._h, feat_ptr, label_ptr, mem_feat_ptr, mem_label_ptr, int(m), tops, stream))
+        self.last_m = int(m)
         return [tops[i] for i in range(5)]
 
     def _memory(self, mem_feat, mem_label, m):
@@ -290,25 +298,45 @@ class Context:
         """npair_forward_async: enqueues the forward and returns at once; tops_out (5 fp32 on the device) receives the tops in stream
         order, all NaN on a device error (see async_status)."""
         self._check(lib().npair_forward_async(self._h, *self._rows(feat, label), _ptr(tops_out, "tops_out", 5), _stream()))
+        self.last_m = 0
         return tops_out
 
     def forward_memory_async(self, feat, label, mem_feat, mem_label, m, tops_out):
         """npair_forward_memory_async: forward_memory with the tops written to tops_out as in forward_async."""
         self._check(lib().npair_forward_memory_async(self._h, *self._rows(feat, label), *self._memory(mem_feat, mem_label, m), int(m),
                                                      _ptr(tops_out, "tops_out", 5), _stream()))
+        self.last_m = int(m)
         return tops_out
+
+    # ---- the memory rows' gradient (DESIGN 4.6) ----
+    def backward_memory(self, loss_weight, diff, mem_diff):
+        """npair_backward_memory: after forward_memory(_async) with m rows, diff [Q, D] receives backward's bits and mem_diff (at least
+        m x D floats) the memory rows' gradient (1/2)(lw/Q) G[:, Q:]^T . x; m = 0 leaves mem_diff untouched."""
+        self._check(lib().npair_backward_memory(self._h, C.c_float(loss_weight), self._grad(diff),
+                                                _ptr(mem_diff, "mem_diff", self.last_m * self.cfg.D), _stream()))
+
+    def backward_memory_device_weight(self, loss_weight, diff, mem_diff):
+        """npair_backward_memory_device_weight: backward_memory with the loss weight read on the device from loss_weight (a one-element
+        CUDA fp32 tensor), as backward_device_weight; capturable after forward_memory_async."""
+        lw = _ptr(loss_weight, "loss_weight", 1)
+        if loss_weight.numel() != 1:
+            raise ValueError("loss_weight is one element")
+        self._check(lib().npair_backward_memory_device_weight(self._h, lw, self._grad(diff),
+                                                              _ptr(mem_diff, "mem_diff", self.last_m * self.cfg.D), _stream()))
 
     # ---- the context's own memory ring (ring=True, DESIGN 4.3.1) ----
     def forward_ring(self, feat, label):
         """npair_forward_ring: forward_memory over the ring's min(count, M) slots, then the batch's rows go into the ring."""
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward_ring(self._h, *self._rows(feat, label), tops, _stream()))
+        self.last_m = 0
         return [tops[i] for i in range(5)]
 
     def forward_ring_async(self, feat, label, tops_out):
         """npair_forward_ring_async: forward_ring with the tops written to tops_out as in forward_async; capturable once the ring is
         full."""
         self._check(lib().npair_forward_ring_async(self._h, *self._rows(feat, label), _ptr(tops_out, "tops_out", 5), _stream()))
+        self.last_m = 0
         return tops_out
 
     def ring_read(self, rows, labels, count):
@@ -358,6 +386,7 @@ class Context:
         tops = (C.c_float * 5)()
         self._check(lib().npair_forward_gathered(self._h, *self._rows(feat_total, label_total, self.cfg.Q * self.cfg.world), tops,
                                                  _stream()))
+        self.last_m = 0
         return [tops[i] for i in range(5)]
 
     def backward_partial(self, loss_weight, local_half, total_half=None):

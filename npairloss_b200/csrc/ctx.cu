@@ -10,6 +10,7 @@
 #include <cudaTypedefs.h>
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -287,7 +288,26 @@ struct CallPlan {
   SplitK grad_split;             // and its split-K
   int n_sym_tiles;
   int sweep_epi;                 // the forward's similarity sweep: statistics, + symmetric tiles, + stores to S if there is one block
+  SplitK mem_grad_split;         // the split-K of the memory-row gradient (npair_backward_memory, DESIGN 4.6); m > 0 only
 };
+
+// The memory-row gradient's split-K: an m x D output over the ceil(Q / 32) K blocks of the Q anchors, cut as the fused gradient's
+static SplitK mem_grad_split(const npair_config& cfg, int sms, int m) {
+  const int kb = (cfg.Q + 31) / 32;
+  return split_k(kb, tile_sched(m, cfg.D, kb).num_tiles(), sms, 8);
+}
+// The most floats its split-K partial products take at any m <= M.  Its split count does not increase with the output's tiles, so the
+// largest m of each tile count is the one to check, and the first tile count with one split ends the search (at most sms tile rows).
+static long long mem_grad_part(const npair_config& cfg, int sms, long long M) {
+  long long most = 0;
+  for (long long rows = 128; rows - 128 < M; rows += 128) {
+    const int m = static_cast<int>(rows < M ? rows : M);
+    const SplitK sk = mem_grad_split(cfg, sms, m);
+    if (sk.splits < 2) break;
+    most = std::max(most, split_part(sk.splits, m, cfg.D));
+  }
+  return most;
+}
 
 // The plan of a call over m cross-batch memory rows (DESIGN 4.3), database columns Q * world + m
 static CallPlan call_plan(const npair_config& cfg, const Plan& p, int sms, int m) {
@@ -308,6 +328,7 @@ static CallPlan call_plan(const npair_config& cfg, const Plan& p, int sms, int m
   // memory rows are no anchors: S is not symmetric, every tile is computed
   if (cfg.world == 1 && tc && !(cfg.flags & NPAIR_INTERNAL_FULL_TILES) && m == 0) cp.n_sym_tiles = static_cast<int>(sym_tile_count(cfg.Q, cp.N));
   cp.sweep_epi = EPI_STATS | (cp.n_sym_tiles ? EPI_SYM : 0) | (p.n_blocks == 1 ? EPI_STORE_S : 0);
+  if (m > 0 && tc && p.fused_grad) cp.mem_grad_split = mem_grad_split(cfg, sms, m);
   return cp;
 }
 
@@ -376,6 +397,7 @@ struct npair_ctx : Plan, CallPlan {
   RowRecord* rs_total = nullptr;   // row-scalar mode: the world's N row records, all-gathered
   float *Ynorm = nullptr, *dY = nullptr, *inv_norm = nullptr;   // normalize_input: x / ||x||, gradient w.r.t. it, 1 / ||x||
   CUtensorMap tm_fB, tm_fS;      // fused gradient kernel: X^T pieces with 32-wide K boxes, 128-row fp32 boxes of S
+  CUtensorMap tm_mX;             // memory-row gradient: the same X^T pieces cut at the Q anchors (its S boxes come through tm_S)
   // peer-memory exchange (world > 1 with a communicator; NPAIR_FLAG_NCCL_FEATURES / _RECORDS fall back to NCCL)
   bool p2p_feat = false, p2p_rec = false;
   float* p2p_region = nullptr;         // laid out by xl (XchgLayout)
@@ -414,6 +436,7 @@ struct npair_ctx : Plan, CallPlan {
     bool rec_gathered = false;     // the NCCL all-gather of the row records has been enqueued (at the first backward)
     bool fwd_done = false;         // the forward succeeded: a backward may follow
     const float* lab_mem = nullptr;   // cross-batch memory: the labels of the caller's memory rows x_total.x1 (only the forward reads them)
+    bool memory = false;           // a forward over a cross-batch memory (any m): npair_backward_memory may follow
   } step;
   StreamOrder order;              // the calls' order across streams; debug_read and profile_read wait for its event
   std::string err;
@@ -450,8 +473,11 @@ static cudaError_t ctx_buffers(npair_ctx* c, DevMem& m) {
   if (c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) m.own(&c->rs_total, sizeof(RowRecord) * N, false);   // gathered row records
   // split-K partial products.  A memory context's calls take the split-K of their own N = Q + m (set_call_rows), which is not monotone
   // in m: the buffer holds split_cap slices of the capacity's N, a bound of every smaller N's count
+  // The memory-row gradient (npair_backward_memory, not on a ring) cuts its own m x D output into splits: the buffer holds those too.
   const int slices = c->mem_cap ? c->split_cap : c->grad_split.splits;
-  if (slices > 1) m.own(&c->part, f * split_part(slices, c->cfg.Q, D), false);
+  long long part = slices > 1 ? split_part(slices, c->cfg.Q, D) : 0;
+  if (c->mem_cap && c->fused_grad && !c->ring) part = std::max(part, mem_grad_part(c->cfg, c->sms, c->mem_cap));
+  if (part) m.own(&c->part, f * part, false);
   m.own_carved(true, [c](Carve& cv) { carve_rows(cv, c->cfg.Q, c->mem_cap, &c->ra); });
   m.own(&c->bs, sizeof(BlockScalars), true);
   m.own(&c->aw, sizeof(AsyncWords), true);
@@ -656,6 +682,8 @@ static bool make_maps(npair_ctx* c, std::string* te) {
   if (c->fused_grad) {
     ok = ok && make_tmap_pieces(&c->tm_fB, c->XsT, N, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, te);
     ok = ok && make_tmap_f32_store(&c->tm_fS, c->S, N, c->s_rows, c->ldS, te, 128);
+    // the memory-row gradient's K = the Q anchors: past them the box reads zeros, not the memory rows' pieces
+    if (c->mem_cap && !c->ring) ok = ok && make_tmap_pieces(&c->tm_mX, c->XsT, Q, D, ns, c->Np, static_cast<long long>(D) * c->Np, 32, 256, te);
   }
   if (c->bwd_mode == NPAIR_BWDMODE_REDUCE_SCATTER) {   // gradient 2: A = HT [N x Q], B = XlT [D x Q]; K = Q
     ok = ok && make_tmap_pieces(&c->tm_b2A, c->HT, Q, N, ns, c->Qp, static_cast<long long>(N) * c->Qp, bkg, 128, te);
@@ -726,6 +754,7 @@ static int create_impl(const npair_config* cfg, const void* id128, void* ext_com
     if (mem_cap) CREATE_TRY(allow_smem(gemm_kernel(c->prec, call_plan(*cfg, *c, c->sms, 0).sweep_epi)));   // its calls with m = 0
     if (c->n_blocks > 1) CREATE_TRY(allow_smem(gemm_kernel(c->prec, EPI_STORE_S)));
     CREATE_TRY(c->fused_grad ? allow_smem(fused_kernel(c->prec)) : allow_smem(gemm_kernel(c->prec, EPI_OUT)));
+    if (c->fused_grad && mem_cap && !ring) CREATE_TRY(allow_smem(fused_kernel(c->prec, true)));   // npair_backward_memory
     // ---- TMA tensor maps (K-major boxes of one swizzle span) ----
     std::string te;
     if (!make_maps(c, &te)) { g_create_err = te; return NPAIR_E_CUDA; }
@@ -932,7 +961,8 @@ static int check_out_aligned(npair_ctx* c, const float* p, const char* name) {
 static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cudaStream_t st);
 // The loss weight of a backward: a host value, or (d_lw, world 1) one fp32 in device memory read in stream order
 struct LossWeight { float host; const float* dev; };
-static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
+static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st,
+                         float* d_mem = nullptr);
 
 // ---- GatherFeatureAndLabel (.cu:17-43) at world > 1: the world's rows and labels into the step, by peer-memory stores or one NCCL
 //      group, device to device over NVLink ----
@@ -978,6 +1008,7 @@ static int begin_step(npair_ctx* c, const StepRows& in, const float** anchors, c
   const bool gathered = in.db == DB_GATHERED;
   const long long r0 = gathered ? static_cast<long long>(c->rank) * c->Q : 0;   // the rank's rows among the gathered ones
   c->step = npair_ctx::Step{};
+  c->step.memory = in.db == DB_MEMORY;
   c->step.label = in.label + r0;
   const float* x = in.x + r0 * c->D;
   if (c->cfg.normalize_input) {               // the layer works on x / ||x|| (1 / ||x|| kept for the rank's rows)
@@ -1288,12 +1319,15 @@ static int forward_impl(npair_ctx* c, const float* d_feat, TopsBlock* tops, cuda
   return NPAIR_OK;
 }
 
-static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st);
-// Backward_gpu (+ the projection of the fused L2Normalize producer: the kernels produce d loss / d y, the caller gets d loss / d x)
-static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
-  if (!c->cfg.normalize_input) return backward_core(c, lw, d_diff, d_total_ext, d_rs_ext, st);
+static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st,
+                         float* d_mem);
+// Backward_gpu (+ the projection of the fused L2Normalize producer: the kernels produce d loss / d y, the caller gets d loss / d x).
+// d_mem: npair_backward_memory's memory-row gradient, with respect to the memory rows as the caller passed them (never normalised)
+static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st,
+                         float* d_mem) {
+  if (!c->cfg.normalize_input) return backward_core(c, lw, d_diff, d_total_ext, d_rs_ext, st, d_mem);
   if (d_total_ext) { c->err = "normalize_input: the partial (pre-all-reduce) backward is not available, its sum over ranks would have to be projected"; return NPAIR_E_STATE; }
-  const int rc = backward_core(c, lw, c->dY, nullptr, d_rs_ext, st);
+  const int rc = backward_core(c, lw, c->dY, nullptr, d_rs_ext, st, d_mem);
   if (rc != NPAIR_OK) return rc;
   PhaseTimer pt(c, 5, st);
   launch_l2norm_bwd(c->Ynorm, c->inv_norm, c->dY, c->Q, c->D, d_diff, st);
@@ -1303,19 +1337,28 @@ static int backward_impl(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
 int npair_bwd_exchange_mode(const npair_ctx* c) { return c ? c->bwd_mode : NPAIR_E_ARG; }
 
 // What a backward continues: the rank's step with the library's own exchange at world > 1, the external collectives' partial sums
-// (npair_backward_partial), or the world's row records the caller gathered (npair_backward_gathered)
-enum BackwardKind { BWD_OWN, BWD_PARTIAL, BWD_GATHERED };
+// (npair_backward_partial), the world's row records the caller gathered (npair_backward_gathered), or a memory step's with the memory
+// rows' gradient (npair_backward_memory)
+enum BackwardKind { BWD_OWN, BWD_PARTIAL, BWD_GATHERED, BWD_MEMORY };
 
 // Every backward entry after its null-pointer check: the preconditions, then the backward.  lw.dev: the asynchronous call.  d_total:
-// npair_backward_partial's addend of the all-reduce (world > 1); d_rs: npair_backward_gathered's N row records.
+// npair_backward_partial's addend of the all-reduce (world > 1); d_rs: npair_backward_gathered's N row records; d_mem:
+// npair_backward_memory's memory-row gradient.
 static int backward_call(npair_ctx* c, const char* name, BackwardKind kind, LossWeight lw, float* d_diff, float* d_total,
-                         const RowRecord* d_rs, void* stream) {
+                         const RowRecord* d_rs, void* stream, float* d_mem = nullptr) {
   int rc;
   bool captured = false;
   if (lw.dev && (rc = async_entry(c, stream, name, &captured)) != NPAIR_OK) return rc;
   if ((rc = check_out_aligned(c, d_diff, kind == BWD_PARTIAL ? "d_local_half" : "the gradient pointer")) != NPAIR_OK) return rc;
   if ((rc = check_out_aligned(c, d_total, "d_total_half")) != NPAIR_OK) return rc;
+  if (kind == BWD_MEMORY && (rc = check_out_aligned(c, d_mem, "d_mem_diff")) != NPAIR_OK) return rc;
   if ((rc = need_forward(c, name)) != NPAIR_OK) return rc;
+  if (kind == BWD_MEMORY) {
+    // after a memory forward (world 1, tensor cores) only NPAIR_FLAG_NO_FUSED_GRAD leaves a context without the fused kernel
+    if (!c->step.memory) { c->err = fmt("%s: the last forward was not npair_forward_memory(_async)", name); return NPAIR_E_STATE; }
+    if (c->ring) { c->err = fmt("%s: the memory rows of a ring context are its detached slots (npair_create_memory_ring)", name); return NPAIR_E_STATE; }
+    if (!c->fused_grad) { c->err = fmt("%s runs on the fused gradient kernel: NPAIR_FLAG_NO_FUSED_GRAD is set", name); return NPAIR_E_ARG; }
+  }
   if (kind == BWD_OWN && (rc = need_comm(c, "npair_backward_partial / npair_backward_gathered")) != NPAIR_OK) return rc;
   if (kind == BWD_PARTIAL && c->bwd_mode == NPAIR_BWDMODE_ROW_SCALARS) {
     c->err = "this context exchanges row scalars: use npair_row_scalars + npair_backward_gathered"; return NPAIR_E_STATE;
@@ -1325,7 +1368,7 @@ static int backward_call(npair_ctx* c, const char* name, BackwardKind kind, Loss
   }
   OrderedCall call(c, stream, captured);
   if ((rc = call.enter()) != NPAIR_OK) return rc;
-  return backward_impl(c, lw, d_diff, d_total, d_rs, call.st);
+  return backward_impl(c, lw, d_diff, d_total, d_rs, call.st, d_mem);
 }
 
 int npair_backward(npair_ctx* c, float loss_weight, float* d_diff, void* stream) {
@@ -1338,6 +1381,19 @@ int npair_backward_device_weight(npair_ctx* c, const float* d_loss_weight, float
   if (!c) return NPAIR_E_ARG;
   if (!d_loss_weight || !d_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
   return backward_call(c, "npair_backward_device_weight", BWD_OWN, LossWeight{0.f, d_loss_weight}, d_diff, nullptr, nullptr, stream);
+}
+
+// The backward of a memory step with the memory rows' gradient too (DESIGN 4.6)
+int npair_backward_memory(npair_ctx* c, float loss_weight, float* d_diff, float* d_mem_diff, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_diff || !d_mem_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  return backward_call(c, "npair_backward_memory", BWD_MEMORY, LossWeight{loss_weight, nullptr}, d_diff, nullptr, nullptr, stream, d_mem_diff);
+}
+int npair_backward_memory_device_weight(npair_ctx* c, const float* d_loss_weight, float* d_diff, float* d_mem_diff, void* stream) {
+  if (!c) return NPAIR_E_ARG;
+  if (!d_loss_weight || !d_diff || !d_mem_diff) { c->err = "null pointer argument"; return NPAIR_E_ARG; }
+  return backward_call(c, "npair_backward_memory_device_weight", BWD_MEMORY, LossWeight{0.f, d_loss_weight}, d_diff, nullptr, nullptr, stream,
+                       d_mem_diff);
 }
 
 /* External-collectives variant of Backward_gpu up to the all-reduce (.cu:420-460):
@@ -1410,7 +1466,8 @@ static int column_records(npair_ctx* c, const RowRecord* d_rs_ext, const RowReco
   }
   return NPAIR_OK;
 }
-static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st) {
+static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_total_ext, const RowRecord* d_rs_ext, cudaStream_t st,
+                         float* d_mem) {
   const int Q = c->Q, N = c->N, D = c->D;
   const MiningParams mp = mining_of(c->cfg);
   // loss_weight / dot_normalizer (.cu:427,448); world scope: the normaliser is the world's batch and the transposed term is not
@@ -1446,17 +1503,31 @@ static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
     // per block of rows of S, starting with the one the forward left in the buffer (a materialised S is the one block): recompute it,
     // then its gradient rows.  The split-K and the chunk key come from the rank's Q rows and 128-row tile indices, so every output
     // bit is the materialised path's
-    PhaseTimer pt(c, 6, st);
-    const int first = c->s_block_row0 >= 0 ? c->s_block_row0 / c->s_rows : 0;
-    for (int k = 0; k < c->n_blocks; ++k) {
-      const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
-      CUDA_TRY(c, recompute_sim_block(c, r0, st));
-      // the fused kernel's rows start at the block: its record, self column and output rows are those of rank row sim.row0
-      const SimRows sim = sim_rows(c, r0, rows);
-      fp.Q = sim.rows; fp.ts = tile_sched(sim.rows, D, c->grad_kblocks, c->grad_split); fp.m_blk0 = sim.row0 / TileShape::BM;
-      fp.rowrec = c->ra.rowrec + sim.row0; fp.self_offset = sim.self_col(sim.row0); fp.out = d_diff + static_cast<long long>(sim.row0) * D;
-      CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
-      if (fp.ts.splits > 1) reduce_splits(c, fp.ts.splits, rows, fp.out, 0.f, st);
+    {
+      PhaseTimer pt(c, 6, st);
+      const int first = c->s_block_row0 >= 0 ? c->s_block_row0 / c->s_rows : 0;
+      for (int k = 0; k < c->n_blocks; ++k) {
+        const int r0 = (first + k) % c->n_blocks * c->s_rows, rows = Q - r0 < c->s_rows ? Q - r0 : c->s_rows;
+        CUDA_TRY(c, recompute_sim_block(c, r0, st));
+        // the fused kernel's rows start at the block: its record, self column and output rows are those of rank row sim.row0
+        const SimRows sim = sim_rows(c, r0, rows);
+        fp.Q = sim.rows; fp.ts = tile_sched(sim.rows, D, c->grad_kblocks, c->grad_split); fp.m_blk0 = sim.row0 / TileShape::BM;
+        fp.rowrec = c->ra.rowrec + sim.row0; fp.self_offset = sim.self_col(sim.row0); fp.out = d_diff + static_cast<long long>(sim.row0) * D;
+        CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_fB, c->tm_fS, fp, c->sms, st));
+        if (fp.ts.splits > 1) reduce_splits(c, fp.ts.splits, rows, fp.out, 0.f, st);
+      }
+    }
+    if (d_mem && N > Q) {
+      // the memory rows' gradient (1/2)(lw/Q) G[:, Q:]^T . x (DESIGN 4.6), with the anchors' alpha and scale: the kernel over the
+      // transposed S (S is materialised whole in a memory step), the memory rows' records as row records -- their own term is 0 -- and
+      // the anchors' as column records, whose transposed term at world 1 is G[anchor][Q + p] exactly.  Self columns lie past K.
+      PhaseTimer pt(c, 7, st);
+      const int m = N - Q;
+      fp.Q = m; fp.N = Q; fp.ts = tile_sched(m, D, (Q + 31) / 32, c->mem_grad_split); fp.m_blk0 = 0;
+      fp.rowrec = c->ra.rowrec + Q; fp.colrec = c->ra.rowrec; fp.self_offset = Q; fp.out = d_mem;
+      fp.inv_world = 1.f; fp.log2_world = 0.f;
+      CUDA_TRY(c, launch_fused_grad(c->prec, c->tm_mX, c->tm_S, fp, c->sms, st, true));
+      if (fp.ts.splits > 1) reduce_splits(c, fp.ts.splits, m, d_mem, 0.f, st);
     }
     CUDA_TRY(c, cudaGetLastError());
     return NPAIR_OK;
@@ -1501,7 +1572,8 @@ static int backward_core(npair_ctx* c, LossWeight lw, float* d_diff, float* d_to
 /* Per-phase CUDA-event timing on the caller's stream (bench.py's roofline leg).  Phases:
  * 0 forward all-gather   8 backward exchange (row-scalar all-gather or reduce-scatter)   1 operand prep (asum/absmax, split, stat init)
  * 2 similarity GEMM + fused statistics   3 thresholds + radix selects   4 forward row pass + finalize
- * 5 backward weight builder   6 gradient GEMM (G . X_total)   7 transposed gradient GEMM (G^T . X_local, world > 1) */
+ * 5 backward weight builder   6 gradient GEMM (G . X_total)   7 transposed gradient GEMM (G^T . X_local, world > 1; the memory-row
+ *   gradient of npair_backward_memory) */
 int npair_profile_enable(npair_ctx* c, int on) {
   if (!c) return NPAIR_E_ARG;
   CUDA_TRY(c, cudaSetDevice(c->device));

@@ -56,14 +56,17 @@ cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorM
   return cudaGetLastError();
 }
 
-FusedKernel fused_kernel(int prec) {
-  return with_prec(prec, [](auto P) {
+// trans_s: the variant over the transposed S tile (the memory-row gradient, grad_fused.cuh)
+FusedKernel fused_kernel(int prec, bool trans_s) {
+  return with_prec(prec, [trans_s](auto P) {
     constexpr SplitFormat f = SPLIT_FORMATS[P];
-    return FusedKernel{fused_grad_kernel<f.pieces, f.bf16>, FusedCfg<f.pieces>::THREADS, FusedCfg<f.pieces>::SMEM_BYTES};
+    return trans_s ? FusedKernel{fused_grad_kernel<f.pieces, f.bf16, true>, FusedCfg<f.pieces, true>::THREADS, FusedCfg<f.pieces, true>::SMEM_BYTES}
+                   : FusedKernel{fused_grad_kernel<f.pieces, f.bf16>, FusedCfg<f.pieces>::THREADS, FusedCfg<f.pieces>::SMEM_BYTES};
   });
 }
-cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st) {
-  const FusedKernel k = fused_kernel(prec);
+cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st,
+                              bool trans_s) {
+  const FusedKernel k = fused_kernel(prec, trans_s);
   k.fn<<<gemm_grid(p.ts, sms), k.threads, k.smem, st>>>(b, sm, p);
   count_launch();
   return cudaGetLastError();

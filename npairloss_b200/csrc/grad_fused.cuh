@@ -9,6 +9,9 @@
 // Requires a bitwise symmetric S (EPI_SYM tiles at world == 1, role-symmetric similarity instructions across ranks).
 // Chunked accumulation: the fp32 accumulator drifts over long K (K = database size), so the K range is cut into chunks of
 // `chunk_kb` K blocks, each accumulated from zero and added to the output in fp32 round-to-nearest by the same thread.
+// TRANS_S (the memory-row gradient of a cross-batch memory step, DESIGN 4.6): the output rows are database columns N .. N + Q - 1 of S
+// and K runs over S's rows, so a stage takes S[m0 .. m0+31][N + row0 .. N + row0 + 127], the transpose of the usual tile, as 32 x 32
+// boxes; with the memory rows' records as row records and the anchors' as column records, each weight is G[anchor][column].
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -48,11 +51,14 @@ struct FusedGradParams {
                                 // accumulation-chunk key uses it; rowrec / out / self_offset are passed already offset
 };
 
-template <int NSPLIT>
+template <int NSPLIT, bool TRANS_S = false>
 struct FusedCfg {
   static constexpr int BM = 128, BN = 256, BK = 32;
   static constexpr int B_PIECE = BN * 64;                 // 64-byte rows (32 x 2-byte), SWIZZLE_64B
-  static constexpr int S_TILE = BM * 128;                 // 128-byte rows (32 x fp32), SWIZZLE_128B
+  // TRANS_S: the transposed tile's 32 x 32 fp32 boxes start at a 16-byte aligned column, N rounded down to a multiple of 4, so its
+  // 128 columns take five boxes (the stage counts stay those of the usual tile's 128-byte rows)
+  static constexpr int S_BOX = 32 * 128;
+  static constexpr int S_TILE = TRANS_S ? 5 * S_BOX : BM * 128;   // 128-byte rows (32 x fp32), SWIZZLE_128B
   static constexpr int CREC = BK * sizeof(RowRecord);     // the K block's column records
   static constexpr int STAGE_BYTES = NSPLIT * B_PIECE + S_TILE + CREC;
   static constexpr int NPASS = mma_passes(NSPLIT);
@@ -169,10 +175,10 @@ __device__ __forceinline__ RowRec load_rowrec(const FusedGradParams& p, int row)
   return r;
 }
 
-template <int NSPLIT, bool BF16>
+template <int NSPLIT, bool BF16, bool TRANS_S = false>
 __global__ void __launch_bounds__(384, 1)
 fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_constant__ CUtensorMap tmapS, const FusedGradParams p) {
-  using Cfg = FusedCfg<NSPLIT>;
+  using Cfg = FusedCfg<NSPLIT, TRANS_S>;
   const int worker = static_cast<int>(blockIdx.x), num_workers = static_cast<int>(gridDim.x);
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -205,7 +211,15 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s)
             ptx::tma_load_3d(st + s * Cfg::B_PIECE, &tmapB, full, m0, t.n_blk * BN, s);
-          ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE, &tmapS, full, m0, t.m_blk * BM);
+          if (TRANS_S) {
+            // the offset N goes into the column coordinate, not the map's base pointer (which TMA needs 16-byte aligned), rounded down to
+            // a 16-byte aligned column; the build adds the remainder N & 3
+#pragma unroll
+            for (int b = 0; b < Cfg::S_TILE / Cfg::S_BOX; ++b)
+              ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE + b * Cfg::S_BOX, &tmapS, full, (p.N & ~3) + t.m_blk * BM + 32 * b, m0);
+          } else {
+            ptx::tma_load_2d(st + NSPLIT * Cfg::B_PIECE, &tmapS, full, m0, t.m_blk * BM);
+          }
           bulk_copy_g2s(st + NSPLIT * Cfg::B_PIECE + Cfg::S_TILE, p.colrec + m0, crec_bytes, full);
           ring.advance();
         }
@@ -247,7 +261,18 @@ fused_grad_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_consta
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int rl = rl0 + 8 * h;
-          s2[t][h] = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
+          if (TRANS_S) {
+            // window column c = rl + (N & 3): box c / 32, row k (and k + 1), column c % 32.  A load's 32 lanes read 8 consecutive columns
+            // for each of four rows k whose k & 7 are the four values of one parity: two lanes of one bank would need columns 4 apart,
+            // one 16-byte chunk apart, whose chunk indices differ in bit 0, which XOR with k & 7 values of one parity cannot undo
+            const int c = rl + (p.N & 3);
+            const uint8_t* box = s_tile + (c >> 5) * Cfg::S_BOX;
+            const int ch = (c & 31) >> 2;
+            s2[t][h].x = *reinterpret_cast<const float*>(box + k * 128 + ((ch ^ (k & 7)) << 4) + (c & 3) * 4);
+            s2[t][h].y = *reinterpret_cast<const float*>(box + (k + 1) * 128 + ((ch ^ ((k + 1) & 7)) << 4) + (c & 3) * 4);
+          } else {
+            s2[t][h] = *reinterpret_cast<const float2*>(s_tile + rl * 128 + (((k >> 2) ^ (rl & 7)) << 4) + (k & 3) * 4);
+          }
         }
       }
       float4 lo[2][2];                            // first record halves {m2c, thr_n, m2, label} of columns m, m + 1 of t = 0, 1

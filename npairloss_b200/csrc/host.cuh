@@ -51,8 +51,9 @@ cudaError_t allow_smem(const K& k) {
 }
 GemmKernel gemm_kernel(int prec, int epi);
 cudaError_t launch_gemm(int prec, int epi, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& sm, const GemmParams& p, int sms, cudaStream_t st);
-FusedKernel fused_kernel(int prec);
-cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st);
+FusedKernel fused_kernel(int prec, bool trans_s = false);
+cudaError_t launch_fused_grad(int prec, const CUtensorMap& b, const CUtensorMap& sm, const FusedGradParams& p, int sms, cudaStream_t st,
+                              bool trans_s = false);
 cudaError_t launch_simt_gemm(int prec, int epi, const uint16_t* A, long long lda, long long psA, const uint16_t* B, long long ldb,
                              long long psB, int K, const GemmParams& p, cudaStream_t st);
 __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, long long n, float* __restrict__ out, float beta);

@@ -39,6 +39,16 @@ third output, the unweighted per-anchor losses -log(A_i / T_i) (not differentiab
 grad_loss * row_loss_i / Z (the analytic one, whatever true_gradient says).  Works with blocking=False and graph capture (w is then a
 static input like the embeddings), memory_rows, normalize_input and world > 1.  A weight outside [0, 1] or NaN makes the blocking
 forward raise capi.NpairError (E_ARG) and the asynchronous one give NaN tops, reported by async_status().
+
+EXTRA ROWS.  loss_fn(x, labels, extra_rows=y, extra_labels=l) adds the m rows of y (CUDA fp32 [m, D], used as given: normalise them
+first) to the database as non-anchor columns (npair_forward_memory, DESIGN 4.3): every anchor is mined and scored against them too.
+When y requires grad, autograd receives its gradient (npair_backward_memory, DESIGN 4.6), so learnable class proxies (Proxy-NCA style:
+one row per class, labels arange(C)) or a second encoder's rows train through the layer; true_gradient=True doubles it as it does the
+embeddings' gradient.  Works with blocking=False and graph capture (y is a static input like the embeddings, m fixed per graph),
+anchor_weight / row_losses and normalize_input (which normalises x only).  Not with memory_rows > 0 (both would fill the memory
+columns), at world > 1, with global_scope, row-block mode or the SIMT backend (ValueError), nor, when y requires grad, with
+FLAG_NO_FUSED_GRAD.  The context is then a memory context whose capacity grows to the largest m seen; later calls without extra rows
+run on it as plain forwards.
 """
 from __future__ import annotations
 
@@ -67,8 +77,9 @@ def _fp32_labels(label):
 
 class _NPairFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, feat, label, weight, owner, want_rows):
-        layer = owner._context(feat)
+    def forward(ctx, feat, label, weight, extra, extra_label, owner, want_rows):
+        m = 0 if extra is None else extra.shape[0]
+        layer = owner._context(feat, m)
         rl = None
         if want_rows or ctx.needs_input_grad[2]:              # the weights' gradient is made of the per-anchor losses
             rl = torch.empty(feat.shape[0], dtype=torch.float32, device=feat.device)
@@ -85,6 +96,8 @@ class _NPairFunction(torch.autograd.Function):
             elif owner._blocking:
                 if owner._mem_cap:
                     tops = owner._forward_memory(layer, feat, label)
+                elif extra is not None:
+                    tops = layer.forward_memory(feat, label, extra, extra_label, m)
                 else:
                     tops = layer.forward(feat, label)         # blocks until the five scalars are on the host (as the reference)
                 t = torch.tensor(tops, dtype=torch.float32, device=feat.device)
@@ -92,6 +105,8 @@ class _NPairFunction(torch.autograd.Function):
                 t = torch.empty(5, dtype=torch.float32, device=feat.device)   # under capture: from the graph's pool
                 if owner._mem_cap:
                     owner._forward_memory(layer, feat, label, t)
+                elif extra is not None:
+                    layer.forward_memory_async(feat, label, extra, extra_label, m, t)
                 else:
                     layer.forward_async(feat, label, t)
         finally:
@@ -101,6 +116,7 @@ class _NPairFunction(torch.autograd.Function):
         ctx.owner, ctx.layer, ctx.generation = owner, layer, owner._generation
         ctx.save_for_backward(feat, label)                    # the C ABI wants both unchanged until the backward is enqueued
         ctx.row_loss = rl
+        ctx.extra_shape = None if extra is None else tuple(extra.shape)
         ctx.norm = feat.shape[0] * (owner._world if owner._config.get("global_scope") else 1)   # Z: Q, or N in world scope
         if want_rows:
             ctx.mark_non_differentiable(t, rl)
@@ -115,17 +131,30 @@ class _NPairFunction(torch.autograd.Function):
                                "context holds the newer batch.  Use one NPairLoss module per outstanding graph.")
         feat, _label = ctx.saved_tensors
         diff = torch.empty_like(feat)
+        mem_diff = None
+        if ctx.needs_input_grad[3]:                           # the extra rows' gradient: npair_backward_memory
+            mem_diff = torch.empty(ctx.extra_shape, dtype=torch.float32, device=feat.device)
+        with_mem = mem_diff is not None and mem_diff.numel() > 0
         if ctx.owner._blocking:
             # the reference scales by top[0]->cpu_diff()[0] (.cu:435): a host scalar, hence the .item()
-            ctx.layer.backward(float(grad_loss.item()), diff)
+            if with_mem:
+                ctx.layer.backward_memory(float(grad_loss.item()), diff, mem_diff)
+            else:
+                ctx.layer.backward(float(grad_loss.item()), diff)
         else:
-            ctx.layer.backward_device_weight(grad_loss.detach().to(torch.float32).contiguous().reshape(1), diff)
+            lw = grad_loss.detach().to(torch.float32).contiguous().reshape(1)
+            if with_mem:
+                ctx.layer.backward_memory_device_weight(lw, diff, mem_diff)
+            else:
+                ctx.layer.backward_device_weight(lw, diff)
         if ctx.owner._true_gradient:
             diff.mul_(2.0)
+            if with_mem:
+                mem_diff.mul_(2.0)
         grad_w = None
         if ctx.needs_input_grad[2]:                           # d loss / d w_i = row_loss_i / Z
             grad_w = grad_loss.to(torch.float32) * ctx.row_loss / ctx.norm
-        return diff, None, grad_w, None, None
+        return diff, None, grad_w, mem_diff, None, None, None
 
 
 class NPairLoss(torch.nn.Module):
@@ -166,8 +195,9 @@ class NPairLoss(torch.nn.Module):
             self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._mem_cap, ring=True)
         elif self._mem_cap:
             self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._mem_cap)
-        else:
-            self._factory = lambda cfg, nid: capi.Context(cfg, nid)
+        else:   # extra_rows: a memory context of the largest m seen
+            self._factory = lambda cfg, nid: capi.Context(cfg, nid, memory_rows=self._extra_cap)
+        self._extra_cap = 0
         self._ctx, self._key = None, None
         self._generation = 0
         self._true_gradient = bool(true_gradient)
@@ -256,10 +286,12 @@ class NPairLoss(torch.nn.Module):
                     f"are missing; run {-(-left // q)} more eager step(s) of {q} rows first")
         return None
 
-    def _context(self, feat):
+    def _context(self, feat, extra_m=0):
         q, d = feat.shape[0], feat[0].numel()
         key = (q, d, feat.device.index)
-        if key != self._key:
+        grow = extra_m > self._extra_cap
+        self._extra_cap = max(self._extra_cap, extra_m)
+        if key != self._key or grow:
             old, old_key = self._ctx, self._key
             cfg = capi.make_config(q, d, world=self._world, rank=self._rank, device=feat.device.index or 0, **self._config)
             # the new context is created BEFORE the old one is closed: contexts made with the same NCCL id share one
@@ -278,11 +310,13 @@ class NPairLoss(torch.nn.Module):
                 old.close()
         return self._ctx
 
-    def forward(self, feat, label, anchor_weight=None, row_losses=False):
+    def forward(self, feat, label, anchor_weight=None, row_losses=False, extra_rows=None, extra_labels=None):
         """(loss, tops), or (loss, tops, row_loss) with row_losses=True; anchor_weight: None or Q fp32 weights in [0, 1] on feat's
-        device (ANCHOR WEIGHTS in the module docstring)."""
+        device (ANCHOR WEIGHTS in the module docstring); extra_rows / extra_labels: None or [m, D] fp32 rows and their m labels on feat's
+        device (EXTRA ROWS in the module docstring)."""
         if feat.dtype != torch.float32:
             raise TypeError("NPairLoss computes in fp32 like the reference (Dtype=float); cast the embeddings")
+        extra_rows, extra_labels = self._extra(feat, extra_rows, extra_labels)
         if anchor_weight is not None:
             if not isinstance(anchor_weight, torch.Tensor) or anchor_weight.dtype != torch.float32:
                 raise TypeError("anchor_weight must be a float32 tensor (weights in [0, 1], one per row of the batch)")
@@ -300,7 +334,36 @@ class NPairLoss(torch.nn.Module):
                                "and count are Python state that the graph would freeze")
         feat2 = feat.reshape(feat.shape[0], -1).contiguous()
         label = _fp32_labels(label).contiguous()               # labels are stored as Dtype in the reference (bottom[1])
-        return _NPairFunction.apply(feat2, label, anchor_weight, self, bool(row_losses))
+        return _NPairFunction.apply(feat2, label, anchor_weight, extra_rows, extra_labels, self, bool(row_losses))
+
+    def _extra(self, feat, rows, labels):
+        """The extra rows and their fp32 labels as the library takes them, after the checks of EXTRA ROWS (module docstring)."""
+        if rows is None and labels is None:
+            return None, None
+        if rows is None or labels is None:
+            raise ValueError("extra_rows and extra_labels go together")
+        if self._mem_cap:
+            raise ValueError("extra_rows cannot be combined with memory_rows > 0: both would be the step's memory columns")
+        if self._world != 1:
+            raise ValueError("extra_rows are defined for world = 1 (a cross-batch memory step is a world-1 step)")
+        cfg = self._config
+        flags = int(cfg.get("flags", 0))
+        if cfg.get("global_scope") or cfg.get("sim_block_rows") or (flags >> capi.SIM_BLOCK_SHIFT) & capi.SIM_BLOCK_MAX_UNITS \
+                or cfg.get("gemm_backend", capi.GEMM_TCGEN05) != capi.GEMM_TCGEN05:
+            raise ValueError("extra_rows run a cross-batch memory step, which needs the tensor-core backend and supports neither "
+                             "global_scope nor row-block similarity mode (sim_block_rows)")
+        if flags & capi.FLAG_NO_FUSED_GRAD and isinstance(rows, torch.Tensor) and rows.requires_grad:
+            raise ValueError("the gradient of extra_rows runs on the fused gradient kernel: drop FLAG_NO_FUSED_GRAD from flags")
+        if not isinstance(rows, torch.Tensor) or rows.dtype != torch.float32:
+            raise TypeError("extra_rows must be a float32 tensor [m, D]")
+        d = feat[0].numel() if feat.dim() else 0
+        if rows.dim() != 2 or rows.shape[1] != d:
+            raise ValueError(f"extra_rows must have shape [m, {d}] (the embeddings' dimension), got {list(rows.shape)}")
+        if not isinstance(labels, torch.Tensor) or labels.dim() != 1 or labels.shape[0] != rows.shape[0]:
+            raise ValueError(f"extra_labels must be a tensor of shape [{rows.shape[0]}] (one label per extra row)")
+        if rows.device != feat.device or labels.device != feat.device:
+            raise ValueError("extra_rows and extra_labels must be on the embeddings' device")
+        return rows.contiguous(), _fp32_labels(labels).contiguous()
 
 
 def recall_at_k(query, qlabel, gallery=None, glabel=None, ks=(1, 2, 4, 8), precision=capi.PREC_FP32_FP16X2, self_offset=None):
