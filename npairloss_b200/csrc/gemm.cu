@@ -1,8 +1,13 @@
 // gemm.cu -- the one unit that instantiates the GEMM kernels: the wgmma similarity and gradient GEMMs (gemm_wgmma.cuh), the fused
-// gradient GEMM (grad_fused.cuh), the SIMT cross-check GEMM and the split-K reduce, with their launchers (declared in host.cuh).
+// gradient GEMM (grad_fused.cuh), the SIMT cross-check GEMM and the split-K reduce, with their launchers and the builders of the TMA
+// maps they take (declared in host.cuh).
+#include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <cudaTypedefs.h>
+
+#include <string>
 
 #include "gemm_wgmma.cuh"
 #include "grad_fused.cuh"
@@ -10,6 +15,74 @@
 #include "kernels.cuh"
 
 namespace npair {
+
+// ------------------------------------------------------------------------------------------------ TMA maps
+static PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
+  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
+  }
+  return fn;
+}
+
+// 3-D map over NSPLIT stacked 2-byte matrices [piece][rows][ld]; inner extent `cols` (<= ld), box {bk, box_rows, 1}
+bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int pieces, long long ld_elems,
+                      long long piece_stride_elems, int bk, int box_rows, std::string* err) {
+  auto fn = tmap_encode_fn();
+  if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
+  cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(pieces)};
+  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld_elems) * 2ull, static_cast<cuuint64_t>(piece_stride_elems) * 2ull};
+  cuuint32_t box[3] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(box_rows), 1u};
+  cuuint32_t estr[3] = {1u, 1u, 1u};
+  const CUtensorMapSwizzle sw = (bk * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *err = fmt("cuTensorMapEncodeTiled failed (%d): cols=%d rows=%d pieces=%d ld=%lld", (int)r, cols, rows, pieces, ld_elems); return false; }
+  return true;
+}
+
+// 4-D map over one side of the similarity GEMM's pieced operands (SimLayout, pieces >= 2): {8 * bk elements, pieces, K blocks, row
+// groups}, box {8 * bk, pieces, 1, box_rows / 8}, no swizzle -- a stage receives [row group][slot][bk / 8 core matrices]
+static bool make_tmap_sim_side(CUtensorMap* m, const void* base, int rows, SimLayout L, int box_rows, std::string* err) {
+  auto fn = tmap_encode_fn();
+  if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
+  const cuuint64_t blk = 8ull * L.bk(), kbs = static_cast<cuuint64_t>(L.Dp / L.bk());
+  cuuint64_t dims[4] = {blk, static_cast<cuuint64_t>(L.pieces), kbs, static_cast<cuuint64_t>(L.padded_rows(rows) / 8)};
+  cuuint64_t strides[3] = {blk * 2ull, blk * 2ull * L.pieces, blk * 2ull * L.pieces * kbs};
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(blk), static_cast<cuuint32_t>(L.pieces), 1u, static_cast<cuuint32_t>(box_rows / 8)};
+  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *err = fmt("cuTensorMapEncodeTiled(sim) failed (%d): rows=%d pieces=%d Dp=%lld", (int)r, rows, L.pieces, L.Dp); return false; }
+  return true;
+}
+
+// The similarity GEMM's operand maps (SimLayout L, written by split_kernel / eval_split_kernel): `a` over rows_a rows from A (128-row
+// boxes), `b` over rows_b rows from B (256-row boxes), both in the layout's K blocks
+bool make_tmap_sim(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, SimLayout L,
+                   std::string* err) {
+  if (L.pieces == 1)
+    return make_tmap_pieces(a, A, static_cast<int>(L.Dp), rows_a, 1, L.Dp, rows_a * L.Dp, L.bk(), 128, err) &&
+           make_tmap_pieces(b, B, static_cast<int>(L.Dp), rows_b, 1, L.Dp, rows_b * L.Dp, L.bk(), 256, err);
+  return make_tmap_sim_side(a, A, rows_a, L, 128, err) && make_tmap_sim_side(b, B, rows_b, L, 256, err);
+}
+
+// 2-D fp32 map over the similarity matrix [rows x ld], inner extent `cols`, box {32, 32}, 128B swizzle (TMA stores)
+bool make_tmap_f32_store(CUtensorMap* m, const void* base, int cols, int rows, long long ld_elems, std::string* err, int box_rows) {
+  auto fn = tmap_encode_fn();
+  if (!fn) { *err = "cuTensorMapEncodeTiled entry point not available"; return false; }
+  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld_elems) * 4ull};
+  cuuint32_t box[2] = {32u, static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t estr[2] = {1u, 1u};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { *err = fmt("cuTensorMapEncodeTiled(S) failed (%d): cols=%d rows=%d ld=%lld", (int)r, cols, rows, ld_elems); return false; }
+  return true;
+}
 
 // ------------------------------------------------------------------------------------------------ GEMM launchers
 static int gemm_grid(const TileSched& ts, int sms) { return ts.num_tiles() < sms ? ts.num_tiles() : sms; }   // one CTA per tile, at most one per SM

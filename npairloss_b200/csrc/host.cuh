@@ -1,5 +1,5 @@
-// host.cuh -- host plumbing of the layer context (ctx.cu), the retrieval evaluator (eval.cu) and the GEMM launchers (gemm.cu).
-// What the header defines is inline or a template; process state (the create error, the caches) has one definition, in ctx.cu.
+// host.cuh -- host plumbing of the layer context (ctx.cu, step.cu), the retrieval evaluator (eval.cu) and the GEMM launchers (gemm.cu).
+// What the header defines is inline or a template; process state (the create error, the caches) has one definition, in a .cu unit.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -27,7 +27,7 @@ inline std::string fmt(const char* f, ...) {
   return std::string(buf);
 }
 
-// ------------------------------------------------------------------------------------------------ TMA maps (ctx.cu)
+// ------------------------------------------------------------------------------------------------ TMA maps (gemm.cu)
 bool make_tmap_pieces(CUtensorMap* m, const void* base, int cols, int rows, int pieces, long long ld_elems, long long piece_stride_elems,
                       int bk, int box_rows, std::string* err);
 bool make_tmap_sim(CUtensorMap* a, CUtensorMap* b, const uint16_t* A, int rows_a, const uint16_t* B, int rows_b, SimLayout L,
