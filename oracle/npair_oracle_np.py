@@ -40,13 +40,27 @@ def _thr_from_sorted(sorted_list: np.ndarray, sn: float) -> np.float32:
     return v if v >= 0 else -FLT_MAX  # .cu:288
 
 
+def weighted_loss(logv, w, Z):
+    """-(1/Z) sum_i w_i logv_i: the fp32 products w_i logv_i summed in fp64 (w None: the unweighted loss, DESIGN 4.5)."""
+    lv = np.asarray(logv, dtype=np.float32)
+    if w is not None:                                         # a row with w = 0 adds nothing, whatever its log value
+        w = np.asarray(w, dtype=np.float32)
+        with np.errstate(invalid="ignore"):
+            lv = np.where(w == 0, np.float32(0), lv * w).astype(np.float32)
+    return np.float32(np.float32(lv.astype(np.float64).sum()) / np.float32(-Z))
+
+
 def forward(x_total, label_total, Q, world=1, rank=0, num_tops=5, margin_ident=0.0, margin_diff=0.0,
             identsn=-1.0, diffsn=-1.0, ap_region=LOCAL, ap_method=RAND, an_region=LOCAL, an_method=RAND,
-            S_inject=None):
+            S_inject=None, anchor_weight=None):
+    """Rank `rank`'s forward over the database x_total: (tops[5], state).  Rows past Q * world are memory rows (DESIGN 4.3), columns
+    and never anchors, at world 1 only.  anchor_weight: the rank's Q weights, which change tops[0] alone (DESIGN 4.5)."""
     x_total = np.ascontiguousarray(x_total, dtype=np.float32)
     lab = np.ascontiguousarray(label_total, dtype=np.float32)
-    N = Q * world
-    assert x_total.shape[0] == N and lab.shape[0] == N
+    N = x_total.shape[0]
+    assert N >= Q * world and lab.shape[0] == N
+    if N > Q * world and world > 1:
+        raise OracleError("memory rows at world > 1")
     xl = x_total[rank * Q:(rank + 1) * Q]
     ll = lab[rank * Q:(rank + 1) * Q]
     # .cu:218 (BLAS accumulation order unspecified -> float64 accumulate, fp32 store)
@@ -113,9 +127,8 @@ def forward(x_total, label_total, Q, world=1, rank=0, num_tops=5, margin_ident=0
     T = (A + B).astype(np.float32)
     with np.errstate(divide="ignore", invalid="ignore"):
         logv = np.where((A == 0) | (T == 0), np.float32(0), np.log((A / T).astype(np.float32))).astype(np.float32)
-    loss = np.float32(np.float32(logv.astype(np.float64).sum()) / np.float32(-Q))
     tops = np.zeros(5, dtype=np.float32)
-    tops[0] = loss
+    tops[0] = weighted_loss(logv, anchor_weight, Q)
     # .cu:173-206, :390-398
     klist = [1, 5, 10, 15]
     for t in range(max(0, num_tops - 2)):
@@ -148,19 +161,34 @@ def grad_weights(state, Q, loss_weight=1.0):
     return (np.float64(np.float32(loss_weight) / np.float32(Q))) * (-W1 + W2 + W3)
 
 
-def step_world(x_total, label_total, Q, world, loss_weight=1.0, S_inject_all=None, **kw):
-    """Emulated multi-rank fwd+bwd: returns (tops[world,5], dX[N,D])."""
+def step_world_fp64(x_total, label_total, Q, world, loss_weight=1.0, S_inject_all=None, anchor_weight=None, **kw):
+    """Emulated multi-rank fwd+bwd: (tops[world,5], dX[N,D] in fp64, the ranks' forward states).  anchor_weight: the Q * world
+    anchors' weights, each rank's G scaled by row.  Memory rows (world 1, rows [Q, N)) get the transposed term alone, 1/2 G[:, Q:]^T x
+    (DESIGN 4.6)."""
     x_total = np.ascontiguousarray(x_total, dtype=np.float32)
     N, D = x_total.shape
+    w = None if anchor_weight is None else np.asarray(anchor_weight, dtype=np.float32)
     tops = np.zeros((world, 5), dtype=np.float32)
     local = np.zeros((N, D), dtype=np.float64)
     total = np.zeros((N, D), dtype=np.float64)
     xd = x_total.astype(np.float64)
+    states = []
     for r in range(world):
-        Sin = None if S_inject_all is None else S_inject_all[r * Q:(r + 1) * Q]
-        tops[r], st = forward(x_total, label_total, Q, world, r, S_inject=Sin, **kw)
+        rows = slice(r * Q, (r + 1) * Q)
+        Sin = None if S_inject_all is None else S_inject_all[rows]
+        wr = None if w is None else w[rows]
+        tops[r], st = forward(x_total, label_total, Q, world, r, S_inject=Sin, anchor_weight=wr, **kw)
         G = grad_weights(st, Q, loss_weight)
-        local[r * Q:(r + 1) * Q] = G @ xd                        # .cu:448-453
-        total += G.T @ xd[r * Q:(r + 1) * Q]                     # .cu:455-460 + all-reduce .cu:467
+        if wr is not None:
+            G = G * wr.astype(np.float64)[:, None]
+        local[rows] = G @ xd                                     # .cu:448-453
+        total += G.T @ xd[rows]                                  # .cu:455-460 + all-reduce .cu:467
+        states.append(st)
     dX = 0.5 * (total / world) + 0.5 * local                     # .cu:474, :492-497
+    return tops, dX, states
+
+
+def step_world(x_total, label_total, Q, world, loss_weight=1.0, S_inject_all=None, anchor_weight=None, **kw):
+    """step_world_fp64 with the gradient rounded to fp32: (tops[world,5], dX[N,D])."""
+    tops, dX, _ = step_world_fp64(x_total, label_total, Q, world, loss_weight, S_inject_all, anchor_weight, **kw)
     return tops, dX.astype(np.float32)

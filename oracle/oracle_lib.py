@@ -10,6 +10,8 @@ import subprocess
 
 import numpy as np
 
+from oracle import npair_oracle_np as onp
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
@@ -105,8 +107,9 @@ def forward(x_total, label_total, cfg: NpoConfig, S_inject=None):
     return tops, out
 
 
-def step_world(x_total, label_total, cfg: NpoConfig, loss_weight=1.0, S_inject_all=None, want_grad=True):
-    """Emulated all-rank fwd(+bwd).  Returns (tops[world,5], dX[N,D] or None)."""
+def step_world(x_total, label_total, cfg: NpoConfig, loss_weight=1.0, S_inject_all=None, want_grad=True, anchor_weight=None):
+    """Emulated all-rank fwd(+bwd).  Returns (tops[world,5], dX[N,D] or None).  anchor_weight: the Q * world anchors' weights
+    (DESIGN 4.5), see _weighted_step."""
     L = lib()
     x_total = np.ascontiguousarray(x_total, dtype=np.float32)
     label_total = np.ascontiguousarray(label_total, dtype=np.float32)
@@ -115,6 +118,9 @@ def step_world(x_total, label_total, cfg: NpoConfig, loss_weight=1.0, S_inject_a
     if S_inject_all is not None:
         S_inject_all = np.ascontiguousarray(S_inject_all, dtype=np.float32)
         assert S_inject_all.shape == (N, N)
+    if anchor_weight is not None:
+        tops, dx = _weighted_step(x_total, label_total, cfg, loss_weight, S_inject_all, anchor_weight)
+        return tops, dx if want_grad else None
     tops = np.zeros((cfg.world, 5), dtype=np.float32)
     dx = np.zeros((N, cfg.D), dtype=np.float32) if want_grad else None
     e = L.npo_step_world(C.byref(cfg), _fp(x_total), _fp(label_total), _fp(S_inject_all), C.c_float(loss_weight),
@@ -122,6 +128,36 @@ def step_world(x_total, label_total, cfg: NpoConfig, loss_weight=1.0, S_inject_a
     if e:
         raise OracleError(e)
     return tops, dx
+
+
+def _weighted_step(x_total, label_total, cfg, loss_weight, S_inject_all, anchor_weight):
+    """The weighted step on the C++ oracle's own backward: each rank's forward (npo_forward), anchor row i of its selected terms
+    temp1 / temp2 scaled by w_i -- which scales W1, W2, W3 and so G by w_i --, npo_backward_partial (fp32 W1..W3 and its GEMMs),
+    then npo_step_world's fp32 all-reduce and blend.  At w = 1: npo_step_world bit for bit."""
+    L = lib()
+    Q, D, world = cfg.Q, cfg.D, cfg.world
+    N = Q * world
+    w = np.asarray(anchor_weight, dtype=np.float32)
+    tops = np.zeros((world, 5), dtype=np.float32)
+    local = np.zeros((N, D), dtype=np.float32)
+    total = np.zeros((N, D), dtype=np.float32)
+    for r in range(world):
+        rows = slice(r * Q, (r + 1) * Q)
+        rcfg = NpoConfig.from_buffer_copy(cfg)
+        rcfg.rank = r
+        tops[r], st = forward(x_total, label_total, rcfg, None if S_inject_all is None else S_inject_all[rows])
+        tops[r, 0] = onp.weighted_loss(st["logv"], w[rows], Q)
+        st["temp1"][:] = (st["temp1"] * w[rows, None]).astype(np.float32)     # views into the state buffer the backward reads
+        st["temp2"][:] = (st["temp2"] * w[rows, None]).astype(np.float32)
+        lh = np.zeros((Q, D), dtype=np.float32)
+        th = np.zeros((N, D), dtype=np.float32)
+        e = L.npo_backward_partial(C.byref(rcfg), _fp(x_total), C.byref(st["_st"]), C.c_float(loss_weight), _fp(lh), _fp(th))
+        if e:
+            raise OracleError(e)
+        local[rows] = lh
+        total += th                                                            # the all-reduce, in rank order
+    td = total * np.float32(np.float32(1.0) / np.float32(world))
+    return tops, (np.float32(0.5) * td + np.float32(0.5) * local).astype(np.float32)
 
 
 def pos(sn, size):

@@ -312,3 +312,16 @@ def check_records(ref, rec, A, T, lab_rows, posi, nega, mining, k, world=1):
             i = int(np.argmax(d))
             bad.append(f"record {name}: {int(d.sum())} rows, row {i} gpu {float(g[i])!r} fp64 {want[i]!r} (j {int(j[i])})")
     return bad, j
+
+
+def weighted_records(rec, w):
+    """The row pass's weighted records [Q, 8] from the unweighted ones of the same forward: m2c - log2f(w) (+inf at w = 0), cA w and
+    cT w; the rest unchanged.  log2 is NumPy's fp32 log2: exact for w = 2^-j, within an ulp of CUDA's log2f otherwise."""
+    rec = np.array(rec, dtype=np.float32).reshape(-1, 8)
+    w = np.asarray(w, dtype=np.float32)
+    out = rec.copy()
+    with np.errstate(divide="ignore", invalid="ignore"):
+        out[:, 0] = np.where(w > 0, (rec[:, 0] - np.log2(w)).astype(np.float32), np.float32(np.inf))
+    out[:, 5] = (rec[:, 5] * w).astype(np.float32)
+    out[:, 6] = (rec[:, 6] * w).astype(np.float32)
+    return out

@@ -8,7 +8,8 @@ precision of the reference layer's own engine.  The step forms (c = lw / Q):
 
     world 1             R = (1/2)(G X + G^T X)
     emulated world W    R[rank r rows] = (1/2) G_r X_total,  R += (1/2)(1/W) G_r^T X_r  for every rank r   (both exchange forms)
-    cross-batch memory  R = (1/2)(G X_total + G[:, 0:Q]^T x)   (the memory rows get no transposed term, DESIGN 4.3)
+    cross-batch memory  R[0:Q] = (1/2)(G X_total + G[:, 0:Q]^T x),  R[Q:N] = (1/2) G[:, Q:]^T x   (the world-1 form over N = Q + m
+                        rows: the memory rows are no anchors and get the transposed term alone, DESIGN 4.3, 4.6)
 
 The checks of a gradient dx against them (violations):
     normwise       ||dx - R||     <= max(rel ||R||, k ||R32 - R||)
@@ -22,7 +23,6 @@ import numpy as np
 
 from npairloss_b200 import capi
 from oracle import npair_oracle_np as onp
-import memory_ref
 
 FP16X2, BF16X3, BF16 = capi.PREC_FP32_FP16X2, capi.PREC_FP32_BF16X3, capi.PREC_BF16
 PASSES = {FP16X2: 3, BF16X3: 6, BF16: 1}      # MMA passes of a product of two split operands (mma_passes, kernels.cuh)
@@ -74,6 +74,17 @@ def cone_inputs(N, D, eps, seed, dup=0, all_equal=False):
     return np.ascontiguousarray(x, dtype=np.float32), lab
 
 
+def make_weights(n, rng, zeros=True):
+    """Anchor weights in [0, 1] with exact 0, exact 1 and powers of two among uniform ones."""
+    w = rng.random(n).astype(np.float32)
+    k = np.arange(n)
+    w[k % 5 == 1] = 1.0
+    w[k % 5 == 2] = np.float32(2.0) ** -rng.integers(1, 12, size=int((k % 5 == 2).sum()))
+    if zeros:
+        w[k % 5 == 3] = 0.0
+    return w
+
+
 def weights(state, Q, loss_weight=1.0):
     """(G, |G|) of one rank's forward state, fp64: G = c (-W1 + W2 + W3) (npair_oracle_np.grad_weights), |G| = c (W1 + W2 + W3)."""
     A = state["A"].astype(np.float64)[:, None]
@@ -89,11 +100,6 @@ def unit_weights(state):
     """The weights before the factor c, as the weight builders form them: g' = -W1 + W2 + W3 (each |g'| <= 1 is the premise of the
     fp16x2 weight scale, weight_scale_log2 in kernels.cuh)."""
     return onp.grad_weights(state, 1, 1.0)
-
-
-def _forward(x, lab, Q, world, rank, S, mining):
-    # num_tops = 2: no retrieval counters, which the gradient does not need and which cost a sort per row
-    return onp.forward(x, lab, Q, world, rank, num_tops=2, S_inject=S, **mining)[1]
 
 
 def _products(x, terms):
@@ -120,34 +126,26 @@ def _products(x, terms):
         torch.backends.cuda.matmul.allow_tf32 = old
 
 
-def step_world(x, lab, Q, world, S_all, loss_weight=1.0, **mining):
-    """The emulated world-W step on x (N = Q * world rows), S_all the N x N similarities of every rank's rows: dict(R, B, R32, G).
+def step(x_total, lab, Q, world, S, anchor_weight=None, loss_weight=1.0, **mining):
+    """The emulated world-W step on the database x_total (the Q * world anchors, then at world 1 any memory rows), S the
+    (Q * world) x N similarities of the anchors' rows (None: the oracle's own): dict(R, B, R32, G) over all N rows, so that rows
+    [Q, N) are the memory rows' gradient.  anchor_weight: the Q * world anchors' weights, each rank's (G, |G|) scaled by row.
     G: the ranks' weights [(G, |G|)]."""
-    x = np.ascontiguousarray(x, dtype=np.float32)
+    x = np.ascontiguousarray(x_total, dtype=np.float32)
+    w = None if anchor_weight is None else np.asarray(anchor_weight, dtype=np.float32).astype(np.float64)
     terms, Gs = [], []
     for r in range(world):
-        G, Gabs = weights(_forward(x, lab, Q, world, r, S_all[r * Q:(r + 1) * Q], mining), Q, loss_weight)
-        terms.append((G, Gabs, slice(r * Q, (r + 1) * Q), 0.5, 0.5 / world))
+        rows = slice(r * Q, (r + 1) * Q)
+        # num_tops = 2: no retrieval counters, which the gradient does not need and which cost a sort per row
+        _, st = onp.forward(x, lab, Q, world, r, num_tops=2, S_inject=None if S is None else S[rows], **mining)
+        G, Gabs = weights(st, Q, loss_weight)
+        if w is not None:
+            G, Gabs = G * w[rows, None], Gabs * w[rows, None]
+        terms.append((G, Gabs, rows, 0.5, 0.5 / world))
         Gs.append((G, Gabs))
     out = _products(x, terms)
     out["G"] = Gs
     return out
-
-
-def step_memory(x, lab, x_mem, lab_mem, S, loss_weight=1.0, **mining):
-    """The cross-batch memory step (Q current rows x, m memory rows), S the Q x (Q + m) similarities: dict(R, B, R32, G) over the Q
-    current rows."""
-    _, st = memory_ref.forward_memory(x, lab, x_mem, lab_mem, num_tops=2, S_inject=S, **mining)
-    Q = np.asarray(x).shape[0]
-    G, Gabs = weights(st, Q, loss_weight)
-    xt = np.ascontiguousarray(st["x_total"], dtype=np.float32)
-    # the transposed term lands on the Q current rows only: products over the database, the current rows' share of them
-    out = _products(xt, [(G, Gabs, slice(0, Q), 0.5, 0.0)])
-    tr = _products(np.ascontiguousarray(xt[:Q]), [(np.ascontiguousarray(G[:, :Q].T), np.ascontiguousarray(Gabs[:, :Q].T),
-                                                    slice(0, Q), 0.5, 0.0)])
-    res = {k: out[k][:Q] + tr[k] for k in ("R", "B", "R32")}
-    res["G"] = [(G, Gabs)]
-    return res
 
 
 def violations(dx, ref, tau, rel=1e-5, k_sgemm=2.0, floor=TINY, row_extra=0.0):

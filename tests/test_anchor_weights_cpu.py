@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-import anchor_weight_ref as awr
+import forward_ref
+import grad_ref
 from npairloss_b200 import capi, synth, torch_api
 from oracle import npair_oracle_np as onp
 
@@ -21,13 +22,13 @@ def test_restatements_agree_weighted_all_modes(oracle, world):
     Q, D = 24, 16
     N = Q * world
     x, lab = synth.make_inputs(N, D, seed=70 + world, imgs_per_class=3, noise=0.7)
-    w = awr.make_weights(N, np.random.default_rng(world))
+    w = grad_ref.make_weights(N, np.random.default_rng(world))
     n = 0
     for apR, apM, anR, anM in itertools.product(REGIONS, METHODS, REGIONS, METHODS):
         kw = dict(margin_ident=0.02, margin_diff=-0.03, identsn=-0.4, diffsn=-0.3,
                   ap_region=apR, ap_method=apM, an_region=anR, an_method=anM)
-        tc, dc = awr.step_world_cpp(oracle, x, lab, Q, world, w, 0.7, **kw)
-        tn, dn = awr.step_world_np(x, lab, Q, world, w, 0.7, **kw)
+        tc, dc = oracle.step_world(x, lab, oracle.make_config(Q, D, world=world, **kw), 0.7, anchor_weight=w)
+        tn, dn = onp.step_world(x, lab, Q, world, 0.7, anchor_weight=w, **kw)
         np.testing.assert_allclose(tc, tn, rtol=2e-6, atol=1e-7, err_msg=str(kw))
         assert np.linalg.norm(dc - dn) <= 2e-6 * max(np.linalg.norm(dn), 1e-12), kw
         n += 1
@@ -40,14 +41,15 @@ def test_unit_weights_are_the_unweighted_oracle_bit_for_bit(oracle, world):
     x, lab = synth.make_inputs(Q * world, D, seed=5, imgs_per_class=2)
     for kw in (dict(synth.USAGE_MINING), dict(ap_region=0, ap_method=3, an_region=1, an_method=4, identsn=-0.4, diffsn=-0.3)):
         t0, d0 = onp.step_world(x, lab, Q, world, 0.9, **kw)
+        # None checks only that no weights take the unweighted path; w = 1 runs the weighted path against it
         for w in (None, np.ones(Q * world, np.float32)):
-            t1, d1 = awr.step_world_np(x, lab, Q, world, w, 0.9, **kw)
+            t1, d1 = onp.step_world(x, lab, Q, world, 0.9, anchor_weight=w, **kw)
             np.testing.assert_array_equal(t1.view(np.uint32), t0.view(np.uint32))
             np.testing.assert_array_equal(d1.view(np.uint32), d0.view(np.uint32))
         cfg = oracle.make_config(Q, 8, world=world, **kw)
         tc0, dc0 = oracle.step_world(x, lab, cfg, 0.9)
         for w in (None, np.ones(Q * world, np.float32)):
-            tc1, dc1 = awr.step_world_cpp(oracle, x, lab, Q, world, w, 0.9, **kw)
+            tc1, dc1 = oracle.step_world(x, lab, cfg, 0.9, anchor_weight=w)
             np.testing.assert_array_equal(tc1.view(np.uint32), tc0.view(np.uint32))
             np.testing.assert_array_equal(dc1.view(np.uint32), dc0.view(np.uint32))
 
@@ -60,13 +62,13 @@ def test_linearity_in_the_weights():
     w = np.array([1.0, 0.0, 0.25, 0.7, 0.5, 0.125], np.float32)
     _, st = onp.forward(x, lab, Q, **kw)
     row_loss = -st["logv"].astype(np.float64)
-    t, dx = awr.step_world_np(x, lab, Q, 1, w.astype(np.float64), **kw)
+    t, dx = onp.step_world(x, lab, Q, 1, anchor_weight=w.astype(np.float64), **kw)
     assert t[0, 0] == pytest.approx(float((w * row_loss).sum() / Q), rel=1e-6)
     acc = np.zeros((Q, D))
     for i in range(Q):
         e = np.zeros(Q)
         e[i] = 1.0
-        acc += w[i] * awr.step_world_np(x, lab, Q, 1, e, **kw)[1].astype(np.float64)
+        acc += w[i] * onp.step_world(x, lab, Q, 1, anchor_weight=e, **kw)[1].astype(np.float64)
     np.testing.assert_allclose(dx, acc, rtol=1e-6, atol=1e-8)
 
 
@@ -79,7 +81,7 @@ def test_finite_differences_of_the_weighted_loss(mining):
     x = x.astype(np.float64)
     kw = dict(synth.USAGE_MINING) if mining == "usage" else dict(ap_method=2, an_method=2)
     w = np.array([1.0, 0.0, 0.5, 0.25, 1.0, 0.0, 0.75, 0.125])
-    _, dx = awr.step_world_np(x, lab, Q, 1, w, **kw)
+    _, dx = onp.step_world(x, lab, Q, 1, anchor_weight=w, **kw)
     _, st = onp.forward(x, lab, Q, **kw)
     sel = st["sel"]
     same = lab[:, None] == lab[None, :]
@@ -109,7 +111,7 @@ def test_finite_differences_of_the_weighted_loss(mining):
 def test_masked_row_with_an_infinite_log_adds_nothing():
     """w = 0 removes a row's term even when its log value is -inf (A / T underflowed): the loss stays finite."""
     logv = np.array([-0.5, -np.inf, -1.25], np.float32)
-    assert awr.weighted_loss(logv, np.array([1.0, 0.0, 0.5], np.float32), 3) == np.float32(np.float32(-0.5 - 0.625) / np.float32(-3))
+    assert onp.weighted_loss(logv, np.array([1.0, 0.0, 0.5], np.float32), 3) == np.float32(np.float32(-0.5 - 0.625) / np.float32(-3))
 
 
 def test_weighted_record_model():
@@ -117,7 +119,7 @@ def test_weighted_record_model():
     rec = rng.standard_normal((10, 8)).astype(np.float32)
     rec[:, 5] = -np.abs(rec[:, 5])
     w = np.array([1, 0, 0.5, 2 ** -10, 0.3, 1, 0, 0.75, 1e-30, 0.999], np.float32)
-    out = awr.weighted_records(rec, w)
+    out = forward_ref.weighted_records(rec, w)
     keep = [1, 2, 3, 4, 7]
     np.testing.assert_array_equal(out[:, keep], rec[:, keep])
     np.testing.assert_array_equal(out[w == 1], rec[w == 1])

@@ -3,7 +3,7 @@ the layer (GPU)."""
 import numpy as np
 import pytest
 
-import anchor_weight_ref as awr
+import grad_ref
 from npairloss_b200 import caffe_layer, synth
 
 THREE_BOTTOMS = caffe_layer.layer_prototxt(synth.USAGE_MINING, 5, anchor_weights=True)
@@ -25,7 +25,7 @@ def test_third_bottom_gives_the_weighted_tops_and_gradient(oracle):
     from npairloss_b200 import capi
     Q, D = 120, 256
     x, lab = synth.make_inputs(Q, D, seed=42, noise=2.5)
-    w = awr.make_weights(Q, np.random.default_rng(42))
+    w = grad_ref.make_weights(Q, np.random.default_rng(42))
 
     def run(prototxt, weights=None):
         layer = caffe_layer.Layer(prototxt, Q, D)
@@ -53,7 +53,8 @@ def test_third_bottom_gives_the_weighted_tops_and_gradient(oracle):
         S = ctx.debug_read(0, Q * Q).reshape(Q, Q)
     finally:
         ctx.close()
-    tops_o, dx_o = awr.step_world_cpp(oracle, x, lab, Q, 1, w, 1.0, S_inject_all=S, faithful_sorts=0, **synth.USAGE_MINING)
+    cfg = oracle.make_config(Q, D, faithful_sorts=0, **synth.USAGE_MINING)
+    tops_o, dx_o = oracle.step_world(x, lab, cfg, 1.0, S_inject_all=S, anchor_weight=w)
     np.testing.assert_allclose(tw[0], tops_o[0, 0], rtol=1e-5, atol=1e-6)
     assert np.linalg.norm(dw - dx_o) <= 1e-5 * np.linalg.norm(dx_o)
     assert np.linalg.norm(dw - d2) > 0

@@ -11,10 +11,11 @@ import itertools
 import numpy as np
 import pytest
 
-import anchor_weight_ref as awr
+import forward_ref
 import grad_ref
 from grad_ref import SGEMM_FACTOR
 from npairloss_b200 import capi, synth, torch_api
+from oracle import npair_oracle_np as onp
 
 pytestmark = pytest.mark.gpu
 
@@ -146,7 +147,7 @@ def test_unit_weights_bit_for_bit_graph_replay(torch):
     ctx = capi.Context(capi.make_config(Q, D, **USAGE))
     try:
         ref = _step(torch, ctx, x, l, set_io=False)
-        w2 = torch.from_numpy(awr.make_weights(Q, np.random.default_rng(4))).cuda()
+        w2 = torch.from_numpy(grad_ref.make_weights(Q, np.random.default_rng(4))).cuda()
         ref2 = _step(torch, ctx, x, l, w2, None)
         tops = torch.zeros(5, device="cuda")
         dx = torch.zeros_like(x)
@@ -231,18 +232,19 @@ def test_emulated_world(torch, oracle, world, bwd_exchange):
         for k in ("tops", "dx", "S", "rec"):
             np.testing.assert_array_equal(_bits(one[k]), _bits(ref[k]), err_msg=f"w{world} x{bwd_exchange} w = 1 {k}")
         np.testing.assert_array_equal(_bits(one["rl"]), _bits(-ref["logv"]))
-        w = awr.make_weights(N, np.random.default_rng(world))
+        w = grad_ref.make_weights(N, np.random.default_rng(world))
         g = _world_step(torch, x, lab, Q, world, w, mining, bwd_exchange)
         np.testing.assert_array_equal(_bits(g["S"]), _bits(ref["S"]))
         _check_records(g["rec"], ref["rec"], w, f"w{world} x{bwd_exchange}")
-        tops_o, dx_o = awr.step_world_cpp(oracle, x, lab, Q, world, w, 0.7, S_inject_all=g["S"], faithful_sorts=0, **mining)
+        cfg = oracle.make_config(Q, D, world=world, faithful_sorts=0, **mining)
+        tops_o, dx_o = oracle.step_world(x, lab, cfg, 0.7, S_inject_all=g["S"], anchor_weight=w)
         _check_oracle(g["tops"], g["dx"], tops_o, dx_o, f"w{world} x{bwd_exchange}")
         np.testing.assert_array_equal(g["tops"][:, 1:], ref["tops"][:, 1:])
 
 
 def _check_records(rec_w, rec_1, w, tag):
     """Records bit for bit the weighted model of the unweighted ones, m2c within an ulp of log2 where w is no power of two."""
-    model = awr.weighted_records(rec_1, w)
+    model = forward_ref.weighted_records(rec_1, w)
     keep = [1, 2, 3, 4, 5, 6, 7]
     np.testing.assert_array_equal(_bits(rec_w[:, keep]), _bits(model[:, keep]), err_msg=f"{tag} records")
     dyadic = (w == 0) | (np.frexp(w)[0] == 0.5)
@@ -267,7 +269,7 @@ def test_all_mining_modes_weighted(torch, oracle, backend):
     """Every (region, method) combination, weights with zeros, the weighted oracle on the GPU's own S; thresholds bit for bit."""
     Q, D = 48, 40
     x, lab = synth.make_inputs(Q, D, seed=101, imgs_per_class=3, noise=0.7)
-    w = awr.make_weights(Q, np.random.default_rng(60))
+    w = grad_ref.make_weights(Q, np.random.default_rng(60))
     xt, lt, wt = _cuda(torch, x, lab, w)
     for apR, apM, anR, anM in itertools.product([0, 1], range(5), [0, 1], range(5)):
         mining = dict(margin_ident=0.02, margin_diff=-0.03, identsn=-0.4, diffsn=-0.3, ap_region=apR, ap_method=apM, an_region=anR,
@@ -287,7 +289,8 @@ def test_all_mining_modes_weighted(torch, oracle, backend):
         _, st = oracle.forward(x, lab, oracle.make_config(Q, D, faithful_sorts=0, **mining), S_inject=S)
         np.testing.assert_array_equal(posi, st["posi_thr"], err_msg=tag)
         np.testing.assert_array_equal(nega, st["nega_thr"], err_msg=tag)
-        tops_o, dx_o = awr.step_world_cpp(oracle, x, lab, Q, 1, w, 0.7, S_inject_all=S, faithful_sorts=0, **mining)
+        cfg = oracle.make_config(Q, D, faithful_sorts=0, **mining)
+        tops_o, dx_o = oracle.step_world(x, lab, cfg, 0.7, S_inject_all=S, anchor_weight=w)
         _check_oracle(tops, dx.cpu().numpy(), tops_o, dx_o, tag)
 
 
@@ -295,7 +298,7 @@ def test_all_mining_modes_weighted(torch, oracle, backend):
 @pytest.mark.parametrize("Q,D", [(5, 3), (129, 33), (257, 130), (999, 101)])
 def test_ragged_shapes_weighted(torch, oracle, Q, D, prec):
     x, lab = synth.make_inputs(Q, D, seed=Q + D, imgs_per_class=3, noise=1.0)
-    w = awr.make_weights(Q, np.random.default_rng(Q))
+    w = grad_ref.make_weights(Q, np.random.default_rng(Q))
     xt, lt, wt = _cuda(torch, x, lab, w)
     rl = torch.zeros(Q, device="cuda")
     ctx = capi.Context(capi.make_config(Q, D, sim_precision=prec, **RAND))
@@ -311,7 +314,8 @@ def test_ragged_shapes_weighted(torch, oracle, Q, D, prec):
     for k in DEBUG_ARRAYS:
         np.testing.assert_array_equal(_bits(stw[k]), _bits(ref[2][k]), err_msg=f"{tag} debug array {k}")
     np.testing.assert_array_equal(tw[1:], ref[0][1:])
-    tops_o, dx_o = awr.step_world_cpp(oracle, x, lab, Q, 1, w, 0.75, S_inject_all=S, faithful_sorts=0, **RAND)
+    cfg = oracle.make_config(Q, D, faithful_sorts=0, **RAND)
+    tops_o, dx_o = oracle.step_world(x, lab, cfg, 0.75, S_inject_all=S, anchor_weight=w)
     _check_oracle(tw[None], dxw, tops_o, dx_o, tag)
 
 
@@ -329,7 +333,7 @@ def _check_fp64(dx, ref, prec, path, N, tag, clustered):
 def test_gradient_against_fp64(torch, kind, Q, D, path):
     """Weighted gradient against fp64 (grad_ref's rules) on spread and clustered rows, up to the flagship shape."""
     x, lab = synth.make_inputs(Q, D, 12, noise=2.5) if kind == "synth" else grad_ref.cone_inputs(Q, D, float(kind), 12)
-    w = awr.make_weights(Q, np.random.default_rng(Q))
+    w = grad_ref.make_weights(Q, np.random.default_rng(Q))
     xt, lt, wt = _cuda(torch, x, lab, w)
     flags = capi.FLAG_NO_FUSED_GRAD if path == "split" else 0
     ctx = capi.Context(capi.make_config(Q, D, num_tops=2, flags=flags, **RAND))
@@ -342,7 +346,7 @@ def test_gradient_against_fp64(torch, kind, Q, D, path):
         S = ctx.debug_read(0, Q * Q).reshape(Q, Q)
     finally:
         ctx.close()
-    ref = awr.grad_ref_step_world(x, lab, Q, 1, S, w, **RAND)
+    ref = grad_ref.step(x, lab, Q, 1, S, w, **RAND)
     _check_fp64(dx.cpu().numpy(), ref, FP16X2, path, Q, f"{kind} {Q}", kind != "synth")
 
 
@@ -351,7 +355,7 @@ def test_memory_step_against_fp64(torch, Q, m):
     D = 128
     x, lab = grad_ref.cone_inputs(Q + m, D, 0.1, 19)
     lab = np.concatenate([lab[:Q], lab[Q:] % (Q // 2)]).astype(np.float32)
-    w = awr.make_weights(Q, np.random.default_rng(m))
+    w = grad_ref.make_weights(Q, np.random.default_rng(m))
     xt, lt, xm, lm, wt = _cuda(torch, x[:Q], lab[:Q], x[Q:], lab[Q:], w)
     ctx = capi.Context(capi.make_config(Q, D, num_tops=2, **USAGE), memory_rows=m)
     try:
@@ -363,7 +367,8 @@ def test_memory_step_against_fp64(torch, Q, m):
         S = ctx.debug_read(0, Q * (Q + m)).reshape(Q, Q + m)
     finally:
         ctx.close()
-    ref = awr.grad_ref_step_memory(x[:Q], lab[:Q], x[Q:], lab[Q:], S, w, **USAGE)
+    ref = grad_ref.step(x, lab, Q, 1, S, w, **USAGE)
+    ref = {k: ref[k][:Q] for k in ("R", "B", "R32")}                            # the anchors' rows
     _check_fp64(dx.cpu().numpy(), ref, FP16X2, "fused", Q + m, f"memory Q {Q} m {m}", True)
 
 
@@ -384,9 +389,10 @@ def test_masking_and_all_zero(torch, oracle):
         tz, dxz, _ = _step(torch, ctx, xt, lt, torch.zeros(Q, device="cuda"), None)
     finally:
         ctx.close()
-    tops_o, dx_o = awr.step_world_cpp(oracle, x, lab, Q, 1, w, 0.75, S_inject_all=S, faithful_sorts=0, **USAGE)
+    cfg = oracle.make_config(Q, D, faithful_sorts=0, **USAGE)
+    tops_o, dx_o = oracle.step_world(x, lab, cfg, 0.75, S_inject_all=S, anchor_weight=w)
     _check_oracle(t[None], dx, tops_o, dx_o, "masked")
-    _, only_cols = awr.step_world_np(x, lab, Q, 1, w, 0.75, S_inject_all=S, **USAGE)
+    _, only_cols = onp.step_world(x, lab, Q, 1, 0.75, S_inject_all=S, anchor_weight=w, **USAGE)
     masked = w == 0
     assert np.linalg.norm(dx[masked] - only_cols[masked]) <= 1e-5 * np.linalg.norm(only_cols[masked])
     assert tz[0] == 0.0 and np.all(dxz == 0.0)
@@ -428,7 +434,7 @@ def test_torch_finite_differences_and_weight_gradient(torch):
     selected); the weights' gradient is row_loss / Q."""
     Q, D = 32, 16
     x, lab = synth.make_inputs(Q, D, seed=72, imgs_per_class=4, noise=1.0)
-    w = awr.make_weights(Q, np.random.default_rng(72))
+    w = grad_ref.make_weights(Q, np.random.default_rng(72))
     m = torch_api.NPairLoss(true_gradient=True, sim_precision=BF16X3, **RAND)
     xt = torch.from_numpy(x).cuda().requires_grad_(True)
     wt = torch.from_numpy(w).cuda().requires_grad_(True)
@@ -476,7 +482,7 @@ def test_torch_graph_step_with_weights(torch):
         loss.backward()
     rng = np.random.default_rng(5)
     for _ in range(2):
-        w = torch.from_numpy(awr.make_weights(Q, rng)).cuda()
+        w = torch.from_numpy(grad_ref.make_weights(Q, rng)).cuda()
         static_w.copy_(w)
         g.replay()
         torch.cuda.synchronize()

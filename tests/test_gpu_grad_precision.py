@@ -58,7 +58,7 @@ def _check(dx, ref, prec, path, tag, kind, N, chunk_cols=0):
 def _world(x, lab, Q, world, mining, prec, path, kind, tag="", backend=TC, **cfg):
     flags = capi.FLAG_NO_FUSED_GRAD if path == "split" and world == 1 else 0
     g = gpu_step_world(x, lab, Q, world, mining, prec, backend, flags=flags, num_tops=2, **cfg)
-    _check(g["dx"], grad_ref.step_world(x, lab, Q, world, g["S"], **mining), prec, path, f"{kind} {tag}", kind, Q * world,
+    _check(g["dx"], grad_ref.step(x, lab, Q, world, g["S"], **mining), prec, path, f"{kind} {tag}", kind, Q * world,
            cfg.get("grad_chunk_cols", 0))
 
 
@@ -144,7 +144,7 @@ def test_row_blocks(torch, kind):
                 S = ctx.debug_read(0, Q * Q).reshape(Q, Q)
         finally:
             ctx.close()
-    _check(out[384], grad_ref.step_world(x, lab, Q, 1, S, **mining), FP16X2, "fused", f"{kind} row blocks", kind, Q)
+    _check(out[384], grad_ref.step(x, lab, Q, 1, S, **mining), FP16X2, "fused", f"{kind} row blocks", kind, Q)
 
 
 # --------------------------------------------------------------------------------------------------- cross-batch memory
@@ -167,5 +167,6 @@ def test_memory_step(torch, Q, m, path):
         S = ctx.debug_read(0, Q * (Q + m)).reshape(Q, Q + m)
     finally:
         ctx.close()
-    ref = grad_ref.step_memory(x[:Q], lab[:Q], x[Q:], lab[Q:], S, **mining)
+    ref = grad_ref.step(x, lab, Q, 1, S, **mining)
+    ref = {k: ref[k][:Q] for k in ("R", "B", "R32")}                            # the anchors' rows
     _check(dx.cpu().numpy(), ref, FP16X2, path, f"memory Q {Q} m {m}", "0.1", Q + m)

@@ -9,7 +9,7 @@ import pytest
 from npairloss_b200 import capi, synth
 from gpu_harness import G_TOL
 import sim_ref
-from memory_ref import step_memory
+from oracle import npair_oracle_np as onp
 
 pytestmark = pytest.mark.gpu
 
@@ -73,11 +73,13 @@ def _same_bits(a, b, tag, S=True):
 
 
 def _check_parity(g, x, l, xm, lm, mining, prec, lw, num_tops=5, tag=""):
-    """Level 1: S against fp64.  Level 2: the test reference's memory step on the GPU's own S."""
+    """Level 1: S against fp64.  Level 2: the NumPy oracle's memory step (world 1 on [x; x_mem]) on the GPU's own S."""
     Q = x.shape[0]
     bad, m = sim_ref.check(g["S"], x, np.concatenate([x, xm]), prec)
     assert not bad, f"{tag} L1 S: {bad} ({m})"
-    tops_o, dx_o, st = step_memory(x, l, xm, lm, lw, S_inject=g["S"], num_tops=num_tops, **mining)
+    tops_o, dx_o, (st,) = onp.step_world_fp64(np.concatenate([x, xm]), np.concatenate([l, lm]), Q, 1, lw, S_inject_all=g["S"],
+                                              num_tops=num_tops, **mining)
+    tops_o, dx_o = tops_o[0], dx_o[:Q]
     np.testing.assert_array_equal(g["dbg"][1], st["posi_thr"], err_msg=f"{tag} posi_thr")
     np.testing.assert_array_equal(g["dbg"][2], st["nega_thr"], err_msg=f"{tag} nega_thr")
     np.testing.assert_allclose(g["tops"][0], tops_o[0], rtol=1e-5, atol=1e-6, err_msg=f"{tag} loss")
@@ -292,7 +294,8 @@ def test_normalize_input_with_a_memory(torch, oracle):
         finally:
             ctx.close()
         y, inv = oracle.l2normalize_forward(raw)
-        tops_o, dy, st = step_memory(y, l[:Q], x[Q:], l[Q:], 1.0, S_inject=g["S"], **synth.USAGE_MINING)
+        tops_o, dy, (st,) = onp.step_world_fp64(np.concatenate([y, x[Q:]]), l, Q, 1, 1.0, S_inject_all=g["S"], **synth.USAGE_MINING)
+        tops_o, dy = tops_o[0], dy[:Q]
         np.testing.assert_allclose(g["tops"][0], tops_o[0], rtol=1e-5, atol=1e-6)
         np.testing.assert_array_equal(g["dbg"][1], st["posi_thr"])
         dx_o = oracle.l2normalize_backward(y, inv, dy.astype(np.float32))

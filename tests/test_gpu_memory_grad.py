@@ -1,7 +1,7 @@
 """The memory rows' gradient on the GPU (DESIGN 4.6): npair_backward_memory's anchor gradient against npair_backward bit for bit, its
 identities (m = 0, device weight, unit anchor weights, repeat runs, capacity and earlier calls), the memory-row gradient against the
-test reference on the GPU's own S and against fp64, against the world-W external-collectives workaround, the refusals, graph capture,
-and NPairLoss(extra_rows=...) with learnable proxies."""
+fp64 step of grad_ref on the GPU's own S (normwise and by its fp64 rules), against the world-W external-collectives workaround, the
+refusals, graph capture, and NPairLoss(extra_rows=...) with learnable proxies."""
 import ctypes as C
 import itertools
 
@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 
 import grad_ref
-import memory_grad_ref as mgr
 from gpu_harness import G_TOL
 from npairloss_b200 import capi, synth
 
@@ -58,6 +57,13 @@ def _mem_splits(Q, D, m):
     s = max(1, min(16, sms // tiles, kb // 8))
     kpb = (kb + s - 1) // s
     return (kb + kpb - 1) // kpb
+
+
+def _mem_ref(x, l, y, ly, S, w=None, loss_weight=1.0, **mining):
+    """R, B and R32 of the memory rows: rows [Q, N) of grad_ref.step over the database [x; y]."""
+    Q = x.shape[0]
+    ref = grad_ref.step(np.concatenate([x, y]), np.concatenate([l, ly]), Q, 1, S, w, loss_weight, **mining)
+    return {k: ref[k][Q:] for k in ("R", "B", "R32")}
 
 
 def _bits(a):
@@ -198,7 +204,7 @@ def test_l2_parity_every_mining_combination(torch, Q, m):
             _, dm, S = _mem_step(torch, ctx, xt, lt, yt, lyt, 1.3, S=True)
         finally:
             ctx.close()
-        ref = mgr.mem_grad(x, l, y, ly, S=S, w=w if i % 2 else None, loss_weight=1.3, **mining)
+        ref = _mem_ref(x, l, y, ly, S, w if i % 2 else None, 1.3, **mining)["R"]
         err = float(np.linalg.norm(dm - ref))
         assert err <= 1e-5 * max(float(np.linalg.norm(ref)), 1e-30), f"{mining} weighted {bool(i % 2)}: {err / np.linalg.norm(ref):.3e}"
         worst = max(worst, err / max(float(np.linalg.norm(ref)), 1e-30))
@@ -216,7 +222,7 @@ def test_l2_parity_other_formats(torch, prec):
             _, dm, S = _mem_step(torch, ctx, xt, lt, yt, lyt, S=True)
         finally:
             ctx.close()
-        ref = mgr.mem_grad(x, l, y, ly, S=S, **mining)
+        ref = _mem_ref(x, l, y, ly, S, **mining)["R"]
         assert np.linalg.norm(dm - ref) <= G_TOL[prec] * max(np.linalg.norm(ref), 1e-30), mining
 
 
@@ -237,7 +243,7 @@ def test_fp64_rules(torch, kind, Q, m, D):
         _, dm, S = _mem_step(torch, ctx, xt, lt, yt, lyt, S=True)
     finally:
         ctx.close()
-    ref = mgr.mem_grad_products(x, l, y, ly, S=S, **USAGE)
+    ref = _mem_ref(x, l, y, ly, S, **USAGE)
     k = grad_ref.SGEMM_FACTOR["accumulator" if kind == "cone" else "spread"]
     bad, meas = grad_ref.violations(dm, ref, grad_ref.tau(FP16X2, "fused", Q), rel=G_TOL[FP16X2], k_sgemm=k)
     print(f"{kind} Q {Q} m {m}: normwise {meas['normwise']:.2e} (sgemm {meas['sgemm']:.2e}) worst row {meas['row']:.3f}, "

@@ -7,7 +7,6 @@ import pytest
 
 from npairloss_b200 import synth
 import grad_ref
-import memory_ref
 import sim_ref
 from grad_ref import U24
 from oracle import npair_oracle_np as onp
@@ -43,9 +42,9 @@ def test_reference_is_the_oracle_step(oracle, world):
         try:
             _, dx_o = oracle.step_world(x, lab, cfg, 1.0, S_inject_all=S)
         except oracle.OracleError:
-            assert _or_refusal(lambda: grad_ref.step_world(x, lab, Q, world, S, **mining)) is None, mining
+            assert _or_refusal(lambda: grad_ref.step(x, lab, Q, world, S, **mining)) is None, mining
             continue
-        ref = grad_ref.step_world(x, lab, Q, world, S, **mining)
+        ref = grad_ref.step(x, lab, Q, world, S, **mining)
         # the C++ oracle runs the reference's fp32 GEMMs: within 1e-5 of the magnitude B; the NumPy one is fp64 rounded to fp32
         assert (np.abs(ref["R"] - dx_o) <= 1e-5 * ref["B"] + 1e-30).all(), mining
         _, dx_np = onp.step_world(x, lab, Q, world, S_inject_all=S, num_tops=2, **mining)
@@ -55,18 +54,20 @@ def test_reference_is_the_oracle_step(oracle, world):
     assert done >= len(SAMPLE) // 2
 
 
-def test_memory_form_is_memory_ref():
+def test_memory_form_is_the_numpy_oracle_step():
+    """The memory step's products on the anchors' rows against the NumPy oracle's fp64 step over [x; x_mem]."""
     Q, m, D = 32, 52, 24
     x, lab = grad_ref.cone_inputs(Q + m, D, 0.5, 5, dup=2)
     lab[Q:] %= Q // 2
     S = _S(x, slice(0, Q))
     done = 0
     for mining in SAMPLE:
-        ref = _or_refusal(lambda: grad_ref.step_memory(x[:Q], lab[:Q], x[Q:], lab[Q:], S, **mining))
+        ref = _or_refusal(lambda: grad_ref.step(x, lab, Q, 1, S, **mining))
         if ref is None:
             continue
-        _, dx, _ = memory_ref.step_memory(x[:Q], lab[:Q], x[Q:], lab[Q:], S_inject=S, **mining)
-        np.testing.assert_allclose(ref["R"], dx, rtol=1e-12, atol=1e-15 * np.abs(dx).max(), err_msg=str(mining))
+        _, dx, _ = onp.step_world_fp64(x, lab, Q, 1, S_inject_all=S, **mining)
+        dx = dx[:Q]
+        np.testing.assert_allclose(ref["R"][:Q], dx, rtol=1e-12, atol=1e-15 * np.abs(dx).max(), err_msg=str(mining))
         done += 1
     assert done >= len(SAMPLE) // 2
 
@@ -136,7 +137,7 @@ def test_checks_flag_the_unscaled_split_on_clustered_rows(eps):
     2^14 scale passes all three."""
     Q, D = 2048, 64
     x, lab = grad_ref.cone_inputs(Q, D, eps, 21)
-    ref = grad_ref.step_world(x, lab, Q, 1, _S(x), **synth.DEFAULT_MINING)
+    ref = grad_ref.step(x, lab, Q, 1, _S(x), **synth.DEFAULT_MINING)
     H, c = _world1_operand(ref["G"][0][0], Q)
     dx = _emulated(H, c, x, 0)
     bad, m = grad_ref.violations(dx, ref, OPERANDS_ONLY)
@@ -153,7 +154,7 @@ def test_checks_flag_kernel_faults():
     catches a dropped K block of dense weights at this N; below 1e-5 of the norm such a block falls only from about N = 40000 on)."""
     Q, D = 4096, 64
     x, lab = synth.make_inputs(Q, D, 22, noise=2.5)
-    ref = grad_ref.step_world(x, lab, Q, 1, _S(x), **synth.DEFAULT_MINING)
+    ref = grad_ref.step(x, lab, Q, 1, _S(x), **synth.DEFAULT_MINING)
     G = ref["G"][0][0]
     H = G + G.T                                        # the world-1 operand, c included
     xd = x.astype(np.float64)

@@ -1,5 +1,5 @@
-"""Cross-batch memory (DESIGN 4.3) without a GPU: the test reference of the memory step against the world-W oracle it must equal at
-m = (W - 1) Q, the workspace sizes, the exported symbols and the host-side argument checks."""
+"""Cross-batch memory (DESIGN 4.3) without a GPU: the NumPy oracle's memory step against the C++ oracle's world-W step it must equal
+at m = (W - 1) Q, the workspace sizes, the exported symbols and the host-side argument checks."""
 import ctypes as C
 import os
 import re
@@ -9,7 +9,6 @@ import pytest
 
 from npairloss_b200 import capi
 from oracle import npair_oracle_np as onp
-from memory_ref import step_memory
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -27,29 +26,31 @@ def _inputs(n, D, classes, seed):
 
 @pytest.mark.parametrize("mining", MINING)
 @pytest.mark.parametrize("W", [2, 3])
-def test_memory_step_is_rank_0_of_a_world_step(mining, W):
+def test_memory_step_is_rank_0_of_a_world_step(oracle, mining, W):
     """At m = (W - 1) Q the memory step is rank 0 of a world-W step on [x; x_mem]: its tops, and its gradient rows 0 .. Q-1 rebuilt
-    from rank 0's halves as d_local_half + W d_total_half."""
+    from rank 0's halves as d_local_half + W d_total_half.  The tops of the world-W step are the C++ oracle's."""
     Q, D = 24, 16
     xt, lt = _inputs(W * Q, D, 7, 11 + W)
-    tops_w, st = onp.forward(xt, lt, Q, W, 0, **mining)
+    tops_w, _ = oracle.forward(xt, lt, oracle.make_config(Q, D, world=W, rank=0, **mining))
+    _, st = onp.forward(xt, lt, Q, W, 0, **mining)                   # rank 0's weights, for the halves in fp64
     G = onp.grad_weights(st, Q, 1.5)
     local = 0.5 * (G @ xt.astype(np.float64))                        # d_local_half
     total = 0.5 / W * (G.T @ xt[:Q].astype(np.float64))              # rank 0's d_total_half
-    tops_m, dx_m, _ = step_memory(xt[:Q], lt[:Q], xt[Q:], lt[Q:], 1.5, **mining)
+    tops_m, dx_m, _ = onp.step_world_fp64(xt, lt, Q, 1, 1.5, **mining)          # world 1 on [x; x_mem]
+    tops_m, dx_m = tops_m[0], dx_m[:Q]
     np.testing.assert_array_equal(tops_m, tops_w)
     np.testing.assert_allclose(dx_m, local + W * total[:Q], rtol=1e-12, atol=1e-15)
-    tops_all, _ = onp.step_world(xt, lt, Q, W, 1.5, **mining)
+    tops_all, _ = oracle.step_world(xt, lt, oracle.make_config(Q, D, world=W, **mining), 1.5)
     np.testing.assert_array_equal(tops_m, tops_all[0])
 
 
 @pytest.mark.parametrize("mining", MINING)
-def test_memory_step_without_memory_is_the_plain_step(mining):
+def test_memory_step_without_memory_is_the_plain_step(oracle, mining):
     Q, D = 30, 12
     x, l = _inputs(Q, D, 6, 5)
-    tops_p, dx_p = onp.step_world(x, l, Q, 1, 0.7, **mining)
-    tops_m, dx_m, _ = step_memory(x, l, np.zeros((0, D), np.float32), np.zeros(0, np.float32), 0.7, **mining)
-    np.testing.assert_array_equal(tops_m, tops_p[0])
+    tops_p, dx_p = oracle.step_world(x, l, oracle.make_config(Q, D, **mining), 0.7)
+    tops_m, dx_m, _ = onp.step_world_fp64(x, l, Q, 1, 0.7, **mining)
+    np.testing.assert_array_equal(tops_m[0], tops_p[0])
     np.testing.assert_allclose(dx_m, dx_p, rtol=2e-6, atol=1e-9)
 
 

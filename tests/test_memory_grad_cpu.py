@@ -1,6 +1,6 @@
-"""The memory rows' gradient (DESIGN 4.6) without a GPU: the test reference against the C++ oracle's world-W backward it must equal at
-m = (W - 1) Q, against finite differences of the loss, its anchor weighting, the exported symbols and the torch API's checks and
-plumbing."""
+"""The memory rows' gradient (DESIGN 4.6) without a GPU: the fp64 reference (rows [Q, N) of grad_ref.step over [x; y]) against the C++
+oracle's world-W backward it must equal at m = (W - 1) Q, against finite differences of the loss, its anchor weighting, the exported
+symbols and the torch API's checks and plumbing."""
 import ctypes as C
 import itertools
 
@@ -8,13 +8,19 @@ import numpy as np
 import pytest
 import torch
 
-import memory_grad_ref as mgr
+import grad_ref
 from npairloss_b200 import capi, synth, torch_api
 from oracle import npair_oracle_np as onp
 
 ALL_MINING = [dict(margin_ident=0.02, margin_diff=-0.03, identsn=-0.4, diffsn=-0.3, ap_region=apR, ap_method=apM, an_region=anR,
                    an_method=anM)
               for apR, apM, anR, anM in itertools.product([0, 1], [0, 1, 2, 3, 4], [0, 1], [0, 1, 2, 3, 4])]
+
+
+def _mem_grad(x, l, y, ly, w=None, **kw):
+    """d_mem_diff in fp64 [m, D]: rows [Q, N) of grad_ref.step over the database [x; y]."""
+    Q = x.shape[0]
+    return grad_ref.step(np.concatenate([x, y]), np.concatenate([l, ly]), Q, 1, None, w, **kw)["R"][Q:]
 
 
 def _unit_rows(n, D, rng):
@@ -41,7 +47,7 @@ def test_reference_is_w_times_the_world_oracles_total_half(oracle, W):
                                       th.ctypes.data_as(fp)) == 0
         total_half = 0.5 / W * th.astype(np.float64)          # the blend's 1/2 and 1/world (.cu:474, :492-497): d_total_half
         want = W * total_half[Q:]
-        got = mgr.mem_grad(xt[:Q], lt[:Q], xt[Q:], lt[Q:], loss_weight=0.7, **kw)
+        got = _mem_grad(xt[:Q], lt[:Q], xt[Q:], lt[Q:], loss_weight=0.7, **kw)
         assert np.linalg.norm(got - want) <= 2e-6 * max(np.linalg.norm(want), 1e-12), kw
 
 
@@ -53,13 +59,32 @@ def _fd_inputs(seed, Q=10, m=7, D=6):
     return x, l, y, ly
 
 
+def _loss(x, l, y, ly, w=None, **mining):
+    """The step's loss in fp64 as a function of the memory rows y (S = x . [x; y]^T in fp64, the forward's selections and maxima
+    evaluated in fp64 too): what finite differences with respect to y differentiate.  Weighted: -(1/Q) sum_i w_i log(A_i / T_i)."""
+    x = np.asarray(x, dtype=np.float64)
+    y = np.asarray(y, dtype=np.float64)
+    Q = x.shape[0]
+    _, st = onp_forward(x.astype(np.float32), l, y.astype(np.float32), ly, **mining)
+    sel1 = st["temp1"] > 0                                      # the forward's selections, held fixed
+    sel2 = st["temp2"] > 0
+    S = x @ np.concatenate([x, y]).T
+    E = np.exp(S - st["max_all"].astype(np.float64)[:, None])
+    A = np.where(sel1, E, 0.0).sum(axis=1)
+    T = A + np.where(sel2, E, 0.0).sum(axis=1)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lv = np.where(A > 0, np.log(A / T), 0.0)
+    wv = np.ones(Q) if w is None else np.asarray(w, dtype=np.float64)
+    return -(wv * lv).sum() / Q
+
+
 def _fd(x, l, y, ly, w=None, h=1e-5, **mining):
     g = np.zeros(y.shape)
     y64 = y.astype(np.float64)
     for p, d in itertools.product(range(y.shape[0]), range(y.shape[1])):
         e = np.zeros_like(y64)
         e[p, d] = h
-        g[p, d] = (mgr.loss(x, l, y64 + e, ly, w, **mining) - mgr.loss(x, l, y64 - e, ly, w, **mining)) / (2 * h)
+        g[p, d] = (_loss(x, l, y64 + e, ly, w, **mining) - _loss(x, l, y64 - e, ly, w, **mining)) / (2 * h)
     return g
 
 
@@ -73,33 +98,32 @@ def test_reference_is_half_the_gradient_of_the_loss(mining):
     for s in (-1e-5, 1e-5):                                 # the selections of the perturbed steps are the unperturbed one's
         _, st2 = onp_forward(x, l, y + np.float32(s), ly, **mining)
         assert np.array_equal(st["temp1"] > 0, st2["temp1"] > 0) and np.array_equal(st["temp2"] > 0, st2["temp2"] > 0), mining
-    got = 2 * mgr.mem_grad(x, l, y, ly, **mining)
+    got = 2 * _mem_grad(x, l, y, ly, **mining)
     fd = _fd(x, l, y, ly, **mining)
     assert np.abs(got).max() > 1e-3
     np.testing.assert_allclose(got, fd, rtol=2e-4, atol=2e-6)
 
 
 def onp_forward(x, l, y, ly, **mining):
-    import memory_ref
-    return memory_ref.forward_memory(x, l, y, ly, num_tops=2, **mining)
+    return onp.forward(np.concatenate([x, y]), np.concatenate([l, ly]), x.shape[0], num_tops=2, **mining)
 
 
 def test_weighted_reference_is_linear_in_w_and_matches_the_weighted_loss():
     x, l, y, ly = _fd_inputs(9)
     Q = x.shape[0]
     w = np.array([1.0, 0.0, 0.5, 0.25, 1.0, 0.0, 0.75, 0.125, 1.0, 0.3], dtype=np.float32)
-    d = mgr.mem_grad(x, l, y, ly, w=w)
+    d = _mem_grad(x, l, y, ly, w=w)
     # linear in w: the sum of each anchor's share
-    parts = sum(w[i] * mgr.mem_grad(x, l, y, ly, w=np.eye(Q, dtype=np.float32)[i]) for i in range(Q))
+    parts = sum(w[i] * _mem_grad(x, l, y, ly, w=np.eye(Q, dtype=np.float32)[i]) for i in range(Q))
     np.testing.assert_allclose(d, parts, rtol=1e-12, atol=1e-15)
     # anchors with w = 0 contribute nothing: their weights rows are exactly 0
-    G, _ = mgr.weights(x, l, y, ly, w=w)
+    G, _ = grad_ref.step(np.concatenate([x, y]), np.concatenate([l, ly]), Q, 1, None, w)["G"][0]
     assert not G[w == 0].any()
     np.testing.assert_allclose(d, 0.5 * G[w > 0, Q:].T @ x[w > 0].astype(np.float64), rtol=1e-12, atol=1e-15)
     # and twice it is the gradient of the weighted loss
     np.testing.assert_allclose(2 * d, _fd(x, l, y, ly, w), rtol=2e-4, atol=2e-6)
     # w = 1 is the unweighted reference
-    np.testing.assert_array_equal(mgr.mem_grad(x, l, y, ly, w=np.ones(Q, np.float32)), mgr.mem_grad(x, l, y, ly))
+    np.testing.assert_array_equal(_mem_grad(x, l, y, ly, w=np.ones(Q, np.float32)), _mem_grad(x, l, y, ly))
 
 
 def test_symbols_are_exported_and_refuse_without_a_context():
